@@ -38,24 +38,7 @@ WORKLOADS = {
 }
 METRIC = "tvl1 flow-pairs/sec at 1920x1080"
 NWIN = 2  # distinct input windows of pairs+1 frames each, alternated between steps (both arms)
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-# captures (scripts/ncu_traffic.py writes this file from the raw CSV pages under profiles/)
-NCU_TRAFFIC_FILE = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-
-
-def ncu_traffic(workload, pairs_per_launch):
-    """Measured DRAM bytes per launch for this workload at the capture whose pairs-per-launch is closest to the
-    run's, scaled by the pair ratio; (None, reason) when no capture is committed."""
-    try:
-        caps = json.load(open(NCU_TRAFFIC_FILE)).get(workload, [])
-    except Exception:
-        caps = []
-    if not caps:
-        return None, "no ncu capture committed for this workload"
-    best = min(caps, key=lambda c_: abs(c_["pairs_per_launch"] - pairs_per_launch))
-    scale = pairs_per_launch / best["pairs_per_launch"]
-    return best["dram_bytes_per_launch"] * scale, "%s (%d-pair launch, %.3f GB DRAM read+write; scaled x%.2f to this run's pairs per launch)" % (
-        best["source"], best["pairs_per_launch"], best["dram_bytes_per_launch"] / 1e9, scale)
+DUMP_BYTES = 64 * 10**6  # --dump-outputs: most bytes written per run
 
 
 def parse():
@@ -77,7 +60,12 @@ def parse():
     # the reference's per-batch chain minus decode / file IO: BGR frames -> gray -> resize -> flow -> quantise -> 2 JPEGs per pair
     ap.add_argument("--chain", action="store_true", help="chain mode: dfb_process_bgr_batch_host on BGR frames of --chain-src size")
     ap.add_argument("--chain-src", default="", help="WxH of the decoded BGR frames (default: the workload's size, i.e. no resize)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the flows of the last timed step as DIR/flow_pairNN.npy (float32 [H,W,2]): "
+                         "evenly spaced pairs of the step, first and last included, at most 64 MB in all")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.list > 0 or args.chain):
+        ap.error("--dump-outputs applies to the default mode (--impl ours, no --list / --chain)")
     if args.pairs <= 0:
         args.pairs = 63 if args.workload in ("tvl1_340x256", "tvl1_256") else 16
     return args
@@ -85,7 +73,7 @@ def parse():
 
 # ---------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -143,7 +131,19 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)).get("hbm_gbs"), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not a measured figure"
+
+
+def dump_flows(out_dir, flows_dev):
+    """--dump-outputs: the flows the last timed step returned, as float32 [H,W,2] per pair.  A step whose flows exceed
+    DUMP_BYTES is sampled: evenly spaced pairs, the first and the last included."""
+    import numpy as np
+    P = flows_dev.shape[0]
+    per_pair = flows_dev[0].numel() * 4 + 128  # + the .npy header
+    n = max(1, min(P, DUMP_BYTES // per_pair))
+    os.makedirs(out_dir, exist_ok=True)
+    for j in sorted({int(round(x)) for x in np.linspace(0, P - 1, n)}):
+        np.save(os.path.join(out_dir, "flow_pair%02d.npy" % j), flows_dev[j].cpu().numpy().astype(np.float32))
 
 
 def make_stream(W, H, n_frames, seed, rank):
@@ -225,7 +225,7 @@ def bench_config(args, alg, W, H, desc):
     P = args.pairs
     return {"workload": desc, "algorithm": alg, "width": W, "height": H, "step": 1, "pairs_per_step": P,
             "frames_per_step": P + 1, "sharding": "one independent frame stream per rank, no collective",
-            "l2": "no explicit flush: per-pair working set (16 fp32 planes x 5 levels, ~0.3 GB x lanes) exceeds the 126 MB L2 "
+            "l2": "no explicit flush: per-pair working set (16 fp32 planes x 5 levels, ~0.3 GB x lanes) exceeds the 50 MB L2 "
                   "and consecutive steps alternate between two input windows",
             "aee_tolerance_px": 0.01}
 
@@ -537,6 +537,8 @@ def main():
     torch.cuda.synchronize(dev)
     tmark1 = sampler.mark()
     dt_dev = ev0.elapsed_time(ev1) / 1e3
+    if args.dump_outputs and rank == 0:
+        dump_flows(args.dump_outputs, flows_dev)
     shard.barrier()
     dt_dev_max = shard.all_max(dt_dev, dev)
     c = eng.counters()
@@ -564,9 +566,6 @@ def main():
         roof = {
             "bound": "hbm", "kernel": "k_tvl1_pair (persistent fused TV-L1 pair kernel)",
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures
-            "traffic": ncu_traffic(args.workload, npairs / c["timed_kernel_launches"])[0],
-            "traffic_source": ncu_traffic(args.workload, npairs / c["timed_kernel_launches"])[1],
             "peak_source": peak_src,
             "formulation": "SURVEY §8d, temporally blocked fused primal+dual: algorithmic bytes = 64 B per pixel per tile visit "
                            "(10 plane reads + 6 writes; up to k=%d iterations stay on chip per visit) x executed pixel-visits "
@@ -594,14 +593,8 @@ def main():
         # = 88 B per level pixel and iteration (SURVEY §8d, fused formulation); pixel_iters is counted by the engine
         b_alg = 88.0 * c["pixel_iters"]
         achieved = b_alg / kt / 1e9
-        t = ncu_traffic(args.workload, min(8, P))  # pairs per launch = the engine's batch of up to 8 pairs (blockIdx.z)
-        if t[0] is not None:
-            # the capture is of a FULL-RESOLUTION launch (649 MB algorithmic for 8 pairs at 1280x720); the run's launches cover all
-            # pyramid levels, so the measured bytes are scaled by the algorithmic bytes of an average launch over those of the captured one
-            full = 88.0 * min(8, P) * W * H
-            t = (t[0] * (b_alg / nl) / full, t[1] + "; a full-resolution launch, scaled by %.3f to the run's average launch over all levels" % ((b_alg / nl) / full))
         roof = {"bound": "hbm", "kernel": "k_box_solve_update<6> (13x13 box mean of M -> 2x2 solve -> rebuild M, one launch per iteration and level, up to 8 pairs per launch)",
-                "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": t[0], "traffic_source": t[1],
+                "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "peak_source": peak_src,
                 "formulation": "SURVEY §8d fused-iteration figure: 88 B per level pixel and iteration x executed pixel-iterations (engine counter), "
                                "over the CUDA-event time of the iteration launches only (one event pair per level); the last iteration of a level "
@@ -678,7 +671,7 @@ def main():
         O.lib().orc_set_num_threads(min(16, usable_cores()))
         step_device(0)  # window 0 again: flows_dev[j] = flow(frame j -> j+1)
         torch.cuda.synchronize(dev)
-        j = P - 1  # the last pair of the step (at 1080p it is in the partial launch)
+        j = P - 1  # the last pair of the step (in the last launch of the step)
         got = flows_dev[j].cpu().numpy()
         if alg == "tvl1":
             ref, ref_log = O.tvl1_calc(frames_np[0][j], frames_np[0][j + 1], return_iters=True)

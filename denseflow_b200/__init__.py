@@ -1,4 +1,4 @@
-"""denseflow_b200 — B200-native (sm_100a) dense optical flow behind the call boundary of open-mmlab/denseflow's
+"""denseflow_b200 — H100-native (sm_90a) dense optical flow behind the call boundary of open-mmlab/denseflow's
 hot path (cv::cuda::OpticalFlowDual_TVL1 / FarnebackOpticalFlow ::calc at src/denseflow_gpu.cpp:327,329)."""
 from .api import DenseOpticalFlow, FarnebackOpticalFlow, OpticalFlowDual_TVL1, create  # noqa: F401
 

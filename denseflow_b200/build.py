@@ -1,7 +1,7 @@
-"""In-tree build of the CUDA extension: nvcc -> denseflow_b200/lib/libdenseflow_b200.so (sm_100a only).
+"""In-tree build of the CUDA extension: nvcc -> denseflow_b200/lib/libdenseflow_b200.so (sm_90a only).
 
-Called by __graft_entry__.build(). nvcc cross-compiles without a GPU. The .so is git-ignored but
-travels to the GPU box with the gpurun snapshot.
+Called by __graft_entry__.build(). nvcc cross-compiles without a GPU. The .so is a build product and
+is git-ignored.
 """
 import os
 import subprocess
@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "-ccbin", "g++",
           "-I", os.path.join(HERE, "..", "include")]
 

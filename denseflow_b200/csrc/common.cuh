@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the sm_100a flow engine (device planes, error plumbing).
+// common.cuh — shared helpers for the sm_90a flow engine (device planes, error plumbing).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -46,7 +46,7 @@ __device__ __forceinline__ uint8_t quantise_px(float v, double L, double H) {
 #endif
 
 // Bump allocator over one cudaMalloc slab: all engine workspace is carved out at create time
-// (180 GB of HBM3e: no allocation ever happens on the per-pair path).
+// (no allocation ever happens on the per-pair path).
 class Slab {
   public:
     Slab() = default;

@@ -296,9 +296,9 @@ extern "C" {
 
 const char *dfb_version(void) {
 #ifdef DFB_STRICT_FP
-    return "denseflow_b200 0.1 (sm_100a, strict-fp)";
+    return "denseflow_b200 0.1 (sm_90a, strict-fp)";
 #else
-    return "denseflow_b200 0.1 (sm_100a)";
+    return "denseflow_b200 0.1 (sm_90a)";
 #endif
 }
 

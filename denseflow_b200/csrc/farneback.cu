@@ -1,4 +1,4 @@
-// farneback.cu — the Farneback path on sm_100a: what cv::cuda::FarnebackOpticalFlow::calc executes with
+// farneback.cu — the Farneback path on sm_90a: what cv::cuda::FarnebackOpticalFlow::calc executes with
 // the argument-less create() defaults the reference uses (/root/reference/src/denseflow_gpu.cpp:301,329;
 // arithmetic per SURVEY.md Appendix B: numLevels 5, pyrScale .5, winSize 13, numIters 10, polyN 5,
 // polySigma 1.1, flags 0 = box filter).
@@ -310,7 +310,7 @@ __device__ __forceinline__ void update_matrices_px(int x, int y, int w, int h, i
     update_matrices_px_r0(x, y, w, h, pitch, dx, dy, r0, R1, m);
 }
 
-// Several independent pairs per launch (blockIdx.z = pair): the coarse levels are far too small to fill 148 SMs and
+// Several independent pairs per launch (blockIdx.z = pair): the coarse levels are far too small to fill 132 SMs and
 // every kernel of the iteration is latency-bound there, so pairs are solved side by side (same idea as the TV-L1 lanes).
 constexpr int kMaxFarnBatch = 8;
 struct PairArgs {
@@ -1140,7 +1140,7 @@ class Farneback final : public FlowAlgorithm {
     static constexpr size_t kMapBytes = (size_t)kMaxLevels * kMaxFarnBatch * 10 * kTensorMapBytes;
     char *d_maps_ = nullptr;
     int maps_w_ = 0, maps_h_ = 0, maps_lanes_ = 0, maps_levels_ = 0;
-    int persistent_ctas_ = 148, use_tma_ = 1;
+    int persistent_ctas_ = 132, use_tma_ = 1;
     void ensure_tensor_maps(const LevelSet &ls) {
         const Level &F = ls.lv[ls.n - 1];
         if (maps_w_ == F.w && maps_h_ == F.h && maps_lanes_ == (int)lanes_.size() && maps_levels_ == ls.n) return;

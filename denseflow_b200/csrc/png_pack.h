@@ -11,7 +11,7 @@ struct PngBounds {
     float min_x, max_x, min_y, max_y;   // minMaxLoc of the two components
 };
 
-constexpr int kPngPackBlocks = 592;  // 4 x 148 SMs
+constexpr int kPngPackBlocks = 528;  // 4 x 132 SMs
 
 size_t png_pack_scratch_bytes();
 // flow_xy: CV_32FC2 rows (pitch in bytes); bgr: packed 3 bytes per pixel (pitch in bytes).  scratch: png_pack_scratch_bytes()

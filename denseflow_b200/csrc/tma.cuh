@@ -1,4 +1,4 @@
-// tma.cuh — sm_100a bulk-tensor (TMA) + mbarrier helpers shared by the stencil kernels: cp.async.bulk.tensor.2d loads of
+// tma.cuh — sm_90a bulk-tensor (TMA) + mbarrier helpers shared by the stencil kernels: cp.async.bulk.tensor.2d loads of
 // fp32 tiles into shared memory (zero fill outside the tensor), completion on an mbarrier, and the host-side descriptor
 // encoder (cuTensorMapEncodeTiled through the runtime's driver entry point: the library does not link libcuda).
 #pragma once

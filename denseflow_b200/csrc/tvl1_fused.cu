@@ -1,4 +1,4 @@
-// tvl1_fused.cu — the persistent fused TV-L1 pair kernel for sm_100a.
+// tvl1_fused.cu — the persistent fused TV-L1 pair kernel for sm_90a.
 //
 // One cooperative launch computes a whole flow field: everything procOneScale does for every
 // scale of cv::cuda::OpticalFlowDual_TVL1::calc (/root/reference/src/denseflow_gpu.cpp:327;
@@ -743,7 +743,7 @@ void fused_encode_tensor_map(void *out, const float *plane, int w, int h, int pi
 int fused_num_sms(int device) {
     static std::mutex m;
     static int num_sms[64] = {};
-    if (device < 0 || device >= 64) return 148;
+    if (device < 0 || device >= 64) return 132;
     std::lock_guard<std::mutex> lk(m);  // handles are created and used from several host threads (list workers)
     if (num_sms[device] == 0) DFB_CUDA(cudaDeviceGetAttribute(&num_sms[device], cudaDevAttrMultiProcessorCount, device));
     return num_sms[device];

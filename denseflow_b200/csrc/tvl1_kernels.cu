@@ -1,4 +1,4 @@
-// tvl1_kernels.cu — stand-alone sm_100a kernels of the TV-L1 path, one launch per step of
+// tvl1_kernels.cu — stand-alone sm_90a kernels of the TV-L1 path, one launch per step of
 // SURVEY.md Appendix A (the reference's launch structure; the fused persistent engine lives in
 // tvl1_fused.cu and reuses tvl1_math.cuh).  All planes are fp32 with 128-byte-aligned rows.
 #include "tvl1.cuh"

@@ -10,38 +10,17 @@
 
 namespace dfb {
 
-// ---- packed fp32 (sm_100a FFMA2 / FADD2 / FMUL2: two IEEE fp32 operations per instruction) -----------------
-// The pairs are two horizontally adjacent pixels: a float4 loaded from a plane is two aligned register pairs, so
-// packing costs no moves.  Every lane of a packed operation rounds exactly like its scalar counterpart (fma.rn /
-// add.rn / mul.rn), so a kernel may mix packed and scalar code for the same formula without changing a bit.
-// NOTE: ptxas fuses mul.rn.f32x2 + add.rn.f32x2 into FFMA2 when the product has a single use (even with -fmad=false),
-// so every place below that wants a fused multiply-add says so explicitly and no bare product feeds a bare sum.
+// ---- fp32 pairs: two horizontally adjacent pixels, each lane an explicitly rounded IEEE operation ------------
+// sm_90 has no packed fp32 instructions, so every pair operation is two scalar fma.rn / add.rn / mul.rn.  The
+// explicit rounding modes keep the compiler from contracting a product into a later sum, so the results do not
+// depend on how ptxas schedules the code: every place below that wants a fused multiply-add says so explicitly.
 #ifndef DFB_STRICT_FP
-#define DFB_PACK2(r, v) asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"((v).x), "f"((v).y))
-#define DFB_UNPACK2(v, r) asm("mov.b64 {%0, %1}, %2;" : "=f"((v).x), "=f"((v).y) : "l"(r))
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    unsigned long long ra, rb, rc, rd;
-    float2 d;
-    DFB_PACK2(ra, a);
-    DFB_PACK2(rb, b);
-    DFB_PACK2(rc, c);
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    DFB_UNPACK2(d, rd);
-    return d;
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-#define DFB_OP2(name, ptx)                                             \
-    __device__ __forceinline__ float2 name(float2 a, float2 b) {       \
-        unsigned long long ra, rb, rd;                                 \
-        float2 d;                                                      \
-        DFB_PACK2(ra, a);                                              \
-        DFB_PACK2(rb, b);                                              \
-        asm(ptx " %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));         \
-        DFB_UNPACK2(d, rd);                                            \
-        return d;                                                      \
-    }
-DFB_OP2(add2, "add.rn.f32x2")
-DFB_OP2(sub2, "sub.rn.f32x2")
-DFB_OP2(mul2, "mul.rn.f32x2")
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 lo2(const float4 &v) { return make_float2(v.x, v.y); }
 __device__ __forceinline__ float2 hi2(const float4 &v) { return make_float2(v.z, v.w); }
 __device__ __forceinline__ float4 cat2(float2 a, float2 b) { return make_float4(a.x, a.y, b.x, b.y); }

@@ -1,5 +1,5 @@
 /*
- * denseflow_b200.h — C ABI of the B200-native dense optical-flow engine.
+ * denseflow_b200.h — C ABI of the H100-native (sm_90a) dense optical-flow engine.
  *
  * This is the drop-in boundary for the one hot path of open-mmlab/denseflow: the body of the
  * per-pair loop in DenseFlow::calc_optflows_imp (/root/reference/src/denseflow_gpu.cpp:313-342).

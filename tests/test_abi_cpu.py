@@ -39,7 +39,7 @@ def test_library_exports_every_declared_symbol(built, variant):
 
 def test_version_and_error_behaviour_without_running_compute(built):
     L = built.load()
-    assert b"sm_100a" in L.dfb_version()
+    assert b"sm_90a" in L.dfb_version()
     h = C.c_void_p()
     # reference error texts (src/denseflow_gpu.cpp:296, :336) come back through dfb_last_error
     assert L.dfb_create(b"lk", 0, 64, 64, C.byref(h)) == built.DFB_ERR_UNKNOWN_ALGORITHM
