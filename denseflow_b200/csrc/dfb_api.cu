@@ -805,6 +805,7 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         const std::string k(kernel);
+        if (h->alg->debug_run(k, in, n_in, out, n_out, width, height, scalars, n_scalars)) return DFB_OK;  // the engine's own stages
         auto sc = [&](int i) { return i < n_scalars ? scalars[i] : 0.0; };
         int ow = width, oh = height;
         if (k == "resize") {

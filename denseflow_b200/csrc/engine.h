@@ -63,6 +63,13 @@ class FlowAlgorithm {
     virtual void phase_ns(uint64_t *out) { for (int i = 0; i < 32; ++i) out[i] = 0; }
     virtual void reset_counters() { launches = 0; pixel_iters = 0; pixel_chunks = 0; }
     virtual void kernel_timing(uint64_t *launches_, uint64_t *ns, uint64_t *pairs) { *launches_ = *ns = *pairs = 0; }
+    // test hook behind dfb_debug_run_kernel: run one stage of this engine, through its own launch code and buffers, on dense
+    // host planes (w x h floats each).  Returns false when `kernel` is not one of the engine's stages.
+    virtual bool debug_run(const std::string &kernel, const float *const *in, int n_in, float *const *out, int n_out, int w, int h,
+                           const double *scalars, int n_scalars) {
+        (void)kernel; (void)in; (void)n_in; (void)out; (void)n_out; (void)w; (void)h; (void)scalars; (void)n_scalars;
+        return false;
+    }
     uint64_t launches = 0;     // kernels launched
     uint64_t pixel_iters = 0;  // tvl1: sum of level pixels over executed inner iterations
     uint64_t pixel_chunks = 0; // fused tvl1: sum of level pixels over tile visits (k iterations each)

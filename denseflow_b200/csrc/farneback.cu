@@ -927,41 +927,14 @@ class Farneback final : public FlowAlgorithm {
         const FarnConsts pc = poly_constants(prm_.poly_n, prm_.poly_sigma);
         for (int f0 = 0; f0 < n; f0 += kMaxPrep) {
             const int nf = std::min(kMaxPrep, n - f0);
-            ensure_prep_scratch(nf);
-            PrepBatch pb{};
-            for (int i = 0; i < nf; ++i) {
-                pb.src[i] = srcs[f0 + i];
-                pb.frame[i] = prep_[i].frame;
-                pb.vn[i] = prep_[i].blurred;
-                pb.img[i] = prep_[i].img;
-            }
-            k_farn_u8_to_f32<<<dim3(ceil_div(w, 128), ceil_div(h, 8), nf), dim3(32, 8), 0, s>>>(pb, pitch_bytes, w, h, pitch_full);
-            DFB_KERNEL_CHECK();
-            ++launches;
+            PrepBatch pb = prep_batch(nf);
+            for (int i = 0; i < nf; ++i) pb.src[i] = srcs[f0 + i];
+            launch_u8_to_f32(pb, nf, pitch_bytes, w, h, pitch_full, s);
             for (int l = 0; l < ls.n; ++l) {
                 const Level &L = ls.lv[l];
-                const GaussKernel gk = gaussian_kernel(L.smooth, L.sigma);
-                if (gk.half > kMaxHalf) throw std::runtime_error("farn: smoothing kernel too large");
-                const float rfx = (float)(1.0 / ((double)L.w / (double)w)), rfy = (float)(1.0 / ((double)L.h / (double)h));
-                const size_t pe = ((size_t)L.pitch * (L.h + 1) + 63) & ~size_t(63);
                 for (int i = 0; i < nf; ++i) pb.r[i] = slots_.at(slots[f0 + i]) + L.r_off;
-                if (L.w == w && L.h == h) {
-                    // full resolution: the resize is the identity (weights 1, 0, 0, 0), blur straight into the level image
-                    k_gauss_blur<<<dim3(ceil_div(w, GT), ceil_div(h, GT), nf), 256, GT * (GT + 2 * gk.half) * sizeof(float), s>>>(pb, w, h, pitch_full, gk);
-                    DFB_KERNEL_CHECK();
-                    launches += 1;
-                } else {
-                    // vn: 2 * H_level <= h rows, fits the full-resolution scratch plane
-                    k_gauss_vert_rows<<<dim3(ceil_div(w, 256), 2 * L.h, nf), 256, 0, s>>>(pb, w, h, pitch_full, L.h, rfy, gk);
-                    DFB_KERNEL_CHECK();
-                    k_gauss_horz_resize<<<dim3(ceil_div(L.w, 32), ceil_div(L.h, 8), nf), dim3(32, 8), 0, s>>>(pb, w, h, pitch_full, L.w, L.h, L.pitch, rfx,
-                                                                                                             rfy, gk);
-                    DFB_KERNEL_CHECK();
-                    launches += 2;
-                }
-                k_poly_exp<5><<<dim3(ceil_div(L.w, PT), ceil_div(L.h, PT), nf), 256, 0, s>>>(pb, L.w, L.h, L.pitch, pe, pc);
-                DFB_KERNEL_CHECK();
-                launches += 1;
+                launch_level_image(pb, nf, w, h, pitch_full, L, s);
+                launch_poly_exp(pb, nf, L, pc, s);
             }
         }
     }
@@ -988,39 +961,10 @@ class Farneback final : public FlowAlgorithm {
             FarnBatchArgs args{};
             for (int l = 0; l < ls.n; ++l) {
                 const Level &L = ls.lv[l];
-                for (int i = 0; i < nb; ++i) {
-                    const Lane &ln = lanes_[i];
-                    PairArgs &a = args.p[i];
-                    a.R0 = r_planes(jobs[j0 + i].slot_a, L);
-                    a.R1 = r_planes(jobs[j0 + i].slot_b, L);
-                    for (int b = 0; b < 2; ++b)
-                        a.M[b] = Plane5{{ln.M[b][0], ln.M[b][1], ln.M[b][2], ln.M[b][3], ln.M[b][4]}, L.w, L.h, L.pitch};
-                    a.fx = Plane{ln.fx[cur], L.w, L.h, L.pitch};
-                    a.fy = Plane{ln.fy[cur], L.w, L.h, L.pitch};
-                    if (l > 0) {
-                        const Level &Pv = ls.lv[l - 1];
-                        a.pfx = Plane{ln.fx[cur ^ 1], Pv.w, Pv.h, Pv.pitch};
-                        a.pfy = Plane{ln.fy[cur ^ 1], Pv.w, Pv.h, Pv.pitch};
-                    }
-                    a.flow_xy = jobs[j0 + i].flow_xy;
-                    a.flow_pitch_bytes = jobs[j0 + i].flow_pitch_bytes;
-                    a.bound = jobs[j0 + i].bound;
-                    a.qx = jobs[j0 + i].qx;
-                    a.qy = jobs[j0 + i].qy;
-                    a.q_pitch = jobs[j0 + i].q_pitch;
-                }
-                const dim3 g8(ceil_div(L.w, 32), ceil_div(L.h, 8), nb), b8(32, 8);
-                float rfx = 1.f, rfy = 1.f;
-                if (l > 0) {
-                    rfx = (float)(1.0 / ((double)L.w / (double)ls.lv[l - 1].w));
-                    rfy = (float)(1.0 / ((double)L.h / (double)ls.lv[l - 1].h));
-                }
-                k_flow_init<<<g8, b8, 0, s>>>(args, l == 0, rfx, rfy, (float)(1.0 / prm_.pyr_scale));
-                DFB_KERNEL_CHECK();
+                for (int i = 0; i < nb; ++i) args.p[i] = pair_args(jobs[j0 + i], lanes_[i], ls, l, cur);
+                launch_flow_init(args, nb, ls, l, s);
                 int mb = 0;
-                k_update_matrices<<<g8, b8, 0, s>>>(args, mb);
-                DFB_KERNEL_CHECK();
-                launches += 2;
+                launch_update_matrices(args, nb, L, mb, s);
                 pixel_iters += (uint64_t)L.w * L.h * prm_.num_iters * nb;
                 if (time_kernels_) {
                     if (timing_used_ == kTimingRing) drain_timing();
@@ -1032,17 +976,7 @@ class Farneback final : public FlowAlgorithm {
                     DFB_CUDA(cudaEventRecord(timing_ev_[timing_used_][0], s));
                 }
                 for (int it = 0; it < prm_.num_iters; ++it) {
-                    const int rebuild = it < prm_.num_iters - 1;
-                    if (use_tma_) {
-                        const int ntx = ceil_div(L.w, BW), nty = ceil_div(L.h, BH);
-                        const int grid = std::min(persistent_ctas_, ntx * nty * nb);
-                        k_box_solve_update_tma<6><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(
-                            args, d_maps_ + (size_t)l * kMaxFarnBatch * 10 * kTensorMapBytes, nb, ntx, nty, mb, rebuild);
-                    } else {
-                        k_box_solve_update<6><<<dim3(ceil_div(L.w, BW), ceil_div(L.h, BH), nb), 256, kBoxSmemBytes, s>>>(args, mb, rebuild);
-                    }
-                    DFB_KERNEL_CHECK();
-                    ++launches;
+                    launch_iteration(args, nb, ls, l, mb, it < prm_.num_iters - 1, s);
                     mb ^= 1;
                 }
                 if (time_kernels_) {
@@ -1050,14 +984,134 @@ class Farneback final : public FlowAlgorithm {
                     ++timing_used_;
                     timed_launches_ += prm_.num_iters;
                 }
-                if (l == ls.n - 1) {  // last processed level is full resolution (k = 0): merge -> CV_32FC2
-                    k_farn_merge<<<g8, b8, 0, s>>>(args);
-                    DFB_KERNEL_CHECK();
-                    ++launches;
-                }
+                if (l == ls.n - 1) launch_merge(args, nb, L, s);  // last processed level is full resolution (k = 0): merge -> CV_32FC2
                 cur ^= 1;
             }
         }
+    }
+
+    // Test hook (dfb_debug_run_kernel): one stage on host planes, launched by the same member functions as prepare_frames /
+    // solve_batch, on the engine's own frame slots, lanes and tensor maps.
+    bool debug_run(const std::string &k, const float *const *in, int n_in, float *const *out, int n_out, int w, int h, const double *scalars,
+                   int n_scalars) override {
+        if (k.compare(0, 5, "farn_") != 0) return false;
+        auto sc = [&](int i, double dflt) { return i < n_scalars ? scalars[i] : dflt; };
+        auto need = [&](int ni, int no) {
+            if (n_in != ni || n_out != no)
+                throw std::runtime_error(k + ": expects " + std::to_string(ni) + " inputs and " + std::to_string(no) + " outputs");
+        };
+        auto fits = [&](int pw, int ph) {
+            if (pw < 1 || ph < 1 || pw > max_w_ || ph > max_h_) throw std::runtime_error(k + ": plane size outside the handle's maximum frame size");
+        };
+        // host row block [row0, row0 + p.h) of a dense host plane of width p.w <-> a pitched device plane
+        auto up = [&](const Plane &p, const float *src, int row0) {
+            DFB_CUDA(cudaMemcpy2D(p.p, (size_t)p.pitch * 4, src + (size_t)row0 * p.w, (size_t)p.w * 4, (size_t)p.w * 4, p.h, cudaMemcpyHostToDevice));
+        };
+        auto down = [&](float *dst, const Plane &p, int row0) {
+            DFB_CUDA(cudaMemcpy2D(dst + (size_t)row0 * p.w, (size_t)p.w * 4, p.p, (size_t)p.pitch * 4, (size_t)p.w * 4, p.h, cudaMemcpyDeviceToHost));
+        };
+        auto plane5 = [](const Plane5 &q, int i) { return Plane{q.p[i], q.w, q.h, q.pitch}; };
+        DFB_CUDA(cudaDeviceSynchronize());  // nothing of an earlier asynchronous call may still use the slots or lanes
+        const cudaStream_t s = nullptr;
+        if (k == "farn_level_image") {  // in {frame (u8 values as floats)}  out {level image}  scalars {k}
+            need(1, 1);
+            fits(w, h);
+            const LevelSet ls = levels_for(w, h, false);
+            const int lk = (int)sc(0, 0);
+            if (lk < 0 || lk >= ls.n) throw std::runtime_error(k + ": level k must be in [0, " + std::to_string(ls.n) + ")");
+            const Level &L = ls.lv[ls.n - 1 - lk];
+            const int pitch_full = round_up(w, 32);
+            PrepBatch pb = prep_batch(1);
+            up(Plane{pb.frame[0], w, h, pitch_full}, in[0], 0);
+            launch_level_image(pb, 1, w, h, pitch_full, L, s);
+            DFB_CUDA(cudaDeviceSynchronize());
+            down(out[0], Plane{pb.img[0], L.w, L.h, L.pitch}, 0);
+            return true;
+        }
+        if (k == "farn_poly_exp") {  // in {level image}  out {R0 .. R4}
+            need(1, 5);
+            fits(w, h);
+            const Level L{w, h, round_up(w, 32), 0, 0.0, 0};
+            PrepBatch pb = prep_batch(1);
+            pb.r[0] = slots_.at(0) + L.r_off;
+            up(Plane{pb.img[0], w, h, L.pitch}, in[0], 0);
+            launch_poly_exp(pb, 1, L, poly_constants(prm_.poly_n, prm_.poly_sigma), s);
+            DFB_CUDA(cudaDeviceSynchronize());
+            const Plane5 R = r_planes(0, L);
+            for (int i = 0; i < 5; ++i) down(out[i], plane5(R, i), 0);
+            return true;
+        }
+        if (k == "farn_flow_init") {  // in {fx, fy of the coarser level}  out {fx, fy}  scalars {level w, level h}
+            need(2, 2);
+            const int lw = (int)sc(0, 0), lh = (int)sc(1, 0);
+            fits(w, h);
+            fits(lw, lh);
+            LevelSet ls;
+            ls.n = 2;
+            ls.lv[0] = Level{w, h, round_up(w, 32), 0, 0.0, 0};
+            ls.lv[1] = Level{lw, lh, round_up(lw, 32), 0, 0.0, 0};
+            ensure_lanes(1);
+            FarnBatchArgs args{};
+            args.p[0] = pair_args(PairJob{0, 1, nullptr, 0}, lanes_[0], ls, 1, 0);
+            up(args.p[0].pfx, in[0], 0);
+            up(args.p[0].pfy, in[1], 0);
+            launch_flow_init(args, 1, ls, 1, s);
+            DFB_CUDA(cudaDeviceSynchronize());
+            down(out[0], args.p[0].fx, 0);
+            down(out[1], args.p[0].fy, 0);
+            return true;
+        }
+        const bool um = k == "farn_update_matrices";
+        if (!um && k != "farn_iteration") return false;
+        // pair stages: every input stacks `pairs` planes of h / pairs rows along its rows, one per pair (pair i = lane i, frame
+        // slots 2i / 2i + 1), so several pairs with different data run in one launch
+        //   farn_update_matrices  in {fx, fy, R0 x 5, R1 x 5}  out {M0 .. M4}                 scalars {pairs}
+        //   farn_iteration        in {M x 5, R0 x 5, R1 x 5}   out {fx, fy, M'0 .. M'4}        scalars {use_tma, rebuild, pairs}
+        const int nb = (int)sc(um ? 0 : 2, 1);
+        if (nb < 1 || nb > kMaxFarnBatch || h % nb) throw std::runtime_error(k + ": pairs must be in [1, 8] and divide the height");
+        const int ph = h / nb;
+        um ? need(12, 5) : need(15, 7);
+        fits(w, ph);
+        const LevelSet ls = levels_for(w, ph, false);
+        const int l = ls.n - 1;  // full resolution
+        ensure_slots(2 * nb);
+        ensure_lanes(nb);
+        FarnBatchArgs args{};
+        for (int i = 0; i < nb; ++i) {
+            PairArgs &a = args.p[i] = pair_args(PairJob{2 * i, 2 * i + 1, nullptr, 0}, lanes_[i], ls, l, 0);
+            const int r = i * ph;
+            if (um) {
+                up(a.fx, in[0], r);
+                up(a.fy, in[1], r);
+            }
+            const float *const *rin = in + (um ? 2 : 5);
+            for (int q = 0; q < 5; ++q) {
+                if (!um) up(plane5(a.M[0], q), in[q], r);
+                up(plane5(a.R0, q), rin[q], r);
+                up(plane5(a.R1, q), rin[5 + q], r);
+                DFB_CUDA(cudaMemset(a.M[1].p[q], 0, (size_t)a.M[1].pitch * (ph + 1) * sizeof(float)));
+            }
+        }
+        if (um) {
+            launch_update_matrices(args, nb, ls.lv[l], 0, s);
+        } else {
+            const int tma = use_tma_;
+            use_tma_ = sc(0, 1) != 0;
+            if (use_tma_) ensure_tensor_maps(ls);
+            launch_iteration(args, nb, ls, l, 0, sc(1, 1) != 0, s);
+            use_tma_ = tma;
+        }
+        DFB_CUDA(cudaDeviceSynchronize());
+        for (int i = 0; i < nb; ++i) {
+            const PairArgs &a = args.p[i];
+            const int r = i * ph;
+            if (!um) {
+                down(out[0], a.fx, r);
+                down(out[1], a.fy, r);
+            }
+            for (int q = 0; q < 5; ++q) down(out[(um ? 0 : 2) + q], plane5(a.M[um ? 0 : 1], q), r);
+        }
+        return true;
     }
 
   private:
@@ -1183,6 +1237,111 @@ class Farneback final : public FlowAlgorithm {
             }
             lanes_.push_back(l);
         }
+    }
+
+    // ---- launches: the one launch path of every kernel, shared by the engine and debug_run ----
+    PrepBatch prep_batch(int nf) {
+        ensure_prep_scratch(nf);
+        PrepBatch pb{};
+        for (int i = 0; i < nf; ++i) {
+            pb.frame[i] = prep_[i].frame;
+            pb.vn[i] = prep_[i].blurred;
+            pb.img[i] = prep_[i].img;
+        }
+        return pb;
+    }
+    void launch_u8_to_f32(const PrepBatch &pb, int nf, size_t pitch_bytes, int w, int h, int pitch_full, cudaStream_t s) {
+        k_farn_u8_to_f32<<<dim3(ceil_div(w, 128), ceil_div(h, 8), nf), dim3(32, 8), 0, s>>>(pb, pitch_bytes, w, h, pitch_full);
+        DFB_KERNEL_CHECK();
+        ++launches;
+    }
+    // pb.frame (w x h, pitch_full) -> pb.img: the Gaussian blur of level L evaluated where the resize to L samples it
+    void launch_level_image(const PrepBatch &pb, int nf, int w, int h, int pitch_full, const Level &L, cudaStream_t s) {
+        const GaussKernel gk = gaussian_kernel(L.smooth, L.sigma);
+        if (gk.half > kMaxHalf) throw std::runtime_error("farn: smoothing kernel too large");
+        const float rfx = (float)(1.0 / ((double)L.w / (double)w)), rfy = (float)(1.0 / ((double)L.h / (double)h));
+        if (L.w == w && L.h == h) {
+            // full resolution: the resize is the identity (weights 1, 0, 0, 0), blur straight into the level image
+            k_gauss_blur<<<dim3(ceil_div(w, GT), ceil_div(h, GT), nf), 256, GT * (GT + 2 * gk.half) * sizeof(float), s>>>(pb, w, h, pitch_full, gk);
+            DFB_KERNEL_CHECK();
+            launches += 1;
+        } else {
+            // vn: 2 * H_level <= h rows, fits the full-resolution scratch plane
+            k_gauss_vert_rows<<<dim3(ceil_div(w, 256), 2 * L.h, nf), 256, 0, s>>>(pb, w, h, pitch_full, L.h, rfy, gk);
+            DFB_KERNEL_CHECK();
+            k_gauss_horz_resize<<<dim3(ceil_div(L.w, 32), ceil_div(L.h, 8), nf), dim3(32, 8), 0, s>>>(pb, w, h, pitch_full, L.w, L.h, L.pitch, rfx, rfy,
+                                                                                                     gk);
+            DFB_KERNEL_CHECK();
+            launches += 2;
+        }
+    }
+    // pb.img (level L) -> the five R planes at pb.r
+    void launch_poly_exp(const PrepBatch &pb, int nf, const Level &L, const FarnConsts &pc, cudaStream_t s) {
+        const size_t pe = ((size_t)L.pitch * (L.h + 1) + 63) & ~size_t(63);
+        k_poly_exp<5><<<dim3(ceil_div(L.w, PT), ceil_div(L.h, PT), nf), 256, 0, s>>>(pb, L.w, L.h, L.pitch, pe, pc);
+        DFB_KERNEL_CHECK();
+        launches += 1;
+    }
+    // the planes of one pair at level l: R of its two frame slots, M and the flow of its lane (flow buffer `cur`, the coarser
+    // level's flow in the other one)
+    PairArgs pair_args(const PairJob &job, const Lane &ln, const LevelSet &ls, int l, int cur) const {
+        const Level &L = ls.lv[l];
+        PairArgs a{};
+        a.R0 = r_planes(job.slot_a, L);
+        a.R1 = r_planes(job.slot_b, L);
+        for (int b = 0; b < 2; ++b) a.M[b] = Plane5{{ln.M[b][0], ln.M[b][1], ln.M[b][2], ln.M[b][3], ln.M[b][4]}, L.w, L.h, L.pitch};
+        a.fx = Plane{ln.fx[cur], L.w, L.h, L.pitch};
+        a.fy = Plane{ln.fy[cur], L.w, L.h, L.pitch};
+        if (l > 0) {
+            const Level &Pv = ls.lv[l - 1];
+            a.pfx = Plane{ln.fx[cur ^ 1], Pv.w, Pv.h, Pv.pitch};
+            a.pfy = Plane{ln.fy[cur ^ 1], Pv.w, Pv.h, Pv.pitch};
+        }
+        a.flow_xy = job.flow_xy;
+        a.flow_pitch_bytes = job.flow_pitch_bytes;
+        a.bound = job.bound;
+        a.qx = job.qx;
+        a.qy = job.qy;
+        a.q_pitch = job.q_pitch;
+        return a;
+    }
+    static dim3 grid8(const Level &L, int nb) { return dim3(ceil_div(L.w, 32), ceil_div(L.h, 8), nb); }
+    // level start: zero at the coarsest level, else the upsampled flow of level l - 1 times 1 / pyrScale
+    void launch_flow_init(const FarnBatchArgs &args, int nb, const LevelSet &ls, int l, cudaStream_t s) {
+        const Level &L = ls.lv[l];
+        float rfx = 1.f, rfy = 1.f;
+        if (l > 0) {
+            rfx = (float)(1.0 / ((double)L.w / (double)ls.lv[l - 1].w));
+            rfy = (float)(1.0 / ((double)L.h / (double)ls.lv[l - 1].h));
+        }
+        k_flow_init<<<grid8(L, nb), dim3(32, 8), 0, s>>>(args, l == 0, rfx, rfy, (float)(1.0 / prm_.pyr_scale));
+        DFB_KERNEL_CHECK();
+        ++launches;
+    }
+    void launch_update_matrices(const FarnBatchArgs &args, int nb, const Level &L, int mb, cudaStream_t s) {
+        k_update_matrices<<<grid8(L, nb), dim3(32, 8), 0, s>>>(args, mb);
+        DFB_KERNEL_CHECK();
+        ++launches;
+    }
+    // one iteration (box mean of M[mb] -> solve -> rebuild into M[mb ^ 1]); the TMA kernel reads level l's tensor maps, which
+    // ensure_tensor_maps(ls) must have encoded
+    void launch_iteration(const FarnBatchArgs &args, int nb, const LevelSet &ls, int l, int mb, int rebuild, cudaStream_t s) {
+        const Level &L = ls.lv[l];
+        if (use_tma_) {
+            const int ntx = ceil_div(L.w, BW), nty = ceil_div(L.h, BH);
+            const int grid = std::min(persistent_ctas_, ntx * nty * nb);
+            k_box_solve_update_tma<6><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(args, d_maps_ + (size_t)l * kMaxFarnBatch * 10 * kTensorMapBytes, nb, ntx,
+                                                                              nty, mb, rebuild);
+        } else {
+            k_box_solve_update<6><<<dim3(ceil_div(L.w, BW), ceil_div(L.h, BH), nb), 256, kBoxSmemBytes, s>>>(args, mb, rebuild);
+        }
+        DFB_KERNEL_CHECK();
+        ++launches;
+    }
+    void launch_merge(const FarnBatchArgs &args, int nb, const Level &L, cudaStream_t s) {
+        k_farn_merge<<<grid8(L, nb), dim3(32, 8), 0, s>>>(args);
+        DFB_KERNEL_CHECK();
+        ++launches;
     }
 };
 

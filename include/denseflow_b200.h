@@ -202,6 +202,16 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
  *   "estimate_u"    in {I1wx,I1wy,grad,rho_c,p11,p12,p21,p22,u1,u2}  out {u1, u2}; scalars {l_t, theta, calc_error}; scalars_out[0] = sum(diff)
  *   "estimate_dual" in {u1,u2,p11,p12,p21,p22}               out {p11,p12,p21,p22}; scalars {taut}
  *   "resize"        in {src (w x h)}                         out {dst (scalars[0] x scalars[1])}; scalars {dw, dh, fx, fy, post_mul}
+ * On a "farn" handle, single Farneback stages, launched by the engine's own launch code on its frame slots and lanes (w, h
+ * at most the handle's maximum frame size):
+ *   "farn_level_image"     in {frame (u8 values as floats)}  out {level image, level k size}; scalars {k}
+ *   "farn_poly_exp"        in {level image}                  out {R0 .. R4}
+ *   "farn_flow_init"       in {fx, fy of the coarser level}  out {fx, fy (scalars[0] x scalars[1])}; scalars {level w, level h}
+ *   "farn_update_matrices" in {fx, fy, R0 x 5 (frame a), R1 x 5 (frame b)}  out {M0 .. M4}; scalars {pairs}
+ *   "farn_iteration"       in {M x 5, R0 x 5, R1 x 5}        out {fx, fy, M'0 .. M'4}; scalars {use_tma, rebuild, pairs}
+ *     (one box mean -> 2x2 solve -> rebuild of M iteration; M' is written only with rebuild = 1)
+ *   The two pair stages run `pairs` (1..8, default 1) pairs in one launch: every plane then stacks the pairs' planes along
+ *   its rows (height = pairs x the pair's height).
  * Not part of the reference's surface.
  */
 int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *in, int n_in, float *const *out, int n_out,
