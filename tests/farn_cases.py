@@ -14,6 +14,14 @@ FRAME_SHAPES = [(1920, 1080), (1280, 720), (340, 256), (131, 97)]
 ITER_W = [32, 33, 40, 47, 64, 65, 72, 97]
 ITER_H = [32, 33, 37, 38, 48, 49]
 ITER_SHAPES = [(w, h) for w in ITER_W for h in ITER_H]
+# frames and planes below the 32-px level cut (tests/geometry_cases.py): the 13-tap box and the 11-tap polynomial window
+# wider than the image below 13, one 32 x 16 tile, a TMA window of 48 floats from x0 - 8 holding both border patches at w <= 8
+SMALL_FRAMES = [(1, 1), (2, 1), (1, 3), (3, 2), (4, 4), (5, 7), (8, 8), (8, 1), (1, 8), (12, 5), (13, 13), (16, 9), (17, 31),
+                (31, 31), (33, 31), (31, 63), (1, 200), (200, 2)]
+SMALL_W = [1, 2, 3, 4, 5, 7, 8, 9, 12, 13, 16, 17, 31]
+SMALL_H = [1, 2, 3, 5, 8, 13, 16, 17, 31]
+ITER_SMALL = sorted({(w, SMALL_H[(3 * i + j) % len(SMALL_H)]) for i, w in enumerate(SMALL_W) for j in range(3)} |
+                    {(1, 1), (8, 8), (13, 13), (31, 31)})
 FLOW_KINDS = ["smooth", "iid", "edges", "far"]
 
 

@@ -246,6 +246,7 @@ def _update_matrices_e(fx, fy, R0, R1):
     fyr = py - y1.astype(np.float32)
     inside = (x1 >= 0) & (y1 >= 0) & (x1 < w - 1) & (y1 < h - 1)
     xs, ys = np.where(inside, x1, 0), np.where(inside, y1, 0)
+    xs1, ys1 = np.minimum(xs + 1, w - 1), np.minimum(ys + 1, h - 1)  # = xs + 1, ys + 1 inside; a 1-px plane has no inside
     one = E(np.float32(1.0))
     efx, efy = E(fxr), E(fyr)
     a00, a01, a10, a11 = (one - efx) * (one - efy), efx * (one - efy), (one - efx) * efy, efx * efy
@@ -253,7 +254,7 @@ def _update_matrices_e(fx, fy, R0, R1):
     s = []
     for k in range(5):
         P = np.asarray(R1[k], np.float32)
-        s.append(a00 * E(P[ys, xs]) + a01 * E(P[ys, xs + 1]) + a10 * E(P[ys + 1, xs]) + a11 * E(P[ys + 1, xs + 1]))
+        s.append(a00 * E(P[ys, xs]) + a01 * E(P[ys, xs1]) + a10 * E(P[ys1, xs]) + a11 * E(P[ys1, xs1]))
     zero = E(np.zeros((h, w)))
     r2 = E.where(inside, s[0], zero)
     r3 = E.where(inside, s[1], zero)

@@ -38,7 +38,7 @@ def _check(variant, name, got, exact, ref64):
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
-@pytest.mark.parametrize("shape", fc.FRAME_SHAPES)
+@pytest.mark.parametrize("shape", fc.FRAME_SHAPES + fc.SMALL_FRAMES)
 def test_level_image_and_poly_exp(oracle, shape, variant):
     """k_gauss_blur (k = 0), k_gauss_vert_rows + k_gauss_horz_resize (k > 0) and k_poly_exp<5> at every level"""
     w, h = shape
@@ -64,11 +64,12 @@ def _split(a, nb):
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
-@pytest.mark.parametrize("w", fc.ITER_W)
+@pytest.mark.parametrize("w", fc.ITER_W + fc.SMALL_W)
 def test_update_matrices(oracle, w, variant):
-    """k_update_matrices: the four flow kinds as four pairs of one launch, every iteration height"""
+    """k_update_matrices: the four flow kinds as four pairs of one launch, every iteration height (every small height for
+    the widths below 32)"""
     e, orc = _engine(variant), fc.Oracle(oracle)
-    for h in fc.ITER_H:
+    for h in (fc.ITER_H if w >= 32 else fc.SMALL_H):
         cases = []
         for p, kind in enumerate(fc.FLOW_KINDS):
             R0, R1 = orc.expansions(w, h, 100 + p)
@@ -90,7 +91,7 @@ def test_iteration(oracle, pairs, use_tma, variant):
     """k_box_solve_update_tma<6> / k_box_solve_update<6>: every iteration shape, with and without the rebuild of M, several
     pairs with different data in one launch (the persistent kernel's tile list runs over pairs x tile rows x tile columns)"""
     e, orc = _engine(variant), fc.Oracle(oracle)
-    for si, (w, h) in enumerate(fc.ITER_SHAPES):
+    for si, (w, h) in enumerate(fc.ITER_SHAPES + fc.ITER_SMALL):
         cases = [orc.pair_case(w, h, 1000 * si + p, fc.FLOW_KINDS[(si + p) % 4]) for p in range(pairs)]
         ins = [_stack([c[2][k] for c in cases]) for k in range(5)]
         ins += [_stack([c[0][k] for c in cases]) for k in range(5)] + [_stack([c[1][k] for c in cases]) for k in range(5)]

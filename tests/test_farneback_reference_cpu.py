@@ -30,7 +30,7 @@ def test_levels_and_constants_match_the_oracle(oracle):
         assert np.all(np.abs(a.astype(np.float64) - b) <= 2 ** -24 * np.abs(b) * 1.0000001)
 
 
-@pytest.mark.parametrize("shape", fc.FRAME_SHAPES)
+@pytest.mark.parametrize("shape", fc.FRAME_SHAPES + fc.SMALL_FRAMES)
 def test_level_image_and_poly_exp_within_bounds(oracle, shape):
     w, h = shape
     orc = fc.Oracle(oracle)
@@ -45,7 +45,8 @@ def test_level_image_and_poly_exp_within_bounds(oracle, shape):
                 _within("level %d R%d" % (k, i), R[i], ref)
 
 
-@pytest.mark.parametrize("shape", [(32, 32), (33, 49), (47, 37), (97, 38), (340, 256)])
+@pytest.mark.parametrize("shape", [(32, 32), (33, 49), (47, 37), (97, 38), (340, 256), (1, 1), (2, 1), (1, 3), (3, 2), (5, 7), (8, 8),
+                                   (12, 5), (13, 13), (17, 31), (1, 200), (200, 2)])
 def test_pair_stages_within_bounds(oracle, shape):
     w, h = shape
     orc = fc.Oracle(oracle)

@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+import geometry_cases as gc
 from oracle import cv_restate as R
 
 cv2 = pytest.importorskip("cv2")
@@ -16,6 +17,14 @@ def test_bgr2gray_matches_opencv():
     assert np.array_equal(R.bgr2gray(full), cv2.cvtColor(full, cv2.COLOR_BGR2GRAY))
 
 
+def test_bgr2gray_matches_opencv_on_every_triple():
+    """all 2^24 BGR triples, as 16 images of 1024 x 1024"""
+    for chunk in range(16):
+        i = np.arange(chunk << 20, (chunk + 1) << 20, dtype=np.uint32)
+        bgr = np.stack([i >> 16, (i >> 8) & 255, i & 255], -1).astype(np.uint8).reshape(1024, 1024, 3)
+        assert np.array_equal(R.bgr2gray(bgr), cv2.cvtColor(bgr, cv2.COLOR_BGR2GRAY)), chunk
+
+
 @pytest.mark.parametrize("dst", [(160, 120), (341, 256), (224, 224), (400, 300), (455, 256), (256, 341), (100, 77), (639, 479),
                                  (340, 256), (33, 500), (320, 240)])
 def test_resize_linear_u8_matches_opencv(dst):
@@ -23,6 +32,13 @@ def test_resize_linear_u8_matches_opencv(dst):
     src = rng.integers(0, 256, (240, 320), dtype=np.uint8)
     dw, dh = dst
     assert np.array_equal(R.resize_linear_u8(src, dw, dh), cv2.resize(src, (dw, dh), interpolation=cv2.INTER_LINEAR))
+
+
+@pytest.mark.parametrize("src, dst", gc.RESIZE_CASES)
+def test_resize_linear_u8_matches_opencv_at_degenerate_sizes(src, dst):
+    (sw, sh), (dw, dh) = src, dst
+    img = np.random.default_rng(sw * 7 + sh).integers(0, 256, (sh, sw), dtype=np.uint8)
+    assert np.array_equal(R.resize_linear_u8(img, dw, dh), cv2.resize(img, (dw, dh), interpolation=cv2.INTER_LINEAR))
 
 
 def test_new_size_rules():

@@ -15,6 +15,7 @@ import itertools
 import numpy as np
 import pytest
 
+import geometry_cases as gc
 import tvl1_pin as pin
 import tvl1_ref64 as r64
 from denseflow_b200 import synth
@@ -71,6 +72,9 @@ def level_shapes():
 
 
 SINGLE_TILE = [(16, 16), (17, 19), (33, 64), (64, 33), (100, 50), (127, 63), (128, 64)]
+# below the 16-px level cut (tests/geometry_cases.py): one warp band holds the image (h < 4), the halo is taller than the
+# image, one four-pixel group holds column 0 and column w - 1 (w < 4); and thin strips
+SMALL = gc.STAGE_SMALL + gc.STAGE_STRIPS
 # (G, lanes, use_tma, flag_sync, check): G = 0 means every CTA the lanes leave; G = 1 puts every tile through one CTA
 CONFIGS = list(itertools.product([1, 3, 0], [1, 3], [1, 0], [1, 0], [1, 0]))
 
@@ -163,6 +167,9 @@ def test_chunks_single_tile(oracle, variant):
         for kk in KS:
             if 2 * kk < h:
                 run_chunks(oracle, variant, w, h, kk, 2, CONFIGS[(3 * j + kk) % len(CONFIGS)], 50 * j + kk)
+    for j, (w, h) in enumerate(SMALL):  # the engine runs these with its default k = 8 as well
+        for kk in (1, 8):
+            run_chunks(oracle, variant, w, h, kk, 1 + (j + kk) % 2, CONFIGS[(3 * j + kk) % len(CONFIGS)], 7000 + 50 * j + kk)
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
@@ -197,7 +204,7 @@ def test_warp_and_level_start(oracle, variant, lanes):
     """phase_level_start (gradient, p = 0, u = 0 at the coarsest level) and phase_warp at every level"""
     L = oracle.lib()
     e = _engine(variant)
-    shapes = level_shapes() + SINGLE_TILE[:4]
+    shapes = level_shapes() + SINGLE_TILE[:4] + SMALL
     for j, (w, h) in enumerate(shapes):
         cases = []
         for i in range(lanes):
@@ -252,42 +259,48 @@ def _ref_upsample(u, dw, dh, mul):
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("lanes", [1, 3])
 def test_upsample_and_merge(oracle, variant, lanes):
-    """phase_upsample between every two consecutive levels (the spare-row clamp at the last source row), phase_merge into
-    the float2 field (bound 0) and into the quantised planes (bound 20) at every level"""
+    """phase_upsample between every two consecutive levels (the spare-row clamp at the last source row) and into planes below
+    the level cut, phase_merge into the float2 field (bound 0) and into the quantised planes (bound 20) at every level and
+    every small plane"""
     e = _engine(variant)
     mul = 1.0 / 0.8
+    ups, merges = [], []
     for w, h in FRAME_SHAPES:
         lv = oracle.tvl1_level_sizes(w, h)
-        for s in range(1, len(lv)):
-            (dw, dh), (sw, sh) = lv[s - 1], lv[s]
-            ins = [[(np.random.default_rng(s * 10 + i + c).standard_normal((sh, sw)) * 4).astype(np.float32) for c in range(2)]
-                   for i in range(lanes)]
-            got, _ = e.debug_run_kernel("tvl1_upsample", [_stack([c[k] for c in ins]) for k in range(2)], 2, [dw, dh, lanes],
-                                        out_shape=(dh * lanes, dw))
-            for i in range(lanes):
-                for c in range(2):
-                    want, fx, fy = _ref_upsample(ins[i][c], dw, dh, mul)
-                    g = _split(got[c], lanes)[i]
-                    tag = "%dx%d -> %dx%d lane %d u%d" % (sw, sh, dw, dh, i, c + 1)
-                    if variant == "strict":
-                        _check(tag, g, want)
-                    else:
-                        v, b = r64.upsample(ins[i][c], dw, dh, fx, fy, mul)
-                        bad = ~(np.abs(g.astype(np.float64) - v) <= b)
-                        assert not bad.any(), (tag, bad.sum(), tuple(np.argwhere(bad)[0]))
-        for mw, mh in lv:
-            ins = [[(np.random.default_rng(mw + i + c).standard_normal((mh, mw)) * 12).astype(np.float32) for c in range(2)] for i in range(lanes)]
-            for c in ins:
-                c[0][::9, ::5] = np.float32(20.0)  # on the quantiser's bound
-            st = [_stack([c[k] for c in ins]) for k in range(2)]
-            got, _ = e.debug_run_kernel("tvl1_merge", st, 2, [0, lanes])
-            _check("%dx%d merge" % (mw, mh), got[0], st[0])
-            _check("%dx%d merge" % (mw, mh), got[1], st[1])
-            q, _ = e.debug_run_kernel("tvl1_merge", st, 2, [20, lanes])
-            for i in range(lanes):
-                ox, oy = oracle.quantise(np.stack(ins[i], axis=-1), 20)
-                _check("%dx%d lane %d qx" % (mw, mh, i), _split(q[0], lanes)[i], ox.astype(np.float32))
-                _check("%dx%d lane %d qy" % (mw, mh, i), _split(q[1], lanes)[i], oy.astype(np.float32))
+        ups += [(lv[s - 1], lv[s]) for s in range(1, len(lv))]
+        merges += lv
+    # destinations below the level cut, from sources one 0.8 step coarser and from a single pixel
+    ups += [((w, h), (max(1, round(0.8 * w)), max(1, round(0.8 * h)))) for w, h in SMALL] + [((w, h), (1, 1)) for w, h in SMALL[::7]]
+    merges += SMALL
+    for s, ((dw, dh), (sw, sh)) in enumerate(ups, 1):
+        ins = [[(np.random.default_rng(s * 10 + i + c).standard_normal((sh, sw)) * 4).astype(np.float32) for c in range(2)]
+               for i in range(lanes)]
+        got, _ = e.debug_run_kernel("tvl1_upsample", [_stack([c[k] for c in ins]) for k in range(2)], 2, [dw, dh, lanes],
+                                    out_shape=(dh * lanes, dw))
+        for i in range(lanes):
+            for c in range(2):
+                want, fx, fy = _ref_upsample(ins[i][c], dw, dh, mul)
+                g = _split(got[c], lanes)[i]
+                tag = "%dx%d -> %dx%d lane %d u%d" % (sw, sh, dw, dh, i, c + 1)
+                if variant == "strict":
+                    _check(tag, g, want)
+                else:
+                    v, b = r64.upsample(ins[i][c], dw, dh, fx, fy, mul)
+                    bad = ~(np.abs(g.astype(np.float64) - v) <= b)
+                    assert not bad.any(), (tag, bad.sum(), tuple(np.argwhere(bad)[0]))
+    for mw, mh in merges:
+        ins = [[(np.random.default_rng(mw + i + c).standard_normal((mh, mw)) * 12).astype(np.float32) for c in range(2)] for i in range(lanes)]
+        for c in ins:
+            c[0][::9, ::5] = np.float32(20.0)  # on the quantiser's bound
+        st = [_stack([c[k] for c in ins]) for k in range(2)]
+        got, _ = e.debug_run_kernel("tvl1_merge", st, 2, [0, lanes])
+        _check("%dx%d merge" % (mw, mh), got[0], st[0])
+        _check("%dx%d merge" % (mw, mh), got[1], st[1])
+        q, _ = e.debug_run_kernel("tvl1_merge", st, 2, [20, lanes])
+        for i in range(lanes):
+            ox, oy = oracle.quantise(np.stack(ins[i], axis=-1), 20)
+            _check("%dx%d lane %d qx" % (mw, mh, i), _split(q[0], lanes)[i], ox.astype(np.float32))
+            _check("%dx%d lane %d qy" % (mw, mh, i), _split(q[1], lanes)[i], oy.astype(np.float32))
 
 
 # ---- end to end ---------------------------------------------------------------------------------------------------------

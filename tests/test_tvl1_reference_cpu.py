@@ -11,6 +11,8 @@ from tvl1_cases import chunk_inputs, warp_flow
 
 L_T, TAUT, THETA = np.float32(0.15 * 0.3), np.float32(0.25 / 0.3), np.float32(0.3)
 SHAPES = [(16, 16), (37, 53), (131, 97), (340, 256)]
+# below the level cut (tests/geometry_cases.py): single pixels, rows, columns, one four-pixel group, thin strips
+SMALL = [(1, 1), (2, 1), (1, 2), (3, 2), (2, 3), (4, 4), (1, 8), (8, 1), (5, 7), (13, 13), (15, 12), (1, 400), (400, 1), (7, 300)]
 
 
 def _within(name, got, ref):
@@ -21,7 +23,7 @@ def _within(name, got, ref):
     assert np.isfinite(b).all()
 
 
-@pytest.mark.parametrize("shape", SHAPES)
+@pytest.mark.parametrize("shape", SHAPES + SMALL)
 def test_gradient_and_warp_within_bounds(oracle, shape):
     w, h = shape
     L = oracle.lib()
@@ -40,7 +42,7 @@ def test_gradient_and_warp_within_bounds(oracle, shape):
         _within(name, got, ref)
 
 
-@pytest.mark.parametrize("shape", SHAPES)
+@pytest.mark.parametrize("shape", SHAPES + SMALL)
 def test_primal_dual_and_error_within_bounds(oracle, shape):
     w, h = shape
     L = oracle.lib()
@@ -59,7 +61,8 @@ def test_primal_dual_and_error_within_bounds(oracle, shape):
         _within("p%d" % k, p[k], ref)
 
 
-@pytest.mark.parametrize("src, dst", [((54, 40), (67, 50)), ((105, 78), (131, 97)), ((272, 205), (340, 256))])
+@pytest.mark.parametrize("src, dst", [((54, 40), (67, 50)), ((105, 78), (131, 97)), ((272, 205), (340, 256)), ((1, 1), (1, 1)),
+                                      ((1, 1), (5, 3)), ((2, 1), (3, 1)), ((1, 6), (1, 8)), ((10, 10), (13, 13)), ((320, 1), (400, 1))])
 def test_upsample_within_bounds(oracle, src, dst):
     (sw, sh), (dw, dh) = src, dst
     u = (np.random.default_rng(sw).standard_normal((sh, sw)) * 4).astype(np.float32)
@@ -96,3 +99,14 @@ def test_oracle_flow_is_independent_of_its_thread_count(oracle, shape):
         L.orc_set_num_threads(min(8, oracle.usable_cores()))
     assert np.array_equal(one, eight) and np.array_equal(log1, log8)
     assert len(errs1) == len(errs8) and np.allclose(errs1[:, 0], errs8[:, 0], rtol=1e-12, atol=0)
+
+
+def test_geometry_cases_count_levels_as_the_oracles_do(oracle):
+    """tests/geometry_cases.py restates both pyramid rules to place its level cuts: they must agree with the oracles'"""
+    import geometry_cases as gc
+    shapes = gc.TINY + gc.SQUARES + gc.STRIPS + gc.LARGE + gc.TVL1_CUTS + gc.FARN_CUTS + gc.STAGE_SMALL + gc.STAGE_STRIPS
+    for w, h in shapes:
+        assert gc.tvl1_levels(w, h) == len(oracle.tvl1_level_sizes(w, h)), (w, h)
+        assert gc.farn_levels(w, h) == len(oracle.farn_levels(w, h)), (w, h)
+    for cuts, levels in ((gc.TVL1_CUTS, gc.tvl1_levels), (gc.FARN_CUTS, gc.farn_levels)):
+        assert all(levels(*cuts[i]) + 1 == levels(*cuts[i + 1]) for i in range(0, len(cuts), 2))
