@@ -89,6 +89,13 @@ SIGNATURES = {
     "dfb_process_bgr_batch_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                              C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_size_t,
                                              C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "dfb_bgr_to_ycc420_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
+                                           C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dfb_jpeg_max_bytes_bgr": (C.c_size_t, [C.c_int, C.c_int]),
+    "dfb_encode_jpeg_bgr_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                             C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]),
+    "dfb_extract_frames_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
     "dfb_debug_run_kernel": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int,
                                        C.c_int, C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_double)]),
     "dfb_debug_time_kernel": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]),

@@ -235,6 +235,60 @@ class DenseOpticalFlow:
         self._check(self._L.dfb_process_bgr_batch_host(self._h, fp, n, step, sw, sh, dw, dh, int(bound), int(quality), xp, yp, cap, lx, ly))
         return [(bx[i][:lx[i]].tobytes(), by[i][:ly[i]].tobytes()) for i in range(m)]
 
+    # -- frame-extraction mode (-s=0, extract_frames_video, src/denseflow_gpu.cpp:82-144): resize + imencode(".jpg") per frame --
+    @staticmethod
+    def _bgr_device(bgr):
+        if bgr.dtype.itemsize != 1 or bgr.dim() != 3 or bgr.shape[2] != 3 or not bgr.is_cuda or bgr.stride(2) != 1 or bgr.stride(1) != 3:
+            raise RuntimeError("expected a packed uint8 [H,W,3] BGR CUDA tensor (rows may be pitched)")
+        return bgr.shape[1], bgr.shape[0]
+
+    def bgr_to_ycc420_device(self, bgr, new_size=None):
+        """bgr: uint8 [H,W,3] CUDA tensor; new_size: (w, h) or None.  Returns the planes libjpeg would DCT for
+        imencode(".jpg", cv::resize(bgr, new_size)): (y [h,w], cb [ceil(h/2),ceil(w/2)], cr [ceil(h/2),ceil(w/2)])."""
+        import torch
+        sw, sh = self._bgr_device(bgr)
+        dw, dh = new_size if new_size else (sw, sh)
+        y = torch.empty((dh, dw), dtype=torch.uint8, device=bgr.device)
+        cb = torch.empty(((dh + 1) // 2, (dw + 1) // 2), dtype=torch.uint8, device=bgr.device)
+        cr = torch.empty_like(cb)
+        s = torch.cuda.current_stream(bgr.device).cuda_stream
+        self._check(self._L.dfb_bgr_to_ycc420_device(self._h, bgr.data_ptr(), bgr.stride(0), sw, sh, dw, dh, y.data_ptr(), dw,
+                                                     cb.data_ptr(), cr.data_ptr(), cb.stride(0), C.c_void_p(s)))
+        return y, cb, cr
+
+    def encode_jpeg_bgr_device(self, bgr, new_size=None, quality=95):
+        """imencode(".jpg", cv::resize(bgr, new_size)) of a uint8 [H,W,3] BGR CUDA tensor, on the GPU.  Returns the bytes."""
+        import torch
+        sw, sh = self._bgr_device(bgr)
+        dw, dh = new_size if new_size else (sw, sh)
+        cap = self._L.dfb_jpeg_max_bytes_bgr(dw, dh)
+        buf = np.empty(cap, np.uint8)
+        n = C.c_size_t()
+        s = torch.cuda.current_stream(bgr.device).cuda_stream
+        self._check(self._L.dfb_encode_jpeg_bgr_device(self._h, bgr.data_ptr(), bgr.stride(0), sw, sh, dw if new_size else 0,
+                                                       dh if new_size else 0, int(quality), buf.ctypes.data, cap, C.byref(n), C.c_void_p(s)))
+        return buf[:n.value].tobytes()
+
+    def extract_frames(self, frames_bgr, new_size=None, quality=95):
+        """frames_bgr: uint8 [H,W,3] host images of one size (pageable or page-locked), or one [N,H,W,3] array.
+        Returns one JPEG bitstream per frame, in order (what extract_frames_video writes as img_%05d.jpg)."""
+        frames = [np.asarray(f) for f in frames_bgr]
+        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != frames[0].shape for f in frames):
+            raise RuntimeError("extract_frames: frames must be uint8 [H,W,3] images of one size")
+        frames = [np.ascontiguousarray(f) for f in frames]
+        n = len(frames)
+        if n == 0:
+            return []
+        sh, sw = frames[0].shape[:2]
+        dw, dh = new_size if new_size else (0, 0)
+        cap = self._L.dfb_jpeg_max_bytes_bgr(*(new_size if new_size else (sw, sh)))
+        bufs = [np.empty(cap, np.uint8) for _ in range(n)]
+        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
+        op = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
+        lens = (C.c_size_t * n)()
+        self._check(self._L.dfb_extract_frames_host(self._h, fp, n, sw, sh, dw, dh, int(quality), op, cap, lens))
+        return [bufs[i][:lens[i]].tobytes() for i in range(n)]
+
     # -- test hook: one stand-alone kernel on host planes --
     def debug_run_kernel(self, kernel, inputs, n_out, scalars=(), out_shape=None, all_scalars=False):
         """returns (output planes, scalars_out[0]), or with all_scalars (output planes, scalars_out[:16])"""

@@ -3,7 +3,6 @@
 // (/root/reference/src/denseflow_gpu.cpp:313-342): upload x2 (:317-318), calc (:327/:329),
 // download (:339) — plus the batch shape of the whole function (:307-342).
 #include <cstdlib>
-#include <type_traits>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -16,6 +15,12 @@
 #include "tvl1.cuh"
 
 using namespace dfb;
+
+// resize coefficient tables on the device, rebuilt when the geometry changes
+struct TapTable {
+    ResizeTap *d = nullptr;
+    int cap = 0, sw = 0, sh = 0, dw = 0, dh = 0;
+};
 
 struct dfb_handle {
     int device = 0;
@@ -48,8 +53,14 @@ struct dfb_handle {
     uint8_t *dec_bgr = nullptr;  // BGR scratch of dfb_decode_jpeg_gray_device
     size_t dec_bgr_cap = 0;
     void *png_scratch = nullptr;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
-    ResizeTap *d_taps = nullptr;  // resize coefficient tables on the device, rebuilt when the geometry changes
-    int taps_cap = 0, taps_sw = 0, taps_sh = 0, taps_dw = 0, taps_dh = 0;
+    TapTable gray_taps;  // dfb_resize_gray_device
+    // scratch of the frame-extraction calls (-s=0), grown on demand
+    TapTable ycc_taps;                          // colour resize of all three calls
+    uint8_t *enc_ycc = nullptr;                 // Y / Cb / Cr planes of dfb_encode_jpeg_bgr_device
+    size_t enc_ycc_cap = 0;
+    uint8_t *ex_bgr = nullptr, *ex_ycc = nullptr;  // dfb_extract_frames_host: two staging frames, planes of two groups
+    size_t ex_bgr_cap = 0, ex_ycc_cap = 0;
+    cudaEvent_t ex_events[8] = {};
 };
 
 namespace {
@@ -127,11 +138,16 @@ uint8_t *stage_q(dfb_handle *h, int r) {
     return h->h_q[r];
 }
 
-void ensure_host_path(dfb_handle *h) {
+void ensure_streams(dfb_handle *h) {
     if (h->s_in) return;
     DFB_CUDA(cudaStreamCreateWithFlags(&h->s_in, cudaStreamNonBlocking));
     DFB_CUDA(cudaStreamCreateWithFlags(&h->s_compute, cudaStreamNonBlocking));
     DFB_CUDA(cudaStreamCreateWithFlags(&h->s_out, cudaStreamNonBlocking));
+}
+
+void ensure_host_path(dfb_handle *h) {
+    ensure_streams(h);
+    if (h->d_frame[0]) return;
     const size_t fpitch = (size_t)round_up(h->max_w, 128);
     h->d_frame_pitch = fpitch;
     for (int i = 0; i < dfb_handle::kFrameRing; ++i) {
@@ -139,6 +155,80 @@ void ensure_host_path(dfb_handle *h) {
         DFB_CUDA(cudaEventCreateWithFlags(&h->ev_in[i], cudaEventDisableTiming));
         DFB_CUDA(cudaEventCreateWithFlags(&h->ev_pyr[i], cudaEventDisableTiming));
     }
+}
+
+// The x and y tables of a sw x sh -> dw x dh INTER_LINEAR resize (x: coefficients reset at the borders, y: rows clamped).
+// A launch with the old tables may still be running on any stream when the geometry changes, hence the device sync.
+const ResizeTap *ensure_taps(TapTable &t, int sw, int sh, int dw, int dh) {
+    if (t.sw != sw || t.sh != sh || t.dw != dw || t.dh != dh) {
+        std::vector<ResizeTap> xt, yt;
+        build_resize_taps(dw, sw, true, xt);
+        build_resize_taps(dh, sh, false, yt);
+        DFB_CUDA(cudaDeviceSynchronize());
+        if (dw + dh > t.cap) {
+            if (t.d) DFB_CUDA(cudaFree(t.d));
+            t.cap = dw + dh;
+            DFB_CUDA(cudaMalloc(&t.d, sizeof(ResizeTap) * t.cap));
+        }
+        DFB_CUDA(cudaMemcpy(t.d, xt.data(), sizeof(ResizeTap) * dw, cudaMemcpyHostToDevice));
+        DFB_CUDA(cudaMemcpy(t.d + dw, yt.data(), sizeof(ResizeTap) * dh, cudaMemcpyHostToDevice));
+        t.sw = sw;
+        t.sh = sh;
+        t.dw = dw;
+        t.dh = dh;
+    }
+    return t.d;
+}
+
+// grows a device scratch buffer; work still reading the old one is waited for first
+template <typename T> void grow_device(T *&ptr, size_t &cap, size_t need) {
+    if (need <= cap) return;
+    DFB_CUDA(cudaDeviceSynchronize());
+    if (ptr) DFB_CUDA(cudaFree(ptr));
+    void *p = nullptr;
+    DFB_CUDA(cudaMalloc(&p, need));
+    ptr = static_cast<T *>(p);
+    cap = need;
+}
+
+// 1: device (or managed) memory a kernel may read and write
+bool is_device_pointer(const void *p) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+// Geometry of a frame-extraction call: source sw x sh (packed BGR rows of bgr_pitch bytes), destination dw x dh, where
+// 0 / 0 means no resize.  Resolves the destination and checks it against the handle's maximum.
+int check_extract_geometry(dfb_handle *h, int sw, int sh, size_t bgr_pitch, int &dw, int &dh) {
+    if (sw <= 0 || sh <= 0 || dw < 0 || dh < 0 || (dw == 0) != (dh == 0) || bgr_pitch < (size_t)sw * 3)
+        return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    if (dw == 0) {
+        dw = sw;
+        dh = sh;
+    }
+    return check_size(h, dw, dh);
+}
+
+// Y / Cb / Cr planes of one dw x dh frame in one scratch block: 64-byte aligned rows, chroma ceil(dw / 2) x ceil(dh / 2)
+struct YccLayout {
+    size_t y_pitch, c_pitch, cb_off, cr_off, bytes;
+    YccLayout(int dw, int dh) {
+        const int cw = (dw + 1) / 2, ch = (dh + 1) / 2;
+        y_pitch = (size_t)round_up(dw, 64);
+        c_pitch = (size_t)round_up(cw, 64);
+        cb_off = y_pitch * dh;
+        cr_off = cb_off + c_pitch * ch;
+        bytes = cr_off + c_pitch * ch;
+    }
+};
+
+// the resize of a frame-extraction call: null tables mean no resize
+const ResizeTap *ycc_tables(dfb_handle *h, int sw, int sh, int dw, int dh) {
+    return (sw == dw && sh == dh) ? nullptr : ensure_taps(h->ycc_taps, sw, sh, dw, dh);
 }
 
 // output ring slots [0, n): allocated on first use (a 1080p handle runs 7 pairs per launch and touches 14 slots, a 340x256
@@ -366,7 +456,10 @@ void dfb_destroy(dfb_handle *h) {
     h->jpeg.reset();
     for (void *p : {(void *)h->pb_bgr, (void *)h->pb_gray, (void *)h->pb_frames, (void *)h->pb_q})
         if (p) cudaFree(p);
-    if (h->d_taps) cudaFree(h->d_taps);
+    for (void *p : {(void *)h->gray_taps.d, (void *)h->ycc_taps.d, (void *)h->enc_ycc, (void *)h->ex_bgr, (void *)h->ex_ycc})
+        if (p) cudaFree(p);
+    for (auto e : h->ex_events)
+        if (e) cudaEventDestroy(e);
     if (h->png_scratch) cudaFree(h->png_scratch);
     if (h->dec_bgr) cudaFree(h->dec_bgr);
     for (auto e : h->pb_events) cudaEventDestroy(e);
@@ -572,26 +665,8 @@ int dfb_resize_gray_device(dfb_handle *h, const uint8_t *src, size_t src_pitch, 
             DFB_CUDA(cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, sw, sh, cudaMemcpyDeviceToDevice, s));
             return DFB_OK;
         }
-        if (h->taps_sw != sw || h->taps_sh != sh || h->taps_dw != dw || h->taps_dh != dh) {
-            std::vector<ResizeTap> xt, yt;
-            build_resize_taps(dw, sw, true, xt);
-            build_resize_taps(dh, sh, false, yt);
-            if (dw + dh > h->taps_cap) {
-                DFB_CUDA(cudaDeviceSynchronize());
-                if (h->d_taps) DFB_CUDA(cudaFree(h->d_taps));
-                h->taps_cap = dw + dh;
-                DFB_CUDA(cudaMalloc(&h->d_taps, sizeof(ResizeTap) * h->taps_cap));
-            } else {
-                DFB_CUDA(cudaDeviceSynchronize());  // a launch with the old tables may still be running
-            }
-            DFB_CUDA(cudaMemcpy(h->d_taps, xt.data(), sizeof(ResizeTap) * dw, cudaMemcpyHostToDevice));
-            DFB_CUDA(cudaMemcpy(h->d_taps + dw, yt.data(), sizeof(ResizeTap) * dh, cudaMemcpyHostToDevice));
-            h->taps_sw = sw;
-            h->taps_sh = sh;
-            h->taps_dw = dw;
-            h->taps_dh = dh;
-        }
-        launch_resize_u8(src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, h->d_taps, h->d_taps + dw, s);
+        const ResizeTap *taps = ensure_taps(h->gray_taps, sw, sh, dw, dh);
+        launch_resize_u8(src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, taps, taps + dw, s);
         ++h->alg->launches;
         return DFB_OK;
     });
@@ -675,15 +750,7 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
         if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
         FlowAlgorithm &alg = *h->alg;
         alg.begin_batch();
-        auto grow = [&](auto *&ptr, size_t &cap, size_t need) {
-            if (need <= cap) return;
-            DFB_CUDA(cudaDeviceSynchronize());
-            if (ptr) DFB_CUDA(cudaFree(ptr));
-            void *p = nullptr;
-            DFB_CUDA(cudaMalloc(&p, need));
-            ptr = static_cast<std::remove_reference_t<decltype(ptr)>>(p);
-            cap = need;
-        };
+        auto grow = [&](uint8_t *&ptr, size_t &cap, size_t need) { grow_device(ptr, cap, need); };
         // Three stages on three streams, groups of B pairs in flight (the reference runs the same three stages as three host
         // threads around queues, include/dense_flow.h:76-80):
         //   s_in      H2D of BGR frame f -> cvtColor -> resize into the gray frame array        (decode stage tail, :163-170)
@@ -791,6 +858,160 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
             if (g > 0) finish_group(g - 1);
         }
         finish_group(G - 1);
+        DFB_CUDA(cudaStreamSynchronize(h->s_in));
+        DFB_CUDA(cudaStreamSynchronize(h->s_compute));
+        DFB_CUDA(cudaStreamSynchronize(h->s_out));
+        return DFB_OK;
+    });
+}
+
+int dfb_bgr_to_ycc420_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int src_width, int src_height, int dst_width,
+                             int dst_height, uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, void *stream) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!bgr || !y || !cb || !cr) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    int dw = dst_width, dh = dst_height;
+    if (int rc = check_extract_geometry(h, src_width, src_height, bgr_pitch, dw, dh)) return rc;
+    if (y_pitch < (size_t)dw || c_pitch < (size_t)(dw + 1) / 2) return fail(h, DFB_ERR_INVALID_ARG, "pitch smaller than a row");
+    for (const void *p : {(const void *)bgr, (const void *)y, (const void *)cb, (const void *)cr})
+        if (!is_device_pointer(p)) return fail(h, DFB_ERR_INVALID_ARG, "bgr / y / cb / cr must be device memory (device entry point)");
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        const ResizeTap *taps = ycc_tables(h, src_width, src_height, dw, dh);
+        launch_bgr_to_ycc420(bgr, bgr_pitch, src_width, src_height, dw, dh, taps, taps ? taps + dw : nullptr, y, y_pitch, cb, cr, c_pitch,
+                             static_cast<cudaStream_t>(stream));
+        ++h->alg->launches;
+        return DFB_OK;
+    });
+}
+
+size_t dfb_jpeg_max_bytes_bgr(int width, int height) {
+    if (width <= 0 || height <= 0) return 0;
+    // 2 bytes per sample of the MCU-padded image: 16 x 16 luma MCUs carry 256 Y and 2 x 64 chroma samples
+    const size_t wp = (size_t)round_up(width, 16), hp = (size_t)round_up(height, 16);
+    return (wp * hp * 3 / 2) * 2 + 4096;
+}
+
+int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int src_width, int src_height, int dst_width,
+                               int dst_height, int quality, uint8_t *out, size_t out_capacity, size_t *out_len, void *stream) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!bgr || !out || !out_len) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    int dw = dst_width, dh = dst_height;
+    if (int rc = check_extract_geometry(h, src_width, src_height, bgr_pitch, dw, dh)) return rc;
+    if (quality < 1 || quality > 100) return fail(h, DFB_ERR_INVALID_ARG, "quality must be in 1..100");
+    if (!is_device_pointer(bgr)) return fail(h, DFB_ERR_INVALID_ARG, "bgr must be device memory (device entry point)");
+    if (host_pointer_kind(out) < 0) return fail(h, DFB_ERR_INVALID_ARG, "out must be host memory");
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        const YccLayout L(dw, dh);
+        grow_device(h->enc_ycc, h->enc_ycc_cap, L.bytes);
+        const ResizeTap *taps = ycc_tables(h, src_width, src_height, dw, dh);
+        uint8_t *p = h->enc_ycc;
+        launch_bgr_to_ycc420(bgr, bgr_pitch, src_width, src_height, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
+                             p + L.cr_off, L.c_pitch, s);
+        ++h->alg->launches;
+        if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
+        h->jpeg->enqueue_ycc420(0, p, L.y_pitch, p + L.cb_off, p + L.cr_off, L.c_pitch, dw, dh, quality, s);
+        DFB_CUDA(cudaStreamSynchronize(s));
+        const size_t len = h->jpeg->length(0, s);
+        if (len > out_capacity)
+            throw std::runtime_error("jpeg output buffer too small: the bitstream needs " + std::to_string(len) + " bytes, capacity is " +
+                                     std::to_string(out_capacity));
+        h->jpeg->fetch(0, out, len, s);
+        DFB_CUDA(cudaStreamSynchronize(s));
+        h->counters.d2h_bytes += len;
+        *out_len = len;
+        return DFB_OK;
+    });
+}
+
+int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int src_width, int src_height, int dst_width,
+                            int dst_height, int quality, uint8_t *const *jpg, size_t capacity, size_t *len) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!bgr || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
+    int dw = dst_width, dh = dst_height;
+    if (int rc = check_extract_geometry(h, src_width, src_height, (size_t)src_width * 3, dw, dh)) return rc;
+    if (quality < 1 || quality > 100) return fail(h, DFB_ERR_INVALID_ARG, "quality must be in 1..100");
+    if (n_frames == 0) return DFB_OK;
+    if (!jpg || !len) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    for (int f = 0; f < n_frames; ++f) {
+        if (!bgr[f] || host_pointer_kind(bgr[f]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "bgr[" + std::to_string(f) + "] is null or a device pointer (host entry point)");
+        if (!jpg[f] || host_pointer_kind(jpg[f]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(f) + " is null or a device pointer (host entry point)");
+    }
+    const int sw = src_width, sh = src_height;
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        ensure_streams(h);
+        if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
+        // extract_frames_video's batch (src/denseflow_gpu.cpp:82-144: resize + imencode(".jpg") per frame) on four streams,
+        // groups of G frames in flight:
+        //   s_in      H2D of frame f into staging buffer f & 1
+        //   s_compute resize + YCbCr 4:2:0 of frame f into the planes of its group
+        //   s_out     the group's encodes, one encoder state per frame
+        //   s_fetch   bitstreams of group g-1 to the host while the GPU works on group g
+        constexpr int G = 8;
+        const size_t bgr_bytes = (size_t)sw * sh * 3;
+        const YccLayout L(dw, dh);
+        grow_device(h->ex_bgr, h->ex_bgr_cap, 2 * bgr_bytes);
+        grow_device(h->ex_ycc, h->ex_ycc_cap, 2 * G * L.bytes);
+        const ResizeTap *taps = ycc_tables(h, sw, sh, dw, dh);
+        for (auto &e : h->ex_events)
+            if (!e) DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        cudaEvent_t *ev_h2d = h->ex_events;       // [2] staging buffer filled
+        cudaEvent_t *ev_conv = h->ex_events + 2;  // [2] staging buffer consumed
+        cudaEvent_t *ev_planes = h->ex_events + 4;  // [2] group's planes ready
+        cudaEvent_t *ev_enc = h->ex_events + 6;   // [2] group's encodes done
+        if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
+        h->jpeg->ensure_states(2 * G);
+
+        auto convert_group = [&](int g) {
+            const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
+            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_enc[slot], 0));  // group g-2's planes have been encoded
+            for (int i = 0; i < m; ++i) {
+                const int f = f0 + i, sb = f & 1;
+                uint8_t *stage = h->ex_bgr + sb * bgr_bytes;
+                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev_conv[sb], 0));
+                DFB_CUDA(cudaMemcpyAsync(stage, bgr[f], bgr_bytes, cudaMemcpyHostToDevice, h->s_in));
+                DFB_CUDA(cudaEventRecord(ev_h2d[sb], h->s_in));
+                h->counters.h2d_bytes += bgr_bytes;
+                DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_h2d[sb], 0));
+                uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
+                launch_bgr_to_ycc420(stage, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
+                                     p + L.cr_off, L.c_pitch, h->s_compute);
+                ++h->alg->launches;
+                DFB_CUDA(cudaEventRecord(ev_conv[sb], h->s_compute));
+            }
+            DFB_CUDA(cudaEventRecord(ev_planes[slot], h->s_compute));
+            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev_planes[slot], 0));
+            for (int i = 0; i < m; ++i) {
+                const uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
+                h->jpeg->enqueue_ycc420(slot * G + i, p, L.y_pitch, p + L.cb_off, p + L.cr_off, L.c_pitch, dw, dh, quality, h->s_out);
+            }
+            DFB_CUDA(cudaEventRecord(ev_enc[slot], h->s_out));
+        };
+        auto finish_group = [&](int g) {
+            const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
+            DFB_CUDA(cudaEventSynchronize(ev_enc[slot]));
+            for (int i = 0; i < m; ++i) {
+                const int st = slot * G + i, f = f0 + i;
+                const size_t n = h->jpeg->length(st, h->s_fetch);
+                if (n > capacity)
+                    throw std::runtime_error("jpeg output buffer too small: frame " + std::to_string(f) + " needs " + std::to_string(n) +
+                                             " bytes, capacity is " + std::to_string(capacity));
+                len[f] = n;
+                h->jpeg->fetch(st, jpg[f], n, h->s_fetch);
+                h->counters.d2h_bytes += n;
+            }
+            DFB_CUDA(cudaStreamSynchronize(h->s_fetch));
+        };
+        const int NG = (n_frames + G - 1) / G;
+        for (int g = 0; g < NG; ++g) {
+            convert_group(g);
+            if (g > 0) finish_group(g - 1);
+        }
+        finish_group(NG - 1);
         DFB_CUDA(cudaStreamSynchronize(h->s_in));
         DFB_CUDA(cudaStreamSynchronize(h->s_compute));
         DFB_CUDA(cudaStreamSynchronize(h->s_out));

@@ -75,6 +75,9 @@ struct JpegEncoder::Impl {
     std::vector<nvjpegEncoderState_t> states;
     nvjpegEncoderParams_t params = nullptr;
     int quality = -1;
+    // colour frames: parameters of their own, so the gray path's sampling factors are never touched (created on first use)
+    nvjpegEncoderParams_t params420 = nullptr;
+    int quality420 = -1;
     nvjpegJpegState_t dec_state = nullptr;  // created on the first decode
 };
 
@@ -89,6 +92,7 @@ JpegEncoder::JpegEncoder() : impl_(new Impl) {
 JpegEncoder::~JpegEncoder() {
     Api &a = api();
     if (impl_->params) a.ParamsDestroy(impl_->params);
+    if (impl_->params420) a.ParamsDestroy(impl_->params420);
     for (auto st : impl_->states)
         if (st) a.StateDestroy(st);
     if (impl_->dec_state && a.JpegStateDestroy) a.JpegStateDestroy(impl_->dec_state);
@@ -118,6 +122,27 @@ void JpegEncoder::enqueue(int state, const uint8_t *gray, size_t pitch, int w, i
     img.channel[0] = const_cast<unsigned char *>(gray);
     img.pitch[0] = pitch;
     check(a.EncodeYUV(impl_->handle, impl_->states[state], impl_->params, &img, NVJPEG_CSS_GRAY, w, h, s), "nvjpegEncodeYUV");
+}
+
+void JpegEncoder::enqueue_ycc420(int state, const uint8_t *y, size_t y_pitch, const uint8_t *cb, const uint8_t *cr, size_t c_pitch, int w,
+                                 int h, int quality, cudaStream_t s) {
+    Api &a = api();
+    ensure_states(state + 1);
+    if (!impl_->params420) check(a.ParamsCreate(impl_->handle, &impl_->params420, nullptr), "nvjpegEncoderParamsCreate");
+    if (quality != impl_->quality420) {
+        check(a.SetQuality(impl_->params420, quality, s), "SetQuality");
+        check(a.SetSampling(impl_->params420, NVJPEG_CSS_420, s), "SetSamplingFactors");
+        check(a.SetOptHuff(impl_->params420, 0, s), "SetOptimizedHuffman");
+        impl_->quality420 = quality;
+    }
+    nvjpegImage_t img{};
+    img.channel[0] = const_cast<unsigned char *>(y);
+    img.pitch[0] = y_pitch;
+    img.channel[1] = const_cast<unsigned char *>(cb);
+    img.pitch[1] = c_pitch;
+    img.channel[2] = const_cast<unsigned char *>(cr);
+    img.pitch[2] = c_pitch;
+    check(a.EncodeYUV(impl_->handle, impl_->states[state], impl_->params420, &img, NVJPEG_CSS_420, w, h, s), "nvjpegEncodeYUV");
 }
 
 size_t JpegEncoder::length(int state, cudaStream_t s) {

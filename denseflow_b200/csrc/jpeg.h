@@ -20,6 +20,10 @@ class JpegEncoder {
     //   fetch(state, out, s)  enqueues the copy of the bitstream into the host buffer on s (any stream; complete after a sync of s)
     void ensure_states(int n);
     void enqueue(int state, const uint8_t *gray, size_t pitch, int w, int h, int quality, cudaStream_t s);
+    // The colour counterpart of enqueue: planar Y (w x h) and Cb / Cr (ceil(w / 2) x ceil(h / 2)) as libjpeg samples them,
+    // encoded as YCbCr 4:2:0 (baseline, standard Huffman tables) with parameters separate from the gray ones.
+    void enqueue_ycc420(int state, const uint8_t *y, size_t y_pitch, const uint8_t *cb, const uint8_t *cr, size_t c_pitch, int w, int h,
+                        int quality, cudaStream_t s);
     size_t length(int state, cudaStream_t s);
     void fetch(int state, uint8_t *out, size_t len, cudaStream_t s);
 

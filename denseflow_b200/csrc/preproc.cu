@@ -5,6 +5,8 @@
 //   gray   = (B*3735 + G*19235 + R*9798 + 2^14) >> 15
 //   resize : 11-bit coefficients cvRound(alpha*2048) (x coefficients reset at the borders, y rows index-clamped
 //            with beta kept), horizontal pass in int, vertical (((b0*(S0>>4))>>16) + ((b1*(S1>>4))>>16) + 2) >> 2
+// The frame-extraction mode (-s=0) resizes the colour frame instead (the same arithmetic per channel) and JPEG-encodes it;
+// k_bgr_to_ycc420 produces exactly the planes libjpeg would hand to its forward DCT, so only the DCT differs from imencode.
 #include <cmath>
 #include <vector>
 
@@ -22,6 +24,20 @@ __global__ void __launch_bounds__(256) k_bgr_to_gray(const uint8_t *__restrict__
     gray[(size_t)y * gray_pitch + x] = (uint8_t)((p[0] * 3735 + p[1] * 19235 + p[2] * 9798 + 16384) >> 15);
 }
 
+// One INTER_LINEAR sample: source bytes i0 / i1 (the x taps, already scaled by the channel count) of the two source rows
+// the y tap selects.  Shared by the gray and the colour resize so both run the same arithmetic.
+__device__ __forceinline__ int resize_sample(const uint8_t *__restrict__ r0, const uint8_t *__restrict__ r1, int i0, int i1,
+                                             const ResizeTap &tx, const ResizeTap &ty) {
+    const int S0 = r0[i0] * tx.a0 + r0[i1] * tx.a1;
+    const int S1 = r1[i0] * tx.a0 + r1[i1] * tx.a1;
+    const int v = (((ty.a0 * (S0 >> 4)) >> 16) + ((ty.a1 * (S1 >> 4)) >> 16) + 2) >> 2;
+    return min(max(v, 0), 255);
+}
+
+__device__ __forceinline__ const uint8_t *resize_row(const uint8_t *src, size_t src_pitch, int sh, int idx) {
+    return src + (size_t)min(max(idx, 0), sh - 1) * src_pitch;
+}
+
 __global__ void __launch_bounds__(256) k_resize_u8(const uint8_t *__restrict__ src, size_t src_pitch, int sw, int sh,
                                                    uint8_t *__restrict__ dst, size_t dst_pitch, int dw, int dh,
                                                    const ResizeTap *__restrict__ xt, const ResizeTap *__restrict__ yt) {
@@ -29,12 +45,63 @@ __global__ void __launch_bounds__(256) k_resize_u8(const uint8_t *__restrict__ s
     if (x >= dw || y >= dh) return;
     const ResizeTap tx = xt[x], ty = yt[y];
     const int x1 = min(tx.idx + 1, sw - 1);
-    const uint8_t *r0 = src + (size_t)min(max(ty.idx, 0), sh - 1) * src_pitch;
-    const uint8_t *r1 = src + (size_t)min(max(ty.idx + 1, 0), sh - 1) * src_pitch;
-    const int S0 = r0[tx.idx] * tx.a0 + r0[x1] * tx.a1;
-    const int S1 = r1[tx.idx] * tx.a0 + r1[x1] * tx.a1;
-    const int v = (((ty.a0 * (S0 >> 4)) >> 16) + ((ty.a1 * (S1 >> 4)) >> 16) + 2) >> 2;
-    dst[(size_t)y * dst_pitch + x] = (uint8_t)min(max(v, 0), 255);
+    const uint8_t *r0 = resize_row(src, src_pitch, sh, ty.idx), *r1 = resize_row(src, src_pitch, sh, ty.idx + 1);
+    dst[(size_t)y * dst_pitch + x] = (uint8_t)resize_sample(r0, r1, tx.idx, x1, tx, ty);
+}
+
+// libjpeg's rgb_ycc_convert (jccolor.c), FIX(x) = (int)(x * 65536 + 0.5); Cb and Cr carry CBCR_OFFSET + ONE_HALF - 1
+__device__ __forceinline__ void bgr_to_ycc(int b, int g, int r, int &y, int &cb, int &cr) {
+    y = (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
+    cb = (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16;
+    cr = (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16;
+}
+
+// Packed BGR (sw x sh) -> cv::resize(INTER_LINEAR) to dw x dh (identity when xt == nullptr) -> JFIF YCbCr -> libjpeg's
+// h2v2_downsample (jcsample.c): one thread per 2 x 2 destination block, whose chroma sample never leaves registers.
+// An odd last column / row is replicated (expand_right_edge, jcsample.c; expand_bottom_edge, jcprepct.c), and the
+// downsampling bias is 1 on even and 2 on odd chroma columns, restarting on every row.
+__global__ void __launch_bounds__(256) k_bgr_to_ycc420(const uint8_t *__restrict__ src, size_t src_pitch, int sw, int sh,
+                                                       int dw, int dh, const ResizeTap *__restrict__ xt,
+                                                       const ResizeTap *__restrict__ yt, uint8_t *__restrict__ yp, size_t y_pitch,
+                                                       uint8_t *__restrict__ cbp, uint8_t *__restrict__ crp, size_t c_pitch) {
+    const int cx = blockIdx.x * 32 + threadIdx.x, cy = blockIdx.y * 8 + threadIdx.y;
+    if (cx >= (dw + 1) >> 1 || cy >= (dh + 1) >> 1) return;
+    int sum_cb = 0, sum_cr = 0;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+        const int y = min(2 * cy + j, dh - 1);
+        const uint8_t *r0, *r1 = nullptr;
+        ResizeTap ty{};
+        if (xt) {
+            ty = yt[y];
+            r0 = resize_row(src, src_pitch, sh, ty.idx);
+            r1 = resize_row(src, src_pitch, sh, ty.idx + 1);
+        } else {
+            r0 = src + (size_t)y * src_pitch;
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int x = min(2 * cx + i, dw - 1);
+            int bgr[3];
+            if (xt) {
+                const ResizeTap tx = xt[x];
+                const int i0 = 3 * tx.idx, i1 = 3 * min(tx.idx + 1, sw - 1);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) bgr[c] = resize_sample(r0, r1, i0 + c, i1 + c, tx, ty);
+            } else {
+#pragma unroll
+                for (int c = 0; c < 3; ++c) bgr[c] = r0[3 * x + c];
+            }
+            int Y, Cb, Cr;
+            bgr_to_ycc(bgr[0], bgr[1], bgr[2], Y, Cb, Cr);
+            if (2 * cx + i < dw && 2 * cy + j < dh) yp[(size_t)(2 * cy + j) * y_pitch + 2 * cx + i] = (uint8_t)Y;
+            sum_cb += Cb;
+            sum_cr += Cr;
+        }
+    }
+    const int bias = 1 + (cx & 1);
+    cbp[(size_t)cy * c_pitch + cx] = (uint8_t)((sum_cb + bias) >> 2);
+    crp[(size_t)cy * c_pitch + cx] = (uint8_t)((sum_cr + bias) >> 2);
 }
 
 }  // namespace
@@ -70,6 +137,13 @@ void launch_bgr_to_gray(const uint8_t *bgr, size_t bgr_pitch, int w, int h, uint
 void launch_resize_u8(const uint8_t *src, size_t src_pitch, int sw, int sh, uint8_t *dst, size_t dst_pitch, int dw, int dh,
                       const ResizeTap *xt, const ResizeTap *yt, cudaStream_t s) {
     k_resize_u8<<<dim3(ceil_div(dw, 32), ceil_div(dh, 8)), dim3(32, 8), 0, s>>>(src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, xt, yt);
+    DFB_KERNEL_CHECK();
+}
+
+void launch_bgr_to_ycc420(const uint8_t *bgr, size_t bgr_pitch, int sw, int sh, int dw, int dh, const ResizeTap *xt, const ResizeTap *yt,
+                          uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, cudaStream_t s) {
+    k_bgr_to_ycc420<<<dim3(ceil_div(ceil_div(dw, 2), 32), ceil_div(ceil_div(dh, 2), 8)), dim3(32, 8), 0, s>>>(
+        bgr, bgr_pitch, sw, sh, dw, dh, xt, yt, y, y_pitch, cb, cr, c_pitch);
     DFB_KERNEL_CHECK();
 }
 

@@ -195,6 +195,47 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
                                uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y);
 
 /*
+ * ---- frame-extraction mode (`-s=0`, the reference CLI's default) ------------------------------------------------------
+ * DenseFlow::extract_frames_video (src/denseflow_gpu.cpp:82-144) resizes each decoded colour frame with
+ * cv::resize(frame, size) [INTER_LINEAR, CV_8UC3] (:146-177), encodes it with imencode(".jpg") [OpenCV defaults: quality
+ * 95, libjpeg YCbCr 4:2:0] and writes img_%05d.jpg (src/common.cpp:73-82).  These calls do the resize and the encode on the
+ * GPU and work on either kind of handle; the destination must fit the handle's max_width x max_height (DFB_ERR_SIZE),
+ * dst 0 / 0 means no resize, and quality is 1..100.
+ *
+ * dfb_bgr_to_ycc420_device: the colour preparation alone, on device buffers.  bgr: packed 8-bit BGR (src_width x
+ * src_height, row pitch in bytes).  Writes y (dst_width x dst_height) and cb, cr (ceil(dst_width / 2) x ceil(dst_height / 2),
+ * sharing c_pitch): the resize is bit-exact to OpenCV's CPU fixed-point arithmetic per channel, the colour conversion is
+ * libjpeg's rgb_ycc_convert and the 2 x 2 chroma downsampling libjpeg's h2v2_downsample with its alternating 1 / 2 bias and
+ * last-column / last-row replication at odd sizes — exactly the samples libjpeg hands to its forward DCT.  Asynchronous.
+ */
+int dfb_bgr_to_ycc420_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int src_width, int src_height, int dst_width,
+                             int dst_height, uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, void *stream);
+/*
+ * Capacity for one colour JPEG of width x height: 2 bytes per sample of the image padded to 16 x 16 MCUs (1.5 samples per
+ * pixel) + 4096.  It holds for i.i.d. noise at quality 100; content built to defeat the Huffman tables can exceed it, and a
+ * bitstream larger than the capacity passed to the calls below fails cleanly with the needed length in the message.
+ */
+size_t dfb_jpeg_max_bytes_bgr(int width, int height);
+/*
+ * One frame: resize + imencode(".jpg", frame) of a BGR frame in device memory.  Baseline, standard Huffman tables, YCbCr
+ * 4:2:0; out is a host buffer of out_capacity bytes, *out_len receives the length.  The work is enqueued on `stream` and
+ * the call blocks until the bitstream is on the host.  Not byte-identical to libjpeg (only the DCT and the padding of the
+ * edge MCUs differ; the reference pins no bytes).
+ */
+int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int src_width, int src_height, int dst_width,
+                               int dst_height, int quality, uint8_t *out, size_t out_capacity, size_t *out_len, void *stream);
+/*
+ * The batch of extract_frames_video: bgr[n_frames] host pointers (pageable or pinned) to dense packed BGR frames of
+ * src_width x src_height.  Frame i's bitstream goes to jpg[i] (host buffers of `capacity` bytes each,
+ * dfb_jpeg_max_bytes_bgr(dst) is the documented size) and its length to len[i], in order, for the host to write as
+ * img_%05d.jpg.  Uploads, colour preparation, encodes and bitstream read-back of successive groups of frames overlap; the host
+ * synchronises once per group.  Gives the bytes dfb_encode_jpeg_bgr_device gives frame by frame.  Blocks until every
+ * bitstream is on the host; n_frames == 0 is a no-op.
+ */
+int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int src_width, int src_height, int dst_width,
+                            int dst_height, int quality, uint8_t *const *jpg, size_t capacity, size_t *len);
+
+/*
  * Test hook: run ONE stand-alone TV-L1 kernel on dense host planes (w*h floats each, uploaded into the engine's pitched
  * layout, downloaded after the launch) so each kernel can be checked against the oracle's building block:
  *   "gradient"      in {I}                                   out {Ix, Iy}
