@@ -16,7 +16,6 @@ LIB_PATHS = {
     "fb4": os.path.join(_HERE, "lib", "libdenseflow_b200_fb4.so"),
     "fb3": os.path.join(_HERE, "lib", "libdenseflow_b200_fb3.so"),
     "hx6": os.path.join(_HERE, "lib", "libdenseflow_b200_hx6.so"),
-    "mB": os.path.join(_HERE, "lib", "libdenseflow_b200_mB.so"),
 }
 
 DFB_OK = 0

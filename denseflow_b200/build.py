@@ -26,8 +26,6 @@ VARIANTS = {
     "t512": ("libdenseflow_b200_t512.so", ["-DDFB_FUSED_THREADS=512"]),
     "fb4": ("libdenseflow_b200_fb4.so", ["-DDFB_FARN_TMA_MINB=4"]),  # Farneback TMA kernel at 4 CTAs / SM (64 registers)
     "fb3": ("libdenseflow_b200_fb3.so", ["-DDFB_FARN_TMA_MINB=3"]),
-    # arithmetic experiments of the TV-L1 inner loop (default build only differs by these flags)
-    "mB": ("libdenseflow_b200_mB.so", ["-DDFB_TWO_RCP"]),  # two reciprocals per pixel in the dual step instead of the shared one
     "hx6": ("libdenseflow_b200_hx6.so", ["-DDFB_FARN_HX=6"]),  # Farneback window without the 32-byte origin alignment
 }
 

@@ -262,9 +262,9 @@ __device__ __forceinline__ void wait_ge(const volatile int *flag, int v) {
         asm volatile("ld.acquire.cta.shared.b32 %0, [%1];" : "=r"(x) : "r"(addr) : "memory");
     } while (x - v < 0);
 }
-__device__ __forceinline__ void signal(volatile int *flag, int v) {
+__device__ __forceinline__ void signal(volatile int *flag, int v, int lane) {
     __syncwarp();
-    if ((threadIdx.x & 31) == 0)  // release store: this warp's rows (ordered before by __syncwarp) are visible before the counter
+    if (lane == 0)  // release store: this warp's rows (ordered before by __syncwarp) are visible before the counter
         asm volatile("st.release.cta.shared.b32 [%0], %1;" ::"r"(smem_u32(const_cast<const int *>(flag))), "r"(v) : "memory");
 }
 
@@ -281,6 +281,7 @@ struct TileCtx {
     bool lane_in;     // ERR: this lane's pixels lie in the interior columns of the tile
     int ry_lo, ry_hi, rows_left;  // ERR: interior rows of the tile, image rows below gy0
     int cols_left;    // ERR: image columns from gx0 (pixel j counts if j < cols_left)
+    int halo_top, halo_bot;  // 1 if the region's top / bottom edge is halo (not the image border), else 0
 };
 
 // One primal + dual iteration of a tile visit.  EDGE: the tile contains the last image column or row (mirror handling
@@ -294,11 +295,28 @@ struct TileCtx {
 // dependencies, so with "all primal, then all dual" every warp of the SM sat in the same phase and the two pipes took
 // turns idling).  It also shortens the cross-warp chain: the warp above needs only this warp's P0 for its D3, and this
 // warp's next P0 needs only the D3 of the warp above.
+//
+// Dead halo rows.  Counted from a region edge that is halo, iteration `it` of a visit needs the primal step only on tile
+// rows [it+1, TH-it) and the dual step only on [it+1, TH-it-1): nothing outside can reach a pixel that is kept after the
+// last iteration.  A warp whose whole row block lies outside skips the arithmetic of the iteration but keeps its waits and
+// signals, so the protocol is the one above; its stale u and p rows feed only dead rows of its neighbours (the p_bot row a
+// live warp below needs was written in the warp's last live iteration).  The waits matter beyond the iteration: without a
+// CTA-wide barrier between tiles (no TMA), they keep a dead warp from moving on and overwriting its rows of the next tile
+// while its neighbours still read them.
 template <bool EDGE, bool ERR>
 __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const Tvl1Consts &c, int it, float4 (&p11)[RPT], float4 (&p12)[RPT],
                                                float4 (&p21)[RPT], float4 (&p22)[RPT], float &err) {
     volatile int *prog = sm.prog;
     const int so0 = t.so0, lane = t.lane, wq = t.wq;
+    if (RPT * wq + RPT - 1 < t.halo_top * (it + 1) || RPT * wq >= TH - t.halo_bot * it) {
+        if (wq > 0 && t.flagsync) wait_ge(&prog[wq - 1], t.base + 2 * it);
+        signal(&prog[wq], t.base + 2 * it + 1, lane);
+        if (!t.flagsync) __syncthreads();
+        if (wq < kWarps - 1 && t.flagsync) wait_ge(&prog[wq + 1], t.base + 2 * it + 1);
+        signal(&prog[wq], t.base + 2 * it + 2, lane);
+        if (!t.flagsync) __syncthreads();
+        return;
+    }
     // p above the region's first row: the image border (p = 0) for tile row 0, halo garbage otherwise
     float4 up12 = zero4(), up22 = zero4();
     if (wq > 0) {
@@ -347,7 +365,7 @@ __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const
         st4(&sm.u[0][so], n1);
         st4(&sm.u[1][so], n2);
         if (r == 0) {
-            signal(&prog[wq], t.base + 2 * it + 1);  // row 0 of the new u is what the warp above waits for
+            signal(&prog[wq], t.base + 2 * it + 1, lane);  // row 0 of the new u is what the warp above waits for
             if (!t.flagsync) __syncthreads();
         } else {
             // -------- dual, row r-1: p <- (p + taut * grad u) / (1 + taut * |grad u|) ------------
@@ -382,7 +400,7 @@ __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const
     }
     st4(&sm.p_bot[0][wq][4 * lane], p12[RPT - 1]);
     st4(&sm.p_bot[1][wq][4 * lane], p22[RPT - 1]);
-    signal(&prog[wq], t.base + 2 * it + 2);
+    signal(&prog[wq], t.base + 2 * it + 2, lane);
     if (!t.flagsync) __syncthreads();
 }
 
@@ -507,11 +525,13 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     t.ry_hi = TH - hy + (ry0 + TH >= H ? hy : 0);
     t.rows_left = H - gy0;
     t.cols_left = W - gx0;
+    t.halo_top = t.ry_lo > 0;
+    t.halo_bot = t.ry_hi < TH;
 
     // make row RPT-1 of p12/p22 visible to the warp below before the first primal step
     st4(&sm.p_bot[0][wq][4 * lane], p12[RPT - 1]);
     st4(&sm.p_bot[1][wq][4 * lane], p22[RPT - 1]);
-    signal(&prog[wq], base);
+    signal(&prog[wq], base, lane);
     if (!flagsync) __syncthreads();
     if (prof_on) {
         const unsigned long long tt = gtime();
