@@ -95,7 +95,12 @@ SIGNATURES = {
                                              C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]),
     "dfb_extract_frames_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
-    "dfb_debug_run_kernel": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int,
+    "dfb_png_max_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "dfb_encode_png_bgr_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
+                                            C.POINTER(C.c_size_t), C.c_void_p]),
+    "dfb_calc_batch_host_png": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                          C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_debug_run_kernel":(C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int,
                                        C.c_int, C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_double)]),
     "dfb_debug_time_kernel": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]),
     "dfb_get_tvl1_stats": (C.c_int, [C.c_void_p, C.POINTER(Tvl1Stats)]),

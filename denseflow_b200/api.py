@@ -289,6 +289,41 @@ class DenseOpticalFlow:
         self._check(self._L.dfb_extract_frames_host(self._h, fp, n, sw, sh, dw, dh, int(quality), op, cap, lens))
         return [bufs[i][:lens[i]].tobytes() for i in range(n)]
 
+    # -- -st=png: imencode(".png") on the GPU, byte-identical to OpenCV's default PNG parameters (src/common.cpp:66-71) --
+    def encode_png_bgr_device(self, bgr, capacity=None):
+        """imencode(".png", bgr) of a uint8 [H,W,3] BGR CUDA tensor (rows may be pitched), on the GPU.  Returns the bytes."""
+        import torch
+        w, h = self._bgr_device(bgr)
+        cap = self._L.dfb_png_max_bytes(w, h) if capacity is None else int(capacity)
+        buf = np.empty(max(cap, 1), np.uint8)
+        n = C.c_size_t()
+        s = torch.cuda.current_stream(bgr.device).cuda_stream
+        self._check(self._L.dfb_encode_png_bgr_device(self._h, bgr.data_ptr(), bgr.stride(0), w, h, buf.ctypes.data, cap, C.byref(n),
+                                                      C.c_void_p(s)))
+        return buf[:n.value].tobytes()
+
+    def calc_batch_png(self, frames, step=1, out=None):
+        """frames: sequence of uint8 [H,W] host arrays (or one [N,H,W] array).  Returns, for each of the M = max(N-|step|,0)
+        pairs, the PNG file writeFlowImagesPng writes: imencode(".png", convertFlowToPngImage(flow)).  out: optional list of
+        M uint8 host buffers (e.g. page-locked) of dfb_png_max_bytes(W, H) bytes or more to encode into."""
+        frames = self._gray_frames(frames)
+        n = len(frames)
+        if n == 0:
+            return []
+        h, w = frames[0].shape
+        m = max(n - abs(step), 0)
+        cap = self._L.dfb_png_max_bytes(w, h)
+        if out is None:
+            out = [np.empty(cap, np.uint8) for _ in range(m)]
+        if len(out) < m or any(not isinstance(b, np.ndarray) or b.dtype != np.uint8 or b.ndim != 1 or b.size < cap
+                               or not b.flags.c_contiguous for b in out[:m]):
+            raise RuntimeError("out: expected %d C-contiguous uint8 buffers of at least %d bytes" % (m, cap))
+        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
+        op = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in out[:m]])
+        lens = (C.c_size_t * max(m, 1))()
+        self._check(self._L.dfb_calc_batch_host_png(self._h, fp, n, step, w, h, op, cap, lens))
+        return [out[i][:lens[i]].tobytes() for i in range(m)]
+
     # -- test hook: one stand-alone kernel on host planes --
     def debug_run_kernel(self, kernel, inputs, n_out, scalars=(), out_shape=None, all_scalars=False):
         """returns (output planes, scalars_out[0]), or with all_scalars (output planes, scalars_out[:16])"""

@@ -10,6 +10,7 @@
 
 #include "engine.h"
 #include "jpeg.h"
+#include "png_encode.h"
 #include "png_pack.h"
 #include "preproc.h"
 #include "tvl1.cuh"
@@ -53,6 +54,10 @@ struct dfb_handle {
     uint8_t *dec_bgr = nullptr;  // BGR scratch of dfb_decode_jpeg_gray_device
     size_t dec_bgr_cap = 0;
     void *png_scratch = nullptr;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
+    std::unique_ptr<PngEncoder> png;  // imencode(".png") workspace and files, created on first use
+    uint8_t *png_bgr = nullptr;       // packed images of dfb_calc_batch_host_png, one per flow ring slot
+    size_t png_bgr_cap = 0;
+    uint64_t *png_lens_host = nullptr;  // pinned file lengths of the two groups in flight
     TapTable gray_taps;  // dfb_resize_gray_device
     // scratch of the frame-extraction calls (-s=0), grown on demand
     TapTable ycc_taps;                          // colour resize of all three calls
@@ -247,10 +252,25 @@ void ensure_flow_ring(dfb_handle *h, int n, bool quantised) {
     }
 }
 
+void ensure_png_scratch(dfb_handle *h) {
+    if (h->png_scratch) return;
+    DFB_CUDA(cudaMalloc(&h->png_scratch, png_pack_scratch_bytes()));
+    DFB_CUDA(cudaMemset(h->png_scratch, 0, png_pack_scratch_bytes()));
+    DFB_CUDA(cudaDeviceSynchronize());
+}
+
+// PNG output of batch_host (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j]
+struct PngSink {
+    uint8_t *const *out;
+    size_t capacity;
+    size_t *len;
+};
+
 // The batch shape of calc_optflows_imp (src/denseflow_gpu.cpp:307-342) over host buffers.
 // quantise: bound > 0 => emit two u8 planes per pair instead of the float2 field.
+// png: non-null => pack every flow field (convertFlowToPngImage) and emit imencode(".png") of it instead of the field.
 int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, float *const *flows,
-               int bound, uint8_t *const *qx, uint8_t *const *qy) {
+               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngSink *png = nullptr) {
     if (int rc = check_size(h, w, hh)) return rc;
     if (n_frames < 0 || !frames) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
@@ -261,7 +281,8 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
         if (!frames[f] || host_pointer_kind(frames[f]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "frames[" + std::to_string(f) + "] is null or a device pointer (host entry point: use dfb_calc_batch_device)");
     for (int j = 0; j < M; ++j) {
-        const void *o0 = bound > 0 ? (const void *)qx[j] : (const void *)flows[j], *o1 = bound > 0 ? (const void *)qy[j] : o0;
+        const void *o0 = png ? (const void *)png->out[j] : bound > 0 ? (const void *)qx[j] : (const void *)flows[j];
+        const void *o1 = bound > 0 ? (const void *)qy[j] : o0;
         if (!o0 || !o1 || host_pointer_kind(o0) < 0 || host_pointer_kind(o1) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
     }
@@ -279,6 +300,30 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
     ensure_flow_ring(h, OR, bound > 0);
     double fused_flag = 1;
     if (bound > 0 && alg.get_param("fused", &fused_flag) && fused_flag == 0) ensure_flow_ring(h, OR, false);
+    const size_t bgr_bytes = fbytes * 3;
+    if (png) {
+        if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
+        ensure_png_scratch(h);
+        grow_device(h->png_bgr, h->png_bgr_cap, OR * bgr_bytes);
+        if (!h->png_lens_host) DFB_CUDA(cudaHostAlloc(&h->png_lens_host, sizeof(uint64_t) * dfb_handle::kFlowRing, cudaHostAllocDefault));
+        if (!h->png) h->png.reset(new PngEncoder());
+    }
+    // -st=png: the files of group g (slot g & 1) are read back while the GPU works on group g + 1
+    auto png_finish = [&](int g) {
+        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
+        DFB_CUDA(cudaEventSynchronize(h->ev_out[(j0 + m - 1) % OR]));
+        for (int i = 0; i < m; ++i) {
+            const size_t n = (size_t)h->png_lens_host[slot * B + i];
+            if (n == 0) throw std::runtime_error("png encoder failed on pair " + std::to_string(j0 + i));
+            if (n > png->capacity)
+                throw std::runtime_error("png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) +
+                                         " bytes, capacity is " + std::to_string(png->capacity));
+            png->len[j0 + i] = n;
+            DFB_CUDA(cudaMemcpyAsync(png->out[j0 + i], h->png->file(slot, i), n, cudaMemcpyDeviceToHost, h->s_fetch));
+            h->counters.d2h_bytes += n;
+        }
+        DFB_CUDA(cudaStreamSynchronize(h->s_fetch));
+    };
 
     int uploaded = 0;  // frames [0, uploaded) have H2D + pyramid enqueued
     auto upload_until = [&](int last) {
@@ -352,6 +397,25 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
             }
         }
         alg.solve_batch(jobs.data(), m, w, hh, h->s_compute);
+        if (png) {
+            // s_compute: convertFlowToPngImage of every pair (src/common.cpp:18-46); s_out: imencode(".png") of the group
+            // (:66-71); s_fetch: the previous group's files to the host
+            const int r0 = j0 % OR, g = j0 / B, slot = g & 1;
+            uint8_t *bgr0 = h->png_bgr + (size_t)r0 * bgr_bytes;
+            for (int i = 0; i < m; ++i)
+                launch_flow_to_png_image(h->d_flow[r0 + i], (size_t)w * 8, w, hh, bgr0 + (size_t)i * bgr_bytes, (size_t)w * 3, h->png_scratch,
+                                         nullptr, h->s_compute);
+            alg.launches += 2 * m;
+            DFB_CUDA(cudaEventRecord(h->ev_done[r0], h->s_compute));
+            DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[r0], 0));
+            alg.launches += h->png->encode(m, bgr0, bgr_bytes, (size_t)w * 3, w, hh, slot, h->s_out);
+            DFB_CUDA(cudaMemcpyAsync(h->png_lens_host + slot * B, h->png->lens(slot), sizeof(uint64_t) * m, cudaMemcpyDeviceToHost, h->s_out));
+            for (int i = 0; i < m; ++i) DFB_CUDA(cudaEventRecord(h->ev_out[r0 + i], h->s_out));
+            h->counters.pairs += m;
+            if (g > 0) png_finish(g - 1);
+            if (j0 + m == M) png_finish(g);
+            continue;
+        }
         DFB_CUDA(cudaEventRecord(h->ev_done[j0 % OR], h->s_compute));
         DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[j0 % OR], 0));
         for (int i = 0; i < m; ++i) {
@@ -461,6 +525,9 @@ void dfb_destroy(dfb_handle *h) {
     for (auto e : h->ex_events)
         if (e) cudaEventDestroy(e);
     if (h->png_scratch) cudaFree(h->png_scratch);
+    h->png.reset();
+    if (h->png_bgr) cudaFree(h->png_bgr);
+    if (h->png_lens_host) cudaFreeHost(h->png_lens_host);
     if (h->dec_bgr) cudaFree(h->dec_bgr);
     for (auto e : h->pb_events) cudaEventDestroy(e);
     if (h->s_fetch) cudaStreamDestroy(h->s_fetch);
@@ -619,11 +686,7 @@ int dfb_flow_to_png_image_device(dfb_handle *h, const float *flow_xy, size_t flo
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
-        if (!h->png_scratch) {
-            DFB_CUDA(cudaMalloc(&h->png_scratch, png_pack_scratch_bytes()));
-            DFB_CUDA(cudaMemset(h->png_scratch, 0, png_pack_scratch_bytes()));
-            DFB_CUDA(cudaDeviceSynchronize());
-        }
+        ensure_png_scratch(h);
         PngBounds *bd = nullptr;
         launch_flow_to_png_image(flow_xy, flow_pitch, width, height, bgr, bgr_pitch, h->png_scratch, &bd, s);
         h->alg->launches += 2;
@@ -1016,6 +1079,47 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
         DFB_CUDA(cudaStreamSynchronize(h->s_compute));
         DFB_CUDA(cudaStreamSynchronize(h->s_out));
         return DFB_OK;
+    });
+}
+
+size_t dfb_png_max_bytes(int width, int height) { return png_max_bytes(width, height); }
+
+int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int width, int height, uint8_t *out, size_t out_capacity,
+                              size_t *out_len, void *stream) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!bgr || !out || !out_len) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    if (width <= 0 || height <= 0 || bgr_pitch < (size_t)width * 3) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    if (int rc = check_size(h, width, height)) return rc;
+    if (!is_device_pointer(bgr)) return fail(h, DFB_ERR_INVALID_ARG, "bgr must be device memory (device entry point)");
+    if (host_pointer_kind(out) < 0) return fail(h, DFB_ERR_INVALID_ARG, "out must be host memory");
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (!h->png) h->png.reset(new PngEncoder());
+        h->alg->launches += h->png->encode(1, bgr, 0, bgr_pitch, width, height, 0, s);
+        uint64_t len = 0;
+        DFB_CUDA(cudaMemcpyAsync(&len, h->png->lens(0), sizeof(len), cudaMemcpyDeviceToHost, s));
+        DFB_CUDA(cudaStreamSynchronize(s));
+        if (len == 0) throw std::runtime_error("png encoder failed");
+        if (len > out_capacity)
+            throw std::runtime_error("png output buffer too small: the file needs " + std::to_string(len) + " bytes, capacity is " +
+                                     std::to_string(out_capacity));
+        DFB_CUDA(cudaMemcpyAsync(out, h->png->file(0, 0), len, cudaMemcpyDeviceToHost, s));
+        DFB_CUDA(cudaStreamSynchronize(s));
+        h->counters.d2h_bytes += len;
+        *out_len = (size_t)len;
+        return DFB_OK;
+    });
+}
+
+int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height, uint8_t *const *png,
+                            size_t capacity, size_t *len) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (n_frames > std::abs(step) && (!png || !len)) return fail(h, DFB_ERR_INVALID_ARG, "png / len is null");
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        const PngSink sink{png, capacity, len};
+        return batch_host(h, frames, n_frames, step, width, height, nullptr, 0, nullptr, nullptr, &sink);
     });
 }
 

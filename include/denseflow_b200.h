@@ -236,6 +236,36 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
                             int dst_height, int quality, uint8_t *const *jpg, size_t capacity, size_t *len);
 
 /*
+ * ---- PNG flow images (-st=png) ---------------------------------------------------------------------------------------
+ * encodeFlowMapPng (src/common.cpp:66-71) writes imencode(".png", img) of the packed image convertFlowToPngImage builds.
+ * These calls run that encode on the GPU and return EXACTLY the bytes of cv2.imencode(".png", img) with OpenCV's default
+ * PNG parameters: filter SUB on every row (NONE when the width is 1), zlib level 1 (Z_BEST_SPEED) with strategy Z_RLE, the
+ * window libpng declares for the data size, and IDAT chunks of 8192 bytes of zlib stream.  An OpenCV built with other
+ * defaults, or a caller that passes IMWRITE_PNG_* parameters, gets other (equally valid) bytes.  Integer-only: both builds
+ * give the same bytes.  They work on either kind of handle; the image must fit the handle's max_width x max_height.
+ *
+ * dfb_png_max_bytes: an upper bound on the file size of a width x height image (every deflate block stored, plus the zlib
+ * and PNG framing).  A pure function; needs no device.
+ */
+size_t dfb_png_max_bytes(int width, int height);
+/*
+ * imencode(".png", img) of one packed 8-bit BGR image in device memory (rows bgr_pitch bytes apart).  out: host buffer of
+ * out_capacity bytes, *out_len receives the length.  Enqueued on `stream`; blocks until the file is on the host.  A file
+ * larger than out_capacity fails with the needed length in the message and writes nothing.
+ */
+int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int width, int height, uint8_t *out,
+                              size_t out_capacity, size_t *out_len, void *stream);
+/*
+ * The -st=png branch of encode_save (src/denseflow_gpu.cpp:442-453) over host frames: for each of the M = max(n_frames -
+ * |step|, 0) pairs, selected as dfb_calc_batch_host selects them, flow -> convertFlowToPngImage -> imencode(".png").
+ * png[j] (host buffers of `capacity` bytes each, dfb_png_max_bytes is always enough) receives exactly what
+ * writeFlowImagesPng writes for pair j, len[j] its length.  Flow and packing, the encodes and the read-back of successive
+ * groups of pairs overlap; the host synchronises once per group.  Blocks until every file is on the host.
+ */
+int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
+                            uint8_t *const *png, size_t capacity, size_t *len);
+
+/*
  * Test hook: run ONE stand-alone TV-L1 kernel on dense host planes (w*h floats each, uploaded into the engine's pitched
  * layout, downloaded after the launch) so each kernel can be checked against the oracle's building block:
  *   "gradient"      in {I}                                   out {Ix, Iy}
