@@ -43,6 +43,13 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const void *tmap, in
                  "l"(tmap), "r"(x), "r"(y), "r"(smem_u32(bar))
                  : "memory");
 }
+// tma_load_2d with an L2 cache policy (createpolicy) for the lines it reads
+__device__ __forceinline__ void tma_load_2d_hint(void *smem_dst, const void *tmap, int x, int y, unsigned long long *bar, unsigned long long pol) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(
+                     smem_u32(smem_dst)),
+                 "l"(tmap), "r"(x), "r"(y), "r"(smem_u32(bar)), "l"(pol)
+                 : "memory");
+}
 // Asks the TMA unit to bring a tile into L2 only (no shared-memory destination, no completion to wait for)
 __device__ __forceinline__ void tma_prefetch_l2_2d(const void *tmap, int x, int y) {
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(x), "r"(y) : "memory");

@@ -11,7 +11,7 @@
 // at a time: lane l of warp q owns pixels x = 4l..4l+3 of rows 4q..4q+3.  The four dual planes
 // (p11,p12,p21,p22) live in registers; u1,u2 and the four per-warp constants (I1wx,I1wy,grad,rho_c)
 // live in shared memory (192 KB), staged there by TMA (cp.async.bulk.tensor.2d + mbarrier, zero
-// fill outside the image) while the threads load the dual planes.  Horizontal neighbours come
+// fill outside the image; each warp its own rows) while the threads load the dual planes.  Horizontal neighbours come
 // from warp shuffles, vertical neighbours from the thread's own rows, the shared u tile, or a
 // one-row shared-memory exchange of p12/p22 between adjacent warps.  k primal+dual iterations run
 // on chip per tile visit (halo = k, the valid region shrinks by one pixel per iteration, exactly
@@ -65,13 +65,36 @@ struct Smem {
     int ibcast[4];
     unsigned long long prof[32];
     int prog[kWarps];  // per-warp progress counters of the tile loop (see process_tile)
-    unsigned long long tma_bar;  // mbarrier the TMA tile loads complete on
+    unsigned long long tma_bar[kWarps];  // per warp: the mbarrier the TMA loads of its rows complete on
+    int4 next[kWarps];  // per warp, lane 0 only: {x, y (< 0: none), level} of the CTA's next tile in the chunk; kept here rather
+                        // than in registers across the tile loop, where they made ptxas spill
     FusedJob job;                // this lane's job description (copied from the device-memory ring at kernel start)
 };
 
 __device__ __forceinline__ float4 ld_cg4(const float *p) { return __ldcg(reinterpret_cast<const float4 *>(p)); }
 __device__ __forceinline__ void st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
 __device__ __forceinline__ float4 zero4() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+// The tile loads (TMA and the dual planes) and the write-back stores leave their lines first in line for eviction from L2, so
+// they do not push out the lines the L2 prefetch of the CTAs' next tiles brought in: a tile's planes are read once per chunk
+// (its halo by the neighbouring tiles, which run at the same time), and the planes written back are read in the next chunk,
+// by when a level's working set has long left the L2.
+__device__ __forceinline__ unsigned long long l2_evict_first_policy() {
+    unsigned long long pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void st4_evict_first(float *p, float4 v, unsigned long long pol) {
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
+                 "f"(v.w), "l"(pol)
+                 : "memory");
+}
+__device__ __forceinline__ float4 ld_cg4_hint(const float *p, unsigned long long pol) {
+    float4 v;
+    asm volatile("ld.global.cg.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                 : "l"(p), "l"(pol));
+    return v;
+}
 
 __device__ __forceinline__ unsigned long long gtime() {
     unsigned long long t;
@@ -300,9 +323,9 @@ struct TileCtx {
 // rows [it+1, TH-it) and the dual step only on [it+1, TH-it-1): nothing outside can reach a pixel that is kept after the
 // last iteration.  A warp whose whole row block lies outside skips the arithmetic of the iteration but keeps its waits and
 // signals, so the protocol is the one above; its stale u and p rows feed only dead rows of its neighbours (the p_bot row a
-// live warp below needs was written in the warp's last live iteration).  The waits matter beyond the iteration: without a
-// CTA-wide barrier between tiles (no TMA), they keep a dead warp from moving on and overwriting its rows of the next tile
-// while its neighbours still read them.
+// live warp below needs was written in the warp's last live iteration).  The waits matter beyond the iteration: no CTA-wide
+// barrier separates two tiles (see process_tile), so they keep a dead warp from moving on and overwriting its rows of the
+// next tile while its neighbours still read them.
 template <bool EDGE, bool ERR>
 __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const Tvl1Consts &c, int it, float4 (&p11)[RPT], float4 (&p12)[RPT],
                                                float4 (&p21)[RPT], float4 (&p22)[RPT], float &err) {
@@ -414,9 +437,43 @@ __device__ __forceinline__ float tile_iterations(Smem &sm, const TileCtx &t, con
     return err;
 }
 
+__device__ __forceinline__ const char *level_maps(const FusedJob &job, int level) {
+    return static_cast<const char *>(job.tmaps) + (size_t)level * kFusedMapsPerLevel * kTensorMapBytes;
+}
+
+// TMA staging of one warp's rows (issued by its lane 0; box 128 x RPT, zero fill outside the image), completing on the warp's
+// mbarrier.  The four constant planes go first, with the expect_tx of all six, and u1,u2 later: the planes were written with
+// plain stores by other CTAs of the lane (previous chunk / warp phase) and published by a grid barrier this thread has passed,
+// so each issue first orders those generic-proxy writes before its async-proxy reads.
+__device__ __forceinline__ void tma_warp_consts(Smem &sm, const char *maps, int rx0, int ry0, int wq) {
+    const int r0 = RPT * wq;
+    fence_proxy_async_global();
+    mbar_expect_tx(&sm.tma_bar[wq], 6u * TW * RPT * (unsigned)sizeof(float));
+#pragma unroll
+    const unsigned long long pol = l2_evict_first_policy();
+    for (int k = 0; k < 4; ++k) tma_load_2d_hint(&sm.consts[k][r0 * TW], maps + k * kTensorMapBytes, rx0, ry0 + r0, &sm.tma_bar[wq], pol);
+}
+__device__ __forceinline__ void tma_warp_u(Smem &sm, const char *maps, int cur, int rx0, int ry0, int wq) {
+    const int r0 = RPT * wq;
+    fence_proxy_async_global();
+    const unsigned long long pol = l2_evict_first_policy();
+    tma_load_2d_hint(&sm.u[0][r0 * TW], maps + (4 + 2 * cur) * kTensorMapBytes, rx0, ry0 + r0, &sm.tma_bar[wq], pol);
+    tma_load_2d_hint(&sm.u[1][r0 * TW], maps + (5 + 2 * cur) * kTensorMapBytes, rx0, ry0 + r0, &sm.tma_bar[wq], pol);
+}
+
+// Tile hand-over.  Every warp loads only its own rows and moves to the next tile of the chunk on its own; no CTA-wide barrier
+// separates two tiles.  Who reads a warp's rows of the shared-memory planes:
+// * constants: the owning thread only (primal steps).  Once a warp's iterations are done they are dead, so while the warp
+//   writes back it already stages the constants of its next tile (first_in_chunk: staged at the start of the visit instead;
+//   no load crosses the grid barrier that ends a chunk).
+// * u: the warp itself, and the warp above reads row 0 in its last dual row.  The u load of the next tile therefore waits for
+//   the warp above to have finished the last dual step of this tile (counter at base - 2 of the next tile).
+// * p_bot: the warp below reads it in its first primal row, and this warp's last dual step of a visit waited for that read.
+// The warp signals `base` once its rows of the new tile are loaded; a neighbour reads them only after waiting for that
+// signal (tests/test_sync_protocol_handover_cpu.py checks both directions over every interleaving).
 __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Consts &c, const FusedLevel &L, int level, int cur, int tx, int ty,
                                               int kk, int hx, int hy, bool check, int base, unsigned tma_parity, Smem &sm,
-                                              bool prof_on, int ntx_next, int nty_next) {
+                                              bool prof_on, bool first_in_chunk, int ntx_next, int nty_next) {
     const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
     unsigned long long t0 = 0;
     if (prof_on) t0 = gtime();
@@ -426,47 +483,39 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     const int gy0 = ry0 + RPT * wq;
     volatile int *prog = sm.prog;
     const bool flagsync = job.flag_sync != 0;
+    const char *maps = level_maps(job, level);
+    const int nrx0 = ntx_next * (TW - 2 * hx), nry0 = nty_next * (TH - 2 * hy);
 
     float4 p11[RPT], p12[RPT], p21[RPT], p22[RPT];
     const int so0 = (RPT * wq) * TW + 4 * lane;  // this thread's slot in row 0 of its warp (thread-private in smem planes)
     const bool use_tma = job.use_tma != 0;
+    // The warp above reads this warp's first u row in its dual steps: it must have finished the previous tile (its counter
+    // reached base - 2 = "last dual step of the previous tile done") before the row is overwritten.  (Without flags the
+    // previous visit ended with a CTA-wide barrier.)
+    if (flagsync && wq > 0) wait_ge(&prog[wq - 1], base - 2);
     if (use_tma) {
-        // One thread stages the six shared-memory-resident planes of the tile (4 constants + u1,u2: 192 KB) with
-        // TMA while every thread loads its share of the four dual planes into registers.  All warps must be done
-        // with the previous tile's shared memory first (the bulk copy overwrites every slot).
+        // this warp's generic-proxy accesses to its rows are ordered before the async-proxy writes of the loads
         fence_proxy_async();
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            const char *maps = static_cast<const char *>(job.tmaps) + (size_t)level * kFusedMapsPerLevel * kTensorMapBytes;
-            // the planes were written with plain stores by other CTAs of the lane (previous chunk / warp phase) and published by
-            // the grid barrier this thread polled: order those generic-proxy writes before the async-proxy reads below
-            fence_proxy_async_global();
-            mbar_expect_tx(&sm.tma_bar, 6u * kConstPlane * (unsigned)sizeof(float));
-            tma_load_2d(sm.consts[0], maps + 0 * kTensorMapBytes, rx0, ry0, &sm.tma_bar);
-            tma_load_2d(sm.consts[1], maps + 1 * kTensorMapBytes, rx0, ry0, &sm.tma_bar);
-            tma_load_2d(sm.consts[2], maps + 2 * kTensorMapBytes, rx0, ry0, &sm.tma_bar);
-            tma_load_2d(sm.consts[3], maps + 3 * kTensorMapBytes, rx0, ry0, &sm.tma_bar);
-            tma_load_2d(sm.u[0], maps + (4 + 2 * cur) * kTensorMapBytes, rx0, ry0, &sm.tma_bar);
-            tma_load_2d(sm.u[1], maps + (5 + 2 * cur) * kTensorMapBytes, rx0, ry0, &sm.tma_bar);
+        __syncwarp();
+        if (lane == 0) {
+            if (first_in_chunk) tma_warp_consts(sm, maps, rx0, ry0, wq);
+            tma_warp_u(sm, maps, cur, rx0, ry0, wq);
         }
-    } else if (flagsync && wq > 0) {
-        // The warp above reads this warp's first u row in its dual steps: it must have finished the previous tile
-        // (its counter reached base - 2 = "last dual step of the previous tile done") before the row is overwritten.
-        wait_ge(&prog[wq - 1], base - 2);
     }
     {
         const float *s0 = L.u1[cur], *s1 = L.u2[cur], *s2 = job.p[cur][0], *s3 = job.p[cur][1], *s4 = job.p[cur][2],
                     *s5 = job.p[cur][3];
         const bool col_ok = gx0 < P;
+        const unsigned long long lpol = l2_evict_first_policy();
 #pragma unroll
         for (int r = 0; r < RPT; ++r) {
             const int gy = gy0 + r;
             const bool ok = col_ok && gy < H;
             const size_t o = ok ? (size_t)gy * P + gx0 : 0;
-            p11[r] = ok ? ld_cg4(s2 + o) : zero4();
-            p12[r] = ok ? ld_cg4(s3 + o) : zero4();
-            p21[r] = ok ? ld_cg4(s4 + o) : zero4();
-            p22[r] = ok ? ld_cg4(s5 + o) : zero4();
+            p11[r] = ok ? ld_cg4_hint(s2 + o, lpol) : zero4();
+            p12[r] = ok ? ld_cg4_hint(s3 + o, lpol) : zero4();
+            p21[r] = ok ? ld_cg4_hint(s4 + o, lpol) : zero4();
+            p22[r] = ok ? ld_cg4_hint(s5 + o, lpol) : zero4();
             if (!use_tma) {
                 const int so = so0 + r * TW;
                 st4(&sm.u[0][so], ok ? ld_cg4(s0 + o) : zero4());
@@ -478,19 +527,20 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
             }
         }
     }
-    if (use_tma) mbar_wait(&sm.tma_bar, tma_parity);
+    if (use_tma) mbar_wait(&sm.tma_bar[wq], tma_parity);
+    if (lane == 0) sm.next[wq] = make_int4(nrx0, ntx_next >= 0 ? nry0 : -1, level, 0);
     if (job.prefetch && ntx_next >= 0) {
         // This CTA's next tile of the chunk: ask for its ten planes to be brought into L2 now, so the copy from HBM runs
-        // under this tile's iterations (with several pairs in flight the planes of a level do not fit the L2).
-        const int nrx0 = ntx_next * (TW - 2 * hx), nry0 = nty_next * (TH - 2 * hy);
-        if (use_tma && threadIdx.x == 0) {
-            const char *maps = static_cast<const char *>(job.tmaps) + (size_t)level * kFusedMapsPerLevel * kTensorMapBytes;
-            tma_prefetch_l2_2d(maps + 0 * kTensorMapBytes, nrx0, nry0);
-            tma_prefetch_l2_2d(maps + 1 * kTensorMapBytes, nrx0, nry0);
-            tma_prefetch_l2_2d(maps + 2 * kTensorMapBytes, nrx0, nry0);
-            tma_prefetch_l2_2d(maps + 3 * kTensorMapBytes, nrx0, nry0);
-            tma_prefetch_l2_2d(maps + (4 + 2 * cur) * kTensorMapBytes, nrx0, nry0);
-            tma_prefetch_l2_2d(maps + (5 + 2 * cur) * kTensorMapBytes, nrx0, nry0);
+        // under this tile's iterations (with several pairs in flight the planes of a level do not fit the L2).  Every warp
+        // asks for its own rows.
+        if (use_tma && lane == 0) {
+            const int nry = nry0 + RPT * wq;
+            tma_prefetch_l2_2d(maps + 0 * kTensorMapBytes, nrx0, nry);
+            tma_prefetch_l2_2d(maps + 1 * kTensorMapBytes, nrx0, nry);
+            tma_prefetch_l2_2d(maps + 2 * kTensorMapBytes, nrx0, nry);
+            tma_prefetch_l2_2d(maps + 3 * kTensorMapBytes, nrx0, nry);
+            tma_prefetch_l2_2d(maps + (4 + 2 * cur) * kTensorMapBytes, nrx0, nry);
+            tma_prefetch_l2_2d(maps + (5 + 2 * cur) * kTensorMapBytes, nrx0, nry);
         }
         if ((lane & 7) == 0) {  // one lane per 128-byte line of the four dual planes
             const int ngx = nrx0 + 4 * lane;
@@ -546,21 +596,30 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
         sm.prof[6] += tt - t0;
         t0 = tt;
     }
+    if (use_tma) {  // this warp's constant rows are dead: stage its rows of the next tile under the write-back
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) {
+            const int4 n = sm.next[wq];
+            if (n.y >= 0) tma_warp_consts(sm, level_maps(job, n.z), n.x, n.y, wq);
+        }
+    }
     // -------- write the interior to the other buffer ---------------------------------------------
     {
         float *d0 = L.u1[cur ^ 1], *d1 = L.u2[cur ^ 1], *d2 = job.p[cur ^ 1][0], *d3 = job.p[cur ^ 1][1],
               *d4 = job.p[cur ^ 1][2], *d5 = job.p[cur ^ 1][3];
 #pragma unroll
+        const unsigned long long pol = l2_evict_first_policy();
         for (int r = 0; r < RPT; ++r) {
             const int ry = RPT * wq + r, gy = gy0 + r;
             if (t.lane_in && ry >= t.ry_lo && ry < t.ry_hi && gy < H) {
                 const size_t o = (size_t)gy * P + gx0;
-                st4(d0 + o, *reinterpret_cast<const float4 *>(&sm.u[0][so0 + r * TW]));
-                st4(d1 + o, *reinterpret_cast<const float4 *>(&sm.u[1][so0 + r * TW]));
-                st4(d2 + o, p11[r]);
-                st4(d3 + o, p12[r]);
-                st4(d4 + o, p21[r]);
-                st4(d5 + o, p22[r]);
+                st4_evict_first(d0 + o, *reinterpret_cast<const float4 *>(&sm.u[0][so0 + r * TW]), pol);
+                st4_evict_first(d1 + o, *reinterpret_cast<const float4 *>(&sm.u[1][so0 + r * TW]), pol);
+                st4_evict_first(d2 + o, p11[r], pol);
+                st4_evict_first(d3 + o, p12[r], pol);
+                st4_evict_first(d4 + o, p21[r], pol);
+                st4_evict_first(d5 + o, p22[r], pol);
             }
         }
     }
@@ -578,7 +637,7 @@ __device__ __forceinline__ void cta_setup(Smem &sm) {
         sm.prog[threadIdx.x] = 0;
         sm.red[threadIdx.x] = 0.0;
     }
-    if (threadIdx.x == 0) mbar_init(&sm.tma_bar, 1);
+    if (threadIdx.x < kWarps) mbar_init(&sm.tma_bar[threadIdx.x], 1);
     __syncthreads();
 }
 
@@ -594,7 +653,7 @@ __device__ __forceinline__ void run_chunk(const FusedJob &job, const Tvl1Consts 
         const int ty = t / ntx, tx = t - ty * ntx;
         const int tn = t + G;
         const int nty_n = tn < ntiles ? tn / ntx : -1, ntx_n = tn < ntiles ? tn - nty_n * ntx : -1;
-        const float e = process_tile(job, c, L, s, cur, tx, ty, kk, hx, hy, chk, tile_base, tma_parity, sm, prof_on, ntx_n, nty_n);
+        const float e = process_tile(job, c, L, s, cur, tx, ty, kk, hx, hy, chk, tile_base, tma_parity, sm, prof_on, t == bid, ntx_n, nty_n);
         tile_base += 2 * kk + 2;
         tma_parity ^= 1u;
         if (chk) {  // per-warp running sums in shared memory: no CTA-wide barrier per tile
@@ -820,7 +879,7 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_stage(const 
 }  // namespace
 
 void fused_encode_tensor_map(void *out, const float *plane, int w, int h, int pitch) {
-    encode_tensor_map_2d(out, plane, w, h, pitch, TW, TH);
+    encode_tensor_map_2d(out, plane, w, h, pitch, TW, RPT);
 }
 
 int fused_num_sms(int device) {

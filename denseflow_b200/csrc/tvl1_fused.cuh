@@ -94,7 +94,8 @@ constexpr int kFusedDefaultK = kFusedTileH >= 64 ? 8 : 4;
 
 int fused_num_sms(int device);
 inline int fused_cta_slots(int device) { return fused_num_sms(device) * kFusedCtasPerSm; }
-// Encodes one 2-D fp32 tile descriptor (box 128 x 64, no swizzle, zero fill out of bounds) into out[128 bytes].
+// Encodes one 2-D fp32 descriptor of one warp's rows of a tile (box 128 x DFB_FUSED_RPT, no swizzle, zero fill out of bounds)
+// into out[128 bytes].
 // plane: base pointer, extent w x h (elements / rows), row pitch in elements.
 void fused_encode_tensor_map(void *out, const float *plane, int w, int h, int pitch);
 // returns the number of kernels launched
