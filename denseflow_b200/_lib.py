@@ -100,6 +100,14 @@ SIGNATURES = {
                                             C.POINTER(C.c_size_t), C.c_void_p]),
     "dfb_calc_batch_host_png": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
                                           C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_decode_jpeg_batch_device": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_void_p,
+                                               C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                               C.c_void_p]),
+    "dfb_process_jpeg_batch_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
+                                              C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_size_t,
+                                              C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "dfb_debug_jpeg_coefficients": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_int),
+                                              C.POINTER(C.c_int)]),
     "dfb_debug_run_kernel":(C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p), C.c_int, C.c_int,
                                        C.c_int, C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_double)]),
     "dfb_debug_time_kernel": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]),

@@ -23,6 +23,7 @@ class DenseOpticalFlow:
         self._h = C.c_void_p()
         self.algorithm = algorithm
         self.device = device
+        self.max_width, self.max_height = max_width, max_height
         rc = self._L.dfb_create(algorithm.encode(), device, max_width, max_height, C.byref(self._h))
         if rc != _lib.DFB_OK:
             msg = self._L.dfb_last_error(None).decode()
@@ -212,6 +213,85 @@ class DenseOpticalFlow:
         self._check(self._L.dfb_decode_jpeg_gray_device(self._h, buf.ctypes.data, buf.size, out.data_ptr(), max_width, max_width, max_height,
                                                         C.byref(w), C.byref(h), C.c_void_p(s)))
         return out[:h.value, :w.value]
+
+    # -- imread(IMREAD_COLOR) [+ cvtColor(BGR2GRAY)] of `-if` frame folders on the GPU, exactly cv2.imdecode's pixels --
+    @staticmethod
+    def _jpeg_buffers(jpegs):
+        """bytes / uint8 numpy arrays / CPU uint8 torch tensors (e.g. page-locked) -> (keep-alive list, pointers, lengths)"""
+        keep, ptrs, lens = [], [], []
+        for j in jpegs:
+            if isinstance(j, (bytes, bytearray, memoryview)):
+                j = np.frombuffer(j, np.uint8)
+            if isinstance(j, np.ndarray):
+                j = np.ascontiguousarray(j.reshape(-1), np.uint8)
+                ptrs.append(j.ctypes.data)
+                lens.append(j.size)
+            else:  # a CPU torch tensor
+                if j.dtype.itemsize != 1 or j.is_cuda or not j.is_contiguous():
+                    raise RuntimeError("JPEG buffers must be contiguous uint8 host memory")
+                ptrs.append(j.data_ptr())
+                lens.append(j.numel())
+            keep.append(j)
+        n = len(ptrs)
+        return keep, (C.c_void_p * max(n, 1))(*ptrs), (C.c_size_t * max(n, 1))(*lens)
+
+    def decode_jpeg_batch(self, jpegs, channels=3, max_width=None, max_height=None, pitch=None, stream=None, device=None):
+        """Decodes JPEG files (bytes, numpy or CPU torch uint8 buffers; sizes and samplings may differ) on the GPU to exactly
+        cv2.imdecode(buf, IMREAD_COLOR) (channels 3: uint8 [h,w,3] BGR CUDA tensors) or its cvtColor(BGR2GRAY) (channels 1:
+        uint8 [h,w]).  max_width / max_height bound the frames (default: the handle's maximum); pitch: output row pitch in
+        bytes (default max_width * channels).  Returns one tensor per file, views into one [n, max_height, pitch] buffer."""
+        import torch
+        dev = device if device is not None else torch.device("cuda", self.device)
+        mw = max_width or self.max_width
+        mh = max_height or self.max_height
+        pitch = pitch or mw * channels
+        keep, ptrs, lens = self._jpeg_buffers(jpegs)
+        n = len(keep)
+        out = torch.empty((max(n, 1), mh, pitch), dtype=torch.uint8, device=dev)
+        ws, hs = (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))()
+        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+        self._check(self._L.dfb_decode_jpeg_batch_device(self._h, ptrs, lens, n, int(channels), out.data_ptr(), pitch, mh * pitch, mw, mh,
+                                                         ws, hs, C.c_void_p(s)))
+        res = []
+        for i in range(n):
+            v = out[i, :hs[i], :ws[i] * channels]
+            res.append(v.unflatten(1, (ws[i], 3)) if channels == 3 else v)
+        return res
+
+    def process_jpeg_batch(self, jpegs, step=1, bound=20, new_size=None, quality=95):
+        """The `-if` flow batch: process_bgr_batch with the frames given as JPEG files of one size, decoded on the GPU to
+        imdecode's pixels.  Returns [(jpg_x bytes, jpg_y bytes)] per pair, byte for byte process_bgr_batch's."""
+        keep, ptrs, lens = self._jpeg_buffers(jpegs)
+        n = len(keep)
+        dw, dh = new_size if new_size else (0, 0)
+        m = max(n - abs(step), 0)
+        if new_size:
+            ow, oh = dw, dh
+        else:
+            ow, oh = self.max_width, self.max_height  # an upper bound of the frame size (checked by the call)
+        cap = self._L.dfb_jpeg_max_bytes(ow, oh)
+        bx = [np.empty(cap, np.uint8) for _ in range(m)]
+        by = [np.empty(cap, np.uint8) for _ in range(m)]
+        xp = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bx])
+        yp = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in by])
+        lx = (C.c_size_t * max(m, 1))()
+        ly = (C.c_size_t * max(m, 1))()
+        self._check(self._L.dfb_process_jpeg_batch_host(self._h, ptrs, lens, n, step, dw, dh, int(bound), int(quality), xp, yp, cap, lx, ly))
+        return [(bx[i][:lx[i]].tobytes(), by[i][:ly[i]].tobytes()) for i in range(m)]
+
+    def debug_jpeg_coefficients(self, jpeg):
+        """Test hook: (int16 [blocks, 64] quantised coefficients in decode order, natural order, absolute DC; sync rounds)."""
+        keep, ptrs, lens = self._jpeg_buffers([jpeg])
+        cap = 1 << 20
+        while True:
+            out = np.empty((cap, 64), np.int16)
+            nb, rounds = C.c_int(), C.c_int()
+            rc = self._L.dfb_debug_jpeg_coefficients(self._h, ptrs[0], lens[0], out.ctypes.data, cap, C.byref(nb), C.byref(rounds))
+            if rc == _lib.DFB_ERR_SIZE and nb.value > cap:
+                cap = nb.value
+                continue
+            self._check(rc)
+            return out[:nb.value], rounds.value
 
     # -- gray -> resize -> flow -> quantise -> JPEG for decoded BGR frames (the reference's chain minus decode / file IO) --
     def process_bgr_batch(self, frames_bgr, step=1, bound=20, new_size=None, quality=95):

@@ -4,12 +4,14 @@
 // download (:339) — plus the batch shape of the whole function (:307-342).
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
 
 #include "engine.h"
 #include "jpeg.h"
+#include "jpeg_decode.h"
 #include "png_encode.h"
 #include "png_pack.h"
 #include "preproc.h"
@@ -52,6 +54,7 @@ struct dfb_handle {
     uint8_t *pb_bgr = nullptr, *pb_gray = nullptr, *pb_frames = nullptr, *pb_q = nullptr;
     size_t pb_bgr_cap = 0, pb_gray_cap = 0, pb_frames_cap = 0, pb_q_cap = 0;
     uint8_t *dec_bgr = nullptr;  // BGR scratch of dfb_decode_jpeg_gray_device
+    std::unique_ptr<JpegDecoder> jdec;  // imdecode-exact JPEG decoder, created on first use
     size_t dec_bgr_cap = 0;
     void *png_scratch = nullptr;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
     std::unique_ptr<PngEncoder> png;  // imencode(".png") workspace and files, created on first use
@@ -526,6 +529,7 @@ void dfb_destroy(dfb_handle *h) {
         if (e) cudaEventDestroy(e);
     if (h->png_scratch) cudaFree(h->png_scratch);
     h->png.reset();
+    h->jdec.reset();
     if (h->png_bgr) cudaFree(h->png_bgr);
     if (h->png_lens_host) cudaFreeHost(h->png_lens_host);
     if (h->dec_bgr) cudaFree(h->dec_bgr);
@@ -784,31 +788,28 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
     });
 }
 
-int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
-                               int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
-                               size_t *len_x, size_t *len_y) {
-    if (!h) return DFB_ERR_INVALID_ARG;
-    if (!bgr || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
-    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
-    if (sw <= 0 || sh <= 0 || dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
-    if (dw == 0) {
-        dw = sw;
-        dh = sh;
-    }
-    if (int rc = check_size(h, dw, dh)) return rc;
-    const int astep = std::abs(step);
-    const int M = std::max(n_frames - astep, 0);
-    if (M == 0) return DFB_OK;
+}  // extern "C"
+
+namespace {
+
+// Output-argument checks shared by the two flow chains below; dw / dh: resolved destination size.
+int check_chain_outputs(dfb_handle *h, int M, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t *len_x, size_t *len_y) {
     if (!jpg_x || !jpg_y || !len_x || !len_y) return fail(h, DFB_ERR_INVALID_ARG, "null output");
-    for (int f = 0; f < n_frames; ++f)
-        if (!bgr[f] || host_pointer_kind(bgr[f]) < 0)
-            return fail(h, DFB_ERR_INVALID_ARG, "bgr[" + std::to_string(f) + "] is null or a device pointer (host entry point)");
     for (int j = 0; j < M; ++j)
         if (!jpg_x[j] || !jpg_y[j] || host_pointer_kind(jpg_x[j]) < 0 || host_pointer_kind(jpg_y[j]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-    return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
+    return DFB_OK;
+}
+
+// The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) -> flow -> quantise -> two JPEGs per pair.
+// `produce(first, last)` enqueues on s_in the work that leaves frames [first, last] in h->pb_frames (dw x dh each, dense)
+// and records ev_frame[f] (h->pb_events[8 + f]) for each; frames are requested in order.  Runs inside guarded().
+int process_chain(dfb_handle *h, int n_frames, int step, int sw, int sh, int dw, int dh, int bound, int jpeg_quality,
+                  uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y,
+                  const std::function<void(int, int)> &produce) {
+    const int astep = std::abs(step);
+    const int M = std::max(n_frames - astep, 0);
+    {
         ensure_host_path(h);
         if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
         FlowAlgorithm &alg = *h->alg;
@@ -816,14 +817,12 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
         auto grow = [&](uint8_t *&ptr, size_t &cap, size_t need) { grow_device(ptr, cap, need); };
         // Three stages on three streams, groups of B pairs in flight (the reference runs the same three stages as three host
         // threads around queues, include/dense_flow.h:76-80):
-        //   s_in      H2D of BGR frame f -> cvtColor -> resize into the gray frame array        (decode stage tail, :163-170)
+        //   s_in      the frame source: decoded frames -> gray -> resize into the gray frame array (decode stage, :154-170)
         //   s_compute pyramids / polynomial expansions + flow of group g, quantised planes out   (:313-342 + src/common.cpp:4-16)
         //   s_out     two JPEG encodes per pair of group g (nvJPEG, one encoder state per plane)  (src/common.cpp:56-57)
         //   s_fetch   bitstreams of group g-1 to the host while the GPU works on group g
         const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
-        const size_t fpx = (size_t)dw * dh, bgr_bytes = (size_t)sw * sh * 3;
-        grow(h->pb_bgr, h->pb_bgr_cap, 2 * bgr_bytes);           // two staging frames: H2D of f+1 overlaps gray/resize of f
-        grow(h->pb_gray, h->pb_gray_cap, (size_t)sw * sh);
+        const size_t fpx = (size_t)dw * dh;
         grow(h->pb_frames, h->pb_frames_cap, fpx * n_frames);
         grow(h->pb_q, h->pb_q_cap, fpx * 2 * 2 * B);              // quantised planes of two groups
         alg.ensure_slots(B + astep + 1);
@@ -834,7 +833,6 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
             h->pb_events.push_back(e);
         }
         cudaEvent_t *ev_frame = h->pb_events.data() + 8;          // [n_frames]
-        cudaEvent_t *ev_gray = h->pb_events.data();                // [2] staging buffer consumed
         cudaEvent_t *ev_flow = h->pb_events.data() + 2;            // [2] group's planes ready
         cudaEvent_t *ev_enc = h->pb_events.data() + 4;             // [2] group's encodes done
         if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
@@ -842,24 +840,10 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
 
         int uploaded = 0;
         auto upload_until = [&](int last) {
-            for (; uploaded <= std::min(last, n_frames - 1); ++uploaded) {
-                const int f = uploaded, sb = f & 1;
-                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev_gray[sb], 0));
-                uint8_t *stage = h->pb_bgr + (size_t)sb * bgr_bytes;
-                DFB_CUDA(cudaMemcpyAsync(stage, bgr[f], bgr_bytes, cudaMemcpyHostToDevice, h->s_in));
-                h->counters.h2d_bytes += bgr_bytes;
-                uint8_t *dst = h->pb_frames + fpx * f;
-                if (dw == sw && dh == sh) {
-                    launch_bgr_to_gray(stage, (size_t)sw * 3, sw, sh, dst, dw, h->s_in);
-                } else {
-                    launch_bgr_to_gray(stage, (size_t)sw * 3, sw, sh, h->pb_gray, sw, h->s_in);
-                    const int rc = dfb_resize_gray_device(h, h->pb_gray, sw, sw, sh, dst, dw, dw, dh, h->s_in);
-                    if (rc != DFB_OK) throw std::runtime_error(h->last_error);
-                }
-                alg.launches += 1;
-                DFB_CUDA(cudaEventRecord(ev_gray[sb], h->s_in));
-                DFB_CUDA(cudaEventRecord(ev_frame[f], h->s_in));
-            }
+            last = std::min(last, n_frames - 1);
+            if (uploaded > last) return;
+            produce(uploaded, last);
+            uploaded = last + 1;
         };
         int prepared = 0;
         std::vector<FlowAlgorithm::PairJob> jobs(B);
@@ -924,6 +908,191 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
         DFB_CUDA(cudaStreamSynchronize(h->s_in));
         DFB_CUDA(cudaStreamSynchronize(h->s_compute));
         DFB_CUDA(cudaStreamSynchronize(h->s_out));
+        return DFB_OK;
+    }
+}
+
+// Every file of a JPEG batch parsed on the host; an unsupported or corrupt header is the call's error.
+int parse_jpegs(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n, std::vector<JpegHeader> &hd) {
+    hd.resize(n);
+    for (int i = 0; i < n; ++i) {
+        if (!jpeg[i] || !len[i]) return fail(h, DFB_ERR_INVALID_ARG, "frame " + std::to_string(i) + ": null or empty JPEG buffer");
+        if (host_pointer_kind(jpeg[i]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "frame " + std::to_string(i) + ": the JPEG bytes must be in host memory");
+        try {
+            hd[i] = parse_jpeg_header(jpeg[i], len[i], i);
+        } catch (const JpegUnsupported &e) {
+            return fail(h, DFB_ERR_UNSUPPORTED, e.what());
+        } catch (const std::exception &e) {
+            return fail(h, DFB_ERR_INVALID_ARG, e.what());
+        }
+    }
+    return DFB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
+                               int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
+                               size_t *len_x, size_t *len_y) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!bgr || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
+    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
+    if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
+    if (sw <= 0 || sh <= 0 || dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    if (dw == 0) {
+        dw = sw;
+        dh = sh;
+    }
+    if (int rc = check_size(h, dw, dh)) return rc;
+    const int M = std::max(n_frames - std::abs(step), 0);
+    if (M == 0) return DFB_OK;
+    if (!jpg_x || !jpg_y || !len_x || !len_y) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    for (int f = 0; f < n_frames; ++f)
+        if (!bgr[f] || host_pointer_kind(bgr[f]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "bgr[" + std::to_string(f) + "] is null or a device pointer (host entry point)");
+    if (int rc = check_chain_outputs(h, M, jpg_x, jpg_y, len_x, len_y)) return rc;
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        // frame source: H2D of BGR frame f into staging buffer f & 1 -> cvtColor -> resize (decode stage tail, :163-170)
+        const size_t fpx = (size_t)dw * dh, bgr_bytes = (size_t)sw * sh * 3;
+        grow_device(h->pb_bgr, h->pb_bgr_cap, 2 * bgr_bytes);  // two staging frames: H2D of f+1 overlaps gray/resize of f
+        grow_device(h->pb_gray, h->pb_gray_cap, (size_t)sw * sh);
+        while ((int)h->pb_events.size() < n_frames + 8) {
+            cudaEvent_t e;
+            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            h->pb_events.push_back(e);
+        }
+        auto produce = [&](int first, int last) {
+            cudaEvent_t *ev_gray = h->pb_events.data();  // [2] staging buffer consumed
+            cudaEvent_t *ev_frame = h->pb_events.data() + 8;
+            for (int f = first; f <= last; ++f) {
+                const int sb = f & 1;
+                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev_gray[sb], 0));
+                uint8_t *stage = h->pb_bgr + (size_t)sb * bgr_bytes;
+                DFB_CUDA(cudaMemcpyAsync(stage, bgr[f], bgr_bytes, cudaMemcpyHostToDevice, h->s_in));
+                h->counters.h2d_bytes += bgr_bytes;
+                uint8_t *dst = h->pb_frames + fpx * f;
+                if (dw == sw && dh == sh) {
+                    launch_bgr_to_gray(stage, (size_t)sw * 3, sw, sh, dst, dw, h->s_in);
+                } else {
+                    launch_bgr_to_gray(stage, (size_t)sw * 3, sw, sh, h->pb_gray, sw, h->s_in);
+                    const int rc = dfb_resize_gray_device(h, h->pb_gray, sw, sw, sh, dst, dw, dw, dh, h->s_in);
+                    if (rc != DFB_OK) throw std::runtime_error(h->last_error);
+                }
+                h->alg->launches += 1;
+                DFB_CUDA(cudaEventRecord(ev_gray[sb], h->s_in));
+                DFB_CUDA(cudaEventRecord(ev_frame[f], h->s_in));
+            }
+        };
+        return process_chain(h, n_frames, step, sw, sh, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
+    });
+}
+
+int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh,
+                                int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
+                                size_t *len_x, size_t *len_y) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!jpeg || !len || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
+    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
+    if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
+    if (dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    const int M = std::max(n_frames - std::abs(step), 0);
+    if (M == 0) return DFB_OK;
+    std::vector<JpegHeader> hd;
+    if (int rc = parse_jpegs(h, jpeg, len, n_frames, hd)) return rc;
+    const int sw = hd[0].w, sh = hd[0].h;
+    for (int f = 1; f < n_frames; ++f)
+        if (hd[f].w != sw || hd[f].h != sh)
+            return fail(h, DFB_ERR_SIZE, "frame " + std::to_string(f) + " is " + std::to_string(hd[f].w) + "x" + std::to_string(hd[f].h) +
+                                             ", frame 0 is " + std::to_string(sw) + "x" + std::to_string(sh) + " (one size per batch)");
+    if (dw == 0) {
+        dw = sw;
+        dh = sh;
+    }
+    if (int rc = check_size(h, dw, dh)) return rc;
+    if (int rc = check_chain_outputs(h, M, jpg_x, jpg_y, len_x, len_y)) return rc;
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        if (!h->jdec) h->jdec.reset(new JpegDecoder());
+        while ((int)h->pb_events.size() < n_frames + 8) {
+            cudaEvent_t e;
+            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            h->pb_events.push_back(e);
+        }
+        // frame source: the requested frames are decoded as one group, straight into the gray frame array when no resize is
+        // asked for, else into scratch and resized frame by frame; only the compressed bytes cross PCIe
+        const size_t fpx = (size_t)dw * dh, spx = (size_t)sw * sh;
+        auto produce = [&](int first, int last) {
+            cudaEvent_t *ev_frame = h->pb_events.data() + 8;
+            const int m = last - first + 1;
+            const bool resize = dw != sw || dh != sh;
+            if (resize) {
+                DFB_CUDA(cudaStreamSynchronize(h->s_in));  // the previous group's resizes have read the scratch
+                grow_device(h->pb_gray, h->pb_gray_cap, spx * m);
+            }
+            uint8_t *dst = resize ? h->pb_gray : h->pb_frames + fpx * first;
+            h->jdec->decode(jpeg + first, len + first, hd.data() + first, m, 1, dst, sw, spx, h->s_in);
+            h->alg->launches += h->jdec->launches;
+            for (int f = first; f <= last; ++f) {
+                h->counters.h2d_bytes += len[f];
+                if (resize) {
+                    const int rc = dfb_resize_gray_device(h, h->pb_gray + spx * (f - first), sw, sw, sh, h->pb_frames + fpx * f, dw, dw, dh, h->s_in);
+                    if (rc != DFB_OK) throw std::runtime_error(h->last_error);
+                }
+                DFB_CUDA(cudaEventRecord(ev_frame[f], h->s_in));
+            }
+        };
+        return process_chain(h, n_frames, step, sw, sh, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
+    });
+}
+
+int dfb_decode_jpeg_batch_device(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n, int channels, uint8_t *out,
+                                 size_t pitch, size_t frame_stride, int max_width, int max_height, int *width, int *height, void *stream) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (n < 0) return fail(h, DFB_ERR_INVALID_ARG, "n must be >= 0");
+    if (n == 0) return DFB_OK;
+    if (!jpeg || !len || !out) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    if (channels != 1 && channels != 3) return fail(h, DFB_ERR_INVALID_ARG, "channels must be 1 (gray) or 3 (BGR)");
+    if (!is_device_pointer(out)) return fail(h, DFB_ERR_INVALID_ARG, "out must be device memory (device entry point)");
+    std::vector<JpegHeader> hd;
+    if (int rc = parse_jpegs(h, jpeg, len, n, hd)) return rc;
+    for (int i = 0; i < n; ++i) {
+        if (width) width[i] = hd[i].w;
+        if (height) height[i] = hd[i].h;
+    }
+    for (int i = 0; i < n; ++i)
+        if (hd[i].w > max_width || hd[i].h > max_height || pitch < (size_t)hd[i].w * channels ||
+            (n > 1 && frame_stride < pitch * hd[i].h))
+            return fail(h, DFB_ERR_SIZE, "frame " + std::to_string(i) + ": " + std::to_string(hd[i].w) + "x" + std::to_string(hd[i].h) +
+                                             " does not fit the output (" + std::to_string(max_width) + "x" + std::to_string(max_height) +
+                                             ", pitch " + std::to_string(pitch) + ", frame stride " + std::to_string(frame_stride) + ")");
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        if (!h->jdec) h->jdec.reset(new JpegDecoder());
+        h->jdec->decode(jpeg, len, hd.data(), n, channels, out, pitch, frame_stride, static_cast<cudaStream_t>(stream));
+        h->alg->launches += h->jdec->launches;
+        for (int i = 0; i < n; ++i) h->counters.h2d_bytes += len[i] - hd[i].data_off;
+        return DFB_OK;
+    });
+}
+
+int dfb_debug_jpeg_coefficients(dfb_handle *h, const uint8_t *jpeg, size_t len, int16_t *out, size_t capacity_blocks, int *n_blocks,
+                                int *sync_rounds) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!jpeg || !out || !n_blocks) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    std::vector<JpegHeader> hd;
+    if (int rc = parse_jpegs(h, &jpeg, &len, 1, hd)) return rc;
+    *n_blocks = hd[0].blocks();
+    if ((size_t)hd[0].blocks() > capacity_blocks)
+        return fail(h, DFB_ERR_SIZE, "the file has " + std::to_string(hd[0].blocks()) + " blocks, capacity is " + std::to_string(capacity_blocks));
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        if (!h->jdec) h->jdec.reset(new JpegDecoder());
+        h->jdec->coefficients(jpeg, len, hd[0], out, nullptr);
+        if (sync_rounds) *sync_rounds = h->jdec->sync_rounds;
         return DFB_OK;
     });
 }

@@ -165,6 +165,48 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
                                 int max_height, int *width, int *height, void *stream);
 
 /*
+ * ---- imdecode-exact JPEG decode of `-if` frame folders --------------------------------------------------------------
+ * The decode stage reads each frame with imread(path, IMREAD_COLOR) and converts it with cvtColor(BGR2GRAY)
+ * (src/denseflow_gpu.cpp:154-163).  These calls decode JPEG files on the GPU to EXACTLY the pixels of
+ * cv2.imdecode(buf, IMREAD_COLOR) with libjpeg-turbo's default decompression as OpenCV sets it up (islow integer IDCT, fancy
+ * upsampling, YCbCr -> BGR table arithmetic).  Integer-only: both builds give the same bytes.  Only the compressed bytes
+ * cross PCIe; the host parses the markers, everything after (de-stuffing, entropy decode, IDCT, upsampling, colour) runs on
+ * the device.  They work on either kind of handle.
+ *
+ * Accepted: baseline or extended sequential Huffman (SOF0 / SOF1), 8-bit samples, one scan holding every component;
+ * 1 component, or 3 that libjpeg treats as YCbCr (JFIF marker, Adobe transform 1, or component ids 1-2-3); chroma sampled
+ * 1x1 with luma h, v in {1, 2} (4:4:4, 4:2:2, 4:4:0, 4:2:0); 8- or 16-bit DQT tables; DRI / RST0-7; APPn and COM
+ * segments are skipped.  DFB_ERR_UNSUPPORTED, with a message naming the feature, for progressive, arithmetic-coded,
+ * lossless or 12-bit files, multi-scan files, other samplings (4:1:1, ...), RGB-coded or CMYK files and an EXIF
+ * orientation other than 1 (imread would rotate the image).  DFB_ERR_INVALID_ARG, naming the frame, for corrupt data: an
+ * invalid Huffman code, data that ends before the last MCU, a wrong RST sequence (libjpeg warns and makes up pixels there;
+ * these calls refuse instead).  Progressive files still decode, approximately, through dfb_decode_jpeg_gray_device.
+ *
+ * dfb_decode_jpeg_batch_device: n files (host buffers jpeg[i] of len[i] bytes; sizes and samplings may differ).
+ * channels 3: imdecode(IMREAD_COLOR), packed BGR; channels 1: cvtColor(BGR2GRAY) of it (the frame the flow sees).  Frame i
+ * goes to out + i * frame_stride (device memory, rows `pitch` bytes apart); width[i] / height[i] (optional arrays of n)
+ * receive the sizes.  A frame larger than max_width x max_height or its pitch / stride: DFB_ERR_SIZE.  Enqueued on
+ * `stream`; blocks until the device has reported every frame's status.  n == 0 is a no-op.
+ */
+int dfb_decode_jpeg_batch_device(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n, int channels, uint8_t *out,
+                                 size_t pitch, size_t frame_stride, int max_width, int max_height, int *width, int *height, void *stream);
+/*
+ * The `-if` flow batch: dfb_process_bgr_batch_host with the frames given as JPEG files (every frame one size, else
+ * DFB_ERR_SIZE naming the frame).  The outputs are byte for byte those of dfb_process_bgr_batch_host on the imdecoded
+ * frames; the decode runs in groups of frames on the chain's input stream.
+ */
+int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dst_width,
+                                int dst_height, int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
+                                size_t *len_x, size_t *len_y);
+/*
+ * Test hook: the entropy decode alone.  out (host, capacity_blocks x 64 int16) receives the quantised coefficients of every
+ * block in decode (MCU) order, natural order, absolute DC; *n_blocks the block count; *sync_rounds (optional) how many
+ * re-decode rounds the subsequence states took to converge.
+ */
+int dfb_debug_jpeg_coefficients(dfb_handle *h, const uint8_t *jpeg, size_t len, int16_t *out, size_t capacity_blocks, int *n_blocks,
+                                int *sync_rounds);
+
+/*
  * Work counters of the most recent calc on this handle (for the roofline arithmetic, SURVEY §8(d)):
  *   iters[nscales*warps] executed inner iterations per (scale, warp), index s*warps + w, s = 0 finest
  *   level_w/level_h[nscales] pyramid sizes
