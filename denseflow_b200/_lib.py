@@ -83,6 +83,8 @@ SIGNATURES = {
     "dfb_jpeg_max_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "dfb_encode_jpeg_gray_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
                                               C.POINTER(C.c_size_t), C.c_void_p]),
+    "dfb_encode_jpeg_gray_batch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                    C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]),
     "dfb_decode_jpeg_gray_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_int),
                                               C.POINTER(C.c_int), C.c_void_p]),
     "dfb_process_bgr_batch_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,

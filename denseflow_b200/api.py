@@ -202,6 +202,24 @@ class DenseOpticalFlow:
                                                         cap, C.byref(n), C.c_void_p(s)))
         return buf[:n.value].tobytes()
 
+    def encode_jpeg_gray_batch_device(self, planes, quality=95, capacity=None):
+        """planes: CUDA uint8 [n, H, W] (rows contiguous; any row and plane stride).  One launch sequence; always the exact
+        encoder: returns [bytes of cv2.imencode(".jpg", planes[i], [IMWRITE_JPEG_QUALITY, quality])]."""
+        import torch
+        n, h, w = planes.shape
+        if n == 0:
+            return []
+        if planes.dtype != torch.uint8 or not planes.is_cuda or planes.stride(2) != 1:
+            raise ValueError("planes must be a CUDA uint8 tensor [n, H, W] with contiguous rows")
+        cap = int(capacity) if capacity is not None else self._L.dfb_jpeg_max_bytes(w, h)
+        bufs = [np.empty(cap, np.uint8) for _ in range(n)]
+        ptrs = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
+        lens = (C.c_size_t * n)()
+        s = torch.cuda.current_stream(planes.device).cuda_stream
+        self._check(self._L.dfb_encode_jpeg_gray_batch_device(self._h, planes.data_ptr(), planes.stride(1), planes.stride(0), n, w, h,
+                                                              int(quality), ptrs, cap, lens, C.c_void_p(s)))
+        return [bufs[i][:lens[i]].tobytes() for i in range(n)]
+
     # -- imread(".jpg") + cvtColor(BGR2GRAY) of an `-if` frame folder on the GPU (nvJPEG decode; not bit-identical to libjpeg-turbo) --
     def decode_jpeg_gray_device(self, jpeg_bytes, max_width, max_height, device=None):
         import torch

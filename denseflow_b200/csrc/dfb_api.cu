@@ -12,6 +12,7 @@
 #include "engine.h"
 #include "jpeg.h"
 #include "jpeg_decode.h"
+#include "jpeg_encode.h"
 #include "png_encode.h"
 #include "png_pack.h"
 #include "preproc.h"
@@ -69,6 +70,11 @@ struct dfb_handle {
     uint8_t *ex_bgr = nullptr, *ex_ycc = nullptr;  // dfb_extract_frames_host: two staging frames, planes of two groups
     size_t ex_bgr_cap = 0, ex_ycc_cap = 0;
     cudaEvent_t ex_events[8] = {};
+    // "jpeg_exact" = 1: every JPEG this handle writes is imencode(".jpg")'s bytes (JpegExactEncoder) instead of nvJPEG's
+    bool jpeg_exact = false;
+    std::unique_ptr<JpegExactEncoder> jex;  // created on first use
+    uint64_t *jex_lens_host = nullptr;      // pinned file lengths of the two groups in flight
+    int jex_lens_n = 0;                     // per slot
 };
 
 namespace {
@@ -237,6 +243,49 @@ struct YccLayout {
 // the resize of a frame-extraction call: null tables mean no resize
 const ResizeTap *ycc_tables(dfb_handle *h, int sw, int sh, int dw, int dh) {
     return (sw == dw && sh == dh) ? nullptr : ensure_taps(h->ycc_taps, sw, sh, dw, dh);
+}
+
+// The imencode-exact JPEG encoder, and pinned room for the file lengths of two groups of n files
+JpegExactEncoder &ensure_jex(dfb_handle *h, int n) {
+    if (!h->jex) h->jex.reset(new JpegExactEncoder());
+    if (h->jex_lens_n < n) {
+        DFB_CUDA(cudaDeviceSynchronize());  // a read-back may still target the old buffer
+        if (h->jex_lens_host) DFB_CUDA(cudaFreeHost(h->jex_lens_host));
+        h->jex_lens_host = nullptr;
+        DFB_CUDA(cudaHostAlloc(&h->jex_lens_host, sizeof(uint64_t) * 2 * n, cudaHostAllocDefault));
+        h->jex_lens_n = n;
+    }
+    return *h->jex;
+}
+
+// the planes of a YccLayout block as the exact encoder reads them
+JpegSrc ycc_src(const uint8_t *base, const YccLayout &L) {
+    JpegSrc src;
+    src.base = base;
+    src.img_stride = L.bytes;
+    src.pitch = L.y_pitch;
+    src.cb_off = L.cb_off;
+    src.cr_off = L.cr_off;
+    src.c_pitch = L.c_pitch;
+    return src;
+}
+
+// Encodes n images of src with the exact encoder into slot 0 and copies file i to out[i] (host), its length to len[i].
+// Blocks until the files are on the host.  `too_small(i, need)` builds the message of a file that does not fit.
+void jex_encode_to_host(dfb_handle *h, int n, const JpegSrc &src, int comps, int w, int hh, int quality, uint8_t *const *out, size_t capacity,
+                        size_t *len, cudaStream_t s, const std::function<std::string(int, size_t)> &too_small) {
+    JpegExactEncoder &jx = ensure_jex(h, n);
+    h->alg->launches += jx.encode(n, src, comps, w, hh, quality, capacity, 0, s);
+    DFB_CUDA(cudaMemcpyAsync(h->jex_lens_host, jx.lens(0), sizeof(uint64_t) * n, cudaMemcpyDeviceToHost, s));
+    DFB_CUDA(cudaStreamSynchronize(s));
+    for (int i = 0; i < n; ++i)
+        if (h->jex_lens_host[i] > capacity) throw std::runtime_error(too_small(i, jx.needed(h->jex_lens_host[i], src, i, comps, w, hh, quality, s)));
+    for (int i = 0; i < n; ++i) {
+        len[i] = (size_t)h->jex_lens_host[i];
+        DFB_CUDA(cudaMemcpyAsync(out[i], jx.file(0, i), len[i], cudaMemcpyDeviceToHost, s));
+        h->counters.d2h_bytes += len[i];
+    }
+    DFB_CUDA(cudaStreamSynchronize(s));
 }
 
 // output ring slots [0, n): allocated on first use (a 1080p handle runs 7 pairs per launch and touches 14 slots, a 340x256
@@ -530,6 +579,8 @@ void dfb_destroy(dfb_handle *h) {
     if (h->png_scratch) cudaFree(h->png_scratch);
     h->png.reset();
     h->jdec.reset();
+    h->jex.reset();
+    if (h->jex_lens_host) cudaFreeHost(h->jex_lens_host);
     if (h->png_bgr) cudaFree(h->png_bgr);
     if (h->png_lens_host) cudaFreeHost(h->png_lens_host);
     if (h->dec_bgr) cudaFree(h->dec_bgr);
@@ -552,12 +603,21 @@ const char *dfb_last_error(const dfb_handle *h) {
 
 int dfb_set_param(dfb_handle *h, const char *name, double value) {
     if (!h || !name) return DFB_ERR_INVALID_ARG;
+    if (!std::strcmp(name, "jpeg_exact")) {  // an output contract of the handle, not of the flow algorithm
+        if (value != 0 && value != 1) return fail(h, DFB_ERR_INVALID_ARG, "jpeg_exact must be 0 or 1");
+        h->jpeg_exact = value == 1;
+        return DFB_OK;
+    }
     if (!h->alg->set_param(name, value)) return fail(h, DFB_ERR_INVALID_ARG, std::string("bad parameter ") + name);
     return DFB_OK;
 }
 
 int dfb_get_param(const dfb_handle *h, const char *name, double *value) {
     if (!h || !name || !value) return DFB_ERR_INVALID_ARG;
+    if (!std::strcmp(name, "jpeg_exact")) {
+        *value = h->jpeg_exact ? 1 : 0;
+        return DFB_OK;
+    }
     return h->alg->get_param(name, value) ? DFB_OK : DFB_ERR_INVALID_ARG;
 }
 
@@ -752,8 +812,45 @@ int dfb_encode_jpeg_gray_device(dfb_handle *h, const uint8_t *gray, size_t gray_
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry or quality");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
+        if (h->jpeg_exact) {
+            JpegSrc src;
+            src.base = gray;
+            src.pitch = gray_pitch;
+            jex_encode_to_host(h, 1, src, 1, width, height, quality, &out, out_capacity, out_len, static_cast<cudaStream_t>(stream),
+                               [&](int, size_t need) {
+                                   return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(out_capacity) + ")";
+                               });
+            return DFB_OK;
+        }
         if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
         *out_len = h->jpeg->encode_gray(gray, gray_pitch, width, height, quality, out, out_capacity, static_cast<cudaStream_t>(stream));
+        return DFB_OK;
+    });
+}
+
+int dfb_encode_jpeg_gray_batch_device(dfb_handle *h, const uint8_t *planes, size_t pitch, size_t plane_stride, int n, int width,
+                                      int height, int quality, uint8_t *const *out, size_t capacity, size_t *len, void *stream) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (n < 0) return fail(h, DFB_ERR_INVALID_ARG, "n must be >= 0");
+    if (n == 0) return DFB_OK;
+    if (!planes || !out || !len) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    if (width <= 0 || height <= 0 || width > 65535 || height > 65535 || pitch < (size_t)width || quality < 1 || quality > 100 ||
+        (n > 1 && plane_stride < pitch * (size_t)(height - 1) + (size_t)width))
+        return fail(h, DFB_ERR_INVALID_ARG, "bad geometry or quality");
+    if (capacity == 0) return fail(h, DFB_ERR_INVALID_ARG, "zero capacity");
+    if (!is_device_pointer(planes)) return fail(h, DFB_ERR_INVALID_ARG, "planes must be device memory (device entry point)");
+    for (int i = 0; i < n; ++i)
+        if (!out[i] || host_pointer_kind(out[i]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(i) + " is null or a device pointer (host entry point)");
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        JpegSrc src;
+        src.base = planes;
+        src.pitch = pitch;
+        src.img_stride = plane_stride;
+        jex_encode_to_host(h, n, src, 1, width, height, quality, out, capacity, len, static_cast<cudaStream_t>(stream), [&](int i, size_t need) {
+            return "jpeg output buffer too small: plane " + std::to_string(i) + " (" + std::to_string(need) + " > " + std::to_string(capacity) + ")";
+        });
         return DFB_OK;
     });
 }
@@ -835,8 +932,21 @@ int process_chain(dfb_handle *h, int n_frames, int step, int sw, int sh, int dw,
         cudaEvent_t *ev_frame = h->pb_events.data() + 8;          // [n_frames]
         cudaEvent_t *ev_flow = h->pb_events.data() + 2;            // [2] group's planes ready
         cudaEvent_t *ev_enc = h->pb_events.data() + 4;             // [2] group's encodes done
-        if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
-        h->jpeg->ensure_states(4 * B);
+        const bool exact = h->jpeg_exact;
+        if (exact) {
+            ensure_jex(h, 2 * B);
+        } else {
+            if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
+            h->jpeg->ensure_states(4 * B);
+        }
+        // the exact encoder reads the group's 2 m planes as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
+        auto group_planes = [&](int slot) {
+            JpegSrc src;
+            src.base = h->pb_q + (size_t)slot * B * 2 * fpx;
+            src.img_stride = fpx;
+            src.pitch = (size_t)dw;
+            return src;
+        };
 
         int uploaded = 0;
         auto upload_until = [&](int last) {
@@ -877,7 +987,12 @@ int process_chain(dfb_handle *h, int n_frames, int step, int sw, int sh, int dw,
             DFB_CUDA(cudaEventRecord(ev_flow[slot], h->s_compute));
             // encode stage (src/common.cpp:48-64): one JPEG per plane
             DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev_flow[slot], 0));
-            for (int i = 0; i < m; ++i) {
+            if (exact) {
+                alg.launches += h->jex->encode(2 * m, group_planes(slot), 1, dw, dh, jpeg_quality, capacity, slot, h->s_out);
+                DFB_CUDA(cudaMemcpyAsync(h->jex_lens_host + (size_t)slot * h->jex_lens_n, h->jex->lens(slot), sizeof(uint64_t) * 2 * m,
+                                         cudaMemcpyDeviceToHost, h->s_out));
+            }
+            for (int i = 0; i < m && !exact; ++i) {
                 const uint8_t *qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
                 h->jpeg->enqueue((slot * B + i) * 2, qx, dw, dw, dh, jpeg_quality, h->s_out);
                 h->jpeg->enqueue((slot * B + i) * 2 + 1, qx + fpx, dw, dw, dh, jpeg_quality, h->s_out);
@@ -888,7 +1003,22 @@ int process_chain(dfb_handle *h, int n_frames, int step, int sw, int sh, int dw,
         auto finish_group = [&](int g) {
             const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
             DFB_CUDA(cudaEventSynchronize(ev_enc[slot]));
-            for (int i = 0; i < m; ++i)
+            if (exact) {
+                const uint64_t *lens = h->jex_lens_host + (size_t)slot * h->jex_lens_n;
+                for (int k = 0; k < 2 * m; ++k)
+                    if (lens[k] > capacity)
+                        throw std::runtime_error("jpeg output buffer too small (" +
+                                                 std::to_string(h->jex->needed(lens[k], group_planes(slot), k, 1, dw, dh, jpeg_quality, h->s_fetch)) +
+                                                 " > " + std::to_string(capacity) + ")");
+                for (int k = 0; k < 2 * m; ++k) {
+                    const int i = k >> 1, c = k & 1;
+                    const size_t len = (size_t)lens[k];
+                    (c ? len_y : len_x)[j0 + i] = len;
+                    DFB_CUDA(cudaMemcpyAsync((c ? jpg_y : jpg_x)[j0 + i], h->jex->file(slot, k), len, cudaMemcpyDeviceToHost, h->s_fetch));
+                    h->counters.d2h_bytes += len;
+                }
+            }
+            for (int i = 0; i < m && !exact; ++i)
                 for (int c = 0; c < 2; ++c) {
                     const int st = (slot * B + i) * 2 + c;
                     const size_t len = h->jpeg->length(st, h->s_fetch);
@@ -1140,8 +1270,15 @@ int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pit
         const ResizeTap *taps = ycc_tables(h, src_width, src_height, dw, dh);
         uint8_t *p = h->enc_ycc;
         launch_bgr_to_ycc420(bgr, bgr_pitch, src_width, src_height, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                             p + L.cr_off, L.c_pitch, s);
+                             p + L.cr_off, L.c_pitch, s, h->jpeg_exact ? jpeg_chroma_cols(dw) : 0);
         ++h->alg->launches;
+        if (h->jpeg_exact) {
+            jex_encode_to_host(h, 1, ycc_src(p, L), 3, dw, dh, quality, &out, out_capacity, out_len, s, [&](int, size_t need) {
+                return "jpeg output buffer too small: the bitstream needs " + std::to_string(need) + " bytes, capacity is " +
+                       std::to_string(out_capacity);
+            });
+            return DFB_OK;
+        }
         if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
         h->jpeg->enqueue_ycc420(0, p, L.y_pitch, p + L.cb_off, p + L.cr_off, L.c_pitch, dw, dh, quality, s);
         DFB_CUDA(cudaStreamSynchronize(s));
@@ -1195,8 +1332,13 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
         cudaEvent_t *ev_conv = h->ex_events + 2;  // [2] staging buffer consumed
         cudaEvent_t *ev_planes = h->ex_events + 4;  // [2] group's planes ready
         cudaEvent_t *ev_enc = h->ex_events + 6;   // [2] group's encodes done
-        if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
-        h->jpeg->ensure_states(2 * G);
+        const bool exact = h->jpeg_exact;
+        if (exact) {
+            ensure_jex(h, G);
+        } else {
+            if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
+            h->jpeg->ensure_states(2 * G);
+        }
 
         auto convert_group = [&](int g) {
             const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
@@ -1211,13 +1353,18 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
                 DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_h2d[sb], 0));
                 uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
                 launch_bgr_to_ycc420(stage, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                                     p + L.cr_off, L.c_pitch, h->s_compute);
+                                     p + L.cr_off, L.c_pitch, h->s_compute, exact ? jpeg_chroma_cols(dw) : 0);
                 ++h->alg->launches;
                 DFB_CUDA(cudaEventRecord(ev_conv[sb], h->s_compute));
             }
             DFB_CUDA(cudaEventRecord(ev_planes[slot], h->s_compute));
             DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev_planes[slot], 0));
-            for (int i = 0; i < m; ++i) {
+            if (exact) {
+                h->alg->launches += h->jex->encode(m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, slot, h->s_out);
+                DFB_CUDA(cudaMemcpyAsync(h->jex_lens_host + (size_t)slot * h->jex_lens_n, h->jex->lens(slot), sizeof(uint64_t) * m,
+                                         cudaMemcpyDeviceToHost, h->s_out));
+            }
+            for (int i = 0; i < m && !exact; ++i) {
                 const uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
                 h->jpeg->enqueue_ycc420(slot * G + i, p, L.y_pitch, p + L.cb_off, p + L.cr_off, L.c_pitch, dw, dh, quality, h->s_out);
             }
@@ -1226,7 +1373,21 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
         auto finish_group = [&](int g) {
             const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
             DFB_CUDA(cudaEventSynchronize(ev_enc[slot]));
-            for (int i = 0; i < m; ++i) {
+            if (exact) {
+                const uint64_t *lens = h->jex_lens_host + (size_t)slot * h->jex_lens_n;
+                const JpegSrc src = ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L);
+                for (int i = 0; i < m; ++i)
+                    if (lens[i] > capacity)
+                        throw std::runtime_error("jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " +
+                                                 std::to_string(h->jex->needed(lens[i], src, i, 3, dw, dh, quality, h->s_fetch)) +
+                                                 " bytes, capacity is " + std::to_string(capacity));
+                for (int i = 0; i < m; ++i) {
+                    len[f0 + i] = (size_t)lens[i];
+                    DFB_CUDA(cudaMemcpyAsync(jpg[f0 + i], h->jex->file(slot, i), len[f0 + i], cudaMemcpyDeviceToHost, h->s_fetch));
+                    h->counters.d2h_bytes += len[f0 + i];
+                }
+            }
+            for (int i = 0; i < m && !exact; ++i) {
                 const int st = slot * G + i, f = f0 + i;
                 const size_t n = h->jpeg->length(st, h->s_fetch);
                 if (n > capacity)

@@ -1,7 +1,8 @@
 // jpeg.cu — GPU JPEG encode of the quantised flow planes through nvJPEG (SURVEY §8 f2): replaces the two
 // imencode(".jpg", flow_img_x / flow_img_y, ...) calls of encodeFlowMap (/root/reference/src/common.cpp:56-57) with
 // OpenCV's defaults (quality 95, baseline sequential, one gray component).  Byte identity with libjpeg-turbo is
-// not a goal (lossy; the reference pins no bytes) — the decoded planes are compared in the tests.
+// not a goal here (lossy) — the decoded planes are compared in the tests; jpeg_encode.cu is the byte-exact encoder behind
+// the handle parameter "jpeg_exact".
 // nvJPEG is loaded lazily with dlopen so the engine itself never depends on it.
 #include <dlfcn.h>
 #include <nvjpeg.h>

@@ -19,6 +19,7 @@
 #include <algorithm>
 #include <stdexcept>
 
+#include "block_scan.cuh"
 #include "common.cuh"
 #include "png_deflate.cuh"
 #include "png_encode.h"
@@ -87,39 +88,6 @@ struct Layout {
     __device__ uint32_t *z(uint8_t *ws, int i) const { return (uint32_t *)(base(ws, i) + o_z); }
     __device__ ImgInfo *info(uint8_t *ws, int i) const { return (ImgInfo *)(base(ws, i) + o_info); }
 };
-
-// exclusive scan over the CTA; *total receives the sum.  sm: NT / 32 words.
-template <int NT, typename T> __device__ T block_scan(T v, T &total, T *sm) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    T x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const T y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) sm[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        T t = lane < NT / 32 ? sm[lane] : T(0);
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const T y = __shfl_up_sync(0xffffffffu, t, o);
-            if (lane >= o) t += y;
-        }
-        if (lane < NT / 32) sm[lane] = t;
-    }
-    __syncthreads();
-    const T base = warp ? sm[warp - 1] : T(0);
-    total = sm[NT / 32 - 1];
-    __syncthreads();
-    return base + x - v;
-}
-
-template <int NT, typename T> __device__ T block_sum(T v, T *sm) {
-    T total;
-    block_scan<NT>(v, total, sm);
-    return total;
-}
 
 __device__ __forceinline__ void or_bits(uint32_t *zw, uint64_t off, uint32_t v, int len) {
     const uint64_t i = off >> 5;

@@ -59,13 +59,15 @@ __device__ __forceinline__ void bgr_to_ycc(int b, int g, int r, int &y, int &cb,
 // Packed BGR (sw x sh) -> cv::resize(INTER_LINEAR) to dw x dh (identity when xt == nullptr) -> JFIF YCbCr -> libjpeg's
 // h2v2_downsample (jcsample.c): one thread per 2 x 2 destination block, whose chroma sample never leaves registers.
 // An odd last column / row is replicated (expand_right_edge, jcsample.c; expand_bottom_edge, jcprepct.c), and the
-// downsampling bias is 1 on even and 2 on odd chroma columns, restarting on every row.
+// downsampling bias is 1 on even and 2 on odd chroma columns, restarting on every row.  Chroma columns up to c_cols are
+// written (past ceil(dw / 2) only the replicated last column contributes).
 __global__ void __launch_bounds__(256) k_bgr_to_ycc420(const uint8_t *__restrict__ src, size_t src_pitch, int sw, int sh,
                                                        int dw, int dh, const ResizeTap *__restrict__ xt,
                                                        const ResizeTap *__restrict__ yt, uint8_t *__restrict__ yp, size_t y_pitch,
-                                                       uint8_t *__restrict__ cbp, uint8_t *__restrict__ crp, size_t c_pitch) {
+                                                       uint8_t *__restrict__ cbp, uint8_t *__restrict__ crp, size_t c_pitch,
+                                                       int c_cols) {
     const int cx = blockIdx.x * 32 + threadIdx.x, cy = blockIdx.y * 8 + threadIdx.y;
-    if (cx >= (dw + 1) >> 1 || cy >= (dh + 1) >> 1) return;
+    if (cx >= c_cols || cy >= (dh + 1) >> 1) return;
     int sum_cb = 0, sum_cr = 0;
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
@@ -141,9 +143,10 @@ void launch_resize_u8(const uint8_t *src, size_t src_pitch, int sw, int sh, uint
 }
 
 void launch_bgr_to_ycc420(const uint8_t *bgr, size_t bgr_pitch, int sw, int sh, int dw, int dh, const ResizeTap *xt, const ResizeTap *yt,
-                          uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, cudaStream_t s) {
-    k_bgr_to_ycc420<<<dim3(ceil_div(ceil_div(dw, 2), 32), ceil_div(ceil_div(dh, 2), 8)), dim3(32, 8), 0, s>>>(
-        bgr, bgr_pitch, sw, sh, dw, dh, xt, yt, y, y_pitch, cb, cr, c_pitch);
+                          uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, cudaStream_t s, int c_cols) {
+    if (c_cols <= 0) c_cols = ceil_div(dw, 2);
+    k_bgr_to_ycc420<<<dim3(ceil_div(c_cols, 32), ceil_div(ceil_div(dh, 2), 8)), dim3(32, 8), 0, s>>>(
+        bgr, bgr_pitch, sw, sh, dw, dh, xt, yt, y, y_pitch, cb, cr, c_pitch, c_cols);
     DFB_KERNEL_CHECK();
 }
 

@@ -69,6 +69,12 @@ const char *dfb_last_error(const dfb_handle *h);
  * second handle's launch fills the SMs the first one's finished lanes free), "time_kernels" (CUDA-event timing of the dominant kernel, see dfb_counters).  farn: "num_levels" "num_iters" "poly_sigma"
  * (winSize 13, polyN 5, pyrScale 0.5 are fixed), "use_tma" (1 = persistent TMA-staged iteration kernel [default], 0 = the
  * LDG-staged one), "time_kernels".  Every combination of the engine knobs produces bit-identical flows.
+ * Both algorithms: "jpeg_exact" (0 [default] = JPEG files through nvJPEG; 1 = every JPEG this handle writes is exactly the
+ * file cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality]) writes with OpenCV's other defaults, libjpeg-turbo 3.x:
+ * baseline, standard Huffman tables, islow DCT, gray or YCbCr 4:2:0, no restart markers).  It covers
+ * dfb_encode_jpeg_gray_device, dfb_encode_jpeg_bgr_device, dfb_process_bgr_batch_host, dfb_process_jpeg_batch_host and
+ * dfb_extract_frames_host; the two settings give different bytes and the same flows.  The exact encoder is the project's
+ * own CUDA and never loads libnvjpeg.  Any other value is DFB_ERR_INVALID_ARG.
  */
 int dfb_set_param(dfb_handle *h, const char *name, double value);
 int dfb_get_param(const dfb_handle *h, const char *name, double *value);
@@ -145,12 +151,23 @@ int dfb_resize_gray_device(dfb_handle *h, const uint8_t *src, size_t src_pitch, 
  * JPEG-encode one uint8 plane that lives in device memory (SURVEY §8 f2).  Replaces
  * imencode(".jpg", flow_img_x, encoded_x) / (..., flow_img_y, ...)  src/common.cpp:56-57 with OpenCV's defaults when
  * quality = 95 (baseline sequential, one gray component).  out is a host buffer of out_capacity bytes
- * (dfb_jpeg_max_bytes(width, height) is always enough); *out_len receives the length.  Blocks until
- * the bitstream is on the host.  Not byte-identical to libjpeg-turbo (lossy; the reference pins no bytes).
+ * (dfb_jpeg_max_bytes(width, height) holds i.i.d. noise at quality 100; a larger file fails cleanly with the needed
+ * length in the message); *out_len receives the length.  Blocks until the bitstream is on the host.  With the handle's
+ * "jpeg_exact" = 0 [default] nvJPEG encodes, not byte-identical to libjpeg-turbo; with 1 the file is imencode(".jpg")'s bytes.
  */
 size_t dfb_jpeg_max_bytes(int width, int height);
 int dfb_encode_jpeg_gray_device(dfb_handle *h, const uint8_t *gray, size_t gray_pitch, int width, int height, int quality,
                                 uint8_t *out, size_t out_capacity, size_t *out_len, void *stream);
+/*
+ * n device planes of one size in one launch sequence, always with the exact encoder: file i is the bytes of
+ * cv2.imencode(".jpg", plane_i, [IMWRITE_JPEG_QUALITY, quality]).  Plane i starts at planes + i * plane_stride, rows pitch
+ * bytes apart (any alignment); out[i] are host buffers of `capacity` bytes each, len[i] receives file i's length.  The work
+ * is enqueued on `stream` and the call blocks until the files are on the host; n == 0 is a no-op.  A file that does not
+ * fit fails the call with the length it needs in the message ("jpeg output buffer too small: plane i (N > capacity)").
+ */
+int dfb_encode_jpeg_gray_batch_device(dfb_handle *h, const uint8_t *planes, size_t pitch, size_t plane_stride, int n,
+                                      int width, int height, int quality, uint8_t *const *out, size_t capacity,
+                                      size_t *len, void *stream);
 
 /*
  * Decode one JPEG frame of an `-if` frame folder on the GPU (SURVEY §8 f3 remainder): replaces imread(path) [IMREAD_COLOR]
@@ -261,8 +278,8 @@ size_t dfb_jpeg_max_bytes_bgr(int width, int height);
 /*
  * One frame: resize + imencode(".jpg", frame) of a BGR frame in device memory.  Baseline, standard Huffman tables, YCbCr
  * 4:2:0; out is a host buffer of out_capacity bytes, *out_len receives the length.  The work is enqueued on `stream` and
- * the call blocks until the bitstream is on the host.  Not byte-identical to libjpeg (only the DCT and the padding of the
- * edge MCUs differ; the reference pins no bytes).
+ * the call blocks until the bitstream is on the host.  With "jpeg_exact" = 0 [default] nvJPEG encodes, not byte-identical
+ * to libjpeg (only the DCT and the padding of the edge MCUs differ); with 1 the file is imencode(".jpg", resized frame)'s bytes.
  */
 int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int src_width, int src_height, int dst_width,
                                int dst_height, int quality, uint8_t *out, size_t out_capacity, size_t *out_len, void *stream);
