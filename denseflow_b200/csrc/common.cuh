@@ -80,4 +80,42 @@ class Slab {
     size_t cap_ = 0, off_ = 0;
 };
 
+// One owned allocation of device memory (Pinned = false: cudaMalloc) or page-locked host memory (true: cudaHostAlloc),
+// sized in bytes and freed by the destructor.
+template <typename T, bool Pinned> class OwnedBuffer {
+  public:
+    OwnedBuffer() = default;
+    ~OwnedBuffer() { release(); }
+    OwnedBuffer(const OwnedBuffer &) = delete;
+    OwnedBuffer &operator=(const OwnedBuffer &) = delete;
+    // Room for at least `bytes`.  Work on any stream may still use the old buffer, so the device is synchronised first.
+    void grow(size_t bytes) {
+        if (bytes <= cap_) return;
+        DFB_CUDA(cudaDeviceSynchronize());
+        allocate(bytes);
+    }
+    // The same without the synchronisation: for a first allocation, or when the caller has waited for the buffer's last user.
+    void allocate(size_t bytes) {
+        if (bytes <= cap_) return;
+        release();
+        void *p = nullptr;
+        DFB_CUDA(Pinned ? cudaHostAlloc(&p, bytes, cudaHostAllocDefault) : cudaMalloc(&p, bytes));
+        p_ = static_cast<T *>(p);
+        cap_ = bytes;
+    }
+    operator T *() const { return p_; }
+    size_t bytes() const { return cap_; }
+
+  private:
+    void release() {
+        if (p_) Pinned ? cudaFreeHost(p_) : cudaFree(p_);
+        p_ = nullptr;
+        cap_ = 0;
+    }
+    T *p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <typename T> using DeviceBuffer = OwnedBuffer<T, false>;
+template <typename T> using PinnedBuffer = OwnedBuffer<T, true>;
+
 }  // namespace dfb

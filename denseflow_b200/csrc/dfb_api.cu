@@ -22,8 +22,30 @@ using namespace dfb;
 
 // resize coefficient tables on the device, rebuilt when the geometry changes
 struct TapTable {
-    ResizeTap *d = nullptr;
-    int cap = 0, sw = 0, sh = 0, dw = 0, dh = 0;
+    DeviceBuffer<ResizeTap> d;
+    int sw = 0, sh = 0, dw = 0, dh = 0;
+};
+
+// CUDA events created on first use and destroyed with their owner
+class Events {
+  public:
+    Events() = default;
+    Events(const Events &) = delete;
+    Events &operator=(const Events &) = delete;
+    ~Events() {
+        for (cudaEvent_t e : e_) cudaEventDestroy(e);
+    }
+    void ensure(size_t n) {
+        while (e_.size() < n) {
+            cudaEvent_t e;
+            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            e_.push_back(e);
+        }
+    }
+    cudaEvent_t operator[](size_t i) const { return e_[i]; }
+
+  private:
+    std::vector<cudaEvent_t> e_;
 };
 
 struct dfb_handle {
@@ -36,45 +58,50 @@ struct dfb_handle {
 
     // host-path plumbing: three streams so H2D of frame i+1, compute of pair i and D2H of flow i-1 overlap
     cudaStream_t s_in = nullptr, s_compute = nullptr, s_out = nullptr;
+    cudaStream_t s_fetch = nullptr;  // file read-back of the encoding pipelines
     static constexpr int kFrameRing = 16; // device u8 frames (dead as soon as their pyramid is built)
     static constexpr int kFlowRing = 128; // device flow / quantised outputs: two launches of up to 64 pairs in flight; slots are
                                           // allocated on first use and a call cycles through 2 x (pairs per launch) of them
-    uint8_t *d_frame[kFrameRing] = {};
+    DeviceBuffer<uint8_t> d_frame[kFrameRing];
     size_t d_frame_pitch = 0;
-    float *d_flow[kFlowRing] = {};
-    uint8_t *d_qx[kFlowRing] = {}, *d_qy[kFlowRing] = {};
-    cudaEvent_t ev_in[kFrameRing] = {}, ev_pyr[kFrameRing] = {}, ev_done[kFlowRing] = {}, ev_out[kFlowRing] = {};
+    DeviceBuffer<float> d_flow[kFlowRing];
+    DeviceBuffer<uint8_t> d_qx[kFlowRing], d_qy[kFlowRing];
+    Events ev_in, ev_pyr;     // [kFrameRing] frame uploaded, its pyramid built
+    Events ev_done, ev_out;   // [kFlowRing] pair solved, its output read back
     // pinned staging for pageable caller buffers
-    uint8_t *h_frame[kFrameRing] = {};
-    float *h_flow[kFlowRing] = {};
-    uint8_t *h_q[kFlowRing] = {};
+    PinnedBuffer<uint8_t> h_frame[kFrameRing];
+    PinnedBuffer<float> h_flow[kFlowRing];
+    PinnedBuffer<uint8_t> h_q[kFlowRing];
     std::unique_ptr<JpegEncoder> jpeg;  // nvJPEG encoder / decoder states, created on first use
-    // scratch of dfb_process_bgr_batch_host (grown on demand)
-    cudaStream_t s_fetch = nullptr;       // bitstream read-back of the BGR chain
-    std::vector<cudaEvent_t> pb_events;   // events of the BGR chain (grown on demand)
-    uint8_t *pb_bgr = nullptr, *pb_gray = nullptr, *pb_frames = nullptr, *pb_q = nullptr;
-    size_t pb_bgr_cap = 0, pb_gray_cap = 0, pb_frames_cap = 0, pb_q_cap = 0;
-    uint8_t *dec_bgr = nullptr;  // BGR scratch of dfb_decode_jpeg_gray_device
+    // scratch of the flow chains (dfb_process_*_batch_host), grown on demand
+    DeviceBuffer<uint8_t> pb_bgr, pb_gray, pb_frames, pb_q;
+    struct {
+        Events frame;      // [n_frames] frame f is in pb_frames
+        Events gray;       // [2] BGR staging buffer consumed
+        Events flow, enc;  // [2] a group's planes ready, its encodes done
+    } chain_ev;
+    DeviceBuffer<uint8_t> dec_bgr;      // BGR scratch of dfb_decode_jpeg_gray_device
     std::unique_ptr<JpegDecoder> jdec;  // imdecode-exact JPEG decoder, created on first use
-    size_t dec_bgr_cap = 0;
-    void *png_scratch = nullptr;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
-    std::unique_ptr<PngEncoder> png;  // imencode(".png") workspace and files, created on first use
-    uint8_t *png_bgr = nullptr;       // packed images of dfb_calc_batch_host_png, one per flow ring slot
-    size_t png_bgr_cap = 0;
-    uint64_t *png_lens_host = nullptr;  // pinned file lengths of the two groups in flight
+    DeviceBuffer<uint8_t> png_scratch;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
+    std::unique_ptr<PngEncoder> png;    // imencode(".png") workspace and files, created on first use
+    DeviceBuffer<uint8_t> png_bgr;      // packed images of dfb_calc_batch_host_png, one per flow ring slot
     TapTable gray_taps;  // dfb_resize_gray_device
     // scratch of the frame-extraction calls (-s=0), grown on demand
-    TapTable ycc_taps;                          // colour resize of all three calls
-    uint8_t *enc_ycc = nullptr;                 // Y / Cb / Cr planes of dfb_encode_jpeg_bgr_device
-    size_t enc_ycc_cap = 0;
-    uint8_t *ex_bgr = nullptr, *ex_ycc = nullptr;  // dfb_extract_frames_host: two staging frames, planes of two groups
-    size_t ex_bgr_cap = 0, ex_ycc_cap = 0;
-    cudaEvent_t ex_events[8] = {};
+    TapTable ycc_taps;                // colour resize of all three calls
+    DeviceBuffer<uint8_t> enc_ycc;    // Y / Cb / Cr planes of dfb_encode_jpeg_bgr_device
+    DeviceBuffer<uint8_t> ex_bgr, ex_ycc;  // dfb_extract_frames_host: two staging frames, planes of two groups
+    struct {
+        Events h2d, conv;     // [2] staging buffer filled, consumed
+        Events planes, enc;   // [2] a group's planes ready, its encodes done
+    } extract_ev;
     // "jpeg_exact" = 1: every JPEG this handle writes is imencode(".jpg")'s bytes (JpegExactEncoder) instead of nvJPEG's
     bool jpeg_exact = false;
     std::unique_ptr<JpegExactEncoder> jex;  // created on first use
-    uint64_t *jex_lens_host = nullptr;      // pinned file lengths of the two groups in flight
-    int jex_lens_n = 0;                     // per slot
+
+    ~dfb_handle() {
+        for (cudaStream_t s : {s_in, s_compute, s_out, s_fetch})
+            if (s) cudaStreamDestroy(s);
+    }
 };
 
 namespace {
@@ -140,15 +167,15 @@ int check_size(dfb_handle *h, int w, int h_) {
 
 // pinned staging buffers exist only for callers that pass pageable memory: allocated on first use
 uint8_t *stage_frame(dfb_handle *h, int r) {
-    if (!h->h_frame[r]) DFB_CUDA(cudaHostAlloc(&h->h_frame[r], (size_t)h->max_w * h->max_h, cudaHostAllocDefault));
+    h->h_frame[r].allocate((size_t)h->max_w * h->max_h);
     return h->h_frame[r];
 }
 float *stage_flow(dfb_handle *h, int r) {
-    if (!h->h_flow[r]) DFB_CUDA(cudaHostAlloc(&h->h_flow[r], (size_t)h->max_w * h->max_h * 2 * sizeof(float), cudaHostAllocDefault));
+    h->h_flow[r].allocate((size_t)h->max_w * h->max_h * 2 * sizeof(float));
     return h->h_flow[r];
 }
 uint8_t *stage_q(dfb_handle *h, int r) {
-    if (!h->h_q[r]) DFB_CUDA(cudaHostAlloc(&h->h_q[r], (size_t)h->max_w * h->max_h * 2, cudaHostAllocDefault));
+    h->h_q[r].allocate((size_t)h->max_w * h->max_h * 2);
     return h->h_q[r];
 }
 
@@ -159,16 +186,17 @@ void ensure_streams(dfb_handle *h) {
     DFB_CUDA(cudaStreamCreateWithFlags(&h->s_out, cudaStreamNonBlocking));
 }
 
+void ensure_fetch_stream(dfb_handle *h) {
+    ensure_streams(h);
+    if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
+}
+
 void ensure_host_path(dfb_handle *h) {
     ensure_streams(h);
-    if (h->d_frame[0]) return;
-    const size_t fpitch = (size_t)round_up(h->max_w, 128);
-    h->d_frame_pitch = fpitch;
-    for (int i = 0; i < dfb_handle::kFrameRing; ++i) {
-        DFB_CUDA(cudaMalloc(&h->d_frame[i], fpitch * h->max_h));
-        DFB_CUDA(cudaEventCreateWithFlags(&h->ev_in[i], cudaEventDisableTiming));
-        DFB_CUDA(cudaEventCreateWithFlags(&h->ev_pyr[i], cudaEventDisableTiming));
-    }
+    h->d_frame_pitch = (size_t)round_up(h->max_w, 128);
+    for (auto &f : h->d_frame) f.allocate(h->d_frame_pitch * h->max_h);
+    h->ev_in.ensure(dfb_handle::kFrameRing);
+    h->ev_pyr.ensure(dfb_handle::kFrameRing);
 }
 
 // The x and y tables of a sw x sh -> dw x dh INTER_LINEAR resize (x: coefficients reset at the borders, y: rows clamped).
@@ -179,11 +207,7 @@ const ResizeTap *ensure_taps(TapTable &t, int sw, int sh, int dw, int dh) {
         build_resize_taps(dw, sw, true, xt);
         build_resize_taps(dh, sh, false, yt);
         DFB_CUDA(cudaDeviceSynchronize());
-        if (dw + dh > t.cap) {
-            if (t.d) DFB_CUDA(cudaFree(t.d));
-            t.cap = dw + dh;
-            DFB_CUDA(cudaMalloc(&t.d, sizeof(ResizeTap) * t.cap));
-        }
+        t.d.allocate(sizeof(ResizeTap) * (dw + dh));
         DFB_CUDA(cudaMemcpy(t.d, xt.data(), sizeof(ResizeTap) * dw, cudaMemcpyHostToDevice));
         DFB_CUDA(cudaMemcpy(t.d + dw, yt.data(), sizeof(ResizeTap) * dh, cudaMemcpyHostToDevice));
         t.sw = sw;
@@ -192,17 +216,6 @@ const ResizeTap *ensure_taps(TapTable &t, int sw, int sh, int dw, int dh) {
         t.dh = dh;
     }
     return t.d;
-}
-
-// grows a device scratch buffer; work still reading the old one is waited for first
-template <typename T> void grow_device(T *&ptr, size_t &cap, size_t need) {
-    if (need <= cap) return;
-    DFB_CUDA(cudaDeviceSynchronize());
-    if (ptr) DFB_CUDA(cudaFree(ptr));
-    void *p = nullptr;
-    DFB_CUDA(cudaMalloc(&p, need));
-    ptr = static_cast<T *>(p);
-    cap = need;
 }
 
 // 1: device (or managed) memory a kernel may read and write
@@ -245,20 +258,15 @@ const ResizeTap *ycc_tables(dfb_handle *h, int sw, int sh, int dw, int dh) {
     return (sw == dw && sh == dh) ? nullptr : ensure_taps(h->ycc_taps, sw, sh, dw, dh);
 }
 
-// The imencode-exact JPEG encoder, and pinned room for the file lengths of two groups of n files
-JpegExactEncoder &ensure_jex(dfb_handle *h, int n) {
-    if (!h->jex) h->jex.reset(new JpegExactEncoder());
-    if (h->jex_lens_n < n) {
-        DFB_CUDA(cudaDeviceSynchronize());  // a read-back may still target the old buffer
-        if (h->jex_lens_host) DFB_CUDA(cudaFreeHost(h->jex_lens_host));
-        h->jex_lens_host = nullptr;
-        DFB_CUDA(cudaHostAlloc(&h->jex_lens_host, sizeof(uint64_t) * 2 * n, cudaHostAllocDefault));
-        h->jex_lens_n = n;
-    }
-    return *h->jex;
+// the out(k, length) of a call that writes one file to out and its length to *out_len
+auto single_out(uint8_t *out, size_t *out_len) {
+    return [=](int, size_t n) {
+        *out_len = n;
+        return out;
+    };
 }
 
-// the planes of a YccLayout block as the exact encoder reads them
+// the planes of a YccLayout block as a JPEG encoder reads them
 JpegSrc ycc_src(const uint8_t *base, const YccLayout &L) {
     JpegSrc src;
     src.base = base;
@@ -270,45 +278,138 @@ JpegSrc ycc_src(const uint8_t *base, const YccLayout &L) {
     return src;
 }
 
-// Encodes n images of src with the exact encoder into slot 0 and copies file i to out[i] (host), its length to len[i].
-// Blocks until the files are on the host.  `too_small(i, need)` builds the message of a file that does not fit.
-void jex_encode_to_host(dfb_handle *h, int n, const JpegSrc &src, int comps, int w, int hh, int quality, uint8_t *const *out, size_t capacity,
-                        size_t *len, cudaStream_t s, const std::function<std::string(int, size_t)> &too_small) {
-    JpegExactEncoder &jx = ensure_jex(h, n);
-    h->alg->launches += jx.encode(n, src, comps, w, hh, quality, capacity, 0, s);
-    DFB_CUDA(cudaMemcpyAsync(h->jex_lens_host, jx.lens(0), sizeof(uint64_t) * n, cudaMemcpyDeviceToHost, s));
-    DFB_CUDA(cudaStreamSynchronize(s));
-    for (int i = 0; i < n; ++i)
-        if (h->jex_lens_host[i] > capacity) throw std::runtime_error(too_small(i, jx.needed(h->jex_lens_host[i], src, i, comps, w, hh, quality, s)));
-    for (int i = 0; i < n; ++i) {
-        len[i] = (size_t)h->jex_lens_host[i];
-        DFB_CUDA(cudaMemcpyAsync(out[i], jx.file(0, i), len[i], cudaMemcpyDeviceToHost, s));
-        h->counters.d2h_bytes += len[i];
+// The JPEG files of a call, encoded in groups into two slots of up to `per_slot` files each, so one group can be read back
+// while the next is encoded.  The handle's "jpeg_exact" picks the encoder: JpegExactEncoder, or nvJPEG with file k of slot s
+// in encoder state s * per_slot + k.
+class JpegSink {
+  public:
+    // slots: how many slots the call uses (1 or 2); always_exact: the call writes imencode's bytes whatever the handle says
+    JpegSink(dfb_handle *h, int per_slot, int slots, bool always_exact = false) : h_(h), per_slot_(per_slot) {
+        if (always_exact || h->jpeg_exact) {
+            if (!h->jex) h->jex.reset(new JpegExactEncoder());
+            jex_ = h->jex.get();
+        } else {
+            if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
+            h->jpeg->ensure_states(slots * per_slot);
+        }
     }
-    DFB_CUDA(cudaStreamSynchronize(s));
-}
+    bool exact() const { return jex_ != nullptr; }
+    // the chroma columns launch_bgr_to_ycc420 writes for this encoder (0: the image's own)
+    int chroma_cols(int w) const { return jex_ ? jpeg_chroma_cols(w) : 0; }
+    // Enqueues the encodes of n images of src into `slot` on s, each file to be at most capacity bytes; the exact encoder's
+    // lengths follow them to the host on s.
+    void encode(int slot, int n, const JpegSrc &src, int components, int w, int hh, int quality, size_t capacity, cudaStream_t s) {
+        group_[slot] = Group{src, components, w, hh, quality, capacity};
+        if (jex_) {
+            h_->alg->launches += jex_->encode(n, src, components, w, hh, quality, capacity, slot, s);
+            return;
+        }
+        for (int k = 0; k < n; ++k) {
+            const uint8_t *p = src.base + (size_t)k * src.img_stride;
+            if (components == 1)
+                h_->jpeg->enqueue(slot * per_slot_ + k, p, src.pitch, w, hh, quality, s);
+            else
+                h_->jpeg->enqueue_ycc420(slot * per_slot_ + k, p, src.pitch, p + src.cb_off, p + src.cr_off, src.c_pitch, w, hh, quality, s);
+        }
+    }
+    // Once the slot's encode is complete: in file order, a file over capacity fails the call with
+    // std::runtime_error(too_small(k, bytes it needs)) for the first such file k.  File k is copied to out(k, length) on s,
+    // the bytes are added to d2h_bytes and s is synchronised.
+    template <typename TooSmall, typename Out> void deliver(int slot, int n, TooSmall &&too_small, Out &&out, cudaStream_t s) {
+        const Group &g = group_[slot];
+        if (jex_) {
+            auto reject = [&](int k, uint64_t reported) {
+                return too_small(k, jex_->needed(reported, g.src, k, g.components, g.w, g.h, g.quality, s));
+            };
+            jex_->files().deliver(slot, n, g.capacity, reject, out, h_->counters.d2h_bytes, s);
+            return;
+        }
+        for (int k = 0; k < n; ++k) {
+            const int st = slot * per_slot_ + k;
+            const size_t len = h_->jpeg->length(st, s);
+            if (len > g.capacity) throw std::runtime_error(too_small(k, len));
+            h_->jpeg->fetch(st, out(k, len), len, s);
+            h_->counters.d2h_bytes += len;
+        }
+        DFB_CUDA(cudaStreamSynchronize(s));
+    }
+
+  private:
+    struct Group {
+        JpegSrc src;
+        int components, w, h, quality;
+        size_t capacity;
+    };
+    dfb_handle *h_;
+    int per_slot_;
+    JpegExactEncoder *jex_ = nullptr;
+    Group group_[2] = {};
+};
 
 // output ring slots [0, n): allocated on first use (a 1080p handle runs 7 pairs per launch and touches 14 slots, a 340x256
 // one up to 64 pairs per launch)
 void ensure_flow_ring(dfb_handle *h, int n, bool quantised) {
+    h->ev_done.ensure(n);
+    h->ev_out.ensure(n);
+    const size_t px = (size_t)h->max_w * h->max_h;
     for (int i = 0; i < n; ++i) {
-        if (!h->ev_done[i]) {
-            DFB_CUDA(cudaEventCreateWithFlags(&h->ev_done[i], cudaEventDisableTiming));
-            DFB_CUDA(cudaEventCreateWithFlags(&h->ev_out[i], cudaEventDisableTiming));
-        }
-        if (!quantised && !h->d_flow[i]) DFB_CUDA(cudaMalloc(&h->d_flow[i], (size_t)h->max_w * h->max_h * 2 * sizeof(float)));
-        if (quantised && !h->d_qx[i]) {
-            DFB_CUDA(cudaMalloc(&h->d_qx[i], (size_t)h->max_w * h->max_h));
-            DFB_CUDA(cudaMalloc(&h->d_qy[i], (size_t)h->max_w * h->max_h));
+        if (quantised) {
+            h->d_qx[i].allocate(px);
+            h->d_qy[i].allocate(px);
+        } else {
+            h->d_flow[i].allocate(px * 2 * sizeof(float));
         }
     }
 }
 
 void ensure_png_scratch(dfb_handle *h) {
     if (h->png_scratch) return;
-    DFB_CUDA(cudaMalloc(&h->png_scratch, png_pack_scratch_bytes()));
+    h->png_scratch.allocate(png_pack_scratch_bytes());
     DFB_CUDA(cudaMemset(h->png_scratch, 0, png_pack_scratch_bytes()));
     DFB_CUDA(cudaDeviceSynchronize());
+}
+
+// Runs stage(g) for the groups g = 0..G-1 and finish(g - 1) after each, then finish(G - 1): the files of group g - 1 are read
+// back while the GPU works on group g.
+template <typename Stage, typename Finish> void run_groups(int G, Stage &&stage, Finish &&finish) {
+    for (int g = 0; g < G; ++g) {
+        stage(g);
+        if (g > 0) finish(g - 1);
+    }
+    finish(G - 1);
+}
+
+// pair j of a batch: frames j and j + |step| (:315-316), in engine slots modulo nslots
+FlowAlgorithm::PairJob pair_job(int j, int step, int nslots) {
+    const int astep = std::abs(step);
+    FlowAlgorithm::PairJob pj{};
+    pj.slot_a = (step > 0 ? j : j + astep) % nslots;
+    pj.slot_b = (step > 0 ? j + astep : j) % nslots;
+    return pj;
+}
+
+// Enqueues on s the preparation of frames [prepared, last] of a dense array (frame f: w x hh bytes at frames + f * w * hh)
+// into their engine slots, as one batch; prepared ends at last + 1.
+void prepare_dense(FlowAlgorithm &alg, const uint8_t *frames, int w, int hh, int &prepared, int last, cudaStream_t s) {
+    std::vector<const uint8_t *> srcs;
+    std::vector<int> slots;
+    for (; prepared <= last; ++prepared) {
+        srcs.push_back(frames + (size_t)w * hh * prepared);
+        slots.push_back(prepared % alg.num_slots());
+    }
+    if (!srcs.empty()) alg.prepare_frames((int)srcs.size(), srcs.data(), w, w, hh, slots.data(), s);
+}
+
+// cv::resize(INTER_LINEAR) of a device gray plane, enqueued on s; an equal size is a copy
+void resize_gray(dfb_handle *h, const uint8_t *src, size_t src_pitch, int sw, int sh, uint8_t *dst, size_t dst_pitch, int dw, int dh,
+                 cudaStream_t s) {
+    if (sw == dw && sh == dh) {
+        DFB_CUDA(cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, sw, sh, cudaMemcpyDeviceToDevice, s));
+        return;
+    }
+    const ResizeTap *taps = ensure_taps(h->gray_taps, sw, sh, dw, dh);
+    launch_resize_u8(src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, taps, taps + dw, s);
+    ++h->alg->launches;
 }
 
 // PNG output of batch_host (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j]
@@ -354,27 +455,26 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
     if (bound > 0 && alg.get_param("fused", &fused_flag) && fused_flag == 0) ensure_flow_ring(h, OR, false);
     const size_t bgr_bytes = fbytes * 3;
     if (png) {
-        if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
+        ensure_fetch_stream(h);
         ensure_png_scratch(h);
-        grow_device(h->png_bgr, h->png_bgr_cap, OR * bgr_bytes);
-        if (!h->png_lens_host) DFB_CUDA(cudaHostAlloc(&h->png_lens_host, sizeof(uint64_t) * dfb_handle::kFlowRing, cudaHostAllocDefault));
+        h->png_bgr.grow(OR * bgr_bytes);
         if (!h->png) h->png.reset(new PngEncoder());
     }
     // -st=png: the files of group g (slot g & 1) are read back while the GPU works on group g + 1
     auto png_finish = [&](int g) {
-        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
+        if (!png) return;
+        const int j0 = g * B, m = std::min(B, M - j0);
         DFB_CUDA(cudaEventSynchronize(h->ev_out[(j0 + m - 1) % OR]));
-        for (int i = 0; i < m; ++i) {
-            const size_t n = (size_t)h->png_lens_host[slot * B + i];
-            if (n == 0) throw std::runtime_error("png encoder failed on pair " + std::to_string(j0 + i));
-            if (n > png->capacity)
-                throw std::runtime_error("png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) +
-                                         " bytes, capacity is " + std::to_string(png->capacity));
+        auto reject = [&](int i, uint64_t n) {
+            if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
+            return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
+                   std::to_string(png->capacity);
+        };
+        auto out = [&](int i, size_t n) {
             png->len[j0 + i] = n;
-            DFB_CUDA(cudaMemcpyAsync(png->out[j0 + i], h->png->file(slot, i), n, cudaMemcpyDeviceToHost, h->s_fetch));
-            h->counters.d2h_bytes += n;
-        }
-        DFB_CUDA(cudaStreamSynchronize(h->s_fetch));
+            return png->out[j0 + i];
+        };
+        h->png->files().deliver(g & 1, m, png->capacity, reject, out, h->counters.d2h_bytes, h->s_fetch);
     };
 
     int uploaded = 0;  // frames [0, uploaded) have H2D + pyramid enqueued
@@ -423,22 +523,18 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
     };
 
     std::vector<FlowAlgorithm::PairJob> jobs(B);
-    for (int j0 = 0; j0 < M; j0 += B) {
-        const int m = std::min(B, M - j0);
+    auto stage = [&](int g) {
+        const int j0 = g * B, m = std::min(B, M - j0);
         // frames of this group (+ one ahead, so its H2D overlaps the solve)
         const int last_needed = j0 + m - 1 + astep;  // pairs j0..j0+m-1 touch frames j0..j0+m-1+|step| for either sign of step
         upload_until(std::min(last_needed + 1, n_frames - 1));
         for (int i = 0; i < m; ++i) {
             const int j = j0 + i;
-            const int a = step > 0 ? j : j + astep;  // :315
-            const int b = step > 0 ? j + astep : j;  // :316
             const int ring = j % OR;
             drain(ring);
             if (j >= OR) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, h->ev_out[ring], 0));  // device output slot is free
             FlowAlgorithm::PairJob &pj = jobs[i];
-            pj = FlowAlgorithm::PairJob{};
-            pj.slot_a = a % nslots;
-            pj.slot_b = b % nslots;
+            pj = pair_job(j, step, nslots);
             pj.flow_xy = h->d_flow[ring];  // null in quantised mode unless the engine needs the scratch (see above)
             pj.flow_pitch_bytes = (size_t)w * 2 * sizeof(float);
             if (bound > 0) {  // f1: the engine's merge epilogue writes the two uint8 planes directly
@@ -452,7 +548,7 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
         if (png) {
             // s_compute: convertFlowToPngImage of every pair (src/common.cpp:18-46); s_out: imencode(".png") of the group
             // (:66-71); s_fetch: the previous group's files to the host
-            const int r0 = j0 % OR, g = j0 / B, slot = g & 1;
+            const int r0 = j0 % OR;
             uint8_t *bgr0 = h->png_bgr + (size_t)r0 * bgr_bytes;
             for (int i = 0; i < m; ++i)
                 launch_flow_to_png_image(h->d_flow[r0 + i], (size_t)w * 8, w, hh, bgr0 + (size_t)i * bgr_bytes, (size_t)w * 3, h->png_scratch,
@@ -460,13 +556,10 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
             alg.launches += 2 * m;
             DFB_CUDA(cudaEventRecord(h->ev_done[r0], h->s_compute));
             DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[r0], 0));
-            alg.launches += h->png->encode(m, bgr0, bgr_bytes, (size_t)w * 3, w, hh, slot, h->s_out);
-            DFB_CUDA(cudaMemcpyAsync(h->png_lens_host + slot * B, h->png->lens(slot), sizeof(uint64_t) * m, cudaMemcpyDeviceToHost, h->s_out));
+            alg.launches += h->png->encode(m, bgr0, bgr_bytes, (size_t)w * 3, w, hh, g & 1, h->s_out);
             for (int i = 0; i < m; ++i) DFB_CUDA(cudaEventRecord(h->ev_out[r0 + i], h->s_out));
             h->counters.pairs += m;
-            if (g > 0) png_finish(g - 1);
-            if (j0 + m == M) png_finish(g);
-            continue;
+            return;
         }
         DFB_CUDA(cudaEventRecord(h->ev_done[j0 % OR], h->s_compute));
         DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[j0 % OR], 0));
@@ -489,7 +582,8 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
             DFB_CUDA(cudaEventRecord(h->ev_out[ring], h->s_out));
             ++h->counters.pairs;  // total_flows += 1 (:340)
         }
-    }
+    };
+    run_groups((M + B - 1) / B, stage, png_finish);
     DFB_CUDA(cudaStreamSynchronize(h->s_out));
     for (int r = 0; r < OR; ++r) drain(r);
     DFB_CUDA(cudaStreamSynchronize(h->s_compute));
@@ -554,42 +648,6 @@ void dfb_destroy(dfb_handle *h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
-    for (int i = 0; i < dfb_handle::kFrameRing; ++i) {
-        if (h->d_frame[i]) cudaFree(h->d_frame[i]);
-        if (h->h_frame[i]) cudaFreeHost(h->h_frame[i]);
-        if (h->ev_in[i]) cudaEventDestroy(h->ev_in[i]);
-        if (h->ev_pyr[i]) cudaEventDestroy(h->ev_pyr[i]);
-    }
-    for (int i = 0; i < dfb_handle::kFlowRing; ++i) {
-        if (h->d_flow[i]) cudaFree(h->d_flow[i]);
-        if (h->d_qx[i]) cudaFree(h->d_qx[i]);
-        if (h->d_qy[i]) cudaFree(h->d_qy[i]);
-        if (h->h_flow[i]) cudaFreeHost(h->h_flow[i]);
-        if (h->h_q[i]) cudaFreeHost(h->h_q[i]);
-        if (h->ev_done[i]) cudaEventDestroy(h->ev_done[i]);
-        if (h->ev_out[i]) cudaEventDestroy(h->ev_out[i]);
-    }
-    h->jpeg.reset();
-    for (void *p : {(void *)h->pb_bgr, (void *)h->pb_gray, (void *)h->pb_frames, (void *)h->pb_q})
-        if (p) cudaFree(p);
-    for (void *p : {(void *)h->gray_taps.d, (void *)h->ycc_taps.d, (void *)h->enc_ycc, (void *)h->ex_bgr, (void *)h->ex_ycc})
-        if (p) cudaFree(p);
-    for (auto e : h->ex_events)
-        if (e) cudaEventDestroy(e);
-    if (h->png_scratch) cudaFree(h->png_scratch);
-    h->png.reset();
-    h->jdec.reset();
-    h->jex.reset();
-    if (h->jex_lens_host) cudaFreeHost(h->jex_lens_host);
-    if (h->png_bgr) cudaFree(h->png_bgr);
-    if (h->png_lens_host) cudaFreeHost(h->png_lens_host);
-    if (h->dec_bgr) cudaFree(h->dec_bgr);
-    for (auto e : h->pb_events) cudaEventDestroy(e);
-    if (h->s_fetch) cudaStreamDestroy(h->s_fetch);
-    if (h->s_in) cudaStreamDestroy(h->s_in);
-    if (h->s_compute) cudaStreamDestroy(h->s_compute);
-    if (h->s_out) cudaStreamDestroy(h->s_out);
-    h->alg.reset();
     delete h;
 }
 
@@ -696,22 +754,10 @@ int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, in
         std::vector<FlowAlgorithm::PairJob> jobs(B);
         for (int j0 = 0; j0 < M; j0 += B) {
             const int m = std::min(B, M - j0);
-            {
-                std::vector<const uint8_t *> srcs;
-                std::vector<int> slots;
-                for (; prepared <= j0 + m - 1 + astep; ++prepared) {
-                    srcs.push_back(frames + (size_t)prepared * fbytes);
-                    slots.push_back(prepared % nslots);
-                }
-                if (!srcs.empty()) alg.prepare_frames((int)srcs.size(), srcs.data(), width, width, height, slots.data(), s);
-            }
+            prepare_dense(alg, frames, width, height, prepared, j0 + m - 1 + astep, s);
             for (int i = 0; i < m; ++i) {
                 const int j = j0 + i;
-                const int a = step > 0 ? j : j + astep;
-                const int b = step > 0 ? j + astep : j;
-                jobs[i] = FlowAlgorithm::PairJob{};
-                jobs[i].slot_a = a % nslots;
-                jobs[i].slot_b = b % nslots;
+                jobs[i] = pair_job(j, step, nslots);
                 jobs[i].flow_xy = flows + (size_t)j * fbytes * 2;
                 jobs[i].flow_pitch_bytes = (size_t)width * 8;
             }
@@ -787,14 +833,7 @@ int dfb_resize_gray_device(dfb_handle *h, const uint8_t *src, size_t src_pitch, 
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
-        cudaStream_t s = static_cast<cudaStream_t>(stream);
-        if (sw == dw && sh == dh) {  // cv::resize with an equal size is a copy
-            DFB_CUDA(cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, sw, sh, cudaMemcpyDeviceToDevice, s));
-            return DFB_OK;
-        }
-        const ResizeTap *taps = ensure_taps(h->gray_taps, sw, sh, dw, dh);
-        launch_resize_u8(src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, taps, taps + dw, s);
-        ++h->alg->launches;
+        resize_gray(h, src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, static_cast<cudaStream_t>(stream));
         return DFB_OK;
     });
 }
@@ -812,18 +851,18 @@ int dfb_encode_jpeg_gray_device(dfb_handle *h, const uint8_t *gray, size_t gray_
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry or quality");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
-        if (h->jpeg_exact) {
-            JpegSrc src;
-            src.base = gray;
-            src.pitch = gray_pitch;
-            jex_encode_to_host(h, 1, src, 1, width, height, quality, &out, out_capacity, out_len, static_cast<cudaStream_t>(stream),
-                               [&](int, size_t need) {
-                                   return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(out_capacity) + ")";
-                               });
-            return DFB_OK;
-        }
-        if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
-        *out_len = h->jpeg->encode_gray(gray, gray_pitch, width, height, quality, out, out_capacity, static_cast<cudaStream_t>(stream));
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        JpegSink sink(h, 1, 1);
+        JpegSrc src;
+        src.base = gray;
+        src.pitch = gray_pitch;
+        sink.encode(0, 1, src, 1, width, height, quality, out_capacity, s);
+        DFB_CUDA(cudaStreamSynchronize(s));
+        auto too_small = [&](int, size_t need) {
+            return std::string(sink.exact() ? "jpeg output" : "nvjpeg: output") + " buffer too small (" + std::to_string(need) + " > " +
+                   std::to_string(out_capacity) + ")";
+        };
+        sink.deliver(0, 1, too_small, single_out(out, out_len), s);
         return DFB_OK;
     });
 }
@@ -844,13 +883,22 @@ int dfb_encode_jpeg_gray_batch_device(dfb_handle *h, const uint8_t *planes, size
             return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(i) + " is null or a device pointer (host entry point)");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        JpegSink sink(h, n, 1, true);
         JpegSrc src;
         src.base = planes;
         src.pitch = pitch;
         src.img_stride = plane_stride;
-        jex_encode_to_host(h, n, src, 1, width, height, quality, out, capacity, len, static_cast<cudaStream_t>(stream), [&](int i, size_t need) {
+        sink.encode(0, n, src, 1, width, height, quality, capacity, s);
+        DFB_CUDA(cudaStreamSynchronize(s));
+        auto too_small = [&](int i, size_t need) {
             return "jpeg output buffer too small: plane " + std::to_string(i) + " (" + std::to_string(need) + " > " + std::to_string(capacity) + ")";
-        });
+        };
+        auto to = [&](int i, size_t n) {
+            len[i] = n;
+            return out[i];
+        };
+        sink.deliver(0, n, too_small, to, s);
         return DFB_OK;
     });
 }
@@ -870,13 +918,7 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
         if (w <= 0 || hh <= 0) return fail(h, DFB_ERR_INVALID_ARG, "not a JPEG image");
         if (w > max_width || hh > max_height || gray_pitch < (size_t)w)
             return fail(h, DFB_ERR_SIZE, "decoded frame " + std::to_string(w) + "x" + std::to_string(hh) + " does not fit the output buffer");
-        const size_t need = (size_t)w * hh * 3;
-        if (need > h->dec_bgr_cap) {
-            DFB_CUDA(cudaDeviceSynchronize());
-            if (h->dec_bgr) DFB_CUDA(cudaFree(h->dec_bgr));
-            DFB_CUDA(cudaMalloc(&h->dec_bgr, need));
-            h->dec_bgr_cap = need;
-        }
+        h->dec_bgr.grow((size_t)w * hh * 3);
         // imread(IMREAD_COLOR) -> BGR, then the decode stage's cvtColor(BGR2GRAY) (src/denseflow_gpu.cpp:160-163), bit-exact from there on
         h->jpeg->decode_bgr(jpeg, jpeg_len, h->dec_bgr, (size_t)w * 3, w, hh, s);
         launch_bgr_to_gray(h->dec_bgr, (size_t)w * 3, w, hh, gray, gray_pitch, s);
@@ -900,146 +942,92 @@ int check_chain_outputs(dfb_handle *h, int M, uint8_t *const *jpg_x, uint8_t *co
 
 // The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) -> flow -> quantise -> two JPEGs per pair.
 // `produce(first, last)` enqueues on s_in the work that leaves frames [first, last] in h->pb_frames (dw x dh each, dense)
-// and records ev_frame[f] (h->pb_events[8 + f]) for each; frames are requested in order.  Runs inside guarded().
-int process_chain(dfb_handle *h, int n_frames, int step, int sw, int sh, int dw, int dh, int bound, int jpeg_quality,
-                  uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y,
-                  const std::function<void(int, int)> &produce) {
+// and records h->chain_ev.frame[f] for each; frames are requested in order.  Runs inside guarded().
+int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, int bound, int jpeg_quality, uint8_t *const *jpg_x,
+                  uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y, const std::function<void(int, int)> &produce) {
     const int astep = std::abs(step);
     const int M = std::max(n_frames - astep, 0);
-    {
-        ensure_host_path(h);
-        if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
-        FlowAlgorithm &alg = *h->alg;
-        alg.begin_batch();
-        auto grow = [&](uint8_t *&ptr, size_t &cap, size_t need) { grow_device(ptr, cap, need); };
-        // Three stages on three streams, groups of B pairs in flight (the reference runs the same three stages as three host
-        // threads around queues, include/dense_flow.h:76-80):
-        //   s_in      the frame source: decoded frames -> gray -> resize into the gray frame array (decode stage, :154-170)
-        //   s_compute pyramids / polynomial expansions + flow of group g, quantised planes out   (:313-342 + src/common.cpp:4-16)
-        //   s_out     two JPEG encodes per pair of group g (nvJPEG, one encoder state per plane)  (src/common.cpp:56-57)
-        //   s_fetch   bitstreams of group g-1 to the host while the GPU works on group g
-        const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
-        const size_t fpx = (size_t)dw * dh;
-        grow(h->pb_frames, h->pb_frames_cap, fpx * n_frames);
-        grow(h->pb_q, h->pb_q_cap, fpx * 2 * 2 * B);              // quantised planes of two groups
-        alg.ensure_slots(B + astep + 1);
-        const int nslots = alg.num_slots();
-        while ((int)h->pb_events.size() < n_frames + 8) {
-            cudaEvent_t e;
-            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->pb_events.push_back(e);
-        }
-        cudaEvent_t *ev_frame = h->pb_events.data() + 8;          // [n_frames]
-        cudaEvent_t *ev_flow = h->pb_events.data() + 2;            // [2] group's planes ready
-        cudaEvent_t *ev_enc = h->pb_events.data() + 4;             // [2] group's encodes done
-        const bool exact = h->jpeg_exact;
-        if (exact) {
-            ensure_jex(h, 2 * B);
-        } else {
-            if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
-            h->jpeg->ensure_states(4 * B);
-        }
-        // the exact encoder reads the group's 2 m planes as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
-        auto group_planes = [&](int slot) {
-            JpegSrc src;
-            src.base = h->pb_q + (size_t)slot * B * 2 * fpx;
-            src.img_stride = fpx;
-            src.pitch = (size_t)dw;
-            return src;
-        };
+    ensure_host_path(h);
+    ensure_fetch_stream(h);
+    FlowAlgorithm &alg = *h->alg;
+    alg.begin_batch();
+    // Three stages on three streams, groups of B pairs in flight (the reference runs the same three stages as three host
+    // threads around queues, include/dense_flow.h:76-80):
+    //   s_in      the frame source: decoded frames -> gray -> resize into the gray frame array (decode stage, :154-170)
+    //   s_compute pyramids / polynomial expansions + flow of group g, quantised planes out   (:313-342 + src/common.cpp:4-16)
+    //   s_out     the two JPEG encodes per pair of group g, as one batch                      (src/common.cpp:56-57)
+    //   s_fetch   files of group g-1 to the host while the GPU works on group g
+    const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
+    const size_t fpx = (size_t)dw * dh;
+    h->pb_frames.grow(fpx * n_frames);
+    h->pb_q.grow(fpx * 2 * 2 * B);  // quantised planes of two groups
+    alg.ensure_slots(B + astep + 1);
+    const int nslots = alg.num_slots();
+    auto &ev = h->chain_ev;
+    ev.frame.ensure(n_frames);
+    ev.gray.ensure(2);
+    ev.flow.ensure(2);
+    ev.enc.ensure(2);
+    JpegSink sink(h, 2 * B, 2);
+    // the group's 2 m planes, encoded as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
+    auto group_planes = [&](int slot) {
+        JpegSrc src;
+        src.base = h->pb_q + (size_t)slot * B * 2 * fpx;
+        src.img_stride = fpx;
+        src.pitch = (size_t)dw;
+        return src;
+    };
 
-        int uploaded = 0;
-        auto upload_until = [&](int last) {
-            last = std::min(last, n_frames - 1);
-            if (uploaded > last) return;
-            produce(uploaded, last);
-            uploaded = last + 1;
-        };
-        int prepared = 0;
-        std::vector<FlowAlgorithm::PairJob> jobs(B);
-        auto flow_group = [&](int g) {
-            const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
-            const int last_frame = j0 + m - 1 + astep;
-            upload_until(last_frame + 1);
-            DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_frame[last_frame], 0));
-            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_enc[slot], 0));  // the planes of group g-2 have been encoded
-            {
-                std::vector<const uint8_t *> srcs;
-                std::vector<int> slots;
-                for (; prepared <= last_frame; ++prepared) {
-                    srcs.push_back(h->pb_frames + fpx * prepared);
-                    slots.push_back(prepared % nslots);
-                }
-                if (!srcs.empty()) alg.prepare_frames((int)srcs.size(), srcs.data(), dw, dw, dh, slots.data(), h->s_compute);
-            }
-            for (int i = 0; i < m; ++i) {
-                const int j = j0 + i;
-                FlowAlgorithm::PairJob &pj = jobs[i];
-                pj = FlowAlgorithm::PairJob{};
-                pj.slot_a = (step > 0 ? j : j + astep) % nslots;  // :315
-                pj.slot_b = (step > 0 ? j + astep : j) % nslots;  // :316
-                pj.bound = bound;
-                pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
-                pj.qy = pj.qx + fpx;
-                pj.q_pitch = (size_t)dw;
-            }
-            alg.solve_batch(jobs.data(), m, dw, dh, h->s_compute);
-            DFB_CUDA(cudaEventRecord(ev_flow[slot], h->s_compute));
-            // encode stage (src/common.cpp:48-64): one JPEG per plane
-            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev_flow[slot], 0));
-            if (exact) {
-                alg.launches += h->jex->encode(2 * m, group_planes(slot), 1, dw, dh, jpeg_quality, capacity, slot, h->s_out);
-                DFB_CUDA(cudaMemcpyAsync(h->jex_lens_host + (size_t)slot * h->jex_lens_n, h->jex->lens(slot), sizeof(uint64_t) * 2 * m,
-                                         cudaMemcpyDeviceToHost, h->s_out));
-            }
-            for (int i = 0; i < m && !exact; ++i) {
-                const uint8_t *qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
-                h->jpeg->enqueue((slot * B + i) * 2, qx, dw, dw, dh, jpeg_quality, h->s_out);
-                h->jpeg->enqueue((slot * B + i) * 2 + 1, qx + fpx, dw, dw, dh, jpeg_quality, h->s_out);
-            }
-            DFB_CUDA(cudaEventRecord(ev_enc[slot], h->s_out));
-            h->counters.pairs += m;
-        };
-        auto finish_group = [&](int g) {
-            const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
-            DFB_CUDA(cudaEventSynchronize(ev_enc[slot]));
-            if (exact) {
-                const uint64_t *lens = h->jex_lens_host + (size_t)slot * h->jex_lens_n;
-                for (int k = 0; k < 2 * m; ++k)
-                    if (lens[k] > capacity)
-                        throw std::runtime_error("jpeg output buffer too small (" +
-                                                 std::to_string(h->jex->needed(lens[k], group_planes(slot), k, 1, dw, dh, jpeg_quality, h->s_fetch)) +
-                                                 " > " + std::to_string(capacity) + ")");
-                for (int k = 0; k < 2 * m; ++k) {
-                    const int i = k >> 1, c = k & 1;
-                    const size_t len = (size_t)lens[k];
-                    (c ? len_y : len_x)[j0 + i] = len;
-                    DFB_CUDA(cudaMemcpyAsync((c ? jpg_y : jpg_x)[j0 + i], h->jex->file(slot, k), len, cudaMemcpyDeviceToHost, h->s_fetch));
-                    h->counters.d2h_bytes += len;
-                }
-            }
-            for (int i = 0; i < m && !exact; ++i)
-                for (int c = 0; c < 2; ++c) {
-                    const int st = (slot * B + i) * 2 + c;
-                    const size_t len = h->jpeg->length(st, h->s_fetch);
-                    if (len > capacity) throw std::runtime_error("jpeg output buffer too small (" + std::to_string(len) + " > " + std::to_string(capacity) + ")");
-                    (c ? len_y : len_x)[j0 + i] = len;
-                    h->jpeg->fetch(st, (c ? jpg_y : jpg_x)[j0 + i], len, h->s_fetch);
-                    h->counters.d2h_bytes += len;
-                }
-            DFB_CUDA(cudaStreamSynchronize(h->s_fetch));
-        };
-        const int G = (M + B - 1) / B;
-        for (int g = 0; g < G; ++g) {
-            flow_group(g);
-            if (g > 0) finish_group(g - 1);
+    int uploaded = 0;
+    auto upload_until = [&](int last) {
+        last = std::min(last, n_frames - 1);
+        if (uploaded > last) return;
+        produce(uploaded, last);
+        uploaded = last + 1;
+    };
+    int prepared = 0;
+    std::vector<FlowAlgorithm::PairJob> jobs(B);
+    auto flow_group = [&](int g) {
+        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
+        const int last_frame = j0 + m - 1 + astep;
+        upload_until(last_frame + 1);
+        DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.frame[last_frame], 0));
+        if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // the planes of group g-2 have been encoded
+        prepare_dense(alg, h->pb_frames, dw, dh, prepared, last_frame, h->s_compute);
+        for (int i = 0; i < m; ++i) {
+            FlowAlgorithm::PairJob &pj = jobs[i];
+            pj = pair_job(j0 + i, step, nslots);
+            pj.bound = bound;
+            pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
+            pj.qy = pj.qx + fpx;
+            pj.q_pitch = (size_t)dw;
         }
-        finish_group(G - 1);
-        DFB_CUDA(cudaStreamSynchronize(h->s_in));
-        DFB_CUDA(cudaStreamSynchronize(h->s_compute));
-        DFB_CUDA(cudaStreamSynchronize(h->s_out));
-        return DFB_OK;
-    }
+        alg.solve_batch(jobs.data(), m, dw, dh, h->s_compute);
+        DFB_CUDA(cudaEventRecord(ev.flow[slot], h->s_compute));
+        // encode stage (src/common.cpp:48-64): one JPEG per plane
+        DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.flow[slot], 0));
+        sink.encode(slot, 2 * m, group_planes(slot), 1, dw, dh, jpeg_quality, capacity, h->s_out);
+        DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
+        h->counters.pairs += m;
+    };
+    auto finish_group = [&](int g) {
+        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
+        DFB_CUDA(cudaEventSynchronize(ev.enc[slot]));
+        auto too_small = [&](int, size_t need) {
+            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(capacity) + ")";
+        };
+        auto out = [&](int k, size_t len) {
+            const int j = j0 + (k >> 1);
+            (k & 1 ? len_y : len_x)[j] = len;
+            return (k & 1 ? jpg_y : jpg_x)[j];
+        };
+        sink.deliver(slot, 2 * m, too_small, out, h->s_fetch);
+    };
+    run_groups((M + B - 1) / B, flow_group, finish_group);
+    DFB_CUDA(cudaStreamSynchronize(h->s_in));
+    DFB_CUDA(cudaStreamSynchronize(h->s_compute));
+    DFB_CUDA(cudaStreamSynchronize(h->s_out));
+    return DFB_OK;
 }
 
 // Every file of a JPEG batch parsed on the host; an unsupported or corrupt header is the call's error.
@@ -1088,19 +1076,13 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
         DFB_CUDA(cudaSetDevice(h->device));
         // frame source: H2D of BGR frame f into staging buffer f & 1 -> cvtColor -> resize (decode stage tail, :163-170)
         const size_t fpx = (size_t)dw * dh, bgr_bytes = (size_t)sw * sh * 3;
-        grow_device(h->pb_bgr, h->pb_bgr_cap, 2 * bgr_bytes);  // two staging frames: H2D of f+1 overlaps gray/resize of f
-        grow_device(h->pb_gray, h->pb_gray_cap, (size_t)sw * sh);
-        while ((int)h->pb_events.size() < n_frames + 8) {
-            cudaEvent_t e;
-            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->pb_events.push_back(e);
-        }
+        h->pb_bgr.grow(2 * bgr_bytes);  // two staging frames: H2D of f+1 overlaps gray/resize of f
+        h->pb_gray.grow((size_t)sw * sh);
         auto produce = [&](int first, int last) {
-            cudaEvent_t *ev_gray = h->pb_events.data();  // [2] staging buffer consumed
-            cudaEvent_t *ev_frame = h->pb_events.data() + 8;
+            auto &ev = h->chain_ev;
             for (int f = first; f <= last; ++f) {
                 const int sb = f & 1;
-                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev_gray[sb], 0));
+                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev.gray[sb], 0));
                 uint8_t *stage = h->pb_bgr + (size_t)sb * bgr_bytes;
                 DFB_CUDA(cudaMemcpyAsync(stage, bgr[f], bgr_bytes, cudaMemcpyHostToDevice, h->s_in));
                 h->counters.h2d_bytes += bgr_bytes;
@@ -1109,15 +1091,14 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
                     launch_bgr_to_gray(stage, (size_t)sw * 3, sw, sh, dst, dw, h->s_in);
                 } else {
                     launch_bgr_to_gray(stage, (size_t)sw * 3, sw, sh, h->pb_gray, sw, h->s_in);
-                    const int rc = dfb_resize_gray_device(h, h->pb_gray, sw, sw, sh, dst, dw, dw, dh, h->s_in);
-                    if (rc != DFB_OK) throw std::runtime_error(h->last_error);
+                    resize_gray(h, h->pb_gray, sw, sw, sh, dst, dw, dw, dh, h->s_in);
                 }
                 h->alg->launches += 1;
-                DFB_CUDA(cudaEventRecord(ev_gray[sb], h->s_in));
-                DFB_CUDA(cudaEventRecord(ev_frame[f], h->s_in));
+                DFB_CUDA(cudaEventRecord(ev.gray[sb], h->s_in));
+                DFB_CUDA(cudaEventRecord(ev.frame[f], h->s_in));
             }
         };
-        return process_chain(h, n_frames, step, sw, sh, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
+        return process_chain(h, n_frames, step, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
     });
 }
 
@@ -1147,35 +1128,26 @@ int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
-        while ((int)h->pb_events.size() < n_frames + 8) {
-            cudaEvent_t e;
-            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->pb_events.push_back(e);
-        }
         // frame source: the requested frames are decoded as one group, straight into the gray frame array when no resize is
         // asked for, else into scratch and resized frame by frame; only the compressed bytes cross PCIe
         const size_t fpx = (size_t)dw * dh, spx = (size_t)sw * sh;
         auto produce = [&](int first, int last) {
-            cudaEvent_t *ev_frame = h->pb_events.data() + 8;
             const int m = last - first + 1;
             const bool resize = dw != sw || dh != sh;
             if (resize) {
                 DFB_CUDA(cudaStreamSynchronize(h->s_in));  // the previous group's resizes have read the scratch
-                grow_device(h->pb_gray, h->pb_gray_cap, spx * m);
+                h->pb_gray.grow(spx * m);
             }
             uint8_t *dst = resize ? h->pb_gray : h->pb_frames + fpx * first;
             h->jdec->decode(jpeg + first, len + first, hd.data() + first, m, 1, dst, sw, spx, h->s_in);
             h->alg->launches += h->jdec->launches;
             for (int f = first; f <= last; ++f) {
                 h->counters.h2d_bytes += len[f];
-                if (resize) {
-                    const int rc = dfb_resize_gray_device(h, h->pb_gray + spx * (f - first), sw, sw, sh, h->pb_frames + fpx * f, dw, dw, dh, h->s_in);
-                    if (rc != DFB_OK) throw std::runtime_error(h->last_error);
-                }
-                DFB_CUDA(cudaEventRecord(ev_frame[f], h->s_in));
+                if (resize) resize_gray(h, h->pb_gray + spx * (f - first), sw, sw, sh, h->pb_frames + fpx * f, dw, dw, dh, h->s_in);
+                DFB_CUDA(cudaEventRecord(h->chain_ev.frame[f], h->s_in));
             }
         };
-        return process_chain(h, n_frames, step, sw, sh, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
+        return process_chain(h, n_frames, step, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
     });
 }
 
@@ -1266,30 +1238,19 @@ int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pit
         DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         const YccLayout L(dw, dh);
-        grow_device(h->enc_ycc, h->enc_ycc_cap, L.bytes);
+        h->enc_ycc.grow(L.bytes);
         const ResizeTap *taps = ycc_tables(h, src_width, src_height, dw, dh);
+        JpegSink sink(h, 1, 1);
         uint8_t *p = h->enc_ycc;
         launch_bgr_to_ycc420(bgr, bgr_pitch, src_width, src_height, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                             p + L.cr_off, L.c_pitch, s, h->jpeg_exact ? jpeg_chroma_cols(dw) : 0);
+                             p + L.cr_off, L.c_pitch, s, sink.chroma_cols(dw));
         ++h->alg->launches;
-        if (h->jpeg_exact) {
-            jex_encode_to_host(h, 1, ycc_src(p, L), 3, dw, dh, quality, &out, out_capacity, out_len, s, [&](int, size_t need) {
-                return "jpeg output buffer too small: the bitstream needs " + std::to_string(need) + " bytes, capacity is " +
-                       std::to_string(out_capacity);
-            });
-            return DFB_OK;
-        }
-        if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
-        h->jpeg->enqueue_ycc420(0, p, L.y_pitch, p + L.cb_off, p + L.cr_off, L.c_pitch, dw, dh, quality, s);
+        sink.encode(0, 1, ycc_src(p, L), 3, dw, dh, quality, out_capacity, s);
         DFB_CUDA(cudaStreamSynchronize(s));
-        const size_t len = h->jpeg->length(0, s);
-        if (len > out_capacity)
-            throw std::runtime_error("jpeg output buffer too small: the bitstream needs " + std::to_string(len) + " bytes, capacity is " +
-                                     std::to_string(out_capacity));
-        h->jpeg->fetch(0, out, len, s);
-        DFB_CUDA(cudaStreamSynchronize(s));
-        h->counters.d2h_bytes += len;
-        *out_len = len;
+        auto too_small = [&](int, size_t need) {
+            return "jpeg output buffer too small: the bitstream needs " + std::to_string(need) + " bytes, capacity is " + std::to_string(out_capacity);
+        };
+        sink.deliver(0, 1, too_small, single_out(out, out_len), s);
         return DFB_OK;
     });
 }
@@ -1312,99 +1273,59 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
     const int sw = src_width, sh = src_height;
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
-        ensure_streams(h);
-        if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
+        ensure_fetch_stream(h);
         // extract_frames_video's batch (src/denseflow_gpu.cpp:82-144: resize + imencode(".jpg") per frame) on four streams,
         // groups of G frames in flight:
         //   s_in      H2D of frame f into staging buffer f & 1
         //   s_compute resize + YCbCr 4:2:0 of frame f into the planes of its group
-        //   s_out     the group's encodes, one encoder state per frame
-        //   s_fetch   bitstreams of group g-1 to the host while the GPU works on group g
+        //   s_out     the group's encodes, as one batch
+        //   s_fetch   files of group g-1 to the host while the GPU works on group g
         constexpr int G = 8;
         const size_t bgr_bytes = (size_t)sw * sh * 3;
         const YccLayout L(dw, dh);
-        grow_device(h->ex_bgr, h->ex_bgr_cap, 2 * bgr_bytes);
-        grow_device(h->ex_ycc, h->ex_ycc_cap, 2 * G * L.bytes);
+        h->ex_bgr.grow(2 * bgr_bytes);
+        h->ex_ycc.grow(2 * G * L.bytes);
         const ResizeTap *taps = ycc_tables(h, sw, sh, dw, dh);
-        for (auto &e : h->ex_events)
-            if (!e) DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        cudaEvent_t *ev_h2d = h->ex_events;       // [2] staging buffer filled
-        cudaEvent_t *ev_conv = h->ex_events + 2;  // [2] staging buffer consumed
-        cudaEvent_t *ev_planes = h->ex_events + 4;  // [2] group's planes ready
-        cudaEvent_t *ev_enc = h->ex_events + 6;   // [2] group's encodes done
-        const bool exact = h->jpeg_exact;
-        if (exact) {
-            ensure_jex(h, G);
-        } else {
-            if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
-            h->jpeg->ensure_states(2 * G);
-        }
+        auto &ev = h->extract_ev;
+        for (Events *e : {&ev.h2d, &ev.conv, &ev.planes, &ev.enc}) e->ensure(2);
+        JpegSink sink(h, G, 2);
 
         auto convert_group = [&](int g) {
             const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
-            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_enc[slot], 0));  // group g-2's planes have been encoded
+            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // group g-2's planes have been encoded
             for (int i = 0; i < m; ++i) {
                 const int f = f0 + i, sb = f & 1;
                 uint8_t *stage = h->ex_bgr + sb * bgr_bytes;
-                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev_conv[sb], 0));
+                if (f >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev.conv[sb], 0));
                 DFB_CUDA(cudaMemcpyAsync(stage, bgr[f], bgr_bytes, cudaMemcpyHostToDevice, h->s_in));
-                DFB_CUDA(cudaEventRecord(ev_h2d[sb], h->s_in));
+                DFB_CUDA(cudaEventRecord(ev.h2d[sb], h->s_in));
                 h->counters.h2d_bytes += bgr_bytes;
-                DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev_h2d[sb], 0));
+                DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.h2d[sb], 0));
                 uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
                 launch_bgr_to_ycc420(stage, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                                     p + L.cr_off, L.c_pitch, h->s_compute, exact ? jpeg_chroma_cols(dw) : 0);
+                                     p + L.cr_off, L.c_pitch, h->s_compute, sink.chroma_cols(dw));
                 ++h->alg->launches;
-                DFB_CUDA(cudaEventRecord(ev_conv[sb], h->s_compute));
+                DFB_CUDA(cudaEventRecord(ev.conv[sb], h->s_compute));
             }
-            DFB_CUDA(cudaEventRecord(ev_planes[slot], h->s_compute));
-            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev_planes[slot], 0));
-            if (exact) {
-                h->alg->launches += h->jex->encode(m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, slot, h->s_out);
-                DFB_CUDA(cudaMemcpyAsync(h->jex_lens_host + (size_t)slot * h->jex_lens_n, h->jex->lens(slot), sizeof(uint64_t) * m,
-                                         cudaMemcpyDeviceToHost, h->s_out));
-            }
-            for (int i = 0; i < m && !exact; ++i) {
-                const uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
-                h->jpeg->enqueue_ycc420(slot * G + i, p, L.y_pitch, p + L.cb_off, p + L.cr_off, L.c_pitch, dw, dh, quality, h->s_out);
-            }
-            DFB_CUDA(cudaEventRecord(ev_enc[slot], h->s_out));
+            DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
+            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.planes[slot], 0));
+            sink.encode(slot, m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, h->s_out);
+            DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
         };
         auto finish_group = [&](int g) {
-            const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
-            DFB_CUDA(cudaEventSynchronize(ev_enc[slot]));
-            if (exact) {
-                const uint64_t *lens = h->jex_lens_host + (size_t)slot * h->jex_lens_n;
-                const JpegSrc src = ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L);
-                for (int i = 0; i < m; ++i)
-                    if (lens[i] > capacity)
-                        throw std::runtime_error("jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " +
-                                                 std::to_string(h->jex->needed(lens[i], src, i, 3, dw, dh, quality, h->s_fetch)) +
-                                                 " bytes, capacity is " + std::to_string(capacity));
-                for (int i = 0; i < m; ++i) {
-                    len[f0 + i] = (size_t)lens[i];
-                    DFB_CUDA(cudaMemcpyAsync(jpg[f0 + i], h->jex->file(slot, i), len[f0 + i], cudaMemcpyDeviceToHost, h->s_fetch));
-                    h->counters.d2h_bytes += len[f0 + i];
-                }
-            }
-            for (int i = 0; i < m && !exact; ++i) {
-                const int st = slot * G + i, f = f0 + i;
-                const size_t n = h->jpeg->length(st, h->s_fetch);
-                if (n > capacity)
-                    throw std::runtime_error("jpeg output buffer too small: frame " + std::to_string(f) + " needs " + std::to_string(n) +
-                                             " bytes, capacity is " + std::to_string(capacity));
-                len[f] = n;
-                h->jpeg->fetch(st, jpg[f], n, h->s_fetch);
-                h->counters.d2h_bytes += n;
-            }
-            DFB_CUDA(cudaStreamSynchronize(h->s_fetch));
+            const int f0 = g * G, m = std::min(G, n_frames - f0);
+            DFB_CUDA(cudaEventSynchronize(ev.enc[g & 1]));
+            auto too_small = [&](int i, size_t need) {
+                return "jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " + std::to_string(need) + " bytes, capacity is " +
+                       std::to_string(capacity);
+            };
+            auto out = [&](int i, size_t n) {
+                len[f0 + i] = n;
+                return jpg[f0 + i];
+            };
+            sink.deliver(g & 1, m, too_small, out, h->s_fetch);
         };
-        const int NG = (n_frames + G - 1) / G;
-        for (int g = 0; g < NG; ++g) {
-            convert_group(g);
-            if (g > 0) finish_group(g - 1);
-        }
-        finish_group(NG - 1);
+        run_groups((n_frames + G - 1) / G, convert_group, finish_group);
         DFB_CUDA(cudaStreamSynchronize(h->s_in));
         DFB_CUDA(cudaStreamSynchronize(h->s_compute));
         DFB_CUDA(cudaStreamSynchronize(h->s_out));
@@ -1427,17 +1348,12 @@ int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitc
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         if (!h->png) h->png.reset(new PngEncoder());
         h->alg->launches += h->png->encode(1, bgr, 0, bgr_pitch, width, height, 0, s);
-        uint64_t len = 0;
-        DFB_CUDA(cudaMemcpyAsync(&len, h->png->lens(0), sizeof(len), cudaMemcpyDeviceToHost, s));
         DFB_CUDA(cudaStreamSynchronize(s));
-        if (len == 0) throw std::runtime_error("png encoder failed");
-        if (len > out_capacity)
-            throw std::runtime_error("png output buffer too small: the file needs " + std::to_string(len) + " bytes, capacity is " +
-                                     std::to_string(out_capacity));
-        DFB_CUDA(cudaMemcpyAsync(out, h->png->file(0, 0), len, cudaMemcpyDeviceToHost, s));
-        DFB_CUDA(cudaStreamSynchronize(s));
-        h->counters.d2h_bytes += len;
-        *out_len = (size_t)len;
+        auto reject = [&](int, uint64_t len) {
+            if (len == 0) return std::string("png encoder failed");
+            return "png output buffer too small: the file needs " + std::to_string(len) + " bytes, capacity is " + std::to_string(out_capacity);
+        };
+        h->png->files().deliver(0, 1, out_capacity, reject, single_out(out, out_len), h->counters.d2h_bytes, s);
         return DFB_OK;
     });
 }

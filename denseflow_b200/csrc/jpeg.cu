@@ -179,15 +179,4 @@ void JpegEncoder::decode_bgr(const uint8_t *jpeg, size_t len, uint8_t *bgr, size
     check(a.Decode(impl_->handle, impl_->dec_state, jpeg, len, NVJPEG_OUTPUT_BGRI, &out, s), "nvjpegDecode");
 }
 
-size_t JpegEncoder::encode_gray(const uint8_t *gray, size_t pitch, int w, int h, int quality, uint8_t *out, size_t out_cap,
-                                cudaStream_t s) {
-    enqueue(0, gray, pitch, w, h, quality, s);
-    DFB_CUDA(cudaStreamSynchronize(s));
-    const size_t len = length(0, s);
-    if (len > out_cap) throw std::runtime_error("nvjpeg: output buffer too small (" + std::to_string(len) + " > " + std::to_string(out_cap) + ")");
-    fetch(0, out, len, s);
-    DFB_CUDA(cudaStreamSynchronize(s));
-    return len;
-}
-
 }  // namespace dfb

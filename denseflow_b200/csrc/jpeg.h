@@ -11,11 +11,9 @@ class JpegEncoder {
     ~JpegEncoder();
     JpegEncoder(const JpegEncoder &) = delete;
     JpegEncoder &operator=(const JpegEncoder &) = delete;
-    // gray: device pointer; out: host buffer. Returns the JPEG length in bytes. Blocks until the bitstream is on the host.
-    size_t encode_gray(const uint8_t *gray, size_t pitch, int w, int h, int quality, uint8_t *out, size_t out_cap, cudaStream_t s);
-    // The same in three steps over a pool of encoder states, so many planes can be in flight and the host synchronises once per
-    // group instead of twice per plane:
-    //   enqueue(state, ...)   asynchronous: the encode is enqueued on s
+    // Encodes in three steps over a pool of encoder states, so many planes can be in flight and the host synchronises once
+    // per group instead of twice per plane:
+    //   enqueue(state, ...)   asynchronous: a gray device plane's encode is enqueued on s
     //   length(state, s)      after s has been synchronised past the enqueue (event or stream sync): size of the bitstream
     //   fetch(state, out, s)  enqueues the copy of the bitstream into the host buffer on s (any stream; complete after a sync of s)
     void ensure_states(int n);

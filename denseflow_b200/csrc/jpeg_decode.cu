@@ -765,12 +765,7 @@ struct JpegDecoder::Layout {
         o_first_dc, o_status, o_flag, o_coef, o_planes, total;
 };
 
-JpegDecoder::~JpegDecoder() {
-    if (d_ws) cudaFree(d_ws);
-    if (h_stage) cudaFreeHost(h_stage);
-    if (h_flag) cudaFreeHost(h_flag);
-    delete L;
-}
+JpegDecoder::~JpegDecoder() { delete L; }
 
 static size_t a256(size_t x) { return (x + 255) & ~size_t(255); }
 
@@ -864,26 +859,11 @@ void JpegDecoder::run_entropy(const uint8_t *const *jpeg, const size_t *len, con
     Y.total = o;
 
     // staging: descriptors, tables, segment geometry and the entropy-coded bytes, in the workspace's layout
-    if (Y.upload > stage_cap) {
-        DFB_CUDA(cudaStreamSynchronize(s));
-        if (h_stage) DFB_CUDA(cudaFreeHost(h_stage));
-        h_stage = nullptr;
-        DFB_CUDA(cudaHostAlloc(&h_stage, Y.upload, cudaHostAllocDefault));
-        stage_cap = Y.upload;
-    }
-    if (Y.total > ws_cap) {
-        DFB_CUDA(cudaStreamSynchronize(s));
-        if (d_ws) DFB_CUDA(cudaFree(d_ws));
-        d_ws = nullptr;
-        DFB_CUDA(cudaMalloc(&d_ws, Y.total));
-        ws_cap = Y.total;
-    }
-    if ((size_t)n + 1 > flag_cap) {
-        if (h_flag) DFB_CUDA(cudaFreeHost(h_flag));
-        h_flag = nullptr;
-        flag_cap = std::max<size_t>(n + 1, 1024);
-        DFB_CUDA(cudaHostAlloc(&h_flag, sizeof(int) * flag_cap, cudaHostAllocDefault));
-    }
+    // the previous call's copies and kernels on s are the only users of the old buffers (the flag words were read after a sync)
+    if (Y.upload > h_stage.bytes() || Y.total > d_ws.bytes()) DFB_CUDA(cudaStreamSynchronize(s));
+    h_stage.allocate(Y.upload);
+    d_ws.allocate(Y.total);
+    h_flag.allocate(sizeof(int) * std::max<size_t>(n + 1, 1024));
     uint8_t *S = h_stage;
     std::memcpy(S + Y.o_frames, fr.data(), sizeof(JFrame) * n);
     HuffTab *tabs = reinterpret_cast<HuffTab *>(S + Y.o_tabs);

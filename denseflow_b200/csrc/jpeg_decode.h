@@ -57,13 +57,10 @@ class JpegDecoder {
     void run_entropy(const uint8_t *const *jpeg, const size_t *len, const JpegHeader *hd, int n, cudaStream_t s);
     void check_status(int n, cudaStream_t s);
 
-    // device workspace (grown on demand)
-    uint8_t *d_ws = nullptr;
-    size_t ws_cap = 0;
-    uint8_t *h_stage = nullptr;  // pinned staging of the descriptors and file bytes
-    size_t stage_cap = 0;
-    int *h_flag = nullptr;  // pinned: the change flag of the sync rounds, then the frame status words
-    size_t flag_cap = 0;
+    // grown on demand
+    DeviceBuffer<uint8_t> d_ws;    // device workspace
+    PinnedBuffer<uint8_t> h_stage;  // staging of the descriptors and file bytes
+    PinnedBuffer<int> h_flag;      // the change flag of the sync rounds, then the frame status words
     // layout of the current call inside d_ws
     struct Layout;
     Layout *L = nullptr;

@@ -580,24 +580,7 @@ __global__ void __launch_bounds__(kTileThreads) k_scatter(uint8_t *ws, Geo G, He
     }
 }
 
-template <typename T> void grow(T *&p, size_t &cap, size_t need) {
-    if (need <= cap) return;
-    DFB_CUDA(cudaDeviceSynchronize());  // work still using the old buffer
-    if (p) DFB_CUDA(cudaFree(p));
-    p = nullptr;
-    DFB_CUDA(cudaMalloc(reinterpret_cast<void **>(&p), need));
-    cap = need;
-}
-
 }  // namespace
-
-JpegExactEncoder::~JpegExactEncoder() {
-    if (ws_) cudaFree(ws_);
-    for (int s = 0; s < 2; ++s) {
-        if (files_[s]) cudaFree(files_[s]);
-        if (lens_[s]) cudaFree(lens_[s]);
-    }
-}
 
 int JpegExactEncoder::encode(int n, const JpegSrc &src, int components, int w, int h, int quality, size_t capacity, int slot,
                              cudaStream_t s) {
@@ -607,22 +590,17 @@ int JpegExactEncoder::encode(int n, const JpegSrc &src, int components, int w, i
     if (quality < 1 || quality > 100) throw std::runtime_error("jpeg: quality must be in 1..100");
     if (capacity == 0) throw std::runtime_error("jpeg: zero capacity");
     const Geo G(components, w, h, capacity);
-    file_cap_ = capacity;
-    grow(files_[slot], files_cap_[slot], (size_t)n * file_cap_);
-    if (lens_n_[slot] < n) {
-        size_t cap = (size_t)lens_n_[slot] * 8;
-        grow(lens_[slot], cap, (size_t)n * 8);
-        lens_n_[slot] = n;
-    }
+    files_.prepare(slot, n, capacity);
     const int E = (int)std::max<size_t>(1, std::min<size_t>((size_t)n, kWorkspaceBudget / G.bytes));
-    grow(ws_, ws_cap_, (size_t)E * G.bytes);
+    ws_.grow((size_t)E * G.bytes);
     int launches = 0;
     for (int i0 = 0; i0 < n; i0 += E) {
         JpegSrc part = src;
         part.base = src.base + (size_t)i0 * src.img_stride;
-        launches += encode_part(std::min(E, n - i0), part, components, w, h, quality, capacity, files_[slot] + (size_t)i0 * file_cap_,
-                                lens_[slot] + i0, s);
+        launches += encode_part(std::min(E, n - i0), part, components, w, h, quality, capacity, files_.file(slot, i0),
+                                files_.lens(slot) + i0, s);
     }
+    files_.read_lens(slot, n, s);
     return launches;
 }
 
@@ -659,10 +637,8 @@ size_t JpegExactEncoder::needed(uint64_t reported, const JpegSrc &src, int i, in
     one.base = src.base + (size_t)i * src.img_stride;
     if (!probe_) probe_.reset(new JpegExactEncoder());
     probe_->encode(1, one, components, w, h, quality, 2 * (size_t)(reported & ~kJpegLenLowerBound), 0, s);
-    uint64_t len = 0;
-    DFB_CUDA(cudaMemcpyAsync(&len, probe_->lens(0), sizeof(len), cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
-    return (size_t)len;
+    return (size_t)probe_->files().host_len(0, 0);
 }
 
 }  // namespace dfb

@@ -3,11 +3,9 @@
 // YCbCr 4:2:0.  See jpeg_encode.cu.
 #pragma once
 
-#include <cuda_runtime.h>
-#include <stddef.h>
-#include <stdint.h>
-
 #include <memory>
+
+#include "file_slots.h"
 
 namespace dfb {
 
@@ -27,22 +25,19 @@ inline int jpeg_chroma_cols(int w) { return ((w + 1) / 2 + 7) / 8 * 8; }
 // Bit 63 of a length: the file did not fit and the value is a lower bound (entropy data before byte stuffing).
 constexpr uint64_t kJpegLenLowerBound = uint64_t(1) << 63;
 
-// Workspace and output files, grown on demand.  Files live in two slots so the read-back of one group can overlap the
-// encode of the next.  Never touches nvJPEG.
+// Workspace and output files, grown on demand.  Never touches nvJPEG.
 class JpegExactEncoder {
   public:
     JpegExactEncoder() = default;
     JpegExactEncoder(const JpegExactEncoder &) = delete;
     JpegExactEncoder &operator=(const JpegExactEncoder &) = delete;
-    ~JpegExactEncoder();
-    // Encodes n w x h images (components 1 or 3) enqueued on s.  File i goes to file(slot, i) (at most capacity bytes),
-    // its length to lens(slot)[i] (device memory): the file length, or when it exceeds capacity the length it needs
-    // (nothing past capacity is written), or that needed length's lower bound | kJpegLenLowerBound.  Returns the number
-    // of kernels launched.
+    // Encodes n w x h images (components 1 or 3) enqueued on s.  File i goes to files().file(slot, i) (at most capacity
+    // bytes); its length follows it to the host (read_lens) on s: the file length, or when it exceeds capacity the length it
+    // needs (nothing past capacity is written), or that needed length's lower bound | kJpegLenLowerBound.  Returns the
+    // number of kernels launched.
     int encode(int n, const JpegSrc &src, int components, int w, int h, int quality, size_t capacity, int slot, cudaStream_t s);
-    const uint8_t *file(int slot, int i) const { return files_[slot] + (size_t)i * file_cap_; }
-    uint64_t *lens(int slot) const { return lens_[slot]; }
-    // The exact length image i of src needs, given a length lens() reported over capacity; synchronises s.  A lower bound is
+    const FileSlots &files() const { return files_; }
+    // The exact length image i of src needs, given a length reported over capacity; synchronises s.  A lower bound is
     // resolved by encoding the image alone in a workspace and files of its own, so encodes of this encoder still in flight
     // on other streams (the next group of a pipeline) are neither read nor overwritten.
     size_t needed(uint64_t reported, const JpegSrc &src, int i, int components, int w, int h, int quality, cudaStream_t s);
@@ -50,13 +45,8 @@ class JpegExactEncoder {
   private:
     int encode_part(int n, const JpegSrc &src, int components, int w, int h, int quality, size_t capacity, uint8_t *files,
                     uint64_t *lens, cudaStream_t s);
-    uint8_t *ws_ = nullptr;
-    size_t ws_cap_ = 0;
-    uint8_t *files_[2] = {};
-    size_t files_cap_[2] = {};
-    uint64_t *lens_[2] = {};
-    int lens_n_[2] = {};
-    size_t file_cap_ = 0;
+    DeviceBuffer<uint8_t> ws_;
+    FileSlots files_;
     std::unique_ptr<JpegExactEncoder> probe_;  // needed()'s own encoder, created on first use
 };
 

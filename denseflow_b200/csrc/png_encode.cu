@@ -492,42 +492,18 @@ size_t png_max_bytes(int w, int h) {
     return Layout(w, h).file_cap;
 }
 
-PngEncoder::~PngEncoder() {
-    if (ws_) cudaFree(ws_);
-    for (int s = 0; s < 2; ++s) {
-        if (files_[s]) cudaFree(files_[s]);
-        if (lens_[s]) cudaFree(lens_[s]);
-    }
-}
-
-namespace {
-template <typename T> void grow(T *&p, size_t &cap, size_t need) {
-    if (need <= cap) return;
-    DFB_CUDA(cudaDeviceSynchronize());  // work still using the old buffer
-    if (p) DFB_CUDA(cudaFree(p));
-    p = nullptr;
-    DFB_CUDA(cudaMalloc(reinterpret_cast<void **>(&p), need));
-    cap = need;
-}
-}  // namespace
-
 int PngEncoder::encode(int n, const uint8_t *src, size_t img_stride, size_t bgr_pitch, int w, int h, int slot, cudaStream_t s) {
     if (n <= 0) return 0;
     if ((size_t)h * (1 + 3 * (size_t)w) >= (size_t(1) << 31)) throw std::runtime_error("png: image too large");
     const Layout L(w, h);
-    file_cap_ = L.file_cap;
-    grow(files_[slot], files_cap_[slot], (size_t)n * file_cap_);
-    if (lens_n_[slot] < n) {
-        size_t cap = (size_t)lens_n_[slot] * 8;
-        grow(lens_[slot], cap, (size_t)n * 8);
-        lens_n_[slot] = n;
-    }
+    files_.prepare(slot, n, L.file_cap);
     const int E = (int)std::max<size_t>(1, std::min<size_t>((size_t)n, kWorkspaceBudget / L.bytes));
-    grow(ws_, ws_cap_, (size_t)E * L.bytes);
+    ws_.grow((size_t)E * L.bytes);
     int launches = 0;
     for (int i0 = 0; i0 < n; i0 += E)
-        launches += encode_part(std::min(E, n - i0), src + (size_t)i0 * img_stride, img_stride, bgr_pitch, w, h,
-                                files_[slot] + (size_t)i0 * file_cap_, lens_[slot] + i0, s);
+        launches += encode_part(std::min(E, n - i0), src + (size_t)i0 * img_stride, img_stride, bgr_pitch, w, h, files_.file(slot, i0),
+                                files_.lens(slot) + i0, s);
+    files_.read_lens(slot, n, s);
     return launches;
 }
 
