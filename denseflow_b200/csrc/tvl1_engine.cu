@@ -201,6 +201,7 @@ class Tvl1 final : public FlowAlgorithm {
     // pairs per fused launch.  Utilisation model: a lane of G = SMs / B CTAs visits tiles(level) tiles
     // in ceil(tiles / G) rounds; weight the levels by where the iterations are (the coarsest scale runs
     // most of them), pick the B with the fewest idle CTA-rounds.
+    static constexpr double kResidentChunkCost = 0.85;  // time of a resident chunk relative to a streamed one (DESIGN §4.4)
     int max_concurrent_pairs(int w, int h) override {
         if (!prm_.fused) return 1;
         if (prm_.lanes > 0) return prm_.lanes;
@@ -223,7 +224,9 @@ class Tvl1 final : public FlowAlgorithm {
                 const int tiles = fused_tiles_along(lv[l].w, kFusedTileW, hx) * fused_tiles_along(lv[l].h, kFusedTileH, hy);
                 const int rounds = (tiles + G - 1) / G;
                 num += wgt * tiles;
-                den += wgt * (double)rounds * G;
+                // a level with a CTA per tile keeps its tiles on chip across chunks (tvl1_fused.cu, level_resident): its chunks
+                // skip most of the tile load and store
+                den += wgt * (double)rounds * G * (tiles <= G ? kResidentChunkCost : 1.0);
             }
             util[B] = num / den * (double)(G * B) / sms;
             best_u = std::max(best_u, util[B]);

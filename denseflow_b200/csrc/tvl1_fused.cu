@@ -471,9 +471,15 @@ __device__ __forceinline__ void tma_warp_u(Smem &sm, const char *maps, int cur, 
 // * p_bot: the warp below reads it in its first primal row, and this warp's last dual step of a visit waited for that read.
 // The warp signals `base` once its rows of the new tile are loaded; a neighbour reads them only after waiting for that
 // signal (tests/test_sync_protocol_handover_cpu.py checks both directions over every interleaving).
+//
+// Resident tiles (run_chunk): when a level has no more tiles than the lane has CTAs, CTA bid keeps tile bid on chip for all
+// chunks of a warp's epoch loop, and the dual planes stay in the caller's registers.  ring_only: only the ring (tile pixels
+// outside the interior, which neighbouring tiles computed) is read back; the interior and the constants are still in shared
+// memory and registers.  band_only: only the band (interior pixels that lie in some other tile's ring) is written.
 __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Consts &c, const FusedLevel &L, int level, int cur, int tx, int ty,
-                                              int kk, int hx, int hy, bool check, int base, unsigned tma_parity, Smem &sm,
-                                              bool prof_on, bool first_in_chunk, int ntx_next, int nty_next) {
+                                              int ntx, int nty, int kk, int hx, int hy, bool check, int base, unsigned tma_parity, Smem &sm,
+                                              bool prof_on, bool first_in_chunk, int ntx_next, int nty_next, bool ring_only, bool band_only,
+                                              float4 (&p11)[RPT], float4 (&p12)[RPT], float4 (&p21)[RPT], float4 (&p22)[RPT]) {
     const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
     unsigned long long t0 = 0;
     if (prof_on) t0 = gtime();
@@ -486,9 +492,24 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     const char *maps = level_maps(job, level);
     const int nrx0 = ntx_next * (TW - 2 * hx), nry0 = nty_next * (TH - 2 * hy);
 
-    float4 p11[RPT], p12[RPT], p21[RPT], p22[RPT];
+    // which of this thread's pixels are interior (written back / counted in the error)
+    const bool lane_in = (tx == 0 || 4 * lane >= hx) && 4 * lane < TW - hx + (rx0 + TW >= W ? hx : 0) && gx0 < W;
+    const int ry_lo = ty == 0 ? 0 : hy;
+    const int ry_hi = TH - hy + (ry0 + TH >= H ? hy : 0);
+    // band: within 2h of a tile edge that has a neighbouring tile, whose ring (its first / last h columns or rows) covers it
+    const bool lane_band = (tx > 0 && 4 * lane < 2 * hx) || (tx < ntx - 1 && 4 * lane >= TW - 2 * hx);
+    unsigned in_rows = 0, store_rows = 0;  // bit r: row r of this thread is interior / is written back
+#pragma unroll
+    for (int r = 0; r < RPT; ++r) {
+        const int ry = RPT * wq + r;
+        const bool in = lane_in && ry >= ry_lo && ry < ry_hi && gy0 + r < H;
+        const bool band = lane_band || (ty > 0 && ry < 2 * hy) || (ty < nty - 1 && ry >= TH - 2 * hy);
+        in_rows |= (unsigned)in << r;
+        store_rows |= (unsigned)(in && (band || !band_only)) << r;
+    }
+
     const int so0 = (RPT * wq) * TW + 4 * lane;  // this thread's slot in row 0 of its warp (thread-private in smem planes)
-    const bool use_tma = job.use_tma != 0;
+    const bool use_tma = job.use_tma != 0 && !ring_only;
     // The warp above reads this warp's first u row in its dual steps: it must have finished the previous tile (its counter
     // reached base - 2 = "last dual step of the previous tile done") before the row is overwritten.  (Without flags the
     // previous visit ended with a CTA-wide barrier.)
@@ -510,6 +531,7 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
 #pragma unroll
         for (int r = 0; r < RPT; ++r) {
             const int gy = gy0 + r;
+            if (ring_only && (in_rows >> r & 1u)) continue;  // interior: still on chip
             const bool ok = col_ok && gy < H;
             const size_t o = ok ? (size_t)gy * P + gx0 : 0;
             p11[r] = ok ? ld_cg4_hint(s2 + o, lpol) : zero4();
@@ -520,10 +542,12 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
                 const int so = so0 + r * TW;
                 st4(&sm.u[0][so], ok ? ld_cg4(s0 + o) : zero4());
                 st4(&sm.u[1][so], ok ? ld_cg4(s1 + o) : zero4());
-                st4(&sm.consts[0][so], ok ? ld_cg4(job.I1wx + o) : zero4());
-                st4(&sm.consts[1][so], ok ? ld_cg4(job.I1wy + o) : zero4());
-                st4(&sm.consts[2][so], ok ? ld_cg4(job.grad + o) : zero4());
-                st4(&sm.consts[3][so], ok ? ld_cg4(job.rho_c + o) : zero4());
+                if (!ring_only) {
+                    st4(&sm.consts[0][so], ok ? ld_cg4(job.I1wx + o) : zero4());
+                    st4(&sm.consts[1][so], ok ? ld_cg4(job.I1wy + o) : zero4());
+                    st4(&sm.consts[2][so], ok ? ld_cg4(job.grad + o) : zero4());
+                    st4(&sm.consts[3][so], ok ? ld_cg4(job.rho_c + o) : zero4());
+                }
             }
         }
     }
@@ -569,10 +593,9 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     t.left_col = tx == 0 && lane == 0;
     t.jlast = W - 1 - gx0;
     t.rbot = H - 1 - gy0;
-    // which of this thread's pixels are interior (written back / counted in the error)
-    t.lane_in = (tx == 0 || 4 * lane >= hx) && 4 * lane < TW - hx + (rx0 + TW >= W ? hx : 0) && gx0 < W;
-    t.ry_lo = ty == 0 ? 0 : hy;
-    t.ry_hi = TH - hy + (ry0 + TH >= H ? hy : 0);
+    t.lane_in = lane_in;
+    t.ry_lo = ry_lo;
+    t.ry_hi = ry_hi;
     t.rows_left = H - gy0;
     t.cols_left = W - gx0;
     t.halo_top = t.ry_lo > 0;
@@ -604,16 +627,15 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
             if (n.y >= 0) tma_warp_consts(sm, level_maps(job, n.z), n.x, n.y, wq);
         }
     }
-    // -------- write the interior to the other buffer ---------------------------------------------
+    // -------- write the interior (or its band) to the other buffer ------------------------------------
     {
         float *d0 = L.u1[cur ^ 1], *d1 = L.u2[cur ^ 1], *d2 = job.p[cur ^ 1][0], *d3 = job.p[cur ^ 1][1],
               *d4 = job.p[cur ^ 1][2], *d5 = job.p[cur ^ 1][3];
-#pragma unroll
         const unsigned long long pol = l2_evict_first_policy();
+#pragma unroll
         for (int r = 0; r < RPT; ++r) {
-            const int ry = RPT * wq + r, gy = gy0 + r;
-            if (t.lane_in && ry >= t.ry_lo && ry < t.ry_hi && gy < H) {
-                const size_t o = (size_t)gy * P + gx0;
+            if (store_rows >> r & 1u) {
+                const size_t o = (size_t)(gy0 + r) * P + gx0;
                 st4_evict_first(d0 + o, *reinterpret_cast<const float4 *>(&sm.u[0][so0 + r * TW]), pol);
                 st4_evict_first(d1 + o, *reinterpret_cast<const float4 *>(&sm.u[1][so0 + r * TW]), pol);
                 st4_evict_first(d2 + o, p11[r], pol);
@@ -641,21 +663,36 @@ __device__ __forceinline__ void cta_setup(Smem &sm) {
     __syncthreads();
 }
 
+// Whether the tiles of level L stay resident across the chunks of a warp's epoch loop: the level is cut at the halo hk of the
+// longest chunk (a halo wider than a chunk's kk keeps every kept pixel valid), and every tile needs a CTA of its own.
+__device__ __forceinline__ bool level_resident(const FusedLevel &L, int hk, int G) {
+    return tiles_along(L.w, TW, (hk + 3) & ~3) * tiles_along(L.h, TH, hk) <= G;
+}
+
+// How a chunk moves tile state.  Streamed: every tile is loaded and its whole interior written back.  Resident (level_resident):
+// CTA bid owns tile bid; the first chunk of a warp's epoch loop loads it whole, later ones only its ring, and a chunk writes
+// only the band unless it ends an epoch, whose state the convergence check, the warp phase and the upsample read whole.
+enum ChunkMode { kStreamed, kResidentFirst, kResidentNext, kResidentFlush };
+
 // One chunk: kk iterations on every tile of level L, tiles t = bid, bid + G, ... one after another, reading state [cur] and
 // writing [cur ^ 1].  chk: this CTA's share of sum(diff) of the chunk's last primal step goes to its convergence partial in
-// set part_sel.  The caller ends the chunk with a grid barrier.
-__device__ __forceinline__ void run_chunk(const FusedJob &job, const Tvl1Consts &c, const FusedLevel &L, int s, int cur, int kk, bool chk, int G,
-                                          int bid, int part_sel, Smem &sm, bool prof_on, int &tile_base, unsigned &tma_parity) {
-    const int hx = (kk + 3) & ~3, hy = kk;
+// set part_sel.  The caller ends the chunk with a grid barrier.  p11..p22 carry a resident tile's dual planes from chunk to chunk.
+__device__ __forceinline__ void run_chunk(const FusedJob &job, const Tvl1Consts &c, const FusedLevel &L, int s, int cur, int kk, int hk, bool chk,
+                                          int G, int bid, int part_sel, Smem &sm, bool prof_on, int &tile_base, unsigned &tma_parity,
+                                          ChunkMode mode, float4 (&p11)[RPT], float4 (&p12)[RPT], float4 (&p21)[RPT], float4 (&p22)[RPT]) {
+    const bool resident = mode != kStreamed;
+    const int hy = resident ? hk : kk, hx = (hy + 3) & ~3;
     const int ntx = tiles_along(L.w, TW, hx), nty = tiles_along(L.h, TH, hy);
     const int ntiles = ntx * nty;
     for (int t = bid; t < ntiles; t += G) {
         const int ty = t / ntx, tx = t - ty * ntx;
-        const int tn = t + G;
+        const int tn = resident ? ntiles : t + G;  // resident: no hand-over and no L2 prefetch (one tile per CTA)
         const int nty_n = tn < ntiles ? tn / ntx : -1, ntx_n = tn < ntiles ? tn - nty_n * ntx : -1;
-        const float e = process_tile(job, c, L, s, cur, tx, ty, kk, hx, hy, chk, tile_base, tma_parity, sm, prof_on, t == bid, ntx_n, nty_n);
+        const bool ring_only = mode == kResidentNext || mode == kResidentFlush;
+        const float e = process_tile(job, c, L, s, cur, tx, ty, ntx, nty, kk, hx, hy, chk, tile_base, tma_parity, sm, prof_on, t == bid, ntx_n,
+                                     nty_n, ring_only, mode == kResidentNext, p11, p12, p21, p22);
         tile_base += 2 * kk + 2;
-        tma_parity ^= 1u;
+        if (job.use_tma && !ring_only) tma_parity ^= 1u;
         if (chk) {  // per-warp running sums in shared memory: no CTA-wide barrier per tile
             double v = (double)e;
 #pragma unroll
@@ -777,6 +814,12 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const _
             prof.mark(3);
             double error = DBL_MAX, prev_error = 0.0;
             int n = 0;
+            // a resident tile's dual planes, kept across the warp's chunks.  Defined here although the first chunk loads them:
+            // otherwise ptxas keeps the previous warp's values alive through phase_warp, which then spills.
+            float4 p11[RPT], p12[RPT], p21[RPT], p22[RPT];
+#pragma unroll
+            for (int r = 0; r < RPT; ++r) p11[r] = p12[r] = p21[r] = p22[r] = zero4();
+            bool first = true;
             while (error > scaled_eps && n < job.iterations) {
                 // plan the epoch: iterations up to and including the next convergence check (A.4)
                 int K = 0, nn = n;
@@ -798,7 +841,9 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const _
                     const int nch = (remaining + job.k - 1) / job.k;
                     const int kk = (remaining + nch - 1) / nch;
                     const bool chk = check && kk == remaining;
-                    run_chunk(job, c, L, s, cur, kk, chk, G, bid, part_sel, sm, prof.on, tile_base, tma_parity);
+                    const ChunkMode mode = !level_resident(L, job.k, G) ? kStreamed : first ? kResidentFirst : kk == remaining ? kResidentFlush : kResidentNext;
+                    run_chunk(job, c, L, s, cur, kk, job.k, chk, G, bid, part_sel, sm, prof.on, tile_base, tma_parity, mode, p11, p12, p21, p22);
+                    first = false;
                     prof.mark(2, 8 + s);
                     if (prof.on) prof.acc[16 + s] += 1;
                     px_chunks += (unsigned long long)(L.w * L.h);
@@ -858,8 +903,14 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_stage(const 
     } else if (a.stage == kFusedStageChunks) {
         unsigned epoch = 0, tma_parity = 0;
         int tile_base = 1, part_sel = 0, cur = 0;
+        const int hk = max(job.k, a.kk);
+        const bool resident = level_resident(L, hk, G);
+        float4 p11[RPT], p12[RPT], p21[RPT], p22[RPT];
         for (int i = 0; i < a.n; ++i) {
-            run_chunk(job, job.c, L, a.level, cur, a.kk, a.check != 0, G, bid, part_sel, sm, false, tile_base, tma_parity);
+            // every checking chunk and the last one end an epoch
+            const ChunkMode mode = !resident ? kStreamed : i == 0 ? kResidentFirst : a.check || i == a.n - 1 ? kResidentFlush : kResidentNext;
+            run_chunk(job, job.c, L, a.level, cur, a.kk, hk, a.check != 0, G, bid, part_sel, sm, false, tile_base, tma_parity, mode, p11, p12, p21,
+                      p22);
             grid_barrier(job.sync, epoch, G, job.ctl);
             cur ^= 1;
             if (a.check) {
