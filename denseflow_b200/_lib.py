@@ -52,6 +52,19 @@ class ListStats(C.Structure):
                 ("kernel_launches", C.c_uint64), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64)]
 
 
+VIDEO_BGR = 0
+VIDEO_JPEG = 1
+SAVE_JPG = 0
+SAVE_PNG = 1
+
+
+class Video(C.Structure):
+    _fields_ = [("kind", C.c_int), ("n_frames", C.c_int), ("bgr", C.POINTER(C.c_void_p)), ("width", C.c_int), ("height", C.c_int),
+                ("jpeg", C.POINTER(C.c_void_p)), ("jpeg_len", C.POINTER(C.c_size_t))]
+
+
+FILES_DONE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t))
+
 CHUNK_DONE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                             C.POINTER(C.c_void_p))
 
@@ -102,6 +115,14 @@ SIGNATURES = {
                                             C.POINTER(C.c_size_t), C.c_void_p]),
     "dfb_calc_batch_host_png": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
                                           C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_process_bgr_batch_host_png": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                 C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_process_jpeg_batch_host_png": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int,
+                                                  C.c_int, C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_extract_frames_jpeg_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
+                                               C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_new_size": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "dfb_jpeg_info": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "dfb_decode_jpeg_batch_device": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_void_p,
                                                C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                                C.c_void_p]),
@@ -126,6 +147,8 @@ SIGNATURES = {
     "dfb_list_run": (C.c_int, [C.c_void_p, C.POINTER(Clip), C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
     "dfb_list_close": (None, [C.c_void_p]),
+    "dfb_list_run_videos": (C.c_int, [C.c_void_p, C.POINTER(Video), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
     "dfb_run_list": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.c_int, C.POINTER(Clip), C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
 }

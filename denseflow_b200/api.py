@@ -400,6 +400,60 @@ class DenseOpticalFlow:
                                                       C.c_void_p(s)))
         return buf[:n.value].tobytes()
 
+    @staticmethod
+    def _bgr_frames(frames_bgr, name):
+        frames = [np.asarray(f) for f in frames_bgr]
+        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != frames[0].shape for f in frames):
+            raise RuntimeError("%s: frames must be uint8 [H,W,3] images of one size" % name)
+        return [np.ascontiguousarray(f) for f in frames]
+
+    def _png_buffers(self, m, w, h):
+        cap = self._L.dfb_png_max_bytes(w, h)
+        bufs = [np.empty(max(cap, 1), np.uint8) for _ in range(m)]
+        return bufs, (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bufs]), (C.c_size_t * max(m, 1))(), cap
+
+    def process_bgr_batch_png(self, frames_bgr, step=1, new_size=None):
+        """-st=png for decoded BGR frames: gray -> resize -> flow -> convertFlowToPngImage -> imencode(".png") on the GPU.
+        frames_bgr: list of uint8 [H,W,3]; new_size: (w, h) or None.  Returns one PNG file (bytes) per pair, byte for byte
+        calc_batch_png of the gray, resized frames."""
+        frames = self._bgr_frames(frames_bgr, "process_bgr_batch_png")
+        n = len(frames)
+        if n == 0:
+            return []
+        sh, sw = frames[0].shape[:2]
+        dw, dh = new_size if new_size else (0, 0)
+        m = max(n - abs(step), 0)
+        bufs, op, lens, cap = self._png_buffers(m, *(new_size if new_size else (sw, sh)))
+        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
+        self._check(self._L.dfb_process_bgr_batch_host_png(self._h, fp, n, step, sw, sh, dw, dh, op, cap, lens))
+        return [bufs[i][:lens[i]].tobytes() for i in range(m)]
+
+    def process_jpeg_batch_png(self, jpegs, step=1, new_size=None):
+        """-if -st=png: process_bgr_batch_png with the frames given as JPEG files of one size, decoded on the GPU to imdecode's
+        pixels.  Returns one PNG file (bytes) per pair."""
+        keep, ptrs, lens = self._jpeg_buffers(jpegs)
+        n = len(keep)
+        dw, dh = new_size if new_size else (0, 0)
+        m = max(n - abs(step), 0)
+        bufs, op, plens, cap = self._png_buffers(m, *(new_size if new_size else (self.max_width, self.max_height)))
+        self._check(self._L.dfb_process_jpeg_batch_host_png(self._h, ptrs, lens, n, step, dw, dh, op, cap, plens))
+        return [bufs[i][:plens[i]].tobytes() for i in range(m)]
+
+    def extract_frames_jpeg(self, jpegs, new_size=None, quality=95):
+        """-if -s=0: extract_frames with the frames given as JPEG files of one size, decoded on the GPU to imdecode's pixels.
+        Returns one JPEG bitstream per frame, in order (img_%05d.jpg)."""
+        keep, ptrs, lens = self._jpeg_buffers(jpegs)
+        n = len(keep)
+        if n == 0:
+            return []
+        dw, dh = new_size if new_size else (0, 0)
+        cap = self._L.dfb_jpeg_max_bytes_bgr(*(new_size if new_size else (self.max_width, self.max_height)))
+        bufs = [np.empty(cap, np.uint8) for _ in range(n)]
+        op = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
+        olens = (C.c_size_t * n)()
+        self._check(self._L.dfb_extract_frames_jpeg_host(self._h, ptrs, lens, n, dw, dh, int(quality), op, cap, olens))
+        return [bufs[i][:olens[i]].tobytes() for i in range(n)]
+
     def calc_batch_png(self, frames, step=1, out=None):
         """frames: sequence of uint8 [H,W] host arrays (or one [N,H,W] array).  Returns, for each of the M = max(N-|step|,0)
         pairs, the PNG file writeFlowImagesPng writes: imencode(".png", convertFlowToPngImage(flow)).  out: optional list of
@@ -473,6 +527,27 @@ class DenseOpticalFlow:
 
     def reset_counters(self):
         self._check(self._L.dfb_reset_counters(self._h))
+
+
+def new_size(width, height, new_width=0, new_height=0, new_short=0, variant="default"):
+    """DenseFlow::get_new_size (src/denseflow_gpu.cpp:44-80) with the -nw / -nh / -ns options: the (w, h) a width x height
+    video is resized to, or its own size when no resize applies.  Raises RuntimeError with check_param's texts."""
+    L = _lib.load(variant)
+    dw, dh = C.c_int(), C.c_int()
+    if L.dfb_new_size(int(width), int(height), int(new_width), int(new_height), int(new_short), C.byref(dw), C.byref(dh)) != _lib.DFB_OK:
+        raise RuntimeError(L.dfb_last_error(None).decode())
+    return dw.value, dh.value
+
+
+def jpeg_info(jpeg, variant="default"):
+    """(width, height) of a JPEG file from its markers; raises RuntimeError for files the GPU decoder refuses."""
+    L = _lib.load(variant)
+    buf = np.frombuffer(jpeg, np.uint8)
+    w, h = C.c_int(), C.c_int()
+    rc = L.dfb_jpeg_info(buf.ctypes.data if buf.size else None, buf.size, C.byref(w), C.byref(h))
+    if rc != _lib.DFB_OK:
+        raise RuntimeError(L.dfb_last_error(None).decode())
+    return w.value, h.value
 
 
 class OpticalFlowDual_TVL1(DenseOpticalFlow):

@@ -2,10 +2,12 @@
 // Replaces the statements of the per-pair loop of DenseFlow::calc_optflows_imp
 // (/root/reference/src/denseflow_gpu.cpp:313-342): upload x2 (:317-318), calc (:327/:329),
 // download (:339) — plus the batch shape of the whole function (:307-342).
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -75,6 +77,7 @@ struct dfb_handle {
     std::unique_ptr<JpegEncoder> jpeg;  // nvJPEG encoder / decoder states, created on first use
     // scratch of the flow chains (dfb_process_*_batch_host), grown on demand
     DeviceBuffer<uint8_t> pb_bgr, pb_gray, pb_frames, pb_q;
+    DeviceBuffer<float> pb_flow;  // flow fields of two groups of the -st=png chains
     struct {
         Events frame;      // [n_frames] frame f is in pb_frames
         Events gray;       // [2] BGR staging buffer consumed
@@ -84,7 +87,7 @@ struct dfb_handle {
     std::unique_ptr<JpegDecoder> jdec;  // imdecode-exact JPEG decoder, created on first use
     DeviceBuffer<uint8_t> png_scratch;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
     std::unique_ptr<PngEncoder> png;    // imencode(".png") workspace and files, created on first use
-    DeviceBuffer<uint8_t> png_bgr;      // packed images of dfb_calc_batch_host_png, one per flow ring slot
+    DeviceBuffer<uint8_t> png_bgr;      // packed images of dfb_calc_batch_host_png (one per flow ring slot) and of the png chains
     TapTable gray_taps;  // dfb_resize_gray_device
     // scratch of the frame-extraction calls (-s=0), grown on demand
     TapTable ycc_taps;                // colour resize of all three calls
@@ -931,20 +934,39 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
 
 namespace {
 
-// Output-argument checks shared by the two flow chains below; dw / dh: resolved destination size.
-int check_chain_outputs(dfb_handle *h, int M, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t *len_x, size_t *len_y) {
-    if (!jpg_x || !jpg_y || !len_x || !len_y) return fail(h, DFB_ERR_INVALID_ARG, "null output");
-    for (int j = 0; j < M; ++j)
-        if (!jpg_x[j] || !jpg_y[j] || host_pointer_kind(jpg_x[j]) < 0 || host_pointer_kind(jpg_y[j]) < 0)
+// Where the files of a flow chain go.  -st=jpg: pair j's two quantised planes (bound) as JPEGs to jpg_x[j] / jpg_y[j];
+// -st=png: pair j's packed flow image (convertFlowToPngImage) as a PNG to png[j].  Every buffer holds `capacity` bytes.
+struct ChainOut {
+    bool as_png = false;
+    int bound = 0, quality = 0;
+    uint8_t *const *jpg_x = nullptr, *const *jpg_y = nullptr;
+    size_t *len_x = nullptr, *len_y = nullptr;
+    uint8_t *const *png = nullptr;
+    size_t *png_len = nullptr;
+    size_t capacity = 0;
+};
+
+bool chain_outputs_null(const ChainOut &o) { return o.as_png ? (!o.png || !o.png_len) : (!o.jpg_x || !o.jpg_y || !o.len_x || !o.len_y); }
+
+// Output-argument checks shared by the flow chains below.
+int check_chain_outputs(dfb_handle *h, int M, const ChainOut &o) {
+    if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    for (int j = 0; j < M; ++j) {
+        if (o.as_png) {
+            if (!o.png[j] || host_pointer_kind(o.png[j]) < 0)
+                return fail(h, DFB_ERR_INVALID_ARG, "png output " + std::to_string(j) + " is null or a device pointer (host entry point)");
+        } else if (!o.jpg_x[j] || !o.jpg_y[j] || host_pointer_kind(o.jpg_x[j]) < 0 || host_pointer_kind(o.jpg_y[j]) < 0) {
             return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(j) + " is null or a device pointer (host entry point)");
+        }
+    }
     return DFB_OK;
 }
 
-// The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) -> flow -> quantise -> two JPEGs per pair.
-// `produce(first, last)` enqueues on s_in the work that leaves frames [first, last] in h->pb_frames (dw x dh each, dense)
-// and records h->chain_ev.frame[f] for each; frames are requested in order.  Runs inside guarded().
-int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, int bound, int jpeg_quality, uint8_t *const *jpg_x,
-                  uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y, const std::function<void(int, int)> &produce) {
+// The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) -> flow -> the output of `o`: quantise and two
+// JPEGs per pair, or convertFlowToPngImage and one PNG per pair.  `produce(first, last)` enqueues on s_in the work that leaves
+// frames [first, last] in h->pb_frames (dw x dh each, dense) and records h->chain_ev.frame[f] for each; frames are requested in
+// order.  Runs inside guarded().
+int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const ChainOut &o, const std::function<void(int, int)> &produce) {
     const int astep = std::abs(step);
     const int M = std::max(n_frames - astep, 0);
     ensure_host_path(h);
@@ -955,12 +977,20 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, int bou
     // threads around queues, include/dense_flow.h:76-80):
     //   s_in      the frame source: decoded frames -> gray -> resize into the gray frame array (decode stage, :154-170)
     //   s_compute pyramids / polynomial expansions + flow of group g, quantised planes out   (:313-342 + src/common.cpp:4-16)
-    //   s_out     the two JPEG encodes per pair of group g, as one batch                      (src/common.cpp:56-57)
+    //             (-st=png: the flow fields, then convertFlowToPngImage of each               src/common.cpp:18-46)
+    //   s_out     the group's encodes, as one batch: two JPEGs per pair (src/common.cpp:56-57) or one PNG (:66-71)
     //   s_fetch   files of group g-1 to the host while the GPU works on group g
     const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
     const size_t fpx = (size_t)dw * dh;
     h->pb_frames.grow(fpx * n_frames);
-    h->pb_q.grow(fpx * 2 * 2 * B);  // quantised planes of two groups
+    if (o.as_png) {
+        h->pb_flow.grow(fpx * 2 * sizeof(float) * 2 * B);  // float2 fields of two groups
+        h->png_bgr.grow(fpx * 3 * 2 * B);    // their packed images
+        ensure_png_scratch(h);
+        if (!h->png) h->png.reset(new PngEncoder());
+    } else {
+        h->pb_q.grow(fpx * 2 * 2 * B);  // quantised planes of two groups
+    }
     alg.ensure_slots(B + astep + 1);
     const int nslots = alg.num_slots();
     auto &ev = h->chain_ev;
@@ -968,7 +998,8 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, int bou
     ev.gray.ensure(2);
     ev.flow.ensure(2);
     ev.enc.ensure(2);
-    JpegSink sink(h, 2 * B, 2);
+    std::optional<JpegSink> sink;
+    if (!o.as_png) sink.emplace(h, 2 * B, 2);
     // the group's 2 m planes, encoded as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
     auto group_planes = [&](int slot) {
         JpegSrc src;
@@ -977,6 +1008,9 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, int bou
         src.pitch = (size_t)dw;
         return src;
     };
+    // pair i of slot's group: its flow field and packed image (-st=png)
+    auto field = [&](int slot, int i) { return h->pb_flow + ((size_t)slot * B + i) * 2 * fpx; };
+    auto image = [&](int slot, int i) { return h->png_bgr + ((size_t)slot * B + i) * 3 * fpx; };
 
     int uploaded = 0;
     auto upload_until = [&](int last) {
@@ -992,36 +1026,63 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, int bou
         const int last_frame = j0 + m - 1 + astep;
         upload_until(last_frame + 1);
         DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.frame[last_frame], 0));
-        if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // the planes of group g-2 have been encoded
+        if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // the outputs of group g-2 have been encoded
         prepare_dense(alg, h->pb_frames, dw, dh, prepared, last_frame, h->s_compute);
         for (int i = 0; i < m; ++i) {
             FlowAlgorithm::PairJob &pj = jobs[i];
             pj = pair_job(j0 + i, step, nslots);
-            pj.bound = bound;
-            pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
-            pj.qy = pj.qx + fpx;
-            pj.q_pitch = (size_t)dw;
+            if (o.as_png) {
+                pj.flow_xy = field(slot, i);
+                pj.flow_pitch_bytes = (size_t)dw * 2 * sizeof(float);
+            } else {
+                pj.bound = o.bound;
+                pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
+                pj.qy = pj.qx + fpx;
+                pj.q_pitch = (size_t)dw;
+            }
         }
         alg.solve_batch(jobs.data(), m, dw, dh, h->s_compute);
+        if (o.as_png) {
+            for (int i = 0; i < m; ++i)
+                launch_flow_to_png_image(field(slot, i), (size_t)dw * 8, dw, dh, image(slot, i), (size_t)dw * 3, h->png_scratch, nullptr,
+                                         h->s_compute);
+            alg.launches += 2 * m;
+        }
         DFB_CUDA(cudaEventRecord(ev.flow[slot], h->s_compute));
-        // encode stage (src/common.cpp:48-64): one JPEG per plane
+        // encode stage (src/common.cpp:48-71)
         DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.flow[slot], 0));
-        sink.encode(slot, 2 * m, group_planes(slot), 1, dw, dh, jpeg_quality, capacity, h->s_out);
+        if (o.as_png)
+            alg.launches += h->png->encode(m, image(slot, 0), 3 * fpx, (size_t)dw * 3, dw, dh, slot, h->s_out);
+        else
+            sink->encode(slot, 2 * m, group_planes(slot), 1, dw, dh, o.quality, o.capacity, h->s_out);
         DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
         h->counters.pairs += m;
     };
     auto finish_group = [&](int g) {
         const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
         DFB_CUDA(cudaEventSynchronize(ev.enc[slot]));
+        if (o.as_png) {
+            auto reject = [&](int i, uint64_t n) {
+                if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
+                return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
+                       std::to_string(o.capacity);
+            };
+            auto out = [&](int i, size_t n) {
+                o.png_len[j0 + i] = n;
+                return o.png[j0 + i];
+            };
+            h->png->files().deliver(slot, m, o.capacity, reject, out, h->counters.d2h_bytes, h->s_fetch);
+            return;
+        }
         auto too_small = [&](int, size_t need) {
-            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(capacity) + ")";
+            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(o.capacity) + ")";
         };
         auto out = [&](int k, size_t len) {
             const int j = j0 + (k >> 1);
-            (k & 1 ? len_y : len_x)[j] = len;
-            return (k & 1 ? jpg_y : jpg_x)[j];
+            (k & 1 ? o.len_y : o.len_x)[j] = len;
+            return (k & 1 ? o.jpg_y : o.jpg_x)[j];
         };
-        sink.deliver(slot, 2 * m, too_small, out, h->s_fetch);
+        sink->deliver(slot, 2 * m, too_small, out, h->s_fetch);
     };
     run_groups((M + B - 1) / B, flow_group, finish_group);
     DFB_CUDA(cudaStreamSynchronize(h->s_in));
@@ -1048,17 +1109,24 @@ int parse_jpegs(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, in
     return DFB_OK;
 }
 
-}  // namespace
+// The files of a JPEG batch parsed, and all of one size: *sw / *sh receive it (n > 0).
+int parse_jpegs_one_size(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n, std::vector<JpegHeader> &hd, int &sw, int &sh) {
+    if (int rc = parse_jpegs(h, jpeg, len, n, hd)) return rc;
+    sw = hd[0].w;
+    sh = hd[0].h;
+    for (int f = 1; f < n; ++f)
+        if (hd[f].w != sw || hd[f].h != sh)
+            return fail(h, DFB_ERR_SIZE, "frame " + std::to_string(f) + " is " + std::to_string(hd[f].w) + "x" + std::to_string(hd[f].h) +
+                                             ", frame 0 is " + std::to_string(sw) + "x" + std::to_string(sh) + " (one size per batch)");
+    return DFB_OK;
+}
 
-extern "C" {
-
-int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
-                               int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
-                               size_t *len_x, size_t *len_y) {
+// dfb_process_bgr_batch_host[_png]: the checks, then the chain with decoded BGR frames as its source
+int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh, const ChainOut &o) {
     if (!h) return DFB_ERR_INVALID_ARG;
     if (!bgr || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
+    if (!o.as_png && o.bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
     if (sw <= 0 || sh <= 0 || dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     if (dw == 0) {
         dw = sw;
@@ -1067,11 +1135,11 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
     if (int rc = check_size(h, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
-    if (!jpg_x || !jpg_y || !len_x || !len_y) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
     for (int f = 0; f < n_frames; ++f)
         if (!bgr[f] || host_pointer_kind(bgr[f]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "bgr[" + std::to_string(f) + "] is null or a device pointer (host entry point)");
-    if (int rc = check_chain_outputs(h, M, jpg_x, jpg_y, len_x, len_y)) return rc;
+    if (int rc = check_chain_outputs(h, M, o)) return rc;
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         // frame source: H2D of BGR frame f into staging buffer f & 1 -> cvtColor -> resize (decode stage tail, :163-170)
@@ -1098,33 +1166,28 @@ int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_f
                 DFB_CUDA(cudaEventRecord(ev.frame[f], h->s_in));
             }
         };
-        return process_chain(h, n_frames, step, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
+        return process_chain(h, n_frames, step, dw, dh, o, produce);
     });
 }
 
-int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh,
-                                int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
-                                size_t *len_x, size_t *len_y) {
+// dfb_process_jpeg_batch_host[_png]: the checks, then the chain with JPEG files decoded on the device as its source
+int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh, const ChainOut &o) {
     if (!h) return DFB_ERR_INVALID_ARG;
     if (!jpeg || !len || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
+    if (!o.as_png && o.bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
     if (dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
     std::vector<JpegHeader> hd;
-    if (int rc = parse_jpegs(h, jpeg, len, n_frames, hd)) return rc;
-    const int sw = hd[0].w, sh = hd[0].h;
-    for (int f = 1; f < n_frames; ++f)
-        if (hd[f].w != sw || hd[f].h != sh)
-            return fail(h, DFB_ERR_SIZE, "frame " + std::to_string(f) + " is " + std::to_string(hd[f].w) + "x" + std::to_string(hd[f].h) +
-                                             ", frame 0 is " + std::to_string(sw) + "x" + std::to_string(sh) + " (one size per batch)");
+    int sw = 0, sh = 0;
+    if (int rc = parse_jpegs_one_size(h, jpeg, len, n_frames, hd, sw, sh)) return rc;
     if (dw == 0) {
         dw = sw;
         dh = sh;
     }
     if (int rc = check_size(h, dw, dh)) return rc;
-    if (int rc = check_chain_outputs(h, M, jpg_x, jpg_y, len_x, len_y)) return rc;
+    if (int rc = check_chain_outputs(h, M, o)) return rc;
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
@@ -1139,7 +1202,7 @@ int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const
                 h->pb_gray.grow(spx * m);
             }
             uint8_t *dst = resize ? h->pb_gray : h->pb_frames + fpx * first;
-            h->jdec->decode(jpeg + first, len + first, hd.data() + first, m, 1, dst, sw, spx, h->s_in);
+            h->jdec->decode(jpeg + first, len + first, hd.data() + first, m, 1, dst, sw, spx, h->s_in, first);
             h->alg->launches += h->jdec->launches;
             for (int f = first; f <= last; ++f) {
                 h->counters.h2d_bytes += len[f];
@@ -1147,8 +1210,100 @@ int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const
                 DFB_CUDA(cudaEventRecord(h->chain_ev.frame[f], h->s_in));
             }
         };
-        return process_chain(h, n_frames, step, dw, dh, bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y, produce);
+        return process_chain(h, n_frames, step, dw, dh, o, produce);
     });
+}
+
+ChainOut jpg_out(int bound, int quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y) {
+    ChainOut o;
+    o.bound = bound;
+    o.quality = quality;
+    o.jpg_x = jpg_x;
+    o.jpg_y = jpg_y;
+    o.len_x = len_x;
+    o.len_y = len_y;
+    o.capacity = capacity;
+    return o;
+}
+
+ChainOut png_out(uint8_t *const *png, size_t capacity, size_t *len) {
+    ChainOut o;
+    o.as_png = true;
+    o.png = png;
+    o.png_len = len;
+    o.capacity = capacity;
+    return o;
+}
+
+}  // namespace
+
+extern "C" {
+
+int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
+                               int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
+                               size_t *len_x, size_t *len_y) {
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, jpg_out(bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y));
+}
+
+int dfb_process_bgr_batch_host_png(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
+                                   uint8_t *const *png, size_t capacity, size_t *len) {
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, png_out(png, capacity, len));
+}
+
+int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh,
+                                int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
+                                size_t *len_x, size_t *len_y) {
+    return jpeg_chain(h, jpeg, len, n_frames, step, dw, dh, jpg_out(bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y));
+}
+
+int dfb_process_jpeg_batch_host_png(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step, int dw,
+                                    int dh, uint8_t *const *png, size_t capacity, size_t *len) {
+    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, png_out(png, capacity, len));
+}
+
+int dfb_new_size(int width, int height, int new_width, int new_height, int new_short, int *dw, int *dh) {
+    if (!dw || !dh) return fail(nullptr, DFB_ERR_INVALID_ARG, "null output");
+    // check_param (src/denseflow_gpu.cpp:27-35)
+    if (new_height < 0 || new_width < 0 || new_short < 0) return fail(nullptr, DFB_ERR_INVALID_ARG, "height and width cannot < 0!");
+    if (new_short > 0 && new_height + new_width != 0) return fail(nullptr, DFB_ERR_INVALID_ARG, "do not set height and width when set short!");
+    if (width <= 0 || height <= 0) return fail(nullptr, DFB_ERR_INVALID_ARG, "width/height must be positive");
+    // get_new_size (:62-79): (int)round(...) of the scaled side
+    auto scaled = [](int a, int b, int n) { return (int)std::round(a * 1.0 / b * n); };
+    *dw = width;
+    *dh = height;
+    if (new_width > 0 && new_height > 0) {
+        *dw = new_width;
+        *dh = new_height;
+    } else if (new_width > 0) {
+        *dw = new_width;
+        *dh = scaled(height, width, new_width);
+    } else if (new_height > 0) {
+        *dw = scaled(width, height, new_height);
+        *dh = new_height;
+    } else if (new_short > 0 && std::min(width, height) > new_short) {
+        if (width < height) {
+            *dw = new_short;
+            *dh = scaled(height, width, new_short);
+        } else {
+            *dw = scaled(width, height, new_short);
+            *dh = new_short;
+        }
+    }
+    return DFB_OK;
+}
+
+int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height) {
+    if (!jpeg || !len || !width || !height) return fail(nullptr, DFB_ERR_INVALID_ARG, "null or empty JPEG buffer");
+    try {
+        const JpegHeader hd = parse_jpeg_header(jpeg, len, 0);
+        *width = hd.w;
+        *height = hd.h;
+        return DFB_OK;
+    } catch (const JpegUnsupported &e) {
+        return fail(nullptr, DFB_ERR_UNSUPPORTED, e.what());
+    } catch (const std::exception &e) {
+        return fail(nullptr, DFB_ERR_INVALID_ARG, e.what());
+    }
 }
 
 int dfb_decode_jpeg_batch_device(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n, int channels, uint8_t *out,
@@ -1307,6 +1462,84 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
                 ++h->alg->launches;
                 DFB_CUDA(cudaEventRecord(ev.conv[sb], h->s_compute));
             }
+            DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
+            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.planes[slot], 0));
+            sink.encode(slot, m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, h->s_out);
+            DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
+        };
+        auto finish_group = [&](int g) {
+            const int f0 = g * G, m = std::min(G, n_frames - f0);
+            DFB_CUDA(cudaEventSynchronize(ev.enc[g & 1]));
+            auto too_small = [&](int i, size_t need) {
+                return "jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " + std::to_string(need) + " bytes, capacity is " +
+                       std::to_string(capacity);
+            };
+            auto out = [&](int i, size_t n) {
+                len[f0 + i] = n;
+                return jpg[f0 + i];
+            };
+            sink.deliver(g & 1, m, too_small, out, h->s_fetch);
+        };
+        run_groups((n_frames + G - 1) / G, convert_group, finish_group);
+        DFB_CUDA(cudaStreamSynchronize(h->s_in));
+        DFB_CUDA(cudaStreamSynchronize(h->s_compute));
+        DFB_CUDA(cudaStreamSynchronize(h->s_out));
+        return DFB_OK;
+    });
+}
+
+int dfb_extract_frames_jpeg_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int dst_width,
+                                 int dst_height, int quality, uint8_t *const *jpg, size_t capacity, size_t *len) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (!jpeg || !jpeg_len || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
+    int dw = dst_width, dh = dst_height;
+    if (dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    if (quality < 1 || quality > 100) return fail(h, DFB_ERR_INVALID_ARG, "quality must be in 1..100");
+    if (n_frames == 0) return DFB_OK;
+    if (!jpg || !len) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    for (int f = 0; f < n_frames; ++f)
+        if (!jpg[f] || host_pointer_kind(jpg[f]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(f) + " is null or a device pointer (host entry point)");
+    std::vector<JpegHeader> hd;
+    int sw = 0, sh = 0;
+    if (int rc = parse_jpegs_one_size(h, jpeg, jpeg_len, n_frames, hd, sw, sh)) return rc;
+    if (int rc = check_extract_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        ensure_fetch_stream(h);
+        if (!h->jdec) h->jdec.reset(new JpegDecoder());
+        // dfb_extract_frames_host's pipeline with the upload replaced by the decode, groups of G frames in flight:
+        //   s_in      imdecode of group g to BGR into staging slot g & 1 (the host waits for the decoder's status)
+        //   s_compute resize + YCbCr 4:2:0 of each frame of the group into the planes of its slot
+        //   s_out     the group's encodes, as one batch
+        //   s_fetch   files of group g-1 to the host while the GPU works on group g
+        constexpr int G = 8;
+        const size_t bgr_bytes = (size_t)sw * sh * 3;
+        const YccLayout L(dw, dh);
+        h->ex_bgr.grow(2 * G * bgr_bytes);
+        h->ex_ycc.grow(2 * G * L.bytes);
+        const ResizeTap *taps = ycc_tables(h, sw, sh, dw, dh);
+        auto &ev = h->extract_ev;
+        for (Events *e : {&ev.h2d, &ev.conv, &ev.planes, &ev.enc}) e->ensure(2);
+        JpegSink sink(h, G, 2);
+
+        auto convert_group = [&](int g) {
+            const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
+            uint8_t *stage = h->ex_bgr + (size_t)slot * G * bgr_bytes;
+            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev.conv[slot], 0));  // group g-2's frames have been converted
+            h->jdec->decode(jpeg + f0, jpeg_len + f0, hd.data() + f0, m, 3, stage, (size_t)sw * 3, bgr_bytes, h->s_in, f0);
+            h->alg->launches += h->jdec->launches;
+            for (int i = 0; i < m; ++i) h->counters.h2d_bytes += jpeg_len[f0 + i];
+            DFB_CUDA(cudaEventRecord(ev.h2d[slot], h->s_in));
+            DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.h2d[slot], 0));
+            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // group g-2's planes have been encoded
+            for (int i = 0; i < m; ++i) {
+                uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
+                launch_bgr_to_ycc420(stage + (size_t)i * bgr_bytes, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch,
+                                     p + L.cb_off, p + L.cr_off, L.c_pitch, h->s_compute, sink.chroma_cols(dw));
+                ++h->alg->launches;
+            }
+            DFB_CUDA(cudaEventRecord(ev.conv[slot], h->s_compute));
             DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
             DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.planes[slot], 0));
             sink.encode(slot, m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, h->s_out);

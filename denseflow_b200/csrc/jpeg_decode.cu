@@ -947,20 +947,20 @@ void JpegDecoder::run_entropy(const uint8_t *const *jpeg, const size_t *len, con
     launches += 4;
 }
 
-void JpegDecoder::check_status(int n, cudaStream_t s) {
+void JpegDecoder::check_status(int n, cudaStream_t s, int index_base) {
     DFB_CUDA(cudaMemcpyAsync(h_flag, d_ws + L->o_status, sizeof(int) * n, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(cudaStreamSynchronize(s));
     for (int i = 0; i < n; ++i) {
-        const int e = h_flag[i];
-        if (e & kErrRst) corrupt(i, "wrong RST marker sequence in the entropy-coded data");
-        if (e & kErrRstCount) corrupt(i, "the number of RST markers does not match the restart interval (truncated or corrupt data)");
-        if (e & kErrCode) corrupt(i, "invalid Huffman code in the entropy-coded data");
-        if (e & kErrShort) corrupt(i, "entropy-coded data ends before the last MCU");
+        const int e = h_flag[i], f = index_base + i;
+        if (e & kErrRst) corrupt(f, "wrong RST marker sequence in the entropy-coded data");
+        if (e & kErrRstCount) corrupt(f, "the number of RST markers does not match the restart interval (truncated or corrupt data)");
+        if (e & kErrCode) corrupt(f, "invalid Huffman code in the entropy-coded data");
+        if (e & kErrShort) corrupt(f, "entropy-coded data ends before the last MCU");
     }
 }
 
 void JpegDecoder::decode(const uint8_t *const *jpeg, const size_t *len, const JpegHeader *hd, int n, int channels, uint8_t *out,
-                         size_t pitch, size_t frame_stride, cudaStream_t s) {
+                         size_t pitch, size_t frame_stride, cudaStream_t s, int index_base) {
     if (n <= 0) return;
     run_entropy(jpeg, len, hd, n, s);
     const Layout &Y = *L;
@@ -979,7 +979,7 @@ void JpegDecoder::decode(const uint8_t *const *jpeg, const size_t *len, const Jp
                                                                                                           pitch, frame_stride);
     DFB_KERNEL_CHECK();
     launches += 2;
-    check_status(n, s);
+    check_status(n, s, index_base);
 }
 
 void JpegDecoder::coefficients(const uint8_t *jpeg, size_t len, const JpegHeader &hd, int16_t *out, cudaStream_t s) {

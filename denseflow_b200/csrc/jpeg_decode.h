@@ -43,9 +43,9 @@ class JpegDecoder {
 
     // Decodes n parsed files.  channels 3: packed BGR rows; 1: cvtColor(BGR2GRAY) of them.  Frame i goes to
     // out + i * frame_stride with rows `pitch` bytes apart.  Enqueued on s; blocks until the device has reported every frame's
-    // status and throws std::runtime_error naming the first corrupt frame.
+    // status and throws std::runtime_error naming the first corrupt frame as index_base + i.
     void decode(const uint8_t *const *jpeg, const size_t *len, const JpegHeader *hd, int n, int channels, uint8_t *out, size_t pitch,
-                size_t frame_stride, cudaStream_t s);
+                size_t frame_stride, cudaStream_t s, int index_base = 0);
     // Test hook: runs only the entropy decode and the DC prefix sums of one file; coefficients in decode (MCU) order, natural
     // order, absolute DC, are copied to the host buffer out (hd.blocks() x 64 int16).
     void coefficients(const uint8_t *jpeg, size_t len, const JpegHeader &hd, int16_t *out, cudaStream_t s);
@@ -55,7 +55,7 @@ class JpegDecoder {
 
   private:
     void run_entropy(const uint8_t *const *jpeg, const size_t *len, const JpegHeader *hd, int n, cudaStream_t s);
-    void check_status(int n, cudaStream_t s);
+    void check_status(int n, cudaStream_t s, int index_base = 0);
 
     // grown on demand
     DeviceBuffer<uint8_t> d_ws;    // device workspace

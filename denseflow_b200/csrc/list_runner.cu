@@ -9,7 +9,11 @@
 // unit of work is one video (its outputs and its completion mark stay together), there is no data-path collective,
 // and completion is reported per chunk with the reference's `last_buffer` meaning.
 //
-// This file is a client of the C ABI (dfb_create / dfb_calc_batch_host[_u8] / dfb_destroy): it adds no arithmetic.
+// dfb_list_run_videos runs the same dispatch over the videos as the reference takes them (colour frames or `-if` JPEG files)
+// and hands out the files the reference writes: flow JPEGs or PNGs, or with step 0 the extracted frames.
+//
+// This file is a client of the C ABI (dfb_create / dfb_calc_batch_host[_u8] / dfb_process_* / dfb_extract_frames_* /
+// dfb_destroy): it adds no arithmetic.
 #include <fcntl.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
@@ -88,6 +92,8 @@ struct dfb_list_runner {
         dfb_handle *h = nullptr;
         void *pinned = nullptr;  // output ring of one chunk: the copy engines write the results straight into it
         size_t pinned_bytes = 0;
+        void *files = nullptr;  // file ring of one chunk of dfb_list_run_videos
+        size_t files_bytes = 0;
     };
     std::vector<Worker> workers;
 };
@@ -126,6 +132,7 @@ void dfb_list_close(dfb_list_runner *r) {
     for (auto &w : r->workers) {
         cudaSetDevice(w.device);
         if (w.pinned) cudaFreeHost(w.pinned);
+        if (w.files) cudaFreeHost(w.files);
         dfb_destroy(w.h);
     }
     delete r;
@@ -244,6 +251,215 @@ int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int ste
     }
     st.seconds = seconds_since(t_start);
     for (auto &w : r->workers) {
+        dfb_counters c{};
+        if (dfb_get_counters(w.h, &c) == DFB_OK) {
+            st.kernel_launches += c.kernel_launches;
+            st.h2d_bytes += c.h2d_bytes;
+            st.d2h_bytes += c.d2h_bytes;
+        }
+    }
+    if (stats) *stats = st;
+    if (failed.load()) {
+        set_err(first_error);
+        return failed.load();
+    }
+    return DFB_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// A chain that saw the frames of video k from f0 on names frame i as "frame i: ..."; the list names it in the video.
+std::string video_error(long k, int f0, const char *msg) {
+    const std::string m = msg ? msg : "";
+    int i = 0, n = 0;
+    if (std::sscanf(m.c_str(), "frame %d: %n", &i, &n) == 1 && n > 0)
+        return "video " + std::to_string(k) + ": frame " + std::to_string(f0 + i) + ": " + m.substr(n);
+    return "video " + std::to_string(k) + ": " + m;
+}
+}  // namespace
+
+extern "C" {
+
+int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_videos, int step, int bound, int save_type, int quality,
+                        int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
+                        dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
+    auto set_err = [&](const std::string &m) {
+        if (err && err_len) std::snprintf(err, err_len, "%s", m.c_str());
+    };
+    if (!r || (!videos && n_videos > 0) || n_videos < 0 || (save_type != DFB_SAVE_JPG && save_type != DFB_SAVE_PNG) ||
+        (jpeg_exact != 0 && jpeg_exact != 1)) {
+        set_err("dfb_list_run_videos: bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
+        return DFB_ERR_INVALID_ARG;
+    }
+    // check_param (src/denseflow_gpu.cpp:23-35): the bound matters only to the flow modes
+    if (step != 0 && bound <= 0) {
+        set_err("bound should > 0!");
+        return DFB_ERR_INVALID_ARG;
+    }
+    const bool writes_jpeg = step == 0 || save_type == DFB_SAVE_JPG;
+    if (writes_jpeg && (quality < 1 || quality > 100)) {
+        set_err("dfb_list_run_videos: quality must be in 1..100");
+        return DFB_ERR_INVALID_ARG;
+    }
+    int dw = 0, dh = 0;
+    if (int rc = dfb_new_size(1, 1, new_width, new_height, new_short, &dw, &dh)) {
+        set_err(dfb_last_error(nullptr));
+        return rc;
+    }
+    if (chunk_flows <= 0) chunk_flows = 64;
+    const int astep = std::abs(step);
+    const int n_workers = (int)r->workers.size();
+    // every video's source and destination size, before any work: get_new_size reads frame 0 (:48-52)
+    struct Geometry {
+        int sw = 0, sh = 0, dw = 0, dh = 0;
+        bool resize = false;
+    };
+    std::vector<Geometry> geo(n_videos);
+    for (int i = 0; i < n_videos; ++i) {
+        const dfb_video &v = videos[i];
+        const bool bgr = v.kind == DFB_VIDEO_BGR;
+        if ((!bgr && v.kind != DFB_VIDEO_JPEG) || v.n_frames < 0 || (v.n_frames > 0 && (bgr ? !v.bgr : (!v.jpeg || !v.jpeg_len))) ||
+            (bgr && (v.width <= 0 || v.height <= 0))) {
+            set_err("dfb_list_run_videos: video " + std::to_string(i) + " is malformed");
+            return DFB_ERR_INVALID_ARG;
+        }
+        Geometry &g = geo[i];
+        if (bgr) {
+            g.sw = v.width;
+            g.sh = v.height;
+        } else if (v.n_frames > 0) {
+            if (int rc = dfb_jpeg_info(v.jpeg[0], v.jpeg_len[0], &g.sw, &g.sh)) {
+                set_err("video " + std::to_string(i) + ": " + dfb_last_error(nullptr));
+                return rc;
+            }
+        } else {
+            continue;  // an empty frame folder: nothing to size
+        }
+        dfb_new_size(g.sw, g.sh, new_width, new_height, new_short, &g.dw, &g.dh);
+        g.resize = g.dw != g.sw || g.dh != g.sh;
+        if (g.dw > r->max_w || g.dh > r->max_h) {
+            set_err("dfb_list_run_videos: video " + std::to_string(i) + " (" + std::to_string(g.dw) + "x" + std::to_string(g.dh) +
+                    " after resizing) exceeds the size given to dfb_list_open");
+            return DFB_ERR_SIZE;
+        }
+    }
+    dfb_list_stats st{};
+    st.workers = n_workers;
+    std::atomic<long> local_next{0};
+    std::atomic<int> failed{0};
+    std::mutex mtx;
+    std::string first_error;
+    auto fail = [&](int code, const std::string &m) {
+        std::lock_guard<std::mutex> lk(mtx);
+        if (!failed.load()) {
+            failed.store(code);
+            first_error = m;
+        }
+    };
+    // the runner owns the handles, so the call's jpeg_exact is set on each of them and restored afterwards
+    std::vector<double> exact_before(n_workers, 0);
+    for (int wi = 0; wi < n_workers; ++wi) {
+        dfb_get_param(r->workers[wi].h, "jpeg_exact", &exact_before[wi]);
+        dfb_set_param(r->workers[wi].h, "jpeg_exact", jpeg_exact);
+    }
+    for (auto &w : r->workers) dfb_reset_counters(w.h);
+    const auto t_start = clk::now();
+
+    auto worker = [&](int wi) {
+        dfb_list_runner::Worker &w = r->workers[wi];
+        cudaSetDevice(w.device);
+        std::vector<uint8_t *> out(2 * chunk_flows), ox(chunk_flows), oy(chunk_flows);
+        std::vector<size_t> lens(2 * chunk_flows), lx(chunk_flows), ly(chunk_flows);
+        double busy = 0;
+        while (!failed.load()) {
+            const long idx = queue ? dfb_queue_next(queue) : local_next.fetch_add(1);
+            if (idx >= n_videos) break;
+            const dfb_video &v = videos[idx];
+            const Geometry &g = geo[idx];
+            const bool bgr = v.kind == DFB_VIDEO_BGR;
+            const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
+            const auto t0 = clk::now();
+            // outputs: flows (:308) or, with step 0, frames; files per output and the capacity of one file
+            const int M = step != 0 ? std::max(v.n_frames - astep, 0) : v.n_frames;
+            const int per = step != 0 && save_type == DFB_SAVE_JPG ? 2 : 1;
+            const size_t cap = step == 0                     ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
+                               : save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
+                                                             : dfb_jpeg_max_bytes(g.dw, g.dh);
+            const size_t need = (size_t)chunk_flows * per * cap;
+            if (M > 0 && w.files_bytes < need) {
+                if (w.files) cudaFreeHost(w.files);
+                w.files = nullptr;
+                w.files_bytes = 0;
+                if (cudaHostAlloc(&w.files, need, cudaHostAllocDefault) != cudaSuccess) {
+                    fail(DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed");
+                    break;
+                }
+                w.files_bytes = need;
+            }
+            uint8_t *ring = static_cast<uint8_t *>(w.files);
+            for (int k = 0; k < per * chunk_flows && ring; ++k) out[k] = ring + (size_t)k * cap;
+            // chunks of outputs [f0, f0 + m); a flow chunk reads frames f0 .. f0 + m - 1 + |step| (see dfb_list_run)
+            int f0 = 0;
+            for (;;) {
+                const int m = std::max(std::min(chunk_flows, M - f0), 0);
+                int rc = DFB_OK;
+                if (m > 0 && step == 0) {
+                    rc = bgr ? dfb_extract_frames_host(w.h, v.bgr + f0, m, g.sw, g.sh, dwa, dha, quality, out.data(), cap, lens.data())
+                             : dfb_extract_frames_jpeg_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m, dwa, dha, quality, out.data(), cap, lens.data());
+                } else if (m > 0 && save_type == DFB_SAVE_PNG) {
+                    rc = bgr ? dfb_process_bgr_batch_host_png(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
+                             : dfb_process_jpeg_batch_host_png(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, out.data(), cap,
+                                                               lens.data());
+                } else if (m > 0) {
+                    for (int i = 0; i < m; ++i) {
+                        ox[i] = out[2 * i];
+                        oy[i] = out[2 * i + 1];
+                    }
+                    rc = bgr ? dfb_process_bgr_batch_host(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, bound, quality, ox.data(), oy.data(),
+                                                          cap, lx.data(), ly.data())
+                             : dfb_process_jpeg_batch_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, bound, quality, ox.data(),
+                                                           oy.data(), cap, lx.data(), ly.data());
+                    for (int i = 0; i < m; ++i) {
+                        lens[2 * i] = lx[i];
+                        lens[2 * i + 1] = ly[i];
+                    }
+                }
+                if (rc != DFB_OK) {
+                    fail(rc, video_error(idx, f0, dfb_last_error(w.h)));
+                    break;
+                }
+                const int last = f0 + m >= M;
+                // every file of this chunk is in host memory now; `last` is FlowBuffer::last_buffer (see dfb_list_run)
+                if (done) done(user, (int)idx, w.device, f0, m, last, out.data(), lens.data());
+                f0 += m;
+                if (last) break;
+            }
+            if (failed.load()) break;
+            busy += seconds_since(t0);
+            std::lock_guard<std::mutex> lk(mtx);
+            ++st.clips;
+            const uint64_t flows = step != 0 ? (uint64_t)M : 0;
+            st.flows += flows;
+            st.frames += (uint64_t)v.n_frames;
+            ++st.clips_per_worker[wi];
+            st.flows_per_worker[wi] += flows;
+        }
+        std::lock_guard<std::mutex> lk(mtx);
+        st.busy_seconds_per_worker[wi] = busy;
+        st.finish_seconds_per_worker[wi] = seconds_since(t_start);
+    };
+
+    if (n_videos > 0) {
+        std::vector<std::thread> threads;
+        for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
+        worker(0);
+        for (auto &t : threads) t.join();
+    }
+    st.seconds = seconds_since(t_start);
+    for (int wi = 0; wi < n_workers; ++wi) {
+        dfb_list_runner::Worker &w = r->workers[wi];
+        dfb_set_param(w.h, "jpeg_exact", exact_before[wi]);
         dfb_counters c{};
         if (dfb_get_counters(w.h, &c) == DFB_OK) {
             st.kernel_launches += c.kernel_launches;

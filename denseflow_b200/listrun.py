@@ -54,6 +54,47 @@ def _pack_clips(clips):
     return arr, shapes, keep
 
 
+def _pack_videos(videos):
+    keep = []
+    arr = (_lib.Video * max(len(videos), 1))()
+    for i, frames in enumerate(videos):
+        v = arr[i]
+        v.n_frames = len(frames)
+        if frames and isinstance(frames[0], (bytes, bytearray, memoryview)):
+            bufs = [np.frombuffer(f, np.uint8) for f in frames]
+            v.kind = _lib.VIDEO_JPEG
+            v.jpeg = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
+            v.jpeg_len = (C.c_size_t * len(bufs))(*[b.size for b in bufs])
+            keep.append((bufs, v.jpeg, v.jpeg_len))
+            continue
+        fr = [np.ascontiguousarray(f) for f in frames]
+        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != fr[0].shape for f in fr):
+            raise RuntimeError("video %d: frames must be uint8 [H,W,3] BGR images of one size, or JPEG files (bytes)" % i)
+        v.kind = _lib.VIDEO_BGR
+        v.bgr = (C.c_void_p * max(len(fr), 1))(*[f.ctypes.data for f in fr])
+        v.height, v.width = fr[0].shape[:2] if fr else (1, 1)
+        keep.append((fr, v.bgr))
+    return arr, keep
+
+
+def output_names(step, first_index, n, save_type="jpg"):
+    """The file names the reference gives a chunk's files (src/common.cpp:73-118), in the order run_videos hands them out:
+    writeFlowImages (flow_x_%05d.jpg / flow_y_%05d.jpg per flow), writeFlowImagesPng (flow_%05d.png) and, with step 0,
+    writeImages (img_%05d.jpg).  Steps > 1 add _p<step>, steps < 0 add _m<|step|> and offset the index by |step|."""
+    if step == 0:
+        return ["img_%05d.jpg" % (first_index + i) for i in range(n)]
+    base = -step if step < 0 else 0
+    tag = "_p%d" % step if step > 1 else "_m%d" % -step if step < 0 else ""
+    names = []
+    for i in range(n):
+        k = first_index + i + base
+        if save_type == "png":
+            names.append("flow%s_%05d.png" % (tag, k))
+        else:
+            names += ["flow_x%s_%05d.jpg" % (tag, k), "flow_y%s_%05d.jpg" % (tag, k)]
+    return names
+
+
 def _callback(on_chunk, shapes):
     if on_chunk is None:
         return None
@@ -104,6 +145,33 @@ class ListRunner:
                                   C.cast(cb, C.c_void_p) if cb else None, None, C.byref(st), err, 512)
         if rc != _lib.DFB_OK:
             raise RuntimeError(err.value.decode() or "dfb_list_run failed (%d)" % rc)
+        return _stats(st)
+
+    def run_videos(self, videos, step=1, bound=20, save_type="jpg", quality=95, jpeg_exact=0, new_width=0, new_height=0, new_short=0,
+                   chunk_flows=0, queue=None, on_chunk=None):
+        """The list as the reference takes it (`denseflow list.txt -s=step -b=bound -st=save_type [-if] [-nw/-nh/-ns]`).
+        videos: one entry per video, a list of uint8 [H,W,3] BGR frames or a list of JPEG files (bytes).  Each video is resized
+        as get_new_size decides and turned into files on the GPU.  on_chunk(video, device, first_index, last_chunk, files) is
+        called on the worker's thread once every file of a chunk is in host memory; files is a list of bytes-like views that
+        die when the callback returns, named as output_names(step, first_index, n, save_type) names them.  last_chunk is the
+        reference's FlowBuffer::last_buffer.  Returns a dict of dfb_list_stats."""
+        if save_type not in ("jpg", "png"):
+            raise RuntimeError("only jpg/png are supported (no %s) for output" % save_type)
+        arr, keep = _pack_videos(videos)
+        per = 2 if step != 0 and save_type == "jpg" else 1
+        cb = None
+        if on_chunk is not None:
+            def _cb(user, video, dev, first, n, last, files, lens):
+                on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
+            cb = _lib.FILES_DONE_FN(_cb)
+        st = _lib.ListStats()
+        err = C.create_string_buffer(512)
+        rc = self._L.dfb_list_run_videos(self._r, arr, len(videos), int(step), int(bound), _lib.SAVE_PNG if save_type == "png" else _lib.SAVE_JPG,
+                                         int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
+                                         queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None, C.byref(st),
+                                         err, 512)
+        if rc != _lib.DFB_OK:
+            raise RuntimeError(err.value.decode() or "dfb_list_run_videos failed (%d)" % rc)
         return _stats(st)
 
     @staticmethod

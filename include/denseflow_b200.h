@@ -73,7 +73,8 @@ const char *dfb_last_error(const dfb_handle *h);
  * file cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality]) writes with OpenCV's other defaults, libjpeg-turbo 3.x:
  * baseline, standard Huffman tables, islow DCT, gray or YCbCr 4:2:0, no restart markers).  It covers
  * dfb_encode_jpeg_gray_device, dfb_encode_jpeg_bgr_device, dfb_process_bgr_batch_host, dfb_process_jpeg_batch_host and
- * dfb_extract_frames_host; the two settings give different bytes and the same flows.  The exact encoder is the project's
+ * dfb_extract_frames_host, dfb_extract_frames_jpeg_host and dfb_list_run_videos; the two settings give different bytes and
+ * the same flows.  The exact encoder is the project's
  * own CUDA and never loads libnvjpeg.  Any other value is DFB_ERR_INVALID_ARG.
  */
 int dfb_set_param(dfb_handle *h, const char *name, double value);
@@ -323,6 +324,36 @@ int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitc
  */
 int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                             uint8_t *const *png, size_t capacity, size_t *len);
+/*
+ * The -st=png branch behind the two colour frame sources: dfb_process_bgr_batch_host / dfb_process_jpeg_batch_host with
+ * flow -> convertFlowToPngImage -> imencode(".png") per pair instead of the two quantised JPEGs.  Pair j's file goes to png[j]
+ * (host buffers of `capacity` bytes each, dfb_png_max_bytes(dst) is always enough), its length to len[j]: byte for byte what
+ * dfb_calc_batch_host_png gives for the gray, resized frames.  Arguments and refusals are those of the JPEG siblings.
+ */
+int dfb_process_bgr_batch_host_png(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int src_width, int src_height,
+                                   int dst_width, int dst_height, uint8_t *const *png, size_t capacity, size_t *len);
+int dfb_process_jpeg_batch_host_png(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step,
+                                    int dst_width, int dst_height, uint8_t *const *png, size_t capacity, size_t *len);
+/*
+ * `-if -s=0`: dfb_extract_frames_host with the frames given as JPEG files of one size (else DFB_ERR_SIZE naming the frame),
+ * decoded on the device to imdecode's BGR pixels.  Frame i's file goes to jpg[i], its length to len[i]: byte for byte what
+ * dfb_extract_frames_host gives for the imdecoded frames.  Refuses what dfb_process_jpeg_batch_host refuses in a file.
+ */
+int dfb_extract_frames_jpeg_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int dst_width,
+                                 int dst_height, int quality, uint8_t *const *jpg, size_t capacity, size_t *len);
+
+/*
+ * ---- size rule and JPEG geometry (pure host functions; no device needed) -----------------------------------------------
+ * dfb_new_size: DenseFlow::get_new_size (src/denseflow_gpu.cpp:44-80) for a w x h source and the -nw / -nh / -ns options:
+ * *dw / *dh receive the destination size, which is the source size when no resize applies (-ns resizes only when
+ * min(w, h) > new_short).  Refuses what check_param (:27-35) refuses, with its texts in dfb_last_error(NULL):
+ * "height and width cannot < 0!" and "do not set height and width when set short!" (DFB_ERR_INVALID_ARG).
+ * dfb_jpeg_info: the frame size of a JPEG file from its markers, so a caller can size a video before decoding it.  Fails as
+ * the imdecode-exact decoder's header parse fails (DFB_ERR_UNSUPPORTED for progressive files, ...; DFB_ERR_INVALID_ARG for
+ * corrupt headers), with the message in dfb_last_error(NULL).
+ */
+int dfb_new_size(int width, int height, int new_width, int new_height, int new_short, int *dw, int *dh);
+int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
 
 /*
  * Test hook: run ONE stand-alone TV-L1 kernel on dense host planes (w*h floats each, uploaded into the engine's pitched
@@ -445,6 +476,38 @@ int dfb_list_open(const char *algorithm, const int *devices, int n_workers, int 
 int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int step, int bound, int chunk_flows, dfb_queue *queue,
                  dfb_chunk_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len);
 void dfb_list_close(dfb_list_runner *r);
+
+/*
+ * ---- the list over videos as the reference takes them: colour frames or `-if` JPEG folders in, files out ------------------
+ * `denseflow list.txt -a=.. -s=S [-if] [-st=jpg|png] [-nw/-nh/-ns]` per video: decode -> get_new_size -> gray / resize -> flow
+ * -> the files writeFlowImages / writeFlowImagesPng write, or with S = 0 extract_frames_video's img files.  Each worker
+ * resolves a video's destination size with dfb_new_size and runs the matching single-handle chain:
+ *   save_type DFB_SAVE_JPG  dfb_process_{bgr,jpeg}_batch_host        files 2 i / 2 i + 1: flow first_index + i's x / y
+ *   save_type DFB_SAVE_PNG  dfb_process_{bgr,jpeg}_batch_host_png    file i: flow first_index + i
+ *   step 0                  dfb_extract_frames_host / dfb_extract_frames_jpeg_host   file i: frame first_index + i (img)
+ * Chunks, queue and stats are those of dfb_list_run (stats: frames = decoded frames, flows = flow fields); max_width /
+ * max_height of dfb_list_open bound the DESTINATION size.  jpeg_exact is set on every worker handle for the call and restored.
+ * `done` runs on the worker's thread once every file of the chunk is in host memory; last_chunk (FlowBuffer::last_buffer) is 1
+ * exactly once per video, after all its files (a video without outputs gets one call with n = 0).  The files live in the
+ * worker's pinned ring and are reused after the callback returns.  bound <= 0 with a flow step is refused ("bound should >
+ * 0!"); step 0 ignores bound.  A refused or corrupt JPEG fails the call with "video k: frame f: ..." (f: index in the video);
+ * the runner stays usable.
+ */
+enum { DFB_VIDEO_BGR = 0, DFB_VIDEO_JPEG = 1 };
+enum { DFB_SAVE_JPG = 0, DFB_SAVE_PNG = 1 };
+typedef struct {
+    int kind;                       /* DFB_VIDEO_BGR or DFB_VIDEO_JPEG */
+    int n_frames;
+    const uint8_t *const *bgr;      /* BGR: n_frames host pointers to dense packed BGR frames of width x height */
+    int width, height;
+    const uint8_t *const *jpeg;     /* JPEG: n_frames host pointers to the files' bytes, jpeg_len[i] bytes each */
+    const size_t *jpeg_len;
+} dfb_video;
+typedef void (*dfb_files_done_fn)(void *user, int video, int device, int first_index, int n, int last_chunk, const uint8_t *const *files,
+                                  const size_t *lens);
+int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_videos, int step, int bound, int save_type, int quality,
+                        int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
+                        dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len);
 
 #ifdef __cplusplus
 }
