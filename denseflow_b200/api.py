@@ -288,12 +288,8 @@ class DenseOpticalFlow:
         else:
             ow, oh = self.max_width, self.max_height  # an upper bound of the frame size (checked by the call)
         cap = self._L.dfb_jpeg_max_bytes(ow, oh)
-        bx = [np.empty(cap, np.uint8) for _ in range(m)]
-        by = [np.empty(cap, np.uint8) for _ in range(m)]
-        xp = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bx])
-        yp = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in by])
-        lx = (C.c_size_t * max(m, 1))()
-        ly = (C.c_size_t * max(m, 1))()
+        bx, xp, lx = self._file_buffers(m, cap)
+        by, yp, ly = self._file_buffers(m, cap)
         self._check(self._L.dfb_process_jpeg_batch_host(self._h, ptrs, lens, n, step, dw, dh, int(bound), int(quality), xp, yp, cap, lx, ly))
         return [(bx[i][:lx[i]].tobytes(), by[i][:ly[i]].tobytes()) for i in range(m)]
 
@@ -323,13 +319,9 @@ class DenseOpticalFlow:
         ow, oh = (dw, dh) if new_size else (sw, sh)
         m = max(n - abs(step), 0)
         cap = self._L.dfb_jpeg_max_bytes(ow, oh)
-        bx = [np.empty(cap, np.uint8) for _ in range(m)]
-        by = [np.empty(cap, np.uint8) for _ in range(m)]
+        bx, xp, lx = self._file_buffers(m, cap)
+        by, yp, ly = self._file_buffers(m, cap)
         fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        xp = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bx])
-        yp = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in by])
-        lx = (C.c_size_t * max(m, 1))()
-        ly = (C.c_size_t * max(m, 1))()
         self._check(self._L.dfb_process_bgr_batch_host(self._h, fp, n, step, sw, sh, dw, dh, int(bound), int(quality), xp, yp, cap, lx, ly))
         return [(bx[i][:lx[i]].tobytes(), by[i][:ly[i]].tobytes()) for i in range(m)]
 
@@ -380,10 +372,8 @@ class DenseOpticalFlow:
         sh, sw = frames[0].shape[:2]
         dw, dh = new_size if new_size else (0, 0)
         cap = self._L.dfb_jpeg_max_bytes_bgr(*(new_size if new_size else (sw, sh)))
-        bufs = [np.empty(cap, np.uint8) for _ in range(n)]
+        bufs, op, lens = self._file_buffers(n, cap)
         fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        op = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        lens = (C.c_size_t * n)()
         self._check(self._L.dfb_extract_frames_host(self._h, fp, n, sw, sh, dw, dh, int(quality), op, cap, lens))
         return [bufs[i][:lens[i]].tobytes() for i in range(n)]
 
@@ -407,10 +397,11 @@ class DenseOpticalFlow:
             raise RuntimeError("%s: frames must be uint8 [H,W,3] images of one size" % name)
         return [np.ascontiguousarray(f) for f in frames]
 
-    def _png_buffers(self, m, w, h):
-        cap = self._L.dfb_png_max_bytes(w, h)
+    @staticmethod
+    def _file_buffers(m, cap):
+        """m host buffers of cap bytes for the files of one call: (buffers, their pointer array, the length array)"""
         bufs = [np.empty(max(cap, 1), np.uint8) for _ in range(m)]
-        return bufs, (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bufs]), (C.c_size_t * max(m, 1))(), cap
+        return bufs, (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bufs]), (C.c_size_t * max(m, 1))()
 
     def process_bgr_batch_png(self, frames_bgr, step=1, new_size=None):
         """-st=png for decoded BGR frames: gray -> resize -> flow -> convertFlowToPngImage -> imencode(".png") on the GPU.
@@ -423,7 +414,8 @@ class DenseOpticalFlow:
         sh, sw = frames[0].shape[:2]
         dw, dh = new_size if new_size else (0, 0)
         m = max(n - abs(step), 0)
-        bufs, op, lens, cap = self._png_buffers(m, *(new_size if new_size else (sw, sh)))
+        cap = self._L.dfb_png_max_bytes(*(new_size if new_size else (sw, sh)))
+        bufs, op, lens = self._file_buffers(m, cap)
         fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
         self._check(self._L.dfb_process_bgr_batch_host_png(self._h, fp, n, step, sw, sh, dw, dh, op, cap, lens))
         return [bufs[i][:lens[i]].tobytes() for i in range(m)]
@@ -435,7 +427,8 @@ class DenseOpticalFlow:
         n = len(keep)
         dw, dh = new_size if new_size else (0, 0)
         m = max(n - abs(step), 0)
-        bufs, op, plens, cap = self._png_buffers(m, *(new_size if new_size else (self.max_width, self.max_height)))
+        cap = self._L.dfb_png_max_bytes(*(new_size if new_size else (self.max_width, self.max_height)))
+        bufs, op, plens = self._file_buffers(m, cap)
         self._check(self._L.dfb_process_jpeg_batch_host_png(self._h, ptrs, lens, n, step, dw, dh, op, cap, plens))
         return [bufs[i][:plens[i]].tobytes() for i in range(m)]
 
@@ -448,9 +441,7 @@ class DenseOpticalFlow:
             return []
         dw, dh = new_size if new_size else (0, 0)
         cap = self._L.dfb_jpeg_max_bytes_bgr(*(new_size if new_size else (self.max_width, self.max_height)))
-        bufs = [np.empty(cap, np.uint8) for _ in range(n)]
-        op = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        olens = (C.c_size_t * n)()
+        bufs, op, olens = self._file_buffers(n, cap)
         self._check(self._L.dfb_extract_frames_jpeg_host(self._h, ptrs, lens, n, dw, dh, int(quality), op, cap, olens))
         return [bufs[i][:olens[i]].tobytes() for i in range(n)]
 

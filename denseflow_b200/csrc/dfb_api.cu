@@ -28,10 +28,10 @@ struct TapTable {
     int sw = 0, sh = 0, dw = 0, dh = 0;
 };
 
-// CUDA events created on first use and destroyed with their owner
+// CUDA events created on first use and destroyed with their owner; they record no time unless flags says so
 class Events {
   public:
-    Events() = default;
+    explicit Events(unsigned flags = cudaEventDisableTiming) : flags_(flags) {}
     Events(const Events &) = delete;
     Events &operator=(const Events &) = delete;
     ~Events() {
@@ -40,13 +40,14 @@ class Events {
     void ensure(size_t n) {
         while (e_.size() < n) {
             cudaEvent_t e;
-            DFB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            DFB_CUDA(cudaEventCreateWithFlags(&e, flags_));
             e_.push_back(e);
         }
     }
     cudaEvent_t operator[](size_t i) const { return e_[i]; }
 
   private:
+    unsigned flags_;
     std::vector<cudaEvent_t> e_;
 };
 
@@ -92,9 +93,9 @@ struct dfb_handle {
     // scratch of the frame-extraction calls (-s=0), grown on demand
     TapTable ycc_taps;                // colour resize of all three calls
     DeviceBuffer<uint8_t> enc_ycc;    // Y / Cb / Cr planes of dfb_encode_jpeg_bgr_device
-    DeviceBuffer<uint8_t> ex_bgr, ex_ycc;  // dfb_extract_frames_host: two staging frames, planes of two groups
+    DeviceBuffer<uint8_t> ex_bgr, ex_ycc;  // the -s=0 pipeline: BGR staging of its frame source, planes of two groups
     struct {
-        Events h2d, conv;     // [2] staging buffer filled, consumed
+        Events h2d, conv;     // [2] BGR staging filled; the BGR source's staging frame consumed
         Events planes, enc;   // [2] a group's planes ready, its encodes done
     } extract_ev;
     // "jpeg_exact" = 1: every JPEG this handle writes is imencode(".jpg")'s bytes (JpegExactEncoder) instead of nvJPEG's
@@ -231,9 +232,9 @@ bool is_device_pointer(const void *p) {
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
-// Geometry of a frame-extraction call: source sw x sh (packed BGR rows of bgr_pitch bytes), destination dw x dh, where
+// Geometry of a call that resizes BGR frames: source sw x sh (packed BGR rows of bgr_pitch bytes), destination dw x dh, where
 // 0 / 0 means no resize.  Resolves the destination and checks it against the handle's maximum.
-int check_extract_geometry(dfb_handle *h, int sw, int sh, size_t bgr_pitch, int &dw, int &dh) {
+int check_geometry(dfb_handle *h, int sw, int sh, size_t bgr_pitch, int &dw, int &dh) {
     if (sw <= 0 || sh <= 0 || dw < 0 || dh < 0 || (dw == 0) != (dh == 0) || bgr_pitch < (size_t)sw * 3)
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     if (dw == 0) {
@@ -415,18 +416,51 @@ void resize_gray(dfb_handle *h, const uint8_t *src, size_t src_pitch, int sw, in
     ++h->alg->launches;
 }
 
-// PNG output of batch_host (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j]
-struct PngSink {
+// The -st=png output of a flow batch (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j];
+// every buffer holds `capacity` bytes.  The stages run on s_compute (pack), s_out (encode) and s_fetch (read-back); the caller
+// records and waits for its own events between them.
+struct PngOut {
     uint8_t *const *out;
     size_t capacity;
     size_t *len;
+
+    // the pack scratch and the encoder, created on first use
+    static void prepare(dfb_handle *h) {
+        ensure_png_scratch(h);
+        if (!h->png) h->png.reset(new PngEncoder());
+    }
+    // s_compute: convertFlowToPngImage (src/common.cpp:18-46) of the m fields field(i) (w x hh float2) into m packed images
+    // from bgr, 3 w hh bytes apart
+    template <typename Field> static void pack(dfb_handle *h, int m, Field &&field, int w, int hh, uint8_t *bgr) {
+        for (int i = 0; i < m; ++i)
+            launch_flow_to_png_image(field(i), (size_t)w * 8, w, hh, bgr + (size_t)i * 3 * w * hh, (size_t)w * 3, h->png_scratch, nullptr,
+                                     h->s_compute);
+        h->alg->launches += 2 * m;
+    }
+    // s_out: imencode(".png") (:66-71) of the m packed images from bgr, as one batch into the encoder's slot
+    static void encode(dfb_handle *h, int m, const uint8_t *bgr, int w, int hh, int slot) {
+        h->alg->launches += h->png->encode(m, bgr, (size_t)3 * w * hh, (size_t)w * 3, w, hh, slot, h->s_out);
+    }
+    // once the slot's encode is complete: the files of pairs j0 .. j0 + m - 1 to the caller on s_fetch
+    void deliver(dfb_handle *h, int j0, int m, int slot) const {
+        auto reject = [&](int i, uint64_t n) {
+            if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
+            return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
+                   std::to_string(capacity);
+        };
+        auto to = [&](int i, size_t n) {
+            len[j0 + i] = n;
+            return out[j0 + i];
+        };
+        h->png->files().deliver(slot, m, capacity, reject, to, h->counters.d2h_bytes, h->s_fetch);
+    }
 };
 
 // The batch shape of calc_optflows_imp (src/denseflow_gpu.cpp:307-342) over host buffers.
 // quantise: bound > 0 => emit two u8 planes per pair instead of the float2 field.
 // png: non-null => pack every flow field (convertFlowToPngImage) and emit imencode(".png") of it instead of the field.
 int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, float *const *flows,
-               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngSink *png = nullptr) {
+               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngOut *png = nullptr) {
     if (int rc = check_size(h, w, hh)) return rc;
     if (n_frames < 0 || !frames) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
@@ -459,25 +493,15 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
     const size_t bgr_bytes = fbytes * 3;
     if (png) {
         ensure_fetch_stream(h);
-        ensure_png_scratch(h);
         h->png_bgr.grow(OR * bgr_bytes);
-        if (!h->png) h->png.reset(new PngEncoder());
+        PngOut::prepare(h);
     }
     // -st=png: the files of group g (slot g & 1) are read back while the GPU works on group g + 1
     auto png_finish = [&](int g) {
         if (!png) return;
         const int j0 = g * B, m = std::min(B, M - j0);
         DFB_CUDA(cudaEventSynchronize(h->ev_out[(j0 + m - 1) % OR]));
-        auto reject = [&](int i, uint64_t n) {
-            if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
-            return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
-                   std::to_string(png->capacity);
-        };
-        auto out = [&](int i, size_t n) {
-            png->len[j0 + i] = n;
-            return png->out[j0 + i];
-        };
-        h->png->files().deliver(g & 1, m, png->capacity, reject, out, h->counters.d2h_bytes, h->s_fetch);
+        png->deliver(h, j0, m, g & 1);
     };
 
     int uploaded = 0;  // frames [0, uploaded) have H2D + pyramid enqueued
@@ -553,13 +577,10 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
             // (:66-71); s_fetch: the previous group's files to the host
             const int r0 = j0 % OR;
             uint8_t *bgr0 = h->png_bgr + (size_t)r0 * bgr_bytes;
-            for (int i = 0; i < m; ++i)
-                launch_flow_to_png_image(h->d_flow[r0 + i], (size_t)w * 8, w, hh, bgr0 + (size_t)i * bgr_bytes, (size_t)w * 3, h->png_scratch,
-                                         nullptr, h->s_compute);
-            alg.launches += 2 * m;
+            PngOut::pack(h, m, [&](int i) -> const float * { return h->d_flow[r0 + i]; }, w, hh, bgr0);
             DFB_CUDA(cudaEventRecord(h->ev_done[r0], h->s_compute));
             DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[r0], 0));
-            alg.launches += h->png->encode(m, bgr0, bgr_bytes, (size_t)w * 3, w, hh, g & 1, h->s_out);
+            PngOut::encode(h, m, bgr0, w, hh, g & 1);
             for (int i = 0; i < m; ++i) DFB_CUDA(cudaEventRecord(h->ev_out[r0 + i], h->s_out));
             h->counters.pairs += m;
             return;
@@ -934,28 +955,33 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
 
 namespace {
 
-// Where the files of a flow chain go.  -st=jpg: pair j's two quantised planes (bound) as JPEGs to jpg_x[j] / jpg_y[j];
-// -st=png: pair j's packed flow image (convertFlowToPngImage) as a PNG to png[j].  Every buffer holds `capacity` bytes.
-struct ChainOut {
-    bool as_png = false;
-    int bound = 0, quality = 0;
-    uint8_t *const *jpg_x = nullptr, *const *jpg_y = nullptr;
-    size_t *len_x = nullptr, *len_y = nullptr;
-    uint8_t *const *png = nullptr;
-    size_t *png_len = nullptr;
-    size_t capacity = 0;
+// -st=jpg output of a flow chain: pair j's two quantised planes (bound) as JPEGs to x[j] / y[j], their lengths to len_x[j] /
+// len_y[j]; every buffer holds `capacity` bytes
+struct JpgOut {
+    int bound, quality;
+    uint8_t *const *x, *const *y;
+    size_t capacity;
+    size_t *len_x, *len_y;
 };
 
-bool chain_outputs_null(const ChainOut &o) { return o.as_png ? (!o.png || !o.png_len) : (!o.jpg_x || !o.jpg_y || !o.len_x || !o.len_y); }
+// Where the files of a flow chain go: exactly one of the two is set.
+struct ChainOut {
+    const JpgOut *jpg;
+    const PngOut *png;
+};
+
+bool chain_outputs_null(const ChainOut &o) {
+    return o.png ? (!o.png->out || !o.png->len) : (!o.jpg->x || !o.jpg->y || !o.jpg->len_x || !o.jpg->len_y);
+}
 
 // Output-argument checks shared by the flow chains below.
 int check_chain_outputs(dfb_handle *h, int M, const ChainOut &o) {
     if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
     for (int j = 0; j < M; ++j) {
-        if (o.as_png) {
-            if (!o.png[j] || host_pointer_kind(o.png[j]) < 0)
+        if (o.png) {
+            if (!o.png->out[j] || host_pointer_kind(o.png->out[j]) < 0)
                 return fail(h, DFB_ERR_INVALID_ARG, "png output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-        } else if (!o.jpg_x[j] || !o.jpg_y[j] || host_pointer_kind(o.jpg_x[j]) < 0 || host_pointer_kind(o.jpg_y[j]) < 0) {
+        } else if (!o.jpg->x[j] || !o.jpg->y[j] || host_pointer_kind(o.jpg->x[j]) < 0 || host_pointer_kind(o.jpg->y[j]) < 0) {
             return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(j) + " is null or a device pointer (host entry point)");
         }
     }
@@ -983,11 +1009,10 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
     const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
     const size_t fpx = (size_t)dw * dh;
     h->pb_frames.grow(fpx * n_frames);
-    if (o.as_png) {
+    if (o.png) {
         h->pb_flow.grow(fpx * 2 * sizeof(float) * 2 * B);  // float2 fields of two groups
         h->png_bgr.grow(fpx * 3 * 2 * B);    // their packed images
-        ensure_png_scratch(h);
-        if (!h->png) h->png.reset(new PngEncoder());
+        PngOut::prepare(h);
     } else {
         h->pb_q.grow(fpx * 2 * 2 * B);  // quantised planes of two groups
     }
@@ -999,7 +1024,7 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
     ev.flow.ensure(2);
     ev.enc.ensure(2);
     std::optional<JpegSink> sink;
-    if (!o.as_png) sink.emplace(h, 2 * B, 2);
+    if (o.jpg) sink.emplace(h, 2 * B, 2);
     // the group's 2 m planes, encoded as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
     auto group_planes = [&](int slot) {
         JpegSrc src;
@@ -1031,56 +1056,43 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
         for (int i = 0; i < m; ++i) {
             FlowAlgorithm::PairJob &pj = jobs[i];
             pj = pair_job(j0 + i, step, nslots);
-            if (o.as_png) {
+            if (o.png) {
                 pj.flow_xy = field(slot, i);
                 pj.flow_pitch_bytes = (size_t)dw * 2 * sizeof(float);
             } else {
-                pj.bound = o.bound;
+                pj.bound = o.jpg->bound;
                 pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
                 pj.qy = pj.qx + fpx;
                 pj.q_pitch = (size_t)dw;
             }
         }
         alg.solve_batch(jobs.data(), m, dw, dh, h->s_compute);
-        if (o.as_png) {
-            for (int i = 0; i < m; ++i)
-                launch_flow_to_png_image(field(slot, i), (size_t)dw * 8, dw, dh, image(slot, i), (size_t)dw * 3, h->png_scratch, nullptr,
-                                         h->s_compute);
-            alg.launches += 2 * m;
-        }
+        if (o.png) PngOut::pack(h, m, [&](int i) { return field(slot, i); }, dw, dh, image(slot, 0));
         DFB_CUDA(cudaEventRecord(ev.flow[slot], h->s_compute));
         // encode stage (src/common.cpp:48-71)
         DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.flow[slot], 0));
-        if (o.as_png)
-            alg.launches += h->png->encode(m, image(slot, 0), 3 * fpx, (size_t)dw * 3, dw, dh, slot, h->s_out);
+        if (o.png)
+            PngOut::encode(h, m, image(slot, 0), dw, dh, slot);
         else
-            sink->encode(slot, 2 * m, group_planes(slot), 1, dw, dh, o.quality, o.capacity, h->s_out);
+            sink->encode(slot, 2 * m, group_planes(slot), 1, dw, dh, o.jpg->quality, o.jpg->capacity, h->s_out);
         DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
         h->counters.pairs += m;
     };
     auto finish_group = [&](int g) {
         const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
         DFB_CUDA(cudaEventSynchronize(ev.enc[slot]));
-        if (o.as_png) {
-            auto reject = [&](int i, uint64_t n) {
-                if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
-                return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
-                       std::to_string(o.capacity);
-            };
-            auto out = [&](int i, size_t n) {
-                o.png_len[j0 + i] = n;
-                return o.png[j0 + i];
-            };
-            h->png->files().deliver(slot, m, o.capacity, reject, out, h->counters.d2h_bytes, h->s_fetch);
+        if (o.png) {
+            o.png->deliver(h, j0, m, slot);
             return;
         }
+        const JpgOut &jo = *o.jpg;
         auto too_small = [&](int, size_t need) {
-            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(o.capacity) + ")";
+            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(jo.capacity) + ")";
         };
         auto out = [&](int k, size_t len) {
             const int j = j0 + (k >> 1);
-            (k & 1 ? o.len_y : o.len_x)[j] = len;
-            return (k & 1 ? o.jpg_y : o.jpg_x)[j];
+            (k & 1 ? jo.len_y : jo.len_x)[j] = len;
+            return (k & 1 ? jo.y : jo.x)[j];
         };
         sink->deliver(slot, 2 * m, too_small, out, h->s_fetch);
     };
@@ -1121,18 +1133,20 @@ int parse_jpegs_one_size(dfb_handle *h, const uint8_t *const *jpeg, const size_t
     return DFB_OK;
 }
 
+// The checks both flow chains make first, in this order: the frame array, step, bound, the requested size (0 / 0: none).
+int check_chain_args(dfb_handle *h, bool frames_null, int n_frames, int step, const ChainOut &o, int dw, int dh) {
+    if (frames_null || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
+    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
+    if (o.jpg && o.jpg->bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
+    if (dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    return DFB_OK;
+}
+
 // dfb_process_bgr_batch_host[_png]: the checks, then the chain with decoded BGR frames as its source
 int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh, const ChainOut &o) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (!bgr || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
-    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    if (!o.as_png && o.bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
-    if (sw <= 0 || sh <= 0 || dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
-    if (dw == 0) {
-        dw = sw;
-        dh = sh;
-    }
-    if (int rc = check_size(h, dw, dh)) return rc;
+    if (int rc = check_chain_args(h, !bgr, n_frames, step, o, dw, dh)) return rc;
+    if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
     if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
@@ -1173,20 +1187,13 @@ int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, 
 // dfb_process_jpeg_batch_host[_png]: the checks, then the chain with JPEG files decoded on the device as its source
 int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh, const ChainOut &o) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (!jpeg || !len || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
-    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    if (!o.as_png && o.bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
-    if (dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
+    if (int rc = check_chain_args(h, !jpeg || !len, n_frames, step, o, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
     std::vector<JpegHeader> hd;
     int sw = 0, sh = 0;
     if (int rc = parse_jpegs_one_size(h, jpeg, len, n_frames, hd, sw, sh)) return rc;
-    if (dw == 0) {
-        dw = sw;
-        dh = sh;
-    }
-    if (int rc = check_size(h, dw, dh)) return rc;
+    if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
     if (int rc = check_chain_outputs(h, M, o)) return rc;
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
@@ -1214,25 +1221,65 @@ int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int
     });
 }
 
-ChainOut jpg_out(int bound, int quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity, size_t *len_x, size_t *len_y) {
-    ChainOut o;
-    o.bound = bound;
-    o.quality = quality;
-    o.jpg_x = jpg_x;
-    o.jpg_y = jpg_y;
-    o.len_x = len_x;
-    o.len_y = len_y;
-    o.capacity = capacity;
-    return o;
-}
+constexpr int kExtractGroup = 8;  // frames per group of the -s=0 pipeline
 
-ChainOut png_out(uint8_t *const *png, size_t capacity, size_t *len) {
-    ChainOut o;
-    o.as_png = true;
-    o.png = png;
-    o.png_len = len;
-    o.capacity = capacity;
-    return o;
+// The frame source of the -s=0 pipeline: source(g, f0, m, convert) enqueues the work that leaves the BGR of group g's frames
+// f0 .. f0 + m - 1 readable by s_compute, and calls convert(i, bgr) for frame f0 + i once it is.
+using ConvertFrame = std::function<void(int, const uint8_t *)>;
+using FrameSource = std::function<void(int, int, int, const ConvertFrame &)>;
+
+// extract_frames_video's batch (src/denseflow_gpu.cpp:82-144: resize + imencode(".jpg") per frame) of n_frames sw x sh BGR frames
+// on four streams, groups of G frames in flight:
+//   s_in      the frame source: the group's frames to BGR in h->ex_bgr (room for `staging` frames)
+//   s_compute resize + YCbCr 4:2:0 of each frame into the planes of its group
+//   s_out     the group's encodes, as one batch
+//   s_fetch   files of group g-1 to the host while the GPU works on group g
+// Runs inside guarded().
+int extract_frames(dfb_handle *h, int n_frames, int sw, int sh, int dw, int dh, int quality, uint8_t *const *jpg, size_t capacity,
+                   size_t *len, int staging, const FrameSource &source) {
+    constexpr int G = kExtractGroup;
+    ensure_fetch_stream(h);
+    const YccLayout L(dw, dh);
+    h->ex_bgr.grow((size_t)staging * sw * sh * 3);
+    h->ex_ycc.grow(2 * G * L.bytes);
+    const ResizeTap *taps = ycc_tables(h, sw, sh, dw, dh);
+    auto &ev = h->extract_ev;
+    for (Events *e : {&ev.h2d, &ev.conv, &ev.planes, &ev.enc}) e->ensure(2);
+    JpegSink sink(h, G, 2);
+
+    auto convert_group = [&](int g) {
+        const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
+        uint8_t *planes = h->ex_ycc + (size_t)slot * G * L.bytes;
+        if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // group g-2's planes have been encoded
+        source(g, f0, m, [&](int i, const uint8_t *bgr) {
+            uint8_t *p = planes + (size_t)i * L.bytes;
+            launch_bgr_to_ycc420(bgr, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
+                                 p + L.cr_off, L.c_pitch, h->s_compute, sink.chroma_cols(dw));
+            ++h->alg->launches;
+        });
+        DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
+        DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.planes[slot], 0));
+        sink.encode(slot, m, ycc_src(planes, L), 3, dw, dh, quality, capacity, h->s_out);
+        DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
+    };
+    auto finish_group = [&](int g) {
+        const int f0 = g * G, m = std::min(G, n_frames - f0);
+        DFB_CUDA(cudaEventSynchronize(ev.enc[g & 1]));
+        auto too_small = [&](int i, size_t need) {
+            return "jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " + std::to_string(need) + " bytes, capacity is " +
+                   std::to_string(capacity);
+        };
+        auto out = [&](int i, size_t n) {
+            len[f0 + i] = n;
+            return jpg[f0 + i];
+        };
+        sink.deliver(g & 1, m, too_small, out, h->s_fetch);
+    };
+    run_groups((n_frames + G - 1) / G, convert_group, finish_group);
+    DFB_CUDA(cudaStreamSynchronize(h->s_in));
+    DFB_CUDA(cudaStreamSynchronize(h->s_compute));
+    DFB_CUDA(cudaStreamSynchronize(h->s_out));
+    return DFB_OK;
 }
 
 }  // namespace
@@ -1242,23 +1289,27 @@ extern "C" {
 int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
                                int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
                                size_t *len_x, size_t *len_y) {
-    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, jpg_out(bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y));
+    const JpgOut o{bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y};
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, {&o, nullptr});
 }
 
 int dfb_process_bgr_batch_host_png(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
                                    uint8_t *const *png, size_t capacity, size_t *len) {
-    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, png_out(png, capacity, len));
+    const PngOut o{png, capacity, len};
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, {nullptr, &o});
 }
 
 int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh,
                                 int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
                                 size_t *len_x, size_t *len_y) {
-    return jpeg_chain(h, jpeg, len, n_frames, step, dw, dh, jpg_out(bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y));
+    const JpgOut o{bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y};
+    return jpeg_chain(h, jpeg, len, n_frames, step, dw, dh, {&o, nullptr});
 }
 
 int dfb_process_jpeg_batch_host_png(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step, int dw,
                                     int dh, uint8_t *const *png, size_t capacity, size_t *len) {
-    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, png_out(png, capacity, len));
+    const PngOut o{png, capacity, len};
+    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, {nullptr, &o});
 }
 
 int dfb_new_size(int width, int height, int new_width, int new_height, int new_short, int *dw, int *dh) {
@@ -1359,7 +1410,7 @@ int dfb_bgr_to_ycc420_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch
     if (!h) return DFB_ERR_INVALID_ARG;
     if (!bgr || !y || !cb || !cr) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     int dw = dst_width, dh = dst_height;
-    if (int rc = check_extract_geometry(h, src_width, src_height, bgr_pitch, dw, dh)) return rc;
+    if (int rc = check_geometry(h, src_width, src_height, bgr_pitch, dw, dh)) return rc;
     if (y_pitch < (size_t)dw || c_pitch < (size_t)(dw + 1) / 2) return fail(h, DFB_ERR_INVALID_ARG, "pitch smaller than a row");
     for (const void *p : {(const void *)bgr, (const void *)y, (const void *)cb, (const void *)cr})
         if (!is_device_pointer(p)) return fail(h, DFB_ERR_INVALID_ARG, "bgr / y / cb / cr must be device memory (device entry point)");
@@ -1385,7 +1436,7 @@ int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pit
     if (!h) return DFB_ERR_INVALID_ARG;
     if (!bgr || !out || !out_len) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     int dw = dst_width, dh = dst_height;
-    if (int rc = check_extract_geometry(h, src_width, src_height, bgr_pitch, dw, dh)) return rc;
+    if (int rc = check_geometry(h, src_width, src_height, bgr_pitch, dw, dh)) return rc;
     if (quality < 1 || quality > 100) return fail(h, DFB_ERR_INVALID_ARG, "quality must be in 1..100");
     if (!is_device_pointer(bgr)) return fail(h, DFB_ERR_INVALID_ARG, "bgr must be device memory (device entry point)");
     if (host_pointer_kind(out) < 0) return fail(h, DFB_ERR_INVALID_ARG, "out must be host memory");
@@ -1415,7 +1466,7 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
     if (!h) return DFB_ERR_INVALID_ARG;
     if (!bgr || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     int dw = dst_width, dh = dst_height;
-    if (int rc = check_extract_geometry(h, src_width, src_height, (size_t)src_width * 3, dw, dh)) return rc;
+    if (int rc = check_geometry(h, src_width, src_height, (size_t)src_width * 3, dw, dh)) return rc;
     if (quality < 1 || quality > 100) return fail(h, DFB_ERR_INVALID_ARG, "quality must be in 1..100");
     if (n_frames == 0) return DFB_OK;
     if (!jpg || !len) return fail(h, DFB_ERR_INVALID_ARG, "null output");
@@ -1428,26 +1479,10 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
     const int sw = src_width, sh = src_height;
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
-        ensure_fetch_stream(h);
-        // extract_frames_video's batch (src/denseflow_gpu.cpp:82-144: resize + imencode(".jpg") per frame) on four streams,
-        // groups of G frames in flight:
-        //   s_in      H2D of frame f into staging buffer f & 1
-        //   s_compute resize + YCbCr 4:2:0 of frame f into the planes of its group
-        //   s_out     the group's encodes, as one batch
-        //   s_fetch   files of group g-1 to the host while the GPU works on group g
-        constexpr int G = 8;
+        // frame source: H2D of frame f into staging frame f & 1, interleaved with the converts
         const size_t bgr_bytes = (size_t)sw * sh * 3;
-        const YccLayout L(dw, dh);
-        h->ex_bgr.grow(2 * bgr_bytes);
-        h->ex_ycc.grow(2 * G * L.bytes);
-        const ResizeTap *taps = ycc_tables(h, sw, sh, dw, dh);
-        auto &ev = h->extract_ev;
-        for (Events *e : {&ev.h2d, &ev.conv, &ev.planes, &ev.enc}) e->ensure(2);
-        JpegSink sink(h, G, 2);
-
-        auto convert_group = [&](int g) {
-            const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
-            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // group g-2's planes have been encoded
+        auto upload = [&](int, int f0, int m, const ConvertFrame &convert) {
+            auto &ev = h->extract_ev;
             for (int i = 0; i < m; ++i) {
                 const int f = f0 + i, sb = f & 1;
                 uint8_t *stage = h->ex_bgr + sb * bgr_bytes;
@@ -1456,35 +1491,11 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
                 DFB_CUDA(cudaEventRecord(ev.h2d[sb], h->s_in));
                 h->counters.h2d_bytes += bgr_bytes;
                 DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.h2d[sb], 0));
-                uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
-                launch_bgr_to_ycc420(stage, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                                     p + L.cr_off, L.c_pitch, h->s_compute, sink.chroma_cols(dw));
-                ++h->alg->launches;
+                convert(i, stage);
                 DFB_CUDA(cudaEventRecord(ev.conv[sb], h->s_compute));
             }
-            DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
-            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.planes[slot], 0));
-            sink.encode(slot, m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, h->s_out);
-            DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
         };
-        auto finish_group = [&](int g) {
-            const int f0 = g * G, m = std::min(G, n_frames - f0);
-            DFB_CUDA(cudaEventSynchronize(ev.enc[g & 1]));
-            auto too_small = [&](int i, size_t need) {
-                return "jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " + std::to_string(need) + " bytes, capacity is " +
-                       std::to_string(capacity);
-            };
-            auto out = [&](int i, size_t n) {
-                len[f0 + i] = n;
-                return jpg[f0 + i];
-            };
-            sink.deliver(g & 1, m, too_small, out, h->s_fetch);
-        };
-        run_groups((n_frames + G - 1) / G, convert_group, finish_group);
-        DFB_CUDA(cudaStreamSynchronize(h->s_in));
-        DFB_CUDA(cudaStreamSynchronize(h->s_compute));
-        DFB_CUDA(cudaStreamSynchronize(h->s_out));
-        return DFB_OK;
+        return extract_frames(h, n_frames, sw, sh, dw, dh, quality, jpg, capacity, len, 2, upload);
     });
 }
 
@@ -1503,66 +1514,26 @@ int dfb_extract_frames_jpeg_host(dfb_handle *h, const uint8_t *const *jpeg, cons
     std::vector<JpegHeader> hd;
     int sw = 0, sh = 0;
     if (int rc = parse_jpegs_one_size(h, jpeg, jpeg_len, n_frames, hd, sw, sh)) return rc;
-    if (int rc = check_extract_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
+    if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
-        ensure_fetch_stream(h);
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
-        // dfb_extract_frames_host's pipeline with the upload replaced by the decode, groups of G frames in flight:
-        //   s_in      imdecode of group g to BGR into staging slot g & 1 (the host waits for the decoder's status)
-        //   s_compute resize + YCbCr 4:2:0 of each frame of the group into the planes of its slot
-        //   s_out     the group's encodes, as one batch
-        //   s_fetch   files of group g-1 to the host while the GPU works on group g
-        constexpr int G = 8;
+        // frame source: imdecode of group g to BGR into staging slot g & 1 (the host waits for the decoder's status)
+        constexpr int G = kExtractGroup;
         const size_t bgr_bytes = (size_t)sw * sh * 3;
-        const YccLayout L(dw, dh);
-        h->ex_bgr.grow(2 * G * bgr_bytes);
-        h->ex_ycc.grow(2 * G * L.bytes);
-        const ResizeTap *taps = ycc_tables(h, sw, sh, dw, dh);
-        auto &ev = h->extract_ev;
-        for (Events *e : {&ev.h2d, &ev.conv, &ev.planes, &ev.enc}) e->ensure(2);
-        JpegSink sink(h, G, 2);
-
-        auto convert_group = [&](int g) {
-            const int f0 = g * G, m = std::min(G, n_frames - f0), slot = g & 1;
+        auto decode = [&](int g, int f0, int m, const ConvertFrame &convert) {
+            auto &ev = h->extract_ev;
+            const int slot = g & 1;
             uint8_t *stage = h->ex_bgr + (size_t)slot * G * bgr_bytes;
-            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev.conv[slot], 0));  // group g-2's frames have been converted
+            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_in, ev.planes[slot], 0));  // group g-2's frames have been converted
             h->jdec->decode(jpeg + f0, jpeg_len + f0, hd.data() + f0, m, 3, stage, (size_t)sw * 3, bgr_bytes, h->s_in, f0);
             h->alg->launches += h->jdec->launches;
             for (int i = 0; i < m; ++i) h->counters.h2d_bytes += jpeg_len[f0 + i];
             DFB_CUDA(cudaEventRecord(ev.h2d[slot], h->s_in));
             DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.h2d[slot], 0));
-            if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // group g-2's planes have been encoded
-            for (int i = 0; i < m; ++i) {
-                uint8_t *p = h->ex_ycc + (size_t)(slot * G + i) * L.bytes;
-                launch_bgr_to_ycc420(stage + (size_t)i * bgr_bytes, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch,
-                                     p + L.cb_off, p + L.cr_off, L.c_pitch, h->s_compute, sink.chroma_cols(dw));
-                ++h->alg->launches;
-            }
-            DFB_CUDA(cudaEventRecord(ev.conv[slot], h->s_compute));
-            DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
-            DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.planes[slot], 0));
-            sink.encode(slot, m, ycc_src(h->ex_ycc + (size_t)slot * G * L.bytes, L), 3, dw, dh, quality, capacity, h->s_out);
-            DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
+            for (int i = 0; i < m; ++i) convert(i, stage + (size_t)i * bgr_bytes);
         };
-        auto finish_group = [&](int g) {
-            const int f0 = g * G, m = std::min(G, n_frames - f0);
-            DFB_CUDA(cudaEventSynchronize(ev.enc[g & 1]));
-            auto too_small = [&](int i, size_t need) {
-                return "jpeg output buffer too small: frame " + std::to_string(f0 + i) + " needs " + std::to_string(need) + " bytes, capacity is " +
-                       std::to_string(capacity);
-            };
-            auto out = [&](int i, size_t n) {
-                len[f0 + i] = n;
-                return jpg[f0 + i];
-            };
-            sink.deliver(g & 1, m, too_small, out, h->s_fetch);
-        };
-        run_groups((n_frames + G - 1) / G, convert_group, finish_group);
-        DFB_CUDA(cudaStreamSynchronize(h->s_in));
-        DFB_CUDA(cudaStreamSynchronize(h->s_compute));
-        DFB_CUDA(cudaStreamSynchronize(h->s_out));
-        return DFB_OK;
+        return extract_frames(h, n_frames, sw, sh, dw, dh, quality, jpg, capacity, len, 2 * G, decode);
     });
 }
 
@@ -1597,8 +1568,8 @@ int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_f
     if (n_frames > std::abs(step) && (!png || !len)) return fail(h, DFB_ERR_INVALID_ARG, "png / len is null");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
-        const PngSink sink{png, capacity, len};
-        return batch_host(h, frames, n_frames, step, width, height, nullptr, 0, nullptr, nullptr, &sink);
+        const PngOut out{png, capacity, len};
+        return batch_host(h, frames, n_frames, step, width, height, nullptr, 0, nullptr, nullptr, &out);
     });
 }
 
@@ -1618,12 +1589,13 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             if (ow <= 0 || oh <= 0) throw std::runtime_error("resize: bad destination size");
         }
         const int pitch = round_up(width, 32), opitch = round_up(ow, 32);
-        std::vector<float *> dev;
+        std::vector<std::unique_ptr<DeviceBuffer<float>>> dev;
         auto alloc = [&](int w_, int h_, int p_) {
-            float *p = nullptr;
-            DFB_CUDA(cudaMalloc(&p, (size_t)p_ * (h_ + 1) * sizeof(float)));
-            DFB_CUDA(cudaMemset(p, 0, (size_t)p_ * (h_ + 1) * sizeof(float)));
-            dev.push_back(p);
+            const size_t bytes = (size_t)p_ * (h_ + 1) * sizeof(float);
+            dev.emplace_back(new DeviceBuffer<float>());
+            dev.back()->allocate(bytes);
+            float *p = *dev.back();
+            DFB_CUDA(cudaMemset(p, 0, bytes));
             return Plane{p, w_, h_, p_};
         };
         std::vector<Plane> pin, pout;
@@ -1631,7 +1603,7 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             pin.push_back(alloc(width, height, pitch));
             DFB_CUDA(cudaMemcpy2D(pin[i].p, (size_t)pitch * 4, in[i], (size_t)width * 4, (size_t)width * 4, height, cudaMemcpyHostToDevice));
         }
-        double *d_part = nullptr, *d_sum = nullptr;
+        DeviceBuffer<double> d_part, d_sum;  // estimate_u's energy partials and their sum, when asked for
         auto need = [&](int ni, int no) {
             if (n_in != ni || n_out != no) throw std::runtime_error(k + ": expects " + std::to_string(ni) + " inputs and " + std::to_string(no) + " outputs");
         };
@@ -1650,8 +1622,8 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             const bool calc = sc(2) != 0;
             const int nblk = estimate_u_blocks(width, height);
             if (calc) {
-                DFB_CUDA(cudaMalloc(&d_part, sizeof(double) * nblk));
-                DFB_CUDA(cudaMalloc(&d_sum, sizeof(double)));
+                d_part.allocate(sizeof(double) * nblk);
+                d_sum.allocate(sizeof(double));
             }
             launch_estimate_u(pin[0], pin[1], pin[2], pin[3], pin[4], pin[5], pin[6], pin[7], pin[8], pin[9], c, d_part, nullptr);
             if (calc) {
@@ -1669,7 +1641,6 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             pout = {alloc(ow, oh, opitch)};
             launch_resize_linear(pin[0], pout[0], (float)sc(2), (float)sc(3), n_scalars > 4 ? (float)sc(4) : 1.0f, nullptr);
         } else {
-            for (float *p : dev) cudaFree(p);
             throw std::runtime_error("unknown debug kernel " + k);
         }
         DFB_CUDA(cudaDeviceSynchronize());
@@ -1677,9 +1648,6 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             const Plane &src = inplace_from >= 0 ? pin[inplace_from + i] : pout[i];
             DFB_CUDA(cudaMemcpy2D(out[i], (size_t)src.w * 4, src.p, (size_t)src.pitch * 4, (size_t)src.w * 4, src.h, cudaMemcpyDeviceToHost));
         }
-        for (float *p : dev) cudaFree(p);
-        if (d_part) cudaFree(d_part);
-        if (d_sum) cudaFree(d_sum);
         return DFB_OK;
     });
 }
@@ -1695,8 +1663,8 @@ int dfb_debug_time_kernel(dfb_handle *h, const char *kernel, int width, int heig
         const int nplanes = primal ? 10 : 6;
         const int pitch = round_up(width, 32);
         const size_t pe = (size_t)pitch * (height + 1);
-        float *buf = nullptr;
-        DFB_CUDA(cudaMalloc(&buf, pe * sizeof(float) * nplanes * sets));
+        DeviceBuffer<float> buf;
+        buf.allocate(pe * sizeof(float) * nplanes * sets);
         auto plane = [&](int set, int i) { return Plane{buf + ((size_t)set * nplanes + i) * pe, width, height, pitch}; };
         for (int sidx = 0; sidx < sets; ++sidx)
             for (int i = 0; i < nplanes; ++i) launch_fill(plane(sidx, i), 0.125f * (float)(i + 1), nullptr);
@@ -1709,19 +1677,15 @@ int dfb_debug_time_kernel(dfb_handle *h, const char *kernel, int width, int heig
                 launch_estimate_dual(plane(sidx, 0), plane(sidx, 1), plane(sidx, 2), plane(sidx, 3), plane(sidx, 4), plane(sidx, 5), c, nullptr);
         };
         for (int i = 0; i < 3; ++i) run(i % sets);
-        cudaEvent_t e0, e1;
-        DFB_CUDA(cudaEventCreate(&e0));
-        DFB_CUDA(cudaEventCreate(&e1));
-        DFB_CUDA(cudaEventRecord(e0, nullptr));
+        Events ev(cudaEventDefault);
+        ev.ensure(2);
+        DFB_CUDA(cudaEventRecord(ev[0], nullptr));
         for (int i = 0; i < reps; ++i) run((i + 3) % sets);
-        DFB_CUDA(cudaEventRecord(e1, nullptr));
-        DFB_CUDA(cudaEventSynchronize(e1));
+        DFB_CUDA(cudaEventRecord(ev[1], nullptr));
+        DFB_CUDA(cudaEventSynchronize(ev[1]));
         float ms = 0.f;
-        DFB_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+        DFB_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
         *ms_per_launch = (double)ms / reps;
-        cudaEventDestroy(e0);
-        cudaEventDestroy(e1);
-        cudaFree(buf);
         return DFB_OK;
     });
 }

@@ -32,6 +32,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/denseflow_b200.h"
+#include "common.cuh"
 
 struct dfb_queue {
     std::atomic<long> *counter = nullptr;  // lives in the shared mapping
@@ -42,6 +43,10 @@ struct dfb_queue {
 namespace {
 using clk = std::chrono::steady_clock;
 double seconds_since(clk::time_point t0) { return std::chrono::duration<double>(clk::now() - t0).count(); }
+
+void set_error(char *err, size_t err_len, const std::string &m) {
+    if (err && err_len) std::snprintf(err, err_len, "%s", m.c_str());
+}
 }  // namespace
 
 extern "C" {
@@ -90,38 +95,33 @@ struct dfb_list_runner {
     struct Worker {
         int device = 0;
         dfb_handle *h = nullptr;
-        void *pinned = nullptr;  // output ring of one chunk: the copy engines write the results straight into it
-        size_t pinned_bytes = 0;
-        void *files = nullptr;  // file ring of one chunk of dfb_list_run_videos
-        size_t files_bytes = 0;
+        dfb::PinnedBuffer<uint8_t> pinned;  // output ring of one chunk: the copy engines write the results straight into it
+        dfb::PinnedBuffer<uint8_t> files;   // file ring of one chunk of dfb_list_run_videos
     };
     std::vector<Worker> workers;
 };
 
 int dfb_list_open(const char *algorithm, const int *devices, int n_workers, int max_width, int max_height, dfb_list_runner **out, char *err,
                   size_t err_len) {
-    auto set_err = [&](const std::string &m) {
-        if (err && err_len) std::snprintf(err, err_len, "%s", m.c_str());
-    };
     if (!out) return DFB_ERR_INVALID_ARG;
     *out = nullptr;
     if (!algorithm || !devices || n_workers < 1 || n_workers > DFB_LIST_MAX_WORKERS || max_width <= 0 || max_height <= 0) {
-        set_err("dfb_list_open: bad arguments");
+        set_error(err, err_len, "dfb_list_open: bad arguments");
         return DFB_ERR_INVALID_ARG;
     }
     dfb_list_runner *r = new dfb_list_runner();
     r->algorithm = algorithm;
     r->max_w = max_width;
     r->max_h = max_height;
+    r->workers = std::vector<dfb_list_runner::Worker>(n_workers);
     for (int wi = 0; wi < n_workers; ++wi) {
-        dfb_list_runner::Worker w;
+        dfb_list_runner::Worker &w = r->workers[wi];
         w.device = devices[wi];
         if (int rc = dfb_create(algorithm, w.device, max_width, max_height, &w.h)) {
-            set_err("worker " + std::to_string(wi) + ": " + dfb_last_error(nullptr));
+            set_error(err, err_len, "worker " + std::to_string(wi) + ": " + dfb_last_error(nullptr));
             dfb_list_close(r);
             return rc;
         }
-        r->workers.push_back(w);
     }
     *out = r;
     return DFB_OK;
@@ -129,121 +129,68 @@ int dfb_list_open(const char *algorithm, const int *devices, int n_workers, int 
 
 void dfb_list_close(dfb_list_runner *r) {
     if (!r) return;
-    for (auto &w : r->workers) {
-        cudaSetDevice(w.device);
-        if (w.pinned) cudaFreeHost(w.pinned);
-        if (w.files) cudaFreeHost(w.files);
-        dfb_destroy(w.h);
-    }
-    delete r;
+    for (auto &w : r->workers) dfb_destroy(w.h);
+    delete r;  // and with it the workers' pinned rings
 }
 
-int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int step, int bound, int chunk_flows, dfb_queue *queue,
-                 dfb_chunk_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
-    auto set_err = [&](const std::string &m) {
-        if (err && err_len) std::snprintf(err, err_len, "%s", m.c_str());
-    };
-    if (!r || (!clips && n_clips > 0) || n_clips < 0 || step == 0 || bound < 0) {
-        set_err("dfb_list_run: bad arguments (step must be non-zero: step 0 is the frame-extraction mode)");
-        return DFB_ERR_INVALID_ARG;
-    }
-    if (chunk_flows <= 0) chunk_flows = 64;
-    const int astep = std::abs(step);
+}  // extern "C"
+
+namespace {
+
+// What one item of a list gives: DFB_OK and the flows and frames it adds to the stats, or the error that ends the run.
+struct ItemResult {
+    int rc = DFB_OK;
+    std::string error;
+    uint64_t flows = 0, frames = 0;
+};
+
+// The dispatch of dfb_list_run and dfb_list_run_videos.  Each worker, on a host thread of its own (worker 0 on the caller's),
+// takes items from `queue` (or from an in-process counter) until all n_items are taken or an item fails; body(wi, idx) runs
+// item idx on worker wi.  The first failure's code is returned and its message written to err; stats receives the run's
+// counters either way.
+template <typename Body>
+int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, dfb_list_stats *stats, char *err, size_t err_len) {
     const int n_workers = (int)r->workers.size();
-    for (int i = 0; i < n_clips; ++i) {
-        if (clips[i].n_frames < 0 || clips[i].width <= 0 || clips[i].height <= 0 || (clips[i].n_frames > 0 && !clips[i].frames)) {
-            set_err("dfb_list_run: clip " + std::to_string(i) + " is malformed");
-            return DFB_ERR_INVALID_ARG;
-        }
-        if (clips[i].width > r->max_w || clips[i].height > r->max_h) {
-            set_err("dfb_list_run: clip " + std::to_string(i) + " exceeds the size given to dfb_list_open");
-            return DFB_ERR_SIZE;
-        }
-    }
     dfb_list_stats st{};
     st.workers = n_workers;
     std::atomic<long> local_next{0};
     std::atomic<int> failed{0};
     std::mutex mtx;
     std::string first_error;
-    auto fail = [&](int code, const std::string &m) {
-        std::lock_guard<std::mutex> lk(mtx);
-        if (!failed.load()) {
-            failed.store(code);
-            first_error = m;
-        }
-    };
-    const size_t px_max = (size_t)r->max_w * r->max_h;
-    const size_t out_bytes = (size_t)chunk_flows * px_max * (bound > 0 ? 2 : 8);
     for (auto &w : r->workers) dfb_reset_counters(w.h);
     const auto t_start = clk::now();
 
     auto worker = [&](int wi) {
-        dfb_list_runner::Worker &w = r->workers[wi];
-        cudaSetDevice(w.device);
-        if (w.pinned_bytes < out_bytes) {
-            if (w.pinned) cudaFreeHost(w.pinned);
-            w.pinned = nullptr;
-            w.pinned_bytes = 0;
-            if (cudaHostAlloc(&w.pinned, out_bytes, cudaHostAllocDefault) != cudaSuccess) {
-                fail(DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned output allocation failed");
-                return;
-            }
-            w.pinned_bytes = out_bytes;
-        }
-        uint8_t *qbuf = bound > 0 ? static_cast<uint8_t *>(w.pinned) : nullptr;
-        float *fbuf = bound > 0 ? nullptr : static_cast<float *>(w.pinned);
-        std::vector<uint8_t *> qx(chunk_flows), qy(chunk_flows);
-        std::vector<float *> fl(chunk_flows);
+        cudaSetDevice(r->workers[wi].device);
         double busy = 0;
         while (!failed.load()) {
             const long idx = queue ? dfb_queue_next(queue) : local_next.fetch_add(1);
-            if (idx >= n_clips) break;
-            const dfb_clip &c = clips[idx];
+            if (idx >= n_items) break;
             const auto t0 = clk::now();
-            const size_t px = (size_t)c.width * c.height;
-            const int M = std::max(c.n_frames - astep, 0);  // src/denseflow_gpu.cpp:308
-            for (int i = 0; i < chunk_flows; ++i) {
-                qx[i] = qbuf ? qbuf + (size_t)(2 * i) * px : nullptr;
-                qy[i] = qbuf ? qbuf + (size_t)(2 * i + 1) * px : nullptr;
-                fl[i] = fbuf ? fbuf + (size_t)i * px * 2 : nullptr;
-            }
-            // chunks of flows [f0, f0 + m): frames f0 .. f0 + m - 1 + |step| (the overlap the reference keeps between its
-            // own <= 512-frame batches, src/denseflow_gpu.cpp:182-189,204-205), so flow indices stay global (base_start)
-            int f0 = 0;
-            for (;;) {
-                const int m = std::max(std::min(chunk_flows, M - f0), 0);
-                int rc = DFB_OK;
-                if (m > 0)
-                    rc = bound > 0 ? dfb_calc_batch_host_u8(w.h, c.frames + f0, m + astep, step, c.width, c.height, bound, qx.data(), qy.data())
-                                   : dfb_calc_batch_host(w.h, c.frames + f0, m + astep, step, c.width, c.height, fl.data());
-                if (rc != DFB_OK) {
-                    fail(rc, "clip " + std::to_string(idx) + ": " + dfb_last_error(w.h));
-                    break;
+            const ItemResult res = body(wi, idx);
+            if (res.rc != DFB_OK) {
+                std::lock_guard<std::mutex> lk(mtx);
+                if (!failed.load()) {
+                    failed.store(res.rc);
+                    first_error = res.error;
                 }
-                const int last = f0 + m >= M;
-                // every output of this chunk is in host memory now; `last` is the reference's FlowBuffer::last_buffer,
-                // the only point at which a video may be marked done
-                if (done) done(user, (int)idx, w.device, f0, m, last, bound > 0 ? qx.data() : nullptr, bound > 0 ? qy.data() : nullptr,
-                               bound > 0 ? nullptr : fl.data());
-                f0 += m;
-                if (last) break;
+                break;
             }
             if (failed.load()) break;
             busy += seconds_since(t0);
             std::lock_guard<std::mutex> lk(mtx);
             ++st.clips;
-            st.flows += (uint64_t)M;
-            st.frames += (uint64_t)c.n_frames;
+            st.flows += res.flows;
+            st.frames += res.frames;
             ++st.clips_per_worker[wi];
-            st.flows_per_worker[wi] += (uint64_t)M;
+            st.flows_per_worker[wi] += res.flows;
         }
         std::lock_guard<std::mutex> lk(mtx);
         st.busy_seconds_per_worker[wi] = busy;
         st.finish_seconds_per_worker[wi] = seconds_since(t_start);
     };
 
-    if (n_clips > 0) {
+    if (n_items > 0) {
         std::vector<std::thread> threads;
         for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
         worker(0);
@@ -260,15 +207,12 @@ int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int ste
     }
     if (stats) *stats = st;
     if (failed.load()) {
-        set_err(first_error);
+        set_error(err, err_len, first_error);
         return failed.load();
     }
     return DFB_OK;
 }
 
-}  // extern "C"
-
-namespace {
 // A chain that saw the frames of video k from f0 on names frame i as "frame i: ..."; the list names it in the video.
 std::string video_error(long k, int f0, const char *msg) {
     const std::string m = msg ? msg : "";
@@ -277,34 +221,95 @@ std::string video_error(long k, int f0, const char *msg) {
         return "video " + std::to_string(k) + ": frame " + std::to_string(f0 + i) + ": " + m.substr(n);
     return "video " + std::to_string(k) + ": " + m;
 }
+
 }  // namespace
 
 extern "C" {
 
+int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int step, int bound, int chunk_flows, dfb_queue *queue,
+                 dfb_chunk_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
+    if (!r || (!clips && n_clips > 0) || n_clips < 0 || step == 0 || bound < 0) {
+        set_error(err, err_len, "dfb_list_run: bad arguments (step must be non-zero: step 0 is the frame-extraction mode)");
+        return DFB_ERR_INVALID_ARG;
+    }
+    if (chunk_flows <= 0) chunk_flows = 64;
+    const int astep = std::abs(step);
+    for (int i = 0; i < n_clips; ++i) {
+        if (clips[i].n_frames < 0 || clips[i].width <= 0 || clips[i].height <= 0 || (clips[i].n_frames > 0 && !clips[i].frames)) {
+            set_error(err, err_len, "dfb_list_run: clip " + std::to_string(i) + " is malformed");
+            return DFB_ERR_INVALID_ARG;
+        }
+        if (clips[i].width > r->max_w || clips[i].height > r->max_h) {
+            set_error(err, err_len, "dfb_list_run: clip " + std::to_string(i) + " exceeds the size given to dfb_list_open");
+            return DFB_ERR_SIZE;
+        }
+    }
+    const size_t px_max = (size_t)r->max_w * r->max_h;
+    const size_t out_bytes = (size_t)chunk_flows * px_max * (bound > 0 ? 2 : 8);
+
+    auto run_clip = [&](int wi, long idx) -> ItemResult {
+        dfb_list_runner::Worker &w = r->workers[wi];
+        try {
+            w.pinned.allocate(out_bytes);
+        } catch (const dfb::CudaError &) {
+            return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned output allocation failed"};
+        }
+        uint8_t *qbuf = bound > 0 ? (uint8_t *)w.pinned : nullptr;
+        float *fbuf = bound > 0 ? nullptr : reinterpret_cast<float *>((uint8_t *)w.pinned);
+        std::vector<uint8_t *> qx(chunk_flows), qy(chunk_flows);
+        std::vector<float *> fl(chunk_flows);
+        const dfb_clip &c = clips[idx];
+        const size_t px = (size_t)c.width * c.height;
+        const int M = std::max(c.n_frames - astep, 0);  // src/denseflow_gpu.cpp:308
+        for (int i = 0; i < chunk_flows; ++i) {
+            qx[i] = qbuf ? qbuf + (size_t)(2 * i) * px : nullptr;
+            qy[i] = qbuf ? qbuf + (size_t)(2 * i + 1) * px : nullptr;
+            fl[i] = fbuf ? fbuf + (size_t)i * px * 2 : nullptr;
+        }
+        // chunks of flows [f0, f0 + m): frames f0 .. f0 + m - 1 + |step| (the overlap the reference keeps between its
+        // own <= 512-frame batches, src/denseflow_gpu.cpp:182-189,204-205), so flow indices stay global (base_start)
+        int f0 = 0;
+        for (;;) {
+            const int m = std::max(std::min(chunk_flows, M - f0), 0);
+            int rc = DFB_OK;
+            if (m > 0)
+                rc = bound > 0 ? dfb_calc_batch_host_u8(w.h, c.frames + f0, m + astep, step, c.width, c.height, bound, qx.data(), qy.data())
+                               : dfb_calc_batch_host(w.h, c.frames + f0, m + astep, step, c.width, c.height, fl.data());
+            if (rc != DFB_OK) return {rc, "clip " + std::to_string(idx) + ": " + dfb_last_error(w.h)};
+            const int last = f0 + m >= M;
+            // every output of this chunk is in host memory now; `last` is the reference's FlowBuffer::last_buffer,
+            // the only point at which a video may be marked done
+            if (done) done(user, (int)idx, w.device, f0, m, last, bound > 0 ? qx.data() : nullptr, bound > 0 ? qy.data() : nullptr,
+                           bound > 0 ? nullptr : fl.data());
+            f0 += m;
+            if (last) break;
+        }
+        return {DFB_OK, {}, (uint64_t)M, (uint64_t)c.n_frames};
+    };
+    return run_items(r, n_clips, queue, run_clip, stats, err, err_len);
+}
+
 int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_videos, int step, int bound, int save_type, int quality,
                         int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
                         dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
-    auto set_err = [&](const std::string &m) {
-        if (err && err_len) std::snprintf(err, err_len, "%s", m.c_str());
-    };
     if (!r || (!videos && n_videos > 0) || n_videos < 0 || (save_type != DFB_SAVE_JPG && save_type != DFB_SAVE_PNG) ||
         (jpeg_exact != 0 && jpeg_exact != 1)) {
-        set_err("dfb_list_run_videos: bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
+        set_error(err, err_len, "dfb_list_run_videos: bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
         return DFB_ERR_INVALID_ARG;
     }
     // check_param (src/denseflow_gpu.cpp:23-35): the bound matters only to the flow modes
     if (step != 0 && bound <= 0) {
-        set_err("bound should > 0!");
+        set_error(err, err_len, "bound should > 0!");
         return DFB_ERR_INVALID_ARG;
     }
     const bool writes_jpeg = step == 0 || save_type == DFB_SAVE_JPG;
     if (writes_jpeg && (quality < 1 || quality > 100)) {
-        set_err("dfb_list_run_videos: quality must be in 1..100");
+        set_error(err, err_len, "dfb_list_run_videos: quality must be in 1..100");
         return DFB_ERR_INVALID_ARG;
     }
     int dw = 0, dh = 0;
     if (int rc = dfb_new_size(1, 1, new_width, new_height, new_short, &dw, &dh)) {
-        set_err(dfb_last_error(nullptr));
+        set_error(err, err_len, dfb_last_error(nullptr));
         return rc;
     }
     if (chunk_flows <= 0) chunk_flows = 64;
@@ -321,7 +326,7 @@ int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_video
         const bool bgr = v.kind == DFB_VIDEO_BGR;
         if ((!bgr && v.kind != DFB_VIDEO_JPEG) || v.n_frames < 0 || (v.n_frames > 0 && (bgr ? !v.bgr : (!v.jpeg || !v.jpeg_len))) ||
             (bgr && (v.width <= 0 || v.height <= 0))) {
-            set_err("dfb_list_run_videos: video " + std::to_string(i) + " is malformed");
+            set_error(err, err_len, "dfb_list_run_videos: video " + std::to_string(i) + " is malformed");
             return DFB_ERR_INVALID_ARG;
         }
         Geometry &g = geo[i];
@@ -330,7 +335,7 @@ int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_video
             g.sh = v.height;
         } else if (v.n_frames > 0) {
             if (int rc = dfb_jpeg_info(v.jpeg[0], v.jpeg_len[0], &g.sw, &g.sh)) {
-                set_err("video " + std::to_string(i) + ": " + dfb_last_error(nullptr));
+                set_error(err, err_len, "video " + std::to_string(i) + ": " + dfb_last_error(nullptr));
                 return rc;
             }
         } else {
@@ -339,150 +344,87 @@ int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_video
         dfb_new_size(g.sw, g.sh, new_width, new_height, new_short, &g.dw, &g.dh);
         g.resize = g.dw != g.sw || g.dh != g.sh;
         if (g.dw > r->max_w || g.dh > r->max_h) {
-            set_err("dfb_list_run_videos: video " + std::to_string(i) + " (" + std::to_string(g.dw) + "x" + std::to_string(g.dh) +
-                    " after resizing) exceeds the size given to dfb_list_open");
+            set_error(err, err_len, "dfb_list_run_videos: video " + std::to_string(i) + " (" + std::to_string(g.dw) + "x" + std::to_string(g.dh) +
+                                        " after resizing) exceeds the size given to dfb_list_open");
             return DFB_ERR_SIZE;
         }
     }
-    dfb_list_stats st{};
-    st.workers = n_workers;
-    std::atomic<long> local_next{0};
-    std::atomic<int> failed{0};
-    std::mutex mtx;
-    std::string first_error;
-    auto fail = [&](int code, const std::string &m) {
-        std::lock_guard<std::mutex> lk(mtx);
-        if (!failed.load()) {
-            failed.store(code);
-            first_error = m;
+
+    auto run_video = [&](int wi, long idx) -> ItemResult {
+        dfb_list_runner::Worker &w = r->workers[wi];
+        const dfb_video &v = videos[idx];
+        const Geometry &g = geo[idx];
+        const bool bgr = v.kind == DFB_VIDEO_BGR;
+        const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
+        // outputs: flows (:308) or, with step 0, frames; files per output and the capacity of one file
+        const int M = step != 0 ? std::max(v.n_frames - astep, 0) : v.n_frames;
+        const int per = step != 0 && save_type == DFB_SAVE_JPG ? 2 : 1;
+        const size_t cap = step == 0                     ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
+                           : save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
+                                                         : dfb_jpeg_max_bytes(g.dw, g.dh);
+        if (M > 0) {
+            try {
+                w.files.allocate((size_t)chunk_flows * per * cap);
+            } catch (const dfb::CudaError &) {
+                return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed"};
+            }
         }
+        std::vector<uint8_t *> out(2 * chunk_flows), ox(chunk_flows), oy(chunk_flows);
+        std::vector<size_t> lens(2 * chunk_flows), lx(chunk_flows), ly(chunk_flows);
+        uint8_t *ring = w.files;
+        for (int k = 0; k < per * chunk_flows && ring; ++k) out[k] = ring + (size_t)k * cap;
+        // chunks of outputs [f0, f0 + m); a flow chunk reads frames f0 .. f0 + m - 1 + |step| (see dfb_list_run)
+        int f0 = 0;
+        for (;;) {
+            const int m = std::max(std::min(chunk_flows, M - f0), 0);
+            int rc = DFB_OK;
+            if (m > 0 && step == 0) {
+                rc = bgr ? dfb_extract_frames_host(w.h, v.bgr + f0, m, g.sw, g.sh, dwa, dha, quality, out.data(), cap, lens.data())
+                         : dfb_extract_frames_jpeg_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m, dwa, dha, quality, out.data(), cap, lens.data());
+            } else if (m > 0 && save_type == DFB_SAVE_PNG) {
+                rc = bgr ? dfb_process_bgr_batch_host_png(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
+                         : dfb_process_jpeg_batch_host_png(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, out.data(), cap,
+                                                           lens.data());
+            } else if (m > 0) {
+                for (int i = 0; i < m; ++i) {
+                    ox[i] = out[2 * i];
+                    oy[i] = out[2 * i + 1];
+                }
+                rc = bgr ? dfb_process_bgr_batch_host(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, bound, quality, ox.data(), oy.data(),
+                                                      cap, lx.data(), ly.data())
+                         : dfb_process_jpeg_batch_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, bound, quality, ox.data(),
+                                                       oy.data(), cap, lx.data(), ly.data());
+                for (int i = 0; i < m; ++i) {
+                    lens[2 * i] = lx[i];
+                    lens[2 * i + 1] = ly[i];
+                }
+            }
+            if (rc != DFB_OK) return {rc, video_error(idx, f0, dfb_last_error(w.h))};
+            const int last = f0 + m >= M;
+            // every file of this chunk is in host memory now; `last` is FlowBuffer::last_buffer (see dfb_list_run)
+            if (done) done(user, (int)idx, w.device, f0, m, last, out.data(), lens.data());
+            f0 += m;
+            if (last) break;
+        }
+        return {DFB_OK, {}, step != 0 ? (uint64_t)M : 0, (uint64_t)v.n_frames};
     };
+
     // the runner owns the handles, so the call's jpeg_exact is set on each of them and restored afterwards
     std::vector<double> exact_before(n_workers, 0);
     for (int wi = 0; wi < n_workers; ++wi) {
         dfb_get_param(r->workers[wi].h, "jpeg_exact", &exact_before[wi]);
         dfb_set_param(r->workers[wi].h, "jpeg_exact", jpeg_exact);
     }
-    for (auto &w : r->workers) dfb_reset_counters(w.h);
-    const auto t_start = clk::now();
-
-    auto worker = [&](int wi) {
-        dfb_list_runner::Worker &w = r->workers[wi];
-        cudaSetDevice(w.device);
-        std::vector<uint8_t *> out(2 * chunk_flows), ox(chunk_flows), oy(chunk_flows);
-        std::vector<size_t> lens(2 * chunk_flows), lx(chunk_flows), ly(chunk_flows);
-        double busy = 0;
-        while (!failed.load()) {
-            const long idx = queue ? dfb_queue_next(queue) : local_next.fetch_add(1);
-            if (idx >= n_videos) break;
-            const dfb_video &v = videos[idx];
-            const Geometry &g = geo[idx];
-            const bool bgr = v.kind == DFB_VIDEO_BGR;
-            const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
-            const auto t0 = clk::now();
-            // outputs: flows (:308) or, with step 0, frames; files per output and the capacity of one file
-            const int M = step != 0 ? std::max(v.n_frames - astep, 0) : v.n_frames;
-            const int per = step != 0 && save_type == DFB_SAVE_JPG ? 2 : 1;
-            const size_t cap = step == 0                     ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
-                               : save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
-                                                             : dfb_jpeg_max_bytes(g.dw, g.dh);
-            const size_t need = (size_t)chunk_flows * per * cap;
-            if (M > 0 && w.files_bytes < need) {
-                if (w.files) cudaFreeHost(w.files);
-                w.files = nullptr;
-                w.files_bytes = 0;
-                if (cudaHostAlloc(&w.files, need, cudaHostAllocDefault) != cudaSuccess) {
-                    fail(DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed");
-                    break;
-                }
-                w.files_bytes = need;
-            }
-            uint8_t *ring = static_cast<uint8_t *>(w.files);
-            for (int k = 0; k < per * chunk_flows && ring; ++k) out[k] = ring + (size_t)k * cap;
-            // chunks of outputs [f0, f0 + m); a flow chunk reads frames f0 .. f0 + m - 1 + |step| (see dfb_list_run)
-            int f0 = 0;
-            for (;;) {
-                const int m = std::max(std::min(chunk_flows, M - f0), 0);
-                int rc = DFB_OK;
-                if (m > 0 && step == 0) {
-                    rc = bgr ? dfb_extract_frames_host(w.h, v.bgr + f0, m, g.sw, g.sh, dwa, dha, quality, out.data(), cap, lens.data())
-                             : dfb_extract_frames_jpeg_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m, dwa, dha, quality, out.data(), cap, lens.data());
-                } else if (m > 0 && save_type == DFB_SAVE_PNG) {
-                    rc = bgr ? dfb_process_bgr_batch_host_png(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
-                             : dfb_process_jpeg_batch_host_png(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, out.data(), cap,
-                                                               lens.data());
-                } else if (m > 0) {
-                    for (int i = 0; i < m; ++i) {
-                        ox[i] = out[2 * i];
-                        oy[i] = out[2 * i + 1];
-                    }
-                    rc = bgr ? dfb_process_bgr_batch_host(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, bound, quality, ox.data(), oy.data(),
-                                                          cap, lx.data(), ly.data())
-                             : dfb_process_jpeg_batch_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, bound, quality, ox.data(),
-                                                           oy.data(), cap, lx.data(), ly.data());
-                    for (int i = 0; i < m; ++i) {
-                        lens[2 * i] = lx[i];
-                        lens[2 * i + 1] = ly[i];
-                    }
-                }
-                if (rc != DFB_OK) {
-                    fail(rc, video_error(idx, f0, dfb_last_error(w.h)));
-                    break;
-                }
-                const int last = f0 + m >= M;
-                // every file of this chunk is in host memory now; `last` is FlowBuffer::last_buffer (see dfb_list_run)
-                if (done) done(user, (int)idx, w.device, f0, m, last, out.data(), lens.data());
-                f0 += m;
-                if (last) break;
-            }
-            if (failed.load()) break;
-            busy += seconds_since(t0);
-            std::lock_guard<std::mutex> lk(mtx);
-            ++st.clips;
-            const uint64_t flows = step != 0 ? (uint64_t)M : 0;
-            st.flows += flows;
-            st.frames += (uint64_t)v.n_frames;
-            ++st.clips_per_worker[wi];
-            st.flows_per_worker[wi] += flows;
-        }
-        std::lock_guard<std::mutex> lk(mtx);
-        st.busy_seconds_per_worker[wi] = busy;
-        st.finish_seconds_per_worker[wi] = seconds_since(t_start);
-    };
-
-    if (n_videos > 0) {
-        std::vector<std::thread> threads;
-        for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
-        worker(0);
-        for (auto &t : threads) t.join();
-    }
-    st.seconds = seconds_since(t_start);
-    for (int wi = 0; wi < n_workers; ++wi) {
-        dfb_list_runner::Worker &w = r->workers[wi];
-        dfb_set_param(w.h, "jpeg_exact", exact_before[wi]);
-        dfb_counters c{};
-        if (dfb_get_counters(w.h, &c) == DFB_OK) {
-            st.kernel_launches += c.kernel_launches;
-            st.h2d_bytes += c.h2d_bytes;
-            st.d2h_bytes += c.d2h_bytes;
-        }
-    }
-    if (stats) *stats = st;
-    if (failed.load()) {
-        set_err(first_error);
-        return failed.load();
-    }
-    return DFB_OK;
+    const int rc = run_items(r, n_videos, queue, run_video, stats, err, err_len);
+    for (int wi = 0; wi < n_workers; ++wi) dfb_set_param(r->workers[wi].h, "jpeg_exact", exact_before[wi]);
+    return rc;
 }
 
 int dfb_run_list(const char *algorithm, const int *devices, int n_workers, const dfb_clip *clips, int n_clips, int step, int bound,
                  int chunk_flows, dfb_queue *queue, dfb_chunk_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
-    auto set_err = [&](const std::string &m) {
-        if (err && err_len) std::snprintf(err, err_len, "%s", m.c_str());
-    };
     if (!algorithm || !devices || n_workers < 1 || n_workers > DFB_LIST_MAX_WORKERS || (!clips && n_clips > 0) || n_clips < 0 || step == 0 ||
         bound < 0) {
-        set_err("dfb_run_list: bad arguments (step must be non-zero: step 0 is the frame-extraction mode)");
+        set_error(err, err_len, "dfb_run_list: bad arguments (step must be non-zero: step 0 is the frame-extraction mode)");
         return DFB_ERR_INVALID_ARG;
     }
     if (n_clips == 0) {  // tools/denseflow.cpp:86: nothing is created when every video of the list is already done
