@@ -65,6 +65,8 @@ class Video(C.Structure):
 
 FILES_DONE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t))
 
+FRAMES_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Video), C.c_void_p, C.c_size_t)
+
 CHUNK_DONE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                             C.POINTER(C.c_void_p))
 
@@ -148,6 +150,8 @@ SIGNATURES = {
                                C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
     "dfb_list_close": (None, [C.c_void_p]),
     "dfb_list_run_videos": (C.c_int, [C.c_void_p, C.POINTER(Video), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
+    "dfb_list_run_stream": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
     "dfb_run_list": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.c_int, C.POINTER(Clip), C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),

@@ -10,7 +10,8 @@
 // and completion is reported per chunk with the reference's `last_buffer` meaning.
 //
 // dfb_list_run_videos runs the same dispatch over the videos as the reference takes them (colour frames or `-if` JPEG files)
-// and hands out the files the reference writes: flow JPEGs or PNGs, or with step 0 the extracted frames.
+// and hands out the files the reference writes: flow JPEGs or PNGs, or with step 0 the extracted frames.  dfb_list_run_stream
+// does the same with frames pulled from the caller one window at a time, so a list of long videos runs in bounded memory.
 //
 // This file is a client of the C ABI (dfb_create / dfb_calc_batch_host[_u8] / dfb_process_* / dfb_extract_frames_* /
 // dfb_destroy): it adds no arithmetic.
@@ -95,8 +96,10 @@ struct dfb_list_runner {
     struct Worker {
         int device = 0;
         dfb_handle *h = nullptr;
+        int max_w = 0, max_h = 0;           // the frame size h was created for (dfb_list_run_stream grows it)
+        dfb_counters retired{};             // counters of the handles this worker replaced during the current run
         dfb::PinnedBuffer<uint8_t> pinned;  // output ring of one chunk: the copy engines write the results straight into it
-        dfb::PinnedBuffer<uint8_t> files;   // file ring of one chunk of dfb_list_run_videos
+        dfb::PinnedBuffer<uint8_t> files;   // file ring of one chunk of dfb_list_run_videos / dfb_list_run_stream
     };
     std::vector<Worker> workers;
 };
@@ -117,6 +120,8 @@ int dfb_list_open(const char *algorithm, const int *devices, int n_workers, int 
     for (int wi = 0; wi < n_workers; ++wi) {
         dfb_list_runner::Worker &w = r->workers[wi];
         w.device = devices[wi];
+        w.max_w = max_width;
+        w.max_h = max_height;
         if (int rc = dfb_create(algorithm, w.device, max_width, max_height, &w.h)) {
             set_error(err, err_len, "worker " + std::to_string(wi) + ": " + dfb_last_error(nullptr));
             dfb_list_close(r);
@@ -157,7 +162,10 @@ int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, df
     std::atomic<int> failed{0};
     std::mutex mtx;
     std::string first_error;
-    for (auto &w : r->workers) dfb_reset_counters(w.h);
+    for (auto &w : r->workers) {
+        dfb_reset_counters(w.h);
+        w.retired = dfb_counters{};
+    }
     const auto t_start = clk::now();
 
     auto worker = [&](int wi) {
@@ -204,6 +212,9 @@ int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, df
             st.h2d_bytes += c.h2d_bytes;
             st.d2h_bytes += c.d2h_bytes;
         }
+        st.kernel_launches += w.retired.kernel_launches;
+        st.h2d_bytes += w.retired.h2d_bytes;
+        st.d2h_bytes += w.retired.d2h_bytes;
     }
     if (stats) *stats = st;
     if (failed.load()) {
@@ -220,6 +231,191 @@ std::string video_error(long k, int f0, const char *msg) {
     if (std::sscanf(m.c_str(), "frame %d: %n", &i, &n) == 1 && n > 0)
         return "video " + std::to_string(k) + ": frame " + std::to_string(f0 + i) + ": " + m.substr(n);
     return "video " + std::to_string(k) + ": " + m;
+}
+
+// The arguments of dfb_list_run_videos and dfb_list_run_stream that every video of the call shares.
+struct VideoArgs {
+    int step = 1, astep = 1, bound = 0, save_type = DFB_SAVE_JPG, quality = 95, new_width = 0, new_height = 0, new_short = 0;
+    int chunk_flows = 64;
+    dfb_files_done_fn done = nullptr;
+    void *user = nullptr;
+};
+
+// The checks both video entry points make first (`name` leads the message of a malformed call), in this order: the call,
+// check_param's bound (src/denseflow_gpu.cpp:23-35: the bound matters only to the flow modes), the quality, the -nw/-nh/-ns
+// rule.  Fills a, or writes the message and returns the code.
+int check_video_args(const char *name, int step, int bound, int save_type, int quality, int jpeg_exact, int new_width, int new_height,
+                     int new_short, int chunk_flows, VideoArgs &a, char *err, size_t err_len) {
+    if ((save_type != DFB_SAVE_JPG && save_type != DFB_SAVE_PNG) || (jpeg_exact != 0 && jpeg_exact != 1)) {
+        set_error(err, err_len, std::string(name) + ": bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
+        return DFB_ERR_INVALID_ARG;
+    }
+    if (step != 0 && bound <= 0) {
+        set_error(err, err_len, "bound should > 0!");
+        return DFB_ERR_INVALID_ARG;
+    }
+    const bool writes_jpeg = step == 0 || save_type == DFB_SAVE_JPG;
+    if (writes_jpeg && (quality < 1 || quality > 100)) {
+        set_error(err, err_len, std::string(name) + ": quality must be in 1..100");
+        return DFB_ERR_INVALID_ARG;
+    }
+    int dw = 0, dh = 0;
+    if (int rc = dfb_new_size(1, 1, new_width, new_height, new_short, &dw, &dh)) {
+        set_error(err, err_len, dfb_last_error(nullptr));
+        return rc;
+    }
+    a.step = step;
+    a.astep = std::abs(step);
+    a.bound = bound;
+    a.save_type = save_type;
+    a.quality = quality;
+    a.new_width = new_width;
+    a.new_height = new_height;
+    a.new_short = new_short;
+    a.chunk_flows = chunk_flows > 0 ? chunk_flows : 64;
+    return DFB_OK;
+}
+
+bool malformed(const dfb_video &v) {
+    const bool bgr = v.kind == DFB_VIDEO_BGR;
+    return (!bgr && v.kind != DFB_VIDEO_JPEG) || v.n_frames < 0 || (v.n_frames > 0 && (bgr ? !v.bgr : (!v.jpeg || !v.jpeg_len))) ||
+           (bgr && (v.width <= 0 || v.height <= 0));
+}
+
+// A video's source and destination size.
+struct Geometry {
+    int sw = 0, sh = 0, dw = 0, dh = 0;
+    bool resize = false;
+};
+
+// get_new_size (src/denseflow_gpu.cpp:44-80) reads frame 0: a BGR video gives its size, a JPEG file the size in its markers.
+// v holds at least one frame, frame 0 at index `off`.
+int size_video(const dfb_video &v, int off, const VideoArgs &a, Geometry &g) {
+    if (v.kind == DFB_VIDEO_BGR) {
+        g.sw = v.width;
+        g.sh = v.height;
+    } else if (int rc = dfb_jpeg_info(v.jpeg[off], v.jpeg_len[off], &g.sw, &g.sh)) {
+        return rc;
+    }
+    dfb_new_size(g.sw, g.sh, a.new_width, a.new_height, a.new_short, &g.dw, &g.dh);
+    g.resize = g.dw != g.sw || g.dh != g.sh;
+    return DFB_OK;
+}
+
+// Frames first .. first + n - 1 of a video: frame first + i is v->bgr[off + i] or v->jpeg[off + i].  `ends`: no frame follows.
+struct Window {
+    const dfb_video *v = nullptr;
+    int off = 0, n = 0;
+    bool ends = false;
+};
+
+// One video through the chains, one window at a time.  fetch(first, max_n, win) returns an ItemResult and fills win with
+// frames first .. first + max_n - 1, fewer when the video ends there; g is the video's geometry by the time the first window
+// with a frame is fetched.  A window serves up to chunk_flows outputs: flows [f0, f0 + m) read frames f0 .. f0 + m - 1 +
+// |step|, so consecutive windows overlap by |step| frames (the overlap the reference keeps between its own <= 512-frame
+// batches, src/denseflow_gpu.cpp:182-189,204-205) and indices stay global (FlowBuffer::base_start).  With step 0 every frame
+// is an output.
+template <typename Fetch>
+ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoArgs &a, const Geometry &g, Fetch &&fetch) {
+    const bool flow = a.step != 0;
+    const int per = flow && a.save_type == DFB_SAVE_JPG ? 2 : 1;
+    const int chunk = a.chunk_flows;
+    std::vector<uint8_t *> out(2 * chunk), ox(chunk), oy(chunk);
+    std::vector<size_t> lens(2 * chunk), lx(chunk), ly(chunk);
+    uint64_t outputs = 0;
+    int f0 = 0;
+    for (;;) {
+        Window win;
+        ItemResult fr = fetch(f0, chunk + a.astep, win);
+        if (fr.rc != DFB_OK) return fr;
+        const int m = flow ? std::max(win.n - a.astep, 0) : win.n;
+        int rc = DFB_OK;
+        if (m > 0) {
+            const dfb_video &v = *win.v;
+            const bool bgr = v.kind == DFB_VIDEO_BGR;
+            const uint8_t *const *bf = bgr ? v.bgr + win.off : nullptr;
+            const uint8_t *const *jf = bgr ? nullptr : v.jpeg + win.off;
+            const size_t *jl = bgr ? nullptr : v.jpeg_len + win.off;
+            const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
+            const size_t cap = !flow                         ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
+                               : a.save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
+                                                             : dfb_jpeg_max_bytes(g.dw, g.dh);
+            try {
+                w.files.allocate((size_t)chunk * per * cap);
+            } catch (const dfb::CudaError &) {
+                return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed"};
+            }
+            for (int k = 0; k < per * chunk; ++k) out[k] = (uint8_t *)w.files + (size_t)k * cap;
+            if (!flow) {
+                rc = bgr ? dfb_extract_frames_host(w.h, bf, m, g.sw, g.sh, dwa, dha, a.quality, out.data(), cap, lens.data())
+                         : dfb_extract_frames_jpeg_host(w.h, jf, jl, m, dwa, dha, a.quality, out.data(), cap, lens.data());
+            } else if (a.save_type == DFB_SAVE_PNG) {
+                rc = bgr ? dfb_process_bgr_batch_host_png(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
+                         : dfb_process_jpeg_batch_host_png(w.h, jf, jl, m + a.astep, a.step, dwa, dha, out.data(), cap, lens.data());
+            } else {
+                for (int i = 0; i < m; ++i) {
+                    ox[i] = out[2 * i];
+                    oy[i] = out[2 * i + 1];
+                }
+                rc = bgr ? dfb_process_bgr_batch_host(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, a.bound, a.quality, ox.data(),
+                                                      oy.data(), cap, lx.data(), ly.data())
+                         : dfb_process_jpeg_batch_host(w.h, jf, jl, m + a.astep, a.step, dwa, dha, a.bound, a.quality, ox.data(), oy.data(),
+                                                       cap, lx.data(), ly.data());
+                for (int i = 0; i < m; ++i) {
+                    lens[2 * i] = lx[i];
+                    lens[2 * i + 1] = ly[i];
+                }
+            }
+        }
+        if (rc != DFB_OK) return {rc, video_error(idx, f0, dfb_last_error(w.h))};
+        // every file of this chunk is in host memory now; win.ends makes it FlowBuffer::last_buffer (see dfb_list_run)
+        if (a.done) a.done(a.user, (int)idx, w.device, f0, m, win.ends, out.data(), lens.data());
+        outputs += m;
+        if (win.ends) return {DFB_OK, {}, flow ? outputs : 0, (uint64_t)f0 + win.n};
+        f0 += m;
+    }
+}
+
+// run_items over videos with the call's jpeg_exact: the runner owns the handles, so it is set on each of them and restored
+// afterwards.
+template <typename Body>
+int run_videos_with(dfb_list_runner *r, int n_videos, dfb_queue *queue, int jpeg_exact, Body &&body, dfb_list_stats *stats, char *err,
+                    size_t err_len) {
+    const int n_workers = (int)r->workers.size();
+    std::vector<double> exact_before(n_workers, 0);
+    for (int wi = 0; wi < n_workers; ++wi) {
+        dfb_get_param(r->workers[wi].h, "jpeg_exact", &exact_before[wi]);
+        dfb_set_param(r->workers[wi].h, "jpeg_exact", jpeg_exact);
+    }
+    const int rc = run_items(r, n_videos, queue, body, stats, err, err_len);
+    for (int wi = 0; wi < n_workers; ++wi) dfb_set_param(r->workers[wi].h, "jpeg_exact", exact_before[wi]);
+    return rc;
+}
+
+// Worker w's handle for destination frames of dw x dh: a smaller handle is replaced by one at least that large in both
+// dimensions, with the old one's jpeg_exact.  Its counters stay in the run's stats.  On failure the old handle stays.
+int fit_worker(dfb_list_runner *r, dfb_list_runner::Worker &w, int dw, int dh, std::string &error) {
+    if (dw <= w.max_w && dh <= w.max_h) return DFB_OK;
+    const int mw = std::max(w.max_w, dw), mh = std::max(w.max_h, dh);
+    dfb_handle *h = nullptr;
+    if (int rc = dfb_create(r->algorithm.c_str(), w.device, mw, mh, &h)) {
+        error = dfb_last_error(nullptr);
+        return rc;
+    }
+    double exact = 0;
+    dfb_get_param(w.h, "jpeg_exact", &exact);
+    dfb_set_param(h, "jpeg_exact", exact);
+    dfb_counters c{};
+    if (dfb_get_counters(w.h, &c) == DFB_OK) {
+        w.retired.kernel_launches += c.kernel_launches;
+        w.retired.h2d_bytes += c.h2d_bytes;
+        w.retired.d2h_bytes += c.d2h_bytes;
+    }
+    dfb_destroy(w.h);
+    w.h = h;
+    w.max_w = mw;
+    w.max_h = mh;
+    return DFB_OK;
 }
 
 }  // namespace
@@ -292,132 +488,97 @@ int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int ste
 int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_videos, int step, int bound, int save_type, int quality,
                         int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
                         dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
-    if (!r || (!videos && n_videos > 0) || n_videos < 0 || (save_type != DFB_SAVE_JPG && save_type != DFB_SAVE_PNG) ||
-        (jpeg_exact != 0 && jpeg_exact != 1)) {
+    if (!r || (!videos && n_videos > 0) || n_videos < 0) {
         set_error(err, err_len, "dfb_list_run_videos: bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
         return DFB_ERR_INVALID_ARG;
     }
-    // check_param (src/denseflow_gpu.cpp:23-35): the bound matters only to the flow modes
-    if (step != 0 && bound <= 0) {
-        set_error(err, err_len, "bound should > 0!");
-        return DFB_ERR_INVALID_ARG;
-    }
-    const bool writes_jpeg = step == 0 || save_type == DFB_SAVE_JPG;
-    if (writes_jpeg && (quality < 1 || quality > 100)) {
-        set_error(err, err_len, "dfb_list_run_videos: quality must be in 1..100");
-        return DFB_ERR_INVALID_ARG;
-    }
-    int dw = 0, dh = 0;
-    if (int rc = dfb_new_size(1, 1, new_width, new_height, new_short, &dw, &dh)) {
-        set_error(err, err_len, dfb_last_error(nullptr));
+    VideoArgs a;
+    if (int rc = check_video_args("dfb_list_run_videos", step, bound, save_type, quality, jpeg_exact, new_width, new_height, new_short,
+                                  chunk_flows, a, err, err_len))
         return rc;
-    }
-    if (chunk_flows <= 0) chunk_flows = 64;
-    const int astep = std::abs(step);
-    const int n_workers = (int)r->workers.size();
-    // every video's source and destination size, before any work: get_new_size reads frame 0 (:48-52)
-    struct Geometry {
-        int sw = 0, sh = 0, dw = 0, dh = 0;
-        bool resize = false;
-    };
+    a.done = done;
+    a.user = user;
+    // every video's source and destination size, before any work
     std::vector<Geometry> geo(n_videos);
     for (int i = 0; i < n_videos; ++i) {
         const dfb_video &v = videos[i];
-        const bool bgr = v.kind == DFB_VIDEO_BGR;
-        if ((!bgr && v.kind != DFB_VIDEO_JPEG) || v.n_frames < 0 || (v.n_frames > 0 && (bgr ? !v.bgr : (!v.jpeg || !v.jpeg_len))) ||
-            (bgr && (v.width <= 0 || v.height <= 0))) {
+        if (malformed(v)) {
             set_error(err, err_len, "dfb_list_run_videos: video " + std::to_string(i) + " is malformed");
             return DFB_ERR_INVALID_ARG;
         }
+        if (v.kind == DFB_VIDEO_JPEG && v.n_frames == 0) continue;  // an empty frame folder: nothing to size
         Geometry &g = geo[i];
-        if (bgr) {
-            g.sw = v.width;
-            g.sh = v.height;
-        } else if (v.n_frames > 0) {
-            if (int rc = dfb_jpeg_info(v.jpeg[0], v.jpeg_len[0], &g.sw, &g.sh)) {
-                set_error(err, err_len, "video " + std::to_string(i) + ": " + dfb_last_error(nullptr));
-                return rc;
-            }
-        } else {
-            continue;  // an empty frame folder: nothing to size
+        if (int rc = size_video(v, 0, a, g)) {
+            set_error(err, err_len, "video " + std::to_string(i) + ": " + dfb_last_error(nullptr));
+            return rc;
         }
-        dfb_new_size(g.sw, g.sh, new_width, new_height, new_short, &g.dw, &g.dh);
-        g.resize = g.dw != g.sw || g.dh != g.sh;
         if (g.dw > r->max_w || g.dh > r->max_h) {
             set_error(err, err_len, "dfb_list_run_videos: video " + std::to_string(i) + " (" + std::to_string(g.dw) + "x" + std::to_string(g.dh) +
                                         " after resizing) exceeds the size given to dfb_list_open");
             return DFB_ERR_SIZE;
         }
     }
-
-    auto run_video = [&](int wi, long idx) -> ItemResult {
-        dfb_list_runner::Worker &w = r->workers[wi];
+    auto body = [&](int wi, long idx) -> ItemResult {
         const dfb_video &v = videos[idx];
-        const Geometry &g = geo[idx];
-        const bool bgr = v.kind == DFB_VIDEO_BGR;
-        const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
-        // outputs: flows (:308) or, with step 0, frames; files per output and the capacity of one file
-        const int M = step != 0 ? std::max(v.n_frames - astep, 0) : v.n_frames;
-        const int per = step != 0 && save_type == DFB_SAVE_JPG ? 2 : 1;
-        const size_t cap = step == 0                     ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
-                           : save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
-                                                         : dfb_jpeg_max_bytes(g.dw, g.dh);
-        if (M > 0) {
-            try {
-                w.files.allocate((size_t)chunk_flows * per * cap);
-            } catch (const dfb::CudaError &) {
-                return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed"};
-            }
-        }
-        std::vector<uint8_t *> out(2 * chunk_flows), ox(chunk_flows), oy(chunk_flows);
-        std::vector<size_t> lens(2 * chunk_flows), lx(chunk_flows), ly(chunk_flows);
-        uint8_t *ring = w.files;
-        for (int k = 0; k < per * chunk_flows && ring; ++k) out[k] = ring + (size_t)k * cap;
-        // chunks of outputs [f0, f0 + m); a flow chunk reads frames f0 .. f0 + m - 1 + |step| (see dfb_list_run)
-        int f0 = 0;
-        for (;;) {
-            const int m = std::max(std::min(chunk_flows, M - f0), 0);
-            int rc = DFB_OK;
-            if (m > 0 && step == 0) {
-                rc = bgr ? dfb_extract_frames_host(w.h, v.bgr + f0, m, g.sw, g.sh, dwa, dha, quality, out.data(), cap, lens.data())
-                         : dfb_extract_frames_jpeg_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m, dwa, dha, quality, out.data(), cap, lens.data());
-            } else if (m > 0 && save_type == DFB_SAVE_PNG) {
-                rc = bgr ? dfb_process_bgr_batch_host_png(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
-                         : dfb_process_jpeg_batch_host_png(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, out.data(), cap,
-                                                           lens.data());
-            } else if (m > 0) {
-                for (int i = 0; i < m; ++i) {
-                    ox[i] = out[2 * i];
-                    oy[i] = out[2 * i + 1];
-                }
-                rc = bgr ? dfb_process_bgr_batch_host(w.h, v.bgr + f0, m + astep, step, g.sw, g.sh, dwa, dha, bound, quality, ox.data(), oy.data(),
-                                                      cap, lx.data(), ly.data())
-                         : dfb_process_jpeg_batch_host(w.h, v.jpeg + f0, v.jpeg_len + f0, m + astep, step, dwa, dha, bound, quality, ox.data(),
-                                                       oy.data(), cap, lx.data(), ly.data());
-                for (int i = 0; i < m; ++i) {
-                    lens[2 * i] = lx[i];
-                    lens[2 * i + 1] = ly[i];
-                }
-            }
-            if (rc != DFB_OK) return {rc, video_error(idx, f0, dfb_last_error(w.h))};
-            const int last = f0 + m >= M;
-            // every file of this chunk is in host memory now; `last` is FlowBuffer::last_buffer (see dfb_list_run)
-            if (done) done(user, (int)idx, w.device, f0, m, last, out.data(), lens.data());
-            f0 += m;
-            if (last) break;
-        }
-        return {DFB_OK, {}, step != 0 ? (uint64_t)M : 0, (uint64_t)v.n_frames};
+        auto fetch = [&](int first, int max_n, Window &win) -> ItemResult {
+            win.v = &v;
+            win.off = first;
+            win.n = std::max(std::min(max_n, v.n_frames - first), 0);
+            win.ends = first + win.n >= v.n_frames;
+            return {};
+        };
+        return run_video(r->workers[wi], wi, idx, a, geo[idx], fetch);
     };
+    return run_videos_with(r, n_videos, queue, jpeg_exact, body, stats, err, err_len);
+}
 
-    // the runner owns the handles, so the call's jpeg_exact is set on each of them and restored afterwards
-    std::vector<double> exact_before(n_workers, 0);
-    for (int wi = 0; wi < n_workers; ++wi) {
-        dfb_get_param(r->workers[wi].h, "jpeg_exact", &exact_before[wi]);
-        dfb_set_param(r->workers[wi].h, "jpeg_exact", jpeg_exact);
+int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, int step, int bound, int save_type, int quality,
+                        int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
+                        dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
+    if (!r || !source || n_videos < 0) {
+        set_error(err, err_len, "dfb_list_run_stream: bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
+        return DFB_ERR_INVALID_ARG;
     }
-    const int rc = run_items(r, n_videos, queue, run_video, stats, err, err_len);
-    for (int wi = 0; wi < n_workers; ++wi) dfb_set_param(r->workers[wi].h, "jpeg_exact", exact_before[wi]);
-    return rc;
+    VideoArgs a;
+    if (int rc = check_video_args("dfb_list_run_stream", step, bound, save_type, quality, jpeg_exact, new_width, new_height, new_short,
+                                  chunk_flows, a, err, err_len))
+        return rc;
+    a.done = done;
+    a.user = user;
+    auto body = [&](int wi, long idx) -> ItemResult {
+        dfb_list_runner::Worker &w = r->workers[wi];
+        const std::string k = "video " + std::to_string(idx) + ": ";
+        Geometry g;
+        dfb_video cur{};  // the source's latest window
+        // the video is sized by its first window with a frame, which also fits the worker's handle to it; every later
+        // frame must have frame 0's size
+        auto fetch = [&](int first, int max_n, Window &win) -> ItemResult {
+            cur = dfb_video{};
+            char msg[512] = "";
+            if (source(user, (int)idx, first, max_n, &cur, msg, sizeof msg) != 0) return {DFB_ERR_INVALID_ARG, k + msg};
+            if (malformed(cur) || cur.n_frames > max_n)
+                return {DFB_ERR_INVALID_ARG, k + "the source returned a malformed window at frame " + std::to_string(first)};
+            win = {&cur, 0, cur.n_frames, cur.n_frames < max_n};
+            if (cur.n_frames == 0) return {};
+            if (first == 0) {
+                if (int rc = size_video(cur, 0, a, g)) return {rc, k + dfb_last_error(nullptr)};
+                std::string e;
+                if (int rc = fit_worker(r, w, g.dw, g.dh, e)) return {rc, k + e};
+            }
+            // a BGR window has one size; a JPEG file that cannot be sized is left to the decoder, which names the fault
+            const int n_check = cur.kind == DFB_VIDEO_BGR ? 1 : cur.n_frames;
+            for (int i = 0; i < n_check; ++i) {
+                int fw = cur.width, fh = cur.height;
+                if (cur.kind == DFB_VIDEO_JPEG && dfb_jpeg_info(cur.jpeg[i], cur.jpeg_len[i], &fw, &fh) != DFB_OK) continue;
+                if (fw != g.sw || fh != g.sh)
+                    return {DFB_ERR_SIZE, k + "frame " + std::to_string(first + i) + ": " + std::to_string(fw) + "x" + std::to_string(fh) +
+                                              ", frame 0 is " + std::to_string(g.sw) + "x" + std::to_string(g.sh)};
+            }
+            return {};
+        };
+        return run_video(w, wi, idx, a, g, fetch);
+    };
+    return run_videos_with(r, n_videos, queue, jpeg_exact, body, stats, err, err_len);
 }
 
 int dfb_run_list(const char *algorithm, const int *devices, int n_workers, const dfb_clip *clips, int n_clips, int step, int bound,

@@ -54,26 +54,35 @@ def _pack_clips(clips):
     return arr, shapes, keep
 
 
+def _pack_video(frames):
+    """One video as a dfb_video, and what keeps its memory alive (the structure holds its pointer tables)."""
+    v = _lib.Video()
+    v.n_frames = len(frames)
+    if frames and isinstance(frames[0], (bytes, bytearray, memoryview)):
+        bufs = [np.frombuffer(f, np.uint8) for f in frames]
+        v.kind = _lib.VIDEO_JPEG
+        v.jpeg = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
+        v.jpeg_len = (C.c_size_t * len(bufs))(*[b.size for b in bufs])
+        return v, (v, bufs)
+    fr = [np.ascontiguousarray(f) for f in frames]
+    if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != fr[0].shape for f in fr):
+        raise RuntimeError("frames must be uint8 [H,W,3] BGR images of one size, or JPEG files (bytes)")
+    v.kind = _lib.VIDEO_BGR
+    v.bgr = (C.c_void_p * max(len(fr), 1))(*[f.ctypes.data for f in fr])
+    v.height, v.width = fr[0].shape[:2] if fr else (1, 1)
+    return v, (v, fr)
+
+
 def _pack_videos(videos):
     keep = []
     arr = (_lib.Video * max(len(videos), 1))()
     for i, frames in enumerate(videos):
-        v = arr[i]
-        v.n_frames = len(frames)
-        if frames and isinstance(frames[0], (bytes, bytearray, memoryview)):
-            bufs = [np.frombuffer(f, np.uint8) for f in frames]
-            v.kind = _lib.VIDEO_JPEG
-            v.jpeg = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
-            v.jpeg_len = (C.c_size_t * len(bufs))(*[b.size for b in bufs])
-            keep.append((bufs, v.jpeg, v.jpeg_len))
-            continue
-        fr = [np.ascontiguousarray(f) for f in frames]
-        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != fr[0].shape for f in fr):
-            raise RuntimeError("video %d: frames must be uint8 [H,W,3] BGR images of one size, or JPEG files (bytes)" % i)
-        v.kind = _lib.VIDEO_BGR
-        v.bgr = (C.c_void_p * max(len(fr), 1))(*[f.ctypes.data for f in fr])
-        v.height, v.width = fr[0].shape[:2] if fr else (1, 1)
-        keep.append((fr, v.bgr))
+        try:
+            v, k = _pack_video(frames)
+        except RuntimeError as ex:
+            raise RuntimeError("video %d: %s" % (i, ex)) from None
+        arr[i] = v
+        keep.append(k)
     return arr, keep
 
 
@@ -172,6 +181,59 @@ class ListRunner:
                                          err, 512)
         if rc != _lib.DFB_OK:
             raise RuntimeError(err.value.decode() or "dfb_list_run_videos failed (%d)" % rc)
+        return _stats(st)
+
+    def run_stream(self, n_videos, source, on_chunk=None, step=1, bound=20, save_type="jpg", quality=95, jpeg_exact=0, new_width=0,
+                   new_height=0, new_short=0, chunk_flows=0, queue=None):
+        """run_videos with the frames pulled from `source` one window at a time (dfb_list_run_stream), so a list of long videos
+        runs in bounded memory.  source(video, first, max_n) returns frames first .. first + max_n - 1 of the video, fewer when
+        the video ends there, as uint8 [H,W,3] BGR frames or JPEG files (bytes).  It runs on the worker's thread, in frame order
+        for each video; consecutive windows overlap by |step| frames.  A window is kept alive until the next call for its
+        video, or until the video's last chunk.  An exception in source ends the run with "video k: <message>"; one in
+        on_chunk ends it too and is raised again here.  on_chunk and the result are those of run_videos, except that a video
+        whose outputs end on a window boundary gets one more on_chunk call with no files and last_chunk True."""
+        if save_type not in ("jpg", "png"):
+            raise RuntimeError("only jpg/png are supported (no %s) for output" % save_type)
+        per = 2 if step != 0 and save_type == "jpg" else 1
+        windows = {}  # video -> the latest window and the memory behind it
+        failures = []
+
+        def _source(user, video, first, max_n, out, msg, msg_len):
+            windows.pop(video, None)  # the worker is done with the previous window
+            try:
+                if failures:
+                    raise RuntimeError("stopped after an on_chunk call failed")
+                v, keep = _pack_video(list(source(video, first, max_n)))
+            except Exception as ex:
+                text = (str(ex) or type(ex).__name__).encode()[:msg_len - 1]
+                C.memmove(msg, text + b"\0", len(text) + 1)
+                return 1
+            out[0] = v
+            windows[video] = keep
+            return 0
+
+        def _done(user, video, dev, first, n, last, files, lens):
+            try:
+                if on_chunk is not None and not failures:
+                    on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
+            except BaseException as ex:
+                failures.append(ex)
+            if last:
+                windows.pop(video, None)
+
+        src = _lib.FRAMES_FN(_source)
+        cb = _lib.FILES_DONE_FN(_done)
+        st = _lib.ListStats()
+        err = C.create_string_buffer(512)
+        rc = self._L.dfb_list_run_stream(self._r, int(n_videos), C.cast(src, C.c_void_p), int(step), int(bound),
+                                         _lib.SAVE_PNG if save_type == "png" else _lib.SAVE_JPG, int(quality), int(jpeg_exact),
+                                         int(new_width), int(new_height), int(new_short), int(chunk_flows),
+                                         queue._q if queue is not None else None, C.cast(cb, C.c_void_p), None, C.byref(st), err, 512)
+        windows.clear()
+        if failures:
+            raise failures[0]
+        if rc != _lib.DFB_OK:
+            raise RuntimeError(err.value.decode() or "dfb_list_run_stream failed (%d)" % rc)
         return _stats(st)
 
     @staticmethod

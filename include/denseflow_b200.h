@@ -509,6 +509,30 @@ int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_video
                         int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
                         dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len);
 
+/*
+ * ---- the same list with frames pulled from the caller, one window at a time -------------------------------------------
+ * dfb_list_run_stream is dfb_list_run_videos for videos the caller decodes while the list runs (a 10-minute 1080p video is
+ * ~110 GB of BGR frames): only n_videos is known up front.  The worker that takes video k calls
+ *   source(user, k, first, max_n, out, msg, msg_len)
+ * for frames first .. first + max_n - 1 and runs them through the same chains.  The source fills *out (kind, n_frames, bgr +
+ * width / height, or jpeg + jpeg_len); n_frames < max_n means the video ends there.  The pointers stay valid until the next
+ * call for this video, or until the video's last `done` call returns.  A nonzero return fails the run with "video k: <msg>".
+ *   - max_n is at most chunk_flows + |step| (chunk_flows with step 0); consecutive windows overlap by |step| frames, the
+ *     overlap the reference keeps between its batches.  The calls for one video come in order from the worker that owns it.
+ *   - The video's size comes from its first window (BGR width / height, or dfb_jpeg_info of JPEG 0); a later frame of another
+ *     size fails the run with "video k: frame f: ...".
+ *   - A worker whose handle is smaller than a video's destination size replaces it with a large enough one (keeping the call's
+ *     jpeg_exact), so max_width / max_height of dfb_list_open are only a starting size here.
+ *   - For the same frames, the files and `done` calls equal dfb_list_run_videos', except that a video whose outputs end on a
+ *     window boundary gets one more `done` call with n = 0 and last_chunk = 1.  last_chunk still comes once per video, after
+ *     all its files.
+ *   - A source error, or a refused or corrupt JPEG, ends the run; the runner stays usable.
+ */
+typedef int (*dfb_frames_fn)(void *user, int video, int first, int max_n, dfb_video *out, char *msg, size_t msg_len);
+int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, int step, int bound, int save_type, int quality,
+                        int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
+                        dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len);
+
 #ifdef __cplusplus
 }
 #endif
