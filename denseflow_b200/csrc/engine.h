@@ -5,6 +5,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdint>
 #include <memory>
 #include <string>
@@ -18,6 +19,11 @@ namespace dfb {
 struct LevelGeom {
     int w, h, pitch;
 };
+
+// set_param's value checks.  NaN fails every comparison and an infinity fails the range, so neither passes; a value that
+// passes converts to int without loss.
+inline bool whole_in(double v, double lo, double hi) { return v >= lo && v <= hi && v == std::floor(v); }
+inline bool is_flag(double v) { return v == 0 || v == 1; }
 
 // Algorithm back-end working on device buffers. One frame "slot" holds everything that depends on
 // a single frame (its fp32 pyramid), so a frame shared by two consecutive pairs is prepared once.

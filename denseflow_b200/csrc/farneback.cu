@@ -9,6 +9,7 @@
 // R / M are stored as five separate planes of one pitch (the reference stacks them in a 5H x W matrix).
 // These kernels are HBM-bound 2-D stencils: separable passes staged through shared-memory tiles,
 // float4 on the interior, index-clamp / reflect-101 border rules applied on image coordinates.
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -868,13 +869,14 @@ class Farneback final : public FlowAlgorithm {
         }
     }
     bool set_param(const std::string &k, double v) override {
-        if (k == "num_levels") { if (v < 0 || v > 5) return false; prm_.num_levels = (int)v; }
-        else if (k == "num_iters") { if (v < 1) return false; prm_.num_iters = (int)v; }
-        else if (k == "poly_sigma") prm_.poly_sigma = v;
+        // a refused value leaves the parameter as it was
+        if (k == "num_levels") { if (!whole_in(v, 0, 5)) return false; prm_.num_levels = (int)v; }
+        else if (k == "num_iters") { if (!whole_in(v, 1, INT_MAX)) return false; prm_.num_iters = (int)v; }
+        else if (k == "poly_sigma") { if (!(std::isfinite(v) && v > 0)) return false; prm_.poly_sigma = v; }
         else if (k == "pyr_scale") return v == 0.5;  // level geometry and the slot layout assume the default
         else if (k == "win_size" || k == "poly_n") return (k == "win_size" ? v == 13 : v == 5);  // compiled-in stencils
-        else if (k == "time_kernels") time_kernels_ = v != 0;
-        else if (k == "use_tma") use_tma_ = v != 0;
+        else if (k == "time_kernels") { if (!is_flag(v)) return false; time_kernels_ = v != 0; }
+        else if (k == "use_tma") { if (!is_flag(v)) return false; use_tma_ = v != 0; }
         else return false;
         return true;
     }

@@ -10,6 +10,7 @@
 //   fused = 0            one kernel per half-step, the reference's launch structure, with the A.4
 //                        state machine on the host (one stream sync per convergence check).
 #include <cfloat>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -23,6 +24,7 @@ namespace dfb {
 namespace {
 
 constexpr int kMaxScales = 16;
+constexpr int kMaxWarps = 16;  // the iteration log holds kMaxScales x kMaxWarps entries per pair
 constexpr double kAllocScaleStep = 0.8;  // scaleStep the slot / lane pyramid layout is sized for (the create() default)
 
 struct Tvl1Params {
@@ -85,27 +87,29 @@ class Tvl1 final : public FlowAlgorithm {
         }
     }
 
+    // A refused value leaves the parameter as it was.  tau and theta must be positive: the dual step's 1 + taut * |grad u|
+    // >= 1 and the primal clamp's l_t >= 0 rely on it (tvl1_math.cuh).
     bool set_param(const std::string &k, double v) override {
-        if (k == "tau") prm_.tau = v;
-        else if (k == "lambda") prm_.lambda = v;
-        else if (k == "theta") prm_.theta = v;
-        else if (k == "nscales") { if (v < 1 || v > kMaxScales) return false; prm_.nscales = (int)v; }
-        else if (k == "warps") { if (v < 1 || v > 16) return false; prm_.warps = (int)v; }
-        else if (k == "epsilon") prm_.epsilon = v;
-        else if (k == "iterations") { if (v < 1) return false; prm_.iterations = (int)v; }
+        if (k == "tau") { if (!(std::isfinite(v) && v > 0)) return false; prm_.tau = v; }
+        else if (k == "lambda") { if (!(std::isfinite(v) && v >= 0)) return false; prm_.lambda = v; }
+        else if (k == "theta") { if (!(std::isfinite(v) && v > 0)) return false; prm_.theta = v; }
+        else if (k == "nscales") { if (!whole_in(v, 1, kMaxScales)) return false; prm_.nscales = (int)v; }
+        else if (k == "warps") { if (!whole_in(v, 1, kMaxWarps)) return false; prm_.warps = (int)v; }
+        else if (k == "epsilon") { if (!std::isfinite(v)) return false; prm_.epsilon = v; }  // <= 0: no convergence checks
+        else if (k == "iterations") { if (!whole_in(v, 1, INT_MAX)) return false; prm_.iterations = (int)v; }
         else if (k == "scale_step") {
             // the pyramid slots were laid out at create time for the default 0.8: a larger factor would not fit them
             if (!(v > 0 && v <= kAllocScaleStep)) return false;
             prm_.scale_step = v;
         }
-        else if (k == "fused") prm_.fused = v != 0;
-        else if (k == "fused_k") { if (v < 1 || v > kFusedMaxK || 2 * v >= kFusedTileH) return false; prm_.fused_k = (int)v; }
-        else if (k == "flag_sync") prm_.flag_sync = (int)v;  // 0 CTA barriers, 1 spin on neighbour flags, n > 1: spin with n ns back-off
-        else if (k == "time_kernels") prm_.time_kernels = v != 0;
-        else if (k == "use_tma") prm_.use_tma = v != 0;
-        else if (k == "prefetch") prm_.prefetch = v != 0;
-        else if (k == "serial_launches") prm_.serial_launches = v != 0;
-        else if (k == "lanes") { if (v < 0 || v > kFusedMaxLanes) return false; prm_.lanes = (int)v; }
+        else if (k == "fused") { if (!is_flag(v)) return false; prm_.fused = (int)v; }
+        else if (k == "fused_k") { if (!whole_in(v, 1, kFusedMaxK) || 2 * v >= kFusedTileH) return false; prm_.fused_k = (int)v; }
+        else if (k == "flag_sync") { if (!whole_in(v, 0, INT_MAX)) return false; prm_.flag_sync = (int)v; }  // 0 CTA barriers, else neighbour flags
+        else if (k == "time_kernels") { if (!is_flag(v)) return false; prm_.time_kernels = (int)v; }
+        else if (k == "use_tma") { if (!is_flag(v)) return false; prm_.use_tma = (int)v; }
+        else if (k == "prefetch") { if (!is_flag(v)) return false; prm_.prefetch = (int)v; }
+        else if (k == "serial_launches") { if (!is_flag(v)) return false; prm_.serial_launches = (int)v; }
+        else if (k == "lanes") { if (!whole_in(v, 0, kFusedMaxLanes)) return false; prm_.lanes = (int)v; }
         else return false;
         return true;
     }
@@ -185,6 +189,7 @@ class Tvl1 final : public FlowAlgorithm {
         LevelGeom lv[kMaxScales];
         const int n = level_geometry(w, h, lv);
         last_nscales_ = n;
+        last_warps_ = prm_.warps;
         std::memcpy(last_lv_, lv, sizeof(lv));
         if (prm_.fused) {
             PairJob one{};
@@ -246,6 +251,7 @@ class Tvl1 final : public FlowAlgorithm {
         LevelGeom lv[kMaxScales];
         const int n = level_geometry(w, h, lv);
         last_nscales_ = n;
+        last_warps_ = prm_.warps;
         std::memcpy(last_lv_, lv, sizeof(lv));
         if (!prm_.fused) {
             for (int i = 0; i < count; ++i) {
@@ -286,7 +292,7 @@ class Tvl1 final : public FlowAlgorithm {
             pixel_chunks += l.host_ctl->px_chunks_total;
         }
         out->nscales = last_nscales_;
-        out->warps = prm_.warps;
+        out->warps = last_warps_;
         for (int s = 0; s < last_nscales_; ++s) {
             out->level_w[s] = last_lv_[s].w;
             out->level_h[s] = last_lv_[s].h;
@@ -309,7 +315,7 @@ class Tvl1 final : public FlowAlgorithm {
         if (idx < 0 || idx >= pair_log_count_ || idx < pair_log_count_ - kPairLog) return false;
         if (stats_pending_) DFB_CUDA(cudaEventSynchronize(stats_event_));
         out->nscales = last_nscales_;
-        out->warps = prm_.warps;
+        out->warps = last_warps_;
         for (int s = 0; s < last_nscales_; ++s) {
             out->level_w[s] = last_lv_[s].w;
             out->level_h[s] = last_lv_[s].h;
@@ -836,7 +842,7 @@ class Tvl1 final : public FlowAlgorithm {
     int pair_log_count_ = 0, last_log_slot_ = 0;
     cudaEvent_t stats_event_ = nullptr;
     bool stats_pending_ = false;
-    int last_nscales_ = 0;
+    int last_nscales_ = 0, last_warps_ = 0;  // the log layout of the most recent call: a later set() does not change it
     LevelGeom last_lv_[kMaxScales] = {};
     int last_iters_[16 * 16] = {};
 };

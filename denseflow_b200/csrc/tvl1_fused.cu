@@ -844,8 +844,8 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const _
                     const ChunkMode mode = !level_resident(L, job.k, G) ? kStreamed : first ? kResidentFirst : kk == remaining ? kResidentFlush : kResidentNext;
                     run_chunk(job, c, L, s, cur, kk, job.k, chk, G, bid, part_sel, sm, prof.on, tile_base, tma_parity, mode, p11, p12, p21, p22);
                     first = false;
-                    prof.mark(2, 8 + s);
-                    if (prof.on) prof.acc[16 + s] += 1;
+                    prof.mark(2, s < 8 ? 8 + s : -1);  // per-scale slots for scales 0..7 only: [8 + s] and [16 + s] must not meet
+                    if (prof.on && s < 8) prof.acc[16 + s] += 1;
                     px_chunks += (unsigned long long)(L.w * L.h);
                     grid_barrier(bar, epoch, G, job.ctl);
                     prof.mark(3);

@@ -59,16 +59,20 @@ const char *dfb_last_error(const dfb_handle *h);
 
 /*
  * Algorithm hyper-parameters.  The reference never sets any (always create() defaults); these exist
- * for tests and benchmarks.  tvl1: "tau" "lambda" "theta" "nscales" "warps" "epsilon" "iterations" "scale_step" (must not
- * exceed the default 0.8 the workspace is sized for); engine knobs: "fused" (1 = persistent fused primal+dual kernel
+ * for tests and benchmarks.  tvl1: "tau" and "theta" (finite, > 0), "lambda" (finite, >= 0), "nscales" (1..16), "warps"
+ * (1..16), "epsilon" (finite; <= 0 = no convergence checks), "iterations" (>= 1), "scale_step" (> 0 and not above the
+ * default 0.8 the workspace is sized for); engine knobs: "fused" (1 = persistent fused primal+dual kernel
  * [default], 0 = one kernel per half-step, the reference's launch structure), "fused_k" (iterations kept on chip per tile
- * visit, default 8), "lanes" (pairs solved side by side per launch, 0 = auto [default], up to 64), "flag_sync" (1 =
+ * visit, 1..8, default 8), "lanes" (pairs solved side by side per launch, 0 = auto [default], up to 64), "flag_sync" (1 =
  * neighbour-warp progress flags in the tile loop [default], 0 = CTA-wide barriers), "use_tma" (1 = TMA staging of the
  * shared-memory tiles [default]), "prefetch" (1 = L2 prefetch of a CTA's next tile during the iterations [default]),
  * "serial_launches" (1 = the fused launches of all handles on one device run strictly one after another; 0 [default] = a
- * second handle's launch fills the SMs the first one's finished lanes free), "time_kernels" (CUDA-event timing of the dominant kernel, see dfb_counters).  farn: "num_levels" "num_iters" "poly_sigma"
- * (winSize 13, polyN 5, pyrScale 0.5 are fixed), "use_tma" (1 = persistent TMA-staged iteration kernel [default], 0 = the
- * LDG-staged one), "time_kernels".  Every combination of the engine knobs produces bit-identical flows.
+ * second handle's launch fills the SMs the first one's finished lanes free), "time_kernels" (CUDA-event timing of the dominant kernel, see dfb_counters).  farn: "num_levels" (0..5)
+ * "num_iters" (>= 1) "poly_sigma" (finite, > 0) (winSize 13, polyN 5, pyrScale 0.5 are fixed), "use_tma" (1 = persistent
+ * TMA-staged iteration kernel [default], 0 = the LDG-staged one), "time_kernels".  Every combination of the engine knobs
+ * produces bit-identical flows.  Counts take whole numbers only, and on/off knobs 0 or 1.  "flag_sync" takes any whole
+ * number >= 0; every value other than 0 means 1.  A refused value (NaN, an infinity, a fraction or
+ * a value out of range) returns DFB_ERR_INVALID_ARG with "bad parameter <name>" and leaves the parameter unchanged.
  * Both algorithms: "jpeg_exact" (0 [default] = JPEG files through nvJPEG; 1 = every JPEG this handle writes is exactly the
  * file cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality]) writes with OpenCV's other defaults, libjpeg-turbo 3.x:
  * baseline, standard Huffman tables, islow DCT, gray or YCbCr 4:2:0, no restart markers).  It covers
@@ -418,7 +422,8 @@ int dfb_get_counters(dfb_handle *h, dfb_counters *out);
  * Where the most recent fused-tvl1 pair's device time went, in ns, as seen by CTA 0 of the persistent
  * kernel (%globaltimer): [0] level start (gradients, zeroing) [1] warps [2] tile iterations
  * [3] grid barriers (includes waiting for slower CTAs) [4] upsample + merge, [8+s] tile iterations at
- * scale s, [16+s] tile visits (chunks) at scale s.  Zeros for other engines.  (The reference has only the
+ * scale s, [16+s] tile visits (chunks) at scale s, for s = 0..7 only (the tile iterations of scales 8..15 count in [2] alone).
+ * Zeros for other engines.  (The reference has only the
  * wall-clock summary line, src/denseflow_gpu.cpp:492-496.)
  */
 int dfb_get_tvl1_phase_ns(dfb_handle *h, uint64_t out[32]);

@@ -24,7 +24,14 @@ from tvl1_cases import chunk_inputs, warp_flow
 pytestmark = pytest.mark.gpu
 VARIANTS = ["strict", "default"]
 TW, TH = 128, 64
-L_T, TAUT, THETA = np.float32(0.15 * 0.3), np.float32(0.25 / 0.3), np.float32(0.3)
+
+
+def consts(tau=0.25, lam=0.15, theta=0.3):
+    """(l_t, taut, theta) as the engine derives them from the handle's tau, lambda and theta: in double, then rounded to fp32"""
+    return np.float32(lam * theta), np.float32(tau / theta), np.float32(theta)
+
+
+L_T, TAUT, THETA = consts()
 FRAME_SHAPES = [(1920, 1080), (1280, 720), (340, 256), (256, 256), (131, 97)]
 KS = [1, 2, 3, 5, 8]
 U = 2.0 ** -24
@@ -97,8 +104,10 @@ def _split(a, nb):
 
 
 # ---- inputs -------------------------------------------------------------------------------------------------------------
-def oracle_chunks(L, ins, kk, n):
-    """n x kk x (orc_tvl1_estimate_u; orc_tvl1_estimate_dual); the convergence sum of the last primal step"""
+def oracle_chunks(L, ins, kk, n, c=(L_T, TAUT, THETA)):
+    """n x kk x (orc_tvl1_estimate_u; orc_tvl1_estimate_dual) at the constants c = (l_t, taut, theta); the convergence sum
+    of the last primal step"""
+    l_t, taut, theta = c
     ix, iy, g, rc, u1, u2, p11, p12, p21, p22 = [a.copy() for a in ins]
     h, w = ix.shape
     err, terms = 0.0, None
@@ -106,36 +115,44 @@ def oracle_chunks(L, ins, kk, n):
         last = i == n * kk - 1
         if last:
             o1, o2 = u1.copy(), u2.copy()
-        err = L.orc_tvl1_estimate_u(ix, iy, g, rc, p11, p12, p21, p22, u1, u2, w, h, L_T, THETA, int(last))
+        err = L.orc_tvl1_estimate_u(ix, iy, g, rc, p11, p12, p21, p22, u1, u2, w, h, l_t, theta, int(last))
         if last:
             terms = ((o1 - u1) * (o1 - u1) + (o2 - u2) * (o2 - u2)).astype(np.float32)
-        L.orc_tvl1_estimate_dual(u1, u2, p11, p12, p21, p22, w, h, TAUT)
+        L.orc_tvl1_estimate_dual(u1, u2, p11, p12, p21, p22, w, h, taut)
     return [u1, u2, p11, p12, p21, p22], err, float(terms.astype(np.float64).sum())
 
 
-def unfused_chunks(e, ins, kk, n):
+def unfused_chunks(e, ins, kk, n, c=(L_T, TAUT, THETA)):
     """the same iterations through the stand-alone kernels of the same build"""
+    l_t, taut, theta = c
     ix, iy, g, rc, u1, u2 = ins[:6]
     p = ins[6:]
     err = 0.0
     for i in range(n * kk):
-        (u1, u2), err = e.debug_run_kernel("estimate_u", [ix, iy, g, rc, *p, u1, u2], 2, [L_T, THETA, int(i == n * kk - 1)])
-        p, _ = e.debug_run_kernel("estimate_dual", [u1, u2, *p], 4, [TAUT])
+        (u1, u2), err = e.debug_run_kernel("estimate_u", [ix, iy, g, rc, *p, u1, u2], 2, [l_t, theta, int(i == n * kk - 1)])
+        p, _ = e.debug_run_kernel("estimate_dual", [u1, u2, *p], 4, [taut])
     return [u1, u2] + list(p), err
 
 
-def run_chunks(oracle, variant, w, h, kk, n, cfg, seed):
+def run_chunks(oracle, variant, w, h, kk, n, cfg, seed, tau=0.25, lam=0.15, theta=0.3):
+    """the chunk stage with the handle's tau, lambda and theta set to these values (restored afterwards)"""
     G, lanes, tma, flag, check = cfg
     e = _engine(variant)
     cases = [chunk_inputs(w, h, seed + 97 * i) for i in range(lanes)]
     ins = [_stack([c[k] for c in cases]) for k in range(10)]
-    got, errs = e.debug_run_kernel("tvl1_chunks", ins, 6, [kk, n, check, G, tma, flag, 1, lanes], all_scalars=True)
-    tag = "%dx%d kk %d n %d G %d lanes %d tma %d flag %d check %d" % (w, h, kk, n, G, lanes, tma, flag, check)
+    keep = [e.get(k) for k in ("tau", "lambda", "theta")]
+    try:
+        e.set("tau", tau).set("lambda", lam).set("theta", theta)
+        got, errs = e.debug_run_kernel("tvl1_chunks", ins, 6, [kk, n, check, G, tma, flag, 1, lanes], all_scalars=True)
+    finally:
+        e.set("tau", keep[0]).set("lambda", keep[1]).set("theta", keep[2])
+    c = consts(tau, lam, theta)
+    tag = "%dx%d kk %d n %d G %d lanes %d tma %d flag %d check %d (l_t, taut, theta) %s" % (w, h, kk, n, G, lanes, tma, flag, check, c)
     for i, case in enumerate(cases):
         if variant == "strict":
-            want, oerr, sabs = oracle_chunks(oracle.lib(), case, kk, n)
+            want, oerr, sabs = oracle_chunks(oracle.lib(), case, kk, n, c)
         else:
-            want, oerr = unfused_chunks(e, case, kk, n)
+            want, oerr = unfused_chunks(e, case, kk, n, c)
             sabs = oerr
         for k, name in enumerate(["u1", "u2", "p11", "p12", "p21", "p22"]):
             _check("%s lane %d %s" % (tag, i, name), _split(got[k], lanes)[i], want[k])
