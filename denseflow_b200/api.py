@@ -469,11 +469,12 @@ class DenseOpticalFlow:
 
     # -- test hook: one stand-alone kernel on host planes --
     def debug_run_kernel(self, kernel, inputs, n_out, scalars=(), out_shape=None, all_scalars=False):
-        """returns (output planes, scalars_out[0]), or with all_scalars (output planes, scalars_out[:16])"""
+        """returns (output planes, scalars_out[0]), or with all_scalars (output planes, scalars_out[:16]); out_shape: the shape of
+        every output, or a list of one shape per output (default: the inputs')"""
         inputs = [np.ascontiguousarray(a, np.float32) for a in inputs]
         h, w = inputs[0].shape
-        oshape = out_shape or (h, w)
-        outs = [np.empty(oshape, np.float32) for _ in range(n_out)]
+        oshapes = out_shape if isinstance(out_shape, list) else [out_shape or (h, w)] * n_out
+        outs = [np.empty(s, np.float32) for s in oshapes]
         ip = (C.c_void_p * len(inputs))(*[a.ctypes.data for a in inputs])
         op = (C.c_void_p * n_out)(*[a.ctypes.data for a in outs])
         sc = (C.c_double * max(len(scalars), 1))(*[float(x) for x in scalars])

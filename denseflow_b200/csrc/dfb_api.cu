@@ -93,6 +93,7 @@ struct dfb_handle {
     // scratch of the frame-extraction calls (-s=0), grown on demand
     TapTable ycc_taps;                // colour resize of all three calls
     DeviceBuffer<uint8_t> enc_ycc;    // Y / Cb / Cr planes of dfb_encode_jpeg_bgr_device
+    DeviceBuffer<uint8_t> enc_gray;   // the block-padded copy of the plane dfb_encode_jpeg_gray_device hands nvJPEG
     DeviceBuffer<uint8_t> ex_bgr, ex_ycc;  // the -s=0 pipeline: BGR staging of its frame source, planes of two groups
     struct {
         Events h2d, conv;     // [2] BGR staging filled; the BGR source's staging frame consumed
@@ -244,16 +245,17 @@ int check_geometry(dfb_handle *h, int sw, int sh, size_t bgr_pitch, int &dw, int
     return check_size(h, dw, dh);
 }
 
-// Y / Cb / Cr planes of one dw x dh frame in one scratch block: 64-byte aligned rows, chroma ceil(dw / 2) x ceil(dh / 2)
+// Y / Cb / Cr planes of one dw x dh frame in one scratch block, with room for whole 16 x 16 MCUs (YccExtent::mcu): 64-byte
+// aligned rows, round16(dh) luma rows, and round8(ceil(dh / 2)) chroma rows of round8(ceil(dw / 2)) samples or more
 struct YccLayout {
     size_t y_pitch, c_pitch, cb_off, cr_off, bytes;
     YccLayout(int dw, int dh) {
-        const int cw = (dw + 1) / 2, ch = (dh + 1) / 2;
+        const int cw = (dw + 1) / 2, crows = round_up((dh + 1) / 2, 8);
         y_pitch = (size_t)round_up(dw, 64);
         c_pitch = (size_t)round_up(cw, 64);
-        cb_off = y_pitch * dh;
-        cr_off = cb_off + c_pitch * ch;
-        bytes = cr_off + c_pitch * ch;
+        cb_off = y_pitch * 2 * crows;
+        cr_off = cb_off + c_pitch * crows;
+        bytes = cr_off + c_pitch * crows;
     }
 };
 
@@ -298,8 +300,10 @@ class JpegSink {
         }
     }
     bool exact() const { return jex_ != nullptr; }
-    // the chroma columns launch_bgr_to_ycc420 writes for this encoder (0: the image's own)
-    int chroma_cols(int w) const { return jex_ ? jpeg_chroma_cols(w) : 0; }
+    // What the encoder reads of a w x h image: JpegExactEncoder replicates edge samples itself, except the padded chroma
+    // columns; nvJPEG reads whole blocks (gray) or MCUs (colour), so the planes must hold libjpeg's padding up to there.
+    YccExtent ycc_extent() const { return jex_ ? YccExtent::chroma_cols : YccExtent::mcu; }
+    bool needs_padded_gray(int w, int hh) const { return !jex_ && (w % 8 || hh % 8); }
     // Enqueues the encodes of n images of src into `slot` on s, each file to be at most capacity bytes; the exact encoder's
     // lengths follow them to the host on s.
     void encode(int slot, int n, const JpegSrc &src, int components, int w, int hh, int quality, size_t capacity, cudaStream_t s) {
@@ -880,6 +884,20 @@ int dfb_encode_jpeg_gray_device(dfb_handle *h, const uint8_t *gray, size_t gray_
         JpegSrc src;
         src.base = gray;
         src.pitch = gray_pitch;
+        if (!sink.exact()) {
+            // nvJPEG gets a copy in handle scratch: it refuses some pitches of block-aligned planes (status 2), and it must not
+            // read the caller's bytes around the plane.  Partial blocks are padded as libjpeg pads them.
+            const int pw = round_up(width, 8), ph = round_up(height, 8);
+            const size_t pitch = (size_t)round_up(pw, 64);
+            h->enc_gray.grow(pitch * ph);
+            DFB_CUDA(cudaMemcpy2DAsync(h->enc_gray, pitch, gray, gray_pitch, width, height, cudaMemcpyDeviceToDevice, s));
+            if (sink.needs_padded_gray(width, height)) {
+                launch_pad_edges(h->enc_gray, pitch, 0, 1, width, height, pw, ph, s);
+                ++h->alg->launches;
+            }
+            src.base = h->enc_gray;
+            src.pitch = pitch;
+        }
         sink.encode(0, 1, src, 1, width, height, quality, out_capacity, s);
         DFB_CUDA(cudaStreamSynchronize(s));
         auto too_small = [&](int, size_t need) {
@@ -1008,13 +1026,16 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
     //   s_fetch   files of group g-1 to the host while the GPU works on group g
     const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
     const size_t fpx = (size_t)dw * dh;
+    // quantised planes: whole 8 x 8 blocks, so nvJPEG reads their edge padding (written by launch_pad_edges) and nothing else
+    const int qw = round_up(dw, 8), qh = round_up(dh, 8);
+    const size_t qpx = (size_t)qw * qh;
     h->pb_frames.grow(fpx * n_frames);
     if (o.png) {
         h->pb_flow.grow(fpx * 2 * sizeof(float) * 2 * B);  // float2 fields of two groups
         h->png_bgr.grow(fpx * 3 * 2 * B);    // their packed images
         PngOut::prepare(h);
     } else {
-        h->pb_q.grow(fpx * 2 * 2 * B);  // quantised planes of two groups
+        h->pb_q.grow(qpx * 2 * 2 * B);  // quantised planes of two groups
     }
     alg.ensure_slots(B + astep + 1);
     const int nslots = alg.num_slots();
@@ -1028,9 +1049,9 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
     // the group's 2 m planes, encoded as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
     auto group_planes = [&](int slot) {
         JpegSrc src;
-        src.base = h->pb_q + (size_t)slot * B * 2 * fpx;
-        src.img_stride = fpx;
-        src.pitch = (size_t)dw;
+        src.base = h->pb_q + (size_t)slot * B * 2 * qpx;
+        src.img_stride = qpx;
+        src.pitch = (size_t)qw;
         return src;
     };
     // pair i of slot's group: its flow field and packed image (-st=png)
@@ -1061,9 +1082,9 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
                 pj.flow_pitch_bytes = (size_t)dw * 2 * sizeof(float);
             } else {
                 pj.bound = o.jpg->bound;
-                pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * fpx;
-                pj.qy = pj.qx + fpx;
-                pj.q_pitch = (size_t)dw;
+                pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * qpx;
+                pj.qy = pj.qx + qpx;
+                pj.q_pitch = (size_t)qw;
             }
         }
         alg.solve_batch(jobs.data(), m, dw, dh, h->s_compute);
@@ -1071,10 +1092,16 @@ int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const C
         DFB_CUDA(cudaEventRecord(ev.flow[slot], h->s_compute));
         // encode stage (src/common.cpp:48-71)
         DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.flow[slot], 0));
-        if (o.png)
+        if (o.png) {
             PngOut::encode(h, m, image(slot, 0), dw, dh, slot);
-        else
-            sink->encode(slot, 2 * m, group_planes(slot), 1, dw, dh, o.jpg->quality, o.jpg->capacity, h->s_out);
+        } else {
+            const JpegSrc src = group_planes(slot);
+            if (sink->needs_padded_gray(dw, dh)) {
+                launch_pad_edges(const_cast<uint8_t *>(src.base), src.pitch, src.img_stride, 2 * m, dw, dh, qw, qh, h->s_out);
+                ++alg.launches;
+            }
+            sink->encode(slot, 2 * m, src, 1, dw, dh, o.jpg->quality, o.jpg->capacity, h->s_out);
+        }
         DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
         h->counters.pairs += m;
     };
@@ -1254,7 +1281,7 @@ int extract_frames(dfb_handle *h, int n_frames, int sw, int sh, int dw, int dh, 
         source(g, f0, m, [&](int i, const uint8_t *bgr) {
             uint8_t *p = planes + (size_t)i * L.bytes;
             launch_bgr_to_ycc420(bgr, (size_t)sw * 3, sw, sh, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                                 p + L.cr_off, L.c_pitch, h->s_compute, sink.chroma_cols(dw));
+                                 p + L.cr_off, L.c_pitch, h->s_compute, sink.ycc_extent());
             ++h->alg->launches;
         });
         DFB_CUDA(cudaEventRecord(ev.planes[slot], h->s_compute));
@@ -1449,7 +1476,7 @@ int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pit
         JpegSink sink(h, 1, 1);
         uint8_t *p = h->enc_ycc;
         launch_bgr_to_ycc420(bgr, bgr_pitch, src_width, src_height, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
-                             p + L.cr_off, L.c_pitch, s, sink.chroma_cols(dw));
+                             p + L.cr_off, L.c_pitch, s, sink.ycc_extent());
         ++h->alg->launches;
         sink.encode(0, 1, ycc_src(p, L), 3, dw, dh, quality, out_capacity, s);
         DFB_CUDA(cudaStreamSynchronize(s));
@@ -1582,6 +1609,42 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
         const std::string k(kernel);
         if (h->alg->debug_run(k, in, n_in, out, n_out, width, height, scalars, n_scalars, scalars_out)) return DFB_OK;  // the engine's own stages
         auto sc = [&](int i) { return i < n_scalars ? scalars[i] : 0.0; };
+        if (k == "jpeg_padded_gray" || k == "jpeg_padded_ycc420") {  // the planes the nvJPEG path hands the encoder
+            const bool gray = k == "jpeg_padded_gray";
+            if (n_in != (gray ? 1 : 3) || n_out != n_in) throw std::runtime_error(k + ": expects " + std::to_string(gray ? 1 : 3) + " inputs and outputs");
+            const size_t px = (size_t)width * height;
+            std::vector<uint8_t> host(px * n_in);
+            for (size_t i = 0; i < px; ++i)  // gray, or packed BGR from the B, G, R planes
+                for (int c = 0; c < n_in; ++c) host[i * n_in + c] = (uint8_t)std::lrint(std::min(std::max(in[c][i], 0.f), 255.f));
+            auto download = [&](float *dst, const uint8_t *src, size_t pitch, int w, int hh) {
+                std::vector<uint8_t> b((size_t)w * hh);
+                DFB_CUDA(cudaMemcpy2D(b.data(), w, src, pitch, w, hh, cudaMemcpyDeviceToHost));
+                for (size_t i = 0; i < b.size(); ++i) dst[i] = b[i];
+            };
+            DeviceBuffer<uint8_t> src, planes;
+            src.allocate(host.size());
+            DFB_CUDA(cudaMemcpy(src, host.data(), host.size(), cudaMemcpyHostToDevice));
+            if (gray) {
+                const int pw = round_up(width, 8), ph = round_up(height, 8);
+                planes.allocate((size_t)pw * ph);
+                DFB_CUDA(cudaMemcpy2D(planes, pw, src, width, width, height, cudaMemcpyDeviceToDevice));
+                launch_pad_edges(planes, pw, 0, 1, width, height, pw, ph, nullptr);
+                download(out[0], planes, pw, pw, ph);
+                return DFB_OK;
+            }
+            const int dw = sc(0) > 0 ? (int)sc(0) : width, dh = sc(1) > 0 ? (int)sc(1) : height;
+            const YccLayout L(dw, dh);
+            planes.allocate(L.bytes);
+            const ResizeTap *taps = ycc_tables(h, width, height, dw, dh);
+            uint8_t *p = planes;
+            launch_bgr_to_ycc420(src, (size_t)width * 3, width, height, dw, dh, taps, taps ? taps + dw : nullptr, p, L.y_pitch, p + L.cb_off,
+                                 p + L.cr_off, L.c_pitch, nullptr, YccExtent::mcu);
+            const int cw = round_up((dw + 1) / 2, 8), ch = round_up((dh + 1) / 2, 8);
+            download(out[0], p, L.y_pitch, 2 * cw, 2 * ch);
+            download(out[1], p + L.cb_off, L.c_pitch, cw, ch);
+            download(out[2], p + L.cr_off, L.c_pitch, cw, ch);
+            return DFB_OK;
+        }
         int ow = width, oh = height;
         if (k == "resize") {
             ow = (int)sc(0);

@@ -60,18 +60,23 @@ __device__ __forceinline__ void bgr_to_ycc(int b, int g, int r, int &y, int &cb,
 // h2v2_downsample (jcsample.c): one thread per 2 x 2 destination block, whose chroma sample never leaves registers.
 // An odd last column / row is replicated (expand_right_edge, jcsample.c; expand_bottom_edge, jcprepct.c), and the
 // downsampling bias is 1 on even and 2 on odd chroma columns, restarting on every row.  Chroma columns up to c_cols are
-// written (past ceil(dw / 2) only the replicated last column contributes).
+// written (past ceil(dw / 2) only the replicated last column contributes), chroma rows up to c_rows (past ceil(dh / 2) a
+// copy of the last chroma row, as expand_bottom_edge leaves the downsampled planes) and luma up to y_cols x y_rows (past
+// dw x dh the last column and row replicated).
 __global__ void __launch_bounds__(256) k_bgr_to_ycc420(const uint8_t *__restrict__ src, size_t src_pitch, int sw, int sh,
                                                        int dw, int dh, const ResizeTap *__restrict__ xt,
                                                        const ResizeTap *__restrict__ yt, uint8_t *__restrict__ yp, size_t y_pitch,
                                                        uint8_t *__restrict__ cbp, uint8_t *__restrict__ crp, size_t c_pitch,
-                                                       int c_cols) {
+                                                       int c_cols, int c_rows, int y_cols, int y_rows) {
     const int cx = blockIdx.x * 32 + threadIdx.x, cy = blockIdx.y * 8 + threadIdx.y;
-    if (cx >= c_cols || cy >= (dh + 1) >> 1) return;
-    int sum_cb = 0, sum_cr = 0;
+    if (cx >= c_cols || cy >= c_rows) return;
+    // a chroma padding row repeats the last chroma row; its luma rows all repeat row dh - 1, the second row that one reads
+    const bool pad_row = cy >= (dh + 1) >> 1;
+    const int cys = pad_row ? ((dh + 1) >> 1) - 1 : cy;
+    int sum_cb = 0, sum_cr = 0, lum[2][2];
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
-        const int y = min(2 * cy + j, dh - 1);
+        const int y = min(2 * cys + j, dh - 1);
         const uint8_t *r0, *r1 = nullptr;
         ResizeTap ty{};
         if (xt) {
@@ -96,14 +101,36 @@ __global__ void __launch_bounds__(256) k_bgr_to_ycc420(const uint8_t *__restrict
             }
             int Y, Cb, Cr;
             bgr_to_ycc(bgr[0], bgr[1], bgr[2], Y, Cb, Cr);
-            if (2 * cx + i < dw && 2 * cy + j < dh) yp[(size_t)(2 * cy + j) * y_pitch + 2 * cx + i] = (uint8_t)Y;
+            lum[j][i] = Y;
             sum_cb += Cb;
             sum_cr += Cr;
         }
     }
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+            if (2 * cx + i < y_cols && 2 * cy + j < y_rows) yp[(size_t)(2 * cy + j) * y_pitch + 2 * cx + i] = (uint8_t)lum[pad_row ? 1 : j][i];
     const int bias = 1 + (cx & 1);
     cbp[(size_t)cy * c_pitch + cx] = (uint8_t)((sum_cb + bias) >> 2);
     crp[(size_t)cy * c_pitch + cx] = (uint8_t)((sum_cr + bias) >> 2);
+}
+
+// launch_pad_edges: thread t < h of plane blockIdx.y fills row t's columns [w, pw), thread h + x fills column x's rows
+// [h, ph).  Both read only pixels inside the image, which nothing writes.
+__global__ void __launch_bounds__(256) k_pad_edges(uint8_t *__restrict__ planes, size_t pitch, size_t plane_stride, int w, int h,
+                                                   int pw, int ph) {
+    const int t = blockIdx.x * 256 + threadIdx.x;
+    uint8_t *p = planes + (size_t)blockIdx.y * plane_stride;
+    if (t < h) {
+        uint8_t *row = p + (size_t)t * pitch;
+        const uint8_t v = row[w - 1];
+        for (int x = w; x < pw; ++x) row[x] = v;
+    } else if (t < h + pw) {
+        const int x = t - h;
+        const uint8_t v = p[(size_t)(h - 1) * pitch + min(x, w - 1)];
+        for (int y = h; y < ph; ++y) p[(size_t)y * pitch + x] = v;
+    }
 }
 
 }  // namespace
@@ -143,10 +170,21 @@ void launch_resize_u8(const uint8_t *src, size_t src_pitch, int sw, int sh, uint
 }
 
 void launch_bgr_to_ycc420(const uint8_t *bgr, size_t bgr_pitch, int sw, int sh, int dw, int dh, const ResizeTap *xt, const ResizeTap *yt,
-                          uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, cudaStream_t s, int c_cols) {
-    if (c_cols <= 0) c_cols = ceil_div(dw, 2);
-    k_bgr_to_ycc420<<<dim3(ceil_div(c_cols, 32), ceil_div(ceil_div(dh, 2), 8)), dim3(32, 8), 0, s>>>(
-        bgr, bgr_pitch, sw, sh, dw, dh, xt, yt, y, y_pitch, cb, cr, c_pitch, c_cols);
+                          uint8_t *y, size_t y_pitch, uint8_t *cb, uint8_t *cr, size_t c_pitch, cudaStream_t s, YccExtent extent) {
+    int c_cols = ceil_div(dw, 2), c_rows = ceil_div(dh, 2), y_cols = dw, y_rows = dh;
+    if (extent != YccExtent::image) c_cols = round_up(c_cols, 8);
+    if (extent == YccExtent::mcu) {
+        c_rows = round_up(c_rows, 8);
+        y_cols = 2 * c_cols;
+        y_rows = 2 * c_rows;
+    }
+    k_bgr_to_ycc420<<<dim3(ceil_div(c_cols, 32), ceil_div(c_rows, 8)), dim3(32, 8), 0, s>>>(
+        bgr, bgr_pitch, sw, sh, dw, dh, xt, yt, y, y_pitch, cb, cr, c_pitch, c_cols, c_rows, y_cols, y_rows);
+    DFB_KERNEL_CHECK();
+}
+
+void launch_pad_edges(uint8_t *planes, size_t pitch, size_t plane_stride, int n, int w, int h, int pw, int ph, cudaStream_t s) {
+    k_pad_edges<<<dim3(ceil_div(h + pw, 256), n), 256, 0, s>>>(planes, pitch, plane_stride, w, h, pw, ph);
     DFB_KERNEL_CHECK();
 }
 

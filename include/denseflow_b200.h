@@ -159,6 +159,8 @@ int dfb_resize_gray_device(dfb_handle *h, const uint8_t *src, size_t src_pitch, 
  * (dfb_jpeg_max_bytes(width, height) holds i.i.d. noise at quality 100; a larger file fails cleanly with the needed
  * length in the message); *out_len receives the length.  Blocks until the bitstream is on the host.  With the handle's
  * "jpeg_exact" = 0 [default] nvJPEG encodes, not byte-identical to libjpeg-turbo; with 1 the file is imencode(".jpg")'s bytes.
+ * Only the width x height plane is read: nvJPEG encodes a copy in handle scratch whose partial 8 x 8 blocks are padded
+ * as libjpeg pads them (last column and row repeated), so the file depends on the plane alone.
  */
 size_t dfb_jpeg_max_bytes(int width, int height);
 int dfb_encode_jpeg_gray_device(dfb_handle *h, const uint8_t *gray, size_t gray_pitch, int width, int height, int quality,
@@ -284,7 +286,11 @@ size_t dfb_jpeg_max_bytes_bgr(int width, int height);
  * One frame: resize + imencode(".jpg", frame) of a BGR frame in device memory.  Baseline, standard Huffman tables, YCbCr
  * 4:2:0; out is a host buffer of out_capacity bytes, *out_len receives the length.  The work is enqueued on `stream` and
  * the call blocks until the bitstream is on the host.  With "jpeg_exact" = 0 [default] nvJPEG encodes, not byte-identical
- * to libjpeg (only the DCT and the padding of the edge MCUs differ); with 1 the file is imencode(".jpg", resized frame)'s bytes.
+ * to libjpeg; with 1 the file is imencode(".jpg", resized frame)'s bytes.  nvJPEG reads whole 16 x 16 MCUs of handle
+ * scratch, padded as libjpeg pads them (luma: last column and row repeated; chroma columns downsampled from the repeated
+ * last column, chroma rows repeating the last one), so only the DCT and the luma blocks wholly past the image (libjpeg's
+ * DC-only dummy blocks) differ, and the file depends on the frame alone.  The same holds for every nvJPEG file of
+ * dfb_extract_frames_host / dfb_extract_frames_jpeg_host, and for the flow chains' gray planes (8 x 8 blocks).
  */
 int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, int src_width, int src_height, int dst_width,
                                int dst_height, int quality, uint8_t *out, size_t out_capacity, size_t *out_len, void *stream);
@@ -391,6 +397,10 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   "tvl1_upsample"    in {u1, u2}                         out {u1, u2 (scalars[0] x scalars[1])}; scalars {dst w, dst h, lanes}
  *                      (resize to the finer level, times 1 / scale_step)
  *   "tvl1_merge"       in {u1, u2}                         out {flow x, flow y} (bound 0) or {qx, qy} as floats; scalars {bound, lanes}
+ *   "jpeg_padded_gray" in {gray}                           out {the plane padded to round8(w) x round8(h)}
+ *   "jpeg_padded_ycc420" in {B, G, R}                      out {Y round16(dw) x round16(dh), Cb, Cr round8(ceil(dw / 2)) x
+ *                      round8(ceil(dh / 2))}; scalars {dst w, dst h} (0 / 0: no resize)
+ *     (the planes the nvJPEG path (jpeg_exact = 0) hands the encoder, with libjpeg's edge padding; inputs hold uint8 values)
  * Not part of the reference's surface.
  */
 int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *in, int n_in, float *const *out, int n_out,
