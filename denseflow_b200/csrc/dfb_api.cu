@@ -1645,6 +1645,31 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             download(out[2], p + L.cr_off, L.c_pitch, cw, ch);
             return DFB_OK;
         }
+        if (k == "png_encode_batch") {  // n images through one PngEncoder::encode call, as the -st=png batch path runs them
+            const int n = (int)sc(0);
+            if (n_in != 3 || n_out != 1) throw std::runtime_error(k + ": expects 3 inputs and 1 output");
+            if (n < 1 || n > 16 || height % n) throw std::runtime_error(k + ": n must be 1..16 and divide the height");
+            const int hh = height / n;
+            const size_t px = (size_t)width * height, cap = png_max_bytes(width, hh);
+            std::vector<uint8_t> host(px * 3);
+            for (size_t i = 0; i < px; ++i)  // packed BGR from the B, G, R planes
+                for (int c = 0; c < 3; ++c) host[i * 3 + c] = (uint8_t)std::lrint(std::min(std::max(in[c][i], 0.f), 255.f));
+            DeviceBuffer<uint8_t> src;
+            src.allocate(host.size());
+            DFB_CUDA(cudaMemcpy(src, host.data(), host.size(), cudaMemcpyHostToDevice));
+            if (!h->png) h->png.reset(new PngEncoder());
+            h->alg->launches += h->png->encode(n, src, (size_t)3 * width * hh, (size_t)3 * width, width, hh, 0, nullptr);
+            DFB_CUDA(cudaStreamSynchronize(nullptr));
+            std::vector<uint8_t> files((size_t)n * cap);
+            auto reject = [&](int i, uint64_t len) { return "png encoder failed on image " + std::to_string(i) + " (" + std::to_string(len) + " bytes)"; };
+            auto to = [&](int i, size_t len) {
+                if (scalars_out) scalars_out[i] = (double)len;
+                return files.data() + (size_t)i * cap;
+            };
+            h->png->files().deliver(0, n, cap, reject, to, h->counters.d2h_bytes, nullptr);
+            for (size_t i = 0; i < files.size(); ++i) out[0][i] = files[i];  // out[0]: n rows of png_max_bytes(w, h / n)
+            return DFB_OK;
+        }
         int ow = width, oh = height;
         if (k == "resize") {
             ow = (int)sc(0);

@@ -401,6 +401,9 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   "jpeg_padded_ycc420" in {B, G, R}                      out {Y round16(dw) x round16(dh), Cb, Cr round8(ceil(dw / 2)) x
  *                      round8(ceil(dh / 2))}; scalars {dst w, dst h} (0 / 0: no resize)
  *     (the planes the nvJPEG path (jpeg_exact = 0) hands the encoder, with libjpeg's edge padding; inputs hold uint8 values)
+ *   "png_encode_batch" in {B, G, R}                        out {files: n rows of dfb_png_max_bytes(w, h / n)}; scalars {n}
+ *                      (n = 1..16 images of h / n rows, stacked along the rows, encoded by one call of the batch PNG
+ *                      encoder that -st=png uses; scalars_out[i] = file i's length, its bytes as floats in row i)
  * Not part of the reference's surface.
  */
 int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *in, int n_in, float *const *out, int n_out,

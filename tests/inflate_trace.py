@@ -24,6 +24,10 @@ class _Bits:
     def align(self):
         self.bits(self.nb & 7)
 
+    def pos(self):
+        """bits consumed from the start of the data"""
+        return 8 * self.i - self.nb
+
 
 def _table(lengths):
     """LSB-first lookup table over the next max-length bits -> (symbol, length)."""
@@ -66,14 +70,17 @@ _ORDER = [16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15]
 
 def trace(zstream):
     """zstream: a zlib stream.  Returns (blocks, data).  Each block is a dict: type ('stored' / 'fixed' / 'dynamic'),
-    final, lit_lengths / dist_lengths (dynamic), symbols (ints for literals, (length, distance) for matches; the end of block
-    is not listed), stored_len."""
+    final, lit_lengths / dist_lengths / code_lengths (dynamic), symbols (ints for literals, (length, distance) for matches;
+    the end of block is not listed), stored_len, and the bit positions in zstream of the block's first bit (start), of the
+    first bit after its header (body: after the tree description of a dynamic block, after the 3 type bits of a fixed one)
+    and of the first bit after the block (end)."""
     br = _Bits(zstream, 2)
     out = bytearray()
     blocks = []
     while True:
+        start = br.pos()
         final, btype = br.bits(1), br.bits(2)
-        blk = {"final": final, "symbols": []}
+        blk = {"final": final, "symbols": [], "start": start}
         blocks.append(blk)
         if btype == 0:
             br.align()
@@ -106,6 +113,7 @@ def trace(zstream):
                         lens += [0] * (11 + br.bits(7))
                 ll, dl = lens[:hlit], lens[hlit:]
                 blk.update(type="dynamic", lit_lengths=ll, dist_lengths=dl, code_lengths=cl)
+            blk["body"] = br.pos()
             lt, dt = _table(ll), _table(dl) if max(dl) else None
             while True:
                 s = _decode(br, lt)
@@ -122,6 +130,7 @@ def trace(zstream):
                     for _ in range(ln):
                         out.append(out[-dist])
                     blk["symbols"].append((ln, dist))
+        blk["end"] = br.pos()
         if final:
             break
     br.align()
