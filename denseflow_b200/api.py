@@ -47,6 +47,10 @@ class DenseOpticalFlow:
             raise RuntimeError(self._L.dfb_last_error(self._h).decode() or "dfb error %d" % rc)
 
     def set(self, name, value):
+        """dfb_set_param: one algorithm parameter or engine knob (include/denseflow_b200.h lists them).  TV-L1 also takes
+        "median_filtering" (0 or 1 = off [default], 3 or 5 = the window of a median of the flow between iterations) and
+        "median_interval" (>= 1, default 30: the median runs before iterations 0, I, 2I, ... of every warp).  A refused
+        value raises RuntimeError("bad parameter <name>") and leaves the parameter as it was.  Returns self."""
         self._check(self._L.dfb_set_param(self._h, name.encode(), float(value)))
         return self
 
@@ -515,7 +519,7 @@ class DenseOpticalFlow:
         v = list(buf)
         return {"level_start": v[0], "warp": v[1], "tiles": v[2], "barrier": v[3], "upsample_merge": v[4],
                 "tile_load": v[5], "tile_iter": v[6], "tile_store": v[7],
-                "tiles_per_scale": v[8:16], "chunks_per_scale": v[16:24]}
+                "tiles_per_scale": v[8:16], "chunks_per_scale": v[16:24], "median": v[24]}
 
     def reset_counters(self):
         self._check(self._L.dfb_reset_counters(self._h))

@@ -41,6 +41,9 @@ struct Tvl1Params {
     int prefetch = 1;
     int lanes = 0;  // pairs solved side by side per fused launch; 0 = choose from the tile counts
     int serial_launches = 0;  // 1: fused launches of all handles on one device execute strictly one after another (event chain)
+    int median_filtering = 0;  // 3 or 5: the window of the median of u1, u2 between iterations (DESIGN §4.3); 0 or 1: off
+    int median_interval = 30;  // the median runs before every iteration n of a warp with n % median_interval == 0
+    int median_k() const { return median_filtering > 1 ? median_filtering : 0; }
 };
 
 class Tvl1 final : public FlowAlgorithm {
@@ -110,6 +113,8 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "prefetch") { if (!is_flag(v)) return false; prm_.prefetch = (int)v; }
         else if (k == "serial_launches") { if (!is_flag(v)) return false; prm_.serial_launches = (int)v; }
         else if (k == "lanes") { if (!whole_in(v, 0, kFusedMaxLanes)) return false; prm_.lanes = (int)v; }
+        else if (k == "median_filtering") { if (!(v == 0 || v == 1 || v == 3 || v == 5)) return false; prm_.median_filtering = (int)v; }
+        else if (k == "median_interval") { if (!whole_in(v, 1, INT_MAX)) return false; prm_.median_interval = (int)v; }
         else return false;
         return true;
     }
@@ -130,6 +135,8 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "prefetch") *v = prm_.prefetch;
         else if (k == "serial_launches") *v = prm_.serial_launches;
         else if (k == "lanes") *v = prm_.lanes;
+        else if (k == "median_filtering") *v = prm_.median_filtering;
+        else if (k == "median_interval") *v = prm_.median_interval;
         else return false;
         return true;
     }
@@ -335,7 +342,8 @@ class Tvl1 final : public FlowAlgorithm {
             int stage, n_in, n_out, n_sc;
         } kStages[] = {{"tvl1_level_start", kFusedStageLevelStart, 3, 8, 2}, {"tvl1_warp", kFusedStageWarp, 6, 4, 1},
                        {"tvl1_gq", kFusedStageGq, 1, 1, 1},        {"tvl1_chunks", kFusedStageChunks, 10, 6, 8},
-                       {"tvl1_upsample", kFusedStageUpsample, 2, 2, 3}, {"tvl1_merge", kFusedStageMerge, 2, 2, 2}};
+                       {"tvl1_upsample", kFusedStageUpsample, 2, 2, 3}, {"tvl1_merge", kFusedStageMerge, 2, 2, 2},
+                       {"tvl1_median", kFusedStageMedian, 2, 2, 2}};
         int si = -1;
         for (int i = 0; i < (int)(sizeof(kStages) / sizeof(kStages[0])); ++i)
             if (k == kStages[i].name) si = i;
@@ -370,6 +378,8 @@ class Tvl1 final : public FlowAlgorithm {
         if (st.stage == kFusedStageChunks && (kk < 1 || kk > kFusedMaxK || 2 * kk >= kFusedTileH || nch < 1))
             throw std::runtime_error(k + ": kk must be in [1, " + std::to_string(kFusedMaxK) + "] and n >= 1");
         const int bound = st.stage == kFusedStageMerge ? (int)sc(0, 0) : 0;
+        const int median_k = st.stage == kFusedStageMedian ? (int)sc(0, 0) : 0;
+        if (st.stage == kFusedStageMedian && median_k != 3 && median_k != 5) throw std::runtime_error(k + ": the window must be 3 or 5");
 
         DFB_CUDA(cudaDeviceSynchronize());  // nothing of an earlier asynchronous call may still use the slots or lanes
         const cudaStream_t s = nullptr;
@@ -397,6 +407,7 @@ class Tvl1 final : public FlowAlgorithm {
                 pj.q_pitch = (size_t)w;
             }
             fill_job(jobs[i], lanes_[i], pj, lv, nl);
+            jobs[i].median_k = median_k;
         }
         prm_ = keep;
 
@@ -446,6 +457,10 @@ class Tvl1 final : public FlowAlgorithm {
                 poison(plane(L.u2[0], 1));
                 ins = {plane(L.u1[0], 1), plane(L.u2[0], 1)};
                 outs[i] = {plane(J.lv[0].u1[0], 0), plane(J.lv[0].u2[0], 0)};
+                break;
+            case kFusedStageMedian:
+                ins = {plane(L.u1[0], 0), plane(L.u2[0], 0)};
+                outs[i] = {plane(L.u1[1], 0), plane(L.u2[1], 0)};
                 break;
             default:  // merge
                 ins = {plane(L.u1[0], 0), plane(L.u2[0], 0)};
@@ -614,12 +629,20 @@ class Tvl1 final : public FlowAlgorithm {
             launches += 5;
             const double scaled_eps = prm_.epsilon * prm_.epsilon * (double)((long)g.w * g.h);
             const int nblk = estimate_u_blocks(g.w, g.h);
+            // the median's destination: this level's plane of the second flow pyramid, which only the fused schedule uses
+            const Plane m1 = level_plane(wk.u1pyr[1], lv, l), m2 = level_plane(wk.u2pyr[1], lv, l);
             for (int wi = 0; wi < prm_.warps; ++wi) {
                 launch_warp_backward(I0, I1, I1x, I1y, u1, u2, I1wx, I1wy, grad, rho_c, s);
                 ++launches;
                 double error = DBL_MAX, prev_error = 0.0;
                 int it = 0;
                 for (; error > scaled_eps && it < prm_.iterations; ++it) {
+                    if (prm_.median_k() && it % prm_.median_interval == 0) {  // the A.4 state does not change
+                        launch_median(u1, u2, m1, m2, prm_.median_k(), s);
+                        ++launches;
+                        DFB_CUDA(cudaMemcpy2DAsync(u1.p, (size_t)u1.pitch * 4, m1.p, (size_t)m1.pitch * 4, (size_t)g.w * 4, g.h, cudaMemcpyDeviceToDevice, s));
+                        DFB_CUDA(cudaMemcpy2DAsync(u2.p, (size_t)u2.pitch * 4, m2.p, (size_t)m2.pitch * 4, (size_t)g.w * 4, g.h, cudaMemcpyDeviceToDevice, s));
+                    }
                     const bool calc_error = prm_.epsilon > 0 && (it & 1) && prev_error < scaled_eps;
                     launch_estimate_u(I1wx, I1wy, grad, rho_c, p11, p12, p21, p22, u1, u2, c,
                                       calc_error ? wk.partials : nullptr, s);
@@ -687,6 +710,8 @@ class Tvl1 final : public FlowAlgorithm {
         job.flag_sync = prm_.flag_sync;
         job.use_tma = prm_.use_tma;
         job.prefetch = prm_.prefetch;
+        job.median_k = prm_.median_k();
+        job.median_interval = prm_.median_interval;
         if (prm_.use_tma) ensure_tensor_maps(wk, lv, n);
         job.tmaps = wk.tmaps;
         job.c = Tvl1Consts{(float)(prm_.lambda * prm_.theta), (float)(prm_.tau / prm_.theta), (float)prm_.theta};

@@ -36,6 +36,7 @@
 #include "tma.cuh"
 #include "tvl1_fused.cuh"
 #include "tvl1_math.cuh"
+#include "tvl1_median.cuh"
 
 namespace dfb {
 
@@ -253,6 +254,22 @@ __device__ __forceinline__ void phase_merge(const int G, const int bid, const Fu
         float2 *row = reinterpret_cast<float2 *>(reinterpret_cast<char *>(job.flow_xy) + (size_t)y * job.flow_pitch_bytes);
         row[x] = make_float2(__ldcg(L.u1[cur] + o), __ldcg(L.u2[cur] + o));
     }
+}
+
+// Median filtering of the flow (DESIGN §4.3): u[cur ^ 1] = M_k(u[cur]) on the image pixels, and the dual planes move to
+// p[cur ^ 1] unchanged, so the caller's cur ^= 1 after the grid barrier carries the whole state across.  The median tiles
+// are staged in the constant planes of shared memory: the chunk that follows loads its tile whole, resident or not.
+static_assert(MedianTile<kThreads>::kStage <= kConstPlane, "median tiles fit a constant plane");
+__device__ __forceinline__ void phase_median(const int G, const int bid, const FusedJob &job, const FusedLevel &L, int cur, Smem &sm) {
+    const int total = L.h * (L.pitch >> 2);
+    for (int i = bid * kThreads + threadIdx.x; i < total; i += G * kThreads) {
+        const size_t o = (size_t)i << 2;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) st4(job.p[cur ^ 1][q] + o, ld_cg4(job.p[cur][q] + o));
+    }
+    median_planes<kThreads>(L.u1[cur], L.u2[cur], L.u1[cur ^ 1], L.u2[cur ^ 1], L.w, L.h, L.pitch, job.median_k, bid, G, sm.consts[0],
+                            sm.consts[1]);
+    fence_proxy_async();  // before the TMA tile loads that follow write these shared-memory planes
 }
 
 // ---- the register-tile inner loop -------------------------------------------------------------
@@ -777,7 +794,8 @@ __device__ __forceinline__ const FusedJob &job_of(const FusedBatch &batch, int l
     return sm.job;
 }
 
-template <class Batch>
+// MEDIAN: the handle's median filtering is on (job.median_k > 0); the default instantiation carries none of its code.
+template <class Batch, bool MEDIAN>
 __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const __grid_constant__ Batch batch) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
@@ -821,6 +839,18 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const _
             for (int r = 0; r < RPT; ++r) p11[r] = p12[r] = p21[r] = p22[r] = zero4();
             bool first = true;
             while (error > scaled_eps && n < job.iterations) {
+                if (MEDIAN && n % job.median_interval == 0) {  // the A.4 state does not change
+                    phase_median(G, bid, job, L, cur, sm);
+                    prof.mark(24);
+                    grid_barrier(bar, epoch, G, job.ctl);
+                    prof.mark(3);
+                    cur ^= 1;
+                    first = true;  // a resident tile's u and constants on chip are stale
+                    // and its dual planes are reloaded whole: ending their live range here keeps ptxas from holding the previous
+                    // chunk's values through phase_median, which then spills
+#pragma unroll
+                    for (int r = 0; r < RPT; ++r) p11[r] = p12[r] = p21[r] = p22[r] = zero4();
+                }
                 // plan the epoch: iterations up to and including the next convergence check (A.4)
                 int K = 0, nn = n;
                 bool check = false;
@@ -835,6 +865,7 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const _
                     }
                     pp -= scaled_eps;
                     if (nn >= job.iterations) break;
+                    if (MEDIAN && nn % job.median_interval == 0) break;  // a median runs before iteration nn
                 }
                 int remaining = K;
                 while (remaining > 0) {
@@ -923,6 +954,8 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_stage(const 
         phase_upsample(G, bid, job, L, job.lv[a.level - 1], 0);
     } else if (a.stage == kFusedStageMerge) {
         phase_merge(G, bid, job, L, 0);
+    } else if (a.stage == kFusedStageMedian) {
+        phase_median(G, bid, job, L, 0, sm);
     }
     lane_exit(job.sync, G);
 }
@@ -991,12 +1024,15 @@ int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, bool 
         std::lock_guard<std::mutex> lk(mtx);
         const int d = device >= 0 && device < 64 ? device : 0;
         if (!configured[d]) {
-            configure_kernel(k_tvl1_pair<FusedBatch>, "k_tvl1_pair");
-            configure_kernel(k_tvl1_pair<FusedBatchParams>, "k_tvl1_pair");
+            configure_kernel(k_tvl1_pair<FusedBatch, false>, "k_tvl1_pair");
+            configure_kernel(k_tvl1_pair<FusedBatchParams, false>, "k_tvl1_pair");
+            configure_kernel(k_tvl1_pair<FusedBatch, true>, "k_tvl1_pair");
+            configure_kernel(k_tvl1_pair<FusedBatchParams, true>, "k_tvl1_pair");
             configured[d] = true;
         }
     }
     static_assert(TW == kFusedTileW && TH == kFusedTileH, "tile geometry is shared with the host heuristics");
+    static_assert(sizeof(FusedBatchParams) <= 32764, "the jobs of a parameter-bank launch fit the kernel parameter space");
     // all CTAs must be co-resident: group * njobs <= SM count x kFusedCtasPerSm, enforced by the cooperative launch
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cooperative_config(batch, s, &attr);
@@ -1015,10 +1051,12 @@ int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, bool 
             if (!last_done[d]) DFB_CUDA(cudaEventCreateWithFlags(&last_done[d], cudaEventDisableTiming));
             else DFB_CUDA(cudaStreamWaitEvent(s, last_done[d], 0));
         }
+        const bool median = batch.host_jobs[0].median_k > 0;  // every lane of a launch has its handle's parameters
         if (batch.njobs <= kFusedParamLanes) {
-            DFB_CUDA(cudaLaunchKernelEx(&cfg, k_tvl1_pair<FusedBatchParams>, param_batch(batch)));
+            DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatchParams, true> : k_tvl1_pair<FusedBatchParams, false>,
+                                        param_batch(batch)));
         } else {
-            DFB_CUDA(cudaLaunchKernelEx(&cfg, k_tvl1_pair<FusedBatch>, batch));
+            DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatch, true> : k_tvl1_pair<FusedBatch, false>, batch));
         }
         if (serialise) DFB_CUDA(cudaEventRecord(last_done[d], s));
     }

@@ -22,7 +22,8 @@ struct FusedHostCtl {
     unsigned long long px_iters_total;  // sum over pairs of (level pixels x executed iterations)
     unsigned long long px_chunks_total; // sum over pairs of (level pixels x tile visits): 64 B of state/constant traffic each
     // CTA-0 view of where the last pair's time went, in ns (globaltimer): [0] level start, [1] warps,
-    // [2] tile compute, [3] grid barriers, [4] upsample+merge, [8+s] tile compute at scale s, [16+s] chunks at scale s
+    // [2] tile compute, [3] grid barriers, [4] upsample+merge, [8+s] tile compute at scale s, [16+s] chunks at scale s,
+    // [24] median filtering
     unsigned long long prof[32];
     // watchdog of the grid barrier: a CTA that polls the arrival counter kFusedStallPolls times (an L2 round trip each: 10-25 s)
     // records {1, blockIdx.x, barrier target, counter value, CTAs per lane, lane} here and traps, so a lost arrival surfaces
@@ -36,6 +37,7 @@ struct FusedJob {
     int flag_sync;  // 1: neighbour-warp progress counters in the tile loop, 0: CTA-wide barriers
     int use_tma;    // 1: constants + u tiles staged by TMA (cp.async.bulk.tensor.2d), 0: LDG -> STS
     int prefetch;   // 1: while a tile iterates, the CTA's next tile of the chunk is prefetched into L2 (TMA prefetch + prefetch.global.L2)
+    int median_k;   // 3 or 5: u1, u2 <- their k x k median before every iteration n of a warp with n % median_interval == 0; 0: off
     // CUtensorMap[nscales][kFusedMapsPerLevel] in global memory: I1wx, I1wy, grad, rho_c, u1[0], u2[0], u1[1], u2[1]
     const void *tmaps;
     double epsilon;
@@ -52,6 +54,7 @@ struct FusedJob {
     size_t flow_pitch_bytes;
     // bound > 0: emit the two quantised uint8 planes instead of the float2 field (PairJob)
     int bound;
+    int median_interval;  // (beside median_k and bound: both fill alignment padding, so the layout of the other fields is unchanged)
     uint8_t *qx, *qy;
     size_t q_pitch;
 };
@@ -109,6 +112,7 @@ enum FusedStage : int {
     kFusedStageChunks,      // n chunks of kk iterations at level `level` from state [0], every one checking when `check`
     kFusedStageUpsample,    // phase_upsample from level `level` (u[0]) to level `level` - 1
     kFusedStageMerge,       // phase_merge of level `level` (u[0])
+    kFusedStageMedian,      // phase_median of level `level` with window kk, u[0] -> u[1]
 };
 struct FusedStageArgs {
     int stage, level, coarsest, kk, n, check;

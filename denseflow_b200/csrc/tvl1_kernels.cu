@@ -3,6 +3,7 @@
 // tvl1_fused.cu and reuses tvl1_math.cuh).  All planes are fp32 with 128-byte-aligned rows.
 #include "tvl1.cuh"
 #include "tvl1_math.cuh"
+#include "tvl1_median.cuh"
 
 namespace dfb {
 
@@ -228,6 +229,13 @@ __global__ void k_fill(Plane dst, float v) {
     st4(dst.p + (size_t)y * dst.pitch + x0, make_float4(v, v, v, v));
 }
 
+// median filtering of the flow between iterations (tvl1_median.cuh), one 32 x 16 tile per block
+constexpr int kMedianThreads = 512;
+__global__ void __launch_bounds__(kMedianThreads) k_median(Plane u1, Plane u2, Plane d1, Plane d2, int k) {
+    __shared__ float s[2][MedianTile<kMedianThreads>::kStage];
+    median_planes<kMedianThreads>(u1.p, u2.p, d1.p, d2.p, u1.w, u1.h, u1.pitch, k, blockIdx.x, gridDim.x, s[0], s[1]);
+}
+
 // A.5: merge(u1, u2) -> CV_32FC2
 __global__ void k_merge_flow(Plane u1, Plane u2, float *flow, size_t flow_pitch_bytes) {
     const int x = blockIdx.x * BX + threadIdx.x;
@@ -302,6 +310,11 @@ void launch_sum_partials(const double *partials, int n, double *out, cudaStream_
 }
 void launch_fill(Plane dst, float v, cudaStream_t s) {
     k_fill<<<dim3(ceil_div(dst.pitch, BX * 4), ceil_div(dst.h, BY)), dim3(BX, BY), 0, s>>>(dst, v);
+    DFB_KERNEL_CHECK();
+}
+void launch_median(Plane u1, Plane u2, Plane d1, Plane d2, int k, cudaStream_t s) {
+    const int tiles = ceil_div(u1.w, kMedianTileW) * ceil_div(u1.h, MedianTile<kMedianThreads>::TH);
+    k_median<<<tiles, kMedianThreads, 0, s>>>(u1, u2, d1, d2, k);
     DFB_KERNEL_CHECK();
 }
 void launch_merge_flow(Plane u1, Plane u2, float *flow_xy, size_t flow_pitch_bytes, cudaStream_t s) {

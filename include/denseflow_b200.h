@@ -61,7 +61,10 @@ const char *dfb_last_error(const dfb_handle *h);
  * Algorithm hyper-parameters.  The reference never sets any (always create() defaults); these exist
  * for tests and benchmarks.  tvl1: "tau" and "theta" (finite, > 0), "lambda" (finite, >= 0), "nscales" (1..16), "warps"
  * (1..16), "epsilon" (finite; <= 0 = no convergence checks), "iterations" (>= 1), "scale_step" (> 0 and not above the
- * default 0.8 the workspace is sized for); engine knobs: "fused" (1 = persistent fused primal+dual kernel
+ * default 0.8 the workspace is sized for), "median_filtering" (0 [default] or 1 = off; 3 or 5 = u1 and u2 are replaced by
+ * their k x k median, replicate borders, before every iteration n of a warp with n % median_interval == 0, so every warp
+ * starts with one; an optional extra of CPU DualTVL1's kind that the reference's CUDA TV-L1 does not have) and
+ * "median_interval" (>= 1, default 30); engine knobs: "fused" (1 = persistent fused primal+dual kernel
  * [default], 0 = one kernel per half-step, the reference's launch structure), "fused_k" (iterations kept on chip per tile
  * visit, 1..8, default 8), "lanes" (pairs solved side by side per launch, 0 = auto [default], up to 64), "flag_sync" (1 =
  * neighbour-warp progress flags in the tile loop [default], 0 = CTA-wide barriers), "use_tma" (1 = TMA staging of the
@@ -397,6 +400,7 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   "tvl1_upsample"    in {u1, u2}                         out {u1, u2 (scalars[0] x scalars[1])}; scalars {dst w, dst h, lanes}
  *                      (resize to the finer level, times 1 / scale_step)
  *   "tvl1_merge"       in {u1, u2}                         out {flow x, flow y} (bound 0) or {qx, qy} as floats; scalars {bound, lanes}
+ *   "tvl1_median"      in {u1, u2}                         out {u1, u2} (their k x k median); scalars {k (3 or 5), lanes}
  *   "jpeg_padded_gray" in {gray}                           out {the plane padded to round8(w) x round8(h)}
  *   "jpeg_padded_ycc420" in {B, G, R}                      out {Y round16(dw) x round16(dh), Cb, Cr round8(ceil(dw / 2)) x
  *                      round8(ceil(dh / 2))}; scalars {dst w, dst h} (0 / 0: no resize)
@@ -434,7 +438,7 @@ int dfb_get_counters(dfb_handle *h, dfb_counters *out);
 /*
  * Where the most recent fused-tvl1 pair's device time went, in ns, as seen by CTA 0 of the persistent
  * kernel (%globaltimer): [0] level start (gradients, zeroing) [1] warps [2] tile iterations
- * [3] grid barriers (includes waiting for slower CTAs) [4] upsample + merge, [8+s] tile iterations at
+ * [3] grid barriers (includes waiting for slower CTAs) [4] upsample + merge, [24] median filtering, [8+s] tile iterations at
  * scale s, [16+s] tile visits (chunks) at scale s, for s = 0..7 only (the tile iterations of scales 8..15 count in [2] alone).
  * Zeros for other engines.  (The reference has only the
  * wall-clock summary line, src/denseflow_gpu.cpp:492-496.)

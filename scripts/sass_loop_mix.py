@@ -3,7 +3,7 @@
   python scripts/sass_loop_mix.py [variant]        variant of denseflow_b200/build.py (default: "default")
 
 Compiles tvl1_fused.cu for sm_90a with the flags of that build variant plus -lineinfo, prints what ptxas reports for
-k_tvl1_pair<FusedBatchParams> (the kernel of launches with <= 16 lanes), and counts the SASS of one tile iteration of an
+k_tvl1_pair<FusedBatchParams, false> (the kernel of launches with <= 16 lanes and no median filtering), and counts the SASS of one tile iteration of an
 interior tile (tile_iterations<false>): the lean instantiation tile_iteration<false, false>, which runs all but the last
 iteration of a checking chunk, and the ERR instantiation tile_iteration<false, true>.  An instruction belongs to an
 instantiation when its inlining chain (nvdisasm -gi) passes through that call of tile_iteration inside the
@@ -21,7 +21,7 @@ sys.path.insert(0, ROOT)
 from denseflow_b200 import build as B  # noqa: E402
 
 SRC = os.path.join(B.CSRC, "tvl1_fused.cu")
-KERNEL = "k_tvl1_pairINS_16FusedBatchParams"
+KERNEL = "k_tvl1_pairINS_16FusedBatchParamsELb0E"
 CUDA_BIN = os.path.dirname(B.NVCC)
 
 
@@ -125,7 +125,7 @@ def main():
         cubin = os.path.join(td, "tvl1_fused.cubin")
         ptxas = compile_cubin(variant, cubin)
         instrs = parse_sass(cubin)
-    print("build variant %r, k_tvl1_pair<FusedBatchParams>, sm_90a" % variant)
+    print("build variant %r, k_tvl1_pair<FusedBatchParams, false>, sm_90a" % variant)
     for l in ptxas:
         print("  ptxas: " + l)
     for n, body in enumerate(loops(instrs, cl["lean"], cl["interior"])):
