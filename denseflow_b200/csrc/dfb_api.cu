@@ -7,7 +7,6 @@
 #include <cstring>
 #include <functional>
 #include <mutex>
-#include <optional>
 #include <string>
 #include <vector>
 
@@ -63,32 +62,32 @@ struct dfb_handle {
     cudaStream_t s_in = nullptr, s_compute = nullptr, s_out = nullptr;
     cudaStream_t s_fetch = nullptr;  // file read-back of the encoding pipelines
     static constexpr int kFrameRing = 16; // device u8 frames (dead as soon as their pyramid is built)
-    static constexpr int kFlowRing = 128; // device flow / quantised outputs: two launches of up to 64 pairs in flight; slots are
-                                          // allocated on first use and a call cycles through 2 x (pairs per launch) of them
+    static constexpr int kMaxGroup = 64;  // pairs per group of the calc calls; two groups are in flight
     DeviceBuffer<uint8_t> d_frame[kFrameRing];
     size_t d_frame_pitch = 0;
-    DeviceBuffer<float> d_flow[kFlowRing];
-    DeviceBuffer<uint8_t> d_qx[kFlowRing], d_qy[kFlowRing];
     Events ev_in, ev_pyr;     // [kFrameRing] frame uploaded, its pyramid built
-    Events ev_done, ev_out;   // [kFlowRing] pair solved, its output read back
-    // pinned staging for pageable caller buffers
+    // pinned staging for pageable caller buffers (outputs: one per pair of the two groups in flight)
     PinnedBuffer<uint8_t> h_frame[kFrameRing];
-    PinnedBuffer<float> h_flow[kFlowRing];
-    PinnedBuffer<uint8_t> h_q[kFlowRing];
+    PinnedBuffer<float> h_flow[2 * kMaxGroup];
+    PinnedBuffer<uint8_t> h_q[2 * kMaxGroup];
+    // the flow group loop (flow_groups): device outputs of two slots of B pairs, grown on demand, and per slot the events
+    // that hand a solved group from s_compute to s_out and mark the slot free once its outputs are read back or encoded
+    DeviceBuffer<uint8_t> flow_out;
+    struct {
+        Events solved, freed;  // [2]
+    } flow_ev;
     std::unique_ptr<JpegEncoder> jpeg;  // nvJPEG encoder / decoder states, created on first use
     // scratch of the flow chains (dfb_process_*_batch_host), grown on demand
-    DeviceBuffer<uint8_t> pb_bgr, pb_gray, pb_frames, pb_q;
-    DeviceBuffer<float> pb_flow;  // flow fields of two groups of the -st=png chains
+    DeviceBuffer<uint8_t> pb_bgr, pb_gray, pb_frames;
     struct {
         Events frame;      // [n_frames] frame f is in pb_frames
         Events gray;       // [2] BGR staging buffer consumed
-        Events flow, enc;  // [2] a group's planes ready, its encodes done
     } chain_ev;
     DeviceBuffer<uint8_t> dec_bgr;      // BGR scratch of dfb_decode_jpeg_gray_device
     std::unique_ptr<JpegDecoder> jdec;  // imdecode-exact JPEG decoder, created on first use
     DeviceBuffer<uint8_t> png_scratch;  // min/max partials + ticket + bounds of dfb_flow_to_png_image_device
     std::unique_ptr<PngEncoder> png;    // imencode(".png") workspace and files, created on first use
-    DeviceBuffer<uint8_t> png_bgr;      // packed images of dfb_calc_batch_host_png (one per flow ring slot) and of the png chains
+    DeviceBuffer<uint8_t> png_bgr;      // packed images of the -st=png flow output, one per pair of its two slots
     TapTable gray_taps;  // dfb_resize_gray_device
     // scratch of the frame-extraction calls (-s=0), grown on demand
     TapTable ycc_taps;                // colour resize of all three calls
@@ -194,14 +193,6 @@ void ensure_streams(dfb_handle *h) {
 void ensure_fetch_stream(dfb_handle *h) {
     ensure_streams(h);
     if (!h->s_fetch) DFB_CUDA(cudaStreamCreateWithFlags(&h->s_fetch, cudaStreamNonBlocking));
-}
-
-void ensure_host_path(dfb_handle *h) {
-    ensure_streams(h);
-    h->d_frame_pitch = (size_t)round_up(h->max_w, 128);
-    for (auto &f : h->d_frame) f.allocate(h->d_frame_pitch * h->max_h);
-    h->ev_in.ensure(dfb_handle::kFrameRing);
-    h->ev_pyr.ensure(dfb_handle::kFrameRing);
 }
 
 // The x and y tables of a sw x sh -> dw x dh INTER_LINEAR resize (x: coefficients reset at the borders, y: rows clamped).
@@ -354,22 +345,6 @@ class JpegSink {
     Group group_[2] = {};
 };
 
-// output ring slots [0, n): allocated on first use (a 1080p handle runs 7 pairs per launch and touches 14 slots, a 340x256
-// one up to 64 pairs per launch)
-void ensure_flow_ring(dfb_handle *h, int n, bool quantised) {
-    h->ev_done.ensure(n);
-    h->ev_out.ensure(n);
-    const size_t px = (size_t)h->max_w * h->max_h;
-    for (int i = 0; i < n; ++i) {
-        if (quantised) {
-            h->d_qx[i].allocate(px);
-            h->d_qy[i].allocate(px);
-        } else {
-            h->d_flow[i].allocate(px * 2 * sizeof(float));
-        }
-    }
-}
-
 void ensure_png_scratch(dfb_handle *h) {
     if (h->png_scratch) return;
     h->png_scratch.allocate(png_pack_scratch_bytes());
@@ -420,98 +395,21 @@ void resize_gray(dfb_handle *h, const uint8_t *src, size_t src_pitch, int sw, in
     ++h->alg->launches;
 }
 
-// The -st=png output of a flow batch (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j];
-// every buffer holds `capacity` bytes.  The stages run on s_compute (pack), s_out (encode) and s_fetch (read-back); the caller
-// records and waits for its own events between them.
-struct PngOut {
-    uint8_t *const *out;
-    size_t capacity;
-    size_t *len;
-
-    // the pack scratch and the encoder, created on first use
-    static void prepare(dfb_handle *h) {
-        ensure_png_scratch(h);
-        if (!h->png) h->png.reset(new PngEncoder());
-    }
-    // s_compute: convertFlowToPngImage (src/common.cpp:18-46) of the m fields field(i) (w x hh float2) into m packed images
-    // from bgr, 3 w hh bytes apart
-    template <typename Field> static void pack(dfb_handle *h, int m, Field &&field, int w, int hh, uint8_t *bgr) {
-        for (int i = 0; i < m; ++i)
-            launch_flow_to_png_image(field(i), (size_t)w * 8, w, hh, bgr + (size_t)i * 3 * w * hh, (size_t)w * 3, h->png_scratch, nullptr,
-                                     h->s_compute);
-        h->alg->launches += 2 * m;
-    }
-    // s_out: imencode(".png") (:66-71) of the m packed images from bgr, as one batch into the encoder's slot
-    static void encode(dfb_handle *h, int m, const uint8_t *bgr, int w, int hh, int slot) {
-        h->alg->launches += h->png->encode(m, bgr, (size_t)3 * w * hh, (size_t)w * 3, w, hh, slot, h->s_out);
-    }
-    // once the slot's encode is complete: the files of pairs j0 .. j0 + m - 1 to the caller on s_fetch
-    void deliver(dfb_handle *h, int j0, int m, int slot) const {
-        auto reject = [&](int i, uint64_t n) {
-            if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
-            return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
-                   std::to_string(capacity);
-        };
-        auto to = [&](int i, size_t n) {
-            len[j0 + i] = n;
-            return out[j0 + i];
-        };
-        h->png->files().deliver(slot, m, capacity, reject, to, h->counters.d2h_bytes, h->s_fetch);
-    }
-};
-
-// The batch shape of calc_optflows_imp (src/denseflow_gpu.cpp:307-342) over host buffers.
-// quantise: bound > 0 => emit two u8 planes per pair instead of the float2 field.
-// png: non-null => pack every flow field (convertFlowToPngImage) and emit imencode(".png") of it instead of the field.
-int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, float *const *flows,
-               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngOut *png = nullptr) {
-    if (int rc = check_size(h, w, hh)) return rc;
-    if (n_frames < 0 || !frames) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
-    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    const int astep = std::abs(step);
-    const int M = std::max(n_frames - astep, 0);  // :308
-    if (M == 0) return DFB_OK;
-    for (int f = 0; f < n_frames; ++f)
-        if (!frames[f] || host_pointer_kind(frames[f]) < 0)
-            return fail(h, DFB_ERR_INVALID_ARG, "frames[" + std::to_string(f) + "] is null or a device pointer (host entry point: use dfb_calc_batch_device)");
-    for (int j = 0; j < M; ++j) {
-        const void *o0 = png ? (const void *)png->out[j] : bound > 0 ? (const void *)qx[j] : (const void *)flows[j];
-        const void *o1 = bound > 0 ? (const void *)qy[j] : o0;
-        if (!o0 || !o1 || host_pointer_kind(o0) < 0 || host_pointer_kind(o1) < 0)
-            return fail(h, DFB_ERR_INVALID_ARG, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-    }
-    ensure_host_path(h);
-    FlowAlgorithm &alg = *h->alg;
-    alg.begin_batch();
-    // pairs per solve_batch call; the frame slots hold one group plus the look-ahead frame
-    const int B = std::max(1, std::min(alg.max_concurrent_pairs(w, hh), dfb_handle::kFlowRing / 2));
-    alg.ensure_slots(B + astep + 1);
-    const int nslots = alg.num_slots();
-    const size_t fbytes = (size_t)w * hh;
+// Frame source of the calc calls: host frames through the handle's ring of kFrameRing device frames (pageable ones through
+// pinned staging, one H2D per frame on s_in), then ONE batched preparation per sub-batch of at most kFrameRing frames on
+// s_compute (the per-frame stages are launch-latency-bound; a ring slot is reused only after its frame has been prepared).
+// Asked for the frames up to `last`, it uploads one more, so that frame's H2D overlaps the solve.
+std::function<void(int)> upload_ring(dfb_handle *h, const uint8_t *const *frames, int n_frames, int w, int hh) {
     constexpr int FR = dfb_handle::kFrameRing;
-    const int OR = 2 * B;  // two groups of pairs in flight
-    // the unfused tvl1 schedule needs the float2 field as scratch even when only the quantised planes are wanted
-    ensure_flow_ring(h, OR, bound > 0);
-    double fused_flag = 1;
-    if (bound > 0 && alg.get_param("fused", &fused_flag) && fused_flag == 0) ensure_flow_ring(h, OR, false);
-    const size_t bgr_bytes = fbytes * 3;
-    if (png) {
-        ensure_fetch_stream(h);
-        h->png_bgr.grow(OR * bgr_bytes);
-        PngOut::prepare(h);
-    }
-    // -st=png: the files of group g (slot g & 1) are read back while the GPU works on group g + 1
-    auto png_finish = [&](int g) {
-        if (!png) return;
-        const int j0 = g * B, m = std::min(B, M - j0);
-        DFB_CUDA(cudaEventSynchronize(h->ev_out[(j0 + m - 1) % OR]));
-        png->deliver(h, j0, m, g & 1);
-    };
-
-    int uploaded = 0;  // frames [0, uploaded) have H2D + pyramid enqueued
-    auto upload_until = [&](int last) {
-        // sub-batches of at most FR frames: one H2D per frame on s_in, then ONE batched preparation on s_compute (the per-frame
-        // stages are launch-latency-bound; a device ring slot is reused only after its frame has been prepared)
+    ensure_streams(h);
+    h->d_frame_pitch = (size_t)round_up(h->max_w, 128);
+    for (auto &f : h->d_frame) f.allocate(h->d_frame_pitch * h->max_h);
+    h->ev_in.ensure(FR);
+    h->ev_pyr.ensure(FR);
+    return [=, uploaded = 0](int last) mutable {  // frames [0, uploaded) have H2D + preparation enqueued
+        const size_t fbytes = (size_t)w * hh;
+        const int nslots = h->alg->num_slots();
+        last = std::min(last + 1, n_frames - 1);
         while (uploaded <= last) {
             const int first = uploaded, cnt = std::min(last - uploaded + 1, FR);
             const uint8_t *srcs[FR];
@@ -533,89 +431,272 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
                 slots[i] = f % nslots;
             }
             DFB_CUDA(cudaStreamWaitEvent(h->s_compute, h->ev_in[(first + cnt - 1) % FR], 0));  // s_in is in order: the last covers all
-            alg.prepare_frames(cnt, srcs, h->d_frame_pitch, w, hh, slots, h->s_compute);
+            h->alg->prepare_frames(cnt, srcs, h->d_frame_pitch, w, hh, slots, h->s_compute);
             for (int i = 0; i < cnt; ++i) DFB_CUDA(cudaEventRecord(h->ev_pyr[(first + i) % FR], h->s_compute));
             uploaded += cnt;
         }
     };
+}
 
-    std::vector<int> pending_copy(OR, -1);  // pair index whose staged output still has to be memcpy'd out
-    auto drain = [&](int ring) {
-        const int j = pending_copy[ring];
-        if (j < 0) return;
-        DFB_CUDA(cudaEventSynchronize(h->ev_out[ring]));
-        if (bound > 0) {
-            std::memcpy(qx[j], h->h_q[ring], fbytes);
-            std::memcpy(qy[j], h->h_q[ring] + fbytes, fbytes);
-        } else {
-            std::memcpy(flows[j], h->h_flow[ring], fbytes * 2 * sizeof(float));
+// Frame source of the flow chains: produce(first, last) enqueues on s_in the work that leaves frames [first, last] in
+// h->pb_frames (w x hh each, dense) and records h->chain_ev.frame[f] for each; frames are requested in order.  Asked for the
+// frames up to `last`, it produces one more, so that frame's decode overlaps the solve.
+std::function<void(int)> dense_frames(dfb_handle *h, int n_frames, int w, int hh, const std::function<void(int, int)> &produce) {
+    h->pb_frames.grow((size_t)w * hh * n_frames);
+    h->chain_ev.frame.ensure(n_frames);
+    return [=, &produce, produced = 0, prepared = 0](int last) mutable {
+        const int ahead = std::min(last + 1, n_frames - 1);
+        if (produced <= ahead) {
+            produce(produced, ahead);
+            produced = ahead + 1;
         }
-        pending_copy[ring] = -1;
+        DFB_CUDA(cudaStreamWaitEvent(h->s_compute, h->chain_ev.frame[last], 0));
+        prepare_dense(*h->alg, h->pb_frames, w, hh, prepared, last, h->s_compute);
     };
+}
 
+// What the flow group loop does with the pairs it solves.  Group g fills output slot g & 1: its pair i is output pair
+// p = slot * B + i, in h->flow_out.
+struct FlowOutput {
+    std::function<void(FlowAlgorithm::PairJob &, int p)> bind;  // where the solve writes output pair p
+    std::function<void(int slot, int m)> pack;                  // optional: s_compute work on the solved group
+    std::function<void(int j0, int m, int slot)> send;          // s_out: the group's outputs leave the slot
+    std::function<void(int j0, int m, int slot)> finish;        // host, a group later: the results to the caller
+};
+
+// dfb_calc_host / dfb_calc_batch_host: pair j's float2 field to flows[j], straight into page-locked memory or through the
+// pair's pinned staging buffer, copied out once the slot has been read back.  px: pixels each pair's field reserves.
+FlowOutput host_flow_output(dfb_handle *h, float *const *flows, int B, int w, int hh, size_t px) {
+    const size_t bytes = (size_t)w * hh * 2 * sizeof(float);
+    h->flow_out.grow(2 * B * px * 2 * sizeof(float));
+    auto field = [=](int p) { return reinterpret_cast<float *>(h->flow_out + (size_t)p * px * 2 * sizeof(float)); };
+    FlowOutput o;
+    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
+        pj.flow_xy = field(p);
+        pj.flow_pitch_bytes = (size_t)w * 2 * sizeof(float);
+    };
+    o.send = [=](int j0, int m, int slot) {
+        for (int i = 0; i < m; ++i) {
+            const int j = j0 + i, p = slot * B + i;
+            float *dst = is_pinned_host(flows[j]) ? flows[j] : stage_flow(h, p);
+            DFB_CUDA(cudaMemcpyAsync(dst, field(p), bytes, cudaMemcpyDeviceToHost, h->s_out));
+            h->counters.d2h_bytes += bytes;
+        }
+    };
+    o.finish = [=](int j0, int m, int slot) {
+        for (int i = 0; i < m; ++i)
+            if (!is_pinned_host(flows[j0 + i])) {
+                DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
+                std::memcpy(flows[j0 + i], h->h_flow[slot * B + i], bytes);
+            }
+    };
+    return o;
+}
+
+// dfb_calc_batch_host_u8: the engine's merge epilogue writes pair j's two uint8 planes (bound), which go to qx[j] / qy[j] as
+// the float2 fields go to flows[j] above.  flow_xy stays null: the engines keep the field in scratch of their own.
+FlowOutput host_u8_output(dfb_handle *h, uint8_t *const *qx, uint8_t *const *qy, int bound, int B, int w, int hh, size_t px) {
+    const size_t bytes = (size_t)w * hh;
+    h->flow_out.grow(2 * B * px * 2);
+    auto plane = [=](int p, int c) { return h->flow_out + ((size_t)p * 2 + c) * px; };
+    auto direct = [=](int j) { return is_pinned_host(qx[j]) && is_pinned_host(qy[j]); };
+    FlowOutput o;
+    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
+        pj.bound = bound;
+        pj.qx = plane(p, 0);
+        pj.qy = plane(p, 1);
+        pj.q_pitch = (size_t)w;
+    };
+    o.send = [=](int j0, int m, int slot) {
+        for (int i = 0; i < m; ++i) {
+            const int j = j0 + i, p = slot * B + i;
+            const bool d = direct(j);
+            uint8_t *dx = d ? qx[j] : stage_q(h, p), *dy = d ? qy[j] : stage_q(h, p) + bytes;
+            DFB_CUDA(cudaMemcpyAsync(dx, plane(p, 0), bytes, cudaMemcpyDeviceToHost, h->s_out));
+            DFB_CUDA(cudaMemcpyAsync(dy, plane(p, 1), bytes, cudaMemcpyDeviceToHost, h->s_out));
+            h->counters.d2h_bytes += 2 * bytes;
+        }
+    };
+    o.finish = [=](int j0, int m, int slot) {
+        for (int i = 0; i < m; ++i)
+            if (!direct(j0 + i)) {
+                DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
+                std::memcpy(qx[j0 + i], h->h_q[slot * B + i], bytes);
+                std::memcpy(qy[j0 + i], h->h_q[slot * B + i] + bytes, bytes);
+            }
+    };
+    return o;
+}
+
+// -st=jpg output of a flow chain: pair j's two quantised planes (bound) as JPEGs to x[j] / y[j], their lengths to len_x[j] /
+// len_y[j]; every buffer holds `capacity` bytes
+struct JpgOut {
+    int bound, quality;
+    uint8_t *const *x, *const *y;
+    size_t capacity;
+    size_t *len_x, *len_y;
+};
+
+// The planes of JpgOut, encoded on s_out as one batch per group (src/common.cpp:56-57) and read back on s_fetch
+FlowOutput jpg_output(dfb_handle *h, const JpgOut &jo, int B, int w, int hh) {
+    // quantised planes: whole 8 x 8 blocks, so nvJPEG reads their edge padding (written by launch_pad_edges) and nothing else
+    const int qw = round_up(w, 8), qh = round_up(hh, 8);
+    const size_t qpx = (size_t)qw * qh;
+    h->flow_out.grow(qpx * 2 * 2 * B);
+    auto sink = std::make_shared<JpegSink>(h, 2 * B, 2);
+    FlowOutput o;
+    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
+        pj.bound = jo.bound;
+        pj.qx = h->flow_out + (size_t)p * 2 * qpx;
+        pj.qy = pj.qx + qpx;
+        pj.q_pitch = (size_t)qw;
+    };
+    o.send = [=](int, int m, int slot) {
+        // the group's 2 m planes: plane 2 i + c of the slot is pair i's x (c = 0) or y
+        JpegSrc src;
+        src.base = h->flow_out + (size_t)slot * B * 2 * qpx;
+        src.img_stride = qpx;
+        src.pitch = (size_t)qw;
+        if (sink->needs_padded_gray(w, hh)) {
+            launch_pad_edges(const_cast<uint8_t *>(src.base), src.pitch, src.img_stride, 2 * m, w, hh, qw, qh, h->s_out);
+            ++h->alg->launches;
+        }
+        sink->encode(slot, 2 * m, src, 1, w, hh, jo.quality, jo.capacity, h->s_out);
+    };
+    o.finish = [=](int j0, int m, int slot) {
+        DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
+        auto too_small = [&](int, size_t need) {
+            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(jo.capacity) + ")";
+        };
+        auto out = [&](int k, size_t len) {
+            const int j = j0 + (k >> 1);
+            (k & 1 ? jo.len_y : jo.len_x)[j] = len;
+            return (k & 1 ? jo.y : jo.x)[j];
+        };
+        sink->deliver(slot, 2 * m, too_small, out, h->s_fetch);
+    };
+    return o;
+}
+
+// -st=png output of a flow batch (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j];
+// every buffer holds `capacity` bytes
+struct PngOut {
+    uint8_t *const *out;
+    size_t capacity;
+    size_t *len;
+};
+
+// The files of PngOut: the flow fields in the slot, convertFlowToPngImage (src/common.cpp:18-46) of each on s_compute,
+// imencode(".png") (:66-71) of the group as one batch into encoder slot `slot` on s_out, read back on s_fetch.  px: pixels
+// each pair's field reserves.
+FlowOutput png_output(dfb_handle *h, const PngOut &po, int B, int w, int hh, size_t px) {
+    const size_t img = (size_t)3 * w * hh;
+    h->flow_out.grow(2 * B * px * 2 * sizeof(float));
+    h->png_bgr.grow(2 * B * img);
+    ensure_png_scratch(h);
+    if (!h->png) h->png.reset(new PngEncoder());
+    auto field = [=](int p) { return reinterpret_cast<float *>(h->flow_out + (size_t)p * px * 2 * sizeof(float)); };
+    FlowOutput o;
+    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
+        pj.flow_xy = field(p);
+        pj.flow_pitch_bytes = (size_t)w * 2 * sizeof(float);
+    };
+    o.pack = [=](int slot, int m) {
+        for (int p = slot * B; p < slot * B + m; ++p)
+            launch_flow_to_png_image(field(p), (size_t)w * 8, w, hh, h->png_bgr + p * img, (size_t)w * 3, h->png_scratch, nullptr, h->s_compute);
+        h->alg->launches += 2 * m;
+    };
+    o.send = [=](int, int m, int slot) {
+        h->alg->launches += h->png->encode(m, h->png_bgr + slot * B * img, img, (size_t)w * 3, w, hh, slot, h->s_out);
+    };
+    o.finish = [=](int j0, int m, int slot) {
+        DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
+        auto reject = [&](int i, uint64_t n) {
+            if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
+            return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
+                   std::to_string(po.capacity);
+        };
+        auto to = [&](int i, size_t n) {
+            po.len[j0 + i] = n;
+            return po.out[j0 + i];
+        };
+        h->png->files().deliver(slot, m, po.capacity, reject, to, h->counters.d2h_bytes, h->s_fetch);
+    };
+    return o;
+}
+
+// The batch shape of calc_optflows_imp (src/denseflow_gpu.cpp:307-342): the M = n_frames - |step| pairs in groups of B on
+// four streams, two groups in flight (the reference runs its stages as host threads around queues, include/dense_flow.h:76-80):
+//   s_in      the frame source's copies and decodes; prepare(last) leaves frames up to `last` prepared in engine slots
+//             f % num_slots(), ordered on s_compute
+//   s_compute pyramids / polynomial expansions + flow of group g into output slot g & 1, then the output's pack
+//   s_out     the output's read-back or encodes of the group
+//   s_fetch   files of group g-1 to the host while the GPU works on group g
+// Runs inside guarded(), for M > 0.
+int flow_groups(dfb_handle *h, int n_frames, int step, int w, int hh, int B, const std::function<void(int)> &prepare,
+                const FlowOutput &o) {
+    const int astep = std::abs(step);
+    const int M = n_frames - astep;  // :308
+    ensure_fetch_stream(h);
+    FlowAlgorithm &alg = *h->alg;
+    alg.begin_batch();
+    alg.ensure_slots(B + astep + 1);  // one group plus the look-ahead frame
+    const int nslots = alg.num_slots();
+    auto &ev = h->flow_ev;
+    ev.solved.ensure(2);
+    ev.freed.ensure(2);
     std::vector<FlowAlgorithm::PairJob> jobs(B);
     auto stage = [&](int g) {
-        const int j0 = g * B, m = std::min(B, M - j0);
-        // frames of this group (+ one ahead, so its H2D overlaps the solve)
-        const int last_needed = j0 + m - 1 + astep;  // pairs j0..j0+m-1 touch frames j0..j0+m-1+|step| for either sign of step
-        upload_until(std::min(last_needed + 1, n_frames - 1));
+        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
+        prepare(j0 + m - 1 + astep);  // pairs j0..j0+m-1 touch frames j0..j0+m-1+|step| for either sign of step
+        if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.freed[slot], 0));  // group g-2 has left the slot
         for (int i = 0; i < m; ++i) {
-            const int j = j0 + i;
-            const int ring = j % OR;
-            drain(ring);
-            if (j >= OR) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, h->ev_out[ring], 0));  // device output slot is free
-            FlowAlgorithm::PairJob &pj = jobs[i];
-            pj = pair_job(j, step, nslots);
-            pj.flow_xy = h->d_flow[ring];  // null in quantised mode unless the engine needs the scratch (see above)
-            pj.flow_pitch_bytes = (size_t)w * 2 * sizeof(float);
-            if (bound > 0) {  // f1: the engine's merge epilogue writes the two uint8 planes directly
-                pj.bound = bound;
-                pj.qx = h->d_qx[ring];
-                pj.qy = h->d_qy[ring];
-                pj.q_pitch = (size_t)w;
-            }
+            jobs[i] = pair_job(j0 + i, step, nslots);
+            o.bind(jobs[i], slot * B + i);
         }
         alg.solve_batch(jobs.data(), m, w, hh, h->s_compute);
-        if (png) {
-            // s_compute: convertFlowToPngImage of every pair (src/common.cpp:18-46); s_out: imencode(".png") of the group
-            // (:66-71); s_fetch: the previous group's files to the host
-            const int r0 = j0 % OR;
-            uint8_t *bgr0 = h->png_bgr + (size_t)r0 * bgr_bytes;
-            PngOut::pack(h, m, [&](int i) -> const float * { return h->d_flow[r0 + i]; }, w, hh, bgr0);
-            DFB_CUDA(cudaEventRecord(h->ev_done[r0], h->s_compute));
-            DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[r0], 0));
-            PngOut::encode(h, m, bgr0, w, hh, g & 1);
-            for (int i = 0; i < m; ++i) DFB_CUDA(cudaEventRecord(h->ev_out[r0 + i], h->s_out));
-            h->counters.pairs += m;
-            return;
-        }
-        DFB_CUDA(cudaEventRecord(h->ev_done[j0 % OR], h->s_compute));
-        DFB_CUDA(cudaStreamWaitEvent(h->s_out, h->ev_done[j0 % OR], 0));
-        for (int i = 0; i < m; ++i) {
-            const int j = j0 + i, ring = j % OR;
-            if (bound > 0) {
-                const bool direct = is_pinned_host(qx[j]) && is_pinned_host(qy[j]);
-                uint8_t *dx = direct ? qx[j] : stage_q(h, ring), *dy = direct ? qy[j] : stage_q(h, ring) + fbytes;
-                DFB_CUDA(cudaMemcpyAsync(dx, h->d_qx[ring], fbytes, cudaMemcpyDeviceToHost, h->s_out));
-                DFB_CUDA(cudaMemcpyAsync(dy, h->d_qy[ring], fbytes, cudaMemcpyDeviceToHost, h->s_out));
-                if (!direct) pending_copy[ring] = j;
-                h->counters.d2h_bytes += 2 * fbytes;
-            } else {
-                const bool direct = is_pinned_host(flows[j]);
-                DFB_CUDA(cudaMemcpyAsync(direct ? flows[j] : stage_flow(h, ring), h->d_flow[ring], fbytes * 2 * sizeof(float),
-                                         cudaMemcpyDeviceToHost, h->s_out));
-                if (!direct) pending_copy[ring] = j;
-                h->counters.d2h_bytes += fbytes * 2 * sizeof(float);
-            }
-            DFB_CUDA(cudaEventRecord(h->ev_out[ring], h->s_out));
-            ++h->counters.pairs;  // total_flows += 1 (:340)
-        }
+        if (o.pack) o.pack(slot, m);
+        DFB_CUDA(cudaEventRecord(ev.solved[slot], h->s_compute));
+        DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.solved[slot], 0));
+        o.send(j0, m, slot);
+        DFB_CUDA(cudaEventRecord(ev.freed[slot], h->s_out));
+        h->counters.pairs += m;  // total_flows += 1 (:340)
     };
-    run_groups((M + B - 1) / B, stage, png_finish);
-    DFB_CUDA(cudaStreamSynchronize(h->s_out));
-    for (int r = 0; r < OR; ++r) drain(r);
+    auto finish = [&](int g) { o.finish(g * B, std::min(B, M - g * B), g & 1); };
+    run_groups((M + B - 1) / B, stage, finish);
+    DFB_CUDA(cudaStreamSynchronize(h->s_in));
     DFB_CUDA(cudaStreamSynchronize(h->s_compute));
+    DFB_CUDA(cudaStreamSynchronize(h->s_out));
     return DFB_OK;
+}
+
+// The calc calls over host buffers.
+// quantise: bound > 0 => emit two u8 planes per pair instead of the float2 field.
+// png: non-null => pack every flow field (convertFlowToPngImage) and emit imencode(".png") of it instead of the field.
+int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, float *const *flows,
+               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngOut *png = nullptr) {
+    if (int rc = check_size(h, w, hh)) return rc;
+    if (n_frames < 0 || !frames) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
+    if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
+    const int M = std::max(n_frames - std::abs(step), 0);  // :308
+    if (M == 0) return DFB_OK;
+    for (int f = 0; f < n_frames; ++f)
+        if (!frames[f] || host_pointer_kind(frames[f]) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "frames[" + std::to_string(f) + "] is null or a device pointer (host entry point: use dfb_calc_batch_device)");
+    for (int j = 0; j < M; ++j) {
+        const void *o0 = png ? (const void *)png->out[j] : bound > 0 ? (const void *)qx[j] : (const void *)flows[j];
+        const void *o1 = bound > 0 ? (const void *)qy[j] : o0;
+        if (!o0 || !o1 || host_pointer_kind(o0) < 0 || host_pointer_kind(o1) < 0)
+            return fail(h, DFB_ERR_INVALID_ARG, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
+    }
+    const int B = std::max(1, std::min(h->alg->max_concurrent_pairs(w, hh), dfb_handle::kMaxGroup));
+    // output slots at the handle's maximum frame, so that calls of other sizes reuse them (a 1080p handle runs 7 pairs per
+    // group, a 340x256 one up to 64)
+    const size_t px = (size_t)h->max_w * h->max_h;
+    const FlowOutput o = png ? png_output(h, *png, B, w, hh, px)
+                         : bound > 0 ? host_u8_output(h, qx, qy, bound, B, w, hh, px)
+                                     : host_flow_output(h, flows, B, w, hh, px);
+    return flow_groups(h, n_frames, step, w, hh, B, upload_ring(h, frames, n_frames, w, hh), o);
 }
 
 }  // namespace
@@ -973,15 +1054,6 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
 
 namespace {
 
-// -st=jpg output of a flow chain: pair j's two quantised planes (bound) as JPEGs to x[j] / y[j], their lengths to len_x[j] /
-// len_y[j]; every buffer holds `capacity` bytes
-struct JpgOut {
-    int bound, quality;
-    uint8_t *const *x, *const *y;
-    size_t capacity;
-    size_t *len_x, *len_y;
-};
-
 // Where the files of a flow chain go: exactly one of the two is set.
 struct ChainOut {
     const JpgOut *jpg;
@@ -1006,128 +1078,12 @@ int check_chain_outputs(dfb_handle *h, int M, const ChainOut &o) {
     return DFB_OK;
 }
 
-// The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) -> flow -> the output of `o`: quantise and two
-// JPEGs per pair, or convertFlowToPngImage and one PNG per pair.  `produce(first, last)` enqueues on s_in the work that leaves
-// frames [first, last] in h->pb_frames (dw x dh each, dense) and records h->chain_ev.frame[f] for each; frames are requested in
-// order.  Runs inside guarded().
+// The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) by `produce` (dense_frames) -> flow -> the
+// output of `o`: quantise and two JPEGs per pair, or convertFlowToPngImage and one PNG per pair.  Runs inside guarded().
 int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const ChainOut &o, const std::function<void(int, int)> &produce) {
-    const int astep = std::abs(step);
-    const int M = std::max(n_frames - astep, 0);
-    ensure_host_path(h);
-    ensure_fetch_stream(h);
-    FlowAlgorithm &alg = *h->alg;
-    alg.begin_batch();
-    // Three stages on three streams, groups of B pairs in flight (the reference runs the same three stages as three host
-    // threads around queues, include/dense_flow.h:76-80):
-    //   s_in      the frame source: decoded frames -> gray -> resize into the gray frame array (decode stage, :154-170)
-    //   s_compute pyramids / polynomial expansions + flow of group g, quantised planes out   (:313-342 + src/common.cpp:4-16)
-    //             (-st=png: the flow fields, then convertFlowToPngImage of each               src/common.cpp:18-46)
-    //   s_out     the group's encodes, as one batch: two JPEGs per pair (src/common.cpp:56-57) or one PNG (:66-71)
-    //   s_fetch   files of group g-1 to the host while the GPU works on group g
-    const int B = std::max(1, std::min(alg.max_concurrent_pairs(dw, dh), 8));
-    const size_t fpx = (size_t)dw * dh;
-    // quantised planes: whole 8 x 8 blocks, so nvJPEG reads their edge padding (written by launch_pad_edges) and nothing else
-    const int qw = round_up(dw, 8), qh = round_up(dh, 8);
-    const size_t qpx = (size_t)qw * qh;
-    h->pb_frames.grow(fpx * n_frames);
-    if (o.png) {
-        h->pb_flow.grow(fpx * 2 * sizeof(float) * 2 * B);  // float2 fields of two groups
-        h->png_bgr.grow(fpx * 3 * 2 * B);    // their packed images
-        PngOut::prepare(h);
-    } else {
-        h->pb_q.grow(qpx * 2 * 2 * B);  // quantised planes of two groups
-    }
-    alg.ensure_slots(B + astep + 1);
-    const int nslots = alg.num_slots();
-    auto &ev = h->chain_ev;
-    ev.frame.ensure(n_frames);
-    ev.gray.ensure(2);
-    ev.flow.ensure(2);
-    ev.enc.ensure(2);
-    std::optional<JpegSink> sink;
-    if (o.jpg) sink.emplace(h, 2 * B, 2);
-    // the group's 2 m planes, encoded as one batch: plane 2 i + c of the slot is pair i's x (c = 0) or y
-    auto group_planes = [&](int slot) {
-        JpegSrc src;
-        src.base = h->pb_q + (size_t)slot * B * 2 * qpx;
-        src.img_stride = qpx;
-        src.pitch = (size_t)qw;
-        return src;
-    };
-    // pair i of slot's group: its flow field and packed image (-st=png)
-    auto field = [&](int slot, int i) { return h->pb_flow + ((size_t)slot * B + i) * 2 * fpx; };
-    auto image = [&](int slot, int i) { return h->png_bgr + ((size_t)slot * B + i) * 3 * fpx; };
-
-    int uploaded = 0;
-    auto upload_until = [&](int last) {
-        last = std::min(last, n_frames - 1);
-        if (uploaded > last) return;
-        produce(uploaded, last);
-        uploaded = last + 1;
-    };
-    int prepared = 0;
-    std::vector<FlowAlgorithm::PairJob> jobs(B);
-    auto flow_group = [&](int g) {
-        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
-        const int last_frame = j0 + m - 1 + astep;
-        upload_until(last_frame + 1);
-        DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.frame[last_frame], 0));
-        if (g >= 2) DFB_CUDA(cudaStreamWaitEvent(h->s_compute, ev.enc[slot], 0));  // the outputs of group g-2 have been encoded
-        prepare_dense(alg, h->pb_frames, dw, dh, prepared, last_frame, h->s_compute);
-        for (int i = 0; i < m; ++i) {
-            FlowAlgorithm::PairJob &pj = jobs[i];
-            pj = pair_job(j0 + i, step, nslots);
-            if (o.png) {
-                pj.flow_xy = field(slot, i);
-                pj.flow_pitch_bytes = (size_t)dw * 2 * sizeof(float);
-            } else {
-                pj.bound = o.jpg->bound;
-                pj.qx = h->pb_q + ((size_t)(slot * B + i) * 2) * qpx;
-                pj.qy = pj.qx + qpx;
-                pj.q_pitch = (size_t)qw;
-            }
-        }
-        alg.solve_batch(jobs.data(), m, dw, dh, h->s_compute);
-        if (o.png) PngOut::pack(h, m, [&](int i) { return field(slot, i); }, dw, dh, image(slot, 0));
-        DFB_CUDA(cudaEventRecord(ev.flow[slot], h->s_compute));
-        // encode stage (src/common.cpp:48-71)
-        DFB_CUDA(cudaStreamWaitEvent(h->s_out, ev.flow[slot], 0));
-        if (o.png) {
-            PngOut::encode(h, m, image(slot, 0), dw, dh, slot);
-        } else {
-            const JpegSrc src = group_planes(slot);
-            if (sink->needs_padded_gray(dw, dh)) {
-                launch_pad_edges(const_cast<uint8_t *>(src.base), src.pitch, src.img_stride, 2 * m, dw, dh, qw, qh, h->s_out);
-                ++alg.launches;
-            }
-            sink->encode(slot, 2 * m, src, 1, dw, dh, o.jpg->quality, o.jpg->capacity, h->s_out);
-        }
-        DFB_CUDA(cudaEventRecord(ev.enc[slot], h->s_out));
-        h->counters.pairs += m;
-    };
-    auto finish_group = [&](int g) {
-        const int j0 = g * B, m = std::min(B, M - j0), slot = g & 1;
-        DFB_CUDA(cudaEventSynchronize(ev.enc[slot]));
-        if (o.png) {
-            o.png->deliver(h, j0, m, slot);
-            return;
-        }
-        const JpgOut &jo = *o.jpg;
-        auto too_small = [&](int, size_t need) {
-            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(jo.capacity) + ")";
-        };
-        auto out = [&](int k, size_t len) {
-            const int j = j0 + (k >> 1);
-            (k & 1 ? jo.len_y : jo.len_x)[j] = len;
-            return (k & 1 ? jo.y : jo.x)[j];
-        };
-        sink->deliver(slot, 2 * m, too_small, out, h->s_fetch);
-    };
-    run_groups((M + B - 1) / B, flow_group, finish_group);
-    DFB_CUDA(cudaStreamSynchronize(h->s_in));
-    DFB_CUDA(cudaStreamSynchronize(h->s_compute));
-    DFB_CUDA(cudaStreamSynchronize(h->s_out));
-    return DFB_OK;
+    const int B = std::max(1, std::min(h->alg->max_concurrent_pairs(dw, dh), 8));
+    const FlowOutput out = o.png ? png_output(h, *o.png, B, dw, dh, (size_t)dw * dh) : jpg_output(h, *o.jpg, B, dw, dh);
+    return flow_groups(h, n_frames, step, dw, dh, B, dense_frames(h, n_frames, dw, dh, produce), out);
 }
 
 // Every file of a JPEG batch parsed on the host; an unsupported or corrupt header is the call's error.
@@ -1187,6 +1143,7 @@ int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, 
         const size_t fpx = (size_t)dw * dh, bgr_bytes = (size_t)sw * sh * 3;
         h->pb_bgr.grow(2 * bgr_bytes);  // two staging frames: H2D of f+1 overlaps gray/resize of f
         h->pb_gray.grow((size_t)sw * sh);
+        h->chain_ev.gray.ensure(2);
         auto produce = [&](int first, int last) {
             auto &ev = h->chain_ev;
             for (int f = first; f <= last; ++f) {

@@ -209,6 +209,12 @@ def test_every_entry_point_at_every_geometry(oracle, case, variant):
     iters = e.tvl1_stats()[0] if alg == "tvl1" else None
     note = _pin_to_oracle(oracle, e, alg, variant, fr, flow, iters, tag)
     _host_batches(e, fr, host, tag)
+    if alg == "tvl1":  # groups of 2 pairs: a call of 5 or more pairs reuses the output slots of its two groups in flight
+        e.set("lanes", 2)
+        try:
+            _host_batches(e, fr, host, tag + " lanes 2")
+        finally:
+            e.set("lanes", 0)
     _device_calls(e, alg, fr, host, tag)
     pin.finish([note])
 
