@@ -16,7 +16,11 @@
 //             until no record changes (the records then equal the sequential decode's, by induction over t).  A scan of
 //             the blocks each subsequence completes gives block indices; a final pass writes de-zig-zagged coefficients
 //             and DC differences, and two more scans turn the differences into absolute DC per component and segment.
-//   k_idct    jpeg_idct_islow per block into component planes padded to whole MCUs
+//   k_idct    jpeg_idct_islow per block into component planes padded to whole MCUs; refuses dequantised values past
+//             kMaxDequant (the most an 8-bit encoder writes) and outputs past -512..511
+//   errors    a frame's status holds, per restart interval, the first error in decode order (an invalid code whose 16-bit
+//             look-ahead runs past the interval's end counts as the interval ending early); the message ranks RST number,
+//             RST count, invalid code, early end, no marker after the data, then out-of-range coefficients
 //   k_color   one thread per 2 x 2 output block: libjpeg's upsampling (fancy h2v1 / h1v2 / h2v2, box when the chroma
 //             plane is at most 2 samples wide for the h2 cases), ycc_rgb_convert, written as BGR, or as BGR2GRAY of it.
 #include <cstring>
@@ -33,7 +37,11 @@ constexpr int kWarmup = 8;      // subsequences decoded from a guess before a st
 constexpr int kDT = 512;        // threads of k_destuff
 constexpr int kDB = 16;         // bytes per thread and tile of k_destuff
 
-enum : int { kErrCode = 1, kErrShort = 2, kErrRst = 4, kErrRstCount = 8 };
+enum : int { kErrCode = 1, kErrShort = 2, kErrRst = 4, kErrRstCount = 8, kErrRange = 16, kErrNoEnd = 32 };
+
+// The largest |coefficient x quantisation value| libjpeg's islow forward DCT and quantiser produce from 8-bit samples at any
+// table entry (DESIGN §7).  Past it imdecode's pixels depend on how libjpeg-turbo was built, so the file is refused.
+constexpr int kMaxDequant = 2048;
 
 struct HuffTab {
     uint16_t fast[512];  // 9-bit look-ahead -> (length << 8) | symbol, length 0: a longer code
@@ -130,6 +138,7 @@ __global__ void __launch_bounds__(kDT) k_destuff(const uint8_t *__restrict__ raw
     }
     if (rcarry != f.nseg - 1) bad |= kErrRstCount;
     if (bad) atomicOr(&status[blockIdx.x], bad);
+    if (end == L && threadIdx.x == 0) atomicOr(&status[blockIdx.x], kErrNoEnd);  // no marker after the data; it still decodes
     const bool fbad = __syncthreads_or(bad != 0);
     // segments and their subsequences; a frame with a bad marker sequence decodes nothing (its status is already set)
     int sub_carry = 0;
@@ -207,7 +216,8 @@ __device__ int run_decode(const uint8_t *ds, uint64_t seg_bit0, uint32_t seg_bit
                     break;
                 }
             }
-            if (!len) return kRunBadCode;
+            // a code that matches nothing only because of bits past the segment's end is the segment ending early
+            if (!len) return R.pos + 16 > seg_bits ? kRunOverrun : kRunBadCode;
         }
         const int nb = R.zz == 0 ? sym : (sym & 15);
         if (R.pos + len + nb > seg_bits) return kRunOverrun;
@@ -269,7 +279,7 @@ struct EntropyArgs {
     const int *seg_sub_base, *seg_nsub, *seg_start, *seg_bytes, *seg_frame, *seg_nblocks;
     const long long *seg_first_block;
     uint64_t *st;
-    int *cnt, *ndc, *dcsum, *dcbase;
+    int *cnt, *ndc, *dcsum, *dcbase, *err;
     long long *blk_off, *first_dc;
     int16_t *coef;
     int *status;
@@ -333,7 +343,8 @@ __global__ void __launch_bounds__(128) k_sync_round(EntropyArgs a, int *changed)
 }
 
 // one warp per segment: exclusive scans over its subsequences.  mode 0: block index of each subsequence's first block (from
-// the blocks the subsequences complete); mode 1: the DC predictor of each component at each subsequence's start.
+// the blocks the subsequences complete); mode 1: the DC predictor of each component at each subsequence's start, and the
+// segment's first error in decode order goes to its frame's status (a subsequence after it started from a guess).
 __global__ void __launch_bounds__(128) k_seg_scan(EntropyArgs a, int n_seg, int mode) {
     const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (s >= n_seg) return;
@@ -359,6 +370,13 @@ __global__ void __launch_bounds__(128) k_seg_scan(EntropyArgs a, int n_seg, int 
             }
             carry[c] += __shfl_sync(0xffffffffu, x, 31);
         }
+        if (mode) {
+            const unsigned m = __ballot_sync(0xffffffffu, k < n && a.err[b + k] != 0);
+            if (m) {
+                if (lane == __ffs(m) - 1) atomicOr(&a.status[a.seg_frame[s]], a.err[b + k]);
+                break;
+            }
+        }
     }
 }
 
@@ -380,11 +398,9 @@ __global__ void __launch_bounds__(128) k_decode_final(EntropyArgs a) {
     a.ndc[t] = R.ndc;
 #pragma unroll
     for (int i = 0; i < 3; ++i) a.dcsum[(size_t)t * 3 + i] = R.dcsum[i];
-    if (a.status[c.frame] & (kErrRst | kErrRstCount)) return;
-    if (rc == kRunBadCode)
-        atomicOr(&a.status[c.frame], kErrCode);
-    else if (rc != kRunBlocksDone && R.done < max_blocks && (last || rc == kRunOverrun))
-        atomicOr(&a.status[c.frame], kErrShort);
+    a.err[t] = rc == kRunBadCode                                                                 ? kErrCode
+               : rc != kRunBlocksDone && R.done < max_blocks && (last || rc == kRunOverrun) ? kErrShort
+                                                                                            : 0;
 }
 
 // absolute DC: each subsequence adds its components' predictors to the differences it decoded
@@ -404,18 +420,20 @@ __global__ void __launch_bounds__(128) k_dc_fix(EntropyArgs a) {
     }
 }
 
-// jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2) of one 8-point column / row
-struct Idct8 {
-    int o[8];
-    __device__ __forceinline__ Idct8(int c0, int c1, int c2, int c3, int c4, int c5, int c6, int c7) {
-        int z1 = (c2 + c6) * 4433;
-        const int tmp2 = z1 + c6 * -15137, tmp3 = z1 + c2 * 6270;
-        const int tmp0 = (c0 + c4) * 8192, tmp1 = (c0 - c4) * 8192;
-        const int t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
-        int o0 = c7, o1 = c5, o2 = c3, o3 = c1;
+// jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2) of one 8-point column / row.  T: int for the columns (inputs within
+// kMaxDequant + 1 stay far from overflow), long long for the rows (a damaged block's columns can reach ~2^16, whose
+// products pass 2^31)
+template <typename T> struct Idct8 {
+    T o[8];
+    __device__ __forceinline__ Idct8(T c0, T c1, T c2, T c3, T c4, T c5, T c6, T c7) {
+        T z1 = (c2 + c6) * 4433;
+        const T tmp2 = z1 + c6 * -15137, tmp3 = z1 + c2 * 6270;
+        const T tmp0 = (c0 + c4) * 8192, tmp1 = (c0 - c4) * 8192;
+        const T t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+        T o0 = c7, o1 = c5, o2 = c3, o3 = c1;
         z1 = o0 + o3;
-        int z2 = o1 + o2, z3 = o0 + o2, z4 = o1 + o3;
-        const int z5 = (z3 + z4) * 9633;
+        T z2 = o1 + o2, z3 = o0 + o2, z4 = o1 + o3;
+        const T z5 = (z3 + z4) * 9633;
         o0 *= 2446;
         o1 *= 16819;
         o2 *= 25172;
@@ -449,9 +467,11 @@ __device__ __forceinline__ int find_frame(const JFrame *F, int n, long long b) {
 }
 
 // one thread per block: dequantise, inverse DCT, range limit (the post-IDCT table of jdmaster.c: the value masked to 10 bits
-// as a signed number, + 128, clamped), into the component plane
+// as a signed number, + 128, clamped), into the component plane.  A dequantised value past kMaxDequant, or an output past
+// -512..511 (where the table wraps and libjpeg-turbo's SIMD IDCT saturates instead), sets kErrRange; the IDCT runs on
+// values clamped to kMaxDequant + 1, so it cannot overflow (the frame is refused anyway).
 __global__ void __launch_bounds__(128) k_idct(const int16_t *__restrict__ coef, const JFrame *__restrict__ F, int n, long long n_blocks,
-                                              const int32_t *__restrict__ quant, uint8_t *__restrict__ planes) {
+                                              const int32_t *__restrict__ quant, uint8_t *__restrict__ planes, int *status) {
     const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= n_blocks) return;
     const int fi = find_frame(F, n, b);
@@ -462,6 +482,7 @@ __global__ void __launch_bounds__(128) k_idct(const int16_t *__restrict__ coef, 
     const int bx = (mcu % f.mcux) * f.ch[ci] + f.lay_bx[k], by = (mcu / f.mcux) * f.cv[ci] + f.lay_by[k];
     const int32_t *q = quant + (size_t)(fi * 4 + f.q[ci]) * 64;
     int c[64];
+    bool out_of_range = false;
     const int4 *src = reinterpret_cast<const int4 *>(coef + b * 64);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -469,31 +490,39 @@ __global__ void __launch_bounds__(128) k_idct(const int16_t *__restrict__ coef, 
         const int w4[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            c[i * 8 + 2 * j] = (int)(int16_t)(w4[j] & 0xFFFF) * __ldg(q + i * 8 + 2 * j);
-            c[i * 8 + 2 * j + 1] = (int)(int16_t)((uint32_t)w4[j] >> 16) * __ldg(q + i * 8 + 2 * j + 1);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int d = (int)(int16_t)(h ? (uint32_t)w4[j] >> 16 : w4[j] & 0xFFFF) * __ldg(q + i * 8 + 2 * j + h);
+                out_of_range |= d > kMaxDequant || d < -kMaxDequant;
+                c[i * 8 + 2 * j + h] = min(max(d, -kMaxDequant - 1), kMaxDequant + 1);
+            }
         }
     }
     int ws[64];
 #pragma unroll
     for (int x = 0; x < 8; ++x) {  // pass 1: columns
-        const Idct8 d(c[x], c[8 + x], c[16 + x], c[24 + x], c[32 + x], c[40 + x], c[48 + x], c[56 + x]);
+        const Idct8<int> d(c[x], c[8 + x], c[16 + x], c[24 + x], c[32 + x], c[40 + x], c[48 + x], c[56 + x]);
 #pragma unroll
         for (int y = 0; y < 8; ++y) ws[y * 8 + x] = (d.o[y] + (1 << 10)) >> 11;
     }
     uint8_t *dst = planes + f.plane_off[ci] + (size_t)(by * 8) * f.plane_pitch[ci] + bx * 8;
 #pragma unroll
     for (int y = 0; y < 8; ++y) {  // pass 2: rows
-        const Idct8 d(ws[y * 8], ws[y * 8 + 1], ws[y * 8 + 2], ws[y * 8 + 3], ws[y * 8 + 4], ws[y * 8 + 5], ws[y * 8 + 6], ws[y * 8 + 7]);
+        const Idct8<long long> d(ws[y * 8], ws[y * 8 + 1], ws[y * 8 + 2], ws[y * 8 + 3], ws[y * 8 + 4], ws[y * 8 + 5], ws[y * 8 + 6],
+                                 ws[y * 8 + 7]);
         uint32_t lo = 0, hi = 0;
 #pragma unroll
         for (int x = 0; x < 8; ++x) {
-            const int v = (d.o[x] + (1 << 17)) >> 18;
+            const long long v64 = (d.o[x] + (1 << 17)) >> 18;
+            out_of_range |= v64 < -512 || v64 > 511;
+            const int v = (int)v64;
             const int s = ((v & 1023) ^ 512) - 512;
             const uint32_t px = (uint32_t)min(max(s + 128, 0), 255);
             if (x < 4) lo |= px << (8 * x); else hi |= px << (8 * (x - 4));
         }
         *reinterpret_cast<uint2 *>(dst + (size_t)y * f.plane_pitch[ci]) = make_uint2(lo, hi);
     }
+    if (out_of_range) atomicOr(&status[fi], kErrRange);
 }
 
 // libjpeg's upsampled chroma sample at output (x, y) of a plane of cw x ch samples (fh, fv: 1 or 2)
@@ -761,7 +790,7 @@ struct JpegDecoder::Layout {
     size_t raw_bytes = 0, plane_bytes = 0;
     // offsets into the workspace; [0, upload) is copied from the staging buffer
     size_t o_frames, o_tabs, o_quant, o_seg_frame, o_seg_first, o_seg_nblocks, o_raw, upload;
-    size_t o_ds, o_seg_start, o_seg_bytes, o_seg_sub_base, o_seg_nsub, o_sub_seg, o_st, o_cnt, o_ndc, o_dcsum, o_dcbase, o_blk_off,
+    size_t o_ds, o_seg_start, o_seg_bytes, o_seg_sub_base, o_seg_nsub, o_sub_seg, o_st, o_cnt, o_ndc, o_dcsum, o_dcbase, o_err, o_blk_off,
         o_first_dc, o_status, o_flag, o_coef, o_planes, total;
 };
 
@@ -850,6 +879,7 @@ void JpegDecoder::run_entropy(const uint8_t *const *jpeg, const size_t *len, con
     Y.o_ndc = take(sizeof(int) * nsub);
     Y.o_dcsum = take(sizeof(int) * 3 * nsub);
     Y.o_dcbase = take(sizeof(int) * 3 * nsub);
+    Y.o_err = take(sizeof(int) * nsub);
     Y.o_blk_off = take(sizeof(long long) * nsub);
     Y.o_first_dc = take(sizeof(long long) * nsub);
     Y.o_status = take(sizeof(int) * (n + 1));
@@ -907,6 +937,7 @@ void JpegDecoder::run_entropy(const uint8_t *const *jpeg, const size_t *len, con
     a.ndc = reinterpret_cast<int *>(W + Y.o_ndc);
     a.dcsum = reinterpret_cast<int *>(W + Y.o_dcsum);
     a.dcbase = reinterpret_cast<int *>(W + Y.o_dcbase);
+    a.err = reinterpret_cast<int *>(W + Y.o_err);
     a.blk_off = reinterpret_cast<long long *>(W + Y.o_blk_off);
     a.first_dc = reinterpret_cast<long long *>(W + Y.o_first_dc);
     a.coef = reinterpret_cast<int16_t *>(W + Y.o_coef);
@@ -956,6 +987,8 @@ void JpegDecoder::check_status(int n, cudaStream_t s, int index_base) {
         if (e & kErrRstCount) corrupt(f, "the number of RST markers does not match the restart interval (truncated or corrupt data)");
         if (e & kErrCode) corrupt(f, "invalid Huffman code in the entropy-coded data");
         if (e & kErrShort) corrupt(f, "entropy-coded data ends before the last MCU");
+        if (e & kErrNoEnd) corrupt(f, "entropy-coded data is not ended by a marker (truncated file)");
+        if (e & kErrRange) corrupt(f, "dequantised DCT coefficient or IDCT output out of range (corrupt data)");
     }
 }
 
@@ -967,7 +1000,8 @@ void JpegDecoder::decode(const uint8_t *const *jpeg, const size_t *len, const Jp
     const JFrame *F = reinterpret_cast<const JFrame *>(d_ws + Y.o_frames);
     if (Y.n_blocks > 0) {
         k_idct<<<(unsigned)((Y.n_blocks + 127) / 128), 128, 0, s>>>(reinterpret_cast<const int16_t *>(d_ws + Y.o_coef), F, n, Y.n_blocks,
-                                                                   reinterpret_cast<const int32_t *>(d_ws + Y.o_quant), d_ws + Y.o_planes);
+                                                                   reinterpret_cast<const int32_t *>(d_ws + Y.o_quant), d_ws + Y.o_planes,
+                                                                   reinterpret_cast<int *>(d_ws + Y.o_status));
         DFB_KERNEL_CHECK();
     }
     int mw = 0, mh = 0;

@@ -205,9 +205,12 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
  * 1x1 with luma h, v in {1, 2} (4:4:4, 4:2:2, 4:4:0, 4:2:0); 8- or 16-bit DQT tables; DRI / RST0-7; APPn and COM
  * segments are skipped.  DFB_ERR_UNSUPPORTED, with a message naming the feature, for progressive, arithmetic-coded,
  * lossless or 12-bit files, multi-scan files, other samplings (4:1:1, ...), RGB-coded or CMYK files and an EXIF
- * orientation other than 1 (imread would rotate the image).  DFB_ERR_INVALID_ARG, naming the frame, for corrupt data: an
- * invalid Huffman code, data that ends before the last MCU, a wrong RST sequence (libjpeg warns and makes up pixels there;
- * these calls refuse instead).  Progressive files still decode, approximately, through dfb_decode_jpeg_gray_device.
+ * orientation other than 1 (imread would rotate the image).  DFB_ERR_INVALID_ARG, naming the frame, for a damaged header
+ * and for corrupt data: an invalid Huffman code, data that ends before the last MCU, a wrong RST sequence or count (libjpeg
+ * warns and makes up pixels there; these calls refuse instead), a scan not ended by a marker, and a dequantised
+ * coefficient past 2048 or an IDCT output past -512..511 (no 8-bit encoder writes the first; past either, imdecode's
+ * pixels depend on how libjpeg-turbo was built).  Progressive files still decode, approximately, through
+ * dfb_decode_jpeg_gray_device.
  *
  * dfb_decode_jpeg_batch_device: n files (host buffers jpeg[i] of len[i] bytes; sizes and samplings may differ).
  * channels 3: imdecode(IMREAD_COLOR), packed BGR; channels 1: cvtColor(BGR2GRAY) of it (the frame the flow sees).  Frame i

@@ -7,8 +7,10 @@ The subset, and the two exceptions it raises:
 * 1 component, or 3 that libjpeg treats as YCbCr (JFIF marker, Adobe transform 1, or component ids 1-2-3);
 * chroma sampled 1 x 1, luma h, v in {1, 2};
 * no EXIF orientation other than 1 (imdecode would rotate).
-Anything else raises `Unsupported`.  Corrupt entropy data (an invalid code, data that ends before the last MCU, a wrong
-RST sequence) raises `Corrupt`: libjpeg warns and fills in pixels there, the decoder refuses instead.
+Anything else raises `Unsupported`.  A damaged header, corrupt entropy data (an invalid code, data that ends before the last
+MCU, a wrong RST sequence or count) and dequantised coefficients past MAX_DEQUANT raise `Corrupt`: libjpeg warns and fills in
+pixels there (or, past MAX_DEQUANT, gives pixels that depend on its build), the decoder refuses instead.  `parse` makes the
+decoder's header checks in its order, with its messages.
 """
 import numpy as np
 
@@ -33,22 +35,22 @@ class Huffman:
     def __init__(self, counts, symbols, is_dc):
         if sum(counts) > 256 or sum(counts) != len(symbols):
             raise Corrupt("bad Huffman table")
-        if is_dc and any(s > 15 for s in symbols):
-            raise Corrupt("bad Huffman table")
         self.counts, self.symbols = list(counts), list(symbols)
         self.length = np.zeros(1 << 16, np.int64)
         self.symbol = np.zeros(1 << 16, np.int64)
         code, k = 0, 0
         for l in range(1, 17):
             for _ in range(counts[l - 1]):
-                if code >= (1 << l):
-                    raise Corrupt("bad Huffman table")
                 lo, hi = code << (16 - l), (code + 1) << (16 - l)
                 self.length[lo:hi] = l
                 self.symbol[lo:hi] = symbols[k]
                 code += 1
                 k += 1
+            if counts[l - 1] and code >= (1 << l):  # jpeg_make_d_derived_tbl: no code may be all ones
+                raise Corrupt("bad Huffman table")
             code <<= 1
+        if is_dc and any(s > 15 for s in symbols):
+            raise Corrupt("bad Huffman table")
 
 
 def _u16(b, i):
@@ -85,7 +87,8 @@ SOF_NAMES = {0xC2: "progressive", 0xC3: "lossless", 0xC5: "differential sequenti
 
 
 def parse(buf):
-    """Markers up to the start of the entropy-coded data.  Returns a dict describing the frame and its one scan."""
+    """Markers up to the start of the entropy-coded data, checked in the decoder's order with its messages.  Returns a dict
+    describing the frame and its one scan."""
     b = bytes(buf)
     if len(b) < 4 or b[0] != 0xFF or b[1] != 0xD8:
         raise Corrupt("not a JPEG file (no SOI marker)")
@@ -103,7 +106,7 @@ def parse(buf):
         m = b[i]
         i += 1
         if m == 0xD8 or m == 0xD9 or 0xD0 <= m <= 0xD7 or m == 0x01:
-            raise Corrupt("unexpected marker 0x%02X before the scan" % m)
+            raise Corrupt("unexpected marker before the scan")
         L = _u16(b, i)
         if L < 2 or i + L > len(b):
             raise Corrupt("marker segment runs past the end of the file")
@@ -112,19 +115,29 @@ def parse(buf):
         if m in SOF_NAMES:
             raise Unsupported("%s JPEG (SOF%d) is not supported" % (SOF_NAMES[m], m - 0xC0))
         if m in (0xC0, 0xC1):
+            if len(p) < 6:
+                raise Corrupt("short frame header")
             prec, h, w, nf = p[0], _u16(p, 1), _u16(p, 3), p[5]
             if prec != 8:
                 raise Unsupported("%d-bit samples are not supported (8-bit only)" % prec)
+            if nf == 4:
+                raise Unsupported("CMYK / 4-component JPEG is not supported")
+            if nf not in (1, 3):
+                raise Unsupported("%d-component JPEG is not supported" % nf)
+            if len(p) < 6 + 3 * nf:
+                raise Corrupt("short frame header")
             comps = [dict(id=p[6 + 3 * k], h=p[7 + 3 * k] >> 4, v=p[7 + 3 * k] & 15, tq=p[8 + 3 * k]) for k in range(nf)]
             sof = dict(w=w, h=h, comps=comps)
         elif m == 0xC4:
             o = 0
             while o < len(p):
+                if o + 17 > len(p):
+                    raise Corrupt("short DHT segment")
                 tc, th = p[o] >> 4, p[o] & 15
-                counts = list(p[o + 1:o + 17])
-                syms = list(p[o + 17:o + 17 + sum(counts)])
                 if th > 3 or tc > 1:
                     raise Corrupt("bad DHT table id")
+                counts = list(p[o + 1:o + 17])
+                syms = list(p[o + 17:o + 17 + sum(counts)])
                 (dc if tc == 0 else ac)[th] = Huffman(counts, syms, tc == 0)
                 o += 17 + sum(counts)
         elif m == 0xDB:
@@ -134,12 +147,16 @@ def parse(buf):
                 if tq > 3:
                     raise Corrupt("bad DQT table id")
                 n = 2 if pq else 1
+                if o + 1 + 64 * n > len(p):
+                    raise Corrupt("short DQT segment")
                 vals = [(_u16(p, o + 1 + 2 * k) if pq else p[o + 1 + k]) for k in range(64)]
                 nat = np.zeros(64, np.int64)
                 nat[NATURAL[:64]] = vals
                 q[tq] = nat
                 o += 1 + 64 * n
         elif m == 0xDD:
+            if len(p) < 2:
+                raise Corrupt("short DRI segment")
             ri = _u16(p, 0)
         elif m == 0xE0:
             jfif = jfif or p[:5] == b"JFIF\x00"
@@ -152,6 +169,8 @@ def parse(buf):
         elif m == 0xDA:
             if sof is None:
                 raise Corrupt("scan before the frame header")
+            if len(p) < 1 or len(p) < 4 + 2 * p[0]:
+                raise Corrupt("short scan header")
             ns = p[0]
             scomps = [(p[1 + 2 * k], p[2 + 2 * k] >> 4, p[2 + 2 * k] & 15) for k in range(ns)]
             ss, se, ahal = p[1 + 2 * ns], p[2 + 2 * ns], p[3 + 2 * ns]
@@ -160,10 +179,6 @@ def parse(buf):
 
 def _validate(sof, scomps, spectral, q, dc, ac, ri, jfif, adobe, orient, data_off, b):
     comps, nf = sof["comps"], len(sof["comps"])
-    if nf == 4:
-        raise Unsupported("CMYK / 4-component JPEG is not supported")
-    if nf not in (1, 3):
-        raise Unsupported("%d-component JPEG is not supported" % nf)
     if sof["w"] == 0 or sof["h"] == 0:
         raise Unsupported("JPEG without its size in the frame header (DNL) is not supported")
     if len(scomps) != nf:
@@ -180,12 +195,12 @@ def _validate(sof, scomps, spectral, q, dc, ac, ri, jfif, adobe, orient, data_of
                               ",".join("%dx%d" % (c["h"], c["v"]) for c in comps))
     if orient in range(2, 9):
         raise Unsupported("EXIF orientation %d is not supported (imdecode would rotate the image)" % orient)
-    byid = {c["id"]: c for c in comps}
     out = []
     for cid, td, ta in scomps:
-        if cid not in byid or td > 3 or ta > 3:
+        match = [c for c in comps if c["id"] == cid]
+        if not match or td > 3 or ta > 3:
             raise Corrupt("scan component does not match the frame")
-        c = dict(byid[cid])
+        c = dict(match[-1])
         if q[c["tq"] & 3] is None or dc[td] is None or ac[ta] is None:
             raise Corrupt("scan uses an undefined table")
         c.update(q=q[c["tq"] & 3].copy(), dc=dc[td], ac=ac[ta])
@@ -195,15 +210,18 @@ def _validate(sof, scomps, spectral, q, dc, ac, ri, jfif, adobe, orient, data_of
         hm = vm = 1
         out[0]["h"] = out[0]["v"] = 1  # a one-component scan is not interleaved: one block per MCU
     else:
-        hm, vm = comps[0]["h"], comps[0]["v"]
+        hm, vm = out[0]["h"], out[0]["v"]
+        if any(c["h"] != 1 or c["v"] != 1 for c in out[1:]):
+            raise Unsupported("a scan that does not start with the luma component is not supported")
     mx, my = -(-w // (8 * hm)), -(-h // (8 * vm))
     return dict(w=w, h=h, comps=out, hmax=hm, vmax=vm, mcux=mx, mcuy=my, ri=ri, data_off=data_off, buf=b)
 
 
 def _segments(hd):
-    """The entropy-coded data cut at its RST markers, stuffed zeros removed.  Returns the list of segments (bytes)."""
+    """The entropy-coded data cut at its RST markers, stuffed zeros removed.  Returns the list of segments (bytes) and
+    whether a marker other than RSTn ends the data (EOI; imdecode refuses a file without one)."""
     b, i = hd["buf"], hd["data_off"]
-    segs, cur, expect = [], bytearray(), 0
+    segs, cur, expect, ended = [], bytearray(), 0, False
     n_mcu = hd["mcux"] * hd["mcuy"]
     nseg = -(-n_mcu // hd["ri"]) if hd["ri"] else 1
     while i < len(b):
@@ -229,11 +247,12 @@ def _segments(hd):
             cur = bytearray()
             i = j + 1
             continue
+        ended = True
         break
     segs.append(bytes(cur))
     if len(segs) != nseg:
         raise Corrupt("%d restart intervals where %d are due" % (len(segs), nseg))
-    return segs
+    return segs, ended
 
 
 def blocks_per_mcu(hd):
@@ -246,63 +265,99 @@ def mcu_layout(hd):
 
 
 def coefficients(hd):
-    """Entropy decode.  Returns int64 [n_blocks, 64] in decode (MCU) order, natural order, absolute DC."""
-    segs = _segments(hd)
+    """Entropy decode.  Returns int64 [n_blocks, 64] in decode (MCU) order, natural order, absolute DC.
+
+    Each restart interval is decoded on its own, up to its first error.  A code whose 16-bit look-ahead reaches past the
+    interval's end and matches no code counts as the interval ending early (what follows the end is not the interval's
+    data).  When intervals fail, an invalid code in any of them is the file's error, else the interval that ends early."""
+    segs, ended = _segments(hd)
     lay = mcu_layout(hd)
     bpm = len(lay)
     n_mcu = hd["mcux"] * hd["mcuy"]
     ri = hd["ri"] or n_mcu
     out = np.zeros((n_mcu * bpm, 64), np.int64)
-    comps = hd["comps"]
+    errors = []
     for s, data in enumerate(segs):
-        nbits = 8 * len(data)
-        d = data + b"\x00" * 8
-        pos = 0
-        pred = [0] * len(comps)
-
-        def peek(p, n):
-            v = int.from_bytes(d[p >> 3:(p >> 3) + 5], "big")
-            return (v >> (40 - (p & 7) - n)) & ((1 << n) - 1)
-
-        def decode(tab, p):
-            k = peek(p, 16)
-            l = int(tab.length[k])
-            if l == 0:
-                raise Corrupt("invalid Huffman code in restart interval %d" % s)
-            return int(tab.symbol[k]), p + l
-
-        def extend(v, n):
-            return v - (1 << n) + 1 if v < (1 << (n - 1)) else v
-
-        m0, m1 = s * ri, min((s + 1) * ri, n_mcu)
-        for m in range(m0, m1):
-            for k, (ci, _, _) in enumerate(lay):
-                c = comps[ci]
-                blk = out[m * bpm + k]
-                sym, pos = decode(c["dc"], pos)
-                diff = 0
-                if sym:
-                    diff = extend(peek(pos, sym), sym)
-                    pos += sym
-                pred[ci] += diff
-                blk[0] = pred[ci]
-                z = 1
-                while z < 64:
-                    sym, pos = decode(c["ac"], pos)
-                    r, n = sym >> 4, sym & 15
-                    if n:
-                        z += r
-                        blk[NATURAL[z]] = extend(peek(pos, n), n)
-                        pos += n
-                    else:
-                        if r != 15:
-                            break
-                        z += 15
-                    z += 1
-                if pos > nbits:
-                    raise Corrupt("entropy-coded data ends before the last MCU of restart interval %d" % s)
+        try:
+            _decode_interval(hd, s, data, out, lay, ri, n_mcu)
+        except Corrupt as e:
+            errors.append(e)
+    if errors:
+        raise next((e for e in errors if "invalid Huffman code" in str(e)), errors[0])
+    if not ended:
+        raise Corrupt("entropy-coded data is not ended by a marker (truncated file)")
     out = ((out + 32768) & 0xFFFF) - 32768  # JCOEF is 16-bit
     return out
+
+
+def _decode_interval(hd, s, data, out, lay, ri, n_mcu):
+    bpm = len(lay)
+    comps = hd["comps"]
+    nbits = 8 * len(data)
+    d = data + b"\x00" * 8
+    pos = 0
+    pred = [0] * len(comps)
+
+    def peek(p, n):
+        v = int.from_bytes(d[p >> 3:(p >> 3) + 5].ljust(5, b"\x00"), "big")
+        return (v >> (40 - (p & 7) - n)) & ((1 << n) - 1)
+
+    def short():
+        return Corrupt("entropy-coded data ends before the last MCU of restart interval %d" % s)
+
+    def decode(tab, p):
+        k = peek(p, 16)
+        l = int(tab.length[k])
+        if l == 0:
+            raise short() if p + 16 > nbits else Corrupt("invalid Huffman code in restart interval %d" % s)
+        return int(tab.symbol[k]), p + l
+
+    def extend(v, n):
+        return v - (1 << n) + 1 if v < (1 << (n - 1)) else v
+
+    for m in range(s * ri, min((s + 1) * ri, n_mcu)):
+        for k, (ci, _, _) in enumerate(lay):
+            c = comps[ci]
+            blk = out[m * bpm + k]
+            sym, pos = decode(c["dc"], pos)
+            diff = 0
+            if sym:
+                diff = extend(peek(pos, sym), sym)
+                pos += sym
+            pred[ci] += diff
+            blk[0] = pred[ci]
+            z = 1
+            while z < 64:
+                sym, pos = decode(c["ac"], pos)
+                r, n = sym >> 4, sym & 15
+                if n:
+                    z += r
+                    blk[NATURAL[z]] = extend(peek(pos, n), n)
+                    pos += n
+                else:
+                    if r != 15:
+                        break
+                    z += 15
+                z += 1
+            if pos > nbits:
+                raise short()
+
+
+# The largest |coefficient x quantisation value| jpeg_fdct_islow and libjpeg-turbo's quantiser produce from 8-bit samples at
+# any 8- or 16-bit table entry (the DC of a flat block of 0 or 255 quantised by 2048; derived in test_jpeg_damage_cpu.py).
+# Past it, the pixels imdecode gives depend on how libjpeg-turbo was built (a single coefficient past the bound already
+# drives the C IDCT's output past the +-512 its range-limit table wraps at, where the SIMD IDCT differs), so the decoder
+# refuses such a file as corrupt.
+MAX_DEQUANT = 2048
+
+
+def check_range(hd, coef):
+    """Raises Corrupt if a dequantised coefficient (int16 coefficient times the int16 table entry) exceeds MAX_DEQUANT."""
+    lay = mcu_layout(hd)
+    for k, (ci, _, _) in enumerate(lay):
+        qt16 = ((np.asarray(hd["comps"][ci]["q"], np.int64) + 32768) & 0xFFFF) - 32768
+        if (np.abs(coef[k::len(lay)] * qt16) > MAX_DEQUANT).any():
+            raise Corrupt("dequantised DCT coefficient or IDCT output out of range (corrupt data)")
 
 
 # jpeg_idct_islow (jidctint.c), CONST_BITS 13, PASS1_BITS 2
@@ -347,6 +402,8 @@ def idct(coef, qt):
     ws = np.stack([_descale(v, 13 - 2) for v in cols], 1)
     rows = _idct_1d(*[ws[:, :, k] for k in range(8)])
     out = np.stack([_descale(v, 13 + 2 + 3) for v in rows], 2)
+    if ((out < -512) | (out > 511)).any():  # the range-limit table wraps here, libjpeg-turbo's SIMD IDCT saturates
+        raise Corrupt("dequantised DCT coefficient or IDCT output out of range (corrupt data)")
     # range_limit[x & RANGE_MASK] of the post-IDCT table: x taken as a signed 10-bit value, + 128, clamped
     s = ((out & 1023) ^ 512) - 512
     return np.clip(s + 128, 0, 255).astype(np.uint8)
@@ -441,5 +498,7 @@ def bgr_to_gray(bgr):
 
 def decode(buf, channels=3):
     hd = parse(buf)
-    bgr = to_bgr(hd, idct_planes(hd, coefficients(hd)))
+    coef = coefficients(hd)
+    check_range(hd, coef)
+    bgr = to_bgr(hd, idct_planes(hd, coef))
     return bgr if channels == 3 else bgr_to_gray(bgr)
