@@ -13,9 +13,6 @@ LIB_PATHS = {
     # geometry experiments (denseflow_b200/build.py VARIANTS), built on request only
     "t256": os.path.join(_HERE, "lib", "libdenseflow_b200_t256.so"),
     "t512": os.path.join(_HERE, "lib", "libdenseflow_b200_t512.so"),
-    "fb4": os.path.join(_HERE, "lib", "libdenseflow_b200_fb4.so"),
-    "fb3": os.path.join(_HERE, "lib", "libdenseflow_b200_fb3.so"),
-    "hx6": os.path.join(_HERE, "lib", "libdenseflow_b200_hx6.so"),
 }
 
 DFB_OK = 0

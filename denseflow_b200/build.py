@@ -24,9 +24,6 @@ VARIANTS = {
     # geometry experiments of the fused tvl1 kernel (not built by default): python -m denseflow_b200.build t256
     "t256": ("libdenseflow_b200_t256.so", ["-DDFB_FUSED_THREADS=256"]),
     "t512": ("libdenseflow_b200_t512.so", ["-DDFB_FUSED_THREADS=512"]),
-    "fb4": ("libdenseflow_b200_fb4.so", ["-DDFB_FARN_TMA_MINB=4"]),  # Farneback TMA kernel at 4 CTAs / SM (64 registers)
-    "fb3": ("libdenseflow_b200_fb3.so", ["-DDFB_FARN_TMA_MINB=3"]),
-    "hx6": ("libdenseflow_b200_hx6.so", ["-DDFB_FARN_HX=6"]),  # Farneback window without the 32-byte origin alignment
 }
 
 

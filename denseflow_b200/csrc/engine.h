@@ -7,6 +7,7 @@
 
 #include <cmath>
 #include <cstdint>
+#include <deque>
 #include <memory>
 #include <string>
 #include <vector>
@@ -25,14 +26,71 @@ struct LevelGeom {
 inline bool whole_in(double v, double lo, double hi) { return v >= lo && v <= hi && v == std::floor(v); }
 inline bool is_flag(double v) { return v == 0 || v == 1; }
 
+// CUDA-event timing of an engine's dominant kernel: one event pair around each timed range of launches on one stream, read
+// lazily so that timing never waits for the GPU inside a flow call.
+class KernelTimer {
+  public:
+    KernelTimer() = default;
+    KernelTimer(const KernelTimer &) = delete;
+    KernelTimer &operator=(const KernelTimer &) = delete;
+    ~KernelTimer() {
+        for (auto &e : ev_)
+            for (auto ev : e)
+                if (ev) cudaEventDestroy(ev);
+    }
+    void begin(cudaStream_t s) {
+        if (used_ == kRing) drain();
+        if (!ev_[0][0])
+            for (auto &e : ev_) {
+                DFB_CUDA(cudaEventCreate(&e[0]));
+                DFB_CUDA(cudaEventCreate(&e[1]));
+            }
+        DFB_CUDA(cudaEventRecord(ev_[used_][0], s));
+    }
+    // the range holds `launches` kernel launches and finishes `pairs` frame pairs
+    void end(cudaStream_t s, uint64_t launches, uint64_t pairs) {
+        DFB_CUDA(cudaEventRecord(ev_[used_][1], s));
+        ++used_;
+        launches_ += launches;
+        pairs_ += pairs;
+    }
+    void read(uint64_t *launches, uint64_t *ns, uint64_t *pairs) {
+        drain();
+        *launches = launches_;
+        *ns = ns_;
+        *pairs = pairs_;
+    }
+    void reset() {
+        drain();
+        launches_ = ns_ = pairs_ = 0;
+    }
+
+  private:
+    void drain() {
+        for (int i = 0; i < used_; ++i) {
+            DFB_CUDA(cudaEventSynchronize(ev_[i][1]));
+            float ms = 0.f;
+            DFB_CUDA(cudaEventElapsedTime(&ms, ev_[i][0], ev_[i][1]));
+            ns_ += (uint64_t)((double)ms * 1e6);
+        }
+        used_ = 0;
+    }
+    static constexpr int kRing = 256;
+    cudaEvent_t ev_[kRing][2] = {};
+    int used_ = 0;
+    uint64_t launches_ = 0, ns_ = 0, pairs_ = 0;
+};
+
 // Algorithm back-end working on device buffers. One frame "slot" holds everything that depends on
 // a single frame (its fp32 pyramid), so a frame shared by two consecutive pairs is prepared once.
 class FlowAlgorithm {
   public:
     virtual ~FlowAlgorithm() = default;
     virtual const char *name() const = 0;
-    virtual int num_slots() const = 0;
-    virtual void ensure_slots(int n) = 0;
+    int num_slots() const { return (int)slots_.size(); }
+    void ensure_slots(int n) {
+        while ((int)slots_.size() < n) slots_.push_back(owned_zeroed(slot_elems_));
+    }
     // per-frame work: u8 -> fp32 (+ pyramid)
     virtual void prepare_frame(const uint8_t *src, size_t pitch_bytes, int w, int h, int slot, cudaStream_t s) = 0;
     // several frames of one size at once (engines whose per-frame stages are launch-latency-bound batch them)
@@ -67,8 +125,13 @@ class FlowAlgorithm {
     virtual void begin_batch() {}
     virtual bool pair_stats(int pair_index, dfb_tvl1_stats *out) { (void)pair_index; *out = dfb_tvl1_stats{}; return false; }
     virtual void phase_ns(uint64_t *out) { for (int i = 0; i < 32; ++i) out[i] = 0; }
-    virtual void reset_counters() { launches = 0; pixel_iters = 0; pixel_chunks = 0; }
-    virtual void kernel_timing(uint64_t *launches_, uint64_t *ns, uint64_t *pairs) { *launches_ = *ns = *pairs = 0; }
+    virtual void reset_counters() {
+        launches = 0;
+        pixel_iters = 0;
+        pixel_chunks = 0;
+        timer_.reset();
+    }
+    void kernel_timing(uint64_t *launches_, uint64_t *ns, uint64_t *pairs) { timer_.read(launches_, ns, pairs); }
     // test hook behind dfb_debug_run_kernel: run one stage of this engine, through its own launch code and buffers, on dense
     // host planes (w x h floats each), with an optional scalar result.  Returns false when `kernel` is not one of the engine's stages.
     virtual bool debug_run(const std::string &kernel, const float *const *in, int n_in, float *const *out, int n_out, int w, int h,
@@ -79,6 +142,30 @@ class FlowAlgorithm {
     uint64_t launches = 0;     // kernels launched
     uint64_t pixel_iters = 0;  // tvl1: sum of level pixels over executed inner iterations
     uint64_t pixel_chunks = 0; // fused tvl1: sum of level pixels over tile visits (k iterations each)
+
+  protected:
+    static constexpr int kInitialSlots = 4;
+    // the first kInitialSlots frame slots, `elems` floats each, come from the engine's slab; ensure_slots() adds owned ones
+    void carve_slots(Slab &slab, size_t elems) {
+        slot_elems_ = elems;
+        for (int i = 0; i < kInitialSlots; ++i) slots_.push_back(slab.take<float>(elems));
+    }
+    // Device memory added after create time, freed with the engine.  It is zeroed because padding columns are read (never
+    // used) by vectorised kernels.  The memset runs on the null stream, which the handle's non-blocking streams do not wait
+    // for: finish it before any of them can touch the memory.
+    float *owned_zeroed(size_t elems) {
+        DeviceBuffer<float> &b = owned_.emplace_back();
+        b.allocate(elems * sizeof(float));
+        DFB_CUDA(cudaMemset(b, 0, b.bytes()));
+        DFB_CUDA(cudaDeviceSynchronize());
+        return b;
+    }
+    std::vector<float *> slots_;
+    KernelTimer timer_;
+
+  private:
+    size_t slot_elems_ = 0;
+    std::deque<DeviceBuffer<float>> owned_;
 };
 
 std::unique_ptr<FlowAlgorithm> make_tvl1(int device, int max_w, int max_h);

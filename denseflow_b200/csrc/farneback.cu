@@ -348,29 +348,21 @@ __global__ void __launch_bounds__(256) k_update_matrices(const __grid_constant__
 // registers.  Global reads of M drop from 13 vertical taps x 5 planes per column to 1.9 per output pixel and plane.
 // M is double-buffered across iterations (Mout != Min): a neighbouring tile's window must still see this iteration's M.
 constexpr int BW = 32;
-#ifndef DFB_FARN_BH
-#define DFB_FARN_BH 16
-#endif
-constexpr int BH = DFB_FARN_BH;  // 16: 512-pixel tiles, 38 KB of shared memory, 5 CTAs / SM (the kernel is latency-bound)
+constexpr int BH = 16;  // 512-pixel tiles (the kernel is latency-bound)
 // The staged window of one M plane: (BH + 2 HALF) rows x RW columns, RW = BW + 2 HX with HX >= HALF rounded up so that the window
 // starts on a 32-byte boundary of the plane row (x0 - HX, x0 a multiple of 32) and its rows are 16-byte multiples (TMA box rule).
-#ifndef DFB_FARN_HX
-#define DFB_FARN_HX 8
-#endif
-constexpr int HX = DFB_FARN_HX;
+constexpr int HX = 8;
 constexpr int RW = BW + 2 * HX;
+constexpr int kBoxMinBlocks = 4;  // CTAs per SM the iteration kernel is compiled for (64 registers)
 constexpr int kBoxPlaneSlot = ((RW * (BH + 12) + 31) / 32) * 32;  // floats per staged window, a multiple of 128 bytes (TMA destination)
 
 // The part of the iteration that works out of shared memory: raw = the five (BH + 2 HALF) x (BW + 2 HALF) windows of M
-// (index-clamped), vs = scratch for the vertical sums.  Shared by the LDG-staged and the TMA-staged kernel.
-struct NoHook {
-    __device__ __forceinline__ void operator()() const {}
-};
-// after_vertical() runs once the vertical sums are in `vs` and every thread is done with `raw` (the TMA kernel asks for the
+// (index-clamped), vs = scratch for the vertical sums.
+// after_vertical() runs once the vertical sums are in `vs` and every thread is done with `raw` (the kernel asks for the
 // next tile's windows there, so they land while this tile's long half — solve, gathers, rebuild — is still running).
-template <int HALF, typename Hook = NoHook>
+template <int HALF, typename Hook>
 __device__ __forceinline__ void box_tile_compute(const float *raw /* [5][kBoxPlaneSlot] */, float (*vs)[BH][BW + 2 * HALF], const PairArgs &a, int mb,
-                                                 int rebuild, int x0, int y0, int tid, Hook after_vertical = Hook()) {
+                                                 int rebuild, int x0, int y0, int tid, Hook after_vertical) {
     const Plane5 Mout = a.M[mb ^ 1], R0 = a.R0, R1 = a.R1;
     const Plane fxp = a.fx, fyp = a.fy;
     constexpr int sw = BW + 2 * HALF;
@@ -484,125 +476,13 @@ __device__ __forceinline__ void box_tile_compute(const float *raw /* [5][kBoxPla
     }
 }
 
-// LDG-staged variant, self-contained (round-1 kernel): one CTA per 32 x 16 tile, window staged with index-clamped scalar loads,
-// 44-float window rows.  Kept as the comparison / fallback path (use_tma = 0); bit-identical to the TMA kernel below.
-template <int HALF>
-__global__ void __launch_bounds__(256) k_box_solve_update(const __grid_constant__ FarnBatchArgs args, int mb, int rebuild) {
-    const PairArgs &a = args.p[blockIdx.z];
-    const Plane5 Min = a.M[mb], Mout = a.M[mb ^ 1], R0 = a.R0, R1 = a.R1;
-    const Plane fxp = a.fx, fyp = a.fy;
-    constexpr int sw = BW + 2 * HALF, sh = BH + 2 * HALF;
-    extern __shared__ float box_smem[];
-    float(*raw)[sh][sw] = reinterpret_cast<float(*)[sh][sw]>(box_smem);               // [5][sh][sw]
-    float(*vs)[BH][sw] = reinterpret_cast<float(*)[BH][sw]>(box_smem + 5 * sh * sw);  // [5][BH][sw]
-    const int x0 = blockIdx.x * BW, y0 = blockIdx.y * BH;
-    const int w = Min.w, h = Min.h, pitch = Min.pitch;
-    const int tid = threadIdx.x;
-    for (int i = tid; i < sh * sw; i += 256) {
-        const int ty = i / sw, tx = i - ty * sw;
-        const int y = max(0, min(y0 + ty - HALF, h - 1));
-        const int x = max(0, min(x0 + tx - HALF, w - 1));
-        const size_t o = (size_t)y * pitch + x;
-#pragma unroll
-        for (int k = 0; k < 5; ++k) raw[k][ty][tx] = Min.p[k][o];
-    }
-    __syncthreads();
-    // vertical sums, register-blocked: one task = 4 vertically consecutive outputs of one column and plane
-    // (16 window reads for 4 sums instead of 52); each sum keeps the reference's order (centre, then symmetric
-    // pairs outward).  Clamped rows are materialised in the window, which equals clamping the tap's row index.
-    constexpr int VG = 4;
-    for (int i = tid; i < 5 * (BH / VG) * sw; i += 256) {
-        const int tx = i % sw, rest = i / sw;
-        const int g = rest % (BH / VG), k = rest / (BH / VG);
-        float v[VG + 2 * HALF];
-#pragma unroll
-        for (int q = 0; q < VG + 2 * HALF; ++q) v[q] = raw[k][g * VG + q][tx];
-#pragma unroll
-        for (int o = 0; o < VG; ++o) {
-            float acc = v[o + HALF];
-#pragma unroll
-            for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]);
-            vs[k][g * VG + o][tx] = acc;
-        }
-    }
-    __syncthreads();
-    // horizontal sums + solve + rebuild: each thread owns PX consecutive pixels of one row
-    constexpr float area_inv = 1.f / (float)((1 + 2 * HALF) * (1 + 2 * HALF));
-    constexpr int PX = BW * BH / 256;
-    static_assert(PX == 1 || PX == 2 || PX == 4, "tile must be 256, 512 or 1024 pixels");
-    static_assert((2 * HALF) % PX == 0 && (BW + 2 * HALF) % PX == 0, "vector-aligned rows");
-    {
-        const int ty = tid / (BW / PX), tx0 = (tid % (BW / PX)) * PX;
-        const int y = y0 + ty;
-        float b[PX][5];
-#pragma unroll
-        for (int k = 0; k < 5; ++k) {
-            float v[PX + 2 * HALF];
-            if (PX == 4) {
-#pragma unroll
-                for (int q = 0; q < (PX + 2 * HALF) / 4; ++q) {
-                    const float4 t = *reinterpret_cast<const float4 *>(&vs[k][ty][tx0 + 4 * q]);
-                    v[4 * q] = t.x;
-                    v[4 * q + 1] = t.y;
-                    v[4 * q + 2] = t.z;
-                    v[4 * q + 3] = t.w;
-                }
-            } else if (PX == 2) {
-#pragma unroll
-                for (int q = 0; q < (PX + 2 * HALF) / 2; ++q) {
-                    const float2 t = *reinterpret_cast<const float2 *>(&vs[k][ty][tx0 + 2 * q]);
-                    v[2 * q] = t.x;
-                    v[2 * q + 1] = t.y;
-                }
-            } else {
-#pragma unroll
-                for (int q = 0; q < PX + 2 * HALF; ++q) v[q] = vs[k][ty][tx0 + q];
-            }
-#pragma unroll
-            for (int o = 0; o < PX; ++o) {
-                float acc = v[o + HALF];
-#pragma unroll
-                for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]);
-                b[o][k] = acc * area_inv;
-            }
-        }
-        // all pixels' gathers are issued before any of them is consumed: coordinates are clamped into the image
-        // (safe reads), only the stores are predicated
-        const int yc = min(y, h - 1);
-        float nfx[PX], nfy[PX], m[PX][5];
-#pragma unroll
-        for (int o = 0; o < PX; ++o) {
-            // updateFlow: g11 = b0, g12 = b1, g22 = b2, h1 = b3, h2 = b4
-            const float det_inv = f_rcp(b[o][0] * b[o][2] - b[o][1] * b[o][1] + 1e-3f);
-            nfx[o] = (b[o][0] * b[o][4] - b[o][1] * b[o][3]) * det_inv;
-            nfy[o] = (b[o][2] * b[o][3] - b[o][1] * b[o][4]) * det_inv;
-        }
-        if (rebuild) {
-#pragma unroll
-            for (int o = 0; o < PX; ++o) update_matrices_px(min(x0 + tx0 + o, w - 1), yc, w, h, pitch, nfx[o], nfy[o], R0, R1, m[o]);
-        }
-#pragma unroll
-        for (int o = 0; o < PX; ++o) {
-            const int x = x0 + tx0 + o;
-            if (x < w && y < h) {
-                const size_t oo = (size_t)y * pitch + x;
-                fxp.p[oo] = nfx[o];
-                fyp.p[oo] = nfy[o];
-                if (rebuild) {
-#pragma unroll
-                    for (int k = 0; k < 5; ++k) Mout.p[k][oo] = m[o][k];
-                }
-            }
-        }
-    }
-}
-// The same iteration as a persistent kernel with TMA-staged windows (the default): a CTA walks the tile list of the whole
-// batch (pairs x tile rows x tile columns).  The five windows of a tile arrive by cp.async.bulk.tensor.2d (completion on an
-// mbarrier, zero fill outside the image).  The staging buffer is free again as soon as the vertical sums are done, so the
-// request for the NEXT tile's windows goes out there and the copy runs under this tile's long half (solve, the R1 gathers,
-// rebuild of M): one buffer, 41 KB of shared memory, five CTAs per SM like the LDG kernel — and no exposed staging loop.
+// The iteration is a persistent kernel with TMA-staged windows: a CTA walks the tile list of the whole batch (pairs x tile
+// rows x tile columns).  The five windows of a tile arrive by cp.async.bulk.tensor.2d (completion on an mbarrier, zero fill
+// outside the image).  The staging buffer is free again as soon as the vertical sums are done, so the request for the NEXT
+// tile's windows goes out there and the copy runs under this tile's long half (solve, the R1 gathers, rebuild of M): one
+// buffer, 41 KB of shared memory, and no exposed staging loop.
 // Index-clamped borders: tiles that touch the image border copy the nearest in-image entry of the window into the
-// zero-filled ones (border tiles only), which reproduces the clamped reads of the LDG kernel bit for bit.
+// zero-filled ones (border tiles only), which reproduces index-clamped reads of M bit for bit.
 template <int HALF>
 struct BoxTmaSmem {
     float raw[5][kBoxPlaneSlot];
@@ -610,11 +490,8 @@ struct BoxTmaSmem {
     unsigned long long bar;
 };
 
-#ifndef DFB_FARN_TMA_MINB
-#define DFB_FARN_TMA_MINB 4
-#endif
 template <int HALF>
-__global__ void __launch_bounds__(256, DFB_FARN_TMA_MINB) k_box_solve_update_tma(const __grid_constant__ FarnBatchArgs args, const char *maps, int nb, int ntx, int nty,
+__global__ void __launch_bounds__(256, kBoxMinBlocks) k_box_solve_update(const __grid_constant__ FarnBatchArgs args, const char *maps, int nb, int ntx, int nty,
                                                                  int mb, int rebuild) {
     constexpr int sh = BH + 2 * HALF;
     static_assert(RW * sh <= kBoxPlaneSlot && (RW * 4) % 16 == 0 && HX >= HALF, "window fits its slot, rows are 16-byte multiples");
@@ -708,8 +585,6 @@ __global__ void __launch_bounds__(256) k_farn_merge(const __grid_constant__ Farn
     float2 *row = reinterpret_cast<float2 *>(reinterpret_cast<char *>(a.flow_xy) + (size_t)y * a.flow_pitch_bytes);
     row[x] = make_float2(u, v);
 }
-
-constexpr size_t kBoxSmemBytes = (size_t)(5 * (BH + 12) * (BW + 12) + 5 * BH * (BW + 12)) * sizeof(float);
 
 struct FarnParams {
     int num_levels = 5;
@@ -825,49 +700,22 @@ class Farneback final : public FlowAlgorithm {
         // a frame slot holds the polynomial expansion of every level (5 planes each): everything that depends on
         // one frame only, so a frame shared by two consecutive pairs is blurred / resized / expanded once
         LevelSet ls = levels_for(max_w_, max_h_, /*max_depth=*/true);
-        slot_elems_ = ls.total_r_elems;
-        const int n_work = 3 /*frame, blurred, img*/;
-        slab_.reserve(kInitialSlots * Slab::padded(slot_elems_, 4) + n_work * Slab::padded(plane_elems_, 4) + (1 << 12));
-        for (int i = 0; i < kInitialSlots; ++i) slots_.push_back(slab_.take<float>(slot_elems_));
-        frame_ = slab_.take<float>(plane_elems_);
-        blurred_ = slab_.take<float>(plane_elems_);
-        img_ = slab_.take<float>(plane_elems_);
+        slab_.reserve(kInitialSlots * Slab::padded(ls.total_r_elems, 4) + (1 << 12));
+        carve_slots(slab_, ls.total_r_elems);
         slab_.zero();
         ensure_lanes(1);
+        ensure_prep_scratch(1);
         DFB_CUDA(cudaFuncSetAttribute(k_gauss_blur, cudaFuncAttributeMaxDynamicSharedMemorySize, GT * (GT + 2 * kMaxHalf) * 4));
-        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBoxSmemBytes));
-        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update_tma<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoxTmaSmem<6>)));
-        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update_tma<6>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoxTmaSmem<6>)));
+        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update<6>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         int per_sm = 0, sms = 0;
-        DFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_box_solve_update_tma<6>, 256, sizeof(BoxTmaSmem<6>)));
+        DFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_box_solve_update<6>, 256, sizeof(BoxTmaSmem<6>)));
         DFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_));
         persistent_ctas_ = std::max(1, per_sm) * sms;
-        DFB_CUDA(cudaMalloc(&d_maps_, kMapBytes));
+        d_maps_.allocate(kMapBytes);
     }
-    ~Farneback() override {
-        cudaSetDevice(device_);
-        for (auto p : extra_slots_) cudaFree(p);
-        for (auto &l : lanes_) cudaFree(l.own);
-        if (d_maps_) cudaFree(d_maps_);
-        for (auto &p : prep_)
-            if (p.own)
-                for (float *q : {p.frame, p.blurred, p.img}) cudaFree(q);
-        for (auto &e : timing_ev_)
-            for (auto ev : e)
-                if (ev) cudaEventDestroy(ev);
-    }
+    ~Farneback() override { cudaSetDevice(device_); }
     const char *name() const override { return "farn"; }
-    int num_slots() const override { return (int)slots_.size(); }
-    void ensure_slots(int n) override {
-        while ((int)slots_.size() < n) {
-            float *p = nullptr;
-            DFB_CUDA(cudaMalloc(&p, slot_elems_ * sizeof(float)));
-            DFB_CUDA(cudaMemset(p, 0, slot_elems_ * sizeof(float)));
-            DFB_CUDA(cudaDeviceSynchronize());  // null-stream memset vs the handle's non-blocking streams
-            extra_slots_.push_back(p);
-            slots_.push_back(p);
-        }
-    }
     bool set_param(const std::string &k, double v) override {
         // a refused value leaves the parameter as it was
         if (k == "num_levels") { if (!whole_in(v, 0, 5)) return false; prm_.num_levels = (int)v; }
@@ -876,7 +724,6 @@ class Farneback final : public FlowAlgorithm {
         else if (k == "pyr_scale") return v == 0.5;  // level geometry and the slot layout assume the default
         else if (k == "win_size" || k == "poly_n") return (k == "win_size" ? v == 13 : v == 5);  // compiled-in stencils
         else if (k == "time_kernels") { if (!is_flag(v)) return false; time_kernels_ = v != 0; }
-        else if (k == "use_tma") { if (!is_flag(v)) return false; use_tma_ = v != 0; }
         else return false;
         return true;
     }
@@ -888,34 +735,8 @@ class Farneback final : public FlowAlgorithm {
         else if (k == "poly_n") *v = prm_.poly_n;
         else if (k == "poly_sigma") *v = prm_.poly_sigma;
         else if (k == "time_kernels") *v = time_kernels_;
-        else if (k == "use_tma") *v = use_tma_;
         else return false;
         return true;
-    }
-
-    // CUDA-event timing of the dominant kernel (k_box_solve_update): one event pair around the iteration launches of every
-    // level (nothing else is enqueued between them), drained lazily
-    void drain_timing() {
-        for (int i = 0; i < timing_used_; ++i) {
-            DFB_CUDA(cudaEventSynchronize(timing_ev_[i][1]));
-            float ms = 0.f;
-            DFB_CUDA(cudaEventElapsedTime(&ms, timing_ev_[i][0], timing_ev_[i][1]));
-            timed_ns_ += (uint64_t)((double)ms * 1e6);
-        }
-        timing_used_ = 0;
-    }
-    void kernel_timing(uint64_t *launches_, uint64_t *ns, uint64_t *pairs) override {
-        drain_timing();
-        *launches_ = timed_launches_;
-        *ns = timed_ns_;
-        *pairs = timed_pairs_;
-    }
-    void reset_counters() override {
-        drain_timing();
-        launches = 0;
-        pixel_iters = 0;
-        pixel_chunks = 0;
-        timed_launches_ = timed_ns_ = timed_pairs_ = 0;
     }
 
     // per-frame work (B.2, B.3): u8 -> fp32, then for every level: Gaussian blur of the FULL-resolution frame,
@@ -954,11 +775,10 @@ class Farneback final : public FlowAlgorithm {
 
     void solve_batch(const PairJob *jobs, int count, int w, int h, cudaStream_t s) override {
         const LevelSet ls = levels_for(w, h, false);
-        timed_pairs_ += time_kernels_ ? count : 0;
         for (int j0 = 0; j0 < count; j0 += kMaxFarnBatch) {
             const int nb = std::min(kMaxFarnBatch, count - j0);
             ensure_lanes(nb);
-            if (use_tma_) ensure_tensor_maps(ls);
+            ensure_tensor_maps(ls);
             int cur = 0;
             FarnBatchArgs args{};
             for (int l = 0; l < ls.n; ++l) {
@@ -968,24 +788,14 @@ class Farneback final : public FlowAlgorithm {
                 int mb = 0;
                 launch_update_matrices(args, nb, L, mb, s);
                 pixel_iters += (uint64_t)L.w * L.h * prm_.num_iters * nb;
-                if (time_kernels_) {
-                    if (timing_used_ == kTimingRing) drain_timing();
-                    if (!timing_ev_[0][0])
-                        for (int i = 0; i < kTimingRing; ++i) {
-                            DFB_CUDA(cudaEventCreate(&timing_ev_[i][0]));
-                            DFB_CUDA(cudaEventCreate(&timing_ev_[i][1]));
-                        }
-                    DFB_CUDA(cudaEventRecord(timing_ev_[timing_used_][0], s));
-                }
+                // time_kernels: one timed range around the iteration launches of every level (nothing else is enqueued
+                // between them); the finest level finishes the chunk's pairs
+                if (time_kernels_) timer_.begin(s);
                 for (int it = 0; it < prm_.num_iters; ++it) {
                     launch_iteration(args, nb, ls, l, mb, it < prm_.num_iters - 1, s);
                     mb ^= 1;
                 }
-                if (time_kernels_) {
-                    DFB_CUDA(cudaEventRecord(timing_ev_[timing_used_][1], s));
-                    ++timing_used_;
-                    timed_launches_ += prm_.num_iters;
-                }
+                if (time_kernels_) timer_.end(s, prm_.num_iters, l == ls.n - 1 ? nb : 0);
                 if (l == ls.n - 1) launch_merge(args, nb, L, s);  // last processed level is full resolution (k = 0): merge -> CV_32FC2
                 cur ^= 1;
             }
@@ -1068,8 +878,8 @@ class Farneback final : public FlowAlgorithm {
         // pair stages: every input stacks `pairs` planes of h / pairs rows along its rows, one per pair (pair i = lane i, frame
         // slots 2i / 2i + 1), so several pairs with different data run in one launch
         //   farn_update_matrices  in {fx, fy, R0 x 5, R1 x 5}  out {M0 .. M4}                 scalars {pairs}
-        //   farn_iteration        in {M x 5, R0 x 5, R1 x 5}   out {fx, fy, M'0 .. M'4}        scalars {use_tma, rebuild, pairs}
-        const int nb = (int)sc(um ? 0 : 2, 1);
+        //   farn_iteration        in {M x 5, R0 x 5, R1 x 5}   out {fx, fy, M'0 .. M'4}        scalars {rebuild, pairs}
+        const int nb = (int)sc(um ? 0 : 1, 1);
         if (nb < 1 || nb > kMaxFarnBatch || h % nb) throw std::runtime_error(k + ": pairs must be in [1, 8] and divide the height");
         const int ph = h / nb;
         um ? need(12, 5) : need(15, 7);
@@ -1097,11 +907,8 @@ class Farneback final : public FlowAlgorithm {
         if (um) {
             launch_update_matrices(args, nb, ls.lv[l], 0, s);
         } else {
-            const int tma = use_tma_;
-            use_tma_ = sc(0, 1) != 0;
-            if (use_tma_) ensure_tensor_maps(ls);
-            launch_iteration(args, nb, ls, l, 0, sc(1, 1) != 0, s);
-            use_tma_ = tma;
+            ensure_tensor_maps(ls);
+            launch_iteration(args, nb, ls, l, 0, sc(0, 1) != 0, s);
         }
         DFB_CUDA(cudaDeviceSynchronize());
         for (int i = 0; i < nb; ++i) {
@@ -1160,43 +967,26 @@ class Farneback final : public FlowAlgorithm {
         return Plane5{{base, base + pe, base + 2 * pe, base + 3 * pe, base + 4 * pe}, L.w, L.h, L.pitch};
     }
 
-    static constexpr int kInitialSlots = 4;
     int device_, max_w_, max_h_, pitch0_ = 0;
-    size_t plane_elems_ = 0, slot_elems_ = 0;
+    size_t plane_elems_ = 0;
     FarnParams prm_;
     Slab slab_;
-    std::vector<float *> slots_, extra_slots_;
-    float *frame_ = nullptr, *blurred_ = nullptr, *img_ = nullptr;  // scratch of the first frame of a preparation batch (slab)
-    struct PrepScratch {
-        float *frame = nullptr, *blurred = nullptr, *img = nullptr;
-        bool own = false;
-    };
-    std::vector<PrepScratch> prep_;
+    // preparation scratch of each frame of a batch: three full-resolution planes (frame, blurred rows, level image)
+    std::vector<float *> prep_;
     void ensure_prep_scratch(int n) {
-        if (prep_.empty()) prep_.push_back(PrepScratch{frame_, blurred_, img_, false});
-        while ((int)prep_.size() < n) {
-            PrepScratch p;
-            p.own = true;
-            for (float **q : {&p.frame, &p.blurred, &p.img}) {
-                DFB_CUDA(cudaMalloc(q, plane_elems_ * sizeof(float)));
-                DFB_CUDA(cudaMemset(*q, 0, plane_elems_ * sizeof(float)));
-            }
-            DFB_CUDA(cudaDeviceSynchronize());
-            prep_.push_back(p);
-        }
+        while ((int)prep_.size() < n) prep_.push_back(owned_zeroed(3 * Slab::padded(plane_elems_, 4) / sizeof(float)));
     }
     // per-pair workspace: M (two buffers of five planes) and the flow of the current + previous level
     struct Lane {
-        float *own = nullptr;
         float *M[2][5] = {};
         float *fx[2] = {}, *fy[2] = {};
     };
     std::vector<Lane> lanes_;
     // TMA descriptors of the M planes: [level][lane][buffer][plane], rebuilt when the frame geometry or the lane count changes
     static constexpr size_t kMapBytes = (size_t)kMaxLevels * kMaxFarnBatch * 10 * kTensorMapBytes;
-    char *d_maps_ = nullptr;
+    DeviceBuffer<char> d_maps_;
     int maps_w_ = 0, maps_h_ = 0, maps_lanes_ = 0, maps_levels_ = 0;
-    int persistent_ctas_ = 132, use_tma_ = 1;
+    int persistent_ctas_ = 132;
     void ensure_tensor_maps(const LevelSet &ls) {
         const Level &F = ls.lv[ls.n - 1];
         if (maps_w_ == F.w && maps_h_ == F.h && maps_lanes_ == (int)lanes_.size() && maps_levels_ == ls.n) return;
@@ -1214,18 +1004,12 @@ class Farneback final : public FlowAlgorithm {
         maps_lanes_ = (int)lanes_.size();
         maps_levels_ = ls.n;
     }
-    static constexpr int kTimingRing = 256;
-    cudaEvent_t timing_ev_[kTimingRing][2] = {};
-    int timing_used_ = 0, time_kernels_ = 0;
-    uint64_t timed_launches_ = 0, timed_ns_ = 0, timed_pairs_ = 0;
+    int time_kernels_ = 0;
     void ensure_lanes(int n) {
         while ((int)lanes_.size() < n) {
             Lane l;
             const size_t pl = Slab::padded(plane_elems_, 4) / sizeof(float);
-            DFB_CUDA(cudaMalloc(&l.own, 14 * pl * sizeof(float)));
-            DFB_CUDA(cudaMemset(l.own, 0, 14 * pl * sizeof(float)));
-            DFB_CUDA(cudaDeviceSynchronize());  // null-stream memset vs the caller's (possibly non-blocking) stream
-            float *c = l.own;
+            float *c = owned_zeroed(14 * pl);
             for (int b = 0; b < 2; ++b)
                 for (int k = 0; k < 5; ++k) {
                     l.M[b][k] = c;
@@ -1245,10 +1029,11 @@ class Farneback final : public FlowAlgorithm {
     PrepBatch prep_batch(int nf) {
         ensure_prep_scratch(nf);
         PrepBatch pb{};
+        const size_t pl = Slab::padded(plane_elems_, 4) / sizeof(float);
         for (int i = 0; i < nf; ++i) {
-            pb.frame[i] = prep_[i].frame;
-            pb.vn[i] = prep_[i].blurred;
-            pb.img[i] = prep_[i].img;
+            pb.frame[i] = prep_[i];
+            pb.vn[i] = prep_[i] + pl;
+            pb.img[i] = prep_[i] + 2 * pl;
         }
         return pb;
     }
@@ -1325,18 +1110,14 @@ class Farneback final : public FlowAlgorithm {
         DFB_KERNEL_CHECK();
         ++launches;
     }
-    // one iteration (box mean of M[mb] -> solve -> rebuild into M[mb ^ 1]); the TMA kernel reads level l's tensor maps, which
+    // one iteration (box mean of M[mb] -> solve -> rebuild into M[mb ^ 1]); the kernel reads level l's tensor maps, which
     // ensure_tensor_maps(ls) must have encoded
     void launch_iteration(const FarnBatchArgs &args, int nb, const LevelSet &ls, int l, int mb, int rebuild, cudaStream_t s) {
         const Level &L = ls.lv[l];
-        if (use_tma_) {
-            const int ntx = ceil_div(L.w, BW), nty = ceil_div(L.h, BH);
-            const int grid = std::min(persistent_ctas_, ntx * nty * nb);
-            k_box_solve_update_tma<6><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(args, d_maps_ + (size_t)l * kMaxFarnBatch * 10 * kTensorMapBytes, nb, ntx,
-                                                                              nty, mb, rebuild);
-        } else {
-            k_box_solve_update<6><<<dim3(ceil_div(L.w, BW), ceil_div(L.h, BH), nb), 256, kBoxSmemBytes, s>>>(args, mb, rebuild);
-        }
+        const int ntx = ceil_div(L.w, BW), nty = ceil_div(L.h, BH);
+        const int grid = std::min(persistent_ctas_, ntx * nty * nb);
+        k_box_solve_update<6><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(args, d_maps_ + (size_t)l * kMaxFarnBatch * 10 * kTensorMapBytes, nb, ntx, nty, mb,
+                                                                      rebuild);
         DFB_KERNEL_CHECK();
         ++launches;
     }

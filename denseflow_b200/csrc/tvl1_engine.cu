@@ -56,7 +56,6 @@ class Tvl1 final : public FlowAlgorithm {
     }
     ~Tvl1() override {
         cudaSetDevice(device_);
-        for (auto p : extra_slots_) cudaFree(p);
         for (auto &l : lanes_) {
             if (l.host_ctl) cudaFreeHost(l.host_ctl);
             if (l.own) cudaFree(l.own);
@@ -70,25 +69,8 @@ class Tvl1 final : public FlowAlgorithm {
             if (job_ring_d_[r]) cudaFree(job_ring_d_[r]);
             if (job_ring_ev_[r]) cudaEventDestroy(job_ring_ev_[r]);
         }
-        for (auto &e : timing_ev_)
-            for (auto ev : e)
-                if (ev) cudaEventDestroy(ev);
     }
     const char *name() const override { return "tvl1"; }
-    int num_slots() const override { return (int)slots_.size(); }
-
-    void ensure_slots(int n) override {
-        while ((int)slots_.size() < n) {
-            float *p = nullptr;
-            DFB_CUDA(cudaMalloc(&p, pyr_elems_ * sizeof(float)));
-            // planes start finite: padding columns are read (never used).  The memset runs on the null stream, which the
-            // handle's non-blocking streams do not wait for: finish it before any of them can touch the slot.
-            DFB_CUDA(cudaMemset(p, 0, pyr_elems_ * sizeof(float)));
-            DFB_CUDA(cudaDeviceSynchronize());
-            extra_slots_.push_back(p);
-            slots_.push_back(p);
-        }
-    }
 
     // A refused value leaves the parameter as it was.  tau and theta must be positive: the dual step's 1 + taut * |grad u|
     // >= 1 and the primal clamp's l_t >= 0 rely on it (tvl1_math.cuh).
@@ -541,9 +523,8 @@ class Tvl1 final : public FlowAlgorithm {
             pyr_elems_ += max_lv_elems_[l];
         }
         plane_elems_ = (size_t)lv[0].pitch * (lv[0].h + 1);
-        constexpr int kInitialSlots = 4;
         slab_.reserve(kInitialSlots * Slab::padded(pyr_elems_, 4) + (1 << 12));
-        for (int i = 0; i < kInitialSlots; ++i) slots_.push_back(slab_.take<float>(pyr_elems_));
+        carve_slots(slab_, pyr_elems_);
         ensure_lanes(1);
         DFB_CUDA(cudaEventCreateWithFlags(&stats_event_, cudaEventDisableTiming));
         DFB_CUDA(cudaHostAlloc(&pair_log_, sizeof(int) * kLogInts * kPairLog, cudaHostAllocMapped));
@@ -775,15 +756,7 @@ class Tvl1 final : public FlowAlgorithm {
         const int hx = 4, hy = 1;
         const int max_tiles = fused_tiles_along(lv[0].w, kFusedTileW, hx) * fused_tiles_along(lv[0].h, kFusedTileH, hy);
         batch.group = std::max(1, std::min(batch.group, max_tiles));
-        if (prm_.time_kernels) {
-            if (timing_used_ == kTimingRing) drain_timing();
-            if (!timing_ev_[0][0])
-                for (int i = 0; i < kTimingRing; ++i) {
-                    DFB_CUDA(cudaEventCreate(&timing_ev_[i][0]));
-                    DFB_CUDA(cudaEventCreate(&timing_ev_[i][1]));
-                }
-            DFB_CUDA(cudaEventRecord(timing_ev_[timing_used_][0], s));
-        }
+        if (prm_.time_kernels) timer_.begin(s);
         if (count > kFusedParamLanes) {  // too many for the parameter bank: through the device-memory ring
             DFB_CUDA(cudaMemcpyAsync(job_ring_d_[jr], host_jobs, sizeof(FusedJob) * count, cudaMemcpyHostToDevice, s));
             DFB_CUDA(cudaEventRecord(job_ring_ev_[jr], s));
@@ -791,33 +764,12 @@ class Tvl1 final : public FlowAlgorithm {
         batch.jobs = job_ring_d_[jr];
         batch.host_jobs = host_jobs;
         launches += launch_tvl1_fused(batch, device_, s, prm_.serial_launches != 0);
-        if (prm_.time_kernels) {
-            DFB_CUDA(cudaEventRecord(timing_ev_[timing_used_][1], s));
-            ++timing_used_;
-            timed_pairs_ += count;
-        }
+        if (prm_.time_kernels) timer_.end(s, 1, count);
         last_lane_ = count - 1;
         DFB_CUDA(cudaEventRecord(stats_event_, s));
         stats_pending_ = true;
     }
 
-    // CUDA-event timing of the dominant kernel (events on the launching stream, drained lazily)
-    void drain_timing() {
-        for (int i = 0; i < timing_used_; ++i) {
-            DFB_CUDA(cudaEventSynchronize(timing_ev_[i][1]));
-            float ms = 0.f;
-            DFB_CUDA(cudaEventElapsedTime(&ms, timing_ev_[i][0], timing_ev_[i][1]));
-            timed_ns_ += (uint64_t)((double)ms * 1e6);
-            ++timed_launches_;
-        }
-        timing_used_ = 0;
-    }
-    void kernel_timing(uint64_t *launches_, uint64_t *ns, uint64_t *pairs) override {
-        drain_timing();
-        *launches_ = timed_launches_;
-        *ns = timed_ns_;
-        *pairs = timed_pairs_;
-    }
     void accumulate_pixel_iters() {
         for (int l = 0; l < last_nscales_; ++l)
             for (int wi = 0; wi < prm_.warps; ++wi)
@@ -828,16 +780,12 @@ class Tvl1 final : public FlowAlgorithm {
             cudaEventSynchronize(stats_event_);
             stats_pending_ = false;
         }
-        launches = 0;
-        pixel_iters = 0;
+        FlowAlgorithm::reset_counters();
         unfused_px_iters_ = 0;
-        drain_timing();
-        timed_launches_ = timed_ns_ = timed_pairs_ = 0;
         for (auto &l : lanes_) {
             l.host_ctl->px_iters_total = 0;
             l.host_ctl->px_chunks_total = 0;
         }
-        pixel_chunks = 0;
     }
     uint64_t unfused_px_iters_ = 0;
     float *unfused_scratch_ = nullptr;
@@ -851,15 +799,9 @@ class Tvl1 final : public FlowAlgorithm {
     int device_, max_w_, max_h_;
     Tvl1Params prm_;
     Slab slab_;
-    std::vector<float *> slots_;
-    std::vector<float *> extra_slots_;
     size_t max_lv_elems_[kMaxScales] = {};
     size_t pyr_elems_ = 0, plane_elems_ = 0;
     std::vector<Lane> lanes_;
-    static constexpr int kTimingRing = 256;
-    cudaEvent_t timing_ev_[kTimingRing][2] = {};
-    int timing_used_ = 0;
-    uint64_t timed_launches_ = 0, timed_ns_ = 0, timed_pairs_ = 0;
     int last_lane_ = 0;
     // iteration logs of the last kPairLog pairs, written by the kernel into mapped host memory
     static constexpr int kPairLog = 256, kLogInts = 16 * 16;

@@ -71,9 +71,8 @@ const char *dfb_last_error(const dfb_handle *h);
  * shared-memory tiles [default]), "prefetch" (1 = L2 prefetch of a CTA's next tile during the iterations [default]),
  * "serial_launches" (1 = the fused launches of all handles on one device run strictly one after another; 0 [default] = a
  * second handle's launch fills the SMs the first one's finished lanes free), "time_kernels" (CUDA-event timing of the dominant kernel, see dfb_counters).  farn: "num_levels" (0..5)
- * "num_iters" (>= 1) "poly_sigma" (finite, > 0) (winSize 13, polyN 5, pyrScale 0.5 are fixed), "use_tma" (1 = persistent
- * TMA-staged iteration kernel [default], 0 = the LDG-staged one), "time_kernels".  Every combination of the engine knobs
- * produces bit-identical flows.  Counts take whole numbers only, and on/off knobs 0 or 1.  "flag_sync" takes any whole
+ * "num_iters" (>= 1) "poly_sigma" (finite, > 0) (winSize 13, polyN 5, pyrScale 0.5 are fixed), "time_kernels".  Every
+ * combination of the engine knobs produces bit-identical flows.  Counts take whole numbers only, and on/off knobs 0 or 1.  "flag_sync" takes any whole
  * number >= 0; every value other than 0 means 1.  A refused value (NaN, an infinity, a fraction or
  * a value out of range) returns DFB_ERR_INVALID_ARG with "bad parameter <name>" and leaves the parameter unchanged.
  * Both algorithms: "jpeg_exact" (0 [default] = JPEG files through nvJPEG; 1 = every JPEG this handle writes is exactly the
@@ -385,7 +384,7 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   "farn_poly_exp"        in {level image}                  out {R0 .. R4}
  *   "farn_flow_init"       in {fx, fy of the coarser level}  out {fx, fy (scalars[0] x scalars[1])}; scalars {level w, level h}
  *   "farn_update_matrices" in {fx, fy, R0 x 5 (frame a), R1 x 5 (frame b)}  out {M0 .. M4}; scalars {pairs}
- *   "farn_iteration"       in {M x 5, R0 x 5, R1 x 5}        out {fx, fy, M'0 .. M'4}; scalars {use_tma, rebuild, pairs}
+ *   "farn_iteration"       in {M x 5, R0 x 5, R1 x 5}        out {fx, fy, M'0 .. M'4}; scalars {rebuild, pairs}
  *     (one box mean -> 2x2 solve -> rebuild of M iteration; M' is written only with rebuild = 1)
  *   The two pair stages run `pairs` (1..8, default 1) pairs in one launch: every plane then stacks the pairs' planes along
  *   its rows (height = pairs x the pair's height).

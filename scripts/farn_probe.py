@@ -1,7 +1,7 @@
-"""Farneback throughput (device-resident frames, 16 pairs per call) with the TMA-staged and the LDG-staged iteration kernel."""
+"""Farneback throughput (device-resident frames, 16 pairs per call) and iteration-kernel bandwidth per build variant."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np, torch
+import torch
 import denseflow_b200 as d
 from denseflow_b200 import synth
 variants = sys.argv[1].split(",") if len(sys.argv) > 1 else ["default"]
@@ -11,10 +11,9 @@ for (W, H) in sizes:
     fr = synth.stream(H, W, N, seed=2)
     dev = torch.from_numpy(fr).cuda()
     out = torch.empty((N - 1, H, W, 2), dtype=torch.float32, device="cuda")
-    ref = None
-    for variant, tma, tk in [(v, t, 1) for v in variants for t in ((0, 1) if v == variants[0] else (1,))]:
+    for variant in variants:
         e = d.FarnebackOpticalFlow.create(0, W, H, variant)
-        e.set("use_tma", tma); e.set("time_kernels", tk)
+        e.set("time_kernels", 1)
         for _ in range(2):
             e.calc_batch_device(dev, 1, out)
         torch.cuda.synchronize(); e.reset_counters()
@@ -25,10 +24,8 @@ for (W, H) in sizes:
         ev1.record(); torch.cuda.synchronize()
         dt = ev0.elapsed_time(ev1) / 1e3 / 3
         c = e.counters()
-        res = out.cpu().numpy()
-        if ref is None: ref = res.copy()
         kt = max(c["timed_kernel_ns"], 1) / 1e9 / 3
         print("%s " % variant, end="")
-        print("%dx%d use_tma=%d: %.3f ms/pair (%.1f pairs/s); iteration kernels %.3f ms/pair = %.0f GB/s at 88 B/px.iter; identical to LDG: %s" % (
-            W, H, tma, dt / (N - 1) * 1e3, (N - 1) / dt, kt / (N - 1) * 1e3, 88.0 * c["pixel_iters"] / 3 / kt / 1e9, np.array_equal(res, ref)))
+        print("%dx%d: %.3f ms/pair (%.1f pairs/s); iteration kernels %.3f ms/pair = %.0f GB/s at 88 B/px.iter" % (
+            W, H, dt / (N - 1) * 1e3, (N - 1) / dt, kt / (N - 1) * 1e3, 88.0 * c["pixel_iters"] / 3 / kt / 1e9))
         e.release()

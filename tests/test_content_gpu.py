@@ -4,7 +4,7 @@ and pan) at 1920 x 1080; and one stream whose consecutive pairs converge thousan
 
 * Strict build: the TV-L1 flow and iteration schedule equal the oracle's bit for bit with the fused kernel and with the
   unfused kernels (tests/tvl1_pin.py decides borderline convergence checks); the Farneback flow equals orc_farn_calc bit for
-  bit with TMA and with LDG staging.
+  bit.
 * Default build: every flow is finite.  A TV-L1 pair that converges somewhere is held to the 0.01 px AEE contract with an
   iteration total within 5 % of the oracle's.  A pair that runs into the 300-iteration cap at every (scale, warp) must have
   the oracle's schedule (300 everywhere); its flow is the result of 7 500 chaotic iterations, and the default build's
@@ -179,16 +179,9 @@ def test_farneback_content(oracle, case, variant):
     e = _handle("farn", variant)
     tag = "farn %s %s %dx%d" % (variant, name, w, h)
     if variant == "strict":
-        keep = e.get("use_tma")
-        try:
-            for tma in (1, 0):
-                e.set("use_tma", tma)
-                flow = e.calc(a, b)
-                diff = np.any(flow != ref, axis=-1)
-                assert not diff.any(), "%s use_tma %d: %d pixels differ from orc_farn_calc, first at %s" % (
-                    tag, tma, diff.sum(), tuple(np.argwhere(diff)[0]))
-        finally:
-            e.set("use_tma", keep)
+        flow = e.calc(a, b)
+        diff = np.any(flow != ref, axis=-1)
+        assert not diff.any(), "%s: %d pixels differ from orc_farn_calc, first at %s" % (tag, diff.sum(), tuple(np.argwhere(diff)[0]))
     else:
         flow = e.calc(a, b)
         assert np.isfinite(flow).all(), tag
@@ -260,7 +253,7 @@ def test_heterogeneous_stream(oracle, alg, variant):
     fr = cc.stream()
     w, h = cc.SIZE
     e = _handle(alg, variant, w, h)
-    single = _check_stream(e, alg, fr, TVL1_SETTINGS if alg == "tvl1" else [{"use_tma": 1}, {"use_tma": 0}])
+    single = _check_stream(e, alg, fr, TVL1_SETTINGS if alg == "tvl1" else [{}])
     notes = []
     if variant == "strict":
         for j, (flow, log) in enumerate(single):

@@ -85,10 +85,9 @@ def test_update_matrices(oracle, w, variant):
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
-@pytest.mark.parametrize("use_tma", [0, 1])
 @pytest.mark.parametrize("pairs", [1, 3, 8])
-def test_iteration(oracle, pairs, use_tma, variant):
-    """k_box_solve_update_tma<6> / k_box_solve_update<6>: every iteration shape, with and without the rebuild of M, several
+def test_iteration(oracle, pairs, variant):
+    """k_box_solve_update<6>: every iteration shape, with and without the rebuild of M, several
     pairs with different data in one launch (the persistent kernel's tile list runs over pairs x tile rows x tile columns)"""
     e, orc = _engine(variant), fc.Oracle(oracle)
     for si, (w, h) in enumerate(fc.ITER_SHAPES + fc.ITER_SMALL):
@@ -96,7 +95,7 @@ def test_iteration(oracle, pairs, use_tma, variant):
         ins = [_stack([c[2][k] for c in cases]) for k in range(5)]
         ins += [_stack([c[0][k] for c in cases]) for k in range(5)] + [_stack([c[1][k] for c in cases]) for k in range(5)]
         for rebuild in (0, 1):
-            out, _ = e.debug_run_kernel("farn_iteration", ins, 7, [use_tma, rebuild, pairs])
+            out, _ = e.debug_run_kernel("farn_iteration", ins, 7, [rebuild, pairs])
             for p, (R0, R1, M) in enumerate(cases):
                 tag = "%dx%d pair %d/%d rebuild %d" % (w, h, p, pairs, rebuild)
                 gx, gy = (_split(out[i], pairs)[p] for i in (0, 1))
@@ -139,13 +138,11 @@ def _assert_equal(got, want, name):
         name, diff.sum(), tuple(np.argwhere(diff)[0]), np.abs(got.astype(np.float64) - want).max())
 
 
-@pytest.mark.parametrize("use_tma", [0, 1])
 @pytest.mark.parametrize("shape", [(256, 256), (256, 340), (97, 131), (64, 64), (360, 640)])
-def test_strict_flow_is_bit_exact(oracle, shape, use_tma):
+def test_strict_flow_is_bit_exact(oracle, shape):
     h, w = shape
     a, b, _ = synth.pair(h, w, 0)
     e = _new(w, h)
-    e.set("use_tma", use_tma)
     _assert_equal(e.calc(a, b), oracle.farn_calc(a, b), "%dx%d" % (w, h))
 
 
@@ -201,11 +198,11 @@ def test_one_handle_many_sizes(oracle, variant):
     smaller frames): every flow equals a fresh handle's (and the oracle's in the strict build)"""
     e = _new(640, 360, variant)
     runs = [((360, 640), {}), ((97, 131), {}), ((64, 64), {"num_iters": 3}), ((201, 333), {"num_levels": 3, "num_iters": 10}),
-            ((360, 640), {"use_tma": 0}), ((97, 131), {"use_tma": 1, "num_levels": 5}), ((256, 340), {"num_iters": 10})]
+            ((360, 640), {}), ((97, 131), {"num_levels": 5}), ((256, 340), {"num_iters": 10})]
     for i, ((h, w), params) in enumerate(runs):
         for k, v in params.items():
             e.set(k, v)
-        cur = {k: e.get(k) for k in ("num_levels", "num_iters", "use_tma")}
+        cur = {k: e.get(k) for k in ("num_levels", "num_iters")}
         a, b, _ = synth.pair(h, w, 20 + i)
         got = e.calc(a, b)
         fresh = _new(w, h, variant)

@@ -345,17 +345,13 @@ def test_farneback_off_defaults(oracle, shape, variant):
             for iters in (1, 25):
                 tag = "farn %s %dx%d poly_sigma %g num_iters %d" % (variant, w, h, sigma, iters)
                 e.set("poly_sigma", sigma).set("num_iters", iters)
-                flows = []
-                for tma in (1, 0):
-                    e.set("use_tma", tma)
-                    flows.append(e.calc(a, b))
-                _same(flows[1], flows[0], tag + " LDG vs TMA staging")
+                flow = e.calc(a, b)
                 if variant == "strict":
-                    _same(flows[0], oracle.farn_calc(a, b, oracle.farn_params(poly_sigma=sigma, num_iters=iters)), tag + " vs orc_farn_calc")
+                    _same(flow, oracle.farn_calc(a, b, oracle.farn_params(poly_sigma=sigma, num_iters=iters)), tag + " vs orc_farn_calc")
                 else:
-                    assert np.isfinite(flows[0]).all(), tag
+                    assert np.isfinite(flow).all(), tag
     finally:
-        e.set("poly_sigma", 1.1).set("num_iters", 10).set("use_tma", 1)
+        e.set("poly_sigma", 1.1).set("num_iters", 10)
 
 
 # ---- refusals -----------------------------------------------------------------------------------------------------------
@@ -371,14 +367,14 @@ REFUSED = {
              "serial_launches": FLAG, "lanes": NOT_FINITE + [-1, 65, 2.5]},
     "farn": {"num_levels": NOT_FINITE + [-1, 6, 2.5], "num_iters": NOT_FINITE + [0, -1, 2.5, 1e10],
              "poly_sigma": NOT_FINITE + [0, -1.1], "pyr_scale": NOT_FINITE + [0, 0.25], "win_size": NOT_FINITE + [15, 13.5],
-             "poly_n": NOT_FINITE + [7], "time_kernels": FLAG, "use_tma": FLAG},
+             "poly_n": NOT_FINITE + [7], "time_kernels": FLAG},
 }
 ACCEPTED = {
     "tvl1": [("nscales", 1), ("nscales", 16), ("warps", 1), ("warps", 16), ("fused_k", 1), ("fused_k", 8), ("lanes", 64), ("lanes", 0),
              ("lambda", 0), ("epsilon", 0), ("epsilon", -1), ("iterations", 1), ("iterations", 2 ** 31 - 1), ("scale_step", 0.8),
              ("scale_step", 0.05), ("tau", 1e-3), ("theta", 5.0), ("flag_sync", 0), ("flag_sync", 200), ("fused", 0)],
     "farn": [("num_levels", 0), ("num_levels", 5), ("num_iters", 1), ("poly_sigma", 0.8), ("pyr_scale", 0.5), ("win_size", 13),
-             ("poly_n", 5), ("use_tma", 0)],
+             ("poly_n", 5)],
 }
 
 
@@ -400,6 +396,13 @@ def test_set_refuses_bad_values_and_keeps_the_old_one(alg, variant):
             after = C.c_double()
             assert L.dfb_get_param(e._h, name.encode(), C.byref(after)) == _lib.DFB_OK
             assert after.value == before, (alg, name, v, after.value, before)
+    if alg == "farn":  # "use_tma" is a TV-L1 knob: a Farneback handle refuses it like any name it does not know
+        before = {n: e.get(n) for n in REFUSED["farn"]}
+        for v in (0, 1):
+            assert L.dfb_set_param(e._h, b"use_tma", float(v)) == _lib.DFB_ERR_INVALID_ARG
+            assert L.dfb_last_error(e._h).decode() == "bad parameter use_tma"
+        assert L.dfb_get_param(e._h, b"use_tma", C.byref(C.c_double())) == _lib.DFB_ERR_INVALID_ARG
+        assert {n: e.get(n) for n in REFUSED["farn"]} == before
     e.release()
     del _handles[(alg, variant, 64, 64)]
 
