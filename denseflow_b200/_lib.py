@@ -10,6 +10,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATHS = {
     "default": os.path.join(_HERE, "lib", "libdenseflow_b200.so"),
     "strict": os.path.join(_HERE, "lib", "libdenseflow_b200_strict.so"),
+    # the default library with the -st=h5 file writer (the reference's -DUSE_HDF5=yes build)
+    "hdf5": os.path.join(_HERE, "lib", "libdenseflow_b200_hdf5.so"),
+    "strict_hdf5": os.path.join(_HERE, "lib", "libdenseflow_b200_strict_hdf5.so"),
     # geometry experiments (denseflow_b200/build.py VARIANTS), built on request only
     "t256": os.path.join(_HERE, "lib", "libdenseflow_b200_t256.so"),
     "t512": os.path.join(_HERE, "lib", "libdenseflow_b200_t512.so"),
@@ -53,6 +56,7 @@ VIDEO_BGR = 0
 VIDEO_JPEG = 1
 SAVE_JPG = 0
 SAVE_PNG = 1
+SAVE_H5 = 2
 
 
 class Video(C.Structure):
@@ -85,6 +89,10 @@ SIGNATURES = {
                                          C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
     "dfb_calc_batch_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                         C.c_void_p]),
+    "dfb_calc_batch_host_planes": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "dfb_calc_batch_device_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                               C.c_void_p]),
     "dfb_quantise_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_void_p, C.c_size_t, C.c_void_p]),
     "dfb_flow_to_png_image_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
@@ -118,6 +126,13 @@ SIGNATURES = {
                                                  C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
     "dfb_process_jpeg_batch_host_png": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int,
                                                   C.c_int, C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "dfb_process_bgr_batch_host_planes": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                    C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "dfb_process_jpeg_batch_host_planes": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int,
+                                                     C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "dfb_h5_create": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),
+    "dfb_h5_write_float": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_void_p]),
+    "dfb_h5_close": (C.c_int, [C.c_void_p]),
     "dfb_extract_frames_jpeg_host": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
                                                C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_size_t)]),
     "dfb_new_size": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

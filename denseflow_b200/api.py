@@ -154,6 +154,82 @@ class DenseOpticalFlow:
                                                   C.c_void_p(s)))
         return flows
 
+    # -- the flow as two float planes per pair: the payloads of -st=h5's flow_x / flow_y datasets --
+    @staticmethod
+    def _plane_ptrs(out, m):
+        xp = (C.c_void_p * max(m, 1))(*[out[i, 0].ctypes.data for i in range(m)])
+        yp = (C.c_void_p * max(m, 1))(*[out[i, 1].ctypes.data for i in range(m)])
+        return xp, yp
+
+    def calc_batch_planes(self, frames, step=1, out=None):
+        """calc_batch with the flow channels first: float32 [M,2,H,W], out[j,0] / out[j,1] bit for bit flows[j,...,0] /
+        flows[j,...,1].  The engines' merge epilogue writes the planes; out may be a caller (e.g. page-locked) array."""
+        frames = self._gray_frames(frames)
+        n = len(frames)
+        if n == 0:
+            return np.empty((0, 2, 0, 0), np.float32)
+        h, w = frames[0].shape
+        m = max(n - abs(step), 0)
+        if out is None:
+            out = np.empty((m, 2, h, w), np.float32)
+        self._check_out(out, (m, 2, h, w), np.float32, "out")
+        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
+        xp, yp = self._plane_ptrs(out, m)
+        self._check(self._L.dfb_calc_batch_host_planes(self._h, fp, n, step, w, h, xp, yp))
+        return out
+
+    def calc_batch_device_planes(self, frames, step=1, planes=None, stream=None):
+        """frames: CUDA uint8 tensor [N,H,W] (contiguous); planes: CUDA float32 [M,2,H,W] (contiguous)."""
+        import torch
+        n, h, w = frames.shape
+        m = max(n - abs(step), 0)
+        if planes is None:
+            planes = torch.empty((m, 2, h, w), dtype=torch.float32, device=frames.device)
+        if planes.dtype != torch.float32 or tuple(planes.shape) != (m, 2, h, w) or not planes.is_contiguous():
+            raise RuntimeError("planes: expected a contiguous float32 CUDA tensor of shape %s" % ((m, 2, h, w),))
+        s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
+        self._check(self._L.dfb_calc_batch_device_planes(self._h, frames.data_ptr(), n, step, w, h, planes.data_ptr(),
+                                                         C.c_void_p(s)))
+        return planes
+
+    def process_bgr_batch_planes(self, frames_bgr, step=1, new_size=None):
+        """-st=h5 payloads for decoded BGR frames: gray -> resize -> flow -> float32 [M,2,dh,dw], bit for bit calc_batch_planes of
+        the gray, resized frames."""
+        frames = self._bgr_frames(frames_bgr, "process_bgr_batch_planes")
+        n = len(frames)
+        if n == 0:
+            return np.empty((0, 2, 0, 0), np.float32)
+        sh, sw = frames[0].shape[:2]
+        dw, dh = new_size if new_size else (0, 0)
+        ow, oh = new_size if new_size else (sw, sh)
+        m = max(n - abs(step), 0)
+        out = np.empty((m, 2, oh, ow), np.float32)
+        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
+        xp, yp = self._plane_ptrs(out, m)
+        self._check(self._L.dfb_process_bgr_batch_host_planes(self._h, fp, n, step, sw, sh, dw, dh, xp, yp))
+        return out
+
+    def process_jpeg_batch_planes(self, jpegs, step=1, new_size=None):
+        """-if -st=h5 payloads: process_bgr_batch_planes with the frames given as JPEG files of one size, decoded on the GPU to
+        imdecode's pixels."""
+        keep, ptrs, lens = self._jpeg_buffers(jpegs)
+        n = len(keep)
+        m = max(n - abs(step), 0)
+        if m == 0:
+            return np.empty((0, 2, 0, 0), np.float32)
+        dw, dh = new_size if new_size else (0, 0)
+        if new_size:
+            ow, oh = new_size
+        else:  # the size of the frames (the call checks that all have frame 0's)
+            w, h = C.c_int(), C.c_int()
+            if self._L.dfb_jpeg_info(ptrs[0], lens[0], C.byref(w), C.byref(h)) != _lib.DFB_OK:
+                raise RuntimeError(self._L.dfb_last_error(None).decode())
+            ow, oh = w.value, h.value
+        out = np.empty((m, 2, oh, ow), np.float32)
+        xp, yp = self._plane_ptrs(out, m)
+        self._check(self._L.dfb_process_jpeg_batch_host_planes(self._h, ptrs, lens, n, step, dw, dh, xp, yp))
+        return out
+
     def quantise_device(self, flow, bound):
         import torch
         h, w = flow.shape[:2]

@@ -24,7 +24,18 @@ VARIANTS = {
     # geometry experiments of the fused tvl1 kernel (not built by default): python -m denseflow_b200.build t256
     "t256": ("libdenseflow_b200_t256.so", ["-DDFB_FUSED_THREADS=256"]),
     "t512": ("libdenseflow_b200_t512.so", ["-DDFB_FUSED_THREADS=512"]),
+    # the reference's -DUSE_HDF5=yes build: the default library plus the -st=h5 file writer
+    "hdf5": ("libdenseflow_b200_hdf5.so", ["-DDFB_USE_HDF5=1"]),
+    # the strict library with the writer: lets tests compare the command's h5 files with the oracle
+    "strict_hdf5": ("libdenseflow_b200_strict_hdf5.so", ["-DDFB_STRICT_FP", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
+                                                         "-DDFB_USE_HDF5=1"]),
 }
+
+# Variants whose macro only some translation units read: (the variant whose objects they link for every other source, those
+# sources).  Only the listed sources are compiled again.
+RELINKED = {"hdf5": ("default", ("h5_writer.cu",)), "strict_hdf5": ("strict", ("h5_writer.cu",))}
+
+DEFAULT_VARIANTS = ("default", "strict", "hdf5", "strict_hdf5")
 
 
 def _sources():
@@ -44,18 +55,29 @@ def _run(cmd):
     return r.stdout + r.stderr
 
 
-def build(variants=("default", "strict"), verbose=False, force=False):
+def build(variants=DEFAULT_VARIANTS, verbose=False, force=False):
     os.makedirs(LIBDIR, exist_ok=True)
     hm = _headers_mtime()
     outs = []
+    # a relinked variant's base is built first (its objects must be current)
+    order = []
     for v in variants:
+        if v in RELINKED and RELINKED[v][0] not in order:
+            order.append(RELINKED[v][0])
+        if v not in order:
+            order.append(v)
+    for v in order:
         out_name, extra = VARIANTS[v]
+        base, own = RELINKED.get(v, (v, None))
         objdir = os.path.join(LIBDIR, "obj_" + v)
         os.makedirs(objdir, exist_ok=True)
         jobs = []
         objs = []
         for src in _sources():
             sp = os.path.join(CSRC, src)
+            if own is not None and src not in own:
+                objs.append(os.path.join(LIBDIR, "obj_" + base, src[:-3] + ".o"))
+                continue
             obj = os.path.join(objdir, src[:-3] + ".o")
             objs.append(obj)
             if force or not os.path.exists(obj) or os.path.getmtime(obj) < max(os.path.getmtime(sp), hm):
@@ -68,12 +90,13 @@ def build(variants=("default", "strict"), verbose=False, force=False):
                 if verbose and log.strip():
                     print(log)
         out = os.path.join(LIBDIR, out_name)
-        if jobs or not os.path.exists(out):
+        if jobs or not os.path.exists(out) or any(os.path.getmtime(o) > os.path.getmtime(out) for o in objs):
             _run([NVCC] + ARCH + ["-shared", "-o", out] + objs + ["-cudart", "shared", "-ldl", "-Xlinker", "-rpath=/usr/local/cuda/lib64"])
-        outs.append(out)
+        if v in variants:
+            outs.append(out)
     return outs
 
 
 if __name__ == "__main__":
-    names = tuple(a for a in sys.argv[1:] if a in VARIANTS) or ("default", "strict")
+    names = tuple(a for a in sys.argv[1:] if a in VARIANTS) or DEFAULT_VARIANTS
     print("\n".join(build(names, verbose="-v" in sys.argv, force="-f" in sys.argv)))

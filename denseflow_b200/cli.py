@@ -7,6 +7,11 @@ takes the reference's flags and writes its file tree: `<o>/[<class>/]<stem>/flow
 skips unless -f is given.  Videos are decoded with cv2.VideoCapture on the worker threads, one window of frames at a time,
 so a list of long videos runs in bounded memory; `-if` folders go to the GPU as JPEG bytes and are decoded there.  Every
 visible GPU runs two workers.  Errors print their message and exit 1, as the reference's main() does.
+
+`-st=h5` in flow mode needs the library built with HDF5 support, the counterpart of the reference's -DUSE_HDF5=yes build:
+`DFB_LIBRARY=hdf5 python -m denseflow_b200 ...` writes each video's flows as float32 datasets /flow_x_%05d and /flow_y_%05d to
+`<output dir>.h5` (`_p<s>` / `_m<|s|>` before `.h5` for other steps).  The default library refuses it with the reference's
+"HDF5 support is not enabled, pls recompile".
 """
 import os
 import re
@@ -289,9 +294,20 @@ def _unsupported_algorithm(L, algorithm):
     return L.dfb_last_error(None).decode()
 
 
+def _unsupported_h5(L):
+    """The library's refusal of -st=h5 when it is built without HDF5 support, or None.  A null path is refused before any
+    file is touched by a library that has the writer."""
+    import ctypes as C
+    from . import _lib
+    f = C.c_void_p()
+    if L.dfb_h5_create(None, C.byref(f)) == _lib.DFB_ERR_UNSUPPORTED:
+        return L.dfb_last_error(None).decode()
+    return None
+
+
 def run(opt, out=_print, variant="default"):
     """calcDenseFlowVideoGPU (src/denseflow_gpu.cpp:479-497) for the planned videos on every visible GPU, with the library
-    `variant` (the command uses the default build)."""
+    `variant` (the command uses $DFB_LIBRARY, default "default")."""
     from . import _lib, listrun
     videos, outdirs, is_record = plan(opt, out)
     if not videos:
@@ -301,9 +317,12 @@ def run(opt, out=_print, variant="default"):
         out(msg)
         raise CliError("check init param error.")
     step, save_type, verbose = opt["step"], opt["saveType"], opt["verbose"]
-    if step != 0 and save_type == "h5":
-        raise CliError("HDF5 support is not enabled, pls recompile")
     L = _lib.load(variant)
+    h5_out = step != 0 and save_type == "h5"
+    if h5_out:
+        refusal = _unsupported_h5(L)
+        if refusal:
+            raise CliError(refusal)
     if step != 0:
         refusal = _unsupported_algorithm(L, opt["algorithm"])
         if refusal:
@@ -327,6 +346,9 @@ def run(opt, out=_print, variant="default"):
             if not files:
                 if verbose:
                     say(quoted(vid) + " is empty!")
+                if h5_out:  # the reference creates the file before it finds no frame, and closes it empty (no marker)
+                    from . import h5
+                    h5.File(listrun.h5_path(outdir, step), variant=variant).close()
                 continue
             jobs.append((vid, outdir, files))
         else:
@@ -337,16 +359,28 @@ def run(opt, out=_print, variant="default"):
 def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
     """The non-empty inputs through ListRunner.run_stream: files into each output directory, then the summary line."""
     from . import _lib, listrun
+    import numpy as np
+    from . import api, h5
     step, save_type = opt["step"], opt["saveType"]
+    h5_out = step != 0 and save_type == "h5"
     readers = {}
+    h5_files = {}  # video -> its open h5 file, from the video's start to its last chunk
+    sizes = {}     # video -> (dh, dw), the size of its flows
     failures = []
 
     def source(video, first, max_n):
         try:
             if first == 0:
-                vid, _, files = jobs[video]
+                vid, outdir, files = jobs[video]
+                if h5_out:  # created (or truncated) before the first frame is decoded
+                    h5_files[video] = h5.File(listrun.h5_path(outdir, step), variant=variant)
                 readers[video] = FolderReader(files) if files is not None else VideoReader(vid)
             frames = readers[video].window(first, max_n)
+            if h5_out and video not in sizes and frames:
+                f0 = frames[0]
+                sw, sh = (f0.shape[1], f0.shape[0]) if hasattr(f0, "shape") else api.jpeg_info(f0, variant)
+                dw, dh = api.new_size(sw, sh, opt["newWidth"], opt["newHeight"], opt["newShort"], variant)
+                sizes[video] = (dh, dw)
             if len(frames) < max_n:
                 readers.pop(video).close()
             return frames
@@ -356,6 +390,19 @@ def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
 
     def on_chunk(video, dev, first, last, files):
         outdir = jobs[video][1]
+        if h5_out:
+            # writeHDF5's order: every x of the chunk, then every y (files 2 i / 2 i + 1 are flow i's x / y plane)
+            n = len(files) // 2
+            f = h5_files[video]
+            for name, k in zip(listrun.h5_names(step, first, n), [2 * i for i in range(n)] + [2 * i + 1 for i in range(n)]):
+                f.write_float(name, np.frombuffer(files[k], np.float32).reshape(sizes[video]))
+            if last:
+                h5_files.pop(video).close()  # before the marker
+                if is_record:
+                    done_file, title = marker(outdir, opt["classFolder"])
+                    open(done_file, "wb").close()
+                    say("done video " + quoted(title))
+            return
         for name, data in zip(listrun.output_names(step, first, len(files) // (2 if step != 0 and save_type == "jpg" else 1), save_type),
                               files):
             with open(path_join(outdir, name), "wb") as f:
@@ -380,6 +427,8 @@ def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
             r.close()
             for rd in readers.values():
                 rd.close()
+            for f in h5_files.values():  # a failed video's file keeps what was written before the failure; it gets no marker
+                f.close()
     t = time.time() - t0
     n, f = st["frames"], st["flows"]
     say("%d videos (%d frames, %d %s flows) processed, using %ss, decoding speed %sfps, flow speed %sfps"
@@ -394,7 +443,11 @@ def main(argv=None, out=_print):
         out(help_text())
         return 0
     try:
-        run(opt, out)
+        variant = os.environ.get("DFB_LIBRARY", "default")
+        from . import _lib
+        if variant not in _lib.LIB_PATHS:
+            raise CliError("unknown DFB_LIBRARY %s (%s)" % (variant, " | ".join(sorted(_lib.LIB_PATHS))))
+        run(opt, out, variant=variant)
     except (CliError, OSError, RuntimeError) as ex:
         out(str(ex))
         return 1

@@ -33,6 +33,9 @@ inline void check(cudaError_t e, const char *what, const char *file, int line) {
 #define DFB_CUDA(x) ::dfb::check((x), #x, __FILE__, __LINE__)
 #define DFB_KERNEL_CHECK() ::dfb::check(cudaGetLastError(), "kernel launch", __FILE__, __LINE__)
 
+// The error of a call without a handle: dfb_last_error(NULL) reports msg afterwards (dfb_api.cu).  Returns code.
+int fail_unbound(int code, const std::string &msg);
+
 // convertFlowToImage, /root/reference/src/common.cpp:4-16: the CAST macro evaluates in double (the bounds are double),
 // left to right, then cvRound (round-half-to-even).  Shared by the stand-alone quantiser and the merge epilogues.
 #ifdef __CUDACC__

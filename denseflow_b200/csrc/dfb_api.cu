@@ -123,6 +123,12 @@ int fail(dfb_handle *h, int code, const std::string &msg) {
     return code;
 }
 
+}  // namespace
+
+int dfb::fail_unbound(int code, const std::string &msg) { return fail(nullptr, code, msg); }
+
+namespace {
+
 // after a failure in the middle of a call no copy into a caller buffer may still be in flight when the call returns
 void quiesce(dfb_handle *h) {
     if (!h) return;
@@ -528,6 +534,46 @@ FlowOutput host_u8_output(dfb_handle *h, uint8_t *const *qx, uint8_t *const *qy,
     return o;
 }
 
+// Where the two float planes of each pair go (-st=h5 payloads): pair j's x plane to x[j], its y plane to y[j], w x h floats each
+struct PlanesOut {
+    float *const *x, *const *y;
+};
+
+// dfb_calc_batch_host_planes and the _planes chains: the engine's merge epilogue writes pair j's u1 / u2 as two dense float
+// planes, which go to x[j] / y[j] as the float2 fields go to flows[j] above (pinned: a direct DMA, else through the pair's
+// pinned staging buffer).  px: pixels each plane reserves.
+FlowOutput planes_output(dfb_handle *h, const PlanesOut &po, int B, int w, int hh, size_t px) {
+    const size_t bytes = (size_t)w * hh * sizeof(float);
+    h->flow_out.grow(2 * B * px * 2 * sizeof(float));
+    auto plane = [=](int p, int c) { return reinterpret_cast<float *>(h->flow_out + ((size_t)p * 2 + c) * px * sizeof(float)); };
+    auto direct = [=](int j) { return is_pinned_host(po.x[j]) && is_pinned_host(po.y[j]); };
+    FlowOutput o;
+    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
+        pj.fx = plane(p, 0);
+        pj.fy = plane(p, 1);
+        pj.f_pitch = (size_t)w * sizeof(float);
+    };
+    o.send = [=](int j0, int m, int slot) {
+        for (int i = 0; i < m; ++i) {
+            const int j = j0 + i, p = slot * B + i;
+            const bool d = direct(j);
+            float *dx = d ? po.x[j] : stage_flow(h, p), *dy = d ? po.y[j] : stage_flow(h, p) + (size_t)w * hh;
+            DFB_CUDA(cudaMemcpyAsync(dx, plane(p, 0), bytes, cudaMemcpyDeviceToHost, h->s_out));
+            DFB_CUDA(cudaMemcpyAsync(dy, plane(p, 1), bytes, cudaMemcpyDeviceToHost, h->s_out));
+            h->counters.d2h_bytes += 2 * bytes;
+        }
+    };
+    o.finish = [=](int j0, int m, int slot) {
+        for (int i = 0; i < m; ++i)
+            if (!direct(j0 + i)) {
+                DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
+                std::memcpy(po.x[j0 + i], h->h_flow[slot * B + i], bytes);
+                std::memcpy(po.y[j0 + i], h->h_flow[slot * B + i] + (size_t)w * hh, bytes);
+            }
+    };
+    return o;
+}
+
 // -st=jpg output of a flow chain: pair j's two quantised planes (bound) as JPEGs to x[j] / y[j], their lengths to len_x[j] /
 // len_y[j]; every buffer holds `capacity` bytes
 struct JpgOut {
@@ -673,8 +719,9 @@ int flow_groups(dfb_handle *h, int n_frames, int step, int w, int hh, int B, con
 // The calc calls over host buffers.
 // quantise: bound > 0 => emit two u8 planes per pair instead of the float2 field.
 // png: non-null => pack every flow field (convertFlowToPngImage) and emit imencode(".png") of it instead of the field.
+// planes: non-null => emit the two float planes of every pair instead of the field.
 int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, float *const *flows,
-               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngOut *png = nullptr) {
+               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngOut *png = nullptr, const PlanesOut *planes = nullptr) {
     if (int rc = check_size(h, w, hh)) return rc;
     if (n_frames < 0 || !frames) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
@@ -684,8 +731,11 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
         if (!frames[f] || host_pointer_kind(frames[f]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "frames[" + std::to_string(f) + "] is null or a device pointer (host entry point: use dfb_calc_batch_device)");
     for (int j = 0; j < M; ++j) {
-        const void *o0 = png ? (const void *)png->out[j] : bound > 0 ? (const void *)qx[j] : (const void *)flows[j];
-        const void *o1 = bound > 0 ? (const void *)qy[j] : o0;
+        const void *o0 = png      ? (const void *)png->out[j]
+                         : bound > 0 ? (const void *)qx[j]
+                         : planes    ? (const void *)planes->x[j]
+                                     : (const void *)flows[j];
+        const void *o1 = bound > 0 ? (const void *)qy[j] : planes ? (const void *)planes->y[j] : o0;
         if (!o0 || !o1 || host_pointer_kind(o0) < 0 || host_pointer_kind(o1) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
     }
@@ -693,8 +743,9 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
     // output slots at the handle's maximum frame, so that calls of other sizes reuse them (a 1080p handle runs 7 pairs per
     // group, a 340x256 one up to 64)
     const size_t px = (size_t)h->max_w * h->max_h;
-    const FlowOutput o = png ? png_output(h, *png, B, w, hh, px)
+    const FlowOutput o = png         ? png_output(h, *png, B, w, hh, px)
                          : bound > 0 ? host_u8_output(h, qx, qy, bound, B, w, hh, px)
+                         : planes    ? planes_output(h, *planes, B, w, hh, px)
                                      : host_flow_output(h, flows, B, w, hh, px);
     return flow_groups(h, n_frames, step, w, hh, B, upload_ring(h, frames, n_frames, w, hh), o);
 }
@@ -841,8 +892,25 @@ int dfb_calc_batch_host_u8(dfb_handle *h, const uint8_t *const *frames, int n_fr
     });
 }
 
-int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height,
-                          float *flows, void *stream) {
+int dfb_calc_batch_host_planes(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
+                               float *const *fx, float *const *fy) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (n_frames > std::abs(step) && (!fx || !fy)) return fail(h, DFB_ERR_INVALID_ARG, "fx/fy is null");
+    const PlanesOut planes{fx, fy};
+    return guarded(h, [&]() {
+        DFB_CUDA(cudaSetDevice(h->device));
+        return batch_host(h, frames, n_frames, step, width, height, nullptr, 0, nullptr, nullptr, nullptr, &planes);
+    });
+}
+
+}  // extern "C"
+
+namespace {
+
+// dfb_calc_batch_device[_planes]: pair j's flow to out + j * 2 w h floats, as one float2 field or (planar) as the x plane
+// followed by the y plane
+int batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height, float *flows, bool planar,
+                 void *stream) {
     if (!h) return DFB_ERR_INVALID_ARG;
     if (int rc = check_size(h, width, height)) return rc;
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
@@ -867,14 +935,35 @@ int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, in
             for (int i = 0; i < m; ++i) {
                 const int j = j0 + i;
                 jobs[i] = pair_job(j, step, nslots);
-                jobs[i].flow_xy = flows + (size_t)j * fbytes * 2;
-                jobs[i].flow_pitch_bytes = (size_t)width * 8;
+                float *out = flows + (size_t)j * fbytes * 2;
+                if (planar) {
+                    jobs[i].fx = out;
+                    jobs[i].fy = out + fbytes;
+                    jobs[i].f_pitch = (size_t)width * 4;
+                } else {
+                    jobs[i].flow_xy = out;
+                    jobs[i].flow_pitch_bytes = (size_t)width * 8;
+                }
             }
             alg.solve_batch(jobs.data(), m, width, height, s);
             h->counters.pairs += m;
         }
         return DFB_OK;
     });
+}
+
+}  // namespace
+
+extern "C" {
+
+int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height,
+                          float *flows, void *stream) {
+    return batch_device(h, frames, n_frames, step, width, height, flows, false, stream);
+}
+
+int dfb_calc_batch_device_planes(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height,
+                                 float *planes, void *stream) {
+    return batch_device(h, frames, n_frames, step, width, height, planes, true, stream);
 }
 
 int dfb_quantise_device(dfb_handle *h, const float *flow_xy, size_t flow_pitch, int width, int height, int bound,
@@ -1054,13 +1143,15 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
 
 namespace {
 
-// Where the files of a flow chain go: exactly one of the two is set.
+// Where the outputs of a flow chain go: exactly one of the three is set.
 struct ChainOut {
     const JpgOut *jpg;
     const PngOut *png;
+    const PlanesOut *planes = nullptr;
 };
 
 bool chain_outputs_null(const ChainOut &o) {
+    if (o.planes) return !o.planes->x || !o.planes->y;
     return o.png ? (!o.png->out || !o.png->len) : (!o.jpg->x || !o.jpg->y || !o.jpg->len_x || !o.jpg->len_y);
 }
 
@@ -1068,7 +1159,10 @@ bool chain_outputs_null(const ChainOut &o) {
 int check_chain_outputs(dfb_handle *h, int M, const ChainOut &o) {
     if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
     for (int j = 0; j < M; ++j) {
-        if (o.png) {
+        if (o.planes) {
+            if (!o.planes->x[j] || !o.planes->y[j] || host_pointer_kind(o.planes->x[j]) < 0 || host_pointer_kind(o.planes->y[j]) < 0)
+                return fail(h, DFB_ERR_INVALID_ARG, "plane output " + std::to_string(j) + " is null or a device pointer (host entry point)");
+        } else if (o.png) {
             if (!o.png->out[j] || host_pointer_kind(o.png->out[j]) < 0)
                 return fail(h, DFB_ERR_INVALID_ARG, "png output " + std::to_string(j) + " is null or a device pointer (host entry point)");
         } else if (!o.jpg->x[j] || !o.jpg->y[j] || host_pointer_kind(o.jpg->x[j]) < 0 || host_pointer_kind(o.jpg->y[j]) < 0) {
@@ -1079,10 +1173,13 @@ int check_chain_outputs(dfb_handle *h, int M, const ChainOut &o) {
 }
 
 // The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) by `produce` (dense_frames) -> flow -> the
-// output of `o`: quantise and two JPEGs per pair, or convertFlowToPngImage and one PNG per pair.  Runs inside guarded().
+// output of `o`: quantise and two JPEGs per pair, convertFlowToPngImage and one PNG per pair, or the two float planes of each
+// pair.  Runs inside guarded().
 int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const ChainOut &o, const std::function<void(int, int)> &produce) {
     const int B = std::max(1, std::min(h->alg->max_concurrent_pairs(dw, dh), 8));
-    const FlowOutput out = o.png ? png_output(h, *o.png, B, dw, dh, (size_t)dw * dh) : jpg_output(h, *o.jpg, B, dw, dh);
+    const FlowOutput out = o.planes ? planes_output(h, *o.planes, B, dw, dh, (size_t)dw * dh)
+                           : o.png  ? png_output(h, *o.png, B, dw, dh, (size_t)dw * dh)
+                                    : jpg_output(h, *o.jpg, B, dw, dh);
     return flow_groups(h, n_frames, step, dw, dh, B, dense_frames(h, n_frames, dw, dh, produce), out);
 }
 
@@ -1294,6 +1391,18 @@ int dfb_process_jpeg_batch_host_png(dfb_handle *h, const uint8_t *const *jpeg, c
                                     int dh, uint8_t *const *png, size_t capacity, size_t *len) {
     const PngOut o{png, capacity, len};
     return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, {nullptr, &o});
+}
+
+int dfb_process_bgr_batch_host_planes(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
+                                      float *const *fx, float *const *fy) {
+    const PlanesOut o{fx, fy};
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, {nullptr, nullptr, &o});
+}
+
+int dfb_process_jpeg_batch_host_planes(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step, int dw,
+                                       int dh, float *const *fx, float *const *fy) {
+    const PlanesOut o{fx, fy};
+    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, {nullptr, nullptr, &o});
 }
 
 int dfb_new_size(int width, int height, int new_width, int new_height, int new_short, int *dw, int *dh) {

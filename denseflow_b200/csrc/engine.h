@@ -111,6 +111,10 @@ class FlowAlgorithm {
         int bound = 0;
         uint8_t *qx = nullptr, *qy = nullptr;
         size_t q_pitch = 0;
+        // fx set (bound = 0): the merge epilogue writes u1 to fx and u2 to fy as two float planes (row pitch f_pitch bytes), the
+        // payloads of an h5 file's flow_x / flow_y datasets, INSTEAD of the float2 field; flow_xy may then be null
+        float *fx = nullptr, *fy = nullptr;
+        size_t f_pitch = 0;
     };
     virtual int max_concurrent_pairs(int w, int h) { (void)w; (void)h; return 1; }
     // after a CUDA error: what the engine's own watchdogs recorded (empty if nothing)

@@ -323,6 +323,8 @@ struct PairArgs {
     int bound;  // > 0: the merge writes the two quantised uint8 planes instead (PairJob)
     uint8_t *qx, *qy;
     size_t q_pitch;
+    float *ox, *oy;  // non-null: the merge writes the two float planes instead (PairJob::fx / fy)
+    size_t o_pitch;
 };
 struct FarnBatchArgs {
     PairArgs p[kMaxFarnBatch];
@@ -580,6 +582,12 @@ __global__ void __launch_bounds__(256) k_farn_merge(const __grid_constant__ Farn
     if (a.bound > 0) {  // convertFlowToImage (src/common.cpp:4-16) as the epilogue
         a.qx[(size_t)y * a.q_pitch + x] = quantise_px(u, -(double)a.bound, (double)a.bound);
         a.qy[(size_t)y * a.q_pitch + x] = quantise_px(v, -(double)a.bound, (double)a.bound);
+        return;
+    }
+    if (a.ox) {
+        const size_t d = (size_t)y * (a.o_pitch >> 2) + x;
+        a.ox[d] = u;
+        a.oy[d] = v;
         return;
     }
     float2 *row = reinterpret_cast<float2 *>(reinterpret_cast<char *>(a.flow_xy) + (size_t)y * a.flow_pitch_bytes);
@@ -1090,6 +1098,9 @@ class Farneback final : public FlowAlgorithm {
         a.qx = job.qx;
         a.qy = job.qy;
         a.q_pitch = job.q_pitch;
+        a.ox = job.fx;
+        a.oy = job.fy;
+        a.o_pitch = job.f_pitch;
         return a;
     }
     static dim3 grid8(const Level &L, int nb) { return dim3(ceil_div(L.w, 32), ceil_div(L.h, 8), nb); }

@@ -246,7 +246,7 @@ struct VideoArgs {
 // rule.  Fills a, or writes the message and returns the code.
 int check_video_args(const char *name, int step, int bound, int save_type, int quality, int jpeg_exact, int new_width, int new_height,
                      int new_short, int chunk_flows, VideoArgs &a, char *err, size_t err_len) {
-    if ((save_type != DFB_SAVE_JPG && save_type != DFB_SAVE_PNG) || (jpeg_exact != 0 && jpeg_exact != 1)) {
+    if ((save_type != DFB_SAVE_JPG && save_type != DFB_SAVE_PNG && save_type != DFB_SAVE_H5) || (jpeg_exact != 0 && jpeg_exact != 1)) {
         set_error(err, err_len, std::string(name) + ": bad arguments (save_type is DFB_SAVE_JPG or DFB_SAVE_PNG, jpeg_exact 0 or 1)");
         return DFB_ERR_INVALID_ARG;
     }
@@ -318,7 +318,7 @@ struct Window {
 template <typename Fetch>
 ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoArgs &a, const Geometry &g, Fetch &&fetch) {
     const bool flow = a.step != 0;
-    const int per = flow && a.save_type == DFB_SAVE_JPG ? 2 : 1;
+    const int per = flow && a.save_type != DFB_SAVE_PNG ? 2 : 1;  // jpg and h5: an x and a y output per flow
     const int chunk = a.chunk_flows;
     std::vector<uint8_t *> out(2 * chunk), ox(chunk), oy(chunk);
     std::vector<size_t> lens(2 * chunk), lx(chunk), ly(chunk);
@@ -339,6 +339,7 @@ ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoAr
             const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
             const size_t cap = !flow                         ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
                                : a.save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
+                               : a.save_type == DFB_SAVE_H5  ? (size_t)g.dw * g.dh * sizeof(float)
                                                              : dfb_jpeg_max_bytes(g.dw, g.dh);
             try {
                 w.files.allocate((size_t)chunk * per * cap);
@@ -352,6 +353,16 @@ ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoAr
             } else if (a.save_type == DFB_SAVE_PNG) {
                 rc = bgr ? dfb_process_bgr_batch_host_png(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
                          : dfb_process_jpeg_batch_host_png(w.h, jf, jl, m + a.astep, a.step, dwa, dha, out.data(), cap, lens.data());
+            } else if (a.save_type == DFB_SAVE_H5) {
+                // the two float planes of flow i straight into files 2 i / 2 i + 1 (pinned: a direct DMA); every file is whole
+                std::vector<float *> px(m), py(m);
+                for (int i = 0; i < m; ++i) {
+                    px[i] = reinterpret_cast<float *>(out[2 * i]);
+                    py[i] = reinterpret_cast<float *>(out[2 * i + 1]);
+                    lens[2 * i] = lens[2 * i + 1] = cap;
+                }
+                rc = bgr ? dfb_process_bgr_batch_host_planes(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, px.data(), py.data())
+                         : dfb_process_jpeg_batch_host_planes(w.h, jf, jl, m + a.astep, a.step, dwa, dha, px.data(), py.data());
             } else {
                 for (int i = 0; i < m; ++i) {
                     ox[i] = out[2 * i];

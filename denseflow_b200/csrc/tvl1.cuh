@@ -70,7 +70,9 @@ void launch_sum_partials(const double *partials, int n, double *out, cudaStream_
 void launch_fill(Plane dst, float v, cudaStream_t s);
 // d1, d2 = the k x k median (k = 3 or 5) of u1, u2 (tvl1_median.cuh), image pixels only; out of place
 void launch_median(Plane u1, Plane u2, Plane d1, Plane d2, int k, cudaStream_t s);
-void launch_merge_flow(Plane u1, Plane u2, float *flow_xy, size_t flow_pitch_bytes, cudaStream_t s);
+// the float2 field, or with fx set the two planes fx / fy (row pitch f_pitch_bytes) instead
+void launch_merge_flow(Plane u1, Plane u2, float *flow_xy, size_t flow_pitch_bytes, cudaStream_t s, float *fx = nullptr,
+                       float *fy = nullptr, size_t f_pitch_bytes = 0);
 void launch_quantise(const float *flow_xy, size_t flow_pitch_bytes, int w, int h, int bound, uint8_t *qx, uint8_t *qy,
                      size_t q_pitch_bytes, cudaStream_t s);
 

@@ -246,6 +246,10 @@ class Tvl1 final : public FlowAlgorithm {
             for (int i = 0; i < count; ++i) {
                 float *flow = jobs[i].flow_xy;
                 size_t pitch = jobs[i].flow_pitch_bytes;
+                if (jobs[i].fx) {  // the merge writes the planes straight from u1 / u2
+                    solve_unfused(jobs[i].slot_a, jobs[i].slot_b, lv, n, nullptr, 0, s, jobs[i].fx, jobs[i].fy, jobs[i].f_pitch);
+                    continue;
+                }
                 if (!flow) {  // quantised output only: the float2 field lives in an engine-owned scratch plane
                     if (!unfused_scratch_) DFB_CUDA(cudaMalloc(&unfused_scratch_, (size_t)max_w_ * max_h_ * 2 * sizeof(float)));
                     flow = unfused_scratch_;
@@ -584,8 +588,9 @@ class Tvl1 final : public FlowAlgorithm {
     Plane work(float *p, const LevelGeom &g) const { return Plane{p, g.w, g.h, g.pitch}; }
 
     // ---- fused = 0: reference launch structure, A.4 state machine on the host ------------------
+    // fx set: the merge writes the two float planes fx / fy (PairJob) instead of the float2 field, and flow_xy may be null
     void solve_unfused(int slot_a, int slot_b, const LevelGeom *lv, int n, float *flow_xy, size_t flow_pitch_bytes,
-                       cudaStream_t s) {
+                       cudaStream_t s, float *fx = nullptr, float *fy = nullptr, size_t f_pitch = 0) {
         const Tvl1Consts c{(float)(prm_.lambda * prm_.theta), (float)(prm_.tau / prm_.theta), (float)prm_.theta};
         std::memset(last_iters_, 0, sizeof(last_iters_));
         Lane &wk = lanes_[0];
@@ -652,7 +657,7 @@ class Tvl1 final : public FlowAlgorithm {
                 launches += 2;
             }
         }
-        launch_merge_flow(level_plane(wk.u1pyr[0], lv, 0), level_plane(wk.u2pyr[0], lv, 0), flow_xy, flow_pitch_bytes, s);
+        launch_merge_flow(level_plane(wk.u1pyr[0], lv, 0), level_plane(wk.u2pyr[0], lv, 0), flow_xy, flow_pitch_bytes, s, fx, fy, f_pitch);
         ++launches;
         stats_pending_ = false;
         std::memcpy(pair_log_ + (size_t)next_log_slot() * kLogInts, last_iters_, sizeof(last_iters_));
@@ -730,6 +735,9 @@ class Tvl1 final : public FlowAlgorithm {
         job.qx = pj.qx;
         job.qy = pj.qy;
         job.q_pitch = pj.q_pitch;
+        job.fx = pj.fx;
+        job.fy = pj.fy;
+        job.f_pitch = pj.f_pitch;
     }
 
     void solve_fused(const PairJob *jobs, int count, const LevelGeom *lv, int n, cudaStream_t s) {

@@ -248,6 +248,16 @@ __device__ __forceinline__ void phase_merge(const int G, const int bid, const Fu
         }
         return;
     }
+    if (job.fx) {  // the two planes of an h5 file's datasets: consecutive threads store consecutive floats of each plane
+        for (int i = bid * kThreads + threadIdx.x; i < total; i += G * kThreads) {
+            const int y = i / L.w, x = i - y * L.w;
+            const size_t o = (size_t)y * L.pitch + x;
+            const size_t d = (size_t)y * (job.f_pitch >> 2) + x;
+            job.fx[d] = __ldcg(L.u1[cur] + o);
+            job.fy[d] = __ldcg(L.u2[cur] + o);
+        }
+        return;
+    }
     for (int i = bid * kThreads + threadIdx.x; i < total; i += G * kThreads) {
         const int y = i / L.w, x = i - y * L.w;
         const size_t o = (size_t)y * L.pitch + x;

@@ -57,6 +57,9 @@ struct FusedJob {
     int median_interval;  // (beside median_k and bound: both fill alignment padding, so the layout of the other fields is unchanged)
     uint8_t *qx, *qy;
     size_t q_pitch;
+    // fx non-null: emit u1 / u2 as two float planes instead of the float2 field (PairJob)
+    float *fx, *fy;
+    size_t f_pitch;
 };
 
 // Several independent pairs ("lanes") per launch: lane i is solved by CTAs [i*group, (i+1)*group) with

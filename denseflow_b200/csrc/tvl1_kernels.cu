@@ -236,11 +236,17 @@ __global__ void __launch_bounds__(kMedianThreads) k_median(Plane u1, Plane u2, P
     median_planes<kMedianThreads>(u1.p, u2.p, d1.p, d2.p, u1.w, u1.h, u1.pitch, k, blockIdx.x, gridDim.x, s[0], s[1]);
 }
 
-// A.5: merge(u1, u2) -> CV_32FC2
-__global__ void k_merge_flow(Plane u1, Plane u2, float *flow, size_t flow_pitch_bytes) {
+// A.5: merge(u1, u2) -> CV_32FC2, or with fx set -> two float planes (PairJob::fx)
+__global__ void k_merge_flow(Plane u1, Plane u2, float *flow, size_t flow_pitch_bytes, float *fx, float *fy, size_t f_pitch_bytes) {
     const int x = blockIdx.x * BX + threadIdx.x;
     const int y = blockIdx.y * BY + threadIdx.y;
     if (x >= u1.w || y >= u1.h) return;
+    if (fx) {
+        const size_t d = (size_t)y * (f_pitch_bytes >> 2) + x;
+        fx[d] = u1.p[(size_t)y * u1.pitch + x];
+        fy[d] = u2.p[(size_t)y * u2.pitch + x];
+        return;
+    }
     float2 *row = reinterpret_cast<float2 *>(reinterpret_cast<char *>(flow) + (size_t)y * flow_pitch_bytes);
     row[x] = make_float2(u1.p[(size_t)y * u1.pitch + x], u2.p[(size_t)y * u2.pitch + x]);
 }
@@ -317,8 +323,9 @@ void launch_median(Plane u1, Plane u2, Plane d1, Plane d2, int k, cudaStream_t s
     k_median<<<tiles, kMedianThreads, 0, s>>>(u1, u2, d1, d2, k);
     DFB_KERNEL_CHECK();
 }
-void launch_merge_flow(Plane u1, Plane u2, float *flow_xy, size_t flow_pitch_bytes, cudaStream_t s) {
-    k_merge_flow<<<grid2d(u1.w, u1.h), dim3(BX, BY), 0, s>>>(u1, u2, flow_xy, flow_pitch_bytes);
+void launch_merge_flow(Plane u1, Plane u2, float *flow_xy, size_t flow_pitch_bytes, cudaStream_t s, float *fx, float *fy,
+                       size_t f_pitch_bytes) {
+    k_merge_flow<<<grid2d(u1.w, u1.h), dim3(BX, BY), 0, s>>>(u1, u2, flow_xy, flow_pitch_bytes, fx, fy, f_pitch_bytes);
     DFB_KERNEL_CHECK();
 }
 void launch_quantise(const float *flow_xy, size_t flow_pitch_bytes, int w, int h, int bound, uint8_t *qx, uint8_t *qy,

@@ -104,6 +104,26 @@ def output_names(step, first_index, n, save_type="jpg"):
     return names
 
 
+def h5_names(step, first_index, n):
+    """The dataset names writeHDF5 gives a chunk's flows (src/common.cpp:120-150), in the order run_videos hands out their
+    h5 files: every flow_x of the chunk, then every flow_y.  Steps > 1 add _p<step>, steps < 0 add _m<|step|> and offset the
+    index by |step|, as output_names does."""
+    base = -step if step < 0 else 0
+    tag = "_p%d" % step if step > 1 else "_m%d" % -step if step < 0 else ""
+    return (["/flow_x%s_%05d" % (tag, first_index + i + base) for i in range(n)] +
+            ["/flow_y%s_%05d" % (tag, first_index + i + base) for i in range(n)])
+
+
+def h5_path(outdir, step):
+    """The file writeHDF5 writes a video's flows to: <outdir>.h5 (step 1), <outdir>_p<s>.h5 (s > 1), <outdir>_m<|s|>.h5 (s < 0)."""
+    outdir = str(outdir).rstrip("/")
+    tag = "_p%d" % step if step > 1 else "_m%d" % -step if step < 0 else ""
+    return outdir + tag + ".h5"
+
+
+_SAVE_TYPES = {"jpg": _lib.SAVE_JPG, "png": _lib.SAVE_PNG, "h5": _lib.SAVE_H5}
+
+
 def _callback(on_chunk, shapes):
     if on_chunk is None:
         return None
@@ -162,12 +182,14 @@ class ListRunner:
         videos: one entry per video, a list of uint8 [H,W,3] BGR frames or a list of JPEG files (bytes).  Each video is resized
         as get_new_size decides and turned into files on the GPU.  on_chunk(video, device, first_index, last_chunk, files) is
         called on the worker's thread once every file of a chunk is in host memory; files is a list of bytes-like views that
-        die when the callback returns, named as output_names(step, first_index, n, save_type) names them.  last_chunk is the
+        die when the callback returns, named as output_names(step, first_index, n, save_type) names them.  With save_type "h5"
+        files 2 i / 2 i + 1 are flow first_index + i's x / y plane as raw float32 [dh, dw] (writeHDF5's datasets, named by
+        h5_names).  last_chunk is the
         reference's FlowBuffer::last_buffer.  Returns a dict of dfb_list_stats."""
-        if save_type not in ("jpg", "png"):
-            raise RuntimeError("only jpg/png are supported (no %s) for output" % save_type)
+        if save_type not in _SAVE_TYPES:
+            raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
         arr, keep = _pack_videos(videos)
-        per = 2 if step != 0 and save_type == "jpg" else 1
+        per = 2 if step != 0 and save_type != "png" else 1
         cb = None
         if on_chunk is not None:
             def _cb(user, video, dev, first, n, last, files, lens):
@@ -175,7 +197,7 @@ class ListRunner:
             cb = _lib.FILES_DONE_FN(_cb)
         st = _lib.ListStats()
         err = C.create_string_buffer(512)
-        rc = self._L.dfb_list_run_videos(self._r, arr, len(videos), int(step), int(bound), _lib.SAVE_PNG if save_type == "png" else _lib.SAVE_JPG,
+        rc = self._L.dfb_list_run_videos(self._r, arr, len(videos), int(step), int(bound), _SAVE_TYPES[save_type],
                                          int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
                                          queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None, C.byref(st),
                                          err, 512)
@@ -192,9 +214,9 @@ class ListRunner:
         video, or until the video's last chunk.  An exception in source ends the run with "video k: <message>"; one in
         on_chunk ends it too and is raised again here.  on_chunk and the result are those of run_videos, except that a video
         whose outputs end on a window boundary gets one more on_chunk call with no files and last_chunk True."""
-        if save_type not in ("jpg", "png"):
-            raise RuntimeError("only jpg/png are supported (no %s) for output" % save_type)
-        per = 2 if step != 0 and save_type == "jpg" else 1
+        if save_type not in _SAVE_TYPES:
+            raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
+        per = 2 if step != 0 and save_type != "png" else 1
         windows = {}  # video -> the latest window and the memory behind it
         failures = []
 
@@ -226,7 +248,7 @@ class ListRunner:
         st = _lib.ListStats()
         err = C.create_string_buffer(512)
         rc = self._L.dfb_list_run_stream(self._r, int(n_videos), C.cast(src, C.c_void_p), int(step), int(bound),
-                                         _lib.SAVE_PNG if save_type == "png" else _lib.SAVE_JPG, int(quality), int(jpeg_exact),
+                                         _SAVE_TYPES[save_type], int(quality), int(jpeg_exact),
                                          int(new_width), int(new_height), int(new_short), int(chunk_flows),
                                          queue._q if queue is not None else None, C.cast(cb, C.c_void_p), None, C.byref(st), err, 512)
         windows.clear()

@@ -127,6 +127,18 @@ int dfb_calc_batch_host_u8(dfb_handle *h, const uint8_t *const *frames, int n_fr
 int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height,
                           float *flows, void *stream);
 
+/*
+ * The same batches with the flow as two float planes per pair, the payloads of the flow_x / flow_y datasets the reference's
+ * USE_HDF5 build writes (cv::split then H5LTmake_dataset_float, src/denseflow_gpu.cpp:223-239): the engines' merge epilogue
+ * writes u1 and u2 as dense planes, so the values are bit for bit the x and y channels of dfb_calc_batch_host's fields.
+ *   fx[M], fy[M] : host pointers, dense width*height float each (page-locked ones take a direct DMA)
+ *   planes       : one device allocation [M][2][height][width] float (pair j's x plane, then its y plane); enqueued on `stream`
+ */
+int dfb_calc_batch_host_planes(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
+                               float *const *fx, float *const *fy);
+int dfb_calc_batch_device_planes(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height,
+                                 float *planes, void *stream);
+
 /* Stand-alone quantiser on device buffers (src/common.cpp:4-16).  flow_xy pitch in bytes. */
 int dfb_quantise_device(dfb_handle *h, const float *flow_xy, size_t flow_pitch, int width, int height, int bound,
                         uint8_t *qx, uint8_t *qy, size_t q_pitch, void *stream);
@@ -138,7 +150,9 @@ int dfb_quantise_device(dfb_handle *h, const float *flow_xy, size_t flow_pitch, 
  * convertTo(CV_8U, 128/bound, 128) [one float fused multiply-add, round-half-even, saturate — OpenCV's vector path], and a
  * third channel holding bound_x/4 in rows 0..h/2 and bound_y/4 below.  bgr: packed 3 bytes per pixel (x, y, bounds).
  * bounds_xy_host (optional, 2 doubles): receives bound_x, bound_y — passing it makes the call block on the stream.
- * -st=h5 stays what it is in a build without HDF5: "HDF5 support is not enabled, pls recompile" (:241) — a host writer.
+ * -st=h5 takes the flow unquantised: dfb_calc_batch_host_planes and the _planes chains below give its payloads, and
+ * dfb_h5_create / dfb_h5_write_float / dfb_h5_close write the file (a build without DFB_USE_HDF5 refuses with the reference's
+ * "HDF5 support is not enabled, pls recompile", :241).
  */
 int dfb_flow_to_png_image_device(dfb_handle *h, const float *flow_xy, size_t flow_pitch, int width, int height, uint8_t *bgr,
                                   size_t bgr_pitch, double *bounds_xy_host, void *stream);
@@ -350,6 +364,31 @@ int dfb_process_bgr_batch_host_png(dfb_handle *h, const uint8_t *const *bgr, int
 int dfb_process_jpeg_batch_host_png(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step,
                                     int dst_width, int dst_height, uint8_t *const *png, size_t capacity, size_t *len);
 /*
+ * The -st=h5 payloads behind the two colour frame sources: the _png chains with pair j's flow as two dense float planes
+ * (dst_width x dst_height each) to fx[j] / fy[j] instead of a PNG file: bit for bit what dfb_calc_batch_host_planes gives for the
+ * gray, resized frames.  Arguments and refusals are those of the _png siblings.
+ */
+int dfb_process_bgr_batch_host_planes(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int src_width, int src_height,
+                                      int dst_width, int dst_height, float *const *fx, float *const *fy);
+int dfb_process_jpeg_batch_host_planes(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step,
+                                       int dst_width, int dst_height, float *const *fx, float *const *fy);
+
+/*
+ * ---- HDF5 flow files (-st=h5; pure host functions, no device needed) ----------------------------------------------------
+ * What the reference's USE_HDF5 build calls (src/utils.cpp:27-41, src/common.cpp:120-150), written by a self-contained
+ * writer: dfb_h5_create is H5Fcreate(path, H5F_ACC_TRUNC), dfb_h5_write_float is H5LTmake_dataset_float(file, name, 2,
+ * {rows, cols}, data) at the root group (a name already written is refused), dfb_h5_close writes the metadata and closes.
+ * The file is the format libhdf5 writes by default (superblock 0, a symbol-table root group, contiguous IEEE f32 LE
+ * datasets); payloads go to the file as they arrive, and the same calls give the same bytes (no timestamps).  Only a library
+ * built with DFB_USE_HDF5 (build variant "hdf5") has the writer: elsewhere dfb_h5_create fails with DFB_ERR_UNSUPPORTED and
+ * "HDF5 support is not enabled, pls recompile" (src/denseflow_gpu.cpp:241) in dfb_last_error(NULL).  Errors go to
+ * dfb_last_error(NULL).  dfb_h5_close always frees the file object, and returns the first error of the file's writes.
+ */
+typedef struct dfb_h5_file dfb_h5_file;
+int dfb_h5_create(const char *path, dfb_h5_file **out);
+int dfb_h5_write_float(dfb_h5_file *f, const char *name, int rows, int cols, const float *data);
+int dfb_h5_close(dfb_h5_file *f);
+/*
  * `-if -s=0`: dfb_extract_frames_host with the frames given as JPEG files of one size (else DFB_ERR_SIZE naming the frame),
  * decoded on the device to imdecode's BGR pixels.  Frame i's file goes to jpg[i], its length to len[i]: byte for byte what
  * dfb_extract_frames_host gives for the imdecoded frames.  Refuses what dfb_process_jpeg_batch_host refuses in a file.
@@ -508,6 +547,9 @@ void dfb_list_close(dfb_list_runner *r);
  * resolves a video's destination size with dfb_new_size and runs the matching single-handle chain:
  *   save_type DFB_SAVE_JPG  dfb_process_{bgr,jpeg}_batch_host        files 2 i / 2 i + 1: flow first_index + i's x / y
  *   save_type DFB_SAVE_PNG  dfb_process_{bgr,jpeg}_batch_host_png    file i: flow first_index + i
+ *   save_type DFB_SAVE_H5   dfb_process_{bgr,jpeg}_batch_host_planes files 2 i / 2 i + 1: flow first_index + i's x / y plane as
+ *                           raw little-endian float32, 4 * dw * dh bytes each (the payloads of writeHDF5's datasets; bound > 0
+ *                           is still required, as check_param requires it, and unused)
  *   step 0                  dfb_extract_frames_host / dfb_extract_frames_jpeg_host   file i: frame first_index + i (img)
  * Chunks, queue and stats are those of dfb_list_run (stats: frames = decoded frames, flows = flow fields); max_width /
  * max_height of dfb_list_open bound the DESTINATION size.  jpeg_exact is set on every worker handle for the call and restored.
@@ -518,7 +560,7 @@ void dfb_list_close(dfb_list_runner *r);
  * the runner stays usable.
  */
 enum { DFB_VIDEO_BGR = 0, DFB_VIDEO_JPEG = 1 };
-enum { DFB_SAVE_JPG = 0, DFB_SAVE_PNG = 1 };
+enum { DFB_SAVE_JPG = 0, DFB_SAVE_PNG = 1, DFB_SAVE_H5 = 2 };
 typedef struct {
     int kind;                       /* DFB_VIDEO_BGR or DFB_VIDEO_JPEG */
     int n_frames;
