@@ -165,6 +165,8 @@ SIGNATURES = {
                                       C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
     "dfb_list_run_stream": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
+    "dfb_list_run_windows": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
     "dfb_run_list": (C.c_int, [C.c_char_p, C.POINTER(C.c_int), C.c_int, C.POINTER(Clip), C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.POINTER(ListStats), C.c_char_p, C.c_size_t]),
 }

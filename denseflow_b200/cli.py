@@ -6,7 +6,9 @@ takes the reference's flags and writes its file tree: `<o>/[<class>/]<stem>/flow
 -s=0 `img_*.jpg`), and for a list in flow mode one `<o>/.done/[<class>/]<stem>` marker per finished video, which a later run
 skips unless -f is given.  Videos are decoded with cv2.VideoCapture on the worker threads, one window of frames at a time,
 so a list of long videos runs in bounded memory; `-if` folders go to the GPU as JPEG bytes and are decoded there.  Every
-visible GPU runs two workers.  Errors print their message and exit 1, as the reference's main() does.
+visible GPU runs two workers.  Each takes whole videos while the list lasts; then idle workers join the unfinished videos
+window by window, so a single video or `-if` folder runs on every worker, one reading its next window while another
+computes.  Errors print their message and exit 1, as the reference's main() does.
 
 `-st=h5` in flow mode needs the library built with HDF5 support, the counterpart of the reference's -DUSE_HDF5=yes build:
 `DFB_LIBRARY=hdf5 python -m denseflow_b200 ...` writes each video's flows as float32 datasets /flow_x_%05d and /flow_y_%05d to
@@ -356,8 +358,25 @@ def run(opt, out=_print, variant="default"):
     return _run_jobs(opt, algorithm, n_dev, jobs, len(videos), is_record, say, variant)
 
 
+def _source_message(error, failures):
+    """The command's message for a failed run: the source exception the runner reported ("video k: <message>") as its own
+    text, as the reference prints it; any other error as it is.  A source call that failed after an earlier window of its
+    video had failed is not the reported error."""
+    for video, ex in failures:
+        prefix = "video %d: " % video
+        text = str(ex) or type(ex).__name__
+        if error.startswith(prefix) and text.startswith(error[len(prefix):]):
+            return str(ex)
+    return error
+
+
 def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
-    """The non-empty inputs through ListRunner.run_stream: files into each output directory, then the summary line."""
+    """The non-empty inputs through ListRunner.run_windows: files into each output directory, then the summary line.
+
+    Once the list is handed out, idle workers join the unfinished videos, so `source` may be called for one video from several
+    threads, but one call at a time and in frame order, and each window's on_chunk comes after its source call and after the
+    video's earlier chunks.  So a video's reader is only touched by one call at a time, its size is recorded by its first
+    window before any chunk needs it, and its h5 file is created by its first window and written in dataset order."""
     from . import _lib, listrun
     import numpy as np
     from . import api, h5
@@ -366,7 +385,7 @@ def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
     readers = {}
     h5_files = {}  # video -> its open h5 file, from the video's start to its last chunk
     sizes = {}     # video -> (dh, dw), the size of its flows
-    failures = []
+    failures = []  # (video, exception) of the source
 
     def source(video, first, max_n):
         try:
@@ -385,7 +404,7 @@ def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
                 readers.pop(video).close()
             return frames
         except Exception as ex:
-            failures.append(ex)
+            failures.append((video, ex))
             raise
 
     def on_chunk(video, dev, first, last, files):
@@ -418,11 +437,11 @@ def _run_jobs(opt, algorithm, n_dev, jobs, n_listed, is_record, say, variant):
         devices = [d for d in range(n_dev) for _ in range(WORKERS_PER_DEVICE)][:_lib.LIST_MAX_WORKERS]
         r = listrun.ListRunner(algorithm, devices, 64, 64, variant=variant)
         try:
-            st = r.run_stream(len(jobs), source, on_chunk, step=step, bound=opt["bound"], save_type=save_type if step != 0 else "jpg",
-                              quality=95, jpeg_exact=1, new_width=opt["newWidth"], new_height=opt["newHeight"],
-                              new_short=opt["newShort"], chunk_flows=CHUNK_FLOWS)
+            st = r.run_windows(len(jobs), source, on_chunk, step=step, bound=opt["bound"], save_type=save_type if step != 0 else "jpg",
+                               quality=95, jpeg_exact=1, new_width=opt["newWidth"], new_height=opt["newHeight"],
+                               new_short=opt["newShort"], chunk_flows=CHUNK_FLOWS)
         except RuntimeError as ex:
-            raise CliError(str(failures[0]) if failures else str(ex)) from None
+            raise CliError(_source_message(str(ex), failures)) from None
         finally:
             r.close()
             for rd in readers.values():

@@ -12,6 +12,8 @@
 // dfb_list_run_videos runs the same dispatch over the videos as the reference takes them (colour frames or `-if` JPEG files)
 // and hands out the files the reference writes: flow JPEGs or PNGs, or with step 0 the extracted frames.  dfb_list_run_stream
 // does the same with frames pulled from the caller one window at a time, so a list of long videos runs in bounded memory.
+// dfb_list_run_windows pulls the same windows but makes the window the unit of work once the queue is empty: idle workers join
+// the unfinished videos, so one video runs on every worker and one worker reads a window while another computes the last.
 //
 // This file is a client of the C ABI (dfb_create / dfb_calc_batch_host[_u8] / dfb_process_* / dfb_extract_frames_* /
 // dfb_destroy): it adds no arithmetic.
@@ -23,8 +25,11 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <climits>
+#include <condition_variable>
 #include <cstdio>
 #include <cstring>
+#include <list>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -149,23 +154,53 @@ struct ItemResult {
     uint64_t flows = 0, frames = 0;
 };
 
-// The dispatch of dfb_list_run and dfb_list_run_videos.  Each worker, on a host thread of its own (worker 0 on the caller's),
-// takes items from `queue` (or from an in-process counter) until all n_items are taken or an item fails; body(wi, idx) runs
-// item idx on worker wi.  The first failure's code is returned and its message written to err; stats receives the run's
-// counters either way.
-template <typename Body>
-int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, dfb_list_stats *stats, char *err, size_t err_len) {
-    const int n_workers = (int)r->workers.size();
-    dfb_list_stats st{};
-    st.workers = n_workers;
-    std::atomic<long> local_next{0};
-    std::atomic<int> failed{0};
-    std::mutex mtx;
-    std::string first_error;
+// The start of a run: the workers' engine counters from zero.
+void begin_run(dfb_list_runner *r, dfb_list_stats &st) {
+    st = dfb_list_stats{};
+    st.workers = (int)r->workers.size();
     for (auto &w : r->workers) {
         dfb_reset_counters(w.h);
         w.retired = dfb_counters{};
     }
+}
+
+// The end of a run: its wall time and the counters of every handle its workers used.
+void end_run(dfb_list_runner *r, dfb_list_stats &st, clk::time_point t_start) {
+    st.seconds = seconds_since(t_start);
+    for (auto &w : r->workers) {
+        dfb_counters c{};
+        if (dfb_get_counters(w.h, &c) == DFB_OK) {
+            st.kernel_launches += c.kernel_launches;
+            st.h2d_bytes += c.h2d_bytes;
+            st.d2h_bytes += c.d2h_bytes;
+        }
+        st.kernel_launches += w.retired.kernel_launches;
+        st.h2d_bytes += w.retired.h2d_bytes;
+        st.d2h_bytes += w.retired.d2h_bytes;
+    }
+}
+
+// Runs worker(wi) for every worker, each on a host thread of its own (worker 0 on the caller's).
+template <typename Worker>
+void run_workers(int n_workers, Worker &&worker) {
+    std::vector<std::thread> threads;
+    for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
+    worker(0);
+    for (auto &t : threads) t.join();
+}
+
+// The dispatch of dfb_list_run, dfb_list_run_videos and dfb_list_run_stream.  Each worker takes items from `queue` (or from
+// an in-process counter) until all n_items are taken or an item fails; body(wi, idx) runs item idx on worker wi.  The first
+// failure's code is returned and its message written to err; stats receives the run's counters either way.
+template <typename Body>
+int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, dfb_list_stats *stats, char *err, size_t err_len) {
+    const int n_workers = (int)r->workers.size();
+    dfb_list_stats st;
+    begin_run(r, st);
+    std::atomic<long> local_next{0};
+    std::atomic<int> failed{0};
+    std::mutex mtx;
+    std::string first_error;
     const auto t_start = clk::now();
 
     auto worker = [&](int wi) {
@@ -198,24 +233,8 @@ int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, df
         st.finish_seconds_per_worker[wi] = seconds_since(t_start);
     };
 
-    if (n_items > 0) {
-        std::vector<std::thread> threads;
-        for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
-        worker(0);
-        for (auto &t : threads) t.join();
-    }
-    st.seconds = seconds_since(t_start);
-    for (auto &w : r->workers) {
-        dfb_counters c{};
-        if (dfb_get_counters(w.h, &c) == DFB_OK) {
-            st.kernel_launches += c.kernel_launches;
-            st.h2d_bytes += c.h2d_bytes;
-            st.d2h_bytes += c.d2h_bytes;
-        }
-        st.kernel_launches += w.retired.kernel_launches;
-        st.h2d_bytes += w.retired.h2d_bytes;
-        st.d2h_bytes += w.retired.d2h_bytes;
-    }
+    if (n_items > 0) run_workers(n_workers, worker);
+    end_run(r, st, t_start);
     if (stats) *stats = st;
     if (failed.load()) {
         set_error(err, err_len, first_error);
@@ -309,98 +328,119 @@ struct Window {
     bool ends = false;
 };
 
-// One video through the chains, one window at a time.  fetch(first, max_n, win) returns an ItemResult and fills win with
-// frames first .. first + max_n - 1, fewer when the video ends there; g is the video's geometry by the time the first window
-// with a frame is fetched.  A window serves up to chunk_flows outputs: flows [f0, f0 + m) read frames f0 .. f0 + m - 1 +
-// |step|, so consecutive windows overlap by |step| frames (the overlap the reference keeps between its own <= 512-frame
-// batches, src/denseflow_gpu.cpp:182-189,204-205) and indices stay global (FlowBuffer::base_start).  With step 0 every frame
-// is an output.
-template <typename Fetch>
-ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoArgs &a, const Geometry &g, Fetch &&fetch) {
+// The outputs of a window: flows [f0, f0 + m) read frames f0 .. f0 + m - 1 + |step|; with step 0 every frame is an output.
+int window_outputs(const VideoArgs &a, const Window &win) { return a.step != 0 ? std::max(win.n - a.astep, 0) : win.n; }
+
+// One window of video idx through the chains.  fetch(f0, max_n, win) returns an ItemResult and fills win with frames f0 ..
+// f0 + max_n - 1, fewer when the video ends there; g is the video's geometry by the time fetch returns a window with a
+// frame.  A window serves up to chunk_flows outputs, so consecutive windows overlap by |step| frames (the overlap the
+// reference keeps between its own <= 512-frame batches, src/denseflow_gpu.cpp:182-189,204-205) and indices stay global
+// (FlowBuffer::base_start).  Once every file of the window is in the worker's pinned ring, deliver(f0, m, win.ends, files,
+// lens) hands them on; a failure returns before it.
+template <typename Fetch, typename Deliver>
+ItemResult run_window(dfb_list_runner::Worker &w, int wi, long idx, const VideoArgs &a, const Geometry &g, int f0, Window &win, Fetch &&fetch,
+                      Deliver &&deliver) {
     const bool flow = a.step != 0;
     const int per = flow && a.save_type != DFB_SAVE_PNG ? 2 : 1;  // jpg and h5: an x and a y output per flow
     const int chunk = a.chunk_flows;
     std::vector<uint8_t *> out(2 * chunk), ox(chunk), oy(chunk);
     std::vector<size_t> lens(2 * chunk), lx(chunk), ly(chunk);
-    uint64_t outputs = 0;
-    int f0 = 0;
-    for (;;) {
-        Window win;
-        ItemResult fr = fetch(f0, chunk + a.astep, win);
-        if (fr.rc != DFB_OK) return fr;
-        const int m = flow ? std::max(win.n - a.astep, 0) : win.n;
-        int rc = DFB_OK;
-        if (m > 0) {
-            const dfb_video &v = *win.v;
-            const bool bgr = v.kind == DFB_VIDEO_BGR;
-            const uint8_t *const *bf = bgr ? v.bgr + win.off : nullptr;
-            const uint8_t *const *jf = bgr ? nullptr : v.jpeg + win.off;
-            const size_t *jl = bgr ? nullptr : v.jpeg_len + win.off;
-            const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
-            const size_t cap = !flow                         ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
-                               : a.save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
-                               : a.save_type == DFB_SAVE_H5  ? (size_t)g.dw * g.dh * sizeof(float)
-                                                             : dfb_jpeg_max_bytes(g.dw, g.dh);
-            try {
-                w.files.allocate((size_t)chunk * per * cap);
-            } catch (const dfb::CudaError &) {
-                return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed"};
+    ItemResult fr = fetch(f0, chunk + a.astep, win);
+    if (fr.rc != DFB_OK) return fr;
+    const int m = window_outputs(a, win);
+    int rc = DFB_OK;
+    if (m > 0) {
+        const dfb_video &v = *win.v;
+        const bool bgr = v.kind == DFB_VIDEO_BGR;
+        const uint8_t *const *bf = bgr ? v.bgr + win.off : nullptr;
+        const uint8_t *const *jf = bgr ? nullptr : v.jpeg + win.off;
+        const size_t *jl = bgr ? nullptr : v.jpeg_len + win.off;
+        const int dwa = g.resize ? g.dw : 0, dha = g.resize ? g.dh : 0;  // 0 / 0: no resize
+        const size_t cap = !flow                         ? dfb_jpeg_max_bytes_bgr(g.dw, g.dh)
+                           : a.save_type == DFB_SAVE_PNG ? dfb_png_max_bytes(g.dw, g.dh)
+                           : a.save_type == DFB_SAVE_H5  ? (size_t)g.dw * g.dh * sizeof(float)
+                                                         : dfb_jpeg_max_bytes(g.dw, g.dh);
+        try {
+            w.files.allocate((size_t)chunk * per * cap);
+        } catch (const dfb::CudaError &) {
+            return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed"};
+        }
+        for (int k = 0; k < per * chunk; ++k) out[k] = (uint8_t *)w.files + (size_t)k * cap;
+        if (!flow) {
+            rc = bgr ? dfb_extract_frames_host(w.h, bf, m, g.sw, g.sh, dwa, dha, a.quality, out.data(), cap, lens.data())
+                     : dfb_extract_frames_jpeg_host(w.h, jf, jl, m, dwa, dha, a.quality, out.data(), cap, lens.data());
+        } else if (a.save_type == DFB_SAVE_PNG) {
+            rc = bgr ? dfb_process_bgr_batch_host_png(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
+                     : dfb_process_jpeg_batch_host_png(w.h, jf, jl, m + a.astep, a.step, dwa, dha, out.data(), cap, lens.data());
+        } else if (a.save_type == DFB_SAVE_H5) {
+            // the two float planes of flow i straight into files 2 i / 2 i + 1 (pinned: a direct DMA); every file is whole
+            std::vector<float *> px(m), py(m);
+            for (int i = 0; i < m; ++i) {
+                px[i] = reinterpret_cast<float *>(out[2 * i]);
+                py[i] = reinterpret_cast<float *>(out[2 * i + 1]);
+                lens[2 * i] = lens[2 * i + 1] = cap;
             }
-            for (int k = 0; k < per * chunk; ++k) out[k] = (uint8_t *)w.files + (size_t)k * cap;
-            if (!flow) {
-                rc = bgr ? dfb_extract_frames_host(w.h, bf, m, g.sw, g.sh, dwa, dha, a.quality, out.data(), cap, lens.data())
-                         : dfb_extract_frames_jpeg_host(w.h, jf, jl, m, dwa, dha, a.quality, out.data(), cap, lens.data());
-            } else if (a.save_type == DFB_SAVE_PNG) {
-                rc = bgr ? dfb_process_bgr_batch_host_png(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, out.data(), cap, lens.data())
-                         : dfb_process_jpeg_batch_host_png(w.h, jf, jl, m + a.astep, a.step, dwa, dha, out.data(), cap, lens.data());
-            } else if (a.save_type == DFB_SAVE_H5) {
-                // the two float planes of flow i straight into files 2 i / 2 i + 1 (pinned: a direct DMA); every file is whole
-                std::vector<float *> px(m), py(m);
-                for (int i = 0; i < m; ++i) {
-                    px[i] = reinterpret_cast<float *>(out[2 * i]);
-                    py[i] = reinterpret_cast<float *>(out[2 * i + 1]);
-                    lens[2 * i] = lens[2 * i + 1] = cap;
-                }
-                rc = bgr ? dfb_process_bgr_batch_host_planes(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, px.data(), py.data())
-                         : dfb_process_jpeg_batch_host_planes(w.h, jf, jl, m + a.astep, a.step, dwa, dha, px.data(), py.data());
-            } else {
-                for (int i = 0; i < m; ++i) {
-                    ox[i] = out[2 * i];
-                    oy[i] = out[2 * i + 1];
-                }
-                rc = bgr ? dfb_process_bgr_batch_host(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, a.bound, a.quality, ox.data(),
-                                                      oy.data(), cap, lx.data(), ly.data())
-                         : dfb_process_jpeg_batch_host(w.h, jf, jl, m + a.astep, a.step, dwa, dha, a.bound, a.quality, ox.data(), oy.data(),
-                                                       cap, lx.data(), ly.data());
-                for (int i = 0; i < m; ++i) {
-                    lens[2 * i] = lx[i];
-                    lens[2 * i + 1] = ly[i];
-                }
+            rc = bgr ? dfb_process_bgr_batch_host_planes(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, px.data(), py.data())
+                     : dfb_process_jpeg_batch_host_planes(w.h, jf, jl, m + a.astep, a.step, dwa, dha, px.data(), py.data());
+        } else {
+            for (int i = 0; i < m; ++i) {
+                ox[i] = out[2 * i];
+                oy[i] = out[2 * i + 1];
+            }
+            rc = bgr ? dfb_process_bgr_batch_host(w.h, bf, m + a.astep, a.step, g.sw, g.sh, dwa, dha, a.bound, a.quality, ox.data(),
+                                                  oy.data(), cap, lx.data(), ly.data())
+                     : dfb_process_jpeg_batch_host(w.h, jf, jl, m + a.astep, a.step, dwa, dha, a.bound, a.quality, ox.data(), oy.data(),
+                                                   cap, lx.data(), ly.data());
+            for (int i = 0; i < m; ++i) {
+                lens[2 * i] = lx[i];
+                lens[2 * i + 1] = ly[i];
             }
         }
-        if (rc != DFB_OK) return {rc, video_error(idx, f0, dfb_last_error(w.h))};
-        // every file of this chunk is in host memory now; win.ends makes it FlowBuffer::last_buffer (see dfb_list_run)
-        if (a.done) a.done(a.user, (int)idx, w.device, f0, m, win.ends, out.data(), lens.data());
+    }
+    if (rc != DFB_OK) return {rc, video_error(idx, f0, dfb_last_error(w.h))};
+    deliver(f0, m, win.ends, out.data(), lens.data());
+    return {};
+}
+
+// One video through the chains on worker w, one window at a time.
+template <typename Fetch>
+ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoArgs &a, const Geometry &g, Fetch &&fetch) {
+    auto deliver = [&](int f0, int m, bool ends, uint8_t *const *files, const size_t *lens) {
+        // every file of this chunk is in host memory now; ends makes it FlowBuffer::last_buffer (see dfb_list_run)
+        if (a.done) a.done(a.user, (int)idx, w.device, f0, m, ends, files, lens);
+    };
+    uint64_t outputs = 0;
+    for (int f0 = 0;;) {
+        Window win;
+        ItemResult res = run_window(w, wi, idx, a, g, f0, win, fetch, deliver);
+        if (res.rc != DFB_OK) return res;
+        const int m = window_outputs(a, win);
         outputs += m;
-        if (win.ends) return {DFB_OK, {}, flow ? outputs : 0, (uint64_t)f0 + win.n};
+        if (win.ends) return {DFB_OK, {}, a.step != 0 ? outputs : 0, (uint64_t)f0 + win.n};
         f0 += m;
     }
 }
 
-// run_items over videos with the call's jpeg_exact: the runner owns the handles, so it is set on each of them and restored
+// run() over videos with the call's jpeg_exact: the runner owns the handles, so it is set on each of them and restored
 // afterwards.
-template <typename Body>
-int run_videos_with(dfb_list_runner *r, int n_videos, dfb_queue *queue, int jpeg_exact, Body &&body, dfb_list_stats *stats, char *err,
-                    size_t err_len) {
+template <typename Run>
+int with_jpeg_exact(dfb_list_runner *r, int jpeg_exact, Run &&run) {
     const int n_workers = (int)r->workers.size();
     std::vector<double> exact_before(n_workers, 0);
     for (int wi = 0; wi < n_workers; ++wi) {
         dfb_get_param(r->workers[wi].h, "jpeg_exact", &exact_before[wi]);
         dfb_set_param(r->workers[wi].h, "jpeg_exact", jpeg_exact);
     }
-    const int rc = run_items(r, n_videos, queue, body, stats, err, err_len);
+    const int rc = run();
     for (int wi = 0; wi < n_workers; ++wi) dfb_set_param(r->workers[wi].h, "jpeg_exact", exact_before[wi]);
     return rc;
+}
+
+// run_items over videos with the call's jpeg_exact.
+template <typename Body>
+int run_videos_with(dfb_list_runner *r, int n_videos, dfb_queue *queue, int jpeg_exact, Body &&body, dfb_list_stats *stats, char *err,
+                    size_t err_len) {
+    return with_jpeg_exact(r, jpeg_exact, [&] { return run_items(r, n_videos, queue, body, stats, err, err_len); });
 }
 
 // Worker w's handle for destination frames of dw x dh: a smaller handle is replaced by one at least that large in both
@@ -426,6 +466,204 @@ int fit_worker(dfb_list_runner *r, dfb_list_runner::Worker &w, int dw, int dh, s
     w.h = h;
     w.max_w = mw;
     w.max_h = mh;
+    return DFB_OK;
+}
+
+// The caller's window of frames first .. first + max_n - 1 of video idx, into cur and win.  The video is sized by its first
+// window with a frame, which also fits `fit`'s handle to it when fit is given; every later frame must have frame 0's size.
+ItemResult fetch_stream_window(dfb_list_runner *r, dfb_frames_fn source, const VideoArgs &a, long idx, int first, int max_n, dfb_video &cur,
+                               Window &win, Geometry &g, dfb_list_runner::Worker *fit) {
+    const std::string k = "video " + std::to_string(idx) + ": ";
+    cur = dfb_video{};
+    char msg[512] = "";
+    if (source(a.user, (int)idx, first, max_n, &cur, msg, sizeof msg) != 0) return {DFB_ERR_INVALID_ARG, k + msg};
+    if (malformed(cur) || cur.n_frames > max_n)
+        return {DFB_ERR_INVALID_ARG, k + "the source returned a malformed window at frame " + std::to_string(first)};
+    win = {&cur, 0, cur.n_frames, cur.n_frames < max_n};
+    if (cur.n_frames == 0) return {};
+    if (first == 0) {
+        if (int rc = size_video(cur, 0, a, g)) return {rc, k + dfb_last_error(nullptr)};
+        std::string e;
+        if (fit)
+            if (int rc = fit_worker(r, *fit, g.dw, g.dh, e)) return {rc, k + e};
+    }
+    // a BGR window has one size; a JPEG file that cannot be sized is left to the decoder, which names the fault
+    const int n_check = cur.kind == DFB_VIDEO_BGR ? 1 : cur.n_frames;
+    for (int i = 0; i < n_check; ++i) {
+        int fw = cur.width, fh = cur.height;
+        if (cur.kind == DFB_VIDEO_JPEG && dfb_jpeg_info(cur.jpeg[i], cur.jpeg_len[i], &fw, &fh) != DFB_OK) continue;
+        if (fw != g.sw || fh != g.sh)
+            return {DFB_ERR_SIZE, k + "frame " + std::to_string(first + i) + ": " + std::to_string(fw) + "x" + std::to_string(fh) +
+                                      ", frame 0 is " + std::to_string(g.sw) + "x" + std::to_string(g.sh)};
+    }
+    return {};
+}
+
+// What the workers of dfb_list_run_windows share about one video they took from the queue, under the run's mutex.
+struct SharedVideo {
+    long idx = 0;
+    int next_first = 0;           // first frame of the next window to read
+    bool reading = false;         // a source call for the video is in progress
+    bool ended = false;           // no window is read any more: the final one has been, or the video was cut
+    int next_deliver = 0;         // first_index of the next window to deliver
+    int cut = INT_MAX;            // windows from this first frame on are not delivered (a failure, or the run stopping)
+    int failed_first = INT_MAX;   // the earliest failed window, and its error
+    ItemResult failure;
+    uint64_t flows = 0;           // outputs of the windows delivered so far
+    Geometry g;                   // set by window 0
+};
+
+// The dispatch of dfb_list_run_windows (its policy is in the header).  A worker holds at most one window: it claims a video's
+// reader, reads the next window, releases the reader, runs the window through run_window and delivers it once every earlier
+// window of the video has been delivered.  Reads of one video are in order and never overlap, so every window read is held by
+// a worker that will deliver or drop it, and a worker waiting for its turn waits only on windows read before its own.
+int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queue *queue, const VideoArgs &a, dfb_list_stats *stats,
+                char *err, size_t err_len) {
+    const int n_workers = (int)r->workers.size();
+    dfb_list_stats st;
+    begin_run(r, st);
+    std::mutex mtx;
+    std::condition_variable cv;
+    std::list<SharedVideo> active;  // videos taken and not finished, in the order they were taken
+    long local_next = 0;
+    bool queue_empty = false;
+    SharedVideo *failed = nullptr;  // the first video to fail; its error is its earliest failed window's
+
+    // Under mtx: no video reads another window, and no window that has not been read is delivered.
+    auto stop = [&] {
+        for (auto &s : active) {
+            s.cut = std::min(s.cut, s.next_first);
+            s.ended = true;
+        }
+        cv.notify_all();
+    };
+    // Under mtx: window `first` of v failed.  An earlier window's failure replaces a later one's.
+    auto fail = [&](SharedVideo &v, int first, ItemResult res) {
+        if (first < v.failed_first) {
+            v.failed_first = first;
+            v.failure = std::move(res);
+        }
+        v.cut = std::min(v.cut, first);
+        if (!failed) failed = &v;
+        stop();
+    };
+    const auto t_start = clk::now();
+
+    auto worker = [&](int wi) {
+        dfb_list_runner::Worker &w = r->workers[wi];
+        cudaSetDevice(w.device);
+        double busy = 0;
+        long own = -1;  // the video this worker took from the queue
+        std::unique_lock<std::mutex> lk(mtx);
+        for (;;) {
+            // While the queue holds videos a worker runs its own video, then takes the next one, as dfb_list_run_stream does.
+            // Then it joins the earliest unfinished video whose reader is free, or waits for one.
+            SharedVideo *v = nullptr;
+            while (!failed) {
+                if (!queue_empty) {
+                    for (auto &s : active)
+                        if (s.idx == own && !s.ended) v = &s;
+                    if (v) break;
+                    const long idx = queue ? dfb_queue_next(queue) : local_next++;
+                    if (idx < n_videos) {
+                        v = &active.emplace_back();
+                        v->idx = own = idx;
+                        break;
+                    }
+                    queue_empty = true;
+                }
+                bool readable = false;  // a window is left to read
+                for (auto &s : active) {
+                    if (s.ended) continue;
+                    readable = true;
+                    if (!s.reading) {
+                        v = &s;
+                        break;
+                    }
+                }
+                if (v || !readable) break;
+                cv.wait(lk);
+            }
+            if (!v) break;
+            v->reading = true;
+            const int f0 = v->next_first;
+            lk.unlock();
+
+            const auto t0 = clk::now();
+            const std::string k = "video " + std::to_string(v->idx) + ": ";
+            dfb_video cur{};
+            Window win;
+            bool dropped = false;
+            auto fetch = [&](int first, int max_n, Window &got) -> ItemResult {
+                ItemResult fr = fetch_stream_window(r, source, a, v->idx, first, max_n, cur, got, v->g, nullptr);
+                const int m = fr.rc == DFB_OK ? window_outputs(a, got) : 0;
+                {
+                    std::lock_guard<std::mutex> g(mtx);
+                    v->reading = false;
+                    if (first >= v->cut) {  // the run stopped while this window was read: neither a window nor a failure
+                        dropped = true;
+                        return {DFB_ERR_INVALID_ARG, {}};
+                    }
+                    if (fr.rc != DFB_OK) {
+                        v->ended = true;
+                        return fr;
+                    }
+                    v->next_first = first + m;
+                    v->ended = got.ends;
+                    cv.notify_all();
+                }
+                // every worker that computes a window of the video, its first included, fits its handle to it here
+                std::string e;
+                if (m > 0)
+                    if (int rc = fit_worker(r, w, v->g.dw, v->g.dh, e)) return {rc, k + e};
+                return fr;
+            };
+            // Everything this window adds to the video and to the stats is recorded under mtx before next_deliver moves
+            // on: from then on the worker holding the video's next window may deliver it, and after the final window it
+            // removes the video.  The worker does not touch v once its window is delivered.
+            auto deliver = [&](int first, int m, bool ends, uint8_t *const *files, const size_t *lens) {
+                std::unique_lock<std::mutex> dl(mtx);
+                cv.wait(dl, [&] { return first >= v->cut || v->next_deliver == first; });
+                if (first >= v->cut) {
+                    dropped = true;
+                    return;
+                }
+                dl.unlock();
+                // every file of this chunk is in host memory now, and every earlier chunk of the video has been delivered
+                if (a.done) a.done(a.user, (int)v->idx, w.device, first, m, ends, files, lens);
+                dl.lock();
+                if (a.step != 0) {
+                    st.flows_per_worker[wi] += m;
+                    v->flows += m;
+                }
+                if (ends) {
+                    ++st.clips;
+                    ++st.clips_per_worker[wi];
+                    st.flows += v->flows;
+                    st.frames += (uint64_t)first + win.n;
+                    active.remove_if([&](const SharedVideo &s) { return &s == v; });
+                } else {
+                    v->next_deliver = first + m;
+                }
+                cv.notify_all();
+            };
+            ItemResult res = run_window(w, wi, v->idx, a, v->g, f0, win, fetch, deliver);
+            busy += seconds_since(t0);
+            lk.lock();
+            // a window that was delivered or dropped is done with; a failed one was never delivered, so v is still listed
+            if (!dropped && res.rc != DFB_OK) fail(*v, f0, std::move(res));
+        }
+        st.busy_seconds_per_worker[wi] = busy;
+        st.finish_seconds_per_worker[wi] = seconds_since(t_start);
+    };
+
+    if (n_videos > 0) run_workers(n_workers, worker);
+    end_run(r, st, t_start);
+    if (stats) *stats = st;
+    if (failed) {
+        set_error(err, err_len, failed->failure.error);
+        return failed->failure.rc;
+    }
     return DFB_OK;
 }
 
@@ -558,38 +796,34 @@ int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, 
     a.user = user;
     auto body = [&](int wi, long idx) -> ItemResult {
         dfb_list_runner::Worker &w = r->workers[wi];
-        const std::string k = "video " + std::to_string(idx) + ": ";
         Geometry g;
         dfb_video cur{};  // the source's latest window
-        // the video is sized by its first window with a frame, which also fits the worker's handle to it; every later
-        // frame must have frame 0's size
         auto fetch = [&](int first, int max_n, Window &win) -> ItemResult {
-            cur = dfb_video{};
-            char msg[512] = "";
-            if (source(user, (int)idx, first, max_n, &cur, msg, sizeof msg) != 0) return {DFB_ERR_INVALID_ARG, k + msg};
-            if (malformed(cur) || cur.n_frames > max_n)
-                return {DFB_ERR_INVALID_ARG, k + "the source returned a malformed window at frame " + std::to_string(first)};
-            win = {&cur, 0, cur.n_frames, cur.n_frames < max_n};
-            if (cur.n_frames == 0) return {};
-            if (first == 0) {
-                if (int rc = size_video(cur, 0, a, g)) return {rc, k + dfb_last_error(nullptr)};
-                std::string e;
-                if (int rc = fit_worker(r, w, g.dw, g.dh, e)) return {rc, k + e};
-            }
-            // a BGR window has one size; a JPEG file that cannot be sized is left to the decoder, which names the fault
-            const int n_check = cur.kind == DFB_VIDEO_BGR ? 1 : cur.n_frames;
-            for (int i = 0; i < n_check; ++i) {
-                int fw = cur.width, fh = cur.height;
-                if (cur.kind == DFB_VIDEO_JPEG && dfb_jpeg_info(cur.jpeg[i], cur.jpeg_len[i], &fw, &fh) != DFB_OK) continue;
-                if (fw != g.sw || fh != g.sh)
-                    return {DFB_ERR_SIZE, k + "frame " + std::to_string(first + i) + ": " + std::to_string(fw) + "x" + std::to_string(fh) +
-                                              ", frame 0 is " + std::to_string(g.sw) + "x" + std::to_string(g.sh)};
-            }
-            return {};
+            return fetch_stream_window(r, source, a, idx, first, max_n, cur, win, g, &w);
         };
         return run_video(w, wi, idx, a, g, fetch);
     };
     return run_videos_with(r, n_videos, queue, jpeg_exact, body, stats, err, err_len);
+}
+
+int dfb_list_run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, int step, int bound, int save_type, int quality,
+                         int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
+                         dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len) {
+    if (!source || n_videos < 0) {
+        set_error(err, err_len, "dfb_list_run_windows: bad arguments (a source is required, n_videos >= 0)");
+        return DFB_ERR_INVALID_ARG;
+    }
+    VideoArgs a;
+    if (int rc = check_video_args("dfb_list_run_windows", step, bound, save_type, quality, jpeg_exact, new_width, new_height, new_short,
+                                  chunk_flows, a, err, err_len))
+        return rc;
+    if (!r) {
+        set_error(err, err_len, "dfb_list_run_windows: bad arguments (no runner)");
+        return DFB_ERR_INVALID_ARG;
+    }
+    a.done = done;
+    a.user = user;
+    return with_jpeg_exact(r, jpeg_exact, [&] { return run_windows(r, n_videos, source, queue, a, stats, err, err_len); });
 }
 
 int dfb_run_list(const char *algorithm, const int *devices, int n_workers, const dfb_clip *clips, int n_clips, int step, int bound,

@@ -214,14 +214,34 @@ class ListRunner:
         video, or until the video's last chunk.  An exception in source ends the run with "video k: <message>"; one in
         on_chunk ends it too and is raised again here.  on_chunk and the result are those of run_videos, except that a video
         whose outputs end on a window boundary gets one more on_chunk call with no files and last_chunk True."""
+        return self._run_source("dfb_list_run_stream", n_videos, source, on_chunk, step, bound, save_type, quality, jpeg_exact,
+                                new_width, new_height, new_short, chunk_flows, queue)
+
+    def run_windows(self, n_videos, source, on_chunk=None, step=1, bound=20, save_type="jpg", quality=95, jpeg_exact=0, new_width=0,
+                    new_height=0, new_short=0, chunk_flows=0, queue=None):
+        """run_stream with a video's windows shared among the workers (dfb_list_run_windows): once the queue is empty, idle
+        workers join the unfinished videos, so a single video runs on every worker.  source is called for one video in frame
+        order, one call at a time, but possibly from different workers' threads.  A window is kept alive until its on_chunk
+        call returns (or until the run ends after a failure).  on_chunk calls for one video come in first_index order, one at
+        a time, on the thread of the worker that computed the window.  Arguments, files, errors and the result are
+        run_stream's; flows_per_worker counts the flows each worker computed."""
+        return self._run_source("dfb_list_run_windows", n_videos, source, on_chunk, step, bound, save_type, quality, jpeg_exact,
+                                new_width, new_height, new_short, chunk_flows, queue)
+
+    def _run_source(self, fn, n_videos, source, on_chunk, step, bound, save_type, quality, jpeg_exact, new_width, new_height, new_short,
+                    chunk_flows, queue):
+        """run_stream and run_windows: they differ in how long a window lives.  dfb_list_run_stream is done with a video's
+        window at its next source call; dfb_list_run_windows with each window once its on_chunk call has returned."""
         if save_type not in _SAVE_TYPES:
             raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
         per = 2 if step != 0 and save_type != "png" else 1
-        windows = {}  # video -> the latest window and the memory behind it
+        shared = fn == "dfb_list_run_windows"
+        windows = {}  # (video, first) or video -> a live window and the memory behind it
         failures = []
 
         def _source(user, video, first, max_n, out, msg, msg_len):
-            windows.pop(video, None)  # the worker is done with the previous window
+            if not shared:
+                windows.pop(video, None)  # the worker is done with the previous window
             try:
                 if failures:
                     raise RuntimeError("stopped after an on_chunk call failed")
@@ -231,7 +251,7 @@ class ListRunner:
                 C.memmove(msg, text + b"\0", len(text) + 1)
                 return 1
             out[0] = v
-            windows[video] = keep
+            windows[(video, first) if shared else video] = keep
             return 0
 
         def _done(user, video, dev, first, n, last, files, lens):
@@ -240,22 +260,23 @@ class ListRunner:
                     on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
             except BaseException as ex:
                 failures.append(ex)
-            if last:
+            if shared:
+                windows.pop((video, first), None)
+            elif last:
                 windows.pop(video, None)
 
         src = _lib.FRAMES_FN(_source)
         cb = _lib.FILES_DONE_FN(_done)
         st = _lib.ListStats()
         err = C.create_string_buffer(512)
-        rc = self._L.dfb_list_run_stream(self._r, int(n_videos), C.cast(src, C.c_void_p), int(step), int(bound),
-                                         _SAVE_TYPES[save_type], int(quality), int(jpeg_exact),
-                                         int(new_width), int(new_height), int(new_short), int(chunk_flows),
-                                         queue._q if queue is not None else None, C.cast(cb, C.c_void_p), None, C.byref(st), err, 512)
+        rc = getattr(self._L, fn)(self._r, int(n_videos), C.cast(src, C.c_void_p), int(step), int(bound), _SAVE_TYPES[save_type],
+                                  int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
+                                  queue._q if queue is not None else None, C.cast(cb, C.c_void_p), None, C.byref(st), err, 512)
         windows.clear()
         if failures:
             raise failures[0]
         if rc != _lib.DFB_OK:
-            raise RuntimeError(err.value.decode() or "dfb_list_run_stream failed (%d)" % rc)
+            raise RuntimeError(err.value.decode() or "%s failed (%d)" % (fn, rc))
         return _stats(st)
 
     @staticmethod

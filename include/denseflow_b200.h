@@ -599,6 +599,39 @@ int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, 
                         int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
                         dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len);
 
+/*
+ * ---- the same windows shared among the workers: one video on every GPU -------------------------------------------------
+ * dfb_list_run_windows takes dfb_list_run_stream's arguments and writes the same files, but a video's windows, not the video,
+ * are the unit of work once the queue is empty, so a single video (or the tail of a list) runs on every worker, and one worker
+ * reads a video's next window while another computes the current one.
+ *   - Windows: the sequence dfb_list_run_stream asks for (max_n = chunk_flows + |step|, chunk_flows at step 0; consecutive
+ *     windows overlap by |step|; a short window ends the video).  The source calls for one video come in frame order and never
+ *     overlap in time, but may come from different workers' threads.
+ *   - Lifetime: what the source returns for a window stays valid until that window's `done` call returns, or until the call
+ *     returns after a failure (not "until the next call for this video").
+ *   - Delivery: the `done` calls for one video come in first_index order, each after the previous one has returned, on the
+ *     thread of the worker that computed the window, with that worker's device.  last_chunk comes once per video, in its last
+ *     call; the n = 0 trailing call follows dfb_list_run_stream's rule.  The files and every other argument equal
+ *     dfb_list_run_stream's for the same source.
+ *   - Scheduling: while the queue (the in-process counter or `queue`) holds videos, a worker runs the video it took and then
+ *     takes the next one, in dfb_list_run_stream's order.  Once the queue is empty, an idle worker joins the earliest
+ *     unfinished video whose reader is free (no source call in progress, final window not read yet), reads its next window and
+ *     computes it; if no reader is free it waits until one is, and stops once no window is left to read.  A worker holds at
+ *     most one window, so at most n_workers windows are alive.
+ *   - Geometry: the video's first window sizes it; a worker that joins fits its handle to the video before it computes.  The
+ *     frame-size checks are dfb_list_run_stream's.
+ *   - Failures: the error reported for a video is the one a one-worker run reports: its earliest failed window's (source,
+ *     size, decode or handle).  Windows before it are computed and delivered; it and every later window of the video get no
+ *     `done` call.  Workers take no new windows, a window whose read completes after the failure is dropped, and the call
+ *     returns once every worker has stopped.  The runner stays usable.
+ *   - Stats: clips, flows and frames are dfb_list_run_stream's; flows_per_worker counts the flows each worker computed and
+ *     clips_per_worker the videos whose last window it delivered.
+ * Sharing one video among processes is not done: a dfb_queue still hands out whole videos.
+ */
+int dfb_list_run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, int step, int bound, int save_type, int quality,
+                         int jpeg_exact, int new_width, int new_height, int new_short, int chunk_flows, dfb_queue *queue,
+                         dfb_files_done_fn done, void *user, dfb_list_stats *stats, char *err, size_t err_len);
+
 #ifdef __cplusplus
 }
 #endif
