@@ -13,9 +13,6 @@ LIB_PATHS = {
     # the default library with the -st=h5 file writer (the reference's -DUSE_HDF5=yes build)
     "hdf5": os.path.join(_HERE, "lib", "libdenseflow_b200_hdf5.so"),
     "strict_hdf5": os.path.join(_HERE, "lib", "libdenseflow_b200_strict_hdf5.so"),
-    # geometry experiments (denseflow_b200/build.py VARIANTS), built on request only
-    "t256": os.path.join(_HERE, "lib", "libdenseflow_b200_t256.so"),
-    "t512": os.path.join(_HERE, "lib", "libdenseflow_b200_t512.so"),
 }
 
 DFB_OK = 0

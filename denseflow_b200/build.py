@@ -21,9 +21,6 @@ VARIANTS = {
     "default": ("libdenseflow_b200.so", []),
     # IEEE arithmetic, no FMA contraction: used by tests to separate restatement bugs from fp noise
     "strict": ("libdenseflow_b200_strict.so", ["-DDFB_STRICT_FP", "-fmad=false", "-prec-div=true", "-prec-sqrt=true"]),
-    # geometry experiments of the fused tvl1 kernel (not built by default): python -m denseflow_b200.build t256
-    "t256": ("libdenseflow_b200_t256.so", ["-DDFB_FUSED_THREADS=256"]),
-    "t512": ("libdenseflow_b200_t512.so", ["-DDFB_FUSED_THREADS=512"]),
     # the reference's -DUSE_HDF5=yes build: the default library plus the -st=h5 file writer
     "hdf5": ("libdenseflow_b200_hdf5.so", ["-DDFB_USE_HDF5=1"]),
     # the strict library with the writer: lets tests compare the command's h5 files with the oracle

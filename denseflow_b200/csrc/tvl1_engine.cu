@@ -35,12 +35,9 @@ struct Tvl1Params {
     double scale_step = 0.8;
     int fused = 1;
     int fused_k = kFusedDefaultK;
-    int flag_sync = 1;
     int time_kernels = 0;
     int use_tma = 1;
-    int prefetch = 1;
     int lanes = 0;  // pairs solved side by side per fused launch; 0 = choose from the tile counts
-    int serial_launches = 0;  // 1: fused launches of all handles on one device execute strictly one after another (event chain)
     int median_filtering = 0;  // 3 or 5: the window of the median of u1, u2 between iterations (DESIGN §4.3); 0 or 1: off
     int median_interval = 30;  // the median runs before every iteration n of a warp with n % median_interval == 0
     int median_k() const { return median_filtering > 1 ? median_filtering : 0; }
@@ -50,8 +47,6 @@ class Tvl1 final : public FlowAlgorithm {
   public:
     Tvl1(int device, int max_w, int max_h) : device_(device), max_w_(max_w), max_h_(max_h) {
         DFB_CUDA(cudaSetDevice(device_));
-        if (const char *e = std::getenv("DFB_TVL1_LANES")) prm_.lanes = std::max(0, std::min(atoi(e), kFusedMaxLanes));  // debugging aid
-        if (const char *e = std::getenv("DFB_TVL1_SERIAL_LAUNCHES")) prm_.serial_launches = atoi(e) != 0;         // debugging aid
         allocate();
     }
     ~Tvl1() override {
@@ -89,11 +84,8 @@ class Tvl1 final : public FlowAlgorithm {
         }
         else if (k == "fused") { if (!is_flag(v)) return false; prm_.fused = (int)v; }
         else if (k == "fused_k") { if (!whole_in(v, 1, kFusedMaxK) || 2 * v >= kFusedTileH) return false; prm_.fused_k = (int)v; }
-        else if (k == "flag_sync") { if (!whole_in(v, 0, INT_MAX)) return false; prm_.flag_sync = (int)v; }  // 0 CTA barriers, else neighbour flags
         else if (k == "time_kernels") { if (!is_flag(v)) return false; prm_.time_kernels = (int)v; }
         else if (k == "use_tma") { if (!is_flag(v)) return false; prm_.use_tma = (int)v; }
-        else if (k == "prefetch") { if (!is_flag(v)) return false; prm_.prefetch = (int)v; }
-        else if (k == "serial_launches") { if (!is_flag(v)) return false; prm_.serial_launches = (int)v; }
         else if (k == "lanes") { if (!whole_in(v, 0, kFusedMaxLanes)) return false; prm_.lanes = (int)v; }
         else if (k == "median_filtering") { if (!(v == 0 || v == 1 || v == 3 || v == 5)) return false; prm_.median_filtering = (int)v; }
         else if (k == "median_interval") { if (!whole_in(v, 1, INT_MAX)) return false; prm_.median_interval = (int)v; }
@@ -111,11 +103,8 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "scale_step") *v = prm_.scale_step;
         else if (k == "fused") *v = prm_.fused;
         else if (k == "fused_k") *v = prm_.fused_k;
-        else if (k == "flag_sync") *v = prm_.flag_sync;
         else if (k == "time_kernels") *v = prm_.time_kernels;
         else if (k == "use_tma") *v = prm_.use_tma;
-        else if (k == "prefetch") *v = prm_.prefetch;
-        else if (k == "serial_launches") *v = prm_.serial_launches;
         else if (k == "lanes") *v = prm_.lanes;
         else if (k == "median_filtering") *v = prm_.median_filtering;
         else if (k == "median_interval") *v = prm_.median_interval;
@@ -327,7 +316,7 @@ class Tvl1 final : public FlowAlgorithm {
             const char *name;
             int stage, n_in, n_out, n_sc;
         } kStages[] = {{"tvl1_level_start", kFusedStageLevelStart, 3, 8, 2}, {"tvl1_warp", kFusedStageWarp, 6, 4, 1},
-                       {"tvl1_gq", kFusedStageGq, 1, 1, 1},        {"tvl1_chunks", kFusedStageChunks, 10, 6, 8},
+                       {"tvl1_gq", kFusedStageGq, 1, 1, 1},        {"tvl1_chunks", kFusedStageChunks, 10, 6, 6},
                        {"tvl1_upsample", kFusedStageUpsample, 2, 2, 3}, {"tvl1_merge", kFusedStageMerge, 2, 2, 2},
                        {"tvl1_median", kFusedStageMedian, 2, 2, 2}};
         int si = -1;
@@ -338,7 +327,8 @@ class Tvl1 final : public FlowAlgorithm {
         if (n_in != st.n_in || n_out != st.n_out)
             throw std::runtime_error(k + ": expects " + std::to_string(st.n_in) + " inputs and " + std::to_string(st.n_out) + " outputs");
         auto sc = [&](int i, double dflt) { return i < n_scalars ? scalars[i] : dflt; };
-        const int nb = (int)sc(st.n_sc - 1, 1);
+        // lanes is the last scalar, also when a call passes more scalars than the stage reads
+        const int nb = n_scalars >= st.n_sc ? (int)scalars[n_scalars - 1] : 1;
         if (nb < 1 || nb > kFusedParamLanes || h % nb) throw std::runtime_error(k + ": lanes must be in [1, 16] and divide the height");
         const int ph = h / nb;
         // level 0 = the planes' size; the upsample runs from level 1 (its inputs) to level 0 (its destination)
@@ -372,11 +362,7 @@ class Tvl1 final : public FlowAlgorithm {
         ensure_slots(2 * nb);
         ensure_lanes(nb);
         const Tvl1Params keep = prm_;
-        if (st.stage == kFusedStageChunks) {
-            prm_.use_tma = sc(4, 1) != 0;
-            prm_.flag_sync = (int)sc(5, 1);
-            prm_.prefetch = sc(6, 1) != 0;
-        }
+        if (st.stage == kFusedStageChunks) prm_.use_tma = sc(4, 1) != 0;
         std::vector<void *> scratch;
         FusedJob jobs[kFusedParamLanes];
         for (int i = 0; i < nb; ++i) {
@@ -693,9 +679,7 @@ class Tvl1 final : public FlowAlgorithm {
         job.iterations = prm_.iterations;
         job.epsilon = prm_.epsilon;
         job.k = prm_.fused_k;
-        job.flag_sync = prm_.flag_sync;
         job.use_tma = prm_.use_tma;
-        job.prefetch = prm_.prefetch;
         job.median_k = prm_.median_k();
         job.median_interval = prm_.median_interval;
         if (prm_.use_tma) ensure_tensor_maps(wk, lv, n);
@@ -771,7 +755,7 @@ class Tvl1 final : public FlowAlgorithm {
         }
         batch.jobs = job_ring_d_[jr];
         batch.host_jobs = host_jobs;
-        launches += launch_tvl1_fused(batch, device_, s, prm_.serial_launches != 0);
+        launches += launch_tvl1_fused(batch, device_, s);
         if (prm_.time_kernels) timer_.end(s, 1, count);
         last_lane_ = count - 1;
         DFB_CUDA(cudaEventRecord(stats_event_, s));

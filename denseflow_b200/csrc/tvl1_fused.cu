@@ -42,16 +42,10 @@ namespace dfb {
 
 namespace {
 
-#ifndef DFB_FUSED_THREADS
-#define DFB_FUSED_THREADS 512
-#endif
-constexpr int kThreads = DFB_FUSED_THREADS;
+constexpr int kThreads = 512;
 constexpr int kWarps = kThreads / 32;
 constexpr int kPartialSet = 256;  // stride between the two sets of per-CTA convergence partials (>= CTAs per lane)
-#ifndef DFB_FUSED_RPT
-#define DFB_FUSED_RPT 4
-#endif
-constexpr int RPT = DFB_FUSED_RPT;  // rows per thread
+constexpr int RPT = 4;            // rows per thread
 constexpr int TW = 128;           // tile width  = 32 lanes x 4 px
 constexpr int TH = kWarps * RPT;  // tile height = 64
 constexpr int kConstPlane = TW * TH;
@@ -324,7 +318,6 @@ struct TileCtx {
     int so0;          // this thread's slot in row 0 of its warp in the shared-memory planes
     int lane, wq;
     int base;         // progress-counter value that means "tile loaded"
-    bool flagsync;    // neighbour-warp progress counters (true) or CTA-wide barriers (false, debug / comparison)
     int jlast, rbot;  // EDGE tiles: pixel j == jlast of this lane is the last image column, row r == rbot of this warp the last image row
     bool edge_x, edge_y;
     bool left_col;    // pixel .x of this thread is image column 0 (lane 0 of tile column 0)
@@ -359,18 +352,16 @@ __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const
     volatile int *prog = sm.prog;
     const int so0 = t.so0, lane = t.lane, wq = t.wq;
     if (RPT * wq + RPT - 1 < t.halo_top * (it + 1) || RPT * wq >= TH - t.halo_bot * it) {
-        if (wq > 0 && t.flagsync) wait_ge(&prog[wq - 1], t.base + 2 * it);
+        if (wq > 0) wait_ge(&prog[wq - 1], t.base + 2 * it);
         signal(&prog[wq], t.base + 2 * it + 1, lane);
-        if (!t.flagsync) __syncthreads();
-        if (wq < kWarps - 1 && t.flagsync) wait_ge(&prog[wq + 1], t.base + 2 * it + 1);
+        if (wq < kWarps - 1) wait_ge(&prog[wq + 1], t.base + 2 * it + 1);
         signal(&prog[wq], t.base + 2 * it + 2, lane);
-        if (!t.flagsync) __syncthreads();
         return;
     }
     // p above the region's first row: the image border (p = 0) for tile row 0, halo garbage otherwise
     float4 up12 = zero4(), up22 = zero4();
     if (wq > 0) {
-        if (t.flagsync) wait_ge(&prog[wq - 1], t.base + 2 * it);  // D3 of the previous iteration of the warp above
+        wait_ge(&prog[wq - 1], t.base + 2 * it);  // D3 of the previous iteration of the warp above
         up12 = *reinterpret_cast<const float4 *>(&sm.p_bot[0][wq - 1][4 * lane]);
         up22 = *reinterpret_cast<const float4 *>(&sm.p_bot[1][wq - 1][4 * lane]);
     }
@@ -416,7 +407,6 @@ __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const
         st4(&sm.u[1][so], n2);
         if (r == 0) {
             signal(&prog[wq], t.base + 2 * it + 1, lane);  // row 0 of the new u is what the warp above waits for
-            if (!t.flagsync) __syncthreads();
         } else {
             // -------- dual, row r-1: p <- (p + taut * grad u) / (1 + taut * |grad u|) ------------
             float r1 = __shfl_down_sync(0xffffffffu, c1.x, 1);
@@ -434,7 +424,7 @@ __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const
     {
         float4 d1 = c1, d2 = c2;  // region's last row: halo, or the mirrored image border
         if (wq < kWarps - 1) {
-            if (t.flagsync) wait_ge(&prog[wq + 1], t.base + 2 * it + 1);
+            wait_ge(&prog[wq + 1], t.base + 2 * it + 1);
             if (!(EDGE && t.edge_y && t.rbot == RPT - 1)) {
                 d1 = *reinterpret_cast<const float4 *>(&sm.u[0][so0 + RPT * TW]);
                 d2 = *reinterpret_cast<const float4 *>(&sm.u[1][so0 + RPT * TW]);
@@ -451,7 +441,6 @@ __device__ __forceinline__ void tile_iteration(Smem &sm, const TileCtx &t, const
     st4(&sm.p_bot[0][wq][4 * lane], p12[RPT - 1]);
     st4(&sm.p_bot[1][wq][4 * lane], p22[RPT - 1]);
     signal(&prog[wq], t.base + 2 * it + 2, lane);
-    if (!t.flagsync) __syncthreads();
 }
 
 template <bool EDGE>
@@ -515,7 +504,6 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     const int gx0 = rx0 + 4 * lane;
     const int gy0 = ry0 + RPT * wq;
     volatile int *prog = sm.prog;
-    const bool flagsync = job.flag_sync != 0;
     const char *maps = level_maps(job, level);
     const int nrx0 = ntx_next * (TW - 2 * hx), nry0 = nty_next * (TH - 2 * hy);
 
@@ -538,9 +526,8 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     const int so0 = (RPT * wq) * TW + 4 * lane;  // this thread's slot in row 0 of its warp (thread-private in smem planes)
     const bool use_tma = job.use_tma != 0 && !ring_only;
     // The warp above reads this warp's first u row in its dual steps: it must have finished the previous tile (its counter
-    // reached base - 2 = "last dual step of the previous tile done") before the row is overwritten.  (Without flags the
-    // previous visit ended with a CTA-wide barrier.)
-    if (flagsync && wq > 0) wait_ge(&prog[wq - 1], base - 2);
+    // reached base - 2 = "last dual step of the previous tile done") before the row is overwritten.
+    if (wq > 0) wait_ge(&prog[wq - 1], base - 2);
     if (use_tma) {
         // this warp's generic-proxy accesses to its rows are ordered before the async-proxy writes of the loads
         fence_proxy_async();
@@ -580,7 +567,7 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     }
     if (use_tma) mbar_wait(&sm.tma_bar[wq], tma_parity);
     if (lane == 0) sm.next[wq] = make_int4(nrx0, ntx_next >= 0 ? nry0 : -1, level, 0);
-    if (job.prefetch && ntx_next >= 0) {
+    if (ntx_next >= 0) {
         // This CTA's next tile of the chunk: ask for its ten planes to be brought into L2 now, so the copy from HBM runs
         // under this tile's iterations (with several pairs in flight the planes of a level do not fit the L2).  Every warp
         // asks for its own rows.
@@ -613,7 +600,6 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     t.lane = lane;
     t.wq = wq;
     t.base = base;
-    t.flagsync = flagsync;
     // image borders inside this tile's region (tile-uniform)
     t.edge_x = W - 1 >= rx0 && W - 1 < rx0 + TW;
     t.edge_y = H - 1 >= ry0 && H - 1 < ry0 + TH;
@@ -632,7 +618,6 @@ __device__ __forceinline__ float process_tile(const FusedJob &job, const Tvl1Con
     st4(&sm.p_bot[0][wq][4 * lane], p12[RPT - 1]);
     st4(&sm.p_bot[1][wq][4 * lane], p22[RPT - 1]);
     signal(&prog[wq], base, lane);
-    if (!flagsync) __syncthreads();
     if (prof_on) {
         const unsigned long long tt = gtime();
         sm.prof[5] += tt - t0;
@@ -1026,7 +1011,7 @@ void launch_tvl1_stage(const FusedBatch &batch, const FusedStageArgs &a, cudaStr
     DFB_CUDA(cudaLaunchKernelEx(&cfg, k_tvl1_stage, param_batch(batch), a));
 }
 
-int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, bool serialise) {
+int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s) {
     // the opt-in shared-memory size is a per-device function attribute: handles on several devices may live in one process
     static std::mutex mtx;
     static bool configured[64] = {};
@@ -1050,25 +1035,13 @@ int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, bool 
     // of the second grid runs as soon as its own CTAs are resident: the second grid fills the SMs the first one's finished
     // lanes leave behind (+3.8 % on the 340x256 list, 4020 vs 3873 pairs/s).  The block scheduler hands out a later grid's
     // CTAs only after every CTA of the earlier grid has been placed, so an earlier grid is never starved by a later one; a
-    // lost arrival would still surface through the barrier watchdog rather than hang.  `serialise` (engine knob
-    // serial_launches) chains the launches of one device through an event for callers that want strict one-at-a-time
-    // execution.
-    {
-        std::lock_guard<std::mutex> lk(mtx);
-        const int d = device >= 0 && device < 64 ? device : 0;
-        static cudaEvent_t last_done[64] = {};
-        if (serialise) {
-            if (!last_done[d]) DFB_CUDA(cudaEventCreateWithFlags(&last_done[d], cudaEventDisableTiming));
-            else DFB_CUDA(cudaStreamWaitEvent(s, last_done[d], 0));
-        }
-        const bool median = batch.host_jobs[0].median_k > 0;  // every lane of a launch has its handle's parameters
-        if (batch.njobs <= kFusedParamLanes) {
-            DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatchParams, true> : k_tvl1_pair<FusedBatchParams, false>,
-                                        param_batch(batch)));
-        } else {
-            DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatch, true> : k_tvl1_pair<FusedBatch, false>, batch));
-        }
-        if (serialise) DFB_CUDA(cudaEventRecord(last_done[d], s));
+    // lost arrival would still surface through the barrier watchdog rather than hang.
+    const bool median = batch.host_jobs[0].median_k > 0;  // every lane of a launch has its handle's parameters
+    if (batch.njobs <= kFusedParamLanes) {
+        DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatchParams, true> : k_tvl1_pair<FusedBatchParams, false>,
+                                    param_batch(batch)));
+    } else {
+        DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatch, true> : k_tvl1_pair<FusedBatch, false>, batch));
     }
     return 1;
 }

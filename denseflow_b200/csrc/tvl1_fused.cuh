@@ -34,9 +34,7 @@ constexpr unsigned kFusedStallPolls = 1u << 25;
 
 struct FusedJob {
     int nscales, warps, iterations, k;
-    int flag_sync;  // 1: neighbour-warp progress counters in the tile loop, 0: CTA-wide barriers
     int use_tma;    // 1: constants + u tiles staged by TMA (cp.async.bulk.tensor.2d), 0: LDG -> STS
-    int prefetch;   // 1: while a tile iterates, the CTA's next tile of the chunk is prefetched into L2 (TMA prefetch + prefetch.global.L2)
     int median_k;   // 3 or 5: u1, u2 <- their k x k median before every iteration n of a warp with n % median_interval == 0; 0: off
     // CUtensorMap[nscales][kFusedMapsPerLevel] in global memory: I1wx, I1wy, grad, rho_c, u1[0], u2[0], u1[1], u2[1]
     const void *tmaps;
@@ -54,7 +52,7 @@ struct FusedJob {
     size_t flow_pitch_bytes;
     // bound > 0: emit the two quantised uint8 planes instead of the float2 field (PairJob)
     int bound;
-    int median_interval;  // (beside median_k and bound: both fill alignment padding, so the layout of the other fields is unchanged)
+    int median_interval;  // see median_k
     uint8_t *qx, *qy;
     size_t q_pitch;
     // fx non-null: emit u1 / u2 as two float planes instead of the float2 field (PairJob)
@@ -85,27 +83,19 @@ __host__ __device__ inline int fused_tiles_along(int n, int T, int h) {
     const int stride = T - 2 * h;
     return n <= T ? 1 : (n - 2 * h + stride - 1) / stride;
 }
-#ifndef DFB_FUSED_THREADS
-#define DFB_FUSED_THREADS 512
-#endif
-#ifndef DFB_FUSED_RPT
-#define DFB_FUSED_RPT 4
-#endif
-constexpr int kFusedTileW = 128, kFusedTileH = DFB_FUSED_THREADS / 32 * DFB_FUSED_RPT;
-// CTAs of the persistent kernel resident per SM: 512-thread CTAs own the whole SM (192 KB tile); 256-thread CTAs
-// (128 x 32 tiles, 96 KB) run two to an SM, so one CTA's MUFU-bound dual half-steps and tile loads overlap the
-// other's FMA-bound primal half-steps (the warps of ONE tile are forced into lock-step by their neighbour dependencies)
-constexpr int kFusedCtasPerSm = DFB_FUSED_THREADS <= 256 ? 2 : 1;
-constexpr int kFusedDefaultK = kFusedTileH >= 64 ? 8 : 4;
+constexpr int kFusedTileW = 128, kFusedTileH = 64;
+// CTAs of the persistent kernel resident per SM: a 512-thread CTA owns the whole SM (192 KB tile)
+constexpr int kFusedCtasPerSm = 1;
+constexpr int kFusedDefaultK = 8;
 
 int fused_num_sms(int device);
 inline int fused_cta_slots(int device) { return fused_num_sms(device) * kFusedCtasPerSm; }
-// Encodes one 2-D fp32 descriptor of one warp's rows of a tile (box 128 x DFB_FUSED_RPT, no swizzle, zero fill out of bounds)
+// Encodes one 2-D fp32 descriptor of one warp's rows of a tile (box 128 x 4, no swizzle, zero fill out of bounds)
 // into out[128 bytes].
 // plane: base pointer, extent w x h (elements / rows), row pitch in elements.
 void fused_encode_tensor_map(void *out, const float *plane, int w, int h, int pitch);
 // returns the number of kernels launched
-int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, bool serialise);
+int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s);
 
 // Test hook: one phase of k_tvl1_pair (its own device functions) on up to kFusedParamLanes lanes in one cooperative launch.
 enum FusedStage : int {

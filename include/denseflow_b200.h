@@ -66,15 +66,13 @@ const char *dfb_last_error(const dfb_handle *h);
  * starts with one; an optional extra of CPU DualTVL1's kind that the reference's CUDA TV-L1 does not have) and
  * "median_interval" (>= 1, default 30); engine knobs: "fused" (1 = persistent fused primal+dual kernel
  * [default], 0 = one kernel per half-step, the reference's launch structure), "fused_k" (iterations kept on chip per tile
- * visit, 1..8, default 8), "lanes" (pairs solved side by side per launch, 0 = auto [default], up to 64), "flag_sync" (1 =
- * neighbour-warp progress flags in the tile loop [default], 0 = CTA-wide barriers), "use_tma" (1 = TMA staging of the
- * shared-memory tiles [default]), "prefetch" (1 = L2 prefetch of a CTA's next tile during the iterations [default]),
- * "serial_launches" (1 = the fused launches of all handles on one device run strictly one after another; 0 [default] = a
- * second handle's launch fills the SMs the first one's finished lanes free), "time_kernels" (CUDA-event timing of the dominant kernel, see dfb_counters).  farn: "num_levels" (0..5)
+ * visit, 1..8, default 8), "lanes" (pairs solved side by side per launch, 0 = auto [default], up to 64), "use_tma"
+ * (1 = TMA staging of the shared-memory tiles [default]), "time_kernels" (CUDA-event timing of the dominant kernel, see
+ * dfb_counters).  farn: "num_levels" (0..5)
  * "num_iters" (>= 1) "poly_sigma" (finite, > 0) (winSize 13, polyN 5, pyrScale 0.5 are fixed), "time_kernels".  Every
- * combination of the engine knobs produces bit-identical flows.  Counts take whole numbers only, and on/off knobs 0 or 1.  "flag_sync" takes any whole
- * number >= 0; every value other than 0 means 1.  A refused value (NaN, an infinity, a fraction or
- * a value out of range) returns DFB_ERR_INVALID_ARG with "bad parameter <name>" and leaves the parameter unchanged.
+ * combination of the engine knobs produces bit-identical flows.  Counts take whole numbers only, and on/off knobs 0 or 1.
+ * A refused value (NaN, an infinity, a fraction or a value out of range) returns DFB_ERR_INVALID_ARG with "bad parameter
+ * <name>" and leaves the parameter unchanged.
  * Both algorithms: "jpeg_exact" (0 [default] = JPEG files through nvJPEG; 1 = every JPEG this handle writes is exactly the
  * file cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality]) writes with OpenCV's other defaults, libjpeg-turbo 3.x:
  * baseline, standard Huffman tables, islow DCT, gray or YCbCr 4:2:0, no restart markers).  It covers
@@ -428,14 +426,15 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   The two pair stages run `pairs` (1..8, default 1) pairs in one launch: every plane then stacks the pairs' planes along
  *   its rows (height = pairs x the pair's height).
  * On a "tvl1" handle, single phases of the fused pair kernel, run by one cooperative launch of its own device code on the
- * engine's lanes, tensor maps and level geometry.  The last scalar is `lanes` (1..16, default 1): every plane stacks one
- * plane per lane along its rows, and lane i runs on its own CTAs and workspace.  G (CTAs per lane) 0 means as many as fit.
+ * engine's lanes, tensor maps and level geometry.  The last scalar is `lanes` (1..16, default 1 when fewer scalars than the
+ * stage lists are given; scalars between the listed ones and the last are not read): every plane stacks one plane per lane
+ * along its rows, and lane i runs on its own CTAs and workspace.  G (CTAs per lane) 0 means as many as fit.
  *   "tvl1_level_start" in {I1, u1, u2}                     out {I1x, I1y, p11, p12, p21, p22, u1, u2}; scalars {coarsest, lanes}
  *   "tvl1_warp"        in {I0, I1, I1x, I1y, u1, u2}       out {I1wx, I1wy, q, rho_c}; scalars {lanes}
  *   "tvl1_gq"          in {grad}                           out {q}; scalars {lanes}
  *     (q: the gradient plane as the inner loop reads it: grad in the strict build, -rcp(grad) or -1e30 in the default build)
  *   "tvl1_chunks"      in {I1wx, I1wy, grad, rho_c, u1, u2, p11, p12, p21, p22}  out {u1, u2, p11, p12, p21, p22};
- *                      scalars {kk, n, check, G, use_tma, flag_sync, prefetch, lanes}; n chunks of kk iterations with the
+ *                      scalars {kk, n, check, G, use_tma, lanes}; n chunks of kk iterations with the
  *                      handle's tau / lambda / theta; check: every chunk sums the convergence error, scalars_out[i] = lane i's
  *                      error of the last chunk (scalars_out must then hold `lanes` doubles)
  *   "tvl1_upsample"    in {u1, u2}                         out {u1, u2 (scalars[0] x scalars[1])}; scalars {dst w, dst h, lanes}

@@ -18,7 +18,6 @@ cfgs = [(v, l, k, 1) for v in variants for k in ks for l in lane_list]
 for variant, lanes, k, fs in cfgs:
     e = d.OpticalFlowDual_TVL1.create(0, W, H, variant)
     e.set("lanes", lanes); e.set("fused_k", k)
-    if os.environ.get("DFB_PREFETCH") is not None: e.set("prefetch", int(os.environ["DFB_PREFETCH"]))
     e.calc_batch_device(dev, 1, out); torch.cuda.synchronize()
     e.reset_counters()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -38,7 +38,7 @@ CASES = [
     ("tvl1", 340, 256, 5, 3, {"fused": 0}),
     ("tvl1", 340, 256, 4, -1, {"fused": 0, "median_filtering": 5, "median_interval": 7}),
     ("tvl1", 340, 256, 6, 1, {"median_filtering": 3, "median_interval": 30}),
-    ("tvl1", 340, 256, 6, 1, {"lanes": 2, "use_tma": 0, "flag_sync": 0, "fused_k": 3}),
+    ("tvl1", 340, 256, 6, 1, {"lanes": 2, "use_tma": 0, "fused_k": 3}),
     ("tvl1", 97, 131, 3, 1, {}),
     ("tvl1", 1080, 7, 3, -1, {}),
     ("tvl1", 1, 1, 2, 1, {}),

@@ -363,8 +363,7 @@ REFUSED = {
              "theta": NOT_FINITE + [0, -0.3], "nscales": NOT_FINITE + [0, -1, 17, 2.5, 1e10], "warps": NOT_FINITE + [0, 17, 2.5],
              "epsilon": NOT_FINITE, "iterations": NOT_FINITE + [0, -3, 2.5, 1e10, 2.0 ** 31],
              "scale_step": NOT_FINITE + [0, -0.5, 0.81, 1.0], "fused": FLAG, "fused_k": NOT_FINITE + [0, 9, 2.5, -1],
-             "flag_sync": NOT_FINITE + [-1, 1.5, 1e10], "time_kernels": FLAG, "use_tma": FLAG, "prefetch": FLAG,
-             "serial_launches": FLAG, "lanes": NOT_FINITE + [-1, 65, 2.5]},
+             "time_kernels": FLAG, "use_tma": FLAG, "lanes": NOT_FINITE + [-1, 65, 2.5]},
     "farn": {"num_levels": NOT_FINITE + [-1, 6, 2.5], "num_iters": NOT_FINITE + [0, -1, 2.5, 1e10],
              "poly_sigma": NOT_FINITE + [0, -1.1], "pyr_scale": NOT_FINITE + [0, 0.25], "win_size": NOT_FINITE + [15, 13.5],
              "poly_n": NOT_FINITE + [7], "time_kernels": FLAG},
@@ -372,7 +371,7 @@ REFUSED = {
 ACCEPTED = {
     "tvl1": [("nscales", 1), ("nscales", 16), ("warps", 1), ("warps", 16), ("fused_k", 1), ("fused_k", 8), ("lanes", 64), ("lanes", 0),
              ("lambda", 0), ("epsilon", 0), ("epsilon", -1), ("iterations", 1), ("iterations", 2 ** 31 - 1), ("scale_step", 0.8),
-             ("scale_step", 0.05), ("tau", 1e-3), ("theta", 5.0), ("flag_sync", 0), ("flag_sync", 200), ("fused", 0)],
+             ("scale_step", 0.05), ("tau", 1e-3), ("theta", 5.0), ("fused", 0)],
     "farn": [("num_levels", 0), ("num_levels", 5), ("num_iters", 1), ("poly_sigma", 0.8), ("pyr_scale", 0.5), ("win_size", 13),
              ("poly_n", 5)],
 }
@@ -396,13 +395,15 @@ def test_set_refuses_bad_values_and_keeps_the_old_one(alg, variant):
             after = C.c_double()
             assert L.dfb_get_param(e._h, name.encode(), C.byref(after)) == _lib.DFB_OK
             assert after.value == before, (alg, name, v, after.value, before)
-    if alg == "farn":  # "use_tma" is a TV-L1 knob: a Farneback handle refuses it like any name it does not know
-        before = {n: e.get(n) for n in REFUSED["farn"]}
+    # names of removed engine knobs: a handle refuses them like any name it does not know
+    removed = ("use_tma",) if alg == "farn" else ("flag_sync", "prefetch", "serial_launches")
+    before = {n: e.get(n) for n in REFUSED[alg]}
+    for name in removed:
         for v in (0, 1):
-            assert L.dfb_set_param(e._h, b"use_tma", float(v)) == _lib.DFB_ERR_INVALID_ARG
-            assert L.dfb_last_error(e._h).decode() == "bad parameter use_tma"
-        assert L.dfb_get_param(e._h, b"use_tma", C.byref(C.c_double())) == _lib.DFB_ERR_INVALID_ARG
-        assert {n: e.get(n) for n in REFUSED["farn"]} == before
+            assert L.dfb_set_param(e._h, name.encode(), float(v)) == _lib.DFB_ERR_INVALID_ARG, (alg, name, v)
+            assert L.dfb_last_error(e._h).decode() == "bad parameter " + name, (alg, name, v)
+        assert L.dfb_get_param(e._h, name.encode(), C.byref(C.c_double())) == _lib.DFB_ERR_INVALID_ARG, (alg, name)
+    assert {n: e.get(n) for n in REFUSED[alg]} == before
     e.release()
     del _handles[(alg, variant, 64, 64)]
 

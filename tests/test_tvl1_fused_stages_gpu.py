@@ -82,8 +82,8 @@ SINGLE_TILE = [(16, 16), (17, 19), (33, 64), (64, 33), (100, 50), (127, 63), (12
 # below the 16-px level cut (tests/geometry_cases.py): one warp band holds the image (h < 4), the halo is taller than the
 # image, one four-pixel group holds column 0 and column w - 1 (w < 4); and thin strips
 SMALL = gc.STAGE_SMALL + gc.STAGE_STRIPS
-# (G, lanes, use_tma, flag_sync, check): G = 0 means every CTA the lanes leave; G = 1 puts every tile through one CTA
-CONFIGS = list(itertools.product([1, 3, 0], [1, 3], [1, 0], [1, 0], [1, 0]))
+# (G, lanes, use_tma, check): G = 0 means every CTA the lanes leave; G = 1 puts every tile through one CTA
+CONFIGS = list(itertools.product([1, 3, 0], [1, 3], [1, 0], [1, 0]))
 
 
 def _check(name, got, want):
@@ -136,18 +136,18 @@ def unfused_chunks(e, ins, kk, n, c=(L_T, TAUT, THETA)):
 
 def run_chunks(oracle, variant, w, h, kk, n, cfg, seed, tau=0.25, lam=0.15, theta=0.3):
     """the chunk stage with the handle's tau, lambda and theta set to these values (restored afterwards)"""
-    G, lanes, tma, flag, check = cfg
+    G, lanes, tma, check = cfg
     e = _engine(variant)
     cases = [chunk_inputs(w, h, seed + 97 * i) for i in range(lanes)]
     ins = [_stack([c[k] for c in cases]) for k in range(10)]
     keep = [e.get(k) for k in ("tau", "lambda", "theta")]
     try:
         e.set("tau", tau).set("lambda", lam).set("theta", theta)
-        got, errs = e.debug_run_kernel("tvl1_chunks", ins, 6, [kk, n, check, G, tma, flag, 1, lanes], all_scalars=True)
+        got, errs = e.debug_run_kernel("tvl1_chunks", ins, 6, [kk, n, check, G, tma, lanes], all_scalars=True)
     finally:
         e.set("tau", keep[0]).set("lambda", keep[1]).set("theta", keep[2])
     c = consts(tau, lam, theta)
-    tag = "%dx%d kk %d n %d G %d lanes %d tma %d flag %d check %d (l_t, taut, theta) %s" % (w, h, kk, n, G, lanes, tma, flag, check, c)
+    tag = "%dx%d kk %d n %d G %d lanes %d tma %d check %d (l_t, taut, theta) %s" % (w, h, kk, n, G, lanes, tma, check, c)
     for i, case in enumerate(cases):
         if variant == "strict":
             want, oerr, sabs = oracle_chunks(oracle.lib(), case, kk, n, c)
@@ -199,7 +199,7 @@ def test_one_step_within_float64_bounds(oracle, variant):
         lanes = 1 + 2 * (j % 2)
         cases = [chunk_inputs(w, h, 300 + 13 * j + i) for i in range(lanes)]
         ins = [_stack([c[k] for c in cases]) for k in range(10)]
-        got, errs = e.debug_run_kernel("tvl1_chunks", ins, 6, [1, 1, 1, 0, j % 2, 1, 1, lanes], all_scalars=True)
+        got, errs = e.debug_run_kernel("tvl1_chunks", ins, 6, [1, 1, 1, 0, j % 2, lanes], all_scalars=True)
         for i, c in enumerate(cases):
             tag = "%dx%d lane %d/%d" % (w, h, i, lanes)
             u1, u2 = (_split(got[k], lanes)[i] for k in (0, 1))

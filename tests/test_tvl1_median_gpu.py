@@ -84,11 +84,11 @@ def test_median_stage_equals_oracle(oracle, variant, lanes, k):
 
 
 # ---- strict build: the whole flow ----------------------------------------------------------------------------------------
-# ((h, w), k, interval, knobs): k 3 / 5, I 1 / 2 / 7 / 30 / 300, fused_k 1 / 3 / 8, TMA / LDG, flag / barrier sync
+# ((h, w), k, interval, knobs): k 3 / 5, I 1 / 2 / 7 / 30 / 300, fused_k 1 / 3 / 8, TMA / LDG
 # (a median every 1 or 2 iterations only on small frames: the reference's median is numpy)
 E2E = [((256, 256), 3, 30, {}), ((97, 131), 5, 1, {}), ((256, 340), 5, 30, {}), ((256, 340), 3, 7, {"fused_k": 3}),
-       ((97, 131), 3, 2, {"use_tma": 0}), ((256, 340), 5, 300, {"flag_sync": 0}), ((97, 131), 3, 1, {"fused_k": 1}),
-       ((97, 131), 5, 7, {"use_tma": 0, "flag_sync": 0}), ((97, 131), 5, 2, {"epsilon": 0.0, "iterations": 23, "fused_k": 3}),
+       ((97, 131), 3, 2, {"use_tma": 0}), ((256, 340), 5, 300, {}), ((97, 131), 3, 1, {"fused_k": 1}),
+       ((97, 131), 5, 7, {"use_tma": 0}), ((97, 131), 5, 2, {"epsilon": 0.0, "iterations": 23, "fused_k": 3}),
        ((360, 640), 5, 30, {}), ((360, 640), 3, 7, {"fused_k": 3}), ((1, 1), 3, 30, {}), ((16, 16), 5, 1, {}),
        ((17, 17), 3, 2, {"fused_k": 1}), ((1080, 7), 5, 30, {}), ((1080, 7), 3, 7, {"use_tma": 0})]
 
@@ -136,7 +136,7 @@ def test_strict_1080p_two_lanes_is_bit_exact(oracle):
 
 
 # ---- default build ----------------------------------------------------------------------------------------------------------
-KNOBS = [dict(fused_k=fk, use_tma=t, flag_sync=f) for fk in (8, 3, 1) for t in (1, 0) for f in (1, 0)] + [dict(fused=0)]
+KNOBS = [dict(fused_k=fk, use_tma=t) for fk in (8, 3, 1) for t in (1, 0)] + [dict(fused=0)]
 
 
 @pytest.mark.parametrize("k, interval", [(5, 7), (3, 30)])
@@ -146,7 +146,7 @@ def test_default_knobs_and_schedules_are_bit_identical(oracle, k, interval):
     e = _new(w, h, "default", median_filtering=k, median_interval=interval)
     ref = None
     for knobs in KNOBS:
-        for n, v in {**dict(fused=1, fused_k=8, use_tma=1, flag_sync=1), **knobs}.items():
+        for n, v in {**dict(fused=1, fused_k=8, use_tma=1), **knobs}.items():
             e.set(n, v)
         flow = e.calc(a, b)
         if ref is None:
