@@ -49,8 +49,11 @@ class DenseOpticalFlow:
     def set(self, name, value):
         """dfb_set_param: one algorithm parameter or engine knob (include/denseflow_b200.h lists them).  TV-L1 also takes
         "median_filtering" (0 or 1 = off [default], 3 or 5 = the window of a median of the flow between iterations) and
-        "median_interval" (>= 1, default 30: the median runs before iterations 0, I, 2I, ... of every warp).  A refused
-        value raises RuntimeError("bad parameter <name>") and leaves the parameter as it was.  Returns self."""
+        "median_interval" (>= 1, default 30: the median runs before iterations 0, I, 2I, ... of every warp).  Both algorithms
+        take "use_initial_flow" (0 [default] or 1: OpenCV's useInitialFlow / OPTFLOW_USE_INITIAL_FLOW): with 1, the flow
+        buffers of calc, calc_batch, calc_batch_device, calc_batch_planes and calc_batch_device_planes are read as each
+        pair's starting flow before they are overwritten, so they must be passed, and every other flow call is refused.  A
+        refused value raises RuntimeError("bad parameter <name>") and leaves the parameter as it was.  Returns self."""
         self._check(self._L.dfb_set_param(self._h, name.encode(), float(value)))
         return self
 
@@ -59,16 +62,23 @@ class DenseOpticalFlow:
         self._check(self._L.dfb_get_param(self._h, name.encode(), C.byref(v)))
         return v.value
 
+    def _reads_flow(self, buf):
+        """buf is None while use_initial_flow is set: the library refuses the call with its message (null flow buffer)"""
+        return buf is None and self.get("use_initial_flow") != 0
+
     # -- calc(I0, I1) -> flow (CV_32FC2), src/denseflow_gpu.cpp:327/:329 --
     def calc(self, a, b, flow=None, stream=None):
         """a, b: uint8 [H,W] numpy arrays (host path: upload, calc, download) or CUDA torch tensors
-        (device path: enqueued on `stream` / torch's current stream, asynchronous)."""
+        (device path: enqueued on `stream` / torch's current stream, asynchronous).  With use_initial_flow set, `flow`
+        ([H,W,2] float32, C-contiguous host array or CUDA tensor) is also the starting flow."""
         if isinstance(a, np.ndarray):
             a = np.ascontiguousarray(a, np.uint8)
             b = np.ascontiguousarray(b, np.uint8)
             if a.ndim != 2 or a.shape != b.shape:
                 raise RuntimeError("calc: frames must be two CV_8UC1 images of the same size")
             h, w = a.shape
+            if self._reads_flow(flow):
+                self._check(self._L.dfb_calc_host(self._h, a.ctypes.data, b.ctypes.data, w, h, None))
             if flow is None:
                 flow = np.empty((h, w, 2), np.float32)
             self._check(self._L.dfb_calc_host(self._h, a.ctypes.data, b.ctypes.data, w, h, flow.ctypes.data))
@@ -78,9 +88,12 @@ class DenseOpticalFlow:
                 or a.stride(1) != 1 or b.stride(1) != 1:
             raise RuntimeError("calc: frames must be two CV_8UC1 CUDA tensors of the same size with unit column stride")
         h, w = a.shape
+        s = stream if stream is not None else torch.cuda.current_stream(a.device).cuda_stream
+        if self._reads_flow(flow):
+            self._check(self._L.dfb_calc_device(self._h, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), w, h, None, w * 8,
+                                                C.c_void_p(s)))
         if flow is None:
             flow = torch.empty((h, w, 2), dtype=torch.float32, device=a.device)
-        s = stream if stream is not None else torch.cuda.current_stream(a.device).cuda_stream
         self._check(self._L.dfb_calc_device(self._h, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), w, h,
                                             flow.data_ptr(), flow.stride(0) * 4, C.c_void_p(s)))
         return flow
@@ -106,7 +119,8 @@ class DenseOpticalFlow:
     def calc_batch(self, frames, step=1, flows=None, bound=None):
         """frames: sequence of uint8 [H,W] host arrays (or one [N,H,W] array).  Returns M = max(N-|step|,0)
         flows [M,H,W,2] float32, or with bound=B the quantised (qx, qy) uint8 [M,H,W] planes
-        (convertFlowToImage, src/common.cpp:4-16, done on the GPU)."""
+        (convertFlowToImage, src/common.cpp:4-16, done on the GPU).  With use_initial_flow set, flows[j] is also pair j's
+        starting flow."""
         frames = self._gray_frames(frames)
         n = len(frames)
         if n == 0:
@@ -115,6 +129,8 @@ class DenseOpticalFlow:
         m = max(n - abs(step), 0)
         fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
         if bound is None:
+            if self._reads_flow(flows) and m > 0:
+                self._check(self._L.dfb_calc_batch_host(self._h, fp, n, step, w, h, None))
             if flows is None:
                 flows = np.empty((m, h, w, 2), np.float32)
             self._check_out(flows, (m, h, w, 2), np.float32, "flows")
@@ -143,13 +159,16 @@ class DenseOpticalFlow:
         return qx, qy
 
     def calc_batch_device(self, frames, step=1, flows=None, stream=None):
-        """frames: CUDA uint8 tensor [N,H,W] (contiguous); flows: CUDA float32 [M,H,W,2]."""
+        """frames: CUDA uint8 tensor [N,H,W] (contiguous); flows: CUDA float32 [M,H,W,2] (contiguous), with use_initial_flow
+        set also the pairs' starting flows."""
         import torch
         n, h, w = frames.shape
         m = max(n - abs(step), 0)
+        s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
+        if self._reads_flow(flows):
+            self._check(self._L.dfb_calc_batch_device(self._h, frames.data_ptr(), n, step, w, h, None, C.c_void_p(s)))
         if flows is None:
             flows = torch.empty((m, h, w, 2), dtype=torch.float32, device=frames.device)
-        s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
         self._check(self._L.dfb_calc_batch_device(self._h, frames.data_ptr(), n, step, w, h, flows.data_ptr(),
                                                   C.c_void_p(s)))
         return flows
@@ -163,26 +182,33 @@ class DenseOpticalFlow:
 
     def calc_batch_planes(self, frames, step=1, out=None):
         """calc_batch with the flow channels first: float32 [M,2,H,W], out[j,0] / out[j,1] bit for bit flows[j,...,0] /
-        flows[j,...,1].  The engines' merge epilogue writes the planes; out may be a caller (e.g. page-locked) array."""
+        flows[j,...,1].  The engines' merge epilogue writes the planes; out may be a caller (e.g. page-locked) array, with
+        use_initial_flow set also the pairs' starting flows."""
         frames = self._gray_frames(frames)
         n = len(frames)
         if n == 0:
             return np.empty((0, 2, 0, 0), np.float32)
         h, w = frames[0].shape
         m = max(n - abs(step), 0)
+        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
+        if self._reads_flow(out) and m > 0:
+            self._check(self._L.dfb_calc_batch_host_planes(self._h, fp, n, step, w, h, None, None))
         if out is None:
             out = np.empty((m, 2, h, w), np.float32)
         self._check_out(out, (m, 2, h, w), np.float32, "out")
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
         xp, yp = self._plane_ptrs(out, m)
         self._check(self._L.dfb_calc_batch_host_planes(self._h, fp, n, step, w, h, xp, yp))
         return out
 
     def calc_batch_device_planes(self, frames, step=1, planes=None, stream=None):
-        """frames: CUDA uint8 tensor [N,H,W] (contiguous); planes: CUDA float32 [M,2,H,W] (contiguous)."""
+        """frames: CUDA uint8 tensor [N,H,W] (contiguous); planes: CUDA float32 [M,2,H,W] (contiguous), with use_initial_flow
+        set also the pairs' starting flows."""
         import torch
         n, h, w = frames.shape
         m = max(n - abs(step), 0)
+        if self._reads_flow(planes):
+            s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
+            self._check(self._L.dfb_calc_batch_device_planes(self._h, frames.data_ptr(), n, step, w, h, None, C.c_void_p(s)))
         if planes is None:
             planes = torch.empty((m, 2, h, w), dtype=torch.float32, device=frames.device)
         if planes.dtype != torch.float32 or tuple(planes.shape) != (m, 2, h, w) or not planes.is_contiguous():

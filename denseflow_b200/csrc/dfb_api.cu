@@ -175,6 +175,23 @@ int check_size(dfb_handle *h, int w, int h_) {
     return DFB_OK;
 }
 
+// use_initial_flow = 1 on the handle: the calls with a float flow buffer read each pair's initial flow from it
+bool initial_flow(const dfb_handle *h) {
+    double v = 0;
+    return h->alg->get_param("use_initial_flow", &v) && v != 0;
+}
+// a missing flow buffer; with use_initial_flow set it is also the missing input
+int null_flow(dfb_handle *h, const std::string &what) {
+    return fail(h, DFB_ERR_INVALID_ARG, initial_flow(h) ? what + ": use_initial_flow is set, so the flow buffer must hold the initial flow" : what);
+}
+// the calls without a float flow buffer have no initial flow to read: refused before anything is enqueued
+int refuse_initial_flow(dfb_handle *h) {
+    if (!initial_flow(h)) return DFB_OK;
+    return fail(h, DFB_ERR_INVALID_ARG,
+                "use_initial_flow is set: only the calls that take a float flow buffer (dfb_calc_device / _host / _batch_host / _batch_device "
+                "and their _planes forms) read an initial flow; set it to 0 for this call");
+}
+
 // pinned staging buffers exist only for callers that pass pageable memory: allocated on first use
 uint8_t *stage_frame(dfb_handle *h, int r) {
     h->h_frame[r].allocate((size_t)h->max_w * h->max_h);
@@ -468,6 +485,8 @@ struct FlowOutput {
     std::function<void(int slot, int m)> pack;                  // optional: s_compute work on the solved group
     std::function<void(int j0, int m, int slot)> send;          // s_out: the group's outputs leave the slot
     std::function<void(int j0, int m, int slot)> finish;        // host, a group later: the results to the caller
+    // optional (use_initial_flow): s_compute copy of pair j's initial flow into output pair p, bound as the solve's start
+    std::function<void(FlowAlgorithm::PairJob &, int j, int p)> load;
 };
 
 // dfb_calc_host / dfb_calc_batch_host: pair j's float2 field to flows[j], straight into page-locked memory or through the
@@ -496,6 +515,18 @@ FlowOutput host_flow_output(dfb_handle *h, float *const *flows, int B, int w, in
                 std::memcpy(flows[j0 + i], h->h_flow[slot * B + i], bytes);
             }
     };
+    // the pair's staging buffer is free: the read-back of the group that last used this slot has been copied out (finish)
+    if (initial_flow(h))
+        o.load = [=](FlowAlgorithm::PairJob &pj, int j, int p) {
+            const float *src = flows[j];
+            if (!is_pinned_host(src)) src = static_cast<float *>(std::memcpy(stage_flow(h, p), src, bytes));
+            DFB_CUDA(cudaMemcpyAsync(field(p), src, bytes, cudaMemcpyHostToDevice, h->s_compute));
+            h->counters.h2d_bytes += bytes;
+            pj.init_x = field(p);
+            pj.init_y = field(p) + 1;
+            pj.init_pitch = (size_t)w * 2;
+            pj.init_step = 2;
+        };
     return o;
 }
 
@@ -571,6 +602,22 @@ FlowOutput planes_output(dfb_handle *h, const PlanesOut &po, int B, int w, int h
                 std::memcpy(po.y[j0 + i], h->h_flow[slot * B + i] + (size_t)w * hh, bytes);
             }
     };
+    if (initial_flow(h))  // as in host_flow_output
+        o.load = [=](FlowAlgorithm::PairJob &pj, int j, int p) {
+            const float *sx = po.x[j], *sy = po.y[j];
+            if (!direct(j)) {
+                float *st = stage_flow(h, p);
+                sx = static_cast<float *>(std::memcpy(st, sx, bytes));
+                sy = static_cast<float *>(std::memcpy(st + (size_t)w * hh, sy, bytes));
+            }
+            DFB_CUDA(cudaMemcpyAsync(plane(p, 0), sx, bytes, cudaMemcpyHostToDevice, h->s_compute));
+            DFB_CUDA(cudaMemcpyAsync(plane(p, 1), sy, bytes, cudaMemcpyHostToDevice, h->s_compute));
+            h->counters.h2d_bytes += 2 * bytes;
+            pj.init_x = plane(p, 0);
+            pj.init_y = plane(p, 1);
+            pj.init_pitch = (size_t)w;
+            pj.init_step = 1;
+        };
     return o;
 }
 
@@ -699,6 +746,7 @@ int flow_groups(dfb_handle *h, int n_frames, int step, int w, int hh, int B, con
         for (int i = 0; i < m; ++i) {
             jobs[i] = pair_job(j0 + i, step, nslots);
             o.bind(jobs[i], slot * B + i);
+            if (o.load) o.load(jobs[i], j0 + i, slot * B + i);
         }
         alg.solve_batch(jobs.data(), m, w, hh, h->s_compute);
         if (o.pack) o.pack(slot, m);
@@ -737,7 +785,7 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
                                      : (const void *)flows[j];
         const void *o1 = bound > 0 ? (const void *)qy[j] : planes ? (const void *)planes->y[j] : o0;
         if (!o0 || !o1 || host_pointer_kind(o0) < 0 || host_pointer_kind(o1) < 0)
-            return fail(h, DFB_ERR_INVALID_ARG, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
+            return null_flow(h, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
     }
     const int B = std::max(1, std::min(h->alg->max_concurrent_pairs(w, hh), dfb_handle::kMaxGroup));
     // output slots at the handle's maximum frame, so that calls of other sizes reuse them (a 1080p handle runs 7 pairs per
@@ -842,7 +890,8 @@ int dfb_get_param(const dfb_handle *h, const char *name, double *value) {
 int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8_t *b, size_t b_pitch, int width,
                     int height, float *flow_xy, size_t flow_pitch, void *stream) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (!a || !b || !flow_xy) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    if (!flow_xy) return null_flow(h, "null buffer");
+    if (!a || !b) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     if (int rc = check_size(h, width, height)) return rc;
     if (a_pitch < (size_t)width || b_pitch < (size_t)width || flow_pitch < (size_t)width * 8)
         return fail(h, DFB_ERR_INVALID_ARG, "pitch smaller than a row");
@@ -854,7 +903,14 @@ int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8
         h->alg->begin_batch();
         h->alg->prepare_frame(a, a_pitch, width, height, 0, s);
         h->alg->prepare_frame(b, b_pitch, width, height, 1, s);
-        h->alg->solve(0, 1, width, height, flow_xy, flow_pitch, s);
+        FlowAlgorithm::PairJob pj{0, 1, flow_xy, flow_pitch};
+        if (initial_flow(h)) {  // read on s before the solve writes the field
+            pj.init_x = flow_xy;
+            pj.init_y = flow_xy + 1;
+            pj.init_pitch = flow_pitch / sizeof(float);
+            pj.init_step = 2;
+        }
+        h->alg->solve_batch(&pj, 1, width, height, s);
         ++h->counters.pairs;
         return DFB_OK;
     });
@@ -862,7 +918,8 @@ int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8
 
 int dfb_calc_host(dfb_handle *h, const uint8_t *a, const uint8_t *b, int width, int height, float *flow_xy) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (!a || !b || !flow_xy) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    if (!flow_xy) return null_flow(h, "null buffer");
+    if (!a || !b) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     const uint8_t *frames[2] = {a, b};
     float *flows[1] = {flow_xy};
     return guarded(h, [&]() {
@@ -874,7 +931,7 @@ int dfb_calc_host(dfb_handle *h, const uint8_t *a, const uint8_t *b, int width, 
 int dfb_calc_batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                         float *const *flows) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (n_frames > std::abs(step) && !flows) return fail(h, DFB_ERR_INVALID_ARG, "flows is null");
+    if (n_frames > std::abs(step) && !flows) return null_flow(h, "flows is null");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         return batch_host(h, frames, n_frames, step, width, height, flows, 0, nullptr, nullptr);
@@ -884,6 +941,7 @@ int dfb_calc_batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frame
 int dfb_calc_batch_host_u8(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                            int bound, uint8_t *const *qx, uint8_t *const *qy) {
     if (!h) return DFB_ERR_INVALID_ARG;
+    if (int rc = refuse_initial_flow(h)) return rc;
     if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");  // check_param, src/denseflow_gpu.cpp:15-18
     if (n_frames > std::abs(step) && (!qx || !qy)) return fail(h, DFB_ERR_INVALID_ARG, "qx/qy is null");
     return guarded(h, [&]() {
@@ -895,7 +953,7 @@ int dfb_calc_batch_host_u8(dfb_handle *h, const uint8_t *const *frames, int n_fr
 int dfb_calc_batch_host_planes(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                                float *const *fx, float *const *fy) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (n_frames > std::abs(step) && (!fx || !fy)) return fail(h, DFB_ERR_INVALID_ARG, "fx/fy is null");
+    if (n_frames > std::abs(step) && (!fx || !fy)) return null_flow(h, "fx/fy is null");
     const PlanesOut planes{fx, fy};
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
@@ -917,7 +975,9 @@ int batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, i
     const int astep = std::abs(step);
     const int M = std::max(n_frames - astep, 0);
     if (M == 0) return DFB_OK;
-    if (!frames || !flows) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    if (!flows) return null_flow(h, "null buffer");
+    if (!frames) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
+    const bool init = initial_flow(h);
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -943,6 +1003,12 @@ int batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, i
                 } else {
                     jobs[i].flow_xy = out;
                     jobs[i].flow_pitch_bytes = (size_t)width * 8;
+                }
+                if (init) {  // the pair's output holds its initial flow: the solve reads it before writing the result
+                    jobs[i].init_x = out;
+                    jobs[i].init_y = planar ? out + fbytes : out + 1;
+                    jobs[i].init_pitch = planar ? (size_t)width : (size_t)width * 2;
+                    jobs[i].init_step = planar ? 1 : 2;
                 }
             }
             alg.solve_batch(jobs.data(), m, width, height, s);
@@ -1225,6 +1291,7 @@ int check_chain_args(dfb_handle *h, bool frames_null, int n_frames, int step, co
 // dfb_process_bgr_batch_host[_png]: the checks, then the chain with decoded BGR frames as its source
 int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh, const ChainOut &o) {
     if (!h) return DFB_ERR_INVALID_ARG;
+    if (int rc = refuse_initial_flow(h)) return rc;
     if (int rc = check_chain_args(h, !bgr, n_frames, step, o, dw, dh)) return rc;
     if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
@@ -1268,6 +1335,7 @@ int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, 
 // dfb_process_jpeg_batch_host[_png]: the checks, then the chain with JPEG files decoded on the device as its source
 int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh, const ChainOut &o) {
     if (!h) return DFB_ERR_INVALID_ARG;
+    if (int rc = refuse_initial_flow(h)) return rc;
     if (int rc = check_chain_args(h, !jpeg || !len, n_frames, step, o, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
@@ -1658,6 +1726,7 @@ int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitc
 int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height, uint8_t *const *png,
                             size_t capacity, size_t *len) {
     if (!h) return DFB_ERR_INVALID_ARG;
+    if (int rc = refuse_initial_flow(h)) return rc;
     if (n_frames > std::abs(step) && (!png || !len)) return fail(h, DFB_ERR_INVALID_ARG, "png / len is null");
     return guarded(h, [&]() {
         DFB_CUDA(cudaSetDevice(h->device));

@@ -115,6 +115,12 @@ class FlowAlgorithm {
         // payloads of an h5 file's flow_x / flow_y datasets, INSTEAD of the float2 field; flow_xy may then be null
         float *fx = nullptr, *fy = nullptr;
         size_t f_pitch = 0;
+        // init_x set (use_initial_flow): the solve starts from this flow instead of zero.  It is read before the pair's output
+        // is written, so it may be the same memory.  Pixel (x, y) of the x channel is init_x[y * init_pitch + x * init_step] and
+        // of the y channel init_y[...]: init_step 2 for a float2 field, 1 for two planes; init_pitch in floats.
+        const float *init_x = nullptr, *init_y = nullptr;
+        size_t init_pitch = 0;
+        int init_step = 1;
     };
     virtual int max_concurrent_pairs(int w, int h) { (void)w; (void)h; return 1; }
     // after a CUDA error: what the engine's own watchdogs recorded (empty if nothing)

@@ -317,7 +317,8 @@ constexpr int kMaxFarnBatch = 8;
 struct PairArgs {
     Plane5 R0, R1, M[2];
     Plane fx, fy;    // this level's flow
-    Plane pfx, pfy;  // previous (coarser) level's flow
+    Plane pfx, pfy;  // previous (coarser) level's flow; at the coarsest level with use_initial_flow, the initial flow
+    int pstep;       // floats between neighbouring pixels of pfx / pfy: 1, or 2 for an initial float2 field
     float *flow_xy;
     size_t flow_pitch_bytes;
     int bound;  // > 0: the merge writes the two quantised uint8 planes instead (PairJob)
@@ -543,7 +544,8 @@ __global__ void __launch_bounds__(256, kBoxMinBlocks) k_box_solve_update(const _
     }
 }
 
-// level start: flow = 0 at the coarsest level, else resize(prev) * (1/pyrScale) (B.2), both components, batched
+// level start: flow = 0 at the coarsest level, else resize(prev) * (1/pyrScale) (B.2), both components, batched.  With
+// use_initial_flow the coarsest level is resize(initial flow) * pyrScale^k the same way (first = 0, pfx / pfy the initial flow).
 __global__ void __launch_bounds__(256) k_flow_init(const __grid_constant__ FarnBatchArgs args, int first, float rfx, float rfy, float mul) {
     const PairArgs &a = args.p[blockIdx.z];
     const int dx = blockIdx.x * 32 + threadIdx.x, dy = blockIdx.y * 8 + threadIdx.y;
@@ -559,7 +561,7 @@ __global__ void __launch_bounds__(256) k_flow_init(const __grid_constant__ FarnB
     const int x1 = __float2int_rd(sx), y1 = __float2int_rd(sy);
     const int x2 = x1 + 1, y2 = y1 + 1;
     const size_t r1 = (size_t)min(y1, s1.h - 1) * s1.pitch, r2 = (size_t)min(y2, s1.h - 1) * s1.pitch;
-    const int x1r = min(x1, s1.w - 1), x2r = min(x2, s1.w - 1);
+    const int x1r = min(x1, s1.w - 1) * a.pstep, x2r = min(x2, s1.w - 1) * a.pstep;
     const float w11 = (x2 - sx) * (y2 - sy), w12 = (sx - x1) * (y2 - sy), w21 = (x2 - sx) * (sy - y1), w22 = (sx - x1) * (sy - y1);
     float o1 = 0.f, o2 = 0.f;
     o1 = o1 + s1.p[r1 + x1r] * w11;
@@ -601,6 +603,7 @@ struct FarnParams {
     int num_iters = 10;
     int poly_n = 5;
     double poly_sigma = 1.1;
+    int use_initial_flow = 0;  // 1: each pair starts from the flow its call passes in (PairJob::init_x; DESIGN §1)
 };
 
 inline int cv_round(double v) { return (int)std::nearbyint(v); }
@@ -732,6 +735,7 @@ class Farneback final : public FlowAlgorithm {
         else if (k == "pyr_scale") return v == 0.5;  // level geometry and the slot layout assume the default
         else if (k == "win_size" || k == "poly_n") return (k == "win_size" ? v == 13 : v == 5);  // compiled-in stencils
         else if (k == "time_kernels") { if (!is_flag(v)) return false; time_kernels_ = v != 0; }
+        else if (k == "use_initial_flow") { if (!is_flag(v)) return false; prm_.use_initial_flow = (int)v; }
         else return false;
         return true;
     }
@@ -743,6 +747,7 @@ class Farneback final : public FlowAlgorithm {
         else if (k == "poly_n") *v = prm_.poly_n;
         else if (k == "poly_sigma") *v = prm_.poly_sigma;
         else if (k == "time_kernels") *v = time_kernels_;
+        else if (k == "use_initial_flow") *v = prm_.use_initial_flow;
         else return false;
         return true;
     }
@@ -792,7 +797,7 @@ class Farneback final : public FlowAlgorithm {
             for (int l = 0; l < ls.n; ++l) {
                 const Level &L = ls.lv[l];
                 for (int i = 0; i < nb; ++i) args.p[i] = pair_args(jobs[j0 + i], lanes_[i], ls, l, cur);
-                launch_flow_init(args, nb, ls, l, s);
+                launch_flow_init(args, nb, ls, l, s, jobs[j0].init_x != nullptr);
                 int mb = 0;
                 launch_update_matrices(args, nb, L, mb, s);
                 pixel_iters += (uint64_t)L.w * L.h * prm_.num_iters * nb;
@@ -1087,10 +1092,16 @@ class Farneback final : public FlowAlgorithm {
         for (int b = 0; b < 2; ++b) a.M[b] = Plane5{{ln.M[b][0], ln.M[b][1], ln.M[b][2], ln.M[b][3], ln.M[b][4]}, L.w, L.h, L.pitch};
         a.fx = Plane{ln.fx[cur], L.w, L.h, L.pitch};
         a.fy = Plane{ln.fy[cur], L.w, L.h, L.pitch};
+        a.pstep = 1;
         if (l > 0) {
             const Level &Pv = ls.lv[l - 1];
             a.pfx = Plane{ln.fx[cur ^ 1], Pv.w, Pv.h, Pv.pitch};
             a.pfy = Plane{ln.fy[cur ^ 1], Pv.w, Pv.h, Pv.pitch};
+        } else if (job.init_x) {  // the initial flow at full resolution
+            const Level &F = ls.lv[ls.n - 1];
+            a.pfx = Plane{const_cast<float *>(job.init_x), F.w, F.h, (int)job.init_pitch};
+            a.pfy = Plane{const_cast<float *>(job.init_y), F.w, F.h, (int)job.init_pitch};
+            a.pstep = job.init_step;
         }
         a.flow_xy = job.flow_xy;
         a.flow_pitch_bytes = job.flow_pitch_bytes;
@@ -1104,15 +1115,22 @@ class Farneback final : public FlowAlgorithm {
         return a;
     }
     static dim3 grid8(const Level &L, int nb) { return dim3(ceil_div(L.w, 32), ceil_div(L.h, 8), nb); }
-    // level start: zero at the coarsest level, else the upsampled flow of level l - 1 times 1 / pyrScale
-    void launch_flow_init(const FarnBatchArgs &args, int nb, const LevelSet &ls, int l, cudaStream_t s) {
+    // level start: zero at the coarsest level, else the upsampled flow of level l - 1 times 1 / pyrScale.  init (every pair of
+    // the launch has an initial flow in pfx / pfy): the coarsest level is the initial flow resized to it, times pyrScale^k.
+    void launch_flow_init(const FarnBatchArgs &args, int nb, const LevelSet &ls, int l, cudaStream_t s, bool init = false) {
         const Level &L = ls.lv[l];
-        float rfx = 1.f, rfy = 1.f;
-        if (l > 0) {
-            rfx = (float)(1.0 / ((double)L.w / (double)ls.lv[l - 1].w));
-            rfy = (float)(1.0 / ((double)L.h / (double)ls.lv[l - 1].h));
+        float rfx = 1.f, rfy = 1.f, mul = (float)(1.0 / prm_.pyr_scale);
+        if (l > 0 || init) {
+            const Level &S = l > 0 ? ls.lv[l - 1] : ls.lv[ls.n - 1];
+            rfx = (float)(1.0 / ((double)L.w / (double)S.w));
+            rfy = (float)(1.0 / ((double)L.h / (double)S.h));
         }
-        k_flow_init<<<grid8(L, nb), dim3(32, 8), 0, s>>>(args, l == 0, rfx, rfy, (float)(1.0 / prm_.pyr_scale));
+        if (l == 0 && init) {
+            double scale = 1.0;
+            for (int i = 0; i < ls.n - 1; ++i) scale *= prm_.pyr_scale;  // level k = n - 1 of B.1
+            mul = (float)scale;
+        }
+        k_flow_init<<<grid8(L, nb), dim3(32, 8), 0, s>>>(args, l == 0 && !init, rfx, rfy, mul);
         DFB_KERNEL_CHECK();
         ++launches;
     }

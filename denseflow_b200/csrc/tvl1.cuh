@@ -56,6 +56,16 @@ void launch_u8_to_f32_batch(const FramePtrs &fp, int n, size_t src_pitch_bytes, 
 // level (src_off, sw, sh, sp) -> level (dst_off, dw, dh, dp) of every frame's slot
 void launch_resize_linear_batch(const FramePtrs &fp, int n, size_t src_off, int sw, int sh, int sp, size_t dst_off, int dw, int dh, int dp, float fx,
                                 float fy, cudaStream_t s);
+// use_initial_flow: pair i's initial field (x at x[i][y * pitch[i] + x * step[i]], y likewise) -> its lane's level-0 u1 / u2
+// planes (row pitch u_pitch), for several pairs of one size at once (blockIdx.z = pair)
+constexpr int kMaxInitFlows = 16;
+struct InitFlows {
+    const float *x[kMaxInitFlows], *y[kMaxInitFlows];
+    size_t pitch[kMaxInitFlows];
+    int step[kMaxInitFlows];
+    float *u1[kMaxInitFlows], *u2[kMaxInitFlows];
+};
+void launch_split_initial_flow(const InitFlows &f, int n, int w, int h, int u_pitch, cudaStream_t s);
 void launch_centered_gradient(Plane src, Plane dx, Plane dy, cudaStream_t s);
 void launch_warp_backward(Plane I0, Plane I1, Plane I1x, Plane I1y, Plane u1, Plane u2, Plane I1wx, Plane I1wy,
                           Plane grad, Plane rho_c, cudaStream_t s);

@@ -40,6 +40,7 @@ struct Tvl1Params {
     int lanes = 0;  // pairs solved side by side per fused launch; 0 = choose from the tile counts
     int median_filtering = 0;  // 3 or 5: the window of the median of u1, u2 between iterations (DESIGN §4.3); 0 or 1: off
     int median_interval = 30;  // the median runs before every iteration n of a warp with n % median_interval == 0
+    int use_initial_flow = 0;  // 1: each pair starts from the flow its call passes in (PairJob::init_x; DESIGN §1)
     int median_k() const { return median_filtering > 1 ? median_filtering : 0; }
 };
 
@@ -89,6 +90,7 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "lanes") { if (!whole_in(v, 0, kFusedMaxLanes)) return false; prm_.lanes = (int)v; }
         else if (k == "median_filtering") { if (!(v == 0 || v == 1 || v == 3 || v == 5)) return false; prm_.median_filtering = (int)v; }
         else if (k == "median_interval") { if (!whole_in(v, 1, INT_MAX)) return false; prm_.median_interval = (int)v; }
+        else if (k == "use_initial_flow") { if (!is_flag(v)) return false; prm_.use_initial_flow = (int)v; }
         else return false;
         return true;
     }
@@ -108,6 +110,7 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "lanes") *v = prm_.lanes;
         else if (k == "median_filtering") *v = prm_.median_filtering;
         else if (k == "median_interval") *v = prm_.median_interval;
+        else if (k == "use_initial_flow") *v = prm_.use_initial_flow;
         else return false;
         return true;
     }
@@ -235,8 +238,10 @@ class Tvl1 final : public FlowAlgorithm {
             for (int i = 0; i < count; ++i) {
                 float *flow = jobs[i].flow_xy;
                 size_t pitch = jobs[i].flow_pitch_bytes;
+                const bool init = jobs[i].init_x != nullptr;
+                if (init) load_initial_flow(jobs + i, 1, lv, n, s);
                 if (jobs[i].fx) {  // the merge writes the planes straight from u1 / u2
-                    solve_unfused(jobs[i].slot_a, jobs[i].slot_b, lv, n, nullptr, 0, s, jobs[i].fx, jobs[i].fy, jobs[i].f_pitch);
+                    solve_unfused(jobs[i].slot_a, jobs[i].slot_b, lv, n, nullptr, 0, s, jobs[i].fx, jobs[i].fy, jobs[i].f_pitch, init);
                     continue;
                 }
                 if (!flow) {  // quantised output only: the float2 field lives in an engine-owned scratch plane
@@ -244,7 +249,7 @@ class Tvl1 final : public FlowAlgorithm {
                     flow = unfused_scratch_;
                     pitch = (size_t)w * 2 * sizeof(float);
                 }
-                solve_unfused(jobs[i].slot_a, jobs[i].slot_b, lv, n, flow, pitch, s);
+                solve_unfused(jobs[i].slot_a, jobs[i].slot_b, lv, n, flow, pitch, s, nullptr, nullptr, 0, init);
                 if (jobs[i].bound > 0) {  // the reference's structure: a separate pass over the finished field
                     launch_quantise(flow, pitch, lv[0].w, lv[0].h, jobs[i].bound, jobs[i].qx, jobs[i].qy, jobs[i].q_pitch, s);
                     ++launches;
@@ -573,10 +578,44 @@ class Tvl1 final : public FlowAlgorithm {
 
     Plane work(float *p, const LevelGeom &g) const { return Plane{p, g.w, g.h, g.pitch}; }
 
+    // use_initial_flow: the initial fields of the pairs jobs[i] that carry one (PairJob::init_x) into lane i's flow pyramid
+    // u1pyr[0] / u2pyr[0], enqueued before the solve.  Level 0 is the field as given; level s is resize_linear of level s - 1
+    // with the frame pyramid's taps (prepare_frame), times float(scale_step) (DESIGN §1).
+    void load_initial_flow(const PairJob *jobs, int count, const LevelGeom *lv, int n, cudaStream_t s) {
+        InitFlows f{};
+        int m = 0;
+        auto flush = [&]() {
+            if (m) launch_split_initial_flow(f, m, lv[0].w, lv[0].h, lv[0].pitch, s);
+            launches += m ? 1 : 0;
+            m = 0;
+        };
+        for (int i = 0; i < count; ++i) {
+            if (!jobs[i].init_x) continue;
+            f.x[m] = jobs[i].init_x;
+            f.y[m] = jobs[i].init_y;
+            f.pitch[m] = jobs[i].init_pitch;
+            f.step[m] = jobs[i].init_step;
+            f.u1[m] = lanes_[i].u1pyr[0];  // level 0 starts the pyramid
+            f.u2[m] = lanes_[i].u2pyr[0];
+            if (++m == kMaxInitFlows) flush();
+        }
+        flush();
+        const float finv = (float)(1.0 / prm_.scale_step), mul = (float)prm_.scale_step;
+        for (int i = 0; i < count; ++i) {
+            if (!jobs[i].init_x) continue;
+            for (int l = 1; l < n; ++l) {
+                launch_resize_linear(level_plane(lanes_[i].u1pyr[0], lv, l - 1), level_plane(lanes_[i].u1pyr[0], lv, l), finv, finv, mul, s);
+                launch_resize_linear(level_plane(lanes_[i].u2pyr[0], lv, l - 1), level_plane(lanes_[i].u2pyr[0], lv, l), finv, finv, mul, s);
+                launches += 2;
+            }
+        }
+    }
+
     // ---- fused = 0: reference launch structure, A.4 state machine on the host ------------------
-    // fx set: the merge writes the two float planes fx / fy (PairJob) instead of the float2 field, and flow_xy may be null
+    // fx set: the merge writes the two float planes fx / fy (PairJob) instead of the float2 field, and flow_xy may be null.
+    // init: lane 0's flow pyramid holds the initial flow (load_initial_flow), the coarsest level starts from it.
     void solve_unfused(int slot_a, int slot_b, const LevelGeom *lv, int n, float *flow_xy, size_t flow_pitch_bytes,
-                       cudaStream_t s, float *fx = nullptr, float *fy = nullptr, size_t f_pitch = 0) {
+                       cudaStream_t s, float *fx = nullptr, float *fy = nullptr, size_t f_pitch = 0, bool init = false) {
         const Tvl1Consts c{(float)(prm_.lambda * prm_.theta), (float)(prm_.tau / prm_.theta), (float)prm_.theta};
         std::memset(last_iters_, 0, sizeof(last_iters_));
         Lane &wk = lanes_[0];
@@ -588,7 +627,7 @@ class Tvl1 final : public FlowAlgorithm {
             const Plane I1x = work(wk.I1x, g), I1y = work(wk.I1y, g), I1wx = work(wk.I1wx, g), I1wy = work(wk.I1wy, g);
             const Plane grad = work(wk.grad, g), rho_c = work(wk.rho_c, g);
             const Plane p11 = work(wk.p[0][0], g), p12 = work(wk.p[0][1], g), p21 = work(wk.p[0][2], g), p22 = work(wk.p[0][3], g);
-            if (l == n - 1) {  // useInitialFlow = false
+            if (l == n - 1 && !init) {  // useInitialFlow = false
                 launch_fill(u1, 0.f, s);
                 launch_fill(u2, 0.f, s);
                 launches += 2;
@@ -682,6 +721,7 @@ class Tvl1 final : public FlowAlgorithm {
         job.use_tma = prm_.use_tma;
         job.median_k = prm_.median_k();
         job.median_interval = prm_.median_interval;
+        job.init_flow = pj.init_x != nullptr;
         if (prm_.use_tma) ensure_tensor_maps(wk, lv, n);
         job.tmaps = wk.tmaps;
         job.c = Tvl1Consts{(float)(prm_.lambda * prm_.theta), (float)(prm_.tau / prm_.theta), (float)prm_.theta};
@@ -744,6 +784,7 @@ class Tvl1 final : public FlowAlgorithm {
             fill_job(host_jobs[i], lanes_[i], jobs[i], lv, n);
             host_jobs[i].iters_log = pair_log_dev_ + (size_t)next_log_slot() * kLogInts;
         }
+        load_initial_flow(jobs, count, lv, n, s);
         // one CTA per SM at most: the tile counts of the largest level bound the useful group size
         const int hx = 4, hy = 1;
         const int max_tiles = fused_tiles_along(lv[0].w, kFusedTileW, hx) * fused_tiles_along(lv[0].h, kFusedTileH, hy);

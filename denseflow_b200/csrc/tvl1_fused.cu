@@ -132,18 +132,18 @@ __device__ __forceinline__ void grid_barrier(unsigned *counter, unsigned &epoch,
 }
 
 // ---- pixel-parallel phases (grid-stride over the level) --------------------------------------
-__device__ __forceinline__ void phase_level_start(const int G, const int bid, const FusedJob &job, const FusedLevel &L, bool coarsest) {
+__device__ __forceinline__ void phase_level_start(const int G, const int bid, const FusedJob &job, const FusedLevel &L, bool zero_u) {
     const int W = L.w, H = L.h, P = L.pitch;
     const int total = H * (P >> 2);
     for (int i = bid * kThreads + threadIdx.x; i < total; i += G * kThreads) {
         const int y = i / (P >> 2), x0 = (i - y * (P >> 2)) << 2;
         const size_t o = (size_t)y * P + x0;
-        // A.2 step 2: p = 0 once per scale; A.2: u = 0 at the coarsest scale
+        // A.2 step 2: p = 0 once per scale; A.2: u = 0 at the coarsest scale (zero_u)
         st4(job.p[0][0] + o, zero4());
         st4(job.p[0][1] + o, zero4());
         st4(job.p[0][2] + o, zero4());
         st4(job.p[0][3] + o, zero4());
-        if (coarsest) {
+        if (zero_u) {
             st4(L.u1[0] + o, zero4());
             st4(L.u2[0] + o, zero4());
         }
@@ -815,7 +815,8 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair(const _
     for (int s = job.nscales - 1; s >= 0; --s) {
         const FusedLevel &L = job.lv[s];
         cur = 0;  // level start: u[0] holds the upsampled (or zero) flow, p[0] is zeroed
-        phase_level_start(G, bid, job, L, s == job.nscales - 1);
+        // with init_flow the coarsest level's u[0] already holds the initial flow's level (use_initial_flow): it is not zeroed
+        phase_level_start(G, bid, job, L, s == job.nscales - 1 && !job.init_flow);
         prof.mark(0);
         grid_barrier(bar, epoch, G, job.ctl);
         prof.mark(3);

@@ -53,6 +53,7 @@ struct FusedJob {
     // bound > 0: emit the two quantised uint8 planes instead of the float2 field (PairJob)
     int bound;
     int median_interval;  // see median_k
+    int init_flow;  // 1: the coarsest level starts from the flow already in its u1[0] / u2[0] (use_initial_flow) instead of 0
     uint8_t *qx, *qy;
     size_t q_pitch;
     // fx non-null: emit u1 / u2 as two float planes instead of the float2 field (PairJob)
@@ -99,7 +100,7 @@ int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s);
 
 // Test hook: one phase of k_tvl1_pair (its own device functions) on up to kFusedParamLanes lanes in one cooperative launch.
 enum FusedStage : int {
-    kFusedStageLevelStart,  // phase_level_start at level `level` (coarsest: zero u too)
+    kFusedStageLevelStart,  // phase_level_start at level `level` (coarsest: zero u too, unless the job's init_flow is set)
     kFusedStageWarp,        // phase_warp at level `level` from u[0]
     kFusedStageGq,          // grad -> tvl1_gq_from_grad(grad) over the level's plane
     kFusedStageChunks,      // n chunks of kk iterations at level `level` from state [0], every one checking when `check`

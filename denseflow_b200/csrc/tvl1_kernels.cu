@@ -95,6 +95,16 @@ __global__ void k_resize_linear_batch(const __grid_constant__ FramePtrs fp, size
     fp.base[blockIdx.z][dst_off + (size_t)dy * dp + dx] = out * 1.0f;
 }
 
+__global__ void k_split_initial_flow(const __grid_constant__ InitFlows f, int w, int h, int u_pitch) {
+    const int x = blockIdx.x * BX + threadIdx.x;
+    const int y = blockIdx.y * BY + threadIdx.y;
+    const int z = blockIdx.z;
+    if (x >= w || y >= h) return;
+    const size_t s = (size_t)y * f.pitch[z] + (size_t)x * f.step[z], d = (size_t)y * u_pitch + x;
+    f.u1[z][d] = f.x[z][s];
+    f.u2[z][d] = f.y[z][s];
+}
+
 // A.2 step 1: half central differences, index-clamped.
 __global__ void k_centered_gradient(Plane src, Plane gx, Plane gy) {
     const int x = blockIdx.x * BX + threadIdx.x;
@@ -281,6 +291,11 @@ void launch_resize_linear_batch(const FramePtrs &fp, int n, size_t src_off, int 
 }
 void launch_resize_linear(Plane src, Plane dst, float fx, float fy, float post_mul, cudaStream_t s) {
     k_resize_linear<<<grid2d(dst.w, dst.h), dim3(BX, BY), 0, s>>>(src, dst, fx, fy, post_mul);
+    DFB_KERNEL_CHECK();
+}
+void launch_split_initial_flow(const InitFlows &f, int n, int w, int h, int u_pitch, cudaStream_t s) {
+    const dim3 g = grid2d(w, h);
+    k_split_initial_flow<<<dim3(g.x, g.y, n), dim3(BX, BY), 0, s>>>(f, w, h, u_pitch);
     DFB_KERNEL_CHECK();
 }
 void launch_centered_gradient(Plane src, Plane dx, Plane dy, cudaStream_t s) {

@@ -73,6 +73,14 @@ const char *dfb_last_error(const dfb_handle *h);
  * combination of the engine knobs produces bit-identical flows.  Counts take whole numbers only, and on/off knobs 0 or 1.
  * A refused value (NaN, an infinity, a fraction or a value out of range) returns DFB_ERR_INVALID_ARG with "bad parameter
  * <name>" and leaves the parameter unchanged.
+ * Both algorithms: "use_initial_flow" (0 [default] or 1; OpenCV's setUseInitialFlow(true) / OPTFLOW_USE_INITIAL_FLOW).  With
+ * 1, the calls that take a float flow buffer (dfb_calc_device, dfb_calc_host, dfb_calc_batch_host, dfb_calc_batch_device and
+ * the two _planes calls) read each pair's flow buffer as its initial flow before overwriting it.  TV-L1: level 0 of the flow
+ * pyramid is that flow, level s the resize of level s - 1 with the frame pyramid's factors, times (float)scale_step, and the
+ * coarsest level starts from it instead of 0.  Farneback: the coarsest level starts from the initial flow resized to it
+ * (explicit size, CUDA convention) times (float)pyrScale^k instead of 0.  A null flow buffer, and every other flow call
+ * (_u8, _png, the dfb_process_* chains), return DFB_ERR_INVALID_ARG with a message naming use_initial_flow before anything
+ * is enqueued; the handle stays usable.  The list runner opens its own handles and never reads an initial flow.
  * Both algorithms: "jpeg_exact" (0 [default] = JPEG files through nvJPEG; 1 = every JPEG this handle writes is exactly the
  * file cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality]) writes with OpenCV's other defaults, libjpeg-turbo 3.x:
  * baseline, standard Huffman tables, islow DCT, gray or YCbCr 4:2:0, no restart markers).  It covers
@@ -90,6 +98,7 @@ int dfb_get_param(const dfb_handle *h, const char *name, double *value);
  *   flow_xy   : CV_32FC2 (u, v interleaved) in device memory, row pitch in bytes; u = x displacement
  *   stream    : cudaStream_t the work is enqueued on (the reference's DenseFlow::stream, include/dense_flow.h:33)
  * Asynchronous w.r.t. the host apart from the convergence read-back of the non-fused engine.
+ * use_initial_flow = 1: flow_xy also holds the initial flow, read on `stream` before the result overwrites it.
  */
 int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8_t *b, size_t b_pitch, int width,
                     int height, float *flow_xy, size_t flow_pitch, void *stream);
@@ -98,6 +107,7 @@ int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8
  * Compute, host buffers: upload a and b, calc, download the flow — the three statements
  * src/denseflow_gpu.cpp:317-318, :327/:329, :339 as one call.  Buffers are dense (pitch = width) and may be
  * pageable; the engine stages through its own pinned ring.  Blocks until flow_xy is complete.
+ * use_initial_flow = 1: flow_xy also holds the initial flow, uploaded through the same staging.
  */
 int dfb_calc_host(dfb_handle *h, const uint8_t *a, const uint8_t *b, int width, int height, float *flow_xy);
 
@@ -106,7 +116,8 @@ int dfb_calc_host(dfb_handle *h, const uint8_t *a, const uint8_t *b, int width, 
  * M = max(N - |s|, 0) flows with pair (a, b) = (i, i+s) for s > 0 and (i-s, i) for s < 0 (:315-316).
  * Each frame is uploaded and pyramided once (the reference does both twice), and copies overlap compute.
  *   frames[n_frames] : host pointers, dense width*height uint8
- *   flows[M]         : host pointers, dense width*height*2 float (CV_32FC2)
+ *   flows[M]         : host pointers, dense width*height*2 float (CV_32FC2); with use_initial_flow = 1 flows[j] also holds
+ *                      pair j's initial flow
  */
 int dfb_calc_batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                         float *const *flows);
@@ -116,12 +127,14 @@ int dfb_calc_batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frame
  * back (SURVEY §8 f1): fuses convertFlowToImage (src/common.cpp:4-16, via encodeFlowMap :48-64 with
  * lowerBound = -bound, higherBound = +bound) into the epilogue.  Bit-exact to the CAST macro.
  *   qx[M], qy[M] : host pointers, dense width*height uint8
+ * Refused while use_initial_flow = 1 (no float flow buffer to read it from).
  */
 int dfb_calc_batch_host_u8(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                            int bound, uint8_t *const *qx, uint8_t *const *qy);
 
 /* Device-resident batch: frames is one device allocation [n_frames][height][width] uint8 (dense),
- * flows one device allocation [M][height][width][2] float.  Enqueued on `stream`. */
+ * flows one device allocation [M][height][width][2] float.  Enqueued on `stream`.  With use_initial_flow = 1 pair j's
+ * field in flows also holds its initial flow. */
 int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, int width, int height,
                           float *flows, void *stream);
 
@@ -131,6 +144,7 @@ int dfb_calc_batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, in
  * writes u1 and u2 as dense planes, so the values are bit for bit the x and y channels of dfb_calc_batch_host's fields.
  *   fx[M], fy[M] : host pointers, dense width*height float each (page-locked ones take a direct DMA)
  *   planes       : one device allocation [M][2][height][width] float (pair j's x plane, then its y plane); enqueued on `stream`
+ * With use_initial_flow = 1 the two planes of pair j also hold its initial flow.
  */
 int dfb_calc_batch_host_planes(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                                float *const *fx, float *const *fy);
@@ -272,6 +286,7 @@ int dfb_get_tvl1_pair_stats(dfb_handle *h, int pair_index, dfb_tvl1_stats *out);
  * the size get_new_size chose (src/denseflow_gpu.cpp:44-80), or 0/0 for no resize.  For each of the
  * M = max(n_frames - |step|, 0) pairs the two JPEG bitstreams are written to jpg_x[i] / jpg_y[i] (host buffers of
  * `capacity` bytes each, dfb_jpeg_max_bytes(dst) is enough) and their lengths to len_x[i] / len_y[i].
+ * Refused while use_initial_flow = 1, as are the other dfb_process_* chains.
  */
 int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int src_width, int src_height,
                                int dst_width, int dst_height, int bound, int jpeg_quality, uint8_t *const *jpg_x,
@@ -348,6 +363,7 @@ int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitc
  * png[j] (host buffers of `capacity` bytes each, dfb_png_max_bytes is always enough) receives exactly what
  * writeFlowImagesPng writes for pair j, len[j] its length.  Flow and packing, the encodes and the read-back of successive
  * groups of pairs overlap; the host synchronises once per group.  Blocks until every file is on the host.
+ * Refused while use_initial_flow = 1, as are all the dfb_process_* chains.
  */
 int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                             uint8_t *const *png, size_t capacity, size_t *len);

@@ -1,0 +1,241 @@
+"""`use_initial_flow` (DESIGN §1) on the GPU, in the default and strict builds.
+
+* A zero initial flow gives the cold start's bits and iteration logs: both engines, TV-L1 fused and unfused, 1, 3 and
+  auto lanes, median filtering on and off.
+* TV-L1 strict build: from a smooth random field, a field past `bound` and the oracle's own cold flow, flows and
+  per-(scale, warp) iteration logs equal the restatement over the C oracle's building blocks (tests/initial_flow_ref.py)
+  bit for bit, fused and unfused; the default build is within 0.01 px.  Farneback is held to its restatement within the
+  tolerances of tests/test_farneback_gpu.py.
+* Host batch = per-pair calls, device batch = host batch, planes = the float2 field; pageable and page-locked host buffers
+  and a non-default stream.
+* Every call without a float flow buffer, and a missing buffer, is refused with a message naming the parameter, launches
+  nothing and leaves the handle computing correct flows; set back to 0 the handle starts cold again; the parameter takes
+  0 and 1 only."""
+import numpy as np
+import pytest
+
+import initial_flow_ref as R
+import tvl1_pin as pin
+from denseflow_b200 import synth
+from test_initial_flow_cpu import smooth_field
+
+pytestmark = pytest.mark.gpu
+VARIANTS = ["strict", "default"]
+AEE_TOL = 0.01  # px, BASELINE.json north_star
+H, W = 97, 131
+SMALL = dict(nscales=3, warps=3, iterations=60)  # keeps the oracle's runs short
+# amplitude of the start field past the quantiser's default bound (20 px): up to 24 px here.  With twice that on this
+# 131 x 97 pair most warps sample outside the frame and the default build's approximate arithmetic moves the result by
+# 0.012 px AEE (measured on an H100 80GB HBM3 at 700 W), while the strict build stays bit-exact.
+PAST_BOUND_AMP = 30.0
+
+
+def _bits_equal(got, want, what):
+    got, want = np.ascontiguousarray(got, np.float32), np.ascontiguousarray(want, np.float32)
+    bad = got.view(np.int32) != want.view(np.int32)
+    assert not bad.any(), "%s: %d of %d differ, first at %s" % (what, bad.sum(), bad.size, tuple(np.argwhere(bad)[0]))
+
+
+def _new(alg, w, h, variant="default", **params):
+    import denseflow_b200 as d
+    e = d.create(alg, 0, w, h, variant)
+    for k, v in params.items():
+        e.set(k, v)
+    return e
+
+
+def _logs(e, m):
+    return [e.tvl1_pair_stats(j).copy() for j in range(m)]
+
+
+# ---- a zero start is the cold start --------------------------------------------------------------------------------------
+TVL1_CONFIGS = [dict(fused=f, lanes=l, median_filtering=mf) for f in (1, 0) for l in ((1, 3, 0) if f else (0,)) for mf in (0, 3)]
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("cfg", TVL1_CONFIGS, ids=["fused%d-lanes%d-median%d" % (c["fused"], c["lanes"], c["median_filtering"])
+                                                   for c in TVL1_CONFIGS])
+def test_tvl1_zero_start_is_the_cold_start(variant, cfg):
+    fr = synth.stream(H, W, 5, seed=2)
+    cold = _new("tvl1", W, H, variant, **cfg)
+    want = cold.calc_batch(list(fr), step=1)
+    want_logs = _logs(cold, 4)
+    warm = _new("tvl1", W, H, variant, use_initial_flow=1, **cfg)
+    got = warm.calc_batch(list(fr), step=1, flows=np.zeros((4, H, W, 2), np.float32))
+    _bits_equal(got, want, "zero start %s" % cfg)
+    for j, (g, w) in enumerate(zip(_logs(warm, 4), want_logs)):
+        assert np.array_equal(g, w), (j, g, w)
+    one = warm.calc(fr[0], fr[1], flow=np.zeros((H, W, 2), np.float32))
+    _bits_equal(one, want[0], "single pair")
+    cold.release()
+    warm.release()
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
+def test_farneback_zero_start_is_the_cold_start(variant):
+    fr = synth.stream(H, W, 5, seed=2)
+    cold = _new("farn", W, H, variant)
+    want = cold.calc_batch(list(fr), step=1)
+    warm = _new("farn", W, H, variant, use_initial_flow=1)
+    _bits_equal(warm.calc_batch(list(fr), step=1, flows=np.zeros((4, H, W, 2), np.float32)), want, "farn zero start")
+    _bits_equal(warm.calc(fr[0], fr[1], flow=np.zeros((H, W, 2), np.float32)), want[0], "farn single pair")
+    cold.release()
+    warm.release()
+
+
+# ---- against the restatements ----------------------------------------------------------------------------------------------
+_REF = {}
+
+
+def _reference(median):
+    """{start: (initial flow, restatement's (flow, log, checks))} of the test pair, computed once per median setting"""
+    if median not in _REF:
+        a, b, _ = synth.pair(H, W, 7)
+        kw = dict(SMALL, median_filtering=median, median_interval=7)
+        starts = {"smooth": smooth_field(H, W, 1), "past_bound": smooth_field(H, W, 2, amp=PAST_BOUND_AMP),
+                  "cold_flow": R.tvl1_calc(a, b, None, **kw)[0]}
+        _REF[median] = {n: (init, R.tvl1_calc(a, b, init, **kw)) for n, init in starts.items()}
+    return _REF[median]
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("fused", [1, 0])
+@pytest.mark.parametrize("median", [0, 5])
+def test_tvl1_matches_the_restatement(oracle, variant, fused, median):
+    a, b, _ = synth.pair(H, W, 7)
+    kw = dict(SMALL, median_filtering=median, median_interval=7)
+    e = _new("tvl1", W, H, variant, use_initial_flow=1, fused=fused, **kw)
+    notes = []
+    for name, (init, out) in _reference(median).items():
+        flow = e.calc(a, b, flow=init.copy())
+        if variant == "strict":
+            notes.append(pin.check(oracle, a, b, flow, e.tvl1_stats()[0], "%s fused %d median %d" % (name, fused, median), oracle_out=out))
+        else:
+            aee = synth.aee(flow, out[0])
+            print("default build from %s, fused %d, median %d: AEE vs restatement %.3g px" % (name, fused, median, aee))
+            assert aee <= AEE_TOL, (name, aee)
+    e.release()
+    pin.finish(notes)
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("num_levels", [0, 5])
+def test_farneback_matches_the_restatement(oracle, variant, num_levels):
+    a, b, _ = synth.pair(H, W, 7)
+    e = _new("farn", W, H, variant, use_initial_flow=1, num_levels=num_levels)
+    for init in (smooth_field(H, W, 3, amp=6.0), R.farn_calc(a, b, None, oracle.farn_params(num_levels=num_levels))):
+        ref = R.farn_calc(a, b, init, oracle.farn_params(num_levels=num_levels))
+        aee = synth.aee(e.calc(a, b, flow=init.copy()), ref)
+        assert aee <= (1e-4 if variant == "strict" else AEE_TOL), aee
+    e.release()
+
+
+# ---- every entry point ---------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("alg", ["tvl1", "farn"])
+@pytest.mark.parametrize("variant", VARIANTS)
+def test_entry_points_agree(alg, variant):
+    import torch
+    fr = synth.stream(H, W, 8, seed=5)
+    m = 7
+    inits = np.stack([smooth_field(H, W, 10 + j, amp=3.0) for j in range(m)])
+    e = _new(alg, W, H, variant, use_initial_flow=1)
+    host = e.calc_batch(list(fr), step=1, flows=inits.copy())
+    for j in range(m):
+        _bits_equal(host[j], e.calc(fr[j], fr[j + 1], flow=inits[j].copy()), "pair %d host batch vs calc" % j)
+    # page-locked caller buffers take the direct copies
+    pinned_t = torch.from_numpy(inits.copy()).pin_memory()
+    pinned = pinned_t.numpy()
+    _bits_equal(e.calc_batch(list(fr), step=1, flows=pinned), host, "pinned host batch")
+    planes = np.ascontiguousarray(inits.transpose(0, 3, 1, 2))
+    _bits_equal(e.calc_batch_planes(list(fr), step=1, out=planes.copy()), host.transpose(0, 3, 1, 2), "host planes")
+    dfr = torch.from_numpy(np.ascontiguousarray(fr)).cuda()
+    s = torch.cuda.Stream()
+    with torch.cuda.stream(s):
+        dev = e.calc_batch_device(dfr, step=1, flows=torch.from_numpy(inits.copy()).cuda(), stream=s.cuda_stream)
+        devp = e.calc_batch_device_planes(dfr, step=1, planes=torch.from_numpy(planes.copy()).cuda(), stream=s.cuda_stream)
+        one = e.calc(dfr[2], dfr[3], flow=torch.from_numpy(inits[2].copy()).cuda(), stream=s.cuda_stream)
+    s.synchronize()
+    _bits_equal(dev.cpu().numpy(), host, "device batch")
+    _bits_equal(devp.cpu().numpy(), host.transpose(0, 3, 1, 2), "device planes")
+    _bits_equal(one.cpu().numpy(), host[2], "device calc on a side stream")
+    # negative steps pair the frames the other way round
+    back = e.calc_batch(list(fr), step=-2, flows=inits[:6].copy())
+    for j in range(6):
+        _bits_equal(back[j], e.calc(fr[j + 2], fr[j], flow=inits[j].copy()), "step -2 pair %d" % j)
+    e.release()
+
+
+def test_set_back_to_zero_starts_cold():
+    """a handle set back to 0 starts cold again, whatever its flow buffer holds"""
+    fr = synth.stream(H, W, 3, seed=9)
+    for alg in ("tvl1", "farn"):
+        e = _new(alg, W, H)
+        cold = e.calc(fr[0], fr[1])
+        e.set("use_initial_flow", 1)
+        warm = e.calc(fr[0], fr[1], flow=smooth_field(H, W, 4, amp=8.0))
+        assert not np.array_equal(warm, cold), alg
+        e.set("use_initial_flow", 0)
+        _bits_equal(e.calc(fr[0], fr[1], flow=smooth_field(H, W, 4, amp=8.0)), cold, alg + " back to 0")
+        e.release()
+
+
+# ---- refusals ------------------------------------------------------------------------------------------------------------------
+def _refusing_calls(e, fr, bgr, jpgs):
+    return {
+        "calc_batch_u8": lambda: e.calc_batch(list(fr), step=1, bound=20),
+        "calc_batch_png": lambda: e.calc_batch_png(list(fr), step=1),
+        "process_bgr_batch": lambda: e.process_bgr_batch(bgr, step=1),
+        "process_bgr_batch_png": lambda: e.process_bgr_batch_png(bgr, step=1),
+        "process_bgr_batch_planes": lambda: e.process_bgr_batch_planes(bgr, step=1),
+        "process_jpeg_batch": lambda: e.process_jpeg_batch(jpgs, step=1),
+        "process_jpeg_batch_png": lambda: e.process_jpeg_batch_png(jpgs, step=1),
+        "process_jpeg_batch_planes": lambda: e.process_jpeg_batch_planes(jpgs, step=1),
+        "calc without flow": lambda: e.calc(fr[0], fr[1]),
+        "calc_batch without flows": lambda: e.calc_batch(list(fr), step=1),
+        "calc_batch_planes without out": lambda: e.calc_batch_planes(list(fr), step=1),
+    }
+
+
+@pytest.mark.parametrize("alg", ["tvl1", "farn"])
+def test_calls_without_an_initial_flow_are_refused(alg):
+    import cv2
+    import torch
+    fr = synth.stream(H, W, 4, seed=3)
+    bgr = np.stack([cv2.cvtColor(f, cv2.COLOR_GRAY2BGR) for f in fr])
+    jpgs = [cv2.imencode(".jpg", f)[1].tobytes() for f in bgr]
+    e = _new(alg, W, H)
+    cold = e.calc(fr[0], fr[1])
+    e.set("use_initial_flow", 1)
+    dfr = torch.from_numpy(np.ascontiguousarray(fr)).cuda()
+    calls = _refusing_calls(e, fr, bgr, jpgs)
+    calls["calc device without flow"] = lambda: e.calc(dfr[0], dfr[1])
+    calls["calc_batch_device without flows"] = lambda: e.calc_batch_device(dfr, step=1)
+    calls["calc_batch_device_planes without planes"] = lambda: e.calc_batch_device_planes(dfr, step=1)
+    for name, call in calls.items():
+        torch.cuda.synchronize()
+        before = e.counters()["kernel_launches"]
+        with pytest.raises(RuntimeError, match="use_initial_flow"):
+            call()
+        assert e.counters()["kernel_launches"] == before, name
+    init = smooth_field(H, W, 6, amp=2.0)
+    warm = e.calc(fr[0], fr[1], flow=init.copy())
+    fresh = _new(alg, W, H, use_initial_flow=1)
+    _bits_equal(warm, fresh.calc(fr[0], fr[1], flow=init.copy()), "after the refusals")
+    e.set("use_initial_flow", 0)
+    _bits_equal(e.calc(fr[0], fr[1]), cold, "cold after the refusals")
+    e.release()
+    fresh.release()
+
+
+@pytest.mark.parametrize("alg", ["tvl1", "farn"])
+def test_parameter_takes_zero_or_one(alg):
+    e = _new(alg, 32, 32)
+    assert e.get("use_initial_flow") == 0
+    for v in (1, 0, 1):
+        e.set("use_initial_flow", v)
+        assert e.get("use_initial_flow") == v
+    for bad in (float("nan"), float("inf"), float("-inf"), 0.5, 2, -1):
+        with pytest.raises(RuntimeError, match="bad parameter use_initial_flow"):
+            e.set("use_initial_flow", bad)
+        assert e.get("use_initial_flow") == 1
+    e.release()
