@@ -5,15 +5,19 @@
 // include/dense_flow.h:10-18) to the writer thread, which marks a video done only after its LAST buffer has been
 // written (src/denseflow_gpu.cpp:456-470).  Here the same list is drained by W workers — one host thread per entry of
 // `devices`, each with its own engine handle, streams and pinned staging — from ONE work queue: an in-process atomic
-// counter, or a counter in POSIX shared memory when the workers are separate processes (one process per GPU).  The
-// unit of work is one video (its outputs and its completion mark stay together), there is no data-path collective,
-// and completion is reported per chunk with the reference's `last_buffer` meaning.
+// counter, or a counter in POSIX shared memory when the workers are separate processes (one process per GPU).  There is
+// no data-path collective.  Every entry point runs one scheduler, run_windows, over windows of a video's frames: a worker
+// reads a window, computes it and delivers it once every earlier window of the video has been delivered, and the video's
+// last window carries the reference's `last_buffer` meaning.  A worker runs the video it took to its end, then takes the
+// next one.
 //
-// dfb_list_run_videos runs the same dispatch over the videos as the reference takes them (colour frames or `-if` JPEG files)
-// and hands out the files the reference writes: flow JPEGs or PNGs, or with step 0 the extracted frames.  dfb_list_run_stream
-// does the same with frames pulled from the caller one window at a time, so a list of long videos runs in bounded memory.
-// dfb_list_run_windows pulls the same windows but makes the window the unit of work once the queue is empty: idle workers join
-// the unfinished videos, so one video runs on every worker and one worker reads a window while another computes the last.
+// The entry points differ in where a window's frames come from and what its outputs are.  dfb_list_run reads gray clips
+// in host memory and hands out flows or quantised planes.  dfb_list_run_videos reads the videos as the reference takes
+// them (colour frames or `-if` JPEG files) and hands out the files the reference writes: flow JPEGs, PNGs or h5 planes, or
+// with step 0 the extracted frames.  dfb_list_run_stream pulls the frames from the caller one window at a time, so a list
+// of long videos runs in bounded memory.  dfb_list_run_windows does the same and also shares a video's windows once the
+// queue is empty: idle workers join the unfinished videos, so one video runs on every worker and one worker reads a
+// window while another computes the last.
 //
 // This file is a client of the C ABI (dfb_create / dfb_calc_batch_host[_u8] / dfb_process_* / dfb_extract_frames_* /
 // dfb_destroy): it adds no arithmetic.
@@ -103,8 +107,7 @@ struct dfb_list_runner {
         dfb_handle *h = nullptr;
         int max_w = 0, max_h = 0;           // the frame size h was created for (dfb_list_run_stream grows it)
         dfb_counters retired{};             // counters of the handles this worker replaced during the current run
-        dfb::PinnedBuffer<uint8_t> pinned;  // output ring of one chunk: the copy engines write the results straight into it
-        dfb::PinnedBuffer<uint8_t> files;   // file ring of one chunk of dfb_list_run_videos / dfb_list_run_stream
+        dfb::PinnedBuffer<uint8_t> pinned;  // outputs of the one window the worker holds: the copy engines write them straight in
     };
     std::vector<Worker> workers;
 };
@@ -147,101 +150,11 @@ void dfb_list_close(dfb_list_runner *r) {
 
 namespace {
 
-// What one item of a list gives: DFB_OK and the flows and frames it adds to the stats, or the error that ends the run.
+// What reading or computing one window gives: DFB_OK, or the error that ends the run.
 struct ItemResult {
     int rc = DFB_OK;
     std::string error;
-    uint64_t flows = 0, frames = 0;
 };
-
-// The start of a run: the workers' engine counters from zero.
-void begin_run(dfb_list_runner *r, dfb_list_stats &st) {
-    st = dfb_list_stats{};
-    st.workers = (int)r->workers.size();
-    for (auto &w : r->workers) {
-        dfb_reset_counters(w.h);
-        w.retired = dfb_counters{};
-    }
-}
-
-// The end of a run: its wall time and the counters of every handle its workers used.
-void end_run(dfb_list_runner *r, dfb_list_stats &st, clk::time_point t_start) {
-    st.seconds = seconds_since(t_start);
-    for (auto &w : r->workers) {
-        dfb_counters c{};
-        if (dfb_get_counters(w.h, &c) == DFB_OK) {
-            st.kernel_launches += c.kernel_launches;
-            st.h2d_bytes += c.h2d_bytes;
-            st.d2h_bytes += c.d2h_bytes;
-        }
-        st.kernel_launches += w.retired.kernel_launches;
-        st.h2d_bytes += w.retired.h2d_bytes;
-        st.d2h_bytes += w.retired.d2h_bytes;
-    }
-}
-
-// Runs worker(wi) for every worker, each on a host thread of its own (worker 0 on the caller's).
-template <typename Worker>
-void run_workers(int n_workers, Worker &&worker) {
-    std::vector<std::thread> threads;
-    for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
-    worker(0);
-    for (auto &t : threads) t.join();
-}
-
-// The dispatch of dfb_list_run, dfb_list_run_videos and dfb_list_run_stream.  Each worker takes items from `queue` (or from
-// an in-process counter) until all n_items are taken or an item fails; body(wi, idx) runs item idx on worker wi.  The first
-// failure's code is returned and its message written to err; stats receives the run's counters either way.
-template <typename Body>
-int run_items(dfb_list_runner *r, int n_items, dfb_queue *queue, Body &&body, dfb_list_stats *stats, char *err, size_t err_len) {
-    const int n_workers = (int)r->workers.size();
-    dfb_list_stats st;
-    begin_run(r, st);
-    std::atomic<long> local_next{0};
-    std::atomic<int> failed{0};
-    std::mutex mtx;
-    std::string first_error;
-    const auto t_start = clk::now();
-
-    auto worker = [&](int wi) {
-        cudaSetDevice(r->workers[wi].device);
-        double busy = 0;
-        while (!failed.load()) {
-            const long idx = queue ? dfb_queue_next(queue) : local_next.fetch_add(1);
-            if (idx >= n_items) break;
-            const auto t0 = clk::now();
-            const ItemResult res = body(wi, idx);
-            if (res.rc != DFB_OK) {
-                std::lock_guard<std::mutex> lk(mtx);
-                if (!failed.load()) {
-                    failed.store(res.rc);
-                    first_error = res.error;
-                }
-                break;
-            }
-            if (failed.load()) break;
-            busy += seconds_since(t0);
-            std::lock_guard<std::mutex> lk(mtx);
-            ++st.clips;
-            st.flows += res.flows;
-            st.frames += res.frames;
-            ++st.clips_per_worker[wi];
-            st.flows_per_worker[wi] += res.flows;
-        }
-        std::lock_guard<std::mutex> lk(mtx);
-        st.busy_seconds_per_worker[wi] = busy;
-        st.finish_seconds_per_worker[wi] = seconds_since(t_start);
-    };
-
-    if (n_items > 0) run_workers(n_workers, worker);
-    end_run(r, st, t_start);
-    if (stats) *stats = st;
-    if (failed.load()) {
-        set_error(err, err_len, first_error);
-        return failed.load();
-    }
-    return DFB_OK;
-}
 
 // A chain that saw the frames of video k from f0 on names frame i as "frame i: ..."; the list names it in the video.
 std::string video_error(long k, int f0, const char *msg) {
@@ -361,11 +274,11 @@ ItemResult run_window(dfb_list_runner::Worker &w, int wi, long idx, const VideoA
                            : a.save_type == DFB_SAVE_H5  ? (size_t)g.dw * g.dh * sizeof(float)
                                                          : dfb_jpeg_max_bytes(g.dw, g.dh);
         try {
-            w.files.allocate((size_t)chunk * per * cap);
+            w.pinned.allocate((size_t)chunk * per * cap);
         } catch (const dfb::CudaError &) {
             return {DFB_ERR_CUDA, "worker " + std::to_string(wi) + ": pinned file ring allocation failed"};
         }
-        for (int k = 0; k < per * chunk; ++k) out[k] = (uint8_t *)w.files + (size_t)k * cap;
+        for (int k = 0; k < per * chunk; ++k) out[k] = (uint8_t *)w.pinned + (size_t)k * cap;
         if (!flow) {
             rc = bgr ? dfb_extract_frames_host(w.h, bf, m, g.sw, g.sh, dwa, dha, a.quality, out.data(), cap, lens.data())
                      : dfb_extract_frames_jpeg_host(w.h, jf, jl, m, dwa, dha, a.quality, out.data(), cap, lens.data());
@@ -402,25 +315,6 @@ ItemResult run_window(dfb_list_runner::Worker &w, int wi, long idx, const VideoA
     return {};
 }
 
-// One video through the chains on worker w, one window at a time.
-template <typename Fetch>
-ItemResult run_video(dfb_list_runner::Worker &w, int wi, long idx, const VideoArgs &a, const Geometry &g, Fetch &&fetch) {
-    auto deliver = [&](int f0, int m, bool ends, uint8_t *const *files, const size_t *lens) {
-        // every file of this chunk is in host memory now; ends makes it FlowBuffer::last_buffer (see dfb_list_run)
-        if (a.done) a.done(a.user, (int)idx, w.device, f0, m, ends, files, lens);
-    };
-    uint64_t outputs = 0;
-    for (int f0 = 0;;) {
-        Window win;
-        ItemResult res = run_window(w, wi, idx, a, g, f0, win, fetch, deliver);
-        if (res.rc != DFB_OK) return res;
-        const int m = window_outputs(a, win);
-        outputs += m;
-        if (win.ends) return {DFB_OK, {}, a.step != 0 ? outputs : 0, (uint64_t)f0 + win.n};
-        f0 += m;
-    }
-}
-
 // run() over videos with the call's jpeg_exact: the runner owns the handles, so it is set on each of them and restored
 // afterwards.
 template <typename Run>
@@ -434,13 +328,6 @@ int with_jpeg_exact(dfb_list_runner *r, int jpeg_exact, Run &&run) {
     const int rc = run();
     for (int wi = 0; wi < n_workers; ++wi) dfb_set_param(r->workers[wi].h, "jpeg_exact", exact_before[wi]);
     return rc;
-}
-
-// run_items over videos with the call's jpeg_exact.
-template <typename Body>
-int run_videos_with(dfb_list_runner *r, int n_videos, dfb_queue *queue, int jpeg_exact, Body &&body, dfb_list_stats *stats, char *err,
-                    size_t err_len) {
-    return with_jpeg_exact(r, jpeg_exact, [&] { return run_items(r, n_videos, queue, body, stats, err, err_len); });
 }
 
 // Worker w's handle for destination frames of dw x dh: a smaller handle is replaced by one at least that large in both
@@ -470,9 +357,9 @@ int fit_worker(dfb_list_runner *r, dfb_list_runner::Worker &w, int dw, int dh, s
 }
 
 // The caller's window of frames first .. first + max_n - 1 of video idx, into cur and win.  The video is sized by its first
-// window with a frame, which also fits `fit`'s handle to it when fit is given; every later frame must have frame 0's size.
-ItemResult fetch_stream_window(dfb_list_runner *r, dfb_frames_fn source, const VideoArgs &a, long idx, int first, int max_n, dfb_video &cur,
-                               Window &win, Geometry &g, dfb_list_runner::Worker *fit) {
+// window with a frame; every later frame must have frame 0's size.
+ItemResult fetch_stream_window(dfb_frames_fn source, const VideoArgs &a, long idx, int first, int max_n, dfb_video &cur, Window &win,
+                               Geometry &g) {
     const std::string k = "video " + std::to_string(idx) + ": ";
     cur = dfb_video{};
     char msg[512] = "";
@@ -481,12 +368,8 @@ ItemResult fetch_stream_window(dfb_list_runner *r, dfb_frames_fn source, const V
         return {DFB_ERR_INVALID_ARG, k + "the source returned a malformed window at frame " + std::to_string(first)};
     win = {&cur, 0, cur.n_frames, cur.n_frames < max_n};
     if (cur.n_frames == 0) return {};
-    if (first == 0) {
+    if (first == 0)
         if (int rc = size_video(cur, 0, a, g)) return {rc, k + dfb_last_error(nullptr)};
-        std::string e;
-        if (fit)
-            if (int rc = fit_worker(r, *fit, g.dw, g.dh, e)) return {rc, k + e};
-    }
     // a BGR window has one size; a JPEG file that cannot be sized is left to the decoder, which names the fault
     const int n_check = cur.kind == DFB_VIDEO_BGR ? 1 : cur.n_frames;
     for (int i = 0; i < n_check; ++i) {
@@ -499,7 +382,7 @@ ItemResult fetch_stream_window(dfb_list_runner *r, dfb_frames_fn source, const V
     return {};
 }
 
-// What the workers of dfb_list_run_windows share about one video they took from the queue, under the run's mutex.
+// What the workers share about one video taken from the queue, under the run's mutex.
 struct SharedVideo {
     long idx = 0;
     int next_first = 0;           // first frame of the next window to read
@@ -513,15 +396,30 @@ struct SharedVideo {
     Geometry g;                   // set by window 0
 };
 
-// The dispatch of dfb_list_run_windows (its policy is in the header).  A worker holds at most one window: it claims a video's
-// reader, reads the next window, releases the reader, runs the window through run_window and delivers it once every earlier
-// window of the video has been delivered.  Reads of one video are in order and never overlap, so every window read is held by
-// a worker that will deliver or drop it, and a worker waiting for its turn waits only on windows read before its own.
-int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queue *queue, const VideoArgs &a, dfb_list_stats *stats,
-                char *err, size_t err_len) {
+// The dispatch of every list entry point (its policy is in the header, under dfb_list_run_windows).  Workers take videos from
+// `queue` (or an in-process counter).  A worker holds at most one window: it claims a video's reader, reads the next window,
+// releases the reader, computes the window and delivers it once every earlier window of the video has been delivered.  Reads
+// of one video are in order and never overlap, so every window read is held by a worker that will deliver or drop it, and a
+// worker waiting for its turn waits only on windows read before its own.
+//   read(wi, idx, first, max_n, win, g)  fills win with frames first .. first + max_n - 1 of video idx, fewer when the video
+//                                        ends there; the read of window 0 sizes the video into g.
+//   body(w, wi, idx, g, f0, win, fetch, deliver)  runs window f0 on worker w: fetch(first, max_n, win) reads it (read, then
+//                                        the scheduler's bookkeeping), and deliver(first, m, ends, call) runs call(), which
+//                                        hands on the window's m outputs, in the video's order.
+// share = false: a worker runs the video it took to its end, then takes the next one, and stops once the queue is empty; a
+// failure cuts only the failed video, and every other worker finishes the video it holds and takes no new one.  share = true:
+// once the queue is empty, an idle worker joins the earliest unfinished video whose reader is free, or waits for one; a
+// failure cuts every video at its next unread window.
+template <typename Read, typename Body>
+int run_windows(dfb_list_runner *r, int n_videos, dfb_queue *queue, bool share, const VideoArgs &a, Read &&read, Body &&body,
+                dfb_list_stats *stats, char *err, size_t err_len) {
     const int n_workers = (int)r->workers.size();
-    dfb_list_stats st;
-    begin_run(r, st);
+    dfb_list_stats st{};
+    st.workers = n_workers;
+    for (auto &w : r->workers) {  // the workers' engine counters from zero
+        dfb_reset_counters(w.h);
+        w.retired = dfb_counters{};
+    }
     std::mutex mtx;
     std::condition_variable cv;
     std::list<SharedVideo> active;  // videos taken and not finished, in the order they were taken
@@ -529,15 +427,8 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
     bool queue_empty = false;
     SharedVideo *failed = nullptr;  // the first video to fail; its error is its earliest failed window's
 
-    // Under mtx: no video reads another window, and no window that has not been read is delivered.
-    auto stop = [&] {
-        for (auto &s : active) {
-            s.cut = std::min(s.cut, s.next_first);
-            s.ended = true;
-        }
-        cv.notify_all();
-    };
-    // Under mtx: window `first` of v failed.  An earlier window's failure replaces a later one's.
+    // Under mtx: window `first` of v failed.  An earlier window's failure replaces a later one's.  The videos it cuts read no
+    // other window, and deliver none that has not been read.
     auto fail = [&](SharedVideo &v, int first, ItemResult res) {
         if (first < v.failed_first) {
             v.failed_first = first;
@@ -545,7 +436,12 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
         }
         v.cut = std::min(v.cut, first);
         if (!failed) failed = &v;
-        stop();
+        for (auto &s : active) {
+            if (!share && &s != &v) continue;
+            s.cut = std::min(s.cut, s.next_first);
+            s.ended = true;
+        }
+        cv.notify_all();
     };
     const auto t_start = clk::now();
 
@@ -556,14 +452,14 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
         long own = -1;  // the video this worker took from the queue
         std::unique_lock<std::mutex> lk(mtx);
         for (;;) {
-            // While the queue holds videos a worker runs its own video, then takes the next one, as dfb_list_run_stream does.
-            // Then it joins the earliest unfinished video whose reader is free, or waits for one.
+            // A worker runs its own video to its end, then takes the next one.  With share, once the queue is empty, it joins
+            // the earliest unfinished video whose reader is free, or waits for one.
             SharedVideo *v = nullptr;
-            while (!failed) {
-                if (!queue_empty) {
+            for (;;) {
+                if (!share || !queue_empty) {
                     for (auto &s : active)
                         if (s.idx == own && !s.ended) v = &s;
-                    if (v) break;
+                    if (v || failed) break;
                     const long idx = queue ? dfb_queue_next(queue) : local_next++;
                     if (idx < n_videos) {
                         v = &active.emplace_back();
@@ -571,7 +467,9 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
                         break;
                     }
                     queue_empty = true;
+                    if (!share) break;
                 }
+                if (failed) break;
                 bool readable = false;  // a window is left to read
                 for (auto &s : active) {
                     if (s.ended) continue;
@@ -591,11 +489,10 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
 
             const auto t0 = clk::now();
             const std::string k = "video " + std::to_string(v->idx) + ": ";
-            dfb_video cur{};
             Window win;
             bool dropped = false;
             auto fetch = [&](int first, int max_n, Window &got) -> ItemResult {
-                ItemResult fr = fetch_stream_window(r, source, a, v->idx, first, max_n, cur, got, v->g, nullptr);
+                ItemResult fr = read(wi, v->idx, first, max_n, got, v->g);
                 const int m = fr.rc == DFB_OK ? window_outputs(a, got) : 0;
                 {
                     std::lock_guard<std::mutex> g(mtx);
@@ -621,7 +518,7 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
             // Everything this window adds to the video and to the stats is recorded under mtx before next_deliver moves
             // on: from then on the worker holding the video's next window may deliver it, and after the final window it
             // removes the video.  The worker does not touch v once its window is delivered.
-            auto deliver = [&](int first, int m, bool ends, uint8_t *const *files, const size_t *lens) {
+            auto deliver = [&](int first, int m, bool ends, auto &&call) {
                 std::unique_lock<std::mutex> dl(mtx);
                 cv.wait(dl, [&] { return first >= v->cut || v->next_deliver == first; });
                 if (first >= v->cut) {
@@ -629,8 +526,9 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
                     return;
                 }
                 dl.unlock();
-                // every file of this chunk is in host memory now, and every earlier chunk of the video has been delivered
-                if (a.done) a.done(a.user, (int)v->idx, w.device, first, m, ends, files, lens);
+                // every output of this window is in host memory now, and every earlier window of the video has been delivered;
+                // `ends` is the reference's FlowBuffer::last_buffer, the only point at which a video may be marked done
+                call();
                 dl.lock();
                 if (a.step != 0) {
                     st.flows_per_worker[wi] += m;
@@ -647,7 +545,7 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
                 }
                 cv.notify_all();
             };
-            ItemResult res = run_window(w, wi, v->idx, a, v->g, f0, win, fetch, deliver);
+            ItemResult res = body(w, wi, v->idx, v->g, f0, win, fetch, deliver);
             busy += seconds_since(t0);
             lk.lock();
             // a window that was delivered or dropped is done with; a failed one was never delivered, so v is still listed
@@ -657,14 +555,61 @@ int run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queu
         st.finish_seconds_per_worker[wi] = seconds_since(t_start);
     };
 
-    if (n_videos > 0) run_workers(n_workers, worker);
-    end_run(r, st, t_start);
+    if (n_videos > 0) {  // each worker on a host thread of its own, worker 0 on the caller's
+        std::vector<std::thread> threads;
+        for (int wi = 1; wi < n_workers; ++wi) threads.emplace_back(worker, wi);
+        worker(0);
+        for (auto &t : threads) t.join();
+    }
+    st.seconds = seconds_since(t_start);
+    for (auto &w : r->workers) {  // the counters of every handle the workers used
+        dfb_counters c{};
+        if (dfb_get_counters(w.h, &c) == DFB_OK) {
+            st.kernel_launches += c.kernel_launches;
+            st.h2d_bytes += c.h2d_bytes;
+            st.d2h_bytes += c.d2h_bytes;
+        }
+        st.kernel_launches += w.retired.kernel_launches;
+        st.h2d_bytes += w.retired.h2d_bytes;
+        st.d2h_bytes += w.retired.d2h_bytes;
+    }
     if (stats) *stats = st;
     if (failed) {
         set_error(err, err_len, failed->failure.error);
         return failed->failure.rc;
     }
     return DFB_OK;
+}
+
+// Frames first .. first + max_n - 1 of a video whose n_frames frames are all in host memory.
+Window slice(const dfb_video *v, int n_frames, int first, int max_n) {
+    const int n = std::max(std::min(max_n, n_frames - first), 0);
+    return {v, first, n, first + n >= n_frames};
+}
+
+// The entry points that hand out files: run_window computes each window, whose files go to a.done, under the call's jpeg_exact.
+template <typename Read>
+int run_files(dfb_list_runner *r, int n_videos, dfb_queue *queue, bool share, int jpeg_exact, const VideoArgs &a, Read &&read,
+              dfb_list_stats *stats, char *err, size_t err_len) {
+    auto body = [&](dfb_list_runner::Worker &w, int wi, long idx, const Geometry &g, int f0, Window &win, auto &fetch, auto &deliver) {
+        return run_window(w, wi, idx, a, g, f0, win, fetch, [&](int first, int m, bool ends, uint8_t *const *files, const size_t *lens) {
+            deliver(first, m, ends, [&] {
+                if (a.done) a.done(a.user, (int)idx, w.device, first, m, ends, files, lens);
+            });
+        });
+    };
+    return with_jpeg_exact(r, jpeg_exact, [&] { return run_windows(r, n_videos, queue, share, a, read, body, stats, err, err_len); });
+}
+
+// dfb_list_run_stream and dfb_list_run_windows: windows from the caller's source.  A worker holds one window at a time, so the
+// latest one it read, cur[wi], is all it keeps.
+int run_source(dfb_list_runner *r, int n_videos, dfb_frames_fn source, dfb_queue *queue, bool share, int jpeg_exact, const VideoArgs &a,
+               dfb_list_stats *stats, char *err, size_t err_len) {
+    std::vector<dfb_video> cur(r->workers.size());
+    auto read = [&](int wi, long idx, int first, int max_n, Window &win, Geometry &g) {
+        return fetch_stream_window(source, a, idx, first, max_n, cur[wi], win, g);
+    };
+    return run_files(r, n_videos, queue, share, jpeg_exact, a, read, stats, err, err_len);
 }
 
 }  // namespace
@@ -691,9 +636,19 @@ int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int ste
     }
     const size_t px_max = (size_t)r->max_w * r->max_h;
     const size_t out_bytes = (size_t)chunk_flows * px_max * (bound > 0 ? 2 : 8);
+    VideoArgs a;  // the windows: flows [f0, f0 + m) of window f0 read frames f0 .. f0 + m - 1 + |step|
+    a.step = step;
+    a.astep = astep;
+    a.chunk_flows = chunk_flows;
 
-    auto run_clip = [&](int wi, long idx) -> ItemResult {
-        dfb_list_runner::Worker &w = r->workers[wi];
+    auto read = [&](int, long idx, int first, int max_n, Window &win, Geometry &) {
+        win = slice(nullptr, clips[idx].n_frames, first, max_n);
+        return ItemResult{};
+    };
+    auto body = [&](dfb_list_runner::Worker &w, int wi, long idx, const Geometry &, int f0, Window &win, auto &fetch,
+                    auto &deliver) -> ItemResult {
+        ItemResult fr = fetch(f0, chunk_flows + astep, win);
+        if (fr.rc != DFB_OK) return fr;
         try {
             w.pinned.allocate(out_bytes);
         } catch (const dfb::CudaError &) {
@@ -705,33 +660,24 @@ int dfb_list_run(dfb_list_runner *r, const dfb_clip *clips, int n_clips, int ste
         std::vector<float *> fl(chunk_flows);
         const dfb_clip &c = clips[idx];
         const size_t px = (size_t)c.width * c.height;
-        const int M = std::max(c.n_frames - astep, 0);  // src/denseflow_gpu.cpp:308
         for (int i = 0; i < chunk_flows; ++i) {
             qx[i] = qbuf ? qbuf + (size_t)(2 * i) * px : nullptr;
             qy[i] = qbuf ? qbuf + (size_t)(2 * i + 1) * px : nullptr;
             fl[i] = fbuf ? fbuf + (size_t)i * px * 2 : nullptr;
         }
-        // chunks of flows [f0, f0 + m): frames f0 .. f0 + m - 1 + |step| (the overlap the reference keeps between its
-        // own <= 512-frame batches, src/denseflow_gpu.cpp:182-189,204-205), so flow indices stay global (base_start)
-        int f0 = 0;
-        for (;;) {
-            const int m = std::max(std::min(chunk_flows, M - f0), 0);
-            int rc = DFB_OK;
-            if (m > 0)
-                rc = bound > 0 ? dfb_calc_batch_host_u8(w.h, c.frames + f0, m + astep, step, c.width, c.height, bound, qx.data(), qy.data())
-                               : dfb_calc_batch_host(w.h, c.frames + f0, m + astep, step, c.width, c.height, fl.data());
-            if (rc != DFB_OK) return {rc, "clip " + std::to_string(idx) + ": " + dfb_last_error(w.h)};
-            const int last = f0 + m >= M;
-            // every output of this chunk is in host memory now; `last` is the reference's FlowBuffer::last_buffer,
-            // the only point at which a video may be marked done
-            if (done) done(user, (int)idx, w.device, f0, m, last, bound > 0 ? qx.data() : nullptr, bound > 0 ? qy.data() : nullptr,
+        const int m = window_outputs(a, win);  // a clip of n frames has max(n - |step|, 0) flows, src/denseflow_gpu.cpp:308
+        int rc = DFB_OK;
+        if (m > 0)
+            rc = bound > 0 ? dfb_calc_batch_host_u8(w.h, c.frames + f0, m + astep, step, c.width, c.height, bound, qx.data(), qy.data())
+                           : dfb_calc_batch_host(w.h, c.frames + f0, m + astep, step, c.width, c.height, fl.data());
+        if (rc != DFB_OK) return {rc, "clip " + std::to_string(idx) + ": " + dfb_last_error(w.h)};
+        deliver(f0, m, win.ends, [&] {
+            if (done) done(user, (int)idx, w.device, f0, m, win.ends, bound > 0 ? qx.data() : nullptr, bound > 0 ? qy.data() : nullptr,
                            bound > 0 ? nullptr : fl.data());
-            f0 += m;
-            if (last) break;
-        }
-        return {DFB_OK, {}, (uint64_t)M, (uint64_t)c.n_frames};
+        });
+        return {};
     };
-    return run_items(r, n_clips, queue, run_clip, stats, err, err_len);
+    return run_windows(r, n_clips, queue, false, a, read, body, stats, err, err_len);
 }
 
 int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_videos, int step, int bound, int save_type, int quality,
@@ -767,18 +713,12 @@ int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_video
             return DFB_ERR_SIZE;
         }
     }
-    auto body = [&](int wi, long idx) -> ItemResult {
-        const dfb_video &v = videos[idx];
-        auto fetch = [&](int first, int max_n, Window &win) -> ItemResult {
-            win.v = &v;
-            win.off = first;
-            win.n = std::max(std::min(max_n, v.n_frames - first), 0);
-            win.ends = first + win.n >= v.n_frames;
-            return {};
-        };
-        return run_video(r->workers[wi], wi, idx, a, geo[idx], fetch);
+    auto read = [&](int, long idx, int first, int max_n, Window &win, Geometry &g) {
+        win = slice(&videos[idx], videos[idx].n_frames, first, max_n);
+        g = geo[idx];
+        return ItemResult{};
     };
-    return run_videos_with(r, n_videos, queue, jpeg_exact, body, stats, err, err_len);
+    return run_files(r, n_videos, queue, false, jpeg_exact, a, read, stats, err, err_len);
 }
 
 int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, int step, int bound, int save_type, int quality,
@@ -794,16 +734,7 @@ int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, 
         return rc;
     a.done = done;
     a.user = user;
-    auto body = [&](int wi, long idx) -> ItemResult {
-        dfb_list_runner::Worker &w = r->workers[wi];
-        Geometry g;
-        dfb_video cur{};  // the source's latest window
-        auto fetch = [&](int first, int max_n, Window &win) -> ItemResult {
-            return fetch_stream_window(r, source, a, idx, first, max_n, cur, win, g, &w);
-        };
-        return run_video(w, wi, idx, a, g, fetch);
-    };
-    return run_videos_with(r, n_videos, queue, jpeg_exact, body, stats, err, err_len);
+    return run_source(r, n_videos, source, queue, false, jpeg_exact, a, stats, err, err_len);
 }
 
 int dfb_list_run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source, int step, int bound, int save_type, int quality,
@@ -823,7 +754,7 @@ int dfb_list_run_windows(dfb_list_runner *r, int n_videos, dfb_frames_fn source,
     }
     a.done = done;
     a.user = user;
-    return with_jpeg_exact(r, jpeg_exact, [&] { return run_windows(r, n_videos, source, queue, a, stats, err, err_len); });
+    return run_source(r, n_videos, source, queue, true, jpeg_exact, a, stats, err, err_len);
 }
 
 int dfb_run_list(const char *algorithm, const int *devices, int n_workers, const dfb_clip *clips, int n_clips, int step, int bound,

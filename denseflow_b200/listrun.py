@@ -210,8 +210,8 @@ class ListRunner:
         """run_videos with the frames pulled from `source` one window at a time (dfb_list_run_stream), so a list of long videos
         runs in bounded memory.  source(video, first, max_n) returns frames first .. first + max_n - 1 of the video, fewer when
         the video ends there, as uint8 [H,W,3] BGR frames or JPEG files (bytes).  It runs on the worker's thread, in frame order
-        for each video; consecutive windows overlap by |step| frames.  A window is kept alive until the next call for its
-        video, or until the video's last chunk.  An exception in source ends the run with "video k: <message>"; one in
+        for each video; consecutive windows overlap by |step| frames.  A window is kept alive until its on_chunk call returns
+        (or until the run ends after a failure).  An exception in source ends the run with "video k: <message>"; one in
         on_chunk ends it too and is raised again here.  on_chunk and the result are those of run_videos, except that a video
         whose outputs end on a window boundary gets one more on_chunk call with no files and last_chunk True."""
         return self._run_source("dfb_list_run_stream", n_videos, source, on_chunk, step, bound, save_type, quality, jpeg_exact,
@@ -230,18 +230,14 @@ class ListRunner:
 
     def _run_source(self, fn, n_videos, source, on_chunk, step, bound, save_type, quality, jpeg_exact, new_width, new_height, new_short,
                     chunk_flows, queue):
-        """run_stream and run_windows: they differ in how long a window lives.  dfb_list_run_stream is done with a video's
-        window at its next source call; dfb_list_run_windows with each window once its on_chunk call has returned."""
+        """run_stream and run_windows: the runner is done with each window once its on_chunk call has returned."""
         if save_type not in _SAVE_TYPES:
             raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
         per = 2 if step != 0 and save_type != "png" else 1
-        shared = fn == "dfb_list_run_windows"
-        windows = {}  # (video, first) or video -> a live window and the memory behind it
+        windows = {}  # (video, first) -> a live window and the memory behind it
         failures = []
 
         def _source(user, video, first, max_n, out, msg, msg_len):
-            if not shared:
-                windows.pop(video, None)  # the worker is done with the previous window
             try:
                 if failures:
                     raise RuntimeError("stopped after an on_chunk call failed")
@@ -251,7 +247,7 @@ class ListRunner:
                 C.memmove(msg, text + b"\0", len(text) + 1)
                 return 1
             out[0] = v
-            windows[(video, first) if shared else video] = keep
+            windows[(video, first)] = keep
             return 0
 
         def _done(user, video, dev, first, n, last, files, lens):
@@ -260,10 +256,7 @@ class ListRunner:
                     on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
             except BaseException as ex:
                 failures.append(ex)
-            if shared:
-                windows.pop((video, first), None)
-            elif last:
-                windows.pop(video, None)
+            windows.pop((video, first), None)
 
         src = _lib.FRAMES_FN(_source)
         cb = _lib.FILES_DONE_FN(_done)

@@ -520,7 +520,10 @@ int dfb_reset_counters(dfb_handle *h);
  *                   create the video's .done marker
  *   qx/qy           bound > 0: the convertFlowToImage planes (width*height uint8 each), flows == NULL
  *   flows           bound == 0: CV_32FC2 fields, qx == qy == NULL
- * The buffers belong to the worker and are reused after the callback returns.
+ * The buffers belong to the worker and are reused after the callback returns.  A failure ends the run with the first failed
+ * video's code and message: the other workers finish the video they hold, every chunk and last_chunk included, and take no
+ * new one.  The stats of a failed call count what was delivered: clips, flows and frames those of the videos whose last chunk
+ * was delivered, flows_per_worker the flows of every delivered chunk.
  */
 typedef struct dfb_queue dfb_queue;
 int dfb_queue_open(const char *name, int create, dfb_queue **out); /* name: "/something" (shm_open); create = 1 also zeroes it */
@@ -596,8 +599,8 @@ int dfb_list_run_videos(dfb_list_runner *r, const dfb_video *videos, int n_video
  * ~110 GB of BGR frames): only n_videos is known up front.  The worker that takes video k calls
  *   source(user, k, first, max_n, out, msg, msg_len)
  * for frames first .. first + max_n - 1 and runs them through the same chains.  The source fills *out (kind, n_frames, bgr +
- * width / height, or jpeg + jpeg_len); n_frames < max_n means the video ends there.  The pointers stay valid until the next
- * call for this video, or until the video's last `done` call returns.  A nonzero return fails the run with "video k: <msg>".
+ * width / height, or jpeg + jpeg_len); n_frames < max_n means the video ends there.  The pointers stay valid until that
+ * window's `done` call returns, or until the call returns after a failure.  A nonzero return fails the run with "video k: <msg>".
  *   - max_n is at most chunk_flows + |step| (chunk_flows with step 0); consecutive windows overlap by |step| frames, the
  *     overlap the reference keeps between its batches.  The calls for one video come in order from the worker that owns it.
  *   - The video's size comes from its first window (BGR width / height, or dfb_jpeg_info of JPEG 0); a later frame of another
@@ -622,8 +625,8 @@ int dfb_list_run_stream(dfb_list_runner *r, int n_videos, dfb_frames_fn source, 
  *   - Windows: the sequence dfb_list_run_stream asks for (max_n = chunk_flows + |step|, chunk_flows at step 0; consecutive
  *     windows overlap by |step|; a short window ends the video).  The source calls for one video come in frame order and never
  *     overlap in time, but may come from different workers' threads.
- *   - Lifetime: what the source returns for a window stays valid until that window's `done` call returns, or until the call
- *     returns after a failure (not "until the next call for this video").
+ *   - Lifetime: dfb_list_run_stream's; what the source returns for a window stays valid until that window's `done` call
+ *     returns, or until the call returns after a failure.
  *   - Delivery: the `done` calls for one video come in first_index order, each after the previous one has returned, on the
  *     thread of the worker that computed the window, with that worker's device.  last_chunk comes once per video, in its last
  *     call; the n = 0 trailing call follows dfb_list_run_stream's rule.  The files and every other argument equal

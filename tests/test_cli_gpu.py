@@ -24,9 +24,10 @@ def jpegs(frames):
     return [J.encode(f, "420", 95) for f in frames]
 
 
-def collect(run, n_videos, step, save_type):
+def collect(run, n_videos, step, save_type, calls=None):
     """Run `run(on_chunk)`; the files per video in index order, after checking that last_chunk comes once per video after
-    all its files and that chunks arrive in order."""
+    all its files, that chunks arrive in order, and that every chunk of a video (and every source call in `calls`, as
+    window_source records them) comes from one thread."""
     per = 2 if step != 0 and save_type == "jpg" else 1
     got = {i: {} for i in range(n_videos)}
     events = []
@@ -36,20 +37,23 @@ def collect(run, n_videos, step, save_type):
         with lock:
             for k, f in enumerate(files):
                 got[video][per * first + k] = bytes(f)
-            events.append((video, first, len(files) // per, last))
+            events.append((video, first, len(files) // per, last, threading.get_ident()))
 
     st = run(on_chunk)
     for i in range(n_videos):
         mine = [ev for ev in events if ev[0] == i]
         assert [ev[3] for ev in mine].count(True) == 1 and mine[-1][3], (i, mine)
         assert [ev[1] for ev in mine] == sorted(ev[1] for ev in mine)
+        threads = {ev[4] for ev in mine} | {c[3] for c in calls or [] if c[0] == i}
+        assert len(threads) == 1, (i, threads)
     return [[got[i][k] for k in range(len(got[i]))] for i in range(n_videos)], st
 
 
 def window_source(videos, calls=None):
+    """source(video, first, max_n) over whole videos in memory; with `calls`, records (video, first, max_n, thread) per call."""
     def source(video, first, max_n):
         if calls is not None:
-            calls.append((video, first, max_n))
+            calls.append((video, first, max_n, threading.get_ident()))
         return videos[video][first:first + max_n]
     return source
 
@@ -82,7 +86,7 @@ def test_run_stream_equals_run_videos(alg):
             want, st_w = collect(lambda cb: whole.run_videos(videos, on_chunk=cb, **kw), len(videos), step, save_type)
             calls = []
             got, st_s = collect(lambda cb: stream.run_stream(len(videos), window_source(videos, calls), cb, **kw), len(videos), step,
-                                save_type)
+                                save_type, calls)
             assert got == want, (step, save_type, ns)
             for k in ("clips", "flows", "frames"):
                 assert st_s[k] == st_w[k], (k, step, save_type)
@@ -181,6 +185,42 @@ def test_failures_name_the_video_and_frame():
         assert got == want and len(got[0]) == 9
     finally:
         r.close()
+
+
+def test_a_failure_lets_the_other_workers_finish_their_videos():
+    """Video 1 fails at its second window while video 0, longer, runs on another worker: video 0 still gets every chunk, its
+    last_chunk included, with a clean run's bytes, and the run reports video 1's error."""
+    from denseflow_b200 import listrun
+    videos = [bgr_frames(4 * 12 + 1, 48, 64, seed=5), bgr_frames(10, 48, 64, seed=6)]
+    failed = threading.Event()
+    threads = {0: set(), 1: set()}
+    chunks = []
+
+    def source(video, first, max_n):
+        threads[video].add(threading.get_ident())
+        if video == 1 and first >= 4:
+            failed.set()
+            raise ValueError("cannot read frame %d" % first)
+        if video == 0 and first == 8:
+            failed.wait(60)  # video 0 is mid-way when video 1 fails
+        return videos[video][first:first + max_n]
+
+    def on_chunk(video, dev, first, last, files):
+        threads[video].add(threading.get_ident())
+        if video == 0:
+            chunks.append((first, last, [bytes(f) for f in files]))
+
+    r = listrun.ListRunner("farn", [0, 0, 0], 64, 48)
+    try:
+        with pytest.raises(RuntimeError, match="^video 1: cannot read frame 4$"):
+            r.run_stream(2, source, on_chunk, step=1, chunk_flows=4, jpeg_exact=1)
+        clean = []
+        r.run_stream(1, window_source(videos), lambda v, d, f, last, fs: clean.append((f, last, [bytes(x) for x in fs])), step=1,
+                     chunk_flows=4, jpeg_exact=1)
+    finally:
+        r.close()
+    assert failed.is_set() and len(threads[0]) == len(threads[1]) == 1 and threads[0] != threads[1], threads
+    assert chunks == clean and clean[-1][1] and sum(len(c[2]) for c in clean) == 2 * 48
 
 
 # ---- the command ---------------------------------------------------------------------------------------------------------

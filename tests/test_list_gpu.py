@@ -32,7 +32,7 @@ def test_list_outputs_match_single_handle(alg):
             assert flows is None
             for k in range(len(qx)):
                 got[clip][first + k] = (qx[k].copy(), qy[k].copy())
-            events.append((clip, first, len(qx), last))
+            events.append((clip, first, len(qx), last, threading.get_ident()))
 
     st = listrun.run_list(alg, [0, 0, 0], clips, step=1, bound=20, chunk_flows=4, on_chunk=on_chunk)
     assert st["clips"] == len(clips) and st["flows"] == sum(max(len(c) - 1, 0) for c in clips)
@@ -45,6 +45,7 @@ def test_list_outputs_match_single_handle(alg):
         ev = [x for x in events if x[0] == i]
         assert [x[3] for x in ev].count(True) == 1 and ev[-1][3]      # done exactly once, on the video's last chunk
         assert [x[1] for x in ev] == list(range(0, max(m, 1), 4))      # chunks of 4 flows, global first_flow indices
+        assert len({x[4] for x in ev}) == 1                            # all from the worker that took the video
 
 
 def test_list_float_flows_and_negative_step():

@@ -3,6 +3,7 @@ single-handle chain's (and, for the strict build, the reference pipeline's own c
 carry global indices, last_chunk fires once per video after all its files, and a refused JPEG names the video and the
 frame without spoiling the runner."""
 import threading
+import time
 
 import cv2
 import numpy as np
@@ -157,7 +158,7 @@ def _run(r, videos, step, save_type, **kw):
             assert len(files) % per == 0
             for k, f in enumerate(files):
                 got[video][per * first + k] = bytes(f)
-            events.append((video, first, len(files) // per, last))
+            events.append((video, first, len(files) // per, last, threading.get_ident()))
 
     st = r.run_videos(videos, step=step, save_type=save_type, chunk_flows=4, on_chunk=on_chunk, **kw)
     for i in range(len(videos)):
@@ -166,6 +167,7 @@ def _run(r, videos, step, save_type, **kw):
         assert len(lasts) == 1 and mine[-1] is lasts[0], (i, mine)  # once, after every other chunk of the video
         firsts = [ev[1] for ev in mine]
         assert firsts == sorted(firsts)
+        assert len({ev[4] for ev in mine}) == 1, (i, mine)  # every chunk from the worker that took the video
     return [[got[i][k] for k in range(len(got[i]))] for i in range(len(videos))], st
 
 
@@ -242,6 +244,41 @@ def test_run_videos_refusals_name_the_video_and_frame():
         _check_run_list(r, "farn")
     finally:
         r.close()
+
+
+def test_a_failure_lets_the_other_workers_finish_their_videos():
+    """Video 1 fails at its second chunk (a corrupt frame 6) while video 0, longer, runs on another worker: video 0 still gets
+    every chunk, its last_chunk included, with a clean run's bytes, and the run reports video 1's error."""
+    from denseflow_b200 import listrun
+    frames = bgr_frames(10, 64, 96, seed=4)
+    bad = jpegs(frames)
+    bad[6] = bad[6][:int(len(bad[6]) * 0.6)] + b"\xff\xd9"
+    videos = [jpegs(bgr_frames(4 * 12 + 1, 64, 96, seed=7)), bad]
+    started = threading.Event()
+    threads = {0: set(), 1: set()}
+    chunks = []
+
+    def on_chunk(video, dev, first, last, files):
+        threads[video].add(threading.get_ident())
+        if video == 1:
+            started.set()
+            return
+        if first == 0:
+            started.wait(60)  # video 1 runs on another worker
+            time.sleep(0.5)   # and fails at its next chunk meanwhile
+        chunks.append((first, last, [bytes(f) for f in files]))
+
+    r = listrun.ListRunner("farn", [0, 0, 0], 96, 64)
+    try:
+        with pytest.raises(RuntimeError, match="^video 1: frame 6: .*ends before the last MCU"):
+            r.run_videos(videos, step=1, chunk_flows=4, jpeg_exact=1, on_chunk=on_chunk)
+        clean = []
+        r.run_videos(videos[:1], step=1, chunk_flows=4, jpeg_exact=1,
+                     on_chunk=lambda v, d, f, last, fs: clean.append((f, last, [bytes(x) for x in fs])))
+    finally:
+        r.close()
+    assert started.is_set() and len(threads[0]) == len(threads[1]) == 1 and threads[0] != threads[1], threads
+    assert chunks == clean and [c[0] for c in clean] == list(range(0, 48, 4)) and [c[1] for c in clean] == [False] * 11 + [True]
 
 
 @pytest.mark.parametrize("alg", ["tvl1", "farn"])
