@@ -886,6 +886,63 @@ class Farneback final : public FlowAlgorithm {
             down(out[1], args.p[0].fy, 0);
             return true;
         }
+        if (k == "farn_initial_flow") {  // in {x, y of every pair's initial flow}  out {fx, fy of the coarsest level}  scalars {step, pitch, pairs}
+            // pair i starts from rows [i * h / pairs, (i + 1) * h / pairs) of the inputs, laid out on the device as the calls pass
+            // it: step 2 a float2 field, step 1 two planes, rows `pitch` floats apart (0: dense); the coarsest level of the
+            // handle's num_levels comes back, stacked along the rows.  The start buffers' padding and the lanes' flow planes hold
+            // NaN first; the flow planes are zero after.
+            need(2, 2);
+            const int step = (int)sc(0, 2), nb = (int)sc(2, 1);
+            if (step != 1 && step != 2) throw std::runtime_error(k + ": step must be 1 or 2");
+            if (nb < 1 || nb > kMaxFarnBatch || h % nb) throw std::runtime_error(k + ": pairs must be in [1, 8] and divide the height");
+            const int ph = h / nb;
+            fits(w, ph);
+            const size_t row = (size_t)w * step, pitch = sc(1, 0) > 0 ? (size_t)sc(1, 0) : row;
+            if (pitch < row) throw std::runtime_error(k + ": pitch smaller than a row");
+            const LevelSet ls = levels_for(w, ph, false);
+            const Level &L = ls.lv[0];
+            ensure_slots(2 * nb);
+            ensure_lanes(nb);
+            const size_t pl_bytes = Slab::padded(plane_elems_, 4), yoff = step == 2 ? 1 : pitch * ph;
+            const size_t buf_elems = pitch * ph * (step == 1 ? 2 : 1);
+            std::vector<float> host(buf_elems);
+            std::vector<float *> bufs(nb);
+            FarnBatchArgs args{};
+            for (int i = 0; i < nb; ++i) {
+                std::memset(host.data(), 0xff, buf_elems * sizeof(float));
+                const float *x = in[0] + (size_t)i * ph * w, *y = in[1] + (size_t)i * ph * w;
+                for (int r = 0; r < ph; ++r)
+                    for (int c = 0; c < w; ++c) {
+                        host[r * pitch + (size_t)c * step] = x[(size_t)r * w + c];
+                        host[yoff + r * pitch + (size_t)c * step] = y[(size_t)r * w + c];
+                    }
+                DFB_CUDA(cudaMalloc(&bufs[i], buf_elems * sizeof(float)));
+                DFB_CUDA(cudaMemcpy(bufs[i], host.data(), buf_elems * sizeof(float), cudaMemcpyHostToDevice));
+                for (int b = 0; b < 2; ++b) {
+                    DFB_CUDA(cudaMemset(lanes_[i].fx[b], 0xff, pl_bytes));
+                    DFB_CUDA(cudaMemset(lanes_[i].fy[b], 0xff, pl_bytes));
+                }
+                PairJob pj{2 * i, 2 * i + 1, nullptr, 0};
+                pj.init_x = bufs[i];
+                pj.init_y = bufs[i] + yoff;
+                pj.init_pitch = pitch;
+                pj.init_step = step;
+                args.p[i] = pair_args(pj, lanes_[i], ls, 0, 0);
+            }
+            launch_flow_init(args, nb, ls, 0, s, true);
+            DFB_CUDA(cudaDeviceSynchronize());
+            for (int i = 0; i < nb; ++i) {
+                down(out[0], args.p[i].fx, i * L.h);
+                down(out[1], args.p[i].fy, i * L.h);
+                for (int b = 0; b < 2; ++b) {
+                    DFB_CUDA(cudaMemset(lanes_[i].fx[b], 0, pl_bytes));
+                    DFB_CUDA(cudaMemset(lanes_[i].fy[b], 0, pl_bytes));
+                }
+                DFB_CUDA(cudaFree(bufs[i]));
+            }
+            DFB_CUDA(cudaDeviceSynchronize());
+            return true;
+        }
         const bool um = k == "farn_update_matrices";
         if (!um && k != "farn_iteration") return false;
         // pair stages: every input stacks `pairs` planes of h / pairs rows along its rows, one per pair (pair i = lane i, frame

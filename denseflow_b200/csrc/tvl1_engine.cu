@@ -317,6 +317,7 @@ class Tvl1 final : public FlowAlgorithm {
     // uploaded, so a stage that reads padding, halo or another lane's rows shows up in the image pixels.
     bool debug_run(const std::string &k, const float *const *in, int n_in, float *const *out, int n_out, int w, int h, const double *scalars,
                    int n_scalars, double *scalar_out) override {
+        if (k == "tvl1_initial_flow") return debug_initial_flow(k, in, n_in, out, n_out, w, h, scalars, n_scalars);
         static const struct {
             const char *name;
             int stage, n_in, n_out, n_sc;
@@ -489,6 +490,72 @@ class Tvl1 final : public FlowAlgorithm {
     }
 
   private:
+    // Test hook "tvl1_initial_flow": load_initial_flow on `lanes` lanes (scalars {step, pitch, lanes}), lane i starting from
+    // rows [i * h / lanes, (i + 1) * h / lanes) of the two input planes, laid out on the device as the calls pass it: step 2 a
+    // float2 field, step 1 two planes, rows `pitch` floats apart (0: dense).  out[0] / out[1]: every lane's u1pyr[0] / u2pyr[0]
+    // at the handle's nscales / scale_step, level after level, each level the lanes' dense planes stacked along the rows.  The lane pyramids and the start
+    // buffers' padding hold NaN first, so a read of padding or a pyramid left unwritten shows; the pyramids are zero after.
+    bool debug_initial_flow(const std::string &k, const float *const *in, int n_in, float *const *out, int n_out, int w, int h,
+                            const double *scalars, int n_scalars) {
+        auto sc = [&](int i, double dflt) { return i < n_scalars ? scalars[i] : dflt; };
+        const int step = (int)sc(0, 2), nb = (int)sc(2, 1);
+        if (n_in != 2) throw std::runtime_error(k + ": expects 2 inputs");
+        if (step != 1 && step != 2) throw std::runtime_error(k + ": step must be 1 or 2");
+        if (nb < 1 || nb > kFusedMaxLanes || h % nb) throw std::runtime_error(k + ": lanes must be in [1, 64] and divide the height");
+        const int ph = h / nb;
+        const size_t row = (size_t)w * step, pitch = sc(1, 0) > 0 ? (size_t)sc(1, 0) : row;
+        if (pitch < row) throw std::runtime_error(k + ": pitch smaller than a row");
+        LevelGeom lv[kMaxScales];
+        const int n = level_geometry(w, ph, lv);
+        if (n_out != 2) throw std::runtime_error(k + ": expects 2 outputs");
+        for (int l = 0; l < n; ++l)
+            if (w < 1 || (size_t)lv[l].pitch * (lv[l].h + 1) > max_lv_elems_[l])
+                throw std::runtime_error(k + ": plane size outside the handle's level " + std::to_string(l));
+
+        DFB_CUDA(cudaDeviceSynchronize());  // nothing of an earlier asynchronous call may still use the lanes
+        const cudaStream_t s = nullptr;
+        ensure_lanes(nb);
+        const size_t pyr_bytes = Slab::padded(pyr_elems_, 4), yoff = step == 2 ? 1 : pitch * ph;
+        const size_t buf_elems = pitch * ph * (step == 1 ? 2 : 1);
+        std::vector<float> host(buf_elems);
+        std::vector<float *> bufs(nb);
+        std::vector<PairJob> jobs(nb);
+        for (int i = 0; i < nb; ++i) {
+            DFB_CUDA(cudaMemset(lanes_[i].u1pyr[0], 0xff, pyr_bytes));
+            DFB_CUDA(cudaMemset(lanes_[i].u2pyr[0], 0xff, pyr_bytes));
+            std::memset(host.data(), 0xff, buf_elems * sizeof(float));
+            const float *x = in[0] + (size_t)i * ph * w, *y = in[1] + (size_t)i * ph * w;
+            for (int r = 0; r < ph; ++r)
+                for (int c = 0; c < w; ++c) {
+                    host[r * pitch + (size_t)c * step] = x[(size_t)r * w + c];
+                    host[yoff + r * pitch + (size_t)c * step] = y[(size_t)r * w + c];
+                }
+            DFB_CUDA(cudaMalloc(&bufs[i], buf_elems * sizeof(float)));
+            DFB_CUDA(cudaMemcpy(bufs[i], host.data(), buf_elems * sizeof(float), cudaMemcpyHostToDevice));
+            jobs[i] = PairJob{2 * i, 2 * i + 1, nullptr, 0};
+            jobs[i].init_x = bufs[i];
+            jobs[i].init_y = bufs[i] + yoff;
+            jobs[i].init_pitch = pitch;
+            jobs[i].init_step = step;
+        }
+        load_initial_flow(jobs.data(), nb, lv, n, s);
+        DFB_CUDA(cudaDeviceSynchronize());
+        for (int i = 0; i < nb; ++i) {
+            size_t off = 0;  // level l's first element in the outputs
+            for (int l = 0; l < n; off += (size_t)nb * lv[l].w * lv[l].h, ++l)
+                for (int c = 0; c < 2; ++c) {
+                    const Plane p = level_plane(c ? lanes_[i].u2pyr[0] : lanes_[i].u1pyr[0], lv, l);
+                    DFB_CUDA(cudaMemcpy2D(out[c] + off + (size_t)i * p.h * p.w, (size_t)p.w * 4, p.p, (size_t)p.pitch * 4, (size_t)p.w * 4, p.h,
+                                          cudaMemcpyDeviceToHost));
+                }
+            DFB_CUDA(cudaMemset(lanes_[i].u1pyr[0], 0, pyr_bytes));  // as ensure_lanes leaves them
+            DFB_CUDA(cudaMemset(lanes_[i].u2pyr[0], 0, pyr_bytes));
+            DFB_CUDA(cudaFree(bufs[i]));
+        }
+        DFB_CUDA(cudaDeviceSynchronize());
+        return true;
+    }
+
     int next_log_slot() {
         last_log_slot_ = pair_log_count_ % kPairLog;
         ++pair_log_count_;

@@ -436,6 +436,9 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   "farn_level_image"     in {frame (u8 values as floats)}  out {level image, level k size}; scalars {k}
  *   "farn_poly_exp"        in {level image}                  out {R0 .. R4}
  *   "farn_flow_init"       in {fx, fy of the coarser level}  out {fx, fy (scalars[0] x scalars[1])}; scalars {level w, level h}
+ *   "farn_initial_flow"    in {x, y of the initial flow}     out {fx, fy of the coarsest level}; scalars {step, pitch, pairs}
+ *     (use_initial_flow's level start: the start resized to the coarsest level of the handle's num_levels, times
+ *     pyrScale^k; step 2 uploads the start as a float2 field, step 1 as two planes, rows `pitch` floats apart, 0 = dense)
  *   "farn_update_matrices" in {fx, fy, R0 x 5 (frame a), R1 x 5 (frame b)}  out {M0 .. M4}; scalars {pairs}
  *   "farn_iteration"       in {M x 5, R0 x 5, R1 x 5}        out {fx, fy, M'0 .. M'4}; scalars {rebuild, pairs}
  *     (one box mean -> 2x2 solve -> rebuild of M iteration; M' is written only with rebuild = 1)
@@ -457,6 +460,11 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *                      (resize to the finer level, times 1 / scale_step)
  *   "tvl1_merge"       in {u1, u2}                         out {flow x, flow y} (bound 0) or {qx, qy} as floats; scalars {bound, lanes}
  *   "tvl1_median"      in {u1, u2}                         out {u1, u2} (their k x k median); scalars {k (3 or 5), lanes}
+ *   "tvl1_initial_flow" in {x, y of the initial flows}     out {u1, u2: every level, one after the other}; scalars {step,
+ *                      pitch, lanes}; use_initial_flow's start pyramid (the batched copy into each lane's level 0, then the
+ *                      resize x scale_step per level) at the handle's nscales / scale_step, on 1..64 lanes, with the start
+ *                      uploaded as a float2 field (step 2) or two planes (step 1), rows `pitch` floats apart (0 = dense);
+ *                      each level of an output holds the lanes' planes of that level stacked along the rows
  *   "jpeg_padded_gray" in {gray}                           out {the plane padded to round8(w) x round8(h)}
  *   "jpeg_padded_ycc420" in {B, G, R}                      out {Y round16(dw) x round16(dh), Cb, Cr round8(ceil(dw / 2)) x
  *                      round8(ceil(dh / 2))}; scalars {dst w, dst h} (0 / 0: no resize)

@@ -331,6 +331,15 @@ def iteration(M, R0, R1, fx_at=None, fy_at=None, ksize=13):
 
 def flow_init(pfx, pfy, lw, lh, pyr_scale=0.5):
     """level start: bilinear resize (CUDA convention) of the coarser flow to lw x lh, times (float)(1 / pyr_scale)"""
+    return level_start(pfx, pfy, lw, lh, 1.0 / pyr_scale)
+
+
+def level_start(pfx, pfy, lw, lh, mul):
+    """bilinear resize (CUDA convention) of a flow of any size to lw x lh, times the fp32 multiplier (float)mul: the upsample
+    between two levels (mul 1 / pyr_scale), or use_initial_flow's coarsest level from the full-resolution start (mul
+    pyr_scale^k)"""
+    m = np.float32(mul)
+    exact = np.frexp(m)[0] == 0.5  # a power of two scales without rounding
     out = []
     for P in (pfx, pfy):
         P = np.asarray(P, np.float32)
@@ -338,5 +347,6 @@ def flow_init(pfx, pfy, lw, lh, pyr_scale=0.5):
         sx, x1, xa, xb = _resize_coords(lw, pw, np.float32(1.0 / (lw / pw)))
         sy, y1, ya, yb = _resize_coords(lh, ph, np.float32(1.0 / (lh / ph)))
         b = [[E(P[np.ix_(r, c)]) for c in (xa, xb)] for r in (ya, yb)]
-        out.append(_bilinear4(b, sx[None, :], x1[None, :], sy[:, None], y1[:, None]).scale2(1.0 / pyr_scale).out())
+        o = _bilinear4(b, sx[None, :], x1[None, :], sy[:, None], y1[:, None])
+        out.append((o.scale2(float(m)) if exact else o * E(m)).out())
     return out

@@ -179,6 +179,26 @@ def numpy_calc(I0u8, I1u8, init=None, tau=0.25, lam=0.15, theta=0.3, nscales=5, 
     return np.stack([u1, u2], -1), log
 
 
+def farn_start(init, params=None):
+    """(fx, fy) of the coarsest Farneback level from the initial flow `init` ([H,W,2] float32): orc_resize_linear to that
+    level's size, times float(pyr_scale^k)"""
+    from oracle import pyoracle
+    L = pyoracle.lib()
+    p = params or pyoracle.farn_params()
+    h, w = init.shape[:2]
+    levels = pyoracle.farn_levels(w, h, p)
+    W, H = levels[0][:2]
+    scale = 1.0
+    for _ in range(len(levels) - 1):
+        scale *= p.pyr_scale
+    rfx, rfy = F(1.0 / (W / w)), F(1.0 / (H / h))
+    fx, fy = np.empty((H, W), F), np.empty((H, W), F)
+    ix, iy = _planes_of(init)
+    L.orc_resize_linear(ix, w, h, fx, W, H, rfx, rfy, p.resize_convention)
+    L.orc_resize_linear(iy, w, h, fy, W, H, rfx, rfy, p.resize_convention)
+    return (fx * F(scale)).astype(F), (fy * F(scale)).astype(F)
+
+
 def farn_calc(a, b, init=None, params=None):
     """orc_farn_calc from the C building blocks, the coarsest level starting from `init` ([H,W,2] float32, None = zero)"""
     from oracle import pyoracle
@@ -194,15 +214,7 @@ def farn_calc(a, b, init=None, params=None):
         if l == 0:
             fx, fy = np.zeros((H, W), F), np.zeros((H, W), F)
             if init is not None:
-                k = len(levels) - 1
-                scale = 1.0
-                for _ in range(k):
-                    scale *= p.pyr_scale
-                rfx, rfy = F(1.0 / (W / w)), F(1.0 / (H / h))
-                ix, iy = _planes_of(init)
-                L.orc_resize_linear(ix, w, h, fx, W, H, rfx, rfy, p.resize_convention)
-                L.orc_resize_linear(iy, w, h, fy, W, H, rfx, rfy, p.resize_convention)
-                fx, fy = (fx * F(scale)).astype(F), (fy * F(scale)).astype(F)
+                fx, fy = farn_start(init, p)
         else:
             pw, ph = fx.shape[1], fx.shape[0]
             rfx, rfy = F(1.0 / (W / pw)), F(1.0 / (H / ph))
