@@ -68,8 +68,7 @@ struct dfb_handle {
     Events ev_in, ev_pyr;     // [kFrameRing] frame uploaded, its pyramid built
     // pinned staging for pageable caller buffers (outputs: one per pair of the two groups in flight)
     PinnedBuffer<uint8_t> h_frame[kFrameRing];
-    PinnedBuffer<float> h_flow[2 * kMaxGroup];
-    PinnedBuffer<uint8_t> h_q[2 * kMaxGroup];
+    PinnedBuffer<uint8_t> h_out[2 * kMaxGroup];
     // the flow group loop (flow_groups): device outputs of two slots of B pairs, grown on demand, and per slot the events
     // that hand a solved group from s_compute to s_out and mark the slot free once its outputs are read back or encoded
     DeviceBuffer<uint8_t> flow_out;
@@ -137,8 +136,10 @@ void quiesce(dfb_handle *h) {
     cudaGetLastError();
 }
 
+// Runs f on the handle's device (h non-null); a CUDA error or an exception becomes the call's error code and message.
 template <typename F> int guarded(dfb_handle *h, F &&f) {
     try {
+        if (h) DFB_CUDA(cudaSetDevice(h->device));
         return f();
     } catch (const CudaError &e) {
         quiesce(h);
@@ -184,12 +185,81 @@ bool initial_flow(const dfb_handle *h) {
 int null_flow(dfb_handle *h, const std::string &what) {
     return fail(h, DFB_ERR_INVALID_ARG, initial_flow(h) ? what + ": use_initial_flow is set, so the flow buffer must hold the initial flow" : what);
 }
-// the calls without a float flow buffer have no initial flow to read: refused before anything is enqueued
-int refuse_initial_flow(dfb_handle *h) {
-    if (!initial_flow(h)) return DFB_OK;
+// Where the outputs of a host flow call go.  Pair j has k buffers, buf[c][j] (c < k): its float2 field, its x and y planes, or
+// its files, whose lengths go to len[c][j] and whose buffers hold `capacity` bytes each.
+struct FlowDest {
+    enum Kind { field, u8_planes, float_planes, jpeg_pair, png } kind;
+    int k;
+    void *const *buf[2];
+    size_t *len[2];
+    size_t capacity;
+    int bound, quality;  // u8_planes and jpeg_pair: the quantisation bound; jpeg_pair: the JPEG quality
+    // the float buffers also hold each pair's initial flow when use_initial_flow is set (the calc calls; the chains refuse it)
+    bool warm;
+    bool files() const { return kind == jpeg_pair || kind == png; }
+    // an output array is null
+    bool missing() const {
+        for (int c = 0; c < k; ++c)
+            if (!buf[c] || (files() && !len[c])) return true;
+        return false;
+    }
+};
+template <typename T> void *const *bytes_of(T *const *a) { return reinterpret_cast<void *const *>(a); }
+FlowDest field_dest(float *const *f) { return {FlowDest::field, 1, {bytes_of(f), nullptr}, {}, 0, 0, 0, true}; }
+FlowDest planes_dest(float *const *x, float *const *y, bool warm) {
+    return {FlowDest::float_planes, 2, {bytes_of(x), bytes_of(y)}, {}, 0, 0, 0, warm};
+}
+FlowDest u8_dest(int bound, uint8_t *const *x, uint8_t *const *y) {
+    return {FlowDest::u8_planes, 2, {bytes_of(x), bytes_of(y)}, {}, 0, bound, 0, false};
+}
+FlowDest png_dest(uint8_t *const *out, size_t capacity, size_t *len) {
+    return {FlowDest::png, 1, {bytes_of(out), nullptr}, {len, nullptr}, capacity, 0, 0, false};
+}
+FlowDest jpeg_dest(int bound, int quality, uint8_t *const *x, uint8_t *const *y, size_t capacity, size_t *len_x, size_t *len_y) {
+    return {FlowDest::jpeg_pair, 2, {bytes_of(x), bytes_of(y)}, {len_x, len_y}, capacity, bound, quality, false};
+}
+
+// the calls whose outputs hold no initial flow have none to read: refused before anything is enqueued
+int refuse_initial_flow(dfb_handle *h, const FlowDest &d) {
+    if (d.warm || !initial_flow(h)) return DFB_OK;
     return fail(h, DFB_ERR_INVALID_ARG,
                 "use_initial_flow is set: only the calls that take a float flow buffer (dfb_calc_device / _host / _batch_host / _batch_device "
                 "and their _planes forms) read an initial flow; set it to 0 for this call");
+}
+
+// Each of the M pairs' output buffers is present and host memory; `label` names them in the message.
+int check_pair_outputs(dfb_handle *h, int M, const FlowDest &d, const char *label) {
+    for (int j = 0; j < M; ++j)
+        for (int c = 0; c < d.k; ++c)
+            if (!d.buf[c][j] || host_pointer_kind(d.buf[c][j]) < 0)
+                return null_flow(h, std::string(label) + " " + std::to_string(j) + " is null or a device pointer (host entry point)");
+    return DFB_OK;
+}
+
+// Where the solve of pj writes its result: a float2 field with rows of `pitch` bytes, two float planes, or (bound > 0) two
+// uint8 planes.  With init, the same float buffers hold the pair's initial flow: the solve reads it before it writes.
+void bind_start(FlowAlgorithm::PairJob &pj, const float *x, const float *y, size_t pitch, int step) {
+    pj.init_x = x;
+    pj.init_y = y;
+    pj.init_pitch = pitch / sizeof(float);
+    pj.init_step = step;
+}
+void bind_field(FlowAlgorithm::PairJob &pj, float *f, size_t pitch, bool init) {
+    pj.flow_xy = f;
+    pj.flow_pitch_bytes = pitch;
+    if (init) bind_start(pj, f, f + 1, pitch, 2);
+}
+void bind_planes(FlowAlgorithm::PairJob &pj, float *x, float *y, size_t pitch, bool init) {
+    pj.fx = x;
+    pj.fy = y;
+    pj.f_pitch = pitch;
+    if (init) bind_start(pj, x, y, pitch, 1);
+}
+void bind_u8(FlowAlgorithm::PairJob &pj, uint8_t *x, uint8_t *y, size_t pitch, int bound) {
+    pj.bound = bound;
+    pj.qx = x;
+    pj.qy = y;
+    pj.q_pitch = pitch;
 }
 
 // pinned staging buffers exist only for callers that pass pageable memory: allocated on first use
@@ -197,13 +267,10 @@ uint8_t *stage_frame(dfb_handle *h, int r) {
     h->h_frame[r].allocate((size_t)h->max_w * h->max_h);
     return h->h_frame[r];
 }
-float *stage_flow(dfb_handle *h, int r) {
-    h->h_flow[r].allocate((size_t)h->max_w * h->max_h * 2 * sizeof(float));
-    return h->h_flow[r];
-}
-uint8_t *stage_q(dfb_handle *h, int r) {
-    h->h_q[r].allocate((size_t)h->max_w * h->max_h * 2);
-    return h->h_q[r];
+// output pair p's staging buffer, px_bytes per pixel of the handle's maximum frame
+uint8_t *stage_out(dfb_handle *h, int p, size_t px_bytes) {
+    h->h_out[p].allocate((size_t)h->max_w * h->max_h * px_bytes);
+    return h->h_out[p];
 }
 
 void ensure_streams(dfb_handle *h) {
@@ -485,153 +552,67 @@ struct FlowOutput {
     std::function<void(int slot, int m)> pack;                  // optional: s_compute work on the solved group
     std::function<void(int j0, int m, int slot)> send;          // s_out: the group's outputs leave the slot
     std::function<void(int j0, int m, int slot)> finish;        // host, a group later: the results to the caller
-    // optional (use_initial_flow): s_compute copy of pair j's initial flow into output pair p, bound as the solve's start
-    std::function<void(FlowAlgorithm::PairJob &, int j, int p)> load;
+    // optional (use_initial_flow): s_compute copy of pair j's initial flow into output pair p, which bind made the solve's start
+    std::function<void(int j, int p)> load;
 };
 
-// dfb_calc_host / dfb_calc_batch_host: pair j's float2 field to flows[j], straight into page-locked memory or through the
-// pair's pinned staging buffer, copied out once the slot has been read back.  px: pixels each pair's field reserves.
-FlowOutput host_flow_output(dfb_handle *h, float *const *flows, int B, int w, int hh, size_t px) {
-    const size_t bytes = (size_t)w * hh * 2 * sizeof(float);
-    h->flow_out.grow(2 * B * px * 2 * sizeof(float));
-    auto field = [=](int p) { return reinterpret_cast<float *>(h->flow_out + (size_t)p * px * 2 * sizeof(float)); };
+// FlowDest's field, float_planes and u8_planes: the k buffers of output pair p (px pixels of bpp bytes each) at
+// (p k + c) px bpp in the slots.  Pair j's buffers go to buf[c][j] straight into page-locked memory when all of them are,
+// else through the pair's pinned staging buffer, copied out once the slot has been read back.
+FlowOutput host_output(dfb_handle *h, const FlowDest &d, int B, int w, int hh, size_t px) {
+    const int k = d.k;
+    const size_t bpp = d.kind == FlowDest::field ? 2 * sizeof(float) : d.kind == FlowDest::float_planes ? sizeof(float) : 1;
+    const size_t bytes = (size_t)w * hh * bpp, row = (size_t)w * bpp;  // one buffer of a pair
+    h->flow_out.grow(2 * B * k * px * bpp);
+    auto slot_buf = [=](int p, int c) { return h->flow_out + ((size_t)p * k + c) * px * bpp; };
+    auto direct = [=](int j) {
+        for (int c = 0; c < k; ++c)
+            if (!is_pinned_host(d.buf[c][j])) return false;
+        return true;
+    };
+    const bool init = d.warm && initial_flow(h);
     FlowOutput o;
     o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
-        pj.flow_xy = field(p);
-        pj.flow_pitch_bytes = (size_t)w * 2 * sizeof(float);
+        float *x = reinterpret_cast<float *>(slot_buf(p, 0)), *y = reinterpret_cast<float *>(slot_buf(p, 1));
+        if (d.kind == FlowDest::field) bind_field(pj, x, row, init);
+        else if (d.kind == FlowDest::float_planes) bind_planes(pj, x, y, row, init);
+        else bind_u8(pj, slot_buf(p, 0), slot_buf(p, 1), row, d.bound);
     };
     o.send = [=](int j0, int m, int slot) {
         for (int i = 0; i < m; ++i) {
             const int j = j0 + i, p = slot * B + i;
-            float *dst = is_pinned_host(flows[j]) ? flows[j] : stage_flow(h, p);
-            DFB_CUDA(cudaMemcpyAsync(dst, field(p), bytes, cudaMemcpyDeviceToHost, h->s_out));
-            h->counters.d2h_bytes += bytes;
+            const bool dir = direct(j);
+            for (int c = 0; c < k; ++c) {
+                void *dst = dir ? d.buf[c][j] : stage_out(h, p, k * bpp) + c * bytes;
+                DFB_CUDA(cudaMemcpyAsync(dst, slot_buf(p, c), bytes, cudaMemcpyDeviceToHost, h->s_out));
+            }
+            h->counters.d2h_bytes += k * bytes;
         }
     };
     o.finish = [=](int j0, int m, int slot) {
         for (int i = 0; i < m; ++i)
-            if (!is_pinned_host(flows[j0 + i])) {
+            if (!direct(j0 + i)) {
                 DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
-                std::memcpy(flows[j0 + i], h->h_flow[slot * B + i], bytes);
+                for (int c = 0; c < k; ++c) std::memcpy(d.buf[c][j0 + i], h->h_out[slot * B + i] + c * bytes, bytes);
             }
     };
     // the pair's staging buffer is free: the read-back of the group that last used this slot has been copied out (finish)
-    if (initial_flow(h))
-        o.load = [=](FlowAlgorithm::PairJob &pj, int j, int p) {
-            const float *src = flows[j];
-            if (!is_pinned_host(src)) src = static_cast<float *>(std::memcpy(stage_flow(h, p), src, bytes));
-            DFB_CUDA(cudaMemcpyAsync(field(p), src, bytes, cudaMemcpyHostToDevice, h->s_compute));
-            h->counters.h2d_bytes += bytes;
-            pj.init_x = field(p);
-            pj.init_y = field(p) + 1;
-            pj.init_pitch = (size_t)w * 2;
-            pj.init_step = 2;
+    if (init)
+        o.load = [=](int j, int p) {
+            const bool dir = direct(j);
+            for (int c = 0; c < k; ++c) {
+                const void *src = d.buf[c][j];
+                if (!dir) src = std::memcpy(stage_out(h, p, k * bpp) + c * bytes, src, bytes);
+                DFB_CUDA(cudaMemcpyAsync(slot_buf(p, c), src, bytes, cudaMemcpyHostToDevice, h->s_compute));
+            }
+            h->counters.h2d_bytes += k * bytes;
         };
     return o;
 }
 
-// dfb_calc_batch_host_u8: the engine's merge epilogue writes pair j's two uint8 planes (bound), which go to qx[j] / qy[j] as
-// the float2 fields go to flows[j] above.  flow_xy stays null: the engines keep the field in scratch of their own.
-FlowOutput host_u8_output(dfb_handle *h, uint8_t *const *qx, uint8_t *const *qy, int bound, int B, int w, int hh, size_t px) {
-    const size_t bytes = (size_t)w * hh;
-    h->flow_out.grow(2 * B * px * 2);
-    auto plane = [=](int p, int c) { return h->flow_out + ((size_t)p * 2 + c) * px; };
-    auto direct = [=](int j) { return is_pinned_host(qx[j]) && is_pinned_host(qy[j]); };
-    FlowOutput o;
-    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
-        pj.bound = bound;
-        pj.qx = plane(p, 0);
-        pj.qy = plane(p, 1);
-        pj.q_pitch = (size_t)w;
-    };
-    o.send = [=](int j0, int m, int slot) {
-        for (int i = 0; i < m; ++i) {
-            const int j = j0 + i, p = slot * B + i;
-            const bool d = direct(j);
-            uint8_t *dx = d ? qx[j] : stage_q(h, p), *dy = d ? qy[j] : stage_q(h, p) + bytes;
-            DFB_CUDA(cudaMemcpyAsync(dx, plane(p, 0), bytes, cudaMemcpyDeviceToHost, h->s_out));
-            DFB_CUDA(cudaMemcpyAsync(dy, plane(p, 1), bytes, cudaMemcpyDeviceToHost, h->s_out));
-            h->counters.d2h_bytes += 2 * bytes;
-        }
-    };
-    o.finish = [=](int j0, int m, int slot) {
-        for (int i = 0; i < m; ++i)
-            if (!direct(j0 + i)) {
-                DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
-                std::memcpy(qx[j0 + i], h->h_q[slot * B + i], bytes);
-                std::memcpy(qy[j0 + i], h->h_q[slot * B + i] + bytes, bytes);
-            }
-    };
-    return o;
-}
-
-// Where the two float planes of each pair go (-st=h5 payloads): pair j's x plane to x[j], its y plane to y[j], w x h floats each
-struct PlanesOut {
-    float *const *x, *const *y;
-};
-
-// dfb_calc_batch_host_planes and the _planes chains: the engine's merge epilogue writes pair j's u1 / u2 as two dense float
-// planes, which go to x[j] / y[j] as the float2 fields go to flows[j] above (pinned: a direct DMA, else through the pair's
-// pinned staging buffer).  px: pixels each plane reserves.
-FlowOutput planes_output(dfb_handle *h, const PlanesOut &po, int B, int w, int hh, size_t px) {
-    const size_t bytes = (size_t)w * hh * sizeof(float);
-    h->flow_out.grow(2 * B * px * 2 * sizeof(float));
-    auto plane = [=](int p, int c) { return reinterpret_cast<float *>(h->flow_out + ((size_t)p * 2 + c) * px * sizeof(float)); };
-    auto direct = [=](int j) { return is_pinned_host(po.x[j]) && is_pinned_host(po.y[j]); };
-    FlowOutput o;
-    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
-        pj.fx = plane(p, 0);
-        pj.fy = plane(p, 1);
-        pj.f_pitch = (size_t)w * sizeof(float);
-    };
-    o.send = [=](int j0, int m, int slot) {
-        for (int i = 0; i < m; ++i) {
-            const int j = j0 + i, p = slot * B + i;
-            const bool d = direct(j);
-            float *dx = d ? po.x[j] : stage_flow(h, p), *dy = d ? po.y[j] : stage_flow(h, p) + (size_t)w * hh;
-            DFB_CUDA(cudaMemcpyAsync(dx, plane(p, 0), bytes, cudaMemcpyDeviceToHost, h->s_out));
-            DFB_CUDA(cudaMemcpyAsync(dy, plane(p, 1), bytes, cudaMemcpyDeviceToHost, h->s_out));
-            h->counters.d2h_bytes += 2 * bytes;
-        }
-    };
-    o.finish = [=](int j0, int m, int slot) {
-        for (int i = 0; i < m; ++i)
-            if (!direct(j0 + i)) {
-                DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
-                std::memcpy(po.x[j0 + i], h->h_flow[slot * B + i], bytes);
-                std::memcpy(po.y[j0 + i], h->h_flow[slot * B + i] + (size_t)w * hh, bytes);
-            }
-    };
-    if (initial_flow(h))  // as in host_flow_output
-        o.load = [=](FlowAlgorithm::PairJob &pj, int j, int p) {
-            const float *sx = po.x[j], *sy = po.y[j];
-            if (!direct(j)) {
-                float *st = stage_flow(h, p);
-                sx = static_cast<float *>(std::memcpy(st, sx, bytes));
-                sy = static_cast<float *>(std::memcpy(st + (size_t)w * hh, sy, bytes));
-            }
-            DFB_CUDA(cudaMemcpyAsync(plane(p, 0), sx, bytes, cudaMemcpyHostToDevice, h->s_compute));
-            DFB_CUDA(cudaMemcpyAsync(plane(p, 1), sy, bytes, cudaMemcpyHostToDevice, h->s_compute));
-            h->counters.h2d_bytes += 2 * bytes;
-            pj.init_x = plane(p, 0);
-            pj.init_y = plane(p, 1);
-            pj.init_pitch = (size_t)w;
-            pj.init_step = 1;
-        };
-    return o;
-}
-
-// -st=jpg output of a flow chain: pair j's two quantised planes (bound) as JPEGs to x[j] / y[j], their lengths to len_x[j] /
-// len_y[j]; every buffer holds `capacity` bytes
-struct JpgOut {
-    int bound, quality;
-    uint8_t *const *x, *const *y;
-    size_t capacity;
-    size_t *len_x, *len_y;
-};
-
-// The planes of JpgOut, encoded on s_out as one batch per group (src/common.cpp:56-57) and read back on s_fetch
-FlowOutput jpg_output(dfb_handle *h, const JpgOut &jo, int B, int w, int hh) {
+// FlowDest's jpeg_pair (-st=jpg of a flow chain): pair j's two quantised planes as JPEGs, encoded on s_out as one batch per group
+// (src/common.cpp:56-57) and read back on s_fetch
+FlowOutput jpg_output(dfb_handle *h, const FlowDest &d, int B, int w, int hh) {
     // quantised planes: whole 8 x 8 blocks, so nvJPEG reads their edge padding (written by launch_pad_edges) and nothing else
     const int qw = round_up(w, 8), qh = round_up(hh, 8);
     const size_t qpx = (size_t)qw * qh;
@@ -639,10 +620,8 @@ FlowOutput jpg_output(dfb_handle *h, const JpgOut &jo, int B, int w, int hh) {
     auto sink = std::make_shared<JpegSink>(h, 2 * B, 2);
     FlowOutput o;
     o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
-        pj.bound = jo.bound;
-        pj.qx = h->flow_out + (size_t)p * 2 * qpx;
-        pj.qy = pj.qx + qpx;
-        pj.q_pitch = (size_t)qw;
+        uint8_t *x = h->flow_out + (size_t)p * 2 * qpx;
+        bind_u8(pj, x, x + qpx, (size_t)qw, d.bound);
     };
     o.send = [=](int, int m, int slot) {
         // the group's 2 m planes: plane 2 i + c of the slot is pair i's x (c = 0) or y
@@ -654,35 +633,27 @@ FlowOutput jpg_output(dfb_handle *h, const JpgOut &jo, int B, int w, int hh) {
             launch_pad_edges(const_cast<uint8_t *>(src.base), src.pitch, src.img_stride, 2 * m, w, hh, qw, qh, h->s_out);
             ++h->alg->launches;
         }
-        sink->encode(slot, 2 * m, src, 1, w, hh, jo.quality, jo.capacity, h->s_out);
+        sink->encode(slot, 2 * m, src, 1, w, hh, d.quality, d.capacity, h->s_out);
     };
     o.finish = [=](int j0, int m, int slot) {
         DFB_CUDA(cudaEventSynchronize(h->flow_ev.freed[slot]));
         auto too_small = [&](int, size_t need) {
-            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(jo.capacity) + ")";
+            return "jpeg output buffer too small (" + std::to_string(need) + " > " + std::to_string(d.capacity) + ")";
         };
         auto out = [&](int k, size_t len) {
             const int j = j0 + (k >> 1);
-            (k & 1 ? jo.len_y : jo.len_x)[j] = len;
-            return (k & 1 ? jo.y : jo.x)[j];
+            d.len[k & 1][j] = len;
+            return static_cast<uint8_t *>(d.buf[k & 1][j]);
         };
         sink->deliver(slot, 2 * m, too_small, out, h->s_fetch);
     };
     return o;
 }
 
-// -st=png output of a flow batch (the -st=png branch of encode_save): pair j's file goes to out[j], its length to len[j];
-// every buffer holds `capacity` bytes
-struct PngOut {
-    uint8_t *const *out;
-    size_t capacity;
-    size_t *len;
-};
-
-// The files of PngOut: the flow fields in the slot, convertFlowToPngImage (src/common.cpp:18-46) of each on s_compute,
-// imencode(".png") (:66-71) of the group as one batch into encoder slot `slot` on s_out, read back on s_fetch.  px: pixels
-// each pair's field reserves.
-FlowOutput png_output(dfb_handle *h, const PngOut &po, int B, int w, int hh, size_t px) {
+// FlowDest's png (the -st=png branch of encode_save): the flow fields in the slot, convertFlowToPngImage (src/common.cpp:18-46)
+// of each on s_compute, imencode(".png") (:66-71) of the group as one batch into encoder slot `slot` on s_out, read back on
+// s_fetch.  px: pixels each pair's field reserves.
+FlowOutput png_output(dfb_handle *h, const FlowDest &d, int B, int w, int hh, size_t px) {
     const size_t img = (size_t)3 * w * hh;
     h->flow_out.grow(2 * B * px * 2 * sizeof(float));
     h->png_bgr.grow(2 * B * img);
@@ -690,10 +661,7 @@ FlowOutput png_output(dfb_handle *h, const PngOut &po, int B, int w, int hh, siz
     if (!h->png) h->png.reset(new PngEncoder());
     auto field = [=](int p) { return reinterpret_cast<float *>(h->flow_out + (size_t)p * px * 2 * sizeof(float)); };
     FlowOutput o;
-    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) {
-        pj.flow_xy = field(p);
-        pj.flow_pitch_bytes = (size_t)w * 2 * sizeof(float);
-    };
+    o.bind = [=](FlowAlgorithm::PairJob &pj, int p) { bind_field(pj, field(p), (size_t)w * 2 * sizeof(float), false); };
     o.pack = [=](int slot, int m) {
         for (int p = slot * B; p < slot * B + m; ++p)
             launch_flow_to_png_image(field(p), (size_t)w * 8, w, hh, h->png_bgr + p * img, (size_t)w * 3, h->png_scratch, nullptr, h->s_compute);
@@ -707,15 +675,22 @@ FlowOutput png_output(dfb_handle *h, const PngOut &po, int B, int w, int hh, siz
         auto reject = [&](int i, uint64_t n) {
             if (n == 0) return "png encoder failed on pair " + std::to_string(j0 + i);
             return "png output buffer too small: pair " + std::to_string(j0 + i) + " needs " + std::to_string(n) + " bytes, capacity is " +
-                   std::to_string(po.capacity);
+                   std::to_string(d.capacity);
         };
         auto to = [&](int i, size_t n) {
-            po.len[j0 + i] = n;
-            return po.out[j0 + i];
+            d.len[0][j0 + i] = n;
+            return static_cast<uint8_t *>(d.buf[0][j0 + i]);
         };
-        h->png->files().deliver(slot, m, po.capacity, reject, to, h->counters.d2h_bytes, h->s_fetch);
+        h->png->files().deliver(slot, m, d.capacity, reject, to, h->counters.d2h_bytes, h->s_fetch);
     };
     return o;
+}
+
+// The output of d for groups of B pairs of w x hh, each pair's field or planes reserving px pixels of the slots
+FlowOutput flow_output(dfb_handle *h, const FlowDest &d, int B, int w, int hh, size_t px) {
+    if (d.kind == FlowDest::png) return png_output(h, d, B, w, hh, px);
+    if (d.kind == FlowDest::jpeg_pair) return jpg_output(h, d, B, w, hh);
+    return host_output(h, d, B, w, hh, px);
 }
 
 // The batch shape of calc_optflows_imp (src/denseflow_gpu.cpp:307-342): the M = n_frames - |step| pairs in groups of B on
@@ -746,7 +721,7 @@ int flow_groups(dfb_handle *h, int n_frames, int step, int w, int hh, int B, con
         for (int i = 0; i < m; ++i) {
             jobs[i] = pair_job(j0 + i, step, nslots);
             o.bind(jobs[i], slot * B + i);
-            if (o.load) o.load(jobs[i], j0 + i, slot * B + i);
+            if (o.load) o.load(j0 + i, slot * B + i);
         }
         alg.solve_batch(jobs.data(), m, w, hh, h->s_compute);
         if (o.pack) o.pack(slot, m);
@@ -764,12 +739,8 @@ int flow_groups(dfb_handle *h, int n_frames, int step, int w, int hh, int B, con
     return DFB_OK;
 }
 
-// The calc calls over host buffers.
-// quantise: bound > 0 => emit two u8 planes per pair instead of the float2 field.
-// png: non-null => pack every flow field (convertFlowToPngImage) and emit imencode(".png") of it instead of the field.
-// planes: non-null => emit the two float planes of every pair instead of the field.
-int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, float *const *flows,
-               int bound, uint8_t *const *qx, uint8_t *const *qy, const PngOut *png = nullptr, const PlanesOut *planes = nullptr) {
+// The calc calls over host buffers: the pairs' outputs go where d says.  Runs inside guarded().
+int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, const FlowDest &d) {
     if (int rc = check_size(h, w, hh)) return rc;
     if (n_frames < 0 || !frames) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
@@ -778,24 +749,22 @@ int batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int st
     for (int f = 0; f < n_frames; ++f)
         if (!frames[f] || host_pointer_kind(frames[f]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "frames[" + std::to_string(f) + "] is null or a device pointer (host entry point: use dfb_calc_batch_device)");
-    for (int j = 0; j < M; ++j) {
-        const void *o0 = png      ? (const void *)png->out[j]
-                         : bound > 0 ? (const void *)qx[j]
-                         : planes    ? (const void *)planes->x[j]
-                                     : (const void *)flows[j];
-        const void *o1 = bound > 0 ? (const void *)qy[j] : planes ? (const void *)planes->y[j] : o0;
-        if (!o0 || !o1 || host_pointer_kind(o0) < 0 || host_pointer_kind(o1) < 0)
-            return null_flow(h, "output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-    }
+    if (int rc = check_pair_outputs(h, M, d, "output")) return rc;
     const int B = std::max(1, std::min(h->alg->max_concurrent_pairs(w, hh), dfb_handle::kMaxGroup));
     // output slots at the handle's maximum frame, so that calls of other sizes reuse them (a 1080p handle runs 7 pairs per
     // group, a 340x256 one up to 64)
     const size_t px = (size_t)h->max_w * h->max_h;
-    const FlowOutput o = png         ? png_output(h, *png, B, w, hh, px)
-                         : bound > 0 ? host_u8_output(h, qx, qy, bound, B, w, hh, px)
-                         : planes    ? planes_output(h, *planes, B, w, hh, px)
-                                     : host_flow_output(h, flows, B, w, hh, px);
-    return flow_groups(h, n_frames, step, w, hh, B, upload_ring(h, frames, n_frames, w, hh), o);
+    return flow_groups(h, n_frames, step, w, hh, B, upload_ring(h, frames, n_frames, w, hh), flow_output(h, d, B, w, hh, px));
+}
+
+// dfb_calc_batch_host[_u8|_planes|_png]: the checks of the output arrays (`missing`: the message when one is null), then the call
+int calc_batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int w, int hh, const FlowDest &d,
+                    const char *missing) {
+    if (!h) return DFB_ERR_INVALID_ARG;
+    if (int rc = refuse_initial_flow(h, d)) return rc;
+    if (d.kind == FlowDest::u8_planes && d.bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");  // check_param, src/denseflow_gpu.cpp:15-18
+    if (n_frames > std::abs(step) && d.missing()) return null_flow(h, missing);
+    return guarded(h, [&]() { return batch_host(h, frames, n_frames, step, w, hh, d); });
 }
 
 }  // namespace
@@ -898,18 +867,12 @@ int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8
     if ((reinterpret_cast<uintptr_t>(flow_xy) | flow_pitch) & 7)
         return fail(h, DFB_ERR_INVALID_ARG, "flow_xy and flow_pitch must be 8-byte aligned (CV_32FC2 rows)");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         h->alg->begin_batch();
         h->alg->prepare_frame(a, a_pitch, width, height, 0, s);
         h->alg->prepare_frame(b, b_pitch, width, height, 1, s);
-        FlowAlgorithm::PairJob pj{0, 1, flow_xy, flow_pitch};
-        if (initial_flow(h)) {  // read on s before the solve writes the field
-            pj.init_x = flow_xy;
-            pj.init_y = flow_xy + 1;
-            pj.init_pitch = flow_pitch / sizeof(float);
-            pj.init_step = 2;
-        }
+        FlowAlgorithm::PairJob pj{0, 1};
+        bind_field(pj, flow_xy, flow_pitch, initial_flow(h));  // the start is read on s before the solve writes the field
         h->alg->solve_batch(&pj, 1, width, height, s);
         ++h->counters.pairs;
         return DFB_OK;
@@ -922,43 +885,27 @@ int dfb_calc_host(dfb_handle *h, const uint8_t *a, const uint8_t *b, int width, 
     if (!a || !b) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     const uint8_t *frames[2] = {a, b};
     float *flows[1] = {flow_xy};
-    return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
-        return batch_host(h, frames, 2, 1, width, height, flows, 0, nullptr, nullptr);
-    });
+    return guarded(h, [&]() { return batch_host(h, frames, 2, 1, width, height, field_dest(flows)); });
 }
 
 int dfb_calc_batch_host(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                         float *const *flows) {
-    if (!h) return DFB_ERR_INVALID_ARG;
-    if (n_frames > std::abs(step) && !flows) return null_flow(h, "flows is null");
-    return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
-        return batch_host(h, frames, n_frames, step, width, height, flows, 0, nullptr, nullptr);
-    });
+    return calc_batch_host(h, frames, n_frames, step, width, height, field_dest(flows), "flows is null");
 }
 
 int dfb_calc_batch_host_u8(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                            int bound, uint8_t *const *qx, uint8_t *const *qy) {
-    if (!h) return DFB_ERR_INVALID_ARG;
-    if (int rc = refuse_initial_flow(h)) return rc;
-    if (bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");  // check_param, src/denseflow_gpu.cpp:15-18
-    if (n_frames > std::abs(step) && (!qx || !qy)) return fail(h, DFB_ERR_INVALID_ARG, "qx/qy is null");
-    return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
-        return batch_host(h, frames, n_frames, step, width, height, nullptr, bound, qx, qy);
-    });
+    return calc_batch_host(h, frames, n_frames, step, width, height, u8_dest(bound, qx, qy), "qx/qy is null");
 }
 
 int dfb_calc_batch_host_planes(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height,
                                float *const *fx, float *const *fy) {
-    if (!h) return DFB_ERR_INVALID_ARG;
-    if (n_frames > std::abs(step) && (!fx || !fy)) return null_flow(h, "fx/fy is null");
-    const PlanesOut planes{fx, fy};
-    return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
-        return batch_host(h, frames, n_frames, step, width, height, nullptr, 0, nullptr, nullptr, nullptr, &planes);
-    });
+    return calc_batch_host(h, frames, n_frames, step, width, height, planes_dest(fx, fy, true), "fx/fy is null");
+}
+
+int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height, uint8_t *const *png,
+                            size_t capacity, size_t *len) {
+    return calc_batch_host(h, frames, n_frames, step, width, height, png_dest(png, capacity, len), "png / len is null");
 }
 
 }  // extern "C"
@@ -979,7 +926,6 @@ int batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, i
     if (!frames) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     const bool init = initial_flow(h);
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         FlowAlgorithm &alg = *h->alg;
         alg.begin_batch();
@@ -995,21 +941,9 @@ int batch_device(dfb_handle *h, const uint8_t *frames, int n_frames, int step, i
             for (int i = 0; i < m; ++i) {
                 const int j = j0 + i;
                 jobs[i] = pair_job(j, step, nslots);
-                float *out = flows + (size_t)j * fbytes * 2;
-                if (planar) {
-                    jobs[i].fx = out;
-                    jobs[i].fy = out + fbytes;
-                    jobs[i].f_pitch = (size_t)width * 4;
-                } else {
-                    jobs[i].flow_xy = out;
-                    jobs[i].flow_pitch_bytes = (size_t)width * 8;
-                }
-                if (init) {  // the pair's output holds its initial flow: the solve reads it before writing the result
-                    jobs[i].init_x = out;
-                    jobs[i].init_y = planar ? out + fbytes : out + 1;
-                    jobs[i].init_pitch = planar ? (size_t)width : (size_t)width * 2;
-                    jobs[i].init_step = planar ? 1 : 2;
-                }
+                float *out = flows + (size_t)j * fbytes * 2;  // with init it holds the pair's initial flow
+                if (planar) bind_planes(jobs[i], out, out + fbytes, (size_t)width * sizeof(float), init);
+                else bind_field(jobs[i], out, (size_t)width * 2 * sizeof(float), init);
             }
             alg.solve_batch(jobs.data(), m, width, height, s);
             h->counters.pairs += m;
@@ -1042,7 +976,6 @@ int dfb_quantise_device(dfb_handle *h, const float *flow_xy, size_t flow_pitch, 
     if ((reinterpret_cast<uintptr_t>(flow_xy) | flow_pitch) & 7)
         return fail(h, DFB_ERR_INVALID_ARG, "flow_xy and flow_pitch must be 8-byte aligned (CV_32FC2 rows)");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         launch_quantise(flow_xy, flow_pitch, width, height, bound, qx, qy, q_pitch, static_cast<cudaStream_t>(stream));
         ++h->alg->launches;
         return DFB_OK;
@@ -1058,7 +991,6 @@ int dfb_flow_to_png_image_device(dfb_handle *h, const float *flow_xy, size_t flo
     if ((reinterpret_cast<uintptr_t>(flow_xy) | flow_pitch) & 7)
         return fail(h, DFB_ERR_INVALID_ARG, "flow_xy and flow_pitch must be 8-byte aligned (CV_32FC2 rows)");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         ensure_png_scratch(h);
         PngBounds *bd = nullptr;
@@ -1082,7 +1014,6 @@ int dfb_bgr_to_gray_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch, 
     if (width <= 0 || height <= 0 || bgr_pitch < (size_t)width * 3 || gray_pitch < (size_t)width)
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         launch_bgr_to_gray(bgr, bgr_pitch, width, height, gray, gray_pitch, static_cast<cudaStream_t>(stream));
         ++h->alg->launches;
         return DFB_OK;
@@ -1096,7 +1027,6 @@ int dfb_resize_gray_device(dfb_handle *h, const uint8_t *src, size_t src_pitch, 
     if (sw <= 0 || sh <= 0 || dw <= 0 || dh <= 0 || src_pitch < (size_t)sw || dst_pitch < (size_t)dw)
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         resize_gray(h, src, src_pitch, sw, sh, dst, dst_pitch, dw, dh, static_cast<cudaStream_t>(stream));
         return DFB_OK;
     });
@@ -1114,7 +1044,6 @@ int dfb_encode_jpeg_gray_device(dfb_handle *h, const uint8_t *gray, size_t gray_
     if (width <= 0 || height <= 0 || gray_pitch < (size_t)width || quality < 1 || quality > 100)
         return fail(h, DFB_ERR_INVALID_ARG, "bad geometry or quality");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         JpegSink sink(h, 1, 1);
         JpegSrc src;
@@ -1160,7 +1089,6 @@ int dfb_encode_jpeg_gray_batch_device(dfb_handle *h, const uint8_t *planes, size
         if (!out[i] || host_pointer_kind(out[i]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(i) + " is null or a device pointer (host entry point)");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         JpegSink sink(h, n, 1, true);
         JpegSrc src;
@@ -1186,7 +1114,6 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
     if (!h) return DFB_ERR_INVALID_ARG;
     if (!jpeg || !jpeg_len || !gray || !width || !height) return fail(h, DFB_ERR_INVALID_ARG, "null buffer");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         if (!h->jpeg) h->jpeg.reset(new JpegEncoder());
         int w = 0, hh = 0, nc = 0;
@@ -1209,44 +1136,12 @@ int dfb_decode_jpeg_gray_device(dfb_handle *h, const uint8_t *jpeg, size_t jpeg_
 
 namespace {
 
-// Where the outputs of a flow chain go: exactly one of the three is set.
-struct ChainOut {
-    const JpgOut *jpg;
-    const PngOut *png;
-    const PlanesOut *planes = nullptr;
-};
-
-bool chain_outputs_null(const ChainOut &o) {
-    if (o.planes) return !o.planes->x || !o.planes->y;
-    return o.png ? (!o.png->out || !o.png->len) : (!o.jpg->x || !o.jpg->y || !o.jpg->len_x || !o.jpg->len_y);
-}
-
-// Output-argument checks shared by the flow chains below.
-int check_chain_outputs(dfb_handle *h, int M, const ChainOut &o) {
-    if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
-    for (int j = 0; j < M; ++j) {
-        if (o.planes) {
-            if (!o.planes->x[j] || !o.planes->y[j] || host_pointer_kind(o.planes->x[j]) < 0 || host_pointer_kind(o.planes->y[j]) < 0)
-                return fail(h, DFB_ERR_INVALID_ARG, "plane output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-        } else if (o.png) {
-            if (!o.png->out[j] || host_pointer_kind(o.png->out[j]) < 0)
-                return fail(h, DFB_ERR_INVALID_ARG, "png output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-        } else if (!o.jpg->x[j] || !o.jpg->y[j] || host_pointer_kind(o.jpg->x[j]) < 0 || host_pointer_kind(o.jpg->y[j]) < 0) {
-            return fail(h, DFB_ERR_INVALID_ARG, "jpeg output " + std::to_string(j) + " is null or a device pointer (host entry point)");
-        }
-    }
-    return DFB_OK;
-}
-
 // The per-batch chain after decode: gray frames (sw x sh, resized to dw x dh) by `produce` (dense_frames) -> flow -> the
-// output of `o`: quantise and two JPEGs per pair, convertFlowToPngImage and one PNG per pair, or the two float planes of each
+// output of `d`: quantise and two JPEGs per pair, convertFlowToPngImage and one PNG per pair, or the two float planes of each
 // pair.  Runs inside guarded().
-int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const ChainOut &o, const std::function<void(int, int)> &produce) {
+int process_chain(dfb_handle *h, int n_frames, int step, int dw, int dh, const FlowDest &d, const std::function<void(int, int)> &produce) {
     const int B = std::max(1, std::min(h->alg->max_concurrent_pairs(dw, dh), 8));
-    const FlowOutput out = o.planes ? planes_output(h, *o.planes, B, dw, dh, (size_t)dw * dh)
-                           : o.png  ? png_output(h, *o.png, B, dw, dh, (size_t)dw * dh)
-                                    : jpg_output(h, *o.jpg, B, dw, dh);
-    return flow_groups(h, n_frames, step, dw, dh, B, dense_frames(h, n_frames, dw, dh, produce), out);
+    return flow_groups(h, n_frames, step, dw, dh, B, dense_frames(h, n_frames, dw, dh, produce), flow_output(h, d, B, dw, dh, (size_t)dw * dh));
 }
 
 // Every file of a JPEG batch parsed on the host; an unsupported or corrupt header is the call's error.
@@ -1279,30 +1174,32 @@ int parse_jpegs_one_size(dfb_handle *h, const uint8_t *const *jpeg, const size_t
     return DFB_OK;
 }
 
-// The checks both flow chains make first, in this order: the frame array, step, bound, the requested size (0 / 0: none).
-int check_chain_args(dfb_handle *h, bool frames_null, int n_frames, int step, const ChainOut &o, int dw, int dh) {
+// The checks both flow chains make first, in this order: use_initial_flow, the frame array, step, bound, the requested size
+// (0 / 0: none).
+int check_chain_args(dfb_handle *h, bool frames_null, int n_frames, int step, const FlowDest &d, int dw, int dh) {
+    if (int rc = refuse_initial_flow(h, d)) return rc;
     if (frames_null || n_frames < 0) return fail(h, DFB_ERR_INVALID_ARG, "frames is null");
     if (step == 0) return fail(h, DFB_ERR_INVALID_ARG, "step must be non-zero for flow extraction");
-    if (o.jpg && o.jpg->bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
+    if (d.kind == FlowDest::jpeg_pair && d.bound <= 0) return fail(h, DFB_ERR_INVALID_ARG, "bound should > 0!");
     if (dw < 0 || dh < 0 || (dw == 0) != (dh == 0)) return fail(h, DFB_ERR_INVALID_ARG, "bad geometry");
     return DFB_OK;
 }
 
-// dfb_process_bgr_batch_host[_png]: the checks, then the chain with decoded BGR frames as its source
-int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh, const ChainOut &o) {
+// dfb_process_bgr_batch_host[_png|_planes]: the checks, then the chain with decoded BGR frames as its source; `label` names the
+// pairs' outputs in the messages
+int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh, const FlowDest &d,
+              const char *label) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (int rc = refuse_initial_flow(h)) return rc;
-    if (int rc = check_chain_args(h, !bgr, n_frames, step, o, dw, dh)) return rc;
+    if (int rc = check_chain_args(h, !bgr, n_frames, step, d, dw, dh)) return rc;
     if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
-    if (chain_outputs_null(o)) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    if (d.missing()) return fail(h, DFB_ERR_INVALID_ARG, "null output");
     for (int f = 0; f < n_frames; ++f)
         if (!bgr[f] || host_pointer_kind(bgr[f]) < 0)
             return fail(h, DFB_ERR_INVALID_ARG, "bgr[" + std::to_string(f) + "] is null or a device pointer (host entry point)");
-    if (int rc = check_chain_outputs(h, M, o)) return rc;
+    if (int rc = check_pair_outputs(h, M, d, label)) return rc;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         // frame source: H2D of BGR frame f into staging buffer f & 1 -> cvtColor -> resize (decode stage tail, :163-170)
         const size_t fpx = (size_t)dw * dh, bgr_bytes = (size_t)sw * sh * 3;
         h->pb_bgr.grow(2 * bgr_bytes);  // two staging frames: H2D of f+1 overlaps gray/resize of f
@@ -1328,24 +1225,24 @@ int bgr_chain(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, 
                 DFB_CUDA(cudaEventRecord(ev.frame[f], h->s_in));
             }
         };
-        return process_chain(h, n_frames, step, dw, dh, o, produce);
+        return process_chain(h, n_frames, step, dw, dh, d, produce);
     });
 }
 
-// dfb_process_jpeg_batch_host[_png]: the checks, then the chain with JPEG files decoded on the device as its source
-int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh, const ChainOut &o) {
+// dfb_process_jpeg_batch_host[_png|_planes]: the checks, then the chain with JPEG files decoded on the device as its source
+int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh, const FlowDest &d,
+               const char *label) {
     if (!h) return DFB_ERR_INVALID_ARG;
-    if (int rc = refuse_initial_flow(h)) return rc;
-    if (int rc = check_chain_args(h, !jpeg || !len, n_frames, step, o, dw, dh)) return rc;
+    if (int rc = check_chain_args(h, !jpeg || !len, n_frames, step, d, dw, dh)) return rc;
     const int M = std::max(n_frames - std::abs(step), 0);
     if (M == 0) return DFB_OK;
     std::vector<JpegHeader> hd;
     int sw = 0, sh = 0;
     if (int rc = parse_jpegs_one_size(h, jpeg, len, n_frames, hd, sw, sh)) return rc;
     if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
-    if (int rc = check_chain_outputs(h, M, o)) return rc;
+    if (d.missing()) return fail(h, DFB_ERR_INVALID_ARG, "null output");
+    if (int rc = check_pair_outputs(h, M, d, label)) return rc;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
         // frame source: the requested frames are decoded as one group, straight into the gray frame array when no resize is
         // asked for, else into scratch and resized frame by frame; only the compressed bytes cross PCIe
@@ -1366,7 +1263,7 @@ int jpeg_chain(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int
                 DFB_CUDA(cudaEventRecord(h->chain_ev.frame[f], h->s_in));
             }
         };
-        return process_chain(h, n_frames, step, dw, dh, o, produce);
+        return process_chain(h, n_frames, step, dw, dh, d, produce);
     });
 }
 
@@ -1438,39 +1335,35 @@ extern "C" {
 int dfb_process_bgr_batch_host(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
                                int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
                                size_t *len_x, size_t *len_y) {
-    const JpgOut o{bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y};
-    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, {&o, nullptr});
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, jpeg_dest(bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y),
+                     "jpeg output");
 }
 
 int dfb_process_bgr_batch_host_png(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
                                    uint8_t *const *png, size_t capacity, size_t *len) {
-    const PngOut o{png, capacity, len};
-    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, {nullptr, &o});
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, png_dest(png, capacity, len), "png output");
 }
 
 int dfb_process_jpeg_batch_host(dfb_handle *h, const uint8_t *const *jpeg, const size_t *len, int n_frames, int step, int dw, int dh,
                                 int bound, int jpeg_quality, uint8_t *const *jpg_x, uint8_t *const *jpg_y, size_t capacity,
                                 size_t *len_x, size_t *len_y) {
-    const JpgOut o{bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y};
-    return jpeg_chain(h, jpeg, len, n_frames, step, dw, dh, {&o, nullptr});
+    return jpeg_chain(h, jpeg, len, n_frames, step, dw, dh, jpeg_dest(bound, jpeg_quality, jpg_x, jpg_y, capacity, len_x, len_y),
+                      "jpeg output");
 }
 
 int dfb_process_jpeg_batch_host_png(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step, int dw,
                                     int dh, uint8_t *const *png, size_t capacity, size_t *len) {
-    const PngOut o{png, capacity, len};
-    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, {nullptr, &o});
+    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, png_dest(png, capacity, len), "png output");
 }
 
 int dfb_process_bgr_batch_host_planes(dfb_handle *h, const uint8_t *const *bgr, int n_frames, int step, int sw, int sh, int dw, int dh,
                                       float *const *fx, float *const *fy) {
-    const PlanesOut o{fx, fy};
-    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, {nullptr, nullptr, &o});
+    return bgr_chain(h, bgr, n_frames, step, sw, sh, dw, dh, planes_dest(fx, fy, false), "plane output");
 }
 
 int dfb_process_jpeg_batch_host_planes(dfb_handle *h, const uint8_t *const *jpeg, const size_t *jpeg_len, int n_frames, int step, int dw,
                                        int dh, float *const *fx, float *const *fy) {
-    const PlanesOut o{fx, fy};
-    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, {nullptr, nullptr, &o});
+    return jpeg_chain(h, jpeg, jpeg_len, n_frames, step, dw, dh, planes_dest(fx, fy, false), "plane output");
 }
 
 int dfb_new_size(int width, int height, int new_width, int new_height, int new_short, int *dw, int *dh) {
@@ -1539,7 +1432,6 @@ int dfb_decode_jpeg_batch_device(dfb_handle *h, const uint8_t *const *jpeg, cons
                                              " does not fit the output (" + std::to_string(max_width) + "x" + std::to_string(max_height) +
                                              ", pitch " + std::to_string(pitch) + ", frame stride " + std::to_string(frame_stride) + ")");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
         h->jdec->decode(jpeg, len, hd.data(), n, channels, out, pitch, frame_stride, static_cast<cudaStream_t>(stream));
         h->alg->launches += h->jdec->launches;
@@ -1558,7 +1450,6 @@ int dfb_debug_jpeg_coefficients(dfb_handle *h, const uint8_t *jpeg, size_t len, 
     if ((size_t)hd[0].blocks() > capacity_blocks)
         return fail(h, DFB_ERR_SIZE, "the file has " + std::to_string(hd[0].blocks()) + " blocks, capacity is " + std::to_string(capacity_blocks));
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
         h->jdec->coefficients(jpeg, len, hd[0], out, nullptr);
         if (sync_rounds) *sync_rounds = h->jdec->sync_rounds;
@@ -1576,7 +1467,6 @@ int dfb_bgr_to_ycc420_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitch
     for (const void *p : {(const void *)bgr, (const void *)y, (const void *)cb, (const void *)cr})
         if (!is_device_pointer(p)) return fail(h, DFB_ERR_INVALID_ARG, "bgr / y / cb / cr must be device memory (device entry point)");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         const ResizeTap *taps = ycc_tables(h, src_width, src_height, dw, dh);
         launch_bgr_to_ycc420(bgr, bgr_pitch, src_width, src_height, dw, dh, taps, taps ? taps + dw : nullptr, y, y_pitch, cb, cr, c_pitch,
                              static_cast<cudaStream_t>(stream));
@@ -1602,7 +1492,6 @@ int dfb_encode_jpeg_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pit
     if (!is_device_pointer(bgr)) return fail(h, DFB_ERR_INVALID_ARG, "bgr must be device memory (device entry point)");
     if (host_pointer_kind(out) < 0) return fail(h, DFB_ERR_INVALID_ARG, "out must be host memory");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         const YccLayout L(dw, dh);
         h->enc_ycc.grow(L.bytes);
@@ -1639,7 +1528,6 @@ int dfb_extract_frames_host(dfb_handle *h, const uint8_t *const *bgr, int n_fram
     }
     const int sw = src_width, sh = src_height;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         // frame source: H2D of frame f into staging frame f & 1, interleaved with the converts
         const size_t bgr_bytes = (size_t)sw * sh * 3;
         auto upload = [&](int, int f0, int m, const ConvertFrame &convert) {
@@ -1677,7 +1565,6 @@ int dfb_extract_frames_jpeg_host(dfb_handle *h, const uint8_t *const *jpeg, cons
     if (int rc = parse_jpegs_one_size(h, jpeg, jpeg_len, n_frames, hd, sw, sh)) return rc;
     if (int rc = check_geometry(h, sw, sh, (size_t)sw * 3, dw, dh)) return rc;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         if (!h->jdec) h->jdec.reset(new JpegDecoder());
         // frame source: imdecode of group g to BGR into staging slot g & 1 (the host waits for the decoder's status)
         constexpr int G = kExtractGroup;
@@ -1709,7 +1596,6 @@ int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitc
     if (!is_device_pointer(bgr)) return fail(h, DFB_ERR_INVALID_ARG, "bgr must be device memory (device entry point)");
     if (host_pointer_kind(out) < 0) return fail(h, DFB_ERR_INVALID_ARG, "out must be host memory");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         if (!h->png) h->png.reset(new PngEncoder());
         h->alg->launches += h->png->encode(1, bgr, 0, bgr_pitch, width, height, 0, s);
@@ -1723,24 +1609,11 @@ int dfb_encode_png_bgr_device(dfb_handle *h, const uint8_t *bgr, size_t bgr_pitc
     });
 }
 
-int dfb_calc_batch_host_png(dfb_handle *h, const uint8_t *const *frames, int n_frames, int step, int width, int height, uint8_t *const *png,
-                            size_t capacity, size_t *len) {
-    if (!h) return DFB_ERR_INVALID_ARG;
-    if (int rc = refuse_initial_flow(h)) return rc;
-    if (n_frames > std::abs(step) && (!png || !len)) return fail(h, DFB_ERR_INVALID_ARG, "png / len is null");
-    return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
-        const PngOut out{png, capacity, len};
-        return batch_host(h, frames, n_frames, step, width, height, nullptr, 0, nullptr, nullptr, &out);
-    });
-}
-
 int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *in, int n_in, float *const *out, int n_out, int width,
                          int height, const double *scalars, int n_scalars, double *scalars_out) {
     if (!h || !kernel) return DFB_ERR_INVALID_ARG;
     if (width <= 0 || height <= 0 || n_in < 0 || n_out < 0 || n_in > 16 || n_out > 16) return fail(h, DFB_ERR_INVALID_ARG, "bad arguments");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         const std::string k(kernel);
         if (h->alg->debug_run(k, in, n_in, out, n_out, width, height, scalars, n_scalars, scalars_out)) return DFB_OK;  // the engine's own stages
         auto sc = [&](int i) { return i < n_scalars ? scalars[i] : 0.0; };
@@ -1879,7 +1752,6 @@ int dfb_debug_time_kernel(dfb_handle *h, const char *kernel, int width, int heig
     if (!h || !kernel || !ms_per_launch) return DFB_ERR_INVALID_ARG;
     if (width <= 0 || height <= 0 || sets < 1 || sets > 64 || reps < 1) return fail(h, DFB_ERR_INVALID_ARG, "bad arguments");
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         const std::string k(kernel);
         const bool primal = k == "estimate_u";
         if (!primal && k != "estimate_dual") throw std::runtime_error("unknown kernel " + k);
@@ -1916,7 +1788,6 @@ int dfb_debug_time_kernel(dfb_handle *h, const char *kernel, int width, int heig
 int dfb_get_tvl1_stats(dfb_handle *h, dfb_tvl1_stats *out) {
     if (!h || !out) return DFB_ERR_INVALID_ARG;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         h->alg->tvl1_stats(out);
         return DFB_OK;
     });
@@ -1925,7 +1796,6 @@ int dfb_get_tvl1_stats(dfb_handle *h, dfb_tvl1_stats *out) {
 int dfb_get_tvl1_pair_stats(dfb_handle *h, int pair_index, dfb_tvl1_stats *out) {
     if (!h || !out) return DFB_ERR_INVALID_ARG;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         if (!h->alg->pair_stats(pair_index, out)) return fail(h, DFB_ERR_INVALID_ARG, "pair_index is not one of the last 256 pairs of the most recent tvl1 batch call");
         return (int)DFB_OK;
     });
@@ -1934,7 +1804,6 @@ int dfb_get_tvl1_pair_stats(dfb_handle *h, int pair_index, dfb_tvl1_stats *out) 
 int dfb_get_counters(dfb_handle *h, dfb_counters *out) {
     if (!h || !out) return DFB_ERR_INVALID_ARG;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         dfb_tvl1_stats st;
         h->alg->tvl1_stats(&st);  // folds a pending fused-kernel log into pixel_iters
         *out = h->counters;
@@ -1949,7 +1818,6 @@ int dfb_get_counters(dfb_handle *h, dfb_counters *out) {
 int dfb_get_tvl1_phase_ns(dfb_handle *h, uint64_t out[32]) {
     if (!h || !out) return DFB_ERR_INVALID_ARG;
     return guarded(h, [&]() {
-        DFB_CUDA(cudaSetDevice(h->device));
         h->alg->phase_ns(out);
         return DFB_OK;
     });
