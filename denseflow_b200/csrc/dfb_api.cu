@@ -869,8 +869,9 @@ int dfb_calc_device(dfb_handle *h, const uint8_t *a, size_t a_pitch, const uint8
     return guarded(h, [&]() {
         cudaStream_t s = static_cast<cudaStream_t>(stream);
         h->alg->begin_batch();
-        h->alg->prepare_frame(a, a_pitch, width, height, 0, s);
-        h->alg->prepare_frame(b, b_pitch, width, height, 1, s);
+        const int slots[2] = {0, 1};  // one call per frame: the two frames' rows may lie at different pitches
+        h->alg->prepare_frames(1, &a, a_pitch, width, height, slots, s);
+        h->alg->prepare_frames(1, &b, b_pitch, width, height, slots + 1, s);
         FlowAlgorithm::PairJob pj{0, 1};
         bind_field(pj, flow_xy, flow_pitch, initial_flow(h));  // the start is read on s before the solve writes the field
         h->alg->solve_batch(&pj, 1, width, height, s);
@@ -1685,19 +1686,18 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             if (ow <= 0 || oh <= 0) throw std::runtime_error("resize: bad destination size");
         }
         const int pitch = round_up(width, 32), opitch = round_up(ow, 32);
-        std::vector<std::unique_ptr<DeviceBuffer<float>>> dev;
+        std::deque<DeviceBuffer<float>> dev;
         auto alloc = [&](int w_, int h_, int p_) {
-            const size_t bytes = (size_t)p_ * (h_ + 1) * sizeof(float);
-            dev.emplace_back(new DeviceBuffer<float>());
-            dev.back()->allocate(bytes);
-            float *p = *dev.back();
-            DFB_CUDA(cudaMemset(p, 0, bytes));
-            return Plane{p, w_, h_, p_};
+            DeviceBuffer<float> &b = dev.emplace_back();
+            b.allocate((size_t)p_ * (h_ + 1) * sizeof(float));
+            const Plane p{b, w_, h_, p_};
+            fill_plane(p, 0);
+            return p;
         };
         std::vector<Plane> pin, pout;
         for (int i = 0; i < n_in; ++i) {
             pin.push_back(alloc(width, height, pitch));
-            DFB_CUDA(cudaMemcpy2D(pin[i].p, (size_t)pitch * 4, in[i], (size_t)width * 4, (size_t)width * 4, height, cudaMemcpyHostToDevice));
+            upload_rows(pin[i], in[i], 0);
         }
         DeviceBuffer<double> d_part, d_sum;  // estimate_u's energy partials and their sum, when asked for
         auto need = [&](int ni, int no) {
@@ -1740,10 +1740,7 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             throw std::runtime_error("unknown debug kernel " + k);
         }
         DFB_CUDA(cudaDeviceSynchronize());
-        for (int i = 0; i < n_out; ++i) {
-            const Plane &src = inplace_from >= 0 ? pin[inplace_from + i] : pout[i];
-            DFB_CUDA(cudaMemcpy2D(out[i], (size_t)src.w * 4, src.p, (size_t)src.pitch * 4, (size_t)src.w * 4, src.h, cudaMemcpyDeviceToHost));
-        }
+        for (int i = 0; i < n_out; ++i) download_rows(out[i], inplace_from >= 0 ? pin[inplace_from + i] : pout[i], 0);
         return DFB_OK;
     });
 }

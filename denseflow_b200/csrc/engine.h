@@ -7,6 +7,7 @@
 
 #include <cmath>
 #include <cstdint>
+#include <cstring>
 #include <deque>
 #include <memory>
 #include <string>
@@ -91,16 +92,11 @@ class FlowAlgorithm {
     void ensure_slots(int n) {
         while ((int)slots_.size() < n) slots_.push_back(owned_zeroed(slot_elems_));
     }
-    // per-frame work: u8 -> fp32 (+ pyramid)
-    virtual void prepare_frame(const uint8_t *src, size_t pitch_bytes, int w, int h, int slot, cudaStream_t s) = 0;
-    // several frames of one size at once (engines whose per-frame stages are launch-latency-bound batch them)
-    virtual void prepare_frames(int n, const uint8_t *const *srcs, size_t pitch_bytes, int w, int h, const int *slots, cudaStream_t s) {
-        for (int i = 0; i < n; ++i) prepare_frame(srcs[i], pitch_bytes, w, h, slots[i], s);
-    }
-    // per-pair work: flow(slot_a -> slot_b) into interleaved float2 rows
-    virtual void solve(int slot_a, int slot_b, int w, int h, float *flow_xy, size_t flow_pitch_bytes,
-                       cudaStream_t s) = 0;
-    // several independent pairs at once (the fused tvl1 engine runs them side by side on disjoint SM groups)
+    // per-frame work, u8 -> fp32 (+ pyramid), for n frames of one size and one row pitch at once (each launch of the per-frame
+    // stages takes several frames: they are launch-latency-bound)
+    virtual void prepare_frames(int n, const uint8_t *const *srcs, size_t pitch_bytes, int w, int h, const int *slots, cudaStream_t s) = 0;
+    // per-pair work: flow(slot_a -> slot_b) of several independent pairs at once (the fused tvl1 engine runs them side by side
+    // on disjoint SM groups)
     struct PairJob {
         int slot_a, slot_b;
         float *flow_xy;
@@ -122,12 +118,10 @@ class FlowAlgorithm {
         size_t init_pitch = 0;
         int init_step = 1;
     };
-    virtual int max_concurrent_pairs(int w, int h) { (void)w; (void)h; return 1; }
+    virtual int max_concurrent_pairs(int w, int h) = 0;
     // after a CUDA error: what the engine's own watchdogs recorded (empty if nothing)
     virtual std::string fault_info() { return {}; }
-    virtual void solve_batch(const PairJob *jobs, int n, int w, int h, cudaStream_t s) {
-        for (int i = 0; i < n; ++i) solve(jobs[i].slot_a, jobs[i].slot_b, w, h, jobs[i].flow_xy, jobs[i].flow_pitch_bytes, s);
-    }
+    virtual void solve_batch(const PairJob *jobs, int n, int w, int h, cudaStream_t s) = 0;
     virtual bool set_param(const std::string &name, double v) = 0;
     virtual bool get_param(const std::string &name, double *v) const = 0;
     virtual void tvl1_stats(dfb_tvl1_stats *out) { *out = dfb_tvl1_stats{}; }
@@ -177,6 +171,41 @@ class FlowAlgorithm {
     size_t slot_elems_ = 0;
     std::deque<DeviceBuffer<float>> owned_;
 };
+
+// Host-plane staging of the test hooks (debug_run, dfb_debug_run_kernel), on the null stream.  fill_plane sets every byte of
+// the pitched plane p, padding and its spare row included; upload_rows (after fill_plane(p, fill) when fill >= 0) copies rows
+// [row0, row0 + p.h) of a dense host plane p.w floats wide into p, and download_rows copies p back to the same rows.
+inline void fill_plane(const Plane &p, int fill) { DFB_CUDA(cudaMemset(p.p, fill, (size_t)p.pitch * (p.h + 1) * sizeof(float))); }
+inline void upload_rows(const Plane &p, const float *src, int row0, int fill = -1) {
+    if (fill >= 0) fill_plane(p, fill);
+    DFB_CUDA(cudaMemcpy2D(p.p, (size_t)p.pitch * 4, src + (size_t)row0 * p.w, (size_t)p.w * 4, (size_t)p.w * 4, p.h, cudaMemcpyHostToDevice));
+}
+inline void download_rows(float *dst, const Plane &p, int row0) {
+    DFB_CUDA(cudaMemcpy2D(dst + (size_t)row0 * p.w, (size_t)p.w * 4, p.p, (size_t)p.pitch * 4, (size_t)p.w * 4, p.h, cudaMemcpyDeviceToHost));
+}
+
+// The start of a warm-started test pair as the flow calls pass one: rows [row0, row0 + h) of the dense host planes x, y (w
+// floats wide), laid out in buf as a float2 field (step 2) or as two planes (step 1), rows `pitch` floats apart, with NaN in
+// the padding.  Points pj's init_* fields at it.
+inline void stage_initial_flow(DeviceBuffer<float> &buf, FlowAlgorithm::PairJob &pj, const float *x, const float *y, int row0, int w,
+                               int h, int step, size_t pitch) {
+    const size_t yoff = step == 2 ? 1 : pitch * h, elems = pitch * h * (step == 1 ? 2 : 1);
+    std::vector<float> host(elems);
+    std::memset(host.data(), 0xff, elems * sizeof(float));
+    x += (size_t)row0 * w;
+    y += (size_t)row0 * w;
+    for (int r = 0; r < h; ++r)
+        for (int c = 0; c < w; ++c) {
+            host[r * pitch + (size_t)c * step] = x[(size_t)r * w + c];
+            host[yoff + r * pitch + (size_t)c * step] = y[(size_t)r * w + c];
+        }
+    buf.allocate(elems * sizeof(float));
+    DFB_CUDA(cudaMemcpy(buf, host.data(), elems * sizeof(float), cudaMemcpyHostToDevice));
+    pj.init_x = buf;
+    pj.init_y = buf + yoff;
+    pj.init_pitch = pitch;
+    pj.init_step = step;
+}
 
 std::unique_ptr<FlowAlgorithm> make_tvl1(int device, int max_w, int max_h);
 std::unique_ptr<FlowAlgorithm> make_farneback(int device, int max_w, int max_h);

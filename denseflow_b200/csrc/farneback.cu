@@ -754,9 +754,6 @@ class Farneback final : public FlowAlgorithm {
 
     // per-frame work (B.2, B.3): u8 -> fp32, then for every level: Gaussian blur of the FULL-resolution frame,
     // bilinear resize to the level, polynomial expansion into the slot's R planes
-    void prepare_frame(const uint8_t *src, size_t pitch_bytes, int w, int h, int slot, cudaStream_t s) override {
-        prepare_frames(1, &src, pitch_bytes, w, h, &slot, s);
-    }
     void prepare_frames(int n, const uint8_t *const *srcs, size_t pitch_bytes, int w, int h, const int *slots, cudaStream_t s) override {
         const LevelSet ls = levels_for(w, h, false);
         const int pitch_full = round_up(w, 32);
@@ -775,17 +772,9 @@ class Farneback final : public FlowAlgorithm {
         }
     }
 
-    // per-pair work (B.4, B.5): coarse -> fine, 10 fused box / solve / rebuild iterations per level
-    void solve(int slot_a, int slot_b, int w, int h, float *flow_xy, size_t flow_pitch_bytes, cudaStream_t s) override {
-        PairJob one{};
-        one.slot_a = slot_a;
-        one.slot_b = slot_b;
-        one.flow_xy = flow_xy;
-        one.flow_pitch_bytes = flow_pitch_bytes;
-        solve_batch(&one, 1, w, h, s);
-    }
     int max_concurrent_pairs(int, int) override { return kMaxFarnBatch; }
 
+    // per-pair work (B.4, B.5): coarse -> fine, 10 fused box / solve / rebuild iterations per level
     void solve_batch(const PairJob *jobs, int count, int w, int h, cudaStream_t s) override {
         const LevelSet ls = levels_for(w, h, false);
         for (int j0 = 0; j0 < count; j0 += kMaxFarnBatch) {
@@ -828,13 +817,6 @@ class Farneback final : public FlowAlgorithm {
         auto fits = [&](int pw, int ph) {
             if (pw < 1 || ph < 1 || pw > max_w_ || ph > max_h_) throw std::runtime_error(k + ": plane size outside the handle's maximum frame size");
         };
-        // host row block [row0, row0 + p.h) of a dense host plane of width p.w <-> a pitched device plane
-        auto up = [&](const Plane &p, const float *src, int row0) {
-            DFB_CUDA(cudaMemcpy2D(p.p, (size_t)p.pitch * 4, src + (size_t)row0 * p.w, (size_t)p.w * 4, (size_t)p.w * 4, p.h, cudaMemcpyHostToDevice));
-        };
-        auto down = [&](float *dst, const Plane &p, int row0) {
-            DFB_CUDA(cudaMemcpy2D(dst + (size_t)row0 * p.w, (size_t)p.w * 4, p.p, (size_t)p.pitch * 4, (size_t)p.w * 4, p.h, cudaMemcpyDeviceToHost));
-        };
         auto plane5 = [](const Plane5 &q, int i) { return Plane{q.p[i], q.w, q.h, q.pitch}; };
         DFB_CUDA(cudaDeviceSynchronize());  // nothing of an earlier asynchronous call may still use the slots or lanes
         const cudaStream_t s = nullptr;
@@ -847,10 +829,10 @@ class Farneback final : public FlowAlgorithm {
             const Level &L = ls.lv[ls.n - 1 - lk];
             const int pitch_full = round_up(w, 32);
             PrepBatch pb = prep_batch(1);
-            up(Plane{pb.frame[0], w, h, pitch_full}, in[0], 0);
+            upload_rows(Plane{pb.frame[0], w, h, pitch_full}, in[0], 0);
             launch_level_image(pb, 1, w, h, pitch_full, L, s);
             DFB_CUDA(cudaDeviceSynchronize());
-            down(out[0], Plane{pb.img[0], L.w, L.h, L.pitch}, 0);
+            download_rows(out[0], Plane{pb.img[0], L.w, L.h, L.pitch}, 0);
             return true;
         }
         if (k == "farn_poly_exp") {  // in {level image}  out {R0 .. R4}
@@ -859,11 +841,11 @@ class Farneback final : public FlowAlgorithm {
             const Level L{w, h, round_up(w, 32), 0, 0.0, 0};
             PrepBatch pb = prep_batch(1);
             pb.r[0] = slots_.at(0) + L.r_off;
-            up(Plane{pb.img[0], w, h, L.pitch}, in[0], 0);
+            upload_rows(Plane{pb.img[0], w, h, L.pitch}, in[0], 0);
             launch_poly_exp(pb, 1, L, poly_constants(prm_.poly_n, prm_.poly_sigma), s);
             DFB_CUDA(cudaDeviceSynchronize());
             const Plane5 R = r_planes(0, L);
-            for (int i = 0; i < 5; ++i) down(out[i], plane5(R, i), 0);
+            for (int i = 0; i < 5; ++i) download_rows(out[i], plane5(R, i), 0);
             return true;
         }
         if (k == "farn_flow_init") {  // in {fx, fy of the coarser level}  out {fx, fy}  scalars {level w, level h}
@@ -878,12 +860,12 @@ class Farneback final : public FlowAlgorithm {
             ensure_lanes(1);
             FarnBatchArgs args{};
             args.p[0] = pair_args(PairJob{0, 1, nullptr, 0}, lanes_[0], ls, 1, 0);
-            up(args.p[0].pfx, in[0], 0);
-            up(args.p[0].pfy, in[1], 0);
+            upload_rows(args.p[0].pfx, in[0], 0);
+            upload_rows(args.p[0].pfy, in[1], 0);
             launch_flow_init(args, 1, ls, 1, s);
             DFB_CUDA(cudaDeviceSynchronize());
-            down(out[0], args.p[0].fx, 0);
-            down(out[1], args.p[0].fy, 0);
+            download_rows(out[0], args.p[0].fx, 0);
+            download_rows(out[1], args.p[0].fy, 0);
             return true;
         }
         if (k == "farn_initial_flow") {  // in {x, y of every pair's initial flow}  out {fx, fy of the coarsest level}  scalars {step, pitch, pairs}
@@ -903,42 +885,27 @@ class Farneback final : public FlowAlgorithm {
             const Level &L = ls.lv[0];
             ensure_slots(2 * nb);
             ensure_lanes(nb);
-            const size_t pl_bytes = Slab::padded(plane_elems_, 4), yoff = step == 2 ? 1 : pitch * ph;
-            const size_t buf_elems = pitch * ph * (step == 1 ? 2 : 1);
-            std::vector<float> host(buf_elems);
-            std::vector<float *> bufs(nb);
+            const size_t pl_bytes = Slab::padded(plane_elems_, 4);
+            std::vector<DeviceBuffer<float>> bufs(nb);
             FarnBatchArgs args{};
             for (int i = 0; i < nb; ++i) {
-                std::memset(host.data(), 0xff, buf_elems * sizeof(float));
-                const float *x = in[0] + (size_t)i * ph * w, *y = in[1] + (size_t)i * ph * w;
-                for (int r = 0; r < ph; ++r)
-                    for (int c = 0; c < w; ++c) {
-                        host[r * pitch + (size_t)c * step] = x[(size_t)r * w + c];
-                        host[yoff + r * pitch + (size_t)c * step] = y[(size_t)r * w + c];
-                    }
-                DFB_CUDA(cudaMalloc(&bufs[i], buf_elems * sizeof(float)));
-                DFB_CUDA(cudaMemcpy(bufs[i], host.data(), buf_elems * sizeof(float), cudaMemcpyHostToDevice));
+                PairJob pj{2 * i, 2 * i + 1, nullptr, 0};
+                stage_initial_flow(bufs[i], pj, in[0], in[1], i * ph, w, ph, step, pitch);
                 for (int b = 0; b < 2; ++b) {
                     DFB_CUDA(cudaMemset(lanes_[i].fx[b], 0xff, pl_bytes));
                     DFB_CUDA(cudaMemset(lanes_[i].fy[b], 0xff, pl_bytes));
                 }
-                PairJob pj{2 * i, 2 * i + 1, nullptr, 0};
-                pj.init_x = bufs[i];
-                pj.init_y = bufs[i] + yoff;
-                pj.init_pitch = pitch;
-                pj.init_step = step;
                 args.p[i] = pair_args(pj, lanes_[i], ls, 0, 0);
             }
             launch_flow_init(args, nb, ls, 0, s, true);
             DFB_CUDA(cudaDeviceSynchronize());
             for (int i = 0; i < nb; ++i) {
-                down(out[0], args.p[i].fx, i * L.h);
-                down(out[1], args.p[i].fy, i * L.h);
+                download_rows(out[0], args.p[i].fx, i * L.h);
+                download_rows(out[1], args.p[i].fy, i * L.h);
                 for (int b = 0; b < 2; ++b) {
                     DFB_CUDA(cudaMemset(lanes_[i].fx[b], 0, pl_bytes));
                     DFB_CUDA(cudaMemset(lanes_[i].fy[b], 0, pl_bytes));
                 }
-                DFB_CUDA(cudaFree(bufs[i]));
             }
             DFB_CUDA(cudaDeviceSynchronize());
             return true;
@@ -963,15 +930,15 @@ class Farneback final : public FlowAlgorithm {
             PairArgs &a = args.p[i] = pair_args(PairJob{2 * i, 2 * i + 1, nullptr, 0}, lanes_[i], ls, l, 0);
             const int r = i * ph;
             if (um) {
-                up(a.fx, in[0], r);
-                up(a.fy, in[1], r);
+                upload_rows(a.fx, in[0], r);
+                upload_rows(a.fy, in[1], r);
             }
             const float *const *rin = in + (um ? 2 : 5);
             for (int q = 0; q < 5; ++q) {
-                if (!um) up(plane5(a.M[0], q), in[q], r);
-                up(plane5(a.R0, q), rin[q], r);
-                up(plane5(a.R1, q), rin[5 + q], r);
-                DFB_CUDA(cudaMemset(a.M[1].p[q], 0, (size_t)a.M[1].pitch * (ph + 1) * sizeof(float)));
+                if (!um) upload_rows(plane5(a.M[0], q), in[q], r);
+                upload_rows(plane5(a.R0, q), rin[q], r);
+                upload_rows(plane5(a.R1, q), rin[5 + q], r);
+                fill_plane(plane5(a.M[1], q), 0);
             }
         }
         if (um) {
@@ -985,10 +952,10 @@ class Farneback final : public FlowAlgorithm {
             const PairArgs &a = args.p[i];
             const int r = i * ph;
             if (!um) {
-                down(out[0], a.fx, r);
-                down(out[1], a.fy, r);
+                download_rows(out[0], a.fx, r);
+                download_rows(out[1], a.fy, r);
             }
-            for (int q = 0; q < 5; ++q) down(out[(um ? 0 : 2) + q], plane5(a.M[um ? 0 : 1], q), r);
+            for (int q = 0; q < 5; ++q) download_rows(out[(um ? 0 : 2) + q], plane5(a.M[um ? 0 : 1], q), r);
         }
         return true;
     }

@@ -43,8 +43,6 @@ struct Tvl1Consts {
 };
 
 // ---- stand-alone kernels (one launch per half-step: the reference's launch structure) -------
-void launch_u8_to_f32(const uint8_t *src, size_t src_pitch_bytes, Plane dst, cudaStream_t s);
-void launch_resize_linear(Plane src, Plane dst, float fx, float fy, float post_mul, cudaStream_t s);
 // the two per-frame stages for several frames of one size at once (blockIdx.z = frame): each launch is latency-bound, a
 // 64-frame clip needs 5 launches instead of 320
 constexpr int kMaxFrameBatch = 16;
@@ -56,6 +54,8 @@ void launch_u8_to_f32_batch(const FramePtrs &fp, int n, size_t src_pitch_bytes, 
 // level (src_off, sw, sh, sp) -> level (dst_off, dw, dh, dp) of every frame's slot
 void launch_resize_linear_batch(const FramePtrs &fp, int n, size_t src_off, int sw, int sh, int sp, size_t dst_off, int dw, int dh, int dp, float fx,
                                 float fy, cudaStream_t s);
+// one plane (the flow upsample and the initial flow's pyramid): the same kernel, times post_mul
+void launch_resize_linear(Plane src, Plane dst, float fx, float fy, float post_mul, cudaStream_t s);
 // use_initial_flow: pair i's initial field (x at x[i][y * pitch[i] + x * step[i]], y likewise) -> its lane's level-0 u1 / u2
 // planes (row pitch u_pitch), for several pairs of one size at once (blockIdx.z = pair)
 constexpr int kMaxInitFlows = 16;

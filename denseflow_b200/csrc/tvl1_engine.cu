@@ -129,23 +129,10 @@ class Tvl1 final : public FlowAlgorithm {
         return n;
     }
 
-    void prepare_frame(const uint8_t *src, size_t pitch_bytes, int w, int h, int slot, cudaStream_t s) override {
-        LevelGeom lv[kMaxScales];
-        const int n = level_geometry(w, h, lv);
-        float *base = slots_.at(slot);
-        launch_u8_to_f32(src, pitch_bytes, level_plane(base, lv, 0), s);
-        ++launches;
-        const float finv = (float)(1.0 / prm_.scale_step);  // dsize empty => fx = float(1/scaleStep)
-        for (int l = 1; l < n; ++l) {
-            launch_resize_linear(level_plane(base, lv, l - 1), level_plane(base, lv, l), finv, finv, 1.0f, s);
-            ++launches;
-        }
-    }
-
     void prepare_frames(int n, const uint8_t *const *srcs, size_t pitch_bytes, int w, int h, const int *slots, cudaStream_t s) override {
         LevelGeom lv[kMaxScales];
         const int nl = level_geometry(w, h, lv);
-        const float finv = (float)(1.0 / prm_.scale_step);
+        const float finv = (float)(1.0 / prm_.scale_step);  // dsize empty => fx = float(1/scaleStep)
         for (int f0 = 0; f0 < n; f0 += kMaxFrameBatch) {
             const int nf = std::min(kMaxFrameBatch, n - f0);
             FramePtrs fp{};
@@ -162,25 +149,6 @@ class Tvl1 final : public FlowAlgorithm {
                 ++launches;
                 off = next;
             }
-        }
-    }
-
-    void solve(int slot_a, int slot_b, int w, int h, float *flow_xy, size_t flow_pitch_bytes,
-               cudaStream_t s) override {
-        LevelGeom lv[kMaxScales];
-        const int n = level_geometry(w, h, lv);
-        last_nscales_ = n;
-        last_warps_ = prm_.warps;
-        std::memcpy(last_lv_, lv, sizeof(lv));
-        if (prm_.fused) {
-            PairJob one{};
-            one.slot_a = slot_a;
-            one.slot_b = slot_b;
-            one.flow_xy = flow_xy;
-            one.flow_pitch_bytes = flow_pitch_bytes;
-            solve_fused(&one, 1, lv, n, s);
-        } else {
-            solve_unfused(slot_a, slot_b, lv, n, flow_xy, flow_pitch_bytes, s);
         }
     }
 
@@ -390,25 +358,18 @@ class Tvl1 final : public FlowAlgorithm {
         prm_ = keep;
 
         auto plane = [&](const float *p, int l) { return Plane{const_cast<float *>(p), lv[l].w, lv[l].h, lv[l].pitch}; };
-        auto poison = [&](const Plane &p) { DFB_CUDA(cudaMemset(p.p, 0x41, (size_t)p.pitch * (p.h + 1) * sizeof(float))); };
-        auto up = [&](const Plane &p, const float *src, int lane) {
-            poison(p);
-            DFB_CUDA(cudaMemcpy2D(p.p, (size_t)p.pitch * 4, src + (size_t)lane * p.h * p.w, (size_t)p.w * 4, (size_t)p.w * 4, p.h, cudaMemcpyHostToDevice));
-        };
-        auto down = [&](float *dst, const Plane &p, int lane) {
-            DFB_CUDA(cudaMemcpy2D(dst + (size_t)lane * p.h * p.w, (size_t)p.w * 4, p.p, (size_t)p.pitch * 4, (size_t)p.w * 4, p.h, cudaMemcpyDeviceToHost));
-        };
+        constexpr int kPoison = 0x41;
         const int cur_out = st.stage == kFusedStageChunks ? nch & 1 : 0;
         std::vector<std::vector<Plane>> outs(nb);
         for (int i = 0; i < nb; ++i) {
             const FusedJob &J = jobs[i];
             const FusedLevel &L = J.lv[level];
             for (int b = 0; b < 2; ++b) {  // every workspace plane the phase may touch starts poisoned
-                poison(plane(J.lv[0].u1[b], 0));
-                poison(plane(J.lv[0].u2[b], 0));
-                for (int q = 0; q < 4; ++q) poison(plane(J.p[b][q], 0));
+                fill_plane(plane(J.lv[0].u1[b], 0), kPoison);
+                fill_plane(plane(J.lv[0].u2[b], 0), kPoison);
+                for (int q = 0; q < 4; ++q) fill_plane(plane(J.p[b][q], 0), kPoison);
             }
-            for (const float *p : {J.I1x, J.I1y, J.I1wx, J.I1wy, J.grad, J.rho_c}) poison(plane(p, 0));
+            for (const float *p : {J.I1x, J.I1y, J.I1wx, J.I1wy, J.grad, J.rho_c}) fill_plane(plane(p, 0), kPoison);
             std::vector<Plane> ins;
             switch (st.stage) {
             case kFusedStageLevelStart:
@@ -431,8 +392,6 @@ class Tvl1 final : public FlowAlgorithm {
                 for (int q = 0; q < 4; ++q) outs[i].push_back(plane(J.p[cur_out][q], 0));
                 break;
             case kFusedStageUpsample:
-                poison(plane(L.u1[0], 1));
-                poison(plane(L.u2[0], 1));
                 ins = {plane(L.u1[0], 1), plane(L.u2[0], 1)};
                 outs[i] = {plane(J.lv[0].u1[0], 0), plane(J.lv[0].u2[0], 0)};
                 break;
@@ -444,7 +403,7 @@ class Tvl1 final : public FlowAlgorithm {
                 ins = {plane(L.u1[0], 0), plane(L.u2[0], 0)};
                 break;
             }
-            for (int q = 0; q < n_in; ++q) up(ins[q], in[q], i);
+            for (int q = 0; q < n_in; ++q) upload_rows(ins[q], in[q], i * ins[q].h, kPoison);
         }
         FusedBatch batch{};
         batch.njobs = nb;
@@ -460,7 +419,7 @@ class Tvl1 final : public FlowAlgorithm {
         DFB_CUDA(cudaDeviceSynchronize());
         for (int i = 0; i < nb; ++i) {
             if (st.stage != kFusedStageMerge) {
-                for (int q = 0; q < n_out; ++q) down(out[q], outs[i][q], i);
+                for (int q = 0; q < n_out; ++q) download_rows(out[q], outs[i][q], i * outs[i][q].h);
                 continue;
             }
             const size_t npx = (size_t)w * ph;
@@ -515,28 +474,14 @@ class Tvl1 final : public FlowAlgorithm {
         DFB_CUDA(cudaDeviceSynchronize());  // nothing of an earlier asynchronous call may still use the lanes
         const cudaStream_t s = nullptr;
         ensure_lanes(nb);
-        const size_t pyr_bytes = Slab::padded(pyr_elems_, 4), yoff = step == 2 ? 1 : pitch * ph;
-        const size_t buf_elems = pitch * ph * (step == 1 ? 2 : 1);
-        std::vector<float> host(buf_elems);
-        std::vector<float *> bufs(nb);
+        const size_t pyr_bytes = Slab::padded(pyr_elems_, 4);
+        std::vector<DeviceBuffer<float>> bufs(nb);
         std::vector<PairJob> jobs(nb);
         for (int i = 0; i < nb; ++i) {
             DFB_CUDA(cudaMemset(lanes_[i].u1pyr[0], 0xff, pyr_bytes));
             DFB_CUDA(cudaMemset(lanes_[i].u2pyr[0], 0xff, pyr_bytes));
-            std::memset(host.data(), 0xff, buf_elems * sizeof(float));
-            const float *x = in[0] + (size_t)i * ph * w, *y = in[1] + (size_t)i * ph * w;
-            for (int r = 0; r < ph; ++r)
-                for (int c = 0; c < w; ++c) {
-                    host[r * pitch + (size_t)c * step] = x[(size_t)r * w + c];
-                    host[yoff + r * pitch + (size_t)c * step] = y[(size_t)r * w + c];
-                }
-            DFB_CUDA(cudaMalloc(&bufs[i], buf_elems * sizeof(float)));
-            DFB_CUDA(cudaMemcpy(bufs[i], host.data(), buf_elems * sizeof(float), cudaMemcpyHostToDevice));
             jobs[i] = PairJob{2 * i, 2 * i + 1, nullptr, 0};
-            jobs[i].init_x = bufs[i];
-            jobs[i].init_y = bufs[i] + yoff;
-            jobs[i].init_pitch = pitch;
-            jobs[i].init_step = step;
+            stage_initial_flow(bufs[i], jobs[i], in[0], in[1], i * ph, w, ph, step, pitch);
         }
         load_initial_flow(jobs.data(), nb, lv, n, s);
         DFB_CUDA(cudaDeviceSynchronize());
@@ -545,12 +490,10 @@ class Tvl1 final : public FlowAlgorithm {
             for (int l = 0; l < n; off += (size_t)nb * lv[l].w * lv[l].h, ++l)
                 for (int c = 0; c < 2; ++c) {
                     const Plane p = level_plane(c ? lanes_[i].u2pyr[0] : lanes_[i].u1pyr[0], lv, l);
-                    DFB_CUDA(cudaMemcpy2D(out[c] + off + (size_t)i * p.h * p.w, (size_t)p.w * 4, p.p, (size_t)p.pitch * 4, (size_t)p.w * 4, p.h,
-                                          cudaMemcpyDeviceToHost));
+                    download_rows(out[c] + off, p, i * p.h);
                 }
             DFB_CUDA(cudaMemset(lanes_[i].u1pyr[0], 0, pyr_bytes));  // as ensure_lanes leaves them
             DFB_CUDA(cudaMemset(lanes_[i].u2pyr[0], 0, pyr_bytes));
-            DFB_CUDA(cudaFree(bufs[i]));
         }
         DFB_CUDA(cudaDeviceSynchronize());
         return true;
@@ -647,7 +590,7 @@ class Tvl1 final : public FlowAlgorithm {
 
     // use_initial_flow: the initial fields of the pairs jobs[i] that carry one (PairJob::init_x) into lane i's flow pyramid
     // u1pyr[0] / u2pyr[0], enqueued before the solve.  Level 0 is the field as given; level s is resize_linear of level s - 1
-    // with the frame pyramid's taps (prepare_frame), times float(scale_step) (DESIGN §1).
+    // with the frame pyramid's taps (prepare_frames), times float(scale_step) (DESIGN §1).
     void load_initial_flow(const PairJob *jobs, int count, const LevelGeom *lv, int n, cudaStream_t s) {
         InitFlows f{};
         int m = 0;

@@ -15,46 +15,8 @@ inline dim3 grid2d(int w, int h, int px_per_thread_x = 1) {
     return dim3(ceil_div(w, BX * px_per_thread_x), ceil_div(h, BY));
 }
 
-// A.1: I0s[0] = float(I0), x1.0.  4 pixels per thread: one 32-bit load -> one float4 store.
-__global__ void k_u8_to_f32(const uint8_t *__restrict__ src, size_t src_pitch, Plane dst) {
-    const int x0 = 4 * (blockIdx.x * BX + threadIdx.x);
-    const int y = blockIdx.y * BY + threadIdx.y;
-    if (y >= dst.h || x0 >= dst.w) return;
-    const uint8_t *row = src + (size_t)y * src_pitch;
-    float4 v;
-    if (x0 + 3 < dst.w && ((reinterpret_cast<uintptr_t>(row + x0) & 3) == 0)) {
-        const uchar4 q = *reinterpret_cast<const uchar4 *>(row + x0);
-        v = make_float4(q.x, q.y, q.z, q.w);
-    } else {
-        v.x = row[x0];
-        v.y = x0 + 1 < dst.w ? row[x0 + 1] : 0.f;
-        v.z = x0 + 2 < dst.w ? row[x0 + 2] : 0.f;
-        v.w = x0 + 3 < dst.w ? row[x0 + 3] : 0.f;
-    }
-    *reinterpret_cast<float4 *>(dst.p + (size_t)y * dst.pitch + x0) = v;  // pitch % 32 == 0: in-bounds
-}
-
-// A.1: cudawarping resize_linear — src = dst * f (no half-pixel offset), x2/y2 reads clamped.
-// post_mul folds the "u *= 1/scaleStep" multiply that follows the flow upsample (A.2 step 4).
-__global__ void k_resize_linear(Plane src, Plane dst, float fx, float fy, float post_mul) {
-    const int dx = blockIdx.x * BX + threadIdx.x;
-    const int dy = blockIdx.y * BY + threadIdx.y;
-    if (dx >= dst.w || dy >= dst.h) return;
-    const float sx = dx * fx, sy = dy * fy;
-    const int x1 = __float2int_rd(sx), y1 = __float2int_rd(sy);
-    const int x2 = x1 + 1, y2 = y1 + 1;
-    const int x1r = min(x1, src.w - 1), y1r = min(y1, src.h - 1);
-    const int x2r = min(x2, src.w - 1), y2r = min(y2, src.h - 1);
-    const float *r1 = src.p + (size_t)y1r * src.pitch;
-    const float *r2 = src.p + (size_t)y2r * src.pitch;
-    float out = 0.f;
-    out = out + r1[x1r] * ((x2 - sx) * (y2 - sy));
-    out = out + r1[x2r] * ((sx - x1) * (y2 - sy));
-    out = out + r2[x1r] * ((x2 - sx) * (sy - y1));
-    out = out + r2[x2r] * ((sx - x1) * (sy - y1));
-    dst.p[(size_t)dy * dst.pitch + dx] = out * post_mul;
-}
-
+// A.1: I0s[0] = float(I0), x1.0, of several frames (blockIdx.z = frame).  4 pixels per thread: one 32-bit load -> one
+// float4 store.
 __global__ void k_u8_to_f32_batch(const __grid_constant__ FramePtrs fp, size_t src_pitch, int w, int h, int pitch) {
     const int x0 = 4 * (blockIdx.x * BX + threadIdx.x);
     const int y = blockIdx.y * BY + threadIdx.y;
@@ -70,16 +32,21 @@ __global__ void k_u8_to_f32_batch(const __grid_constant__ FramePtrs fp, size_t s
         v.z = x0 + 2 < w ? row[x0 + 2] : 0.f;
         v.w = x0 + 3 < w ? row[x0 + 3] : 0.f;
     }
-    *reinterpret_cast<float4 *>(fp.base[blockIdx.z] + (size_t)y * pitch + x0) = v;
+    *reinterpret_cast<float4 *>(fp.base[blockIdx.z] + (size_t)y * pitch + x0) = v;  // pitch % 32 == 0: in-bounds
 }
 
-// same arithmetic as k_resize_linear (post_mul = 1)
-__global__ void k_resize_linear_batch(const __grid_constant__ FramePtrs fp, size_t src_off, int sw, int sh, int sp, size_t dst_off, int dw, int dh,
-                                      int dp, float fx, float fy) {
+// A.1: cudawarping resize_linear — src = dst * f (no half-pixel offset), x2/y2 reads clamped — of several planes of one
+// size (blockIdx.z = plane).  post_mul folds the "u *= 1/scaleStep" multiply that follows the flow upsample (A.2 step 4).
+struct ResizePtrs {
+    const float *src[kMaxFrameBatch];
+    float *dst[kMaxFrameBatch];
+};
+__global__ void k_resize_linear(const __grid_constant__ ResizePtrs rp, int sw, int sh, int sp, int dw, int dh, int dp, float fx, float fy,
+                                float post_mul) {
     const int dx = blockIdx.x * BX + threadIdx.x;
     const int dy = blockIdx.y * BY + threadIdx.y;
     if (dx >= dw || dy >= dh) return;
-    const float *src = fp.base[blockIdx.z] + src_off;
+    const float *src = rp.src[blockIdx.z];
     const float sx = dx * fx, sy = dy * fy;
     const int x1 = __float2int_rd(sx), y1 = __float2int_rd(sy);
     const int x2 = x1 + 1, y2 = y1 + 1;
@@ -92,7 +59,7 @@ __global__ void k_resize_linear_batch(const __grid_constant__ FramePtrs fp, size
     out = out + r1[x2r] * ((sx - x1) * (y2 - sy));
     out = out + r2[x1r] * ((x2 - sx) * (sy - y1));
     out = out + r2[x2r] * ((sx - x1) * (sy - y1));
-    fp.base[blockIdx.z][dst_off + (size_t)dy * dp + dx] = out * 1.0f;
+    rp.dst[blockIdx.z][(size_t)dy * dp + dx] = out * post_mul;
 }
 
 __global__ void k_split_initial_flow(const __grid_constant__ InitFlows f, int w, int h, int u_pitch) {
@@ -274,10 +241,6 @@ __global__ void k_quantise(const float *flow, size_t flow_pitch_bytes, int w, in
 
 }  // namespace
 
-void launch_u8_to_f32(const uint8_t *src, size_t src_pitch_bytes, Plane dst, cudaStream_t s) {
-    k_u8_to_f32<<<grid2d(dst.w, dst.h, 4), dim3(BX, BY), 0, s>>>(src, src_pitch_bytes, dst);
-    DFB_KERNEL_CHECK();
-}
 void launch_u8_to_f32_batch(const FramePtrs &fp, int n, size_t src_pitch_bytes, int w, int h, int pitch, cudaStream_t s) {
     const dim3 g = grid2d(w, h, 4);
     k_u8_to_f32_batch<<<dim3(g.x, g.y, n), dim3(BX, BY), 0, s>>>(fp, src_pitch_bytes, w, h, pitch);
@@ -285,12 +248,20 @@ void launch_u8_to_f32_batch(const FramePtrs &fp, int n, size_t src_pitch_bytes, 
 }
 void launch_resize_linear_batch(const FramePtrs &fp, int n, size_t src_off, int sw, int sh, int sp, size_t dst_off, int dw, int dh, int dp, float fx,
                                 float fy, cudaStream_t s) {
+    ResizePtrs rp{};
+    for (int i = 0; i < n; ++i) {
+        rp.src[i] = fp.base[i] + src_off;
+        rp.dst[i] = fp.base[i] + dst_off;
+    }
     const dim3 g = grid2d(dw, dh);
-    k_resize_linear_batch<<<dim3(g.x, g.y, n), dim3(BX, BY), 0, s>>>(fp, src_off, sw, sh, sp, dst_off, dw, dh, dp, fx, fy);
+    k_resize_linear<<<dim3(g.x, g.y, n), dim3(BX, BY), 0, s>>>(rp, sw, sh, sp, dw, dh, dp, fx, fy, 1.0f);
     DFB_KERNEL_CHECK();
 }
 void launch_resize_linear(Plane src, Plane dst, float fx, float fy, float post_mul, cudaStream_t s) {
-    k_resize_linear<<<grid2d(dst.w, dst.h), dim3(BX, BY), 0, s>>>(src, dst, fx, fy, post_mul);
+    ResizePtrs rp{};
+    rp.src[0] = src.p;
+    rp.dst[0] = dst.p;
+    k_resize_linear<<<grid2d(dst.w, dst.h), dim3(BX, BY), 0, s>>>(rp, src.w, src.h, src.pitch, dst.w, dst.h, dst.pitch, fx, fy, post_mul);
     DFB_KERNEL_CHECK();
 }
 void launch_split_initial_flow(const InitFlows &f, int n, int w, int h, int u_pitch, cudaStream_t s) {

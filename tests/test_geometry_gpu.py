@@ -153,7 +153,7 @@ def _device_calls(e, alg, fr, host, tag):
     got = e.calc(dfr[0], dfr[1])
     torch.cuda.synchronize()
     _same(got.cpu().numpy(), want, tag + " calc_device dense")
-    # pitched views whose base is 1..3 bytes past an aligned address (the uchar4 loads of k_u8_to_f32 must not be taken),
+    # pitched views whose base is 1..3 bytes past an aligned address (the uchar4 loads of k_u8_to_f32_batch must not be taken),
     # into a flow whose rows are longer than the image
     for off in (1, 2, 3):
         pitch = w + 8 + 2 * off + 1
