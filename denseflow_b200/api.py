@@ -13,6 +13,76 @@ import numpy as np
 from . import _lib
 
 
+def _pairs(n, step):
+    """M = max(N - |step|, 0): the flows of N frames at `step` (src/denseflow_gpu.cpp:308)"""
+    return max(n - abs(step), 0)
+
+
+def _sizes(new_size, w, h):
+    """((dw, dh), (ow, oh)): the resize a call is asked for ((0, 0): none) and the size of its outputs, for w x h frames"""
+    return (new_size or (0, 0)), (new_size or (w, h))
+
+
+def _stream(device, stream=None):
+    """The stream a device call is enqueued on: `stream`, or torch's current stream on `device`."""
+    import torch
+    return C.c_void_p(stream if stream is not None else torch.cuda.current_stream(device).cuda_stream)
+
+
+def _ptrs(addrs):
+    """A pointer array for the C side; an empty one still has one (null) entry."""
+    return (C.c_void_p * max(len(addrs), 1))(*addrs)
+
+
+def _frame_source(frames):
+    """Host frames of one size as the frame source of a call: (frames, (their pointer array,), n, width, height)"""
+    h, w = frames[0].shape[:2]
+    return frames, (_ptrs([f.ctypes.data for f in frames]),), len(frames), w, h
+
+
+def _check_out(a, shape, dtype, name):
+    if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape[1:] != tuple(shape[1:]) or a.shape[0] < shape[0] \
+            or not all(a[i].flags.c_contiguous for i in range(shape[0])):
+        raise RuntimeError("%s: expected a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, tuple(shape)))
+
+
+# The outputs of a host batch call: each builder returns the call's output arguments and a collector of its result.
+def _field(flows, m, h, w):
+    """float32 [M,H,W,2]: `flows`, or a new array"""
+    if flows is None:
+        flows = np.empty((m, h, w, 2), np.float32)
+    _check_out(flows, (m, h, w, 2), np.float32, "flows")
+    return (_ptrs([flows[i].ctypes.data for i in range(m)]),), lambda: flows
+
+
+def _u8_planes(qx, qy, m, h, w):
+    """the quantised planes qx, qy, uint8 [M,H,W] each"""
+    _check_out(qx, (m, h, w), np.uint8, "qx")
+    _check_out(qy, (m, h, w), np.uint8, "qy")
+    return tuple(_ptrs([q[i].ctypes.data for i in range(m)]) for q in (qx, qy)), lambda: (qx, qy)
+
+
+def _float_planes(out, m, h, w):
+    """float32 [M,2,H,W], out[j, 0] / out[j, 1] pair j's x / y plane: `out`, or a new array"""
+    if out is None:
+        out = np.empty((m, 2, h, w), np.float32)
+    _check_out(out, (m, 2, h, w), np.float32, "out")
+    return tuple(_ptrs([out[i, c].ctypes.data for i in range(m)]) for c in (0, 1)), lambda: out
+
+
+def _files(k, m, cap, bufs=None):
+    """k files for each of m items in host buffers of cap bytes (bufs: k lists of the caller's): the arguments (k pointer
+    arrays, cap, k length arrays) and the files' bytes, one per item or a k-tuple per item."""
+    if bufs is None:
+        bufs = [[np.empty(max(cap, 1), np.uint8) for _ in range(m)] for _ in range(k)]
+    lens = [(C.c_size_t * max(m, 1))() for _ in range(k)]
+
+    def collect():
+        files = [tuple(b[i][:ln[i]].tobytes() for b, ln in zip(bufs, lens)) for i in range(m)]
+        return files if k > 1 else [f for f, in files]
+    return (*[_ptrs([b.ctypes.data for b in bb]) for bb in bufs], cap, *lens), collect
+
+
 class DenseOpticalFlow:
     """cv::cuda::DenseOpticalFlow look-alike bound to one GPU."""
 
@@ -62,9 +132,11 @@ class DenseOpticalFlow:
         self._check(self._L.dfb_get_param(self._h, name.encode(), C.byref(v)))
         return v.value
 
-    def _reads_flow(self, buf):
-        """buf is None while use_initial_flow is set: the library refuses the call with its message (null flow buffer)"""
-        return buf is None and self.get("use_initial_flow") != 0
+    def _warm_start_probe(self, flow, call, *nulls, pairs=1):
+        """With use_initial_flow set a call reads its flow buffer, so one without (flow None) must fail: call(*nulls), the
+        call with null flow arguments, raises the library's refusal.  A call without pairs reads nothing."""
+        if flow is None and self.get("use_initial_flow") != 0 and pairs:
+            self._check(call(*nulls))
 
     # -- calc(I0, I1) -> flow (CV_32FC2), src/denseflow_gpu.cpp:327/:329 --
     def calc(self, a, b, flow=None, stream=None):
@@ -77,43 +149,49 @@ class DenseOpticalFlow:
             if a.ndim != 2 or a.shape != b.shape:
                 raise RuntimeError("calc: frames must be two CV_8UC1 images of the same size")
             h, w = a.shape
-            if self._reads_flow(flow):
-                self._check(self._L.dfb_calc_host(self._h, a.ctypes.data, b.ctypes.data, w, h, None))
+            call = lambda f: self._L.dfb_calc_host(self._h, a.ctypes.data, b.ctypes.data, w, h, f)  # noqa: E731
+            self._warm_start_probe(flow, call, None)
             if flow is None:
                 flow = np.empty((h, w, 2), np.float32)
-            self._check(self._L.dfb_calc_host(self._h, a.ctypes.data, b.ctypes.data, w, h, flow.ctypes.data))
+            self._check(call(flow.ctypes.data))
             return flow
         import torch
         if a.dtype != torch.uint8 or b.dtype != torch.uint8 or a.dim() != 2 or a.shape != b.shape or not a.is_cuda or not b.is_cuda \
                 or a.stride(1) != 1 or b.stride(1) != 1:
             raise RuntimeError("calc: frames must be two CV_8UC1 CUDA tensors of the same size with unit column stride")
         h, w = a.shape
-        s = stream if stream is not None else torch.cuda.current_stream(a.device).cuda_stream
-        if self._reads_flow(flow):
-            self._check(self._L.dfb_calc_device(self._h, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), w, h, None, w * 8,
-                                                C.c_void_p(s)))
+        s = _stream(a.device, stream)
+        call = lambda f, pitch: self._L.dfb_calc_device(self._h, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), w, h,  # noqa: E731
+                                                        f, pitch, s)
+        self._warm_start_probe(flow, call, None, w * 8)
         if flow is None:
             flow = torch.empty((h, w, 2), dtype=torch.float32, device=a.device)
-        self._check(self._L.dfb_calc_device(self._h, a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), w, h,
-                                            flow.data_ptr(), flow.stride(0) * 4, C.c_void_p(s)))
+        self._check(call(flow.data_ptr(), flow.stride(0) * 4))
         return flow
 
+    # -- the frame sources of the host batch calls: (keep-alive list, the call's frame arguments, n, width, height) --
     @staticmethod
     def _gray_frames(frames):
         """Every frame must be a CV_8UC1 image of the first frame's size (the C side reads width*height bytes of each)."""
-        out = []
+        keep = []
         for i, f in enumerate(frames):
             f = np.asarray(f)
-            if f.dtype != np.uint8 or f.ndim != 2 or (out and f.shape != out[0].shape):
+            if f.dtype != np.uint8 or f.ndim != 2 or (keep and f.shape != keep[0].shape):
                 raise RuntimeError("frame %d: expected a uint8 [H,W] image of the same size as frame 0" % i)
-            out.append(np.ascontiguousarray(f))
-        return out
+            keep.append(np.ascontiguousarray(f))
+        return _frame_source(keep)
 
     @staticmethod
-    def _check_out(a, shape, dtype, name):
-        if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape[1:] != tuple(shape[1:]) or a.shape[0] < shape[0] \
-                or not all(a[i].flags.c_contiguous for i in range(shape[0])):
-            raise RuntimeError("%s: expected a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, tuple(shape)))
+    def _bgr_frames(frames_bgr, name):
+        frames = [np.asarray(f) for f in frames_bgr]
+        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != frames[0].shape for f in frames):
+            raise RuntimeError("%s: frames must be uint8 [H,W,3] images of one size" % name)
+        return _frame_source([np.ascontiguousarray(f) for f in frames])
+
+    def _jpeg_frames(self, jpegs):
+        """JPEG files of one size (the call checks it): their size is bounded by the handle's maximum."""
+        keep, ptrs, lens = self._jpeg_buffers(jpegs)
+        return keep, (ptrs, lens), len(keep), self.max_width, self.max_height
 
     # -- the batch shape of calc_optflows_imp (src/denseflow_gpu.cpp:307-342) --
     def calc_batch(self, frames, step=1, flows=None, bound=None):
@@ -121,149 +199,102 @@ class DenseOpticalFlow:
         flows [M,H,W,2] float32, or with bound=B the quantised (qx, qy) uint8 [M,H,W] planes
         (convertFlowToImage, src/common.cpp:4-16, done on the GPU).  With use_initial_flow set, flows[j] is also pair j's
         starting flow."""
-        frames = self._gray_frames(frames)
-        n = len(frames)
-        if n == 0:
+        if len(frames) == 0:
             return np.empty((0, 0, 0, 2), np.float32)
-        h, w = frames[0].shape
-        m = max(n - abs(step), 0)
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        if bound is None:
-            if self._reads_flow(flows) and m > 0:
-                self._check(self._L.dfb_calc_batch_host(self._h, fp, n, step, w, h, None))
-            if flows is None:
-                flows = np.empty((m, h, w, 2), np.float32)
-            self._check_out(flows, (m, h, w, 2), np.float32, "flows")
-            op = (C.c_void_p * max(m, 1))(*[flows[i].ctypes.data for i in range(m)])
-            self._check(self._L.dfb_calc_batch_host(self._h, fp, n, step, w, h, op))
-            return flows
-        qx = np.empty((m, h, w), np.uint8)
-        qy = np.empty((m, h, w), np.uint8)
-        xp = (C.c_void_p * max(m, 1))(*[qx[i].ctypes.data for i in range(m)])
-        yp = (C.c_void_p * max(m, 1))(*[qy[i].ctypes.data for i in range(m)])
-        self._check(self._L.dfb_calc_batch_host_u8(self._h, fp, n, step, w, h, int(bound), xp, yp))
-        return qx, qy
+        keep, src, n, w, h = self._gray_frames(frames)
+        m = _pairs(n, step)
+        if bound is not None:
+            return self.calc_batch_u8_into(keep, step, bound, np.empty((m, h, w), np.uint8), np.empty((m, h, w), np.uint8))
+        call = lambda op: self._L.dfb_calc_batch_host(self._h, *src, n, step, w, h, op)  # noqa: E731
+        self._warm_start_probe(flows, call, None, pairs=m)
+        out, collect = _field(flows, m, h, w)
+        self._check(call(*out))
+        return collect()
 
     def calc_batch_u8_into(self, frames, step, bound, qx, qy):
         """calc_batch(..., bound=B) writing into caller-provided (e.g. pinned) uint8 arrays qx, qy of shape [M,H,W]."""
-        frames = self._gray_frames(frames)
-        n = len(frames)
-        h, w = frames[0].shape
-        m = max(n - abs(step), 0)
-        self._check_out(qx, (m, h, w), np.uint8, "qx")
-        self._check_out(qy, (m, h, w), np.uint8, "qy")
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        xp = (C.c_void_p * max(m, 1))(*[qx[i].ctypes.data for i in range(m)])
-        yp = (C.c_void_p * max(m, 1))(*[qy[i].ctypes.data for i in range(m)])
-        self._check(self._L.dfb_calc_batch_host_u8(self._h, fp, n, step, w, h, int(bound), xp, yp))
-        return qx, qy
+        keep, src, n, w, h = self._gray_frames(frames)
+        out, collect = _u8_planes(qx, qy, _pairs(n, step), h, w)
+        self._check(self._L.dfb_calc_batch_host_u8(self._h, *src, n, step, w, h, int(bound), *out))
+        return collect()
 
     def calc_batch_device(self, frames, step=1, flows=None, stream=None):
         """frames: CUDA uint8 tensor [N,H,W] (contiguous); flows: CUDA float32 [M,H,W,2] (contiguous), with use_initial_flow
         set also the pairs' starting flows."""
         import torch
         n, h, w = frames.shape
-        m = max(n - abs(step), 0)
-        s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
-        if self._reads_flow(flows):
-            self._check(self._L.dfb_calc_batch_device(self._h, frames.data_ptr(), n, step, w, h, None, C.c_void_p(s)))
+        s = _stream(frames.device, stream)
+        call = lambda f: self._L.dfb_calc_batch_device(self._h, frames.data_ptr(), n, step, w, h, f, s)  # noqa: E731
+        self._warm_start_probe(flows, call, None)
         if flows is None:
-            flows = torch.empty((m, h, w, 2), dtype=torch.float32, device=frames.device)
-        self._check(self._L.dfb_calc_batch_device(self._h, frames.data_ptr(), n, step, w, h, flows.data_ptr(),
-                                                  C.c_void_p(s)))
+            flows = torch.empty((_pairs(n, step), h, w, 2), dtype=torch.float32, device=frames.device)
+        self._check(call(flows.data_ptr()))
         return flows
 
     # -- the flow as two float planes per pair: the payloads of -st=h5's flow_x / flow_y datasets --
-    @staticmethod
-    def _plane_ptrs(out, m):
-        xp = (C.c_void_p * max(m, 1))(*[out[i, 0].ctypes.data for i in range(m)])
-        yp = (C.c_void_p * max(m, 1))(*[out[i, 1].ctypes.data for i in range(m)])
-        return xp, yp
-
     def calc_batch_planes(self, frames, step=1, out=None):
         """calc_batch with the flow channels first: float32 [M,2,H,W], out[j,0] / out[j,1] bit for bit flows[j,...,0] /
         flows[j,...,1].  The engines' merge epilogue writes the planes; out may be a caller (e.g. page-locked) array, with
         use_initial_flow set also the pairs' starting flows."""
-        frames = self._gray_frames(frames)
-        n = len(frames)
-        if n == 0:
+        if len(frames) == 0:
             return np.empty((0, 2, 0, 0), np.float32)
-        h, w = frames[0].shape
-        m = max(n - abs(step), 0)
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        if self._reads_flow(out) and m > 0:
-            self._check(self._L.dfb_calc_batch_host_planes(self._h, fp, n, step, w, h, None, None))
-        if out is None:
-            out = np.empty((m, 2, h, w), np.float32)
-        self._check_out(out, (m, 2, h, w), np.float32, "out")
-        xp, yp = self._plane_ptrs(out, m)
-        self._check(self._L.dfb_calc_batch_host_planes(self._h, fp, n, step, w, h, xp, yp))
-        return out
+        keep, src, n, w, h = self._gray_frames(frames)
+        m = _pairs(n, step)
+        call = lambda xp, yp: self._L.dfb_calc_batch_host_planes(self._h, *src, n, step, w, h, xp, yp)  # noqa: E731
+        self._warm_start_probe(out, call, None, None, pairs=m)
+        args, collect = _float_planes(out, m, h, w)
+        self._check(call(*args))
+        return collect()
 
     def calc_batch_device_planes(self, frames, step=1, planes=None, stream=None):
         """frames: CUDA uint8 tensor [N,H,W] (contiguous); planes: CUDA float32 [M,2,H,W] (contiguous), with use_initial_flow
         set also the pairs' starting flows."""
         import torch
         n, h, w = frames.shape
-        m = max(n - abs(step), 0)
-        if self._reads_flow(planes):
-            s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
-            self._check(self._L.dfb_calc_batch_device_planes(self._h, frames.data_ptr(), n, step, w, h, None, C.c_void_p(s)))
+        m = _pairs(n, step)
+        s = _stream(frames.device, stream)
+        call = lambda p: self._L.dfb_calc_batch_device_planes(self._h, frames.data_ptr(), n, step, w, h, p, s)  # noqa: E731
+        self._warm_start_probe(planes, call, None)
         if planes is None:
             planes = torch.empty((m, 2, h, w), dtype=torch.float32, device=frames.device)
         if planes.dtype != torch.float32 or tuple(planes.shape) != (m, 2, h, w) or not planes.is_contiguous():
             raise RuntimeError("planes: expected a contiguous float32 CUDA tensor of shape %s" % ((m, 2, h, w),))
-        s = stream if stream is not None else torch.cuda.current_stream(frames.device).cuda_stream
-        self._check(self._L.dfb_calc_batch_device_planes(self._h, frames.data_ptr(), n, step, w, h, planes.data_ptr(),
-                                                         C.c_void_p(s)))
+        self._check(call(planes.data_ptr()))
         return planes
 
     def process_bgr_batch_planes(self, frames_bgr, step=1, new_size=None):
         """-st=h5 payloads for decoded BGR frames: gray -> resize -> flow -> float32 [M,2,dh,dw], bit for bit calc_batch_planes of
         the gray, resized frames."""
-        frames = self._bgr_frames(frames_bgr, "process_bgr_batch_planes")
-        n = len(frames)
-        if n == 0:
+        if len(frames_bgr) == 0:
             return np.empty((0, 2, 0, 0), np.float32)
-        sh, sw = frames[0].shape[:2]
-        dw, dh = new_size if new_size else (0, 0)
-        ow, oh = new_size if new_size else (sw, sh)
-        m = max(n - abs(step), 0)
-        out = np.empty((m, 2, oh, ow), np.float32)
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        xp, yp = self._plane_ptrs(out, m)
-        self._check(self._L.dfb_process_bgr_batch_host_planes(self._h, fp, n, step, sw, sh, dw, dh, xp, yp))
-        return out
+        keep, src, n, sw, sh = self._bgr_frames(frames_bgr, "process_bgr_batch_planes")
+        (dw, dh), (ow, oh) = _sizes(new_size, sw, sh)
+        out, collect = _float_planes(None, _pairs(n, step), oh, ow)
+        self._check(self._L.dfb_process_bgr_batch_host_planes(self._h, *src, n, step, sw, sh, dw, dh, *out))
+        return collect()
 
     def process_jpeg_batch_planes(self, jpegs, step=1, new_size=None):
         """-if -st=h5 payloads: process_bgr_batch_planes with the frames given as JPEG files of one size, decoded on the GPU to
         imdecode's pixels."""
-        keep, ptrs, lens = self._jpeg_buffers(jpegs)
-        n = len(keep)
-        m = max(n - abs(step), 0)
+        keep, (ptrs, lens), n, _, _ = self._jpeg_frames(jpegs)
+        m = _pairs(n, step)
         if m == 0:
             return np.empty((0, 2, 0, 0), np.float32)
-        dw, dh = new_size if new_size else (0, 0)
-        if new_size:
-            ow, oh = new_size
-        else:  # the size of the frames (the call checks that all have frame 0's)
-            w, h = C.c_int(), C.c_int()
-            if self._L.dfb_jpeg_info(ptrs[0], lens[0], C.byref(w), C.byref(h)) != _lib.DFB_OK:
-                raise RuntimeError(self._L.dfb_last_error(None).decode())
-            ow, oh = w.value, h.value
-        out = np.empty((m, 2, oh, ow), np.float32)
-        xp, yp = self._plane_ptrs(out, m)
-        self._check(self._L.dfb_process_jpeg_batch_host_planes(self._h, ptrs, lens, n, step, dw, dh, xp, yp))
-        return out
+        w, h = C.c_int(), C.c_int()  # without a resize, the outputs have frame 0's size (the call checks that all have it)
+        if not new_size and self._L.dfb_jpeg_info(ptrs[0], lens[0], C.byref(w), C.byref(h)) != _lib.DFB_OK:
+            raise RuntimeError(self._L.dfb_last_error(None).decode())
+        (dw, dh), (ow, oh) = _sizes(new_size, w.value, h.value)
+        out, collect = _float_planes(None, m, oh, ow)
+        self._check(self._L.dfb_process_jpeg_batch_host_planes(self._h, ptrs, lens, n, step, dw, dh, *out))
+        return collect()
 
     def quantise_device(self, flow, bound):
         import torch
         h, w = flow.shape[:2]
         qx = torch.empty((h, w), dtype=torch.uint8, device=flow.device)
         qy = torch.empty((h, w), dtype=torch.uint8, device=flow.device)
-        s = torch.cuda.current_stream(flow.device).cuda_stream
         self._check(self._L.dfb_quantise_device(self._h, flow.data_ptr(), flow.stride(0) * 4, w, h, int(bound),
-                                                qx.data_ptr(), qy.data_ptr(), w, C.c_void_p(s)))
+                                                qx.data_ptr(), qy.data_ptr(), w, _stream(flow.device)))
         return qx, qy
 
     # -- convertFlowToPngImage (src/common.cpp:18-46): the CV_8UC3 image `-st=png` encodes --
@@ -273,9 +304,8 @@ class DenseOpticalFlow:
         h, w = flow.shape[:2]
         bgr = torch.empty((h, w, 3), dtype=torch.uint8, device=flow.device)
         b = (C.c_double * 2)()
-        s = torch.cuda.current_stream(flow.device).cuda_stream
         self._check(self._L.dfb_flow_to_png_image_device(self._h, flow.data_ptr(), flow.stride(0) * 4, w, h, bgr.data_ptr(), w * 3,
-                                                         b if return_bounds else None, C.c_void_p(s)))
+                                                         b if return_bounds else None, _stream(flow.device)))
         return bgr, ((b[0], b[1]) if return_bounds else None)
 
     # -- frame preparation (cvtColor BGR2GRAY + resize INTER_LINEAR, src/denseflow_gpu.cpp:163-170), bit-exact to OpenCV CPU --
@@ -283,29 +313,25 @@ class DenseOpticalFlow:
         import torch
         h, w = bgr.shape[:2]
         gray = torch.empty((h, w), dtype=torch.uint8, device=bgr.device)
-        s = torch.cuda.current_stream(bgr.device).cuda_stream
-        self._check(self._L.dfb_bgr_to_gray_device(self._h, bgr.data_ptr(), bgr.stride(0), w, h, gray.data_ptr(), w, C.c_void_p(s)))
+        self._check(self._L.dfb_bgr_to_gray_device(self._h, bgr.data_ptr(), bgr.stride(0), w, h, gray.data_ptr(), w, _stream(bgr.device)))
         return gray
 
     def resize_gray_device(self, gray, dst_width, dst_height):
         import torch
         h, w = gray.shape
         out = torch.empty((dst_height, dst_width), dtype=torch.uint8, device=gray.device)
-        s = torch.cuda.current_stream(gray.device).cuda_stream
         self._check(self._L.dfb_resize_gray_device(self._h, gray.data_ptr(), gray.stride(0), w, h, out.data_ptr(), dst_width,
-                                                   dst_width, dst_height, C.c_void_p(s)))
+                                                   dst_width, dst_height, _stream(gray.device)))
         return out
 
     # -- imencode(".jpg", plane) on the GPU (src/common.cpp:56-57), OpenCV default quality 95 --
     def encode_jpeg_gray_device(self, gray, quality=95):
-        import torch
         h, w = gray.shape
         cap = self._L.dfb_jpeg_max_bytes(w, h)
         buf = np.empty(cap, np.uint8)
         n = C.c_size_t()
-        s = torch.cuda.current_stream(gray.device).cuda_stream
         self._check(self._L.dfb_encode_jpeg_gray_device(self._h, gray.data_ptr(), gray.stride(0), w, h, int(quality), buf.ctypes.data,
-                                                        cap, C.byref(n), C.c_void_p(s)))
+                                                        cap, C.byref(n), _stream(gray.device)))
         return buf[:n.value].tobytes()
 
     def encode_jpeg_gray_batch_device(self, planes, quality=95, capacity=None):
@@ -318,13 +344,10 @@ class DenseOpticalFlow:
         if planes.dtype != torch.uint8 or not planes.is_cuda or planes.stride(2) != 1:
             raise ValueError("planes must be a CUDA uint8 tensor [n, H, W] with contiguous rows")
         cap = int(capacity) if capacity is not None else self._L.dfb_jpeg_max_bytes(w, h)
-        bufs = [np.empty(cap, np.uint8) for _ in range(n)]
-        ptrs = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        lens = (C.c_size_t * n)()
-        s = torch.cuda.current_stream(planes.device).cuda_stream
+        out, collect = _files(1, n, cap)
         self._check(self._L.dfb_encode_jpeg_gray_batch_device(self._h, planes.data_ptr(), planes.stride(1), planes.stride(0), n, w, h,
-                                                              int(quality), ptrs, cap, lens, C.c_void_p(s)))
-        return [bufs[i][:lens[i]].tobytes() for i in range(n)]
+                                                              int(quality), *out, _stream(planes.device)))
+        return collect()
 
     # -- imread(".jpg") + cvtColor(BGR2GRAY) of an `-if` frame folder on the GPU (nvJPEG decode; not bit-identical to libjpeg-turbo) --
     def decode_jpeg_gray_device(self, jpeg_bytes, max_width, max_height, device=None):
@@ -333,9 +356,8 @@ class DenseOpticalFlow:
         buf = np.frombuffer(jpeg_bytes, np.uint8)
         out = torch.empty((max_height, max_width), dtype=torch.uint8, device=dev)
         w, h = C.c_int(), C.c_int()
-        s = torch.cuda.current_stream(dev).cuda_stream
         self._check(self._L.dfb_decode_jpeg_gray_device(self._h, buf.ctypes.data, buf.size, out.data_ptr(), max_width, max_width, max_height,
-                                                        C.byref(w), C.byref(h), C.c_void_p(s)))
+                                                        C.byref(w), C.byref(h), _stream(dev)))
         return out[:h.value, :w.value]
 
     # -- imread(IMREAD_COLOR) [+ cvtColor(BGR2GRAY)] of `-if` frame folders on the GPU, exactly cv2.imdecode's pixels --
@@ -356,8 +378,7 @@ class DenseOpticalFlow:
                 ptrs.append(j.data_ptr())
                 lens.append(j.numel())
             keep.append(j)
-        n = len(ptrs)
-        return keep, (C.c_void_p * max(n, 1))(*ptrs), (C.c_size_t * max(n, 1))(*lens)
+        return keep, _ptrs(ptrs), (C.c_size_t * max(len(lens), 1))(*lens)
 
     def decode_jpeg_batch(self, jpegs, channels=3, max_width=None, max_height=None, pitch=None, stream=None, device=None):
         """Decodes JPEG files (bytes, numpy or CPU torch uint8 buffers; sizes and samplings may differ) on the GPU to exactly
@@ -373,9 +394,8 @@ class DenseOpticalFlow:
         n = len(keep)
         out = torch.empty((max(n, 1), mh, pitch), dtype=torch.uint8, device=dev)
         ws, hs = (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))()
-        s = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
         self._check(self._L.dfb_decode_jpeg_batch_device(self._h, ptrs, lens, n, int(channels), out.data_ptr(), pitch, mh * pitch, mw, mh,
-                                                         ws, hs, C.c_void_p(s)))
+                                                         ws, hs, _stream(dev, stream)))
         res = []
         for i in range(n):
             v = out[i, :hs[i], :ws[i] * channels]
@@ -385,19 +405,11 @@ class DenseOpticalFlow:
     def process_jpeg_batch(self, jpegs, step=1, bound=20, new_size=None, quality=95):
         """The `-if` flow batch: process_bgr_batch with the frames given as JPEG files of one size, decoded on the GPU to
         imdecode's pixels.  Returns [(jpg_x bytes, jpg_y bytes)] per pair, byte for byte process_bgr_batch's."""
-        keep, ptrs, lens = self._jpeg_buffers(jpegs)
-        n = len(keep)
-        dw, dh = new_size if new_size else (0, 0)
-        m = max(n - abs(step), 0)
-        if new_size:
-            ow, oh = dw, dh
-        else:
-            ow, oh = self.max_width, self.max_height  # an upper bound of the frame size (checked by the call)
-        cap = self._L.dfb_jpeg_max_bytes(ow, oh)
-        bx, xp, lx = self._file_buffers(m, cap)
-        by, yp, ly = self._file_buffers(m, cap)
-        self._check(self._L.dfb_process_jpeg_batch_host(self._h, ptrs, lens, n, step, dw, dh, int(bound), int(quality), xp, yp, cap, lx, ly))
-        return [(bx[i][:lx[i]].tobytes(), by[i][:ly[i]].tobytes()) for i in range(m)]
+        keep, src, n, w, h = self._jpeg_frames(jpegs)
+        (dw, dh), (ow, oh) = _sizes(new_size, w, h)
+        out, collect = _files(2, _pairs(n, step), self._L.dfb_jpeg_max_bytes(ow, oh))
+        self._check(self._L.dfb_process_jpeg_batch_host(self._h, *src, n, step, dw, dh, int(bound), int(quality), *out))
+        return collect()
 
     def debug_jpeg_coefficients(self, jpeg):
         """Test hook: (int16 [blocks, 64] quantised coefficients in decode order, natural order, absolute DC; sync rounds)."""
@@ -416,20 +428,12 @@ class DenseOpticalFlow:
     # -- gray -> resize -> flow -> quantise -> JPEG for decoded BGR frames (the reference's chain minus decode / file IO) --
     def process_bgr_batch(self, frames_bgr, step=1, bound=20, new_size=None, quality=95):
         """frames_bgr: list of uint8 [H,W,3]; new_size: (w, h) or None.  Returns [(jpg_x bytes, jpg_y bytes)] per pair."""
-        frames = [np.ascontiguousarray(f, np.uint8) for f in frames_bgr]
-        n = len(frames)
-        if any(f.ndim != 3 or f.shape != frames[0].shape or f.shape[2] != 3 for f in frames):
-            raise RuntimeError("process_bgr_batch: frames must be uint8 [H,W,3] images of one size")
-        sh, sw = frames[0].shape[:2]
-        dw, dh = new_size if new_size else (0, 0)
-        ow, oh = (dw, dh) if new_size else (sw, sh)
-        m = max(n - abs(step), 0)
-        cap = self._L.dfb_jpeg_max_bytes(ow, oh)
-        bx, xp, lx = self._file_buffers(m, cap)
-        by, yp, ly = self._file_buffers(m, cap)
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        self._check(self._L.dfb_process_bgr_batch_host(self._h, fp, n, step, sw, sh, dw, dh, int(bound), int(quality), xp, yp, cap, lx, ly))
-        return [(bx[i][:lx[i]].tobytes(), by[i][:ly[i]].tobytes()) for i in range(m)]
+        frames = [np.ascontiguousarray(f, np.uint8) for f in frames_bgr]  # any dtype is converted, unlike the other BGR entries
+        keep, src, n, sw, sh = self._bgr_frames(frames, "process_bgr_batch")
+        (dw, dh), (ow, oh) = _sizes(new_size, sw, sh)
+        out, collect = _files(2, _pairs(n, step), self._L.dfb_jpeg_max_bytes(ow, oh))
+        self._check(self._L.dfb_process_bgr_batch_host(self._h, *src, n, step, sw, sh, dw, dh, int(bound), int(quality), *out))
+        return collect()
 
     # -- frame-extraction mode (-s=0, extract_frames_video, src/denseflow_gpu.cpp:82-144): resize + imencode(".jpg") per frame --
     @staticmethod
@@ -447,131 +451,90 @@ class DenseOpticalFlow:
         y = torch.empty((dh, dw), dtype=torch.uint8, device=bgr.device)
         cb = torch.empty(((dh + 1) // 2, (dw + 1) // 2), dtype=torch.uint8, device=bgr.device)
         cr = torch.empty_like(cb)
-        s = torch.cuda.current_stream(bgr.device).cuda_stream
         self._check(self._L.dfb_bgr_to_ycc420_device(self._h, bgr.data_ptr(), bgr.stride(0), sw, sh, dw, dh, y.data_ptr(), dw,
-                                                     cb.data_ptr(), cr.data_ptr(), cb.stride(0), C.c_void_p(s)))
+                                                     cb.data_ptr(), cr.data_ptr(), cb.stride(0), _stream(bgr.device)))
         return y, cb, cr
 
     def encode_jpeg_bgr_device(self, bgr, new_size=None, quality=95):
         """imencode(".jpg", cv::resize(bgr, new_size)) of a uint8 [H,W,3] BGR CUDA tensor, on the GPU.  Returns the bytes."""
-        import torch
         sw, sh = self._bgr_device(bgr)
-        dw, dh = new_size if new_size else (sw, sh)
-        cap = self._L.dfb_jpeg_max_bytes_bgr(dw, dh)
+        (dw, dh), (ow, oh) = _sizes(new_size, sw, sh)
+        cap = self._L.dfb_jpeg_max_bytes_bgr(ow, oh)
         buf = np.empty(cap, np.uint8)
         n = C.c_size_t()
-        s = torch.cuda.current_stream(bgr.device).cuda_stream
-        self._check(self._L.dfb_encode_jpeg_bgr_device(self._h, bgr.data_ptr(), bgr.stride(0), sw, sh, dw if new_size else 0,
-                                                       dh if new_size else 0, int(quality), buf.ctypes.data, cap, C.byref(n), C.c_void_p(s)))
+        self._check(self._L.dfb_encode_jpeg_bgr_device(self._h, bgr.data_ptr(), bgr.stride(0), sw, sh, dw, dh, int(quality), buf.ctypes.data,
+                                                       cap, C.byref(n), _stream(bgr.device)))
         return buf[:n.value].tobytes()
 
     def extract_frames(self, frames_bgr, new_size=None, quality=95):
         """frames_bgr: uint8 [H,W,3] host images of one size (pageable or page-locked), or one [N,H,W,3] array.
         Returns one JPEG bitstream per frame, in order (what extract_frames_video writes as img_%05d.jpg)."""
-        frames = [np.asarray(f) for f in frames_bgr]
-        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != frames[0].shape for f in frames):
-            raise RuntimeError("extract_frames: frames must be uint8 [H,W,3] images of one size")
-        frames = [np.ascontiguousarray(f) for f in frames]
-        n = len(frames)
-        if n == 0:
+        if len(frames_bgr) == 0:
             return []
-        sh, sw = frames[0].shape[:2]
-        dw, dh = new_size if new_size else (0, 0)
-        cap = self._L.dfb_jpeg_max_bytes_bgr(*(new_size if new_size else (sw, sh)))
-        bufs, op, lens = self._file_buffers(n, cap)
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        self._check(self._L.dfb_extract_frames_host(self._h, fp, n, sw, sh, dw, dh, int(quality), op, cap, lens))
-        return [bufs[i][:lens[i]].tobytes() for i in range(n)]
+        keep, src, n, sw, sh = self._bgr_frames(frames_bgr, "extract_frames")
+        (dw, dh), (ow, oh) = _sizes(new_size, sw, sh)
+        out, collect = _files(1, n, self._L.dfb_jpeg_max_bytes_bgr(ow, oh))
+        self._check(self._L.dfb_extract_frames_host(self._h, *src, n, sw, sh, dw, dh, int(quality), *out))
+        return collect()
 
     # -- -st=png: imencode(".png") on the GPU, byte-identical to OpenCV's default PNG parameters (src/common.cpp:66-71) --
     def encode_png_bgr_device(self, bgr, capacity=None):
         """imencode(".png", bgr) of a uint8 [H,W,3] BGR CUDA tensor (rows may be pitched), on the GPU.  Returns the bytes."""
-        import torch
         w, h = self._bgr_device(bgr)
         cap = self._L.dfb_png_max_bytes(w, h) if capacity is None else int(capacity)
         buf = np.empty(max(cap, 1), np.uint8)
         n = C.c_size_t()
-        s = torch.cuda.current_stream(bgr.device).cuda_stream
         self._check(self._L.dfb_encode_png_bgr_device(self._h, bgr.data_ptr(), bgr.stride(0), w, h, buf.ctypes.data, cap, C.byref(n),
-                                                      C.c_void_p(s)))
+                                                      _stream(bgr.device)))
         return buf[:n.value].tobytes()
-
-    @staticmethod
-    def _bgr_frames(frames_bgr, name):
-        frames = [np.asarray(f) for f in frames_bgr]
-        if any(f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 or f.shape != frames[0].shape for f in frames):
-            raise RuntimeError("%s: frames must be uint8 [H,W,3] images of one size" % name)
-        return [np.ascontiguousarray(f) for f in frames]
-
-    @staticmethod
-    def _file_buffers(m, cap):
-        """m host buffers of cap bytes for the files of one call: (buffers, their pointer array, the length array)"""
-        bufs = [np.empty(max(cap, 1), np.uint8) for _ in range(m)]
-        return bufs, (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in bufs]), (C.c_size_t * max(m, 1))()
 
     def process_bgr_batch_png(self, frames_bgr, step=1, new_size=None):
         """-st=png for decoded BGR frames: gray -> resize -> flow -> convertFlowToPngImage -> imencode(".png") on the GPU.
         frames_bgr: list of uint8 [H,W,3]; new_size: (w, h) or None.  Returns one PNG file (bytes) per pair, byte for byte
         calc_batch_png of the gray, resized frames."""
-        frames = self._bgr_frames(frames_bgr, "process_bgr_batch_png")
-        n = len(frames)
-        if n == 0:
+        if len(frames_bgr) == 0:
             return []
-        sh, sw = frames[0].shape[:2]
-        dw, dh = new_size if new_size else (0, 0)
-        m = max(n - abs(step), 0)
-        cap = self._L.dfb_png_max_bytes(*(new_size if new_size else (sw, sh)))
-        bufs, op, lens = self._file_buffers(m, cap)
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        self._check(self._L.dfb_process_bgr_batch_host_png(self._h, fp, n, step, sw, sh, dw, dh, op, cap, lens))
-        return [bufs[i][:lens[i]].tobytes() for i in range(m)]
+        keep, src, n, sw, sh = self._bgr_frames(frames_bgr, "process_bgr_batch_png")
+        (dw, dh), (ow, oh) = _sizes(new_size, sw, sh)
+        out, collect = _files(1, _pairs(n, step), self._L.dfb_png_max_bytes(ow, oh))
+        self._check(self._L.dfb_process_bgr_batch_host_png(self._h, *src, n, step, sw, sh, dw, dh, *out))
+        return collect()
 
     def process_jpeg_batch_png(self, jpegs, step=1, new_size=None):
         """-if -st=png: process_bgr_batch_png with the frames given as JPEG files of one size, decoded on the GPU to imdecode's
         pixels.  Returns one PNG file (bytes) per pair."""
-        keep, ptrs, lens = self._jpeg_buffers(jpegs)
-        n = len(keep)
-        dw, dh = new_size if new_size else (0, 0)
-        m = max(n - abs(step), 0)
-        cap = self._L.dfb_png_max_bytes(*(new_size if new_size else (self.max_width, self.max_height)))
-        bufs, op, plens = self._file_buffers(m, cap)
-        self._check(self._L.dfb_process_jpeg_batch_host_png(self._h, ptrs, lens, n, step, dw, dh, op, cap, plens))
-        return [bufs[i][:plens[i]].tobytes() for i in range(m)]
+        keep, src, n, w, h = self._jpeg_frames(jpegs)
+        (dw, dh), (ow, oh) = _sizes(new_size, w, h)
+        out, collect = _files(1, _pairs(n, step), self._L.dfb_png_max_bytes(ow, oh))
+        self._check(self._L.dfb_process_jpeg_batch_host_png(self._h, *src, n, step, dw, dh, *out))
+        return collect()
 
     def extract_frames_jpeg(self, jpegs, new_size=None, quality=95):
         """-if -s=0: extract_frames with the frames given as JPEG files of one size, decoded on the GPU to imdecode's pixels.
         Returns one JPEG bitstream per frame, in order (img_%05d.jpg)."""
-        keep, ptrs, lens = self._jpeg_buffers(jpegs)
-        n = len(keep)
+        keep, src, n, w, h = self._jpeg_frames(jpegs)
         if n == 0:
             return []
-        dw, dh = new_size if new_size else (0, 0)
-        cap = self._L.dfb_jpeg_max_bytes_bgr(*(new_size if new_size else (self.max_width, self.max_height)))
-        bufs, op, olens = self._file_buffers(n, cap)
-        self._check(self._L.dfb_extract_frames_jpeg_host(self._h, ptrs, lens, n, dw, dh, int(quality), op, cap, olens))
-        return [bufs[i][:olens[i]].tobytes() for i in range(n)]
+        (dw, dh), (ow, oh) = _sizes(new_size, w, h)
+        out, collect = _files(1, n, self._L.dfb_jpeg_max_bytes_bgr(ow, oh))
+        self._check(self._L.dfb_extract_frames_jpeg_host(self._h, *src, n, dw, dh, int(quality), *out))
+        return collect()
 
     def calc_batch_png(self, frames, step=1, out=None):
         """frames: sequence of uint8 [H,W] host arrays (or one [N,H,W] array).  Returns, for each of the M = max(N-|step|,0)
         pairs, the PNG file writeFlowImagesPng writes: imencode(".png", convertFlowToPngImage(flow)).  out: optional list of
         M uint8 host buffers (e.g. page-locked) of dfb_png_max_bytes(W, H) bytes or more to encode into."""
-        frames = self._gray_frames(frames)
-        n = len(frames)
-        if n == 0:
+        if len(frames) == 0:
             return []
-        h, w = frames[0].shape
-        m = max(n - abs(step), 0)
+        keep, src, n, w, h = self._gray_frames(frames)
+        m = _pairs(n, step)
         cap = self._L.dfb_png_max_bytes(w, h)
-        if out is None:
-            out = [np.empty(cap, np.uint8) for _ in range(m)]
-        if len(out) < m or any(not isinstance(b, np.ndarray) or b.dtype != np.uint8 or b.ndim != 1 or b.size < cap
-                               or not b.flags.c_contiguous for b in out[:m]):
+        if out is not None and (len(out) < m or any(not isinstance(b, np.ndarray) or b.dtype != np.uint8 or b.ndim != 1 or b.size < cap
+                                                    or not b.flags.c_contiguous for b in out[:m])):
             raise RuntimeError("out: expected %d C-contiguous uint8 buffers of at least %d bytes" % (m, cap))
-        fp = (C.c_void_p * n)(*[f.ctypes.data for f in frames])
-        op = (C.c_void_p * max(m, 1))(*[b.ctypes.data for b in out[:m]])
-        lens = (C.c_size_t * max(m, 1))()
-        self._check(self._L.dfb_calc_batch_host_png(self._h, fp, n, step, w, h, op, cap, lens))
-        return [out[i][:lens[i]].tobytes() for i in range(m)]
+        args, collect = _files(1, m, cap, None if out is None else [out[:m]])
+        self._check(self._L.dfb_calc_batch_host_png(self._h, *src, n, step, w, h, *args))
+        return collect()
 
     # -- test hook: one stand-alone kernel on host planes --
     def debug_run_kernel(self, kernel, inputs, n_out, scalars=(), out_shape=None, all_scalars=False):

@@ -150,6 +150,31 @@ def _stats(st):
             "kernel_launches": st.kernel_launches, "h2d_bytes": st.h2d_bytes, "d2h_bytes": st.d2h_bytes}
 
 
+def _call(L, fn, *args, stats=True):
+    """L.<fn>(*args, [&stats,] err, 512): raises the runner's message, or "<fn> failed (<rc>)" when it leaves none; returns the
+    dict of dfb_list_stats."""
+    st = _lib.ListStats()
+    err = C.create_string_buffer(512)
+    rc = getattr(L, fn)(*args, *([C.byref(st)] if stats else []), err, 512)
+    if rc != _lib.DFB_OK:
+        raise RuntimeError(err.value.decode() or "%s failed (%d)" % (fn, rc))
+    return _stats(st)
+
+
+def _files_per_flow(step, save_type):
+    """The files of one output in an on_chunk call: a flow's x and y (jpg, h5) or its PNG, or a frame's JPEG with step 0."""
+    if save_type not in _SAVE_TYPES:
+        raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
+    return 2 if step != 0 and save_type != "png" else 1
+
+
+def _on_files(on_chunk, per):
+    """A FILES_DONE_FN body: hands on_chunk(video, device, first_index, last_chunk, files) the chunk's files as bytes."""
+    def done(user, video, dev, first, n, last, files, lens):
+        on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
+    return done
+
+
 class ListRunner:
     """Workers kept alive between lists (dfb_list_open / dfb_list_run / dfb_list_close): worker i owns an engine handle on
     devices[i]; a device may appear more than once."""
@@ -158,23 +183,15 @@ class ListRunner:
         self._L = _lib.load(variant)
         self._r = C.c_void_p()
         devs = (C.c_int * len(devices))(*devices)
-        err = C.create_string_buffer(512)
-        rc = self._L.dfb_list_open(algorithm.encode(), devs, len(devices), int(max_width), int(max_height), C.byref(self._r), err, 512)
-        if rc != _lib.DFB_OK:
-            self._r = None
-            raise RuntimeError(err.value.decode() or "dfb_list_open failed (%d)" % rc)
+        _call(self._L, "dfb_list_open", algorithm.encode(), devs, len(devices), int(max_width), int(max_height), C.byref(self._r),
+              stats=False)  # a refused open leaves the runner null
 
     def run(self, clips, step=1, bound=32, chunk_flows=0, queue=None, on_chunk=None, packed=None):
         """packed: the result of a previous pack(clips) (building the pointer tables of a long list takes a while)."""
         arr, shapes, keep = packed if packed is not None else _pack_clips(clips)
         cb = _callback(on_chunk, shapes)
-        st = _lib.ListStats()
-        err = C.create_string_buffer(512)
-        rc = self._L.dfb_list_run(self._r, arr, len(shapes), int(step), int(bound), int(chunk_flows), queue._q if queue is not None else None,
-                                  C.cast(cb, C.c_void_p) if cb else None, None, C.byref(st), err, 512)
-        if rc != _lib.DFB_OK:
-            raise RuntimeError(err.value.decode() or "dfb_list_run failed (%d)" % rc)
-        return _stats(st)
+        return _call(self._L, "dfb_list_run", self._r, arr, len(shapes), int(step), int(bound), int(chunk_flows),
+                     queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None)
 
     def run_videos(self, videos, step=1, bound=20, save_type="jpg", quality=95, jpeg_exact=0, new_width=0, new_height=0, new_short=0,
                    chunk_flows=0, queue=None, on_chunk=None):
@@ -186,24 +203,12 @@ class ListRunner:
         files 2 i / 2 i + 1 are flow first_index + i's x / y plane as raw float32 [dh, dw] (writeHDF5's datasets, named by
         h5_names).  last_chunk is the
         reference's FlowBuffer::last_buffer.  Returns a dict of dfb_list_stats."""
-        if save_type not in _SAVE_TYPES:
-            raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
+        per = _files_per_flow(step, save_type)
         arr, keep = _pack_videos(videos)
-        per = 2 if step != 0 and save_type != "png" else 1
-        cb = None
-        if on_chunk is not None:
-            def _cb(user, video, dev, first, n, last, files, lens):
-                on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
-            cb = _lib.FILES_DONE_FN(_cb)
-        st = _lib.ListStats()
-        err = C.create_string_buffer(512)
-        rc = self._L.dfb_list_run_videos(self._r, arr, len(videos), int(step), int(bound), _SAVE_TYPES[save_type],
-                                         int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
-                                         queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None, C.byref(st),
-                                         err, 512)
-        if rc != _lib.DFB_OK:
-            raise RuntimeError(err.value.decode() or "dfb_list_run_videos failed (%d)" % rc)
-        return _stats(st)
+        cb = _lib.FILES_DONE_FN(_on_files(on_chunk, per)) if on_chunk is not None else None
+        return _call(self._L, "dfb_list_run_videos", self._r, arr, len(videos), int(step), int(bound), _SAVE_TYPES[save_type],
+                     int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
+                     queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None)
 
     def run_stream(self, n_videos, source, on_chunk=None, step=1, bound=20, save_type="jpg", quality=95, jpeg_exact=0, new_width=0,
                    new_height=0, new_short=0, chunk_flows=0, queue=None):
@@ -231,9 +236,8 @@ class ListRunner:
     def _run_source(self, fn, n_videos, source, on_chunk, step, bound, save_type, quality, jpeg_exact, new_width, new_height, new_short,
                     chunk_flows, queue):
         """run_stream and run_windows: the runner is done with each window once its on_chunk call has returned."""
-        if save_type not in _SAVE_TYPES:
-            raise RuntimeError("only jpg/png/h5 are supported (no %s) for output" % save_type)
-        per = 2 if step != 0 and save_type != "png" else 1
+        per = _files_per_flow(step, save_type)
+        deliver = _on_files(on_chunk, per) if on_chunk is not None else None
         windows = {}  # (video, first) -> a live window and the memory behind it
         failures = []
 
@@ -252,25 +256,22 @@ class ListRunner:
 
         def _done(user, video, dev, first, n, last, files, lens):
             try:
-                if on_chunk is not None and not failures:
-                    on_chunk(video, dev, first, bool(last), [C.string_at(files[i], lens[i]) for i in range(per * n)])
+                if deliver is not None and not failures:
+                    deliver(user, video, dev, first, n, last, files, lens)
             except BaseException as ex:
                 failures.append(ex)
             windows.pop((video, first), None)
 
         src = _lib.FRAMES_FN(_source)
         cb = _lib.FILES_DONE_FN(_done)
-        st = _lib.ListStats()
-        err = C.create_string_buffer(512)
-        rc = getattr(self._L, fn)(self._r, int(n_videos), C.cast(src, C.c_void_p), int(step), int(bound), _SAVE_TYPES[save_type],
-                                  int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
-                                  queue._q if queue is not None else None, C.cast(cb, C.c_void_p), None, C.byref(st), err, 512)
-        windows.clear()
-        if failures:
-            raise failures[0]
-        if rc != _lib.DFB_OK:
-            raise RuntimeError(err.value.decode() or "%s failed (%d)" % (fn, rc))
-        return _stats(st)
+        try:
+            return _call(self._L, fn, self._r, int(n_videos), C.cast(src, C.c_void_p), int(step), int(bound), _SAVE_TYPES[save_type],
+                         int(quality), int(jpeg_exact), int(new_width), int(new_height), int(new_short), int(chunk_flows),
+                         queue._q if queue is not None else None, C.cast(cb, C.c_void_p), None)
+        finally:
+            windows.clear()
+            if failures:  # an on_chunk failure is the cause of any refusal that followed it, and is raised instead
+                raise failures[0]
 
     @staticmethod
     def pack(clips):
@@ -298,10 +299,5 @@ def run_list(algorithm, devices, clips, step=1, bound=32, chunk_flows=0, queue=N
     arr, shapes, keep = _pack_clips(clips)
     cb = _callback(on_chunk, shapes)
     devs = (C.c_int * len(devices))(*devices)
-    st = _lib.ListStats()
-    err = C.create_string_buffer(512)
-    rc = L.dfb_run_list(algorithm.encode(), devs, len(devices), arr, len(clips), int(step), int(bound), int(chunk_flows),
-                        queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None, C.byref(st), err, 512)
-    if rc != _lib.DFB_OK:
-        raise RuntimeError(err.value.decode() or "dfb_run_list failed (%d)" % rc)
-    return _stats(st)
+    return _call(L, "dfb_run_list", algorithm.encode(), devs, len(devices), arr, len(clips), int(step), int(bound), int(chunk_flows),
+                 queue._q if queue is not None else None, C.cast(cb, C.c_void_p) if cb else None, None)
