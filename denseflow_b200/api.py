@@ -119,7 +119,9 @@ class DenseOpticalFlow:
     def set(self, name, value):
         """dfb_set_param: one algorithm parameter or engine knob (include/denseflow_b200.h lists them).  TV-L1 also takes
         "median_filtering" (0 or 1 = off [default], 3 or 5 = the window of a median of the flow between iterations) and
-        "median_interval" (>= 1, default 30: the median runs before iterations 0, I, 2I, ... of every warp).  Both algorithms
+        "median_interval" (>= 1, default 30: the median runs before iterations 0, I, 2I, ... of every warp) and "gamma"
+        (finite, >= 0, default 0: OpenCV's setGamma, the weight of an illumination field that absorbs brightness changes
+        between the two frames; both schedules take it and give the same bits).  Both algorithms
         take "use_initial_flow" (0 [default] or 1: OpenCV's useInitialFlow / OPTFLOW_USE_INITIAL_FLOW): with 1, the flow
         buffers of calc, calc_batch, calc_batch_device, calc_batch_planes and calc_batch_device_planes are read as each
         pair's starting flow before they are overwritten, so they must be passed, and every other flow call is refused.  A

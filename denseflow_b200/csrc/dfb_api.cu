@@ -1732,6 +1732,26 @@ int dfb_debug_run_kernel(dfb_handle *h, const char *kernel, const float *const *
             const Tvl1Consts c{0.f, (float)sc(0), 0.f};
             launch_estimate_dual(pin[0], pin[1], pin[2], pin[3], pin[4], pin[5], c, nullptr);
             inplace_from = 2;
+        } else if (k == "estimate_u_gamma") {  // estimate_u's inputs with p31, p32 after p22 and u3 after u2; scalars + gamma
+            need(13, 3);
+            const Tvl1Consts c{(float)sc(0), 0.f, (float)sc(1)};
+            const bool calc = sc(2) != 0;
+            const int nblk = estimate_u_blocks(width, height);
+            if (calc) {
+                d_part.allocate(sizeof(double) * nblk);
+                d_sum.allocate(sizeof(double));
+            }
+            launch_estimate_u_gamma(pin[0], pin[1], pin[2], pin[3], &pin[4], pin[10], pin[11], pin[12], c, (float)sc(3), d_part, nullptr);
+            if (calc) {
+                launch_sum_partials(d_part, nblk, d_sum, nullptr);
+                if (scalars_out) DFB_CUDA(cudaMemcpy(scalars_out, d_sum, sizeof(double), cudaMemcpyDeviceToHost));
+            }
+            inplace_from = 10;
+        } else if (k == "estimate_dual_gamma") {  // u1, u2, u3, p11 .. p32
+            need(9, 6);
+            const Tvl1Consts c{0.f, (float)sc(0), 0.f};
+            launch_estimate_dual_gamma(pin[0], pin[1], pin[2], &pin[3], c, nullptr);
+            inplace_from = 3;
         } else if (k == "resize") {
             need(1, 1);
             pout = {alloc(ow, oh, opitch)};

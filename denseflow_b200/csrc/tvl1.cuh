@@ -75,6 +75,11 @@ void launch_estimate_u(Plane I1wx, Plane I1wy, Plane grad, Plane rho_c, Plane p1
                        Plane u1, Plane u2, Tvl1Consts c, double *err_partials, cudaStream_t s);
 void launch_estimate_dual(Plane u1, Plane u2, Plane p11, Plane p12, Plane p21, Plane p22, Tvl1Consts c,
                           cudaStream_t s);
+// gamma > 0 (SURVEY A.8): the same two half-steps with the illumination field u3; p = {p11, p12, p21, p22, p31, p32}.  The
+// error partials (estimate_u_blocks of them) sum (du1)^2 + (du2)^2 only.
+void launch_estimate_u_gamma(Plane I1wx, Plane I1wy, Plane grad, Plane rho_c, const Plane *p, Plane u1, Plane u2, Plane u3, Tvl1Consts c,
+                             float gamma, double *err_partials, cudaStream_t s);
+void launch_estimate_dual_gamma(Plane u1, Plane u2, Plane u3, const Plane *p, Tvl1Consts c, cudaStream_t s);
 // fixed-order sum of n partials into *out (device or mapped host memory)
 void launch_sum_partials(const double *partials, int n, double *out, cudaStream_t s);
 void launch_fill(Plane dst, float v, cudaStream_t s);

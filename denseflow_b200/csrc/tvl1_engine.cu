@@ -41,6 +41,7 @@ struct Tvl1Params {
     int median_filtering = 0;  // 3 or 5: the window of the median of u1, u2 between iterations (DESIGN §4.3); 0 or 1: off
     int median_interval = 30;  // the median runs before every iteration n of a warp with n % median_interval == 0
     int use_initial_flow = 0;  // 1: each pair starts from the flow its call passes in (PairJob::init_x; DESIGN §1)
+    double gamma = 0;  // > 0: weight of the illumination field u3 (SURVEY A.8; DESIGN §4.3)
     int median_k() const { return median_filtering > 1 ? median_filtering : 0; }
 };
 
@@ -60,6 +61,8 @@ class Tvl1 final : public FlowAlgorithm {
         if (stats_event_) cudaEventDestroy(stats_event_);
         if (pair_log_) cudaFreeHost(pair_log_);
         if (unfused_scratch_) cudaFree(unfused_scratch_);
+        for (auto &l : lanes_)
+            if (l.gamma_own) cudaFree(l.gamma_own);
         for (int r = 0; r < kJobRing; ++r) {
             if (job_ring_h_[r]) cudaFreeHost(job_ring_h_[r]);
             if (job_ring_d_[r]) cudaFree(job_ring_d_[r]);
@@ -91,6 +94,7 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "median_filtering") { if (!(v == 0 || v == 1 || v == 3 || v == 5)) return false; prm_.median_filtering = (int)v; }
         else if (k == "median_interval") { if (!whole_in(v, 1, INT_MAX)) return false; prm_.median_interval = (int)v; }
         else if (k == "use_initial_flow") { if (!is_flag(v)) return false; prm_.use_initial_flow = (int)v; }
+        else if (k == "gamma") { if (!(std::isfinite(v) && v >= 0)) return false; prm_.gamma = v; }
         else return false;
         return true;
     }
@@ -111,6 +115,7 @@ class Tvl1 final : public FlowAlgorithm {
         else if (k == "median_filtering") *v = prm_.median_filtering;
         else if (k == "median_interval") *v = prm_.median_interval;
         else if (k == "use_initial_flow") *v = prm_.use_initial_flow;
+        else if (k == "gamma") *v = prm_.gamma;
         else return false;
         return true;
     }
@@ -164,7 +169,7 @@ class Tvl1 final : public FlowAlgorithm {
         const int sms = fused_cta_slots(device_);
         const int hy = prm_.fused_k, hx = (hy + 3) & ~3;
         // lanes are sized for the handle's MAXIMUM frame: keep their total workspace under 8 GB
-        const size_t lane_bytes = 4 * Slab::padded(pyr_elems_, 4) + 14 * Slab::padded(plane_elems_, 4);
+        const size_t lane_bytes = 4 * Slab::padded(pyr_elems_, 4) + 14 * Slab::padded(plane_elems_, 4) + (prm_.gamma > 0 ? gamma_lane_bytes() : 0);
         const int mem_cap = (int)std::max<size_t>(1, (size_t(8) << 30) / std::max<size_t>(lane_bytes, 1));
         const int maxB = std::min(kFusedMaxLanes, mem_cap);
         double util[kFusedMaxLanes + 1] = {};
@@ -550,6 +555,8 @@ class Tvl1 final : public FlowAlgorithm {
         unsigned *sync = nullptr;
         FusedHostCtl *host_ctl = nullptr, *dev_ctl = nullptr;
         void *tmaps = nullptr;  // device array CUtensorMap[kMaxScales][kFusedMapsPerLevel]
+        void *gamma_own = nullptr;  // gamma > 0 (ensure_gamma_lanes): the u3 pyramid and p31 / p32
+        float *u3pyr = nullptr, *p3[2] = {};
         int tmap_w = 0, tmap_h = 0, tmap_n = 0;
         double tmap_ss = 0;
     };
@@ -587,6 +594,24 @@ class Tvl1 final : public FlowAlgorithm {
     }
 
     Plane work(float *p, const LevelGeom &g) const { return Plane{p, g.w, g.h, g.pitch}; }
+
+    // gamma > 0: each lane's u3 pyramid and p31 / p32 planes, allocated when a gamma solve first needs the lane
+    size_t gamma_lane_bytes() const { return Slab::padded(pyr_elems_, 4) + 2 * Slab::padded(plane_elems_, 4); }
+    void ensure_gamma_lanes(int n) {
+        ensure_lanes(n);
+        for (int i = 0; i < n; ++i) {
+            Lane &l = lanes_[i];
+            if (l.gamma_own) continue;
+            const size_t pyr = Slab::padded(pyr_elems_, 4), pl = Slab::padded(plane_elems_, 4);
+            DFB_CUDA(cudaMalloc(&l.gamma_own, gamma_lane_bytes()));
+            DFB_CUDA(cudaMemset(l.gamma_own, 0, gamma_lane_bytes()));  // padding columns are read (never used) by the vector loads
+            DFB_CUDA(cudaDeviceSynchronize());  // null-stream memset vs the caller's (possibly non-blocking) stream
+            char *c = static_cast<char *>(l.gamma_own);
+            l.u3pyr = reinterpret_cast<float *>(c);
+            l.p3[0] = reinterpret_cast<float *>(c + pyr);
+            l.p3[1] = reinterpret_cast<float *>(c + pyr + pl);
+        }
+    }
 
     // use_initial_flow: the initial fields of the pairs jobs[i] that carry one (PairJob::init_x) into lane i's flow pyramid
     // u1pyr[0] / u2pyr[0], enqueued before the solve.  Level 0 is the field as given; level s is resize_linear of level s - 1
@@ -627,6 +652,9 @@ class Tvl1 final : public FlowAlgorithm {
     void solve_unfused(int slot_a, int slot_b, const LevelGeom *lv, int n, float *flow_xy, size_t flow_pitch_bytes,
                        cudaStream_t s, float *fx = nullptr, float *fy = nullptr, size_t f_pitch = 0, bool init = false) {
         const Tvl1Consts c{(float)(prm_.lambda * prm_.theta), (float)(prm_.tau / prm_.theta), (float)prm_.theta};
+        const bool gam = prm_.gamma > 0;
+        const float gamma = (float)prm_.gamma;
+        if (gam) ensure_gamma_lanes(1);
         std::memset(last_iters_, 0, sizeof(last_iters_));
         Lane &wk = lanes_[0];
         float *I0b = slots_.at(slot_a), *I1b = slots_.at(slot_b);
@@ -640,6 +668,20 @@ class Tvl1 final : public FlowAlgorithm {
             if (l == n - 1 && !init) {  // useInitialFlow = false
                 launch_fill(u1, 0.f, s);
                 launch_fill(u2, 0.f, s);
+                launches += 2;
+            }
+            // gamma: u3 starts at 0 on the coarsest level (initial flow or not), p31 / p32 at every scale like p11 .. p22
+            Plane u3{}, pg[6] = {p11, p12, p21, p22, {}, {}};
+            if (gam) {
+                u3 = level_plane(wk.u3pyr, lv, l);
+                pg[4] = work(wk.p3[0], g);
+                pg[5] = work(wk.p3[1], g);
+                if (l == n - 1) {
+                    launch_fill(u3, 0.f, s);
+                    ++launches;
+                }
+                launch_fill(pg[4], 0.f, s);
+                launch_fill(pg[5], 0.f, s);
                 launches += 2;
             }
             launch_centered_gradient(I1, I1x, I1y, s);
@@ -665,8 +707,11 @@ class Tvl1 final : public FlowAlgorithm {
                         DFB_CUDA(cudaMemcpy2DAsync(u2.p, (size_t)u2.pitch * 4, m2.p, (size_t)m2.pitch * 4, (size_t)g.w * 4, g.h, cudaMemcpyDeviceToDevice, s));
                     }
                     const bool calc_error = prm_.epsilon > 0 && (it & 1) && prev_error < scaled_eps;
-                    launch_estimate_u(I1wx, I1wy, grad, rho_c, p11, p12, p21, p22, u1, u2, c,
-                                      calc_error ? wk.partials : nullptr, s);
+                    if (gam)
+                        launch_estimate_u_gamma(I1wx, I1wy, grad, rho_c, pg, u1, u2, u3, c, gamma, calc_error ? wk.partials : nullptr, s);
+                    else
+                        launch_estimate_u(I1wx, I1wy, grad, rho_c, p11, p12, p21, p22, u1, u2, c,
+                                          calc_error ? wk.partials : nullptr, s);
                     ++launches;
                     if (calc_error) {
                         launch_sum_partials(wk.partials, nblk, &wk.dev_ctl->error, s);
@@ -678,7 +723,10 @@ class Tvl1 final : public FlowAlgorithm {
                         error = DBL_MAX;
                         prev_error -= scaled_eps;
                     }
-                    launch_estimate_dual(u1, u2, p11, p12, p21, p22, c, s);
+                    if (gam)
+                        launch_estimate_dual_gamma(u1, u2, u3, pg, c, s);
+                    else
+                        launch_estimate_dual(u1, u2, p11, p12, p21, p22, c, s);
                     ++launches;
                 }
                 last_iters_[l * prm_.warps + wi] = it;
@@ -690,6 +738,10 @@ class Tvl1 final : public FlowAlgorithm {
                 launch_resize_linear(u1, level_plane(wk.u1pyr[0], lv, l - 1), ufx, ufy, mul, s);
                 launch_resize_linear(u2, level_plane(wk.u2pyr[0], lv, l - 1), ufx, ufy, mul, s);
                 launches += 2;
+                if (gam) {  // u3 is an intensity, not a displacement: no 1 / scaleStep
+                    launch_resize_linear(u3, level_plane(wk.u3pyr, lv, l - 1), ufx, ufy, 1.0f, s);
+                    ++launches;
+                }
             }
         }
         launch_merge_flow(level_plane(wk.u1pyr[0], lv, 0), level_plane(wk.u2pyr[0], lv, 0), flow_xy, flow_pitch_bytes, s, fx, fy, f_pitch);
@@ -806,7 +858,20 @@ class Tvl1 final : public FlowAlgorithm {
         }
         batch.jobs = job_ring_d_[jr];
         batch.host_jobs = host_jobs;
-        launches += launch_tvl1_fused(batch, device_, s);
+        if (prm_.gamma > 0) {  // the gamma kernel: its planes travel beside the jobs
+            ensure_gamma_lanes(count);
+            if (!gamma_params_) gamma_params_.reset(new FusedGamma());
+            FusedGamma &gm = *gamma_params_;
+            gm.gamma = (float)prm_.gamma;
+            for (int i = 0; i < count; ++i) {
+                for (int l = 0; l < n; ++l) gm.lane[i].u3[l] = level_plane(lanes_[i].u3pyr, lv, l).p;
+                gm.lane[i].p31 = lanes_[i].p3[0];
+                gm.lane[i].p32 = lanes_[i].p3[1];
+            }
+            launches += launch_tvl1_fused(batch, device_, s, &gm);
+        } else {
+            launches += launch_tvl1_fused(batch, device_, s);
+        }
         if (prm_.time_kernels) timer_.end(s, 1, count);
         last_lane_ = count - 1;
         DFB_CUDA(cudaEventRecord(stats_event_, s));
@@ -830,6 +895,7 @@ class Tvl1 final : public FlowAlgorithm {
             l.host_ctl->px_chunks_total = 0;
         }
     }
+    std::unique_ptr<FusedGamma> gamma_params_;  // copied into the launch's parameters
     uint64_t unfused_px_iters_ = 0;
     float *unfused_scratch_ = nullptr;
     static constexpr int kJobRing = 8;

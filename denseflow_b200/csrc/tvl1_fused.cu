@@ -956,6 +956,152 @@ __global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_stage(const 
     lane_exit(job.sync, G);
 }
 
+// ---- gamma > 0 (SURVEY A.8) ----------------------------------------------------------------------------------------------
+// The per-pair structure of k_tvl1_pair (level start, warps, the A.4 state machine on the device, upsample, merge, median,
+// lanes and their grid barriers) with the inner loop as two pixel-parallel passes per iteration, each followed by the lane's
+// grid barrier: the primal step (tvl1_gamma_primal_quad) in place on u1, u2, u3, then the dual step (tvl1_gamma_dual_quad)
+// in place on the six dual planes.  The quad functions are the ones the stand-alone gamma kernels run, so the two schedules
+// give the same bits.  The tile loop is not used: fused_k, use_tma and resident levels do not apply to it (DESIGN §4.3).
+__device__ __forceinline__ void gamma_primal(const int G, const int bid, const FusedJob &job, const FusedLevel &L, int cur, float *u3,
+                                             const FusedGammaLane &gl, float gamma, bool calc, int part_sel, Smem &sm) {
+    const int W = L.w, H = L.h, P = L.pitch, qx = (W + 3) >> 2;
+    const float *p[6] = {job.p[cur][0], job.p[cur][1], job.p[cur][2], job.p[cur][3], gl.p31, gl.p32};
+    double err = 0.0;
+    for (int i = bid * kThreads + threadIdx.x; i < H * qx; i += G * kThreads) {
+        const int y = i / qx, x0 = (i - y * qx) << 2;
+        const float4 gq = *reinterpret_cast<const float4 *>(job.grad + (size_t)y * P + x0);  // phase_warp stored the gq form
+        if (calc)
+            err += tvl1_gamma_primal_quad<true>(job.I1wx, job.I1wy, gq, job.rho_c, p, L.u1[cur], L.u2[cur], u3, x0, y, W, P, job.c, gamma);
+        else
+            tvl1_gamma_primal_quad<false>(job.I1wx, job.I1wy, gq, job.rho_c, p, L.u1[cur], L.u2[cur], u3, x0, y, W, P, job.c, gamma);
+    }
+    if (calc) {  // fixed order: warp shuffle tree, then thread 0 adds the warp sums
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) err += __shfl_xor_sync(0xffffffffu, err, o);
+        if ((threadIdx.x & 31) == 0) sm.red[threadIdx.x >> 5] = err;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double bs = 0.0;
+            for (int k = 0; k < kWarps; ++k) bs += sm.red[k];
+            job.partials[part_sel * kPartialSet + bid] = bs;
+        }
+    }
+}
+__device__ __forceinline__ void gamma_dual(const int G, const int bid, const FusedJob &job, const FusedLevel &L, int cur, const float *u3,
+                                           const FusedGammaLane &gl) {
+    const int W = L.w, H = L.h, P = L.pitch, qx = (W + 3) >> 2;
+    float *p[6] = {job.p[cur][0], job.p[cur][1], job.p[cur][2], job.p[cur][3], gl.p31, gl.p32};
+    for (int i = bid * kThreads + threadIdx.x; i < H * qx; i += G * kThreads) {
+        const int y = i / qx, x0 = (i - y * qx) << 2;
+        tvl1_gamma_dual_quad(L.u1[cur], L.u2[cur], u3, p, x0, y, W, H, P, job.c.taut);
+    }
+}
+// level start of the gamma planes: p31 = p32 = 0 at every scale, u3 = 0 at the coarsest (also with init_flow)
+__device__ __forceinline__ void gamma_level_start(const int G, const int bid, const FusedLevel &L, const FusedGammaLane &gl, float *u3, bool coarsest) {
+    const int total = L.h * (L.pitch >> 2);
+    for (int i = bid * kThreads + threadIdx.x; i < total; i += G * kThreads) {
+        const size_t o = (size_t)i << 2;
+        st4(gl.p31 + o, zero4());
+        st4(gl.p32 + o, zero4());
+        if (coarsest) st4(u3 + o, zero4());
+    }
+}
+// u3 to the next finer level: the flow's resize (phase_upsample, k_resize_linear) without the 1 / scale_step factor
+__device__ __forceinline__ void gamma_upsample(const int G, const int bid, const FusedLevel &L, const FusedLevel &F, const float *src, float *dst) {
+    const int total = F.h * F.w;
+    for (int i = bid * kThreads + threadIdx.x; i < total; i += G * kThreads) {
+        const int dy = i / F.w, dx = i - dy * F.w;
+        const float sx = dx * L.up_fx, sy = dy * L.up_fy;
+        const int x1 = __float2int_rd(sx), y1 = __float2int_rd(sy);
+        const int x2 = x1 + 1, y2 = y1 + 1;
+        const size_t r1 = (size_t)min(y1, L.h - 1) * L.pitch, r2 = (size_t)min(y2, L.h - 1) * L.pitch;
+        const int x1r = min(x1, L.w - 1), x2r = min(x2, L.w - 1);
+        float o = 0.f;
+        o = o + __ldcg(src + r1 + x1r) * ((x2 - sx) * (y2 - sy));
+        o = o + __ldcg(src + r1 + x2r) * ((sx - x1) * (y2 - sy));
+        o = o + __ldcg(src + r2 + x1r) * ((x2 - sx) * (sy - y1));
+        o = o + __ldcg(src + r2 + x2r) * ((sx - x1) * (sy - y1));
+        dst[(size_t)dy * F.pitch + dx] = o;
+    }
+}
+
+template <class Batch>
+__global__ void __launch_bounds__(kThreads, kFusedCtasPerSm) k_tvl1_pair_gamma(const __grid_constant__ Batch batch, const __grid_constant__ FusedGamma gm) {
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    Smem &sm = *reinterpret_cast<Smem *>(smem_raw);
+    const int G = batch.group;
+    const int lane_id = blockIdx.x / G, bid = blockIdx.x - lane_id * G;
+    const FusedJob &job = job_of(batch, lane_id, sm);
+    const FusedGammaLane &gl = gm.lane[lane_id];
+    unsigned epoch = 0;
+    unsigned *bar = job.sync;
+    int cur = 0, part_sel = 0;
+    unsigned long long px_iters = 0;
+    Prof prof;
+    prof.init(sm.prof, bid == 0);
+    cta_setup(sm);
+    for (int s = job.nscales - 1; s >= 0; --s) {
+        const FusedLevel &L = job.lv[s];
+        float *u3 = gl.u3[s];
+        cur = 0;
+        phase_level_start(G, bid, job, L, s == job.nscales - 1 && !job.init_flow);
+        gamma_level_start(G, bid, L, gl, u3, s == job.nscales - 1);
+        prof.mark(0);
+        grid_barrier(bar, epoch, G, job.ctl);
+        prof.mark(3);
+        const double scaled_eps = job.epsilon * job.epsilon * (double)((long long)L.w * L.h);  // A.4
+        for (int wi = 0; wi < job.warps; ++wi) {
+            phase_warp(G, bid, job, L, cur);
+            prof.mark(1);
+            grid_barrier(bar, epoch, G, job.ctl);
+            prof.mark(3);
+            double error = DBL_MAX, prev_error = 0.0;
+            int n = 0;
+            for (; error > scaled_eps && n < job.iterations; ++n) {
+                if (job.median_k && n % job.median_interval == 0) {  // u1, u2 only; the A.4 state does not change
+                    phase_median(G, bid, job, L, cur, sm);
+                    prof.mark(24);
+                    grid_barrier(bar, epoch, G, job.ctl);
+                    prof.mark(3);
+                    cur ^= 1;
+                }
+                const bool calc = job.epsilon > 0 && (n & 1) && prev_error < scaled_eps;
+                gamma_primal(G, bid, job, L, cur, u3, gl, gm.gamma, calc, part_sel, sm);
+                prof.mark(2, s < 8 ? 8 + s : -1);
+                grid_barrier(bar, epoch, G, job.ctl);
+                prof.mark(3);
+                if (calc) {
+                    error = lane_error(job, G, part_sel, sm);
+                    part_sel ^= 1;
+                    prev_error = error;
+                } else {
+                    error = DBL_MAX;
+                    prev_error -= scaled_eps;
+                }
+                gamma_dual(G, bid, job, L, cur, u3, gl);
+                prof.mark(2, s < 8 ? 8 + s : -1);
+                grid_barrier(bar, epoch, G, job.ctl);
+                prof.mark(3);
+            }
+            if (bid == 0 && threadIdx.x == 0) job.iters_log[s * job.warps + wi] = n;
+            px_iters += (unsigned long long)n * (unsigned long long)(L.w * L.h);
+        }
+        if (s > 0) {
+            phase_upsample(G, bid, job, L, job.lv[s - 1], cur);
+            gamma_upsample(G, bid, L, job.lv[s - 1], u3, gl.u3[s - 1]);
+            prof.mark(4);
+            grid_barrier(bar, epoch, G, job.ctl);
+            prof.mark(3);
+        }
+    }
+    phase_merge(G, bid, job, job.lv[0], cur);
+    prof.mark(4);
+    if (prof.on)
+        for (int i = 0; i < 32; ++i) job.ctl->prof[i] = prof.acc[i];
+    if (bid == 0 && threadIdx.x == 0) job.ctl->px_iters_total += px_iters;
+    lane_exit(bar, G);
+}
+
 }  // namespace
 
 void fused_encode_tensor_map(void *out, const float *plane, int w, int h, int pitch) {
@@ -1012,7 +1158,7 @@ void launch_tvl1_stage(const FusedBatch &batch, const FusedStageArgs &a, cudaStr
     DFB_CUDA(cudaLaunchKernelEx(&cfg, k_tvl1_stage, param_batch(batch), a));
 }
 
-int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s) {
+int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, const FusedGamma *gm) {
     // the opt-in shared-memory size is a per-device function attribute: handles on several devices may live in one process
     static std::mutex mtx;
     static bool configured[64] = {};
@@ -1024,6 +1170,8 @@ int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s) {
             configure_kernel(k_tvl1_pair<FusedBatchParams, false>, "k_tvl1_pair");
             configure_kernel(k_tvl1_pair<FusedBatch, true>, "k_tvl1_pair");
             configure_kernel(k_tvl1_pair<FusedBatchParams, true>, "k_tvl1_pair");
+            configure_kernel(k_tvl1_pair_gamma<FusedBatch>, "k_tvl1_pair_gamma");
+            configure_kernel(k_tvl1_pair_gamma<FusedBatchParams>, "k_tvl1_pair_gamma");
             configured[d] = true;
         }
     }
@@ -1037,6 +1185,14 @@ int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s) {
     // lanes leave behind (+3.8 % on the 340x256 list, 4020 vs 3873 pairs/s).  The block scheduler hands out a later grid's
     // CTAs only after every CTA of the earlier grid has been placed, so an earlier grid is never starved by a later one; a
     // lost arrival would still surface through the barrier watchdog rather than hang.
+    static_assert(sizeof(FusedBatchParams) + sizeof(FusedGamma) <= 32764, "the gamma kernel's parameters fit the parameter space");
+    if (gm) {
+        if (batch.njobs <= kFusedParamLanes)
+            DFB_CUDA(cudaLaunchKernelEx(&cfg, k_tvl1_pair_gamma<FusedBatchParams>, param_batch(batch), *gm));
+        else
+            DFB_CUDA(cudaLaunchKernelEx(&cfg, k_tvl1_pair_gamma<FusedBatch>, batch, *gm));
+        return 1;
+    }
     const bool median = batch.host_jobs[0].median_k > 0;  // every lane of a launch has its handle's parameters
     if (batch.njobs <= kFusedParamLanes) {
         DFB_CUDA(cudaLaunchKernelEx(&cfg, median ? k_tvl1_pair<FusedBatchParams, true> : k_tvl1_pair<FusedBatchParams, false>,

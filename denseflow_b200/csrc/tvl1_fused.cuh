@@ -95,8 +95,18 @@ inline int fused_cta_slots(int device) { return fused_num_sms(device) * kFusedCt
 // into out[128 bytes].
 // plane: base pointer, extent w x h (elements / rows), row pitch in elements.
 void fused_encode_tensor_map(void *out, const float *plane, int w, int h, int pitch);
-// returns the number of kernels launched
-int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s);
+// gamma > 0 (SURVEY A.8): lane i's illumination field (u3[l]: level l of its pyramid) and dual planes p31, p32.  Passed beside
+// the jobs rather than in FusedJob, so k_tvl1_pair's job layout and code do not change.
+struct FusedGammaLane {
+    float *u3[16];
+    float *p31, *p32;
+};
+struct FusedGamma {
+    float gamma;
+    FusedGammaLane lane[kFusedMaxLanes];
+};
+// returns the number of kernels launched; gm non-null (gamma > 0): the gamma kernel k_tvl1_pair_gamma (DESIGN §4.3)
+int launch_tvl1_fused(const FusedBatch &batch, int device, cudaStream_t s, const FusedGamma *gm = nullptr);
 
 // Test hook: one phase of k_tvl1_pair (its own device functions) on up to kFusedParamLanes lanes in one cooperative launch.
 enum FusedStage : int {

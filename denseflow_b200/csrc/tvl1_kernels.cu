@@ -183,6 +183,49 @@ __global__ void __launch_bounds__(BX *BY)
     st4(p22.p + i, b22);
 }
 
+// The error partials of a block: the fixed warp-shuffle / shared-memory tree of k_estimate_u
+__device__ __forceinline__ void block_err_partial(double err, double *__restrict__ err_partials) {
+    __shared__ double warp_sums[BY];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) err += __shfl_xor_sync(0xffffffffu, err, o);
+    if (threadIdx.x == 0) warp_sums[threadIdx.y] = err;
+    __syncthreads();
+    if (threadIdx.x == 0 && threadIdx.y == 0) {
+        double s = 0.0;
+#pragma unroll
+        for (int k = 0; k < BY; ++k) s += warp_sums[k];
+        err_partials[blockIdx.y * gridDim.x + blockIdx.x] = s;
+    }
+}
+
+// gamma > 0 (SURVEY A.8): k_estimate_u with the illumination field u3 and its dual planes p31, p32 (tvl1_gamma_primal_quad).
+// 64 B/px.
+template <bool CALC_ERROR>
+__global__ void __launch_bounds__(BX *BY)
+    k_estimate_u_gamma(Plane I1wx, Plane I1wy, Plane grad, Plane rho_c, Plane p11, Plane p12, Plane p21, Plane p22, Plane p31, Plane p32,
+                       Plane u1, Plane u2, Plane u3, Tvl1Consts c, float gamma, double *__restrict__ err_partials) {
+    const int x0 = 4 * (blockIdx.x * BX + threadIdx.x);
+    const int y = blockIdx.y * BY + threadIdx.y;
+    double err = 0.0;
+    if (y < u1.h && x0 < u1.w) {
+        const float4 g = ld4(grad.p + (size_t)y * u1.pitch + x0);
+        const float4 gq = make_float4(tvl1_gq_from_grad(g.x), tvl1_gq_from_grad(g.y), tvl1_gq_from_grad(g.z), tvl1_gq_from_grad(g.w));
+        const float *p[6] = {p11.p, p12.p, p21.p, p22.p, p31.p, p32.p};
+        err = tvl1_gamma_primal_quad<CALC_ERROR>(I1wx.p, I1wy.p, gq, rho_c.p, p, u1.p, u2.p, u3.p, x0, y, u1.w, u1.pitch, c, gamma);
+    }
+    if (CALC_ERROR) block_err_partial(err, err_partials);
+}
+
+// gamma > 0: k_estimate_dual with p31, p32 from the forward differences of the new u3 (tvl1_gamma_dual_quad).  60 B/px.
+__global__ void __launch_bounds__(BX *BY)
+    k_estimate_dual_gamma(Plane u1, Plane u2, Plane u3, Plane p11, Plane p12, Plane p21, Plane p22, Plane p31, Plane p32, Tvl1Consts c) {
+    const int x0 = 4 * (blockIdx.x * BX + threadIdx.x);
+    const int y = blockIdx.y * BY + threadIdx.y;
+    if (y >= u1.h || x0 >= u1.w) return;
+    float *p[6] = {p11.p, p12.p, p21.p, p22.p, p31.p, p32.p};
+    tvl1_gamma_dual_quad(u1.p, u2.p, u3.p, p, x0, y, u1.w, u1.h, u1.pitch, c.taut);
+}
+
 __global__ void k_sum_partials(const double *__restrict__ partials, int n, double *out) {
     // fixed-order tree: thread t sums partials[t], [t+256], ...; then a fixed shuffle/smem tree
     double s = 0.0;
@@ -294,6 +337,21 @@ void launch_estimate_u(Plane I1wx, Plane I1wy, Plane grad, Plane rho_c, Plane p1
 void launch_estimate_dual(Plane u1, Plane u2, Plane p11, Plane p12, Plane p21, Plane p22, Tvl1Consts c,
                           cudaStream_t s) {
     k_estimate_dual<<<grid2d(u1.w, u1.h, 4), dim3(BX, BY), 0, s>>>(u1, u2, p11, p12, p21, p22, c);
+    DFB_KERNEL_CHECK();
+}
+void launch_estimate_u_gamma(Plane I1wx, Plane I1wy, Plane grad, Plane rho_c, const Plane *p, Plane u1, Plane u2, Plane u3, Tvl1Consts c,
+                             float gamma, double *err_partials, cudaStream_t s) {
+    const dim3 g = grid2d(u1.w, u1.h, 4);
+    if (err_partials)
+        k_estimate_u_gamma<true><<<g, dim3(BX, BY), 0, s>>>(I1wx, I1wy, grad, rho_c, p[0], p[1], p[2], p[3], p[4], p[5], u1, u2, u3, c, gamma,
+                                                            err_partials);
+    else
+        k_estimate_u_gamma<false><<<g, dim3(BX, BY), 0, s>>>(I1wx, I1wy, grad, rho_c, p[0], p[1], p[2], p[3], p[4], p[5], u1, u2, u3, c, gamma,
+                                                             nullptr);
+    DFB_KERNEL_CHECK();
+}
+void launch_estimate_dual_gamma(Plane u1, Plane u2, Plane u3, const Plane *p, Tvl1Consts c, cudaStream_t s) {
+    k_estimate_dual_gamma<<<grid2d(u1.w, u1.h, 4), dim3(BX, BY), 0, s>>>(u1, u2, u3, p[0], p[1], p[2], p[3], p[4], p[5], c);
     DFB_KERNEL_CHECK();
 }
 void launch_sum_partials(const double *partials, int n, double *out, cudaStream_t s) {

@@ -144,6 +144,144 @@ __device__ __forceinline__ void tvl1_dual_row(const float4 &c1, const float4 &c2
     tvl1_dual_px(r1 - c1.w, d1.w - c1.w, r2 - c2.w, d2.w - c2.w, taut, p11.w, p12.w, p21.w, p22.w);
 }
 
+// ---- gamma > 0: the illumination field u3 with its dual planes p31, p32 (SURVEY A.8) -------------------------------------
+// The gamma = 0 functions above keep their instruction sequence; these are used only by the gamma kernels.  The decision f
+// is the one of tvl1_primal_px with gamma * u3 added to rho, and u3 moves by f * gamma; the convergence error stays
+// (du1)^2 + (du2)^2.
+#ifdef DFB_STRICT_FP
+// rho = rho_c + ((I1wx*u1 + I1wy*u2) + gamma*u3), the reference's parenthesised sum
+__device__ __forceinline__ void tvl1_primal_px_g(float ix, float iy, float g, float rc, float u1o, float u2o, float u3o, float div1,
+                                                 float div2, float div3, const Tvl1Consts &c, float gamma, float &u1n, float &u2n,
+                                                 float &u3n) {
+    const float rho = rc + ((ix * u1o + iy * u2o) + gamma * u3o);
+    const float thr = c.l_t * g;
+    float f = g > FLT_EPSILON ? f_div(-rho, g) : 0.f;
+    f = rho > thr ? -c.l_t : f;
+    f = rho < -thr ? c.l_t : f;
+    const float d1 = f * ix, d2 = f * iy, d3 = f * gamma;
+    u1n = (u1o + d1) + c.theta * div1;
+    u2n = (u2o + d2) + c.theta * div2;
+    u3n = (u3o + d3) + c.theta * div3;
+}
+#else
+// rho = rho_c + gamma*u3 + I1wy*u2 + I1wx*u1 as three chained FMAs;  u3' = u3 + f*gamma + theta*div3 like u1, u2
+__device__ __forceinline__ void tvl1_primal_px_g(float ix, float iy, float gq, float rc, float u1o, float u2o, float u3o, float div1,
+                                                 float div2, float div3, const Tvl1Consts &c, float gamma, float &u1n, float &u2n,
+                                                 float &u3n) {
+    const float rho = __fmaf_rn(ix, u1o, __fmaf_rn(iy, u2o, __fmaf_rn(gamma, u3o, rc)));
+    const float f = fminf(fmaxf(__fmul_rn(rho, gq), -c.l_t), c.l_t);
+    u1n = __fmaf_rn(c.theta, div1, __fmaf_rn(f, ix, u1o));
+    u2n = __fmaf_rn(c.theta, div2, __fmaf_rn(f, iy, u2o));
+    u3n = __fmaf_rn(c.theta, div3, __fmaf_rn(f, gamma, u3o));
+}
+#endif
+
+// Dual half-step of one field (u3: p31, p32), |grad u3| exactly as tvl1_dual_px takes |grad u1|
+__device__ __forceinline__ void tvl1_dual_px1(float ux, float uy, float taut, float &pa, float &pb) {
+#ifdef DFB_STRICT_FP
+    const float ng = 1.0f + taut * f_hypot(ux, uy);
+    pa = f_div(pa + taut * ux, ng);
+    pb = f_div(pb + taut * uy, ng);
+#else
+    const float r = f_rcp(__fmaf_rn(taut, f_sqrt(__fmaf_rn(ux, ux, __fmul_rn(uy, uy))), 1.0f));
+    pa = __fmul_rn(__fmaf_rn(taut, ux, pa), r);
+    pb = __fmul_rn(__fmaf_rn(taut, uy, pb), r);
+#endif
+}
+
+// tvl1_primal_row with u3: u3o its four pixels, p31 / l31 / p32 / up32 as p11 / l11 / p12 / up12
+__device__ __forceinline__ void tvl1_primal_row_g(const float4 &ix, const float4 &iy, const float4 &gq, const float4 &rc, const float4 &u1o,
+                                                  const float4 &u2o, const float4 &u3o, const float4 &p11, float l11, const float4 &p12,
+                                                  const float4 &up12, const float4 &p21, float l21, const float4 &p22, const float4 &up22,
+                                                  const float4 &p31, float l31, const float4 &p32, const float4 &up32, bool left_col,
+                                                  const Tvl1Consts &c, float gamma, float4 &n1, float4 &n2, float4 &n3) {
+#ifdef DFB_STRICT_FP
+    const float div1x = left_col ? (p11.x + p12.x) - up12.x : (p11.x - l11) + (p12.x - up12.x);
+    const float div2x = left_col ? (p21.x + p22.x) - up22.x : (p21.x - l21) + (p22.x - up22.x);
+    const float div3x = left_col ? (p31.x + p32.x) - up32.x : (p31.x - l31) + (p32.x - up32.x);
+#else
+    (void)left_col;
+    const float div1x = (p11.x - l11) + (p12.x - up12.x);
+    const float div2x = (p21.x - l21) + (p22.x - up22.x);
+    const float div3x = (p31.x - l31) + (p32.x - up32.x);
+#endif
+    tvl1_primal_px_g(ix.x, iy.x, gq.x, rc.x, u1o.x, u2o.x, u3o.x, div1x, div2x, div3x, c, gamma, n1.x, n2.x, n3.x);
+    tvl1_primal_px_g(ix.y, iy.y, gq.y, rc.y, u1o.y, u2o.y, u3o.y, (p11.y - p11.x) + (p12.y - up12.y), (p21.y - p21.x) + (p22.y - up22.y),
+                     (p31.y - p31.x) + (p32.y - up32.y), c, gamma, n1.y, n2.y, n3.y);
+    tvl1_primal_px_g(ix.z, iy.z, gq.z, rc.z, u1o.z, u2o.z, u3o.z, (p11.z - p11.y) + (p12.z - up12.z), (p21.z - p21.y) + (p22.z - up22.z),
+                     (p31.z - p31.y) + (p32.z - up32.z), c, gamma, n1.z, n2.z, n3.z);
+    tvl1_primal_px_g(ix.w, iy.w, gq.w, rc.w, u1o.w, u2o.w, u3o.w, (p11.w - p11.z) + (p12.w - up12.w), (p21.w - p21.z) + (p22.w - up22.w),
+                     (p31.w - p31.z) + (p32.w - up32.w), c, gamma, n1.w, n2.w, n3.w);
+}
+
+// tvl1_dual_row for the one field u3 (c3: this row, d3: the row below, r3: the pixel right of .w; clamped by the caller)
+__device__ __forceinline__ void tvl1_dual_row1(const float4 &c3, const float4 &d3, float r3, float taut, float4 &p31, float4 &p32) {
+    tvl1_dual_px1(c3.y - c3.x, d3.x - c3.x, taut, p31.x, p32.x);
+    tvl1_dual_px1(c3.z - c3.y, d3.y - c3.y, taut, p31.y, p32.y);
+    tvl1_dual_px1(c3.w - c3.z, d3.z - c3.z, taut, p31.z, p32.z);
+    tvl1_dual_px1(r3 - c3.w, d3.w - c3.w, taut, p31.w, p32.w);
+}
+
+// One quad of the gamma schedule (pixels x0 .. x0 + 3 of row y, x0 < W; all planes share `pitch`), shared by the stand-alone
+// kernels and the fused gamma kernel so both schedules compute the same bits.  p = {p11, p12, p21, p22, p31, p32}.
+// Primal, in place on u1, u2, u3 (pointwise in u, reads p only); gq = tvl1_gq_from_grad of the quad.  Returns the quad's
+// sum of (du1)^2 + (du2)^2 over its image pixels when ERR.
+template <bool ERR>
+__device__ __forceinline__ double tvl1_gamma_primal_quad(const float *I1wx, const float *I1wy, const float4 &gq, const float *rho_c,
+                                                         const float *const *p, float *u1, float *u2, float *u3, int x0, int y, int W,
+                                                         int pitch, const Tvl1Consts &c, float gamma) {
+    auto ld = [](const float *q) { return *reinterpret_cast<const float4 *>(q); };
+    const size_t i = (size_t)y * pitch + x0;
+    const float4 ix = ld(I1wx + i), iy = ld(I1wy + i), rc = ld(rho_c + i);
+    const float4 a11 = ld(p[0] + i), a12 = ld(p[1] + i), a21 = ld(p[2] + i), a22 = ld(p[3] + i), a31 = ld(p[4] + i), a32 = ld(p[5] + i);
+    const float4 uo1 = ld(u1 + i), uo2 = ld(u2 + i), uo3 = ld(u3 + i);
+    // backward differences; p outside the image is 0 (A.3 div)
+    const float l11 = x0 > 0 ? p[0][i - 1] : 0.f, l21 = x0 > 0 ? p[2][i - 1] : 0.f, l31 = x0 > 0 ? p[4][i - 1] : 0.f;
+    float4 t12 = make_float4(0.f, 0.f, 0.f, 0.f), t22 = t12, t32 = t12;
+    if (y > 0) {
+        t12 = ld(p[1] + i - pitch);
+        t22 = ld(p[3] + i - pitch);
+        t32 = ld(p[5] + i - pitch);
+    }
+    float4 n1, n2, n3;
+    tvl1_primal_row_g(ix, iy, gq, rc, uo1, uo2, uo3, a11, l11, a12, t12, a21, l21, a22, t22, a31, l31, a32, t32, x0 == 0, c, gamma, n1, n2, n3);
+    *reinterpret_cast<float4 *>(u1 + i) = n1;
+    *reinterpret_cast<float4 *>(u2 + i) = n2;
+    *reinterpret_cast<float4 *>(u3 + i) = n3;
+    double err = 0.0;
+    if (ERR) {  // u3 does not enter the error
+        const float4 d = tvl1_diff_row(uo1, uo2, n1, n2);
+        err += (double)d.x;
+        if (x0 + 1 < W) err += (double)d.y;
+        if (x0 + 2 < W) err += (double)d.z;
+        if (x0 + 3 < W) err += (double)d.w;
+    }
+    return err;
+}
+
+// Dual, in place on p (pointwise in p, reads u only): forward differences of the new u1, u2, u3, index-clamped; the last image
+// column is mirrored into the pixels right of it (their results land in padding columns, never read as image data).
+__device__ __forceinline__ void tvl1_gamma_dual_quad(const float *u1, const float *u2, const float *u3, float *const *p, int x0, int y, int W,
+                                                     int H, int pitch, float taut) {
+    auto ld = [](const float *q) { return *reinterpret_cast<const float4 *>(q); };
+    const size_t i = (size_t)y * pitch + x0;
+    const size_t id = (size_t)min(y + 1, H - 1) * pitch + x0;
+    const size_t ir = (size_t)y * pitch + min(x0 + 4, W - 1);
+    float4 c1 = ld(u1 + i), c2 = ld(u2 + i), c3 = ld(u3 + i);
+    const float4 d1 = ld(u1 + id), d2 = ld(u2 + id), d3 = ld(u3 + id);
+    float4 b[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) b[k] = ld(p[k] + i);
+    if (x0 + 1 >= W) { c1.y = c1.x; c2.y = c2.x; c3.y = c3.x; }
+    if (x0 + 2 >= W) { c1.z = c1.y; c2.z = c2.y; c3.z = c3.y; }
+    if (x0 + 3 >= W) { c1.w = c1.z; c2.w = c2.z; c3.w = c3.z; }
+    const bool in = x0 + 4 < W;
+    tvl1_dual_row(c1, c2, d1, d2, in ? u1[ir] : c1.w, in ? u2[ir] : c2.w, taut, b[0], b[1], b[2], b[3]);
+    tvl1_dual_row1(c3, d3, in ? u3[ir] : c3.w, taut, b[4], b[5]);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) *reinterpret_cast<float4 *>(p[k] + i) = b[k];
+}
+
 // Keys cubic (a = -0.5), SURVEY A.2 "Warp"
 __device__ __forceinline__ float bicubic_coeff(float x) {
     x = fabsf(x);

@@ -64,7 +64,11 @@ const char *dfb_last_error(const dfb_handle *h);
  * default 0.8 the workspace is sized for), "median_filtering" (0 [default] or 1 = off; 3 or 5 = u1 and u2 are replaced by
  * their k x k median, replicate borders, before every iteration n of a warp with n % median_interval == 0, so every warp
  * starts with one; an optional extra of CPU DualTVL1's kind that the reference's CUDA TV-L1 does not have) and
- * "median_interval" (>= 1, default 30); engine knobs: "fused" (1 = persistent fused primal+dual kernel
+ * "median_interval" (>= 1, default 30), "gamma" (finite, >= 0, default 0: OpenCV's setGamma, the weight of an illumination
+ * field u3 solved beside the flow so that brightness changes between the frames are not read as motion; u3 starts at 0,
+ * is resized between scales without the 1/scale_step factor and is discarded at the end; both schedules take it and give
+ * the same bits, every flow call takes it, the list runner never sets it);
+ * engine knobs: "fused" (1 = persistent fused primal+dual kernel
  * [default], 0 = one kernel per half-step, the reference's launch structure), "fused_k" (iterations kept on chip per tile
  * visit, 1..8, default 8), "lanes" (pairs solved side by side per launch, 0 = auto [default], up to 64), "use_tma"
  * (1 = TMA staging of the shared-memory tiles [default]), "time_kernels" (CUDA-event timing of the dominant kernel, see
