@@ -1,5 +1,5 @@
 """No GPU: what the TV-L1 illumination term (`gamma`, SURVEY.md A.8) does to accuracy, computed with the CPU oracle's
-building blocks and the gamma steps of tests/tvl1_gamma_ref.py.  AEE against the analytic ground-truth flow of synth.pair
+building blocks and the gamma steps of tests/tvl1_restate.py.  AEE against the analytic ground-truth flow of synth.pair
 for gamma 0, 0.1 and 1, on the pair as it is, with frame b brightened (b * gain + offset) and with a horizontal brightness
 ramp across frame b (0 at the left edge, `--ramp` grey levels at the right).  Prints a table and one JSON line.
 
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-import tvl1_gamma_ref as R  # noqa: E402
+import tvl1_restate as T  # noqa: E402
 from denseflow_b200 import synth  # noqa: E402
 
 GAMMAS = [0.0, 0.1, 1.0]
@@ -42,7 +42,7 @@ def main():
         inputs = {"unchanged": b, "gain+offset": _u8(bf * args.gain + args.offset), "ramp": _u8(bf + ramp)}
         for kind, fb in inputs.items():
             for g in GAMMAS:
-                flow, log, _ = R.tvl1_calc(a, fb, g)
+                flow, log, _ = T.tvl1_calc(a, fb, gamma=g)
                 rows.append({"seed": seed, "input": kind, "gamma": g, "aee_px": round(float(synth.aee(flow, gt)), 4),
                              "iterations": int(log.sum())})
                 print("seed %d %-12s gamma %-4g: AEE %.4f px, %d iterations" % (seed, kind, g, rows[-1]["aee_px"], rows[-1]["iterations"]))

@@ -1,5 +1,5 @@
 """No GPU: what the median filtering of the TV-L1 flow does to accuracy, computed with the CPU oracle's building blocks and
-the median of tests/tvl1_median_ref.py.  AEE against the
+the median of tests/tvl1_restate.py.  AEE against the
 analytic ground-truth flow of synth.pair, with the median off and at window 3 and 5 every 30 and every 300 iterations, on
 the clean pair and on the same pair with salt-and-pepper pixels (each frame on its own, `--noise` of the pixels set to 0
 or 255).  Prints a table and one JSON line.
@@ -17,7 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-import tvl1_median_ref as R  # noqa: E402
+import tvl1_restate as T  # noqa: E402
 from denseflow_b200 import synth  # noqa: E402
 
 CONFIGS = [(0, 30), (3, 30), (5, 30), (3, 300), (5, 300)]
@@ -43,7 +43,7 @@ def main():
         inputs = {"clean": (a, b), "salt-and-pepper": (salt_and_pepper(a, args.noise, rng), salt_and_pepper(b, args.noise, rng))}
         for kind, (fa, fb) in inputs.items():
             for k, interval in CONFIGS:
-                flow, log, _ = R.tvl1_calc(fa, fb, k, interval)
+                flow, log, _ = T.tvl1_calc(fa, fb, median_filtering=k, median_interval=interval)
                 rows.append({"seed": seed, "input": kind, "median_filtering": k, "median_interval": interval,
                              "aee_px": round(float(synth.aee(flow, gt)), 4), "iterations": int(log.sum())})
                 print("seed %d %-15s median %d every %3d: AEE %.4f px, %d iterations" % (seed, kind, k, interval, rows[-1]["aee_px"],

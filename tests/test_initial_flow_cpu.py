@@ -1,5 +1,5 @@
-"""`use_initial_flow` in its restatements (tests/initial_flow_ref.py), before the GPU builds are pinned to them
-(tests/test_initial_flow_gpu.py).
+"""`use_initial_flow` in its restatements (tests/tvl1_restate.py, tests/initial_flow_ref.py), before the GPU builds are
+pinned to them (tests/test_initial_flow_gpu.py).
 
 * TV-L1: the initial-flow pyramid over the C oracle's building blocks and over oracle/tvl1_numpy.py's agree bit for bit,
   at 1, 5 and 16 levels, small scale steps, and tiny and thin frames whose pyramid stops at 16 pixels; the two whole
@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 import initial_flow_ref as R
+import tvl1_restate as T
 from denseflow_b200 import synth
 
 F = np.float32
@@ -39,8 +40,8 @@ PYRAMIDS = [(96, 80, 1, 0.8), (96, 80, 5, 0.8), (340, 256, 16, 0.8), (340, 256, 
 def test_initial_flow_pyramids_agree_bit_for_bit(oracle, w, h, nscales, step):
     init = smooth_field(h, w, w * 7 + h, amp=5.0)
     lv = oracle.tvl1_level_sizes(w, h, oracle.tvl1_params(nscales=nscales, scale_step=step))
-    c1, c2 = R.tvl1_init_pyramid(init, lv, step)
-    n1, n2 = R.numpy_init_pyramid(init, nscales, step)
+    c1, c2 = T.tvl1_init_pyramid(init, lv, step)
+    n1, n2 = T.numpy_init_pyramid(init, nscales, step)
     assert [p.shape[::-1] for p in c1] == list(lv) == [p.shape[::-1] for p in n1]
     assert lv[-1][0] >= 16 and lv[-1][1] >= 16 or len(lv) == 1
     for s in range(len(lv)):
@@ -69,13 +70,13 @@ def test_two_tvl1_restatements_agree_from_an_initial_flow(oracle, kw, start):
     a, b, _ = synth.pair(80, 96, 6)
     init = {"smooth": lambda: smooth_field(80, 96, 1),
             "past_bound": lambda: smooth_field(80, 96, 2, amp=60.0),
-            "cold_flow": lambda: R.tvl1_calc(a, b, None, **kw)[0]}[start]()
-    fc, lc, _ = R.tvl1_calc(a, b, init, **kw)
-    fn, ln = R.numpy_calc(a, b, init, **_numpy_kw(kw))
+            "cold_flow": lambda: T.tvl1_calc(a, b, **kw)[0]}[start]()
+    fc, lc, _ = T.tvl1_calc(a, b, init=init, **kw)
+    fn, ln = T.numpy_calc(a, b, init=init, **_numpy_kw(kw))
     assert np.array_equal(lc, ln), (lc.tolist(), ln.tolist())
     assert np.isfinite(fc).all()
     assert np.abs(fc - fn).max() < 5e-4 and synth.aee(fc, fn) < 2e-5
-    cold = R.tvl1_calc(a, b, None, **kw)[0]
+    cold = T.tvl1_calc(a, b, **kw)[0]
     assert not np.array_equal(fc, cold), "the initial flow did not change the result"
 
 
@@ -84,14 +85,14 @@ def test_two_tvl1_restatements_agree_from_an_initial_flow(oracle, kw, start):
 def test_zero_initial_flow_is_the_cold_oracle(oracle, kw):
     a, b, _ = synth.pair(80, 96, 6)
     zero = np.zeros((80, 96, 2), F)
-    f0, l0, e0 = R.tvl1_calc(a, b, zero, **kw)
-    fn, ln, en = R.tvl1_calc(a, b, None, **kw)
+    f0, l0, e0 = T.tvl1_calc(a, b, init=zero, **kw)
+    fn, ln, en = T.tvl1_calc(a, b, **kw)
     assert np.array_equal(f0.view(np.int32), fn.view(np.int32)) and np.array_equal(l0, ln) and np.array_equal(e0, en)
     if "median_filtering" not in kw:
         ref, log = oracle.tvl1_calc(a, b, oracle.tvl1_params(**kw), return_iters=True)
         assert np.array_equal(f0.view(np.int32), ref.view(np.int32)) and np.array_equal(l0, log)
-    g0, m0 = R.numpy_calc(a, b, zero, **_numpy_kw(kw))
-    gn, mn = R.numpy_calc(a, b, None, **_numpy_kw(kw))
+    g0, m0 = T.numpy_calc(a, b, init=zero, **_numpy_kw(kw))
+    gn, mn = T.numpy_calc(a, b, **_numpy_kw(kw))
     assert np.array_equal(g0.view(np.int32), gn.view(np.int32)) and np.array_equal(m0, mn)
 
 

@@ -4,9 +4,9 @@
   auto lanes, median filtering on and off.
 * At 131 x 97, from a smooth random field, a field past `bound` and the oracle's own cold flow: the TV-L1 strict build's
   flows and per-(scale, warp) iteration logs equal the restatement over the C oracle's building blocks
-  (tests/initial_flow_ref.py) bit for bit, fused and unfused, and the Farneback strict build's flows do too; the default
-  builds are within 0.01 px.  Other frame sizes, lane counts, groups and chained starts: tests/test_initial_flow_paths_gpu.py;
-  the start pyramids alone: tests/test_initial_flow_stages_gpu.py.
+  (tests/tvl1_restate.py) bit for bit, fused and unfused, and the Farneback strict build's flows equal
+  tests/initial_flow_ref.py's; the default builds are within 0.01 px.  Other frame sizes, lane counts, groups and chained
+  starts: tests/test_initial_flow_paths_gpu.py; the start pyramids alone: tests/test_initial_flow_stages_gpu.py.
 * Host batch = per-pair calls, device batch = host batch, planes = the float2 field; pageable and page-locked host buffers
   and a non-default stream.
 * Every call without a float flow buffer, and a missing buffer, is refused with a message naming the parameter, launches
@@ -17,6 +17,7 @@ import pytest
 
 import initial_flow_ref as R
 import tvl1_pin as pin
+import tvl1_restate as T
 from denseflow_b200 import synth
 from test_initial_flow_cpu import smooth_field
 
@@ -94,8 +95,8 @@ def _reference(median):
         a, b, _ = synth.pair(H, W, 7)
         kw = dict(SMALL, median_filtering=median, median_interval=7)
         starts = {"smooth": smooth_field(H, W, 1), "past_bound": smooth_field(H, W, 2, amp=PAST_BOUND_AMP),
-                  "cold_flow": R.tvl1_calc(a, b, None, **kw)[0]}
-        _REF[median] = {n: (init, R.tvl1_calc(a, b, init, **kw)) for n, init in starts.items()}
+                  "cold_flow": T.tvl1_calc(a, b, **kw)[0]}
+        _REF[median] = {n: (init, T.tvl1_calc(a, b, init=init, **kw)) for n, init in starts.items()}
     return _REF[median]
 
 

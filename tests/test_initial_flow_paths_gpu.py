@@ -1,7 +1,7 @@
 """Warm starts (`use_initial_flow`, DESIGN §1) end to end, through the paths a start takes beyond the one 131 x 97 corner of
 tests/test_initial_flow_gpu.py.  The strict build is pinned bit for bit (flows and TV-L1 iteration logs, tests/tvl1_pin.py)
-to the restatements of tests/initial_flow_ref.py; the default build is held to 0.01 px and to its own bits across lane
-counts and entry points.
+to the restatements of tests/tvl1_restate.py (TV-L1) and tests/initial_flow_ref.py (Farneback); the default build is held
+to 0.01 px and to its own bits across lane counts and entry points.
 
 * Geometry: tiny frames, the squares around the tile and level cuts, 7 x 1080 / 1080 x 7, both engines; TV-L1 at the
   create() defaults at 340 x 256.
@@ -18,6 +18,7 @@ import pytest
 
 import initial_flow_ref as R
 import tvl1_pin as pin
+import tvl1_restate as T
 from denseflow_b200 import synth
 from test_initial_flow_cpu import smooth_field
 
@@ -65,7 +66,7 @@ def test_geometry_strict_bit_exact(oracle, alg):
         init = smooth_field(h, w, 30 + k, amp=3.0)
         flow = e.calc(a, b, flow=init.copy())
         if alg == "tvl1":
-            notes.append(pin.check(oracle, a, b, flow, e.tvl1_stats()[0], "%dx%d" % (w, h), oracle_out=R.tvl1_calc(a, b, init, **SMALL)))
+            notes.append(pin.check(oracle, a, b, flow, e.tvl1_stats()[0], "%dx%d" % (w, h), oracle_out=T.tvl1_calc(a, b, init=init, **SMALL)))
         else:
             _bits_equal(flow, R.farn_calc(a, b, init, _farn_params(oracle)), "%dx%d" % (w, h))
     e.release()
@@ -75,7 +76,7 @@ def test_geometry_strict_bit_exact(oracle, alg):
         init = smooth_field(h, w, 8, amp=5.0)
         e = _new(alg, w, h, "strict")
         notes.append(pin.check(oracle, a, b, e.calc(a, b, flow=init.copy()), e.tvl1_stats()[0], "340x256 defaults",
-                               oracle_out=R.tvl1_calc(a, b, init)))
+                               oracle_out=T.tvl1_calc(a, b, init=init)))
         e.release()
     pin.finish(notes)
 
@@ -93,7 +94,7 @@ def _ring_case(median):
         starts = _starts(RING_PAIRS, h, w, 200)
         kw = dict(SMALL, **(MEDIAN if median else {}))
         pick = [0, 15, 16, 17, RING_PAIRS - 1]
-        _RING[median] = (fr, starts, {j: R.tvl1_calc(fr[j], fr[j + 1], starts[j], **kw) for j in pick})
+        _RING[median] = (fr, starts, {j: T.tvl1_calc(fr[j], fr[j + 1], init=starts[j], **kw) for j in pick})
     return _RING[median]
 
 
@@ -154,7 +155,7 @@ def test_host_groups(oracle, alg, variant):
         for j in firsts:
             if alg == "tvl1":
                 notes.append(pin.check(oracle, fr[j], fr[j + 1], host[j], iters[j], "pair %d" % j,
-                                       oracle_out=R.tvl1_calc(fr[j], fr[j + 1], starts[j], **SMALL)))
+                                       oracle_out=T.tvl1_calc(fr[j], fr[j + 1], init=starts[j], **SMALL)))
             else:
                 _bits_equal(host[j], R.farn_calc(fr[j], fr[j + 1], starts[j], _farn_params(oracle)), "pair %d" % j)
         pin.finish(notes)
@@ -189,7 +190,7 @@ def test_chained_starts(oracle, alg):
     kw = SMALL if alg == "tvl1" else {}
     refs, prev, notes = [], np.zeros((h, w, 2), np.float32), []
     for j in range(n - 1):
-        out = R.tvl1_calc(fr[j], fr[j + 1], prev, **kw) if alg == "tvl1" else (R.farn_calc(fr[j], fr[j + 1], prev, _farn_params(oracle)),)
+        out = T.tvl1_calc(fr[j], fr[j + 1], init=prev, **kw) if alg == "tvl1" else (R.farn_calc(fr[j], fr[j + 1], prev, _farn_params(oracle)),)
         refs.append(out)
         prev = out[0]
     e = _new(alg, w, h, "strict", **kw)
@@ -247,7 +248,7 @@ def test_default_warm_regression_guard(oracle, alg):
     e = _new(alg, w, h, "default")
     flow = e.calc(a, b, flow=init.copy())
     e.release()
-    ref = R.tvl1_calc(a, b, init)[0] if alg == "tvl1" else R.farn_calc(a, b, init, _farn_params(oracle))
+    ref = T.tvl1_calc(a, b, init=init)[0] if alg == "tvl1" else R.farn_calc(a, b, init, _farn_params(oracle))
     epe = np.hypot(*(flow.astype(np.float64) - ref).transpose(2, 0, 1))
     band = np.ones((h, w), bool)
     band[6:-6, 6:-6] = False

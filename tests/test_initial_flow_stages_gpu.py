@@ -1,7 +1,7 @@
 """The start of a warm solve (`use_initial_flow`, DESIGN §1) as a stage of its own, through the `tvl1_initial_flow` and
 `farn_initial_flow` stages of dfb_debug_run_kernel (the engines' own load_initial_flow / launch_flow_init):
 
-* TV-L1: every level of every lane's start pyramid.  Strict build: equal to tests/initial_flow_ref.tvl1_init_pyramid bit
+* TV-L1: every level of every lane's start pyramid.  Strict build: equal to tests/tvl1_restate.tvl1_init_pyramid bit
   for bit.  Default build: level 0 is the start itself, every coarser level within the float64 bound of
   tvl1_ref64.upsample(level above, ..., float(scale_step)), element by element.
 * Farneback: the coarsest level's start.  Strict build: equal to initial_flow_ref.farn_start (orc_resize_linear x
@@ -21,6 +21,7 @@ import farn_ref64 as f64
 import geometry_cases as gc
 import initial_flow_ref as R
 import tvl1_ref64 as t64
+import tvl1_restate as T
 from test_initial_flow_cpu import PYRAMIDS, smooth_field
 
 pytestmark = pytest.mark.gpu
@@ -112,7 +113,7 @@ def tvl1_case(oracle, e, variant, w, h, nscales, scale_step, starts, step, pitch
         got = [[lev[i] for lev in levels[c]] for c in (0, 1)]
         tag = "%s %dx%d nscales %d step %g lane %d of %d, start step %d pitch %d" % (what, w, h, nscales, scale_step, i, n, step, pitch)
         if variant == "strict":
-            want = R.tvl1_init_pyramid(init, lv, scale_step)
+            want = T.tvl1_init_pyramid(init, lv, scale_step)
             for c in (0, 1):
                 for s in range(len(lv)):
                     _bits_equal(got[c][s], want[c][s], "%s: u%d level %d" % (tag, c + 1, s))

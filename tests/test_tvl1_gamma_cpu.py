@@ -1,4 +1,4 @@
-"""The TV-L1 illumination term (`gamma`; SURVEY.md A.8) in its two restatements (tests/tvl1_gamma_ref.py), before the GPU
+"""The TV-L1 illumination term (`gamma`; SURVEY.md A.8) in its two restatements (tests/tvl1_restate.py), before the GPU
 builds are pinned to them (tests/test_tvl1_gamma_gpu.py).
 
 * At gamma = 0 each restatement is its oracle bit for bit: flows and iteration logs (and the C one every convergence check).
@@ -10,7 +10,7 @@ builds are pinned to them (tests/test_tvl1_gamma_gpu.py).
 import numpy as np
 import pytest
 
-import tvl1_gamma_ref as R
+import tvl1_restate as T
 from denseflow_b200 import synth
 
 BASE = dict(nscales=3, warps=3, iterations=60)
@@ -32,11 +32,11 @@ def test_gamma_zero_is_each_oracle(oracle, kw):
     h, w = (256, 256) if not kw else (80, 96)
     a, b, _ = synth.pair(h, w, 0 if not kw else 6)
     ref, log, errs = oracle.tvl1_calc(a, b, oracle.tvl1_params(**kw), return_iters=True, return_errors=True)
-    f, lg, e = R.tvl1_calc(a, b, 0.0, **kw)
+    f, lg, e = T.tvl1_calc(a, b, gamma=0.0, **kw)
     assert np.array_equal(f.view(np.int32), ref.view(np.int32)) and np.array_equal(lg, log) and _same_checks(e, errs)
     nkw = {("lam" if k == "lambda" else k): v for k, v in kw.items()}
     nref, nlog = N.calc(a, b, **nkw)
-    fn, ln = R.numpy_calc(a, b, 0.0, **nkw)
+    fn, ln = T.numpy_calc(a, b, gamma=0.0, **nkw)
     assert np.array_equal(fn.view(np.int32), nref.view(np.int32)) and np.array_equal(ln, nlog)
 
 
@@ -57,8 +57,8 @@ def test_restatements_agree(oracle, case):
     init = None
     if kw.pop("warm", False):
         init = (gt * 0.5).astype(np.float32)
-    fc, lc, _ = R.tvl1_calc(a, b, gamma, init=init, **kw)
-    fn, ln = R.numpy_calc(a, b, gamma, init=init, **kw)
+    fc, lc, _ = T.tvl1_calc(a, b, gamma=gamma, init=init, **kw)
+    fn, ln = T.numpy_calc(a, b, gamma=gamma, init=init, **kw)
     assert np.array_equal(lc, ln), (lc.tolist(), ln.tolist())
     assert np.isfinite(fc).all()
     # the tolerance of the cold restatements' comparison (tests/test_tvl1_median_cpu.py)
@@ -69,8 +69,8 @@ def test_restatements_agree(oracle, case):
 def test_brightness_change_moves_u3_and_the_flow(gamma):
     a, b, gt = synth.pair(80, 96, 2)
     b = _brighter(b, 1.15, 10.0)
-    f, _, _, u3 = R.tvl1_calc(a, b, gamma, return_u3=True, **BASE)
-    f0 = R.tvl1_calc(a, b, 0.0, **BASE)[0]
+    f, _, _, u3 = T.tvl1_calc(a, b, gamma=gamma, return_u3=True, **BASE)
+    f0 = T.tvl1_calc(a, b, gamma=0.0, **BASE)[0]
     assert np.abs(u3).max() > 0.1 and np.isfinite(u3).all()
     assert (f != f0).any()
     if gamma == 1.0:  # the term absorbs the brightness change that gamma = 0 reads as motion
@@ -81,9 +81,9 @@ def test_restatements_refuse_bad_gamma():
     a, b, _ = synth.pair(32, 32, 1)
     for g in (-0.5, -1e-9, float("nan"), float("inf"), float("-inf")):
         with pytest.raises(ValueError):
-            R.tvl1_calc(a, b, g)
+            T.tvl1_calc(a, b, gamma=g)
         with pytest.raises(ValueError):
-            R.numpy_calc(a, b, g)
+            T.numpy_calc(a, b, gamma=g)
 
 
 def test_print_quality_table():
@@ -113,7 +113,7 @@ def test_gamma_steps_at_zero_are_the_oracle_steps(oracle, shape):
     u1, u2 = (rng.standard_normal((h, w)).astype(np.float32) for _ in range(2))
     zero = np.zeros((h, w), np.float32)
     l_t, theta = np.float32(0.15 * 0.3), np.float32(0.3)
-    n1, n2, n3, e = R.estimate_u_gamma(ix, iy, grad, rho_c, *p, zero, zero, u1, u2, zero, l_t, theta, 0.0)
+    n1, n2, n3, e = T.estimate_u_gamma(ix, iy, grad, rho_c, *p, zero, zero, u1, u2, zero, l_t, theta, 0.0)
     r1, r2 = u1.copy(), u2.copy()
     er = oracle.lib().orc_tvl1_estimate_u(ix, iy, grad, rho_c, *p, r1, r2, w, h, l_t, theta, 1)
     assert np.array_equal(n1.view(np.int32), r1.view(np.int32)) and np.array_equal(n2.view(np.int32), r2.view(np.int32))

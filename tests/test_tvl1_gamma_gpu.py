@@ -1,7 +1,7 @@
 """The TV-L1 illumination term (`gamma`; SURVEY.md A.8, DESIGN §4.3) on the GPU.
 
 * Stages: the gamma primal and dual kernels (the `estimate_u_gamma` / `estimate_dual_gamma` stages of dfb_debug_run_kernel)
-  equal the restatement's steps (tests/tvl1_gamma_ref.py) bit for bit in the strict build, on frame-sized, tiny and thin
+  equal the restatement's steps (tests/tvl1_restate.py) bit for bit in the strict build, on frame-sized, tiny and thin
   planes, convergence sum included.
 * Strict build: flows and per-(scale, warp) iteration logs equal the restatement over the C oracle's building blocks bit for
   bit, in both schedules (the fused gamma kernel k_tvl1_pair_gamma and the per-half-step kernels), on 256 x 256, the tiny and
@@ -22,8 +22,8 @@ import pytest
 
 import content_cases as cc
 import geometry_cases as gc
-import tvl1_gamma_ref as R
 import tvl1_pin as pin
+import tvl1_restate as T
 from denseflow_b200 import _lib, synth
 from oracle import cv_restate
 
@@ -55,7 +55,7 @@ ORACLE_KEYS = ("nscales", "warps", "iterations", "epsilon", "tau", "theta", "lam
 def _reference(a, b, gamma, params, init=None):
     op = {n: v for n, v in params.items() if n in ORACLE_KEYS}
     med = {n: v for n, v in params.items() if n.startswith("median_")}
-    return R.tvl1_calc(a, b, gamma, init=init, **med, **op)
+    return T.tvl1_calc(a, b, gamma=gamma, init=init, **med, **op)
 
 
 # ---- stages --------------------------------------------------------------------------------------------------------------
@@ -82,11 +82,11 @@ def test_stages_equal_the_restatement(variant, gamma):
     l_t, theta, taut = np.float32(0.15 * 0.3), np.float32(0.3), np.float32(0.25 / 0.3)
     for j, (w, h) in enumerate(STAGE_SHAPES):
         ix, iy, grad, rho_c, p, u = _stage_inputs(w, h, 100 * j + int(gamma * 10))
-        r1, r2, r3, err_ref = R.estimate_u_gamma(ix, iy, grad, rho_c, *p, *u, l_t, theta, gamma)
+        r1, r2, r3, err_ref = T.estimate_u_gamma(ix, iy, grad, rho_c, *p, *u, l_t, theta, gamma)
         (g1, g2, g3), err = e.debug_run_kernel("estimate_u_gamma", [ix, iy, grad, rho_c, *p, *u], 3,
                                                [float(l_t), float(theta), 1, gamma])
         pr = [q.copy() for q in p]
-        R.estimate_dual_gamma(r1, r2, r3, pr, taut)
+        T.estimate_dual_gamma(r1, r2, r3, pr, taut)
         got, _ = e.debug_run_kernel("estimate_dual_gamma", [r1, r2, r3, *p], 6, [float(taut)])
         what = "%dx%d gamma %g %s" % (w, h, gamma, variant)
         if variant == "strict":
@@ -145,7 +145,7 @@ def test_strict_clip_is_bit_exact(oracle, lanes):
     e = _new(w, h, lanes=lanes, fused_k=3, gamma=0.8)
     flows = e.calc_batch(list(fr), step=1)
     pin.finish([pin.check(oracle, fr[j], fr[j + 1], flows[j], e.tvl1_pair_stats(j), "lanes %d pair %d" % (lanes, j),
-                          oracle_out=R.tvl1_calc(fr[j], fr[j + 1], 0.8)) for j in range(flows.shape[0])])
+                          oracle_out=T.tvl1_calc(fr[j], fr[j + 1], gamma=0.8)) for j in range(flows.shape[0])])
     e.release()
 
 
@@ -154,7 +154,7 @@ def test_strict_warm_start_is_bit_exact(oracle):
     a, b, gt = synth.pair(h, w, 4)
     b = _brighter(b)
     start = (gt * 0.75).astype(np.float32)
-    want = R.tvl1_calc(a, b, 1.0, init=start)
+    want = T.tvl1_calc(a, b, gamma=1.0, init=start)
     notes = []
     for fused in (1, 0):
         e = _new(w, h, gamma=1.0, use_initial_flow=1, fused=fused)
@@ -233,7 +233,7 @@ def test_default_is_near_the_restatement(gamma):
     e = _new(w, h, "default", gamma=gamma)
     ref = e.calc(a, b)
     _bits_equal(e.set("fused", 0).calc(a, b), ref, "gamma %g, unfused" % gamma)
-    o = R.tvl1_calc(a, b, gamma)[0]
+    o = T.tvl1_calc(a, b, gamma=gamma)[0]
     epe = np.hypot(*(ref.astype(np.float64) - o).transpose(2, 0, 1))
     print("default build with gamma %g vs the restatement: AEE %.3g, p99.9 EPE %.3g px" % (gamma, epe.mean(), np.percentile(epe, 99.9)))
     assert epe.mean() <= AEE_TOL, epe.mean()

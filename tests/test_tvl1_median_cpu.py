@@ -1,4 +1,4 @@
-"""The optional median filtering of the TV-L1 flow (DESIGN §4.3) in its two restatements (tests/tvl1_median_ref.py), before
+"""The optional median filtering of the TV-L1 flow (DESIGN §4.3) in its two restatements (tests/tvl1_restate.py), before
 the GPU builds are pinned to them (tests/test_tvl1_median_gpu.py).
 
 * M_k: the key-ordered median and the by-value median equal cv2.medianBlur at k = 3 and 5.  cv2 is compared by value: the
@@ -15,7 +15,7 @@ import cv2
 import numpy as np
 import pytest
 
-import tvl1_median_ref as R
+import tvl1_restate as T
 from denseflow_b200 import synth
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -42,9 +42,9 @@ def test_median_blur_equals_cv2(k):
         for name, a in _planes(w, h, 100 * k + j):
             want = cv2.medianBlur(a, k)
             what = "%dx%d %s k %d" % (w, h, name, k)
-            c = R.median_blur(a, k)
+            c = T.median_blur(a, k)
             _same_values(c, want, what + " by key")
-            n = R.median_blur_by_value(a, k)
+            n = T.median_blur_by_value(a, k)
             _same_values(n, want, what + " by value")
             assert np.array_equal(c.view(np.int32), n.view(np.int32)), what + ": the two restatements differ in a bit"
 
@@ -52,7 +52,7 @@ def test_median_blur_equals_cv2(k):
 @pytest.mark.parametrize("k", [3, 5])
 def test_median_blur_1080p_equals_cv2(k):
     a = (np.random.default_rng(k).standard_normal((1080, 1920)) * 4).astype(np.float32)
-    _same_values(R.median_blur(a, k), cv2.medianBlur(a, k), "1920x1080 k %d" % k)
+    _same_values(T.median_blur(a, k), cv2.medianBlur(a, k), "1920x1080 k %d" % k)
 
 
 def _rule(a, k):
@@ -73,7 +73,7 @@ def test_signed_zeros_follow_the_contract(k):
     for j, (w, h) in enumerate([(1, 1), (3, 2), (7, 5), (24, 19)]):
         a = rng.choice(np.float32([-0.0, 0.0, -0.0, 0.0, 1.0, -1.0]), (h, w)).astype(np.float32)
         want = _rule(a, k)
-        for name, got in (("by key", R.median_blur(a, k)), ("by value", R.median_blur_by_value(a, k))):
+        for name, got in (("by key", T.median_blur(a, k)), ("by value", T.median_blur_by_value(a, k))):
             assert np.array_equal(got.view(np.int32), want.view(np.int32)), "%dx%d k %d %s: the sign of a zero differs" % (w, h, k, name)
         if w * h > 100:  # the case exists: zeros of both signs in the result
             z = want[want == 0]
@@ -98,8 +98,8 @@ def test_c_oracle_agrees_with_numpy_restatement(oracle, case):
     k, interval, prm = case
     kw = dict(BASE, **prm)
     a, b, _ = synth.pair(80, 96, 6)
-    fc, lc, _ = R.tvl1_calc(a, b, k, interval, **kw)
-    fn, ln = R.numpy_calc(a, b, median_filtering=k, median_interval=interval, **kw)
+    fc, lc, _ = T.tvl1_calc(a, b, median_filtering=k, median_interval=interval, **kw)
+    fn, ln = T.numpy_calc(a, b, median_filtering=k, median_interval=interval, **kw)
     assert np.array_equal(lc, ln), (lc.tolist(), ln.tolist())
     if prm.get("epsilon") == 1.0:  # every warp converges at its first check
         n = len(oracle.tvl1_level_sizes(96, 80, oracle.tvl1_params(nscales=kw["nscales"])))
@@ -126,13 +126,13 @@ def test_median_off_is_the_c_oracle(oracle):
     assert np.array_equal(log, gold["iters"])
     assert np.array_equal(ref[::4, ::4], gold["flow_s4"])
     for mf, interval in ((0, 30), (1, 30), (0, 1), (1, 7)):
-        f, lg, e = R.tvl1_calc(a, b, mf, interval)
+        f, lg, e = T.tvl1_calc(a, b, median_filtering=mf, median_interval=interval)
         assert np.array_equal(f.view(np.int32), ref.view(np.int32)) and np.array_equal(lg, log), (mf, interval)
         assert _same_checks(e, errs), (mf, interval)
     a, b, _ = synth.pair(80, 96, 6)
     for kw in (dict(BASE), dict(BASE, epsilon=0.0, iterations=9), dict(BASE, epsilon=1.0), dict(tau=0.5, theta=0.05, nscales=2)):
         ref, log, errs = oracle.tvl1_calc(a, b, oracle.tvl1_params(**kw), return_iters=True, return_errors=True)
-        f, lg, e = R.tvl1_calc(a, b, 0, 30, **kw)
+        f, lg, e = T.tvl1_calc(a, b, median_filtering=0, median_interval=30, **kw)
         assert np.array_equal(f.view(np.int32), ref.view(np.int32)) and np.array_equal(lg, log) and _same_checks(e, errs), kw
 
 
@@ -140,9 +140,9 @@ def test_restatements_refuse_bad_median_parameters():
     a, b, _ = synth.pair(32, 32, 1)
     for mf, interval in ((2, 30), (4, 30), (7, 30), (-1, 30), (3, 0), (5, -4)):
         with pytest.raises(ValueError):
-            R.tvl1_calc(a, b, mf, interval)
+            T.tvl1_calc(a, b, median_filtering=mf, median_interval=interval)
         with pytest.raises(ValueError):
-            R.numpy_calc(a, b, median_filtering=mf, median_interval=interval)
+            T.numpy_calc(a, b, median_filtering=mf, median_interval=interval)
     for k in (1, 4, 7):
         with pytest.raises(ValueError):
-            R.median_blur(np.zeros((4, 4), np.float32), k)
+            T.median_blur(np.zeros((4, 4), np.float32), k)

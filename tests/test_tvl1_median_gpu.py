@@ -1,9 +1,9 @@
 """The optional median filtering of the TV-L1 flow (`median_filtering`, `median_interval`; DESIGN §4.3) on the GPU.
 
 * Stage: the fused kernel's phase_median (the `tvl1_median` stage of dfb_debug_run_kernel, workspace padding poisoned)
-  equals the contract's median (tests/tvl1_median_ref.py) bit for bit, the sign of a zero included, at every pyramid level of the frame shapes, the small
+  equals the contract's median (tests/tvl1_restate.py) bit for bit, the sign of a zero included, at every pyramid level of the frame shapes, the small
   planes and thin strips, on 1 and 3 lanes.
-* Strict build: flows and per-(scale, warp) iteration logs equal the C oracle's with the median (tests/tvl1_median_ref.py), fused and unfused, across
+* Strict build: flows and per-(scale, warp) iteration logs equal the C oracle's with the median (tests/tvl1_restate.py), fused and unfused, across
   the kernel's knobs, on single pairs and on batches whose lanes keep tiles resident on chip.
 * Default build: every knob combination and both schedules give the same bits; the flow is within 0.01 px of the oracle
   and within a regression guard of ten times its measured residual.
@@ -19,8 +19,8 @@ import pytest
 
 import geometry_cases as gc
 import test_tvl1_fused_stages_gpu as fs
-import tvl1_median_ref as R
 import tvl1_pin as pin
+import tvl1_restate as T
 from denseflow_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
@@ -39,7 +39,7 @@ def _new(w, h, variant="strict", **params):
 def _reference(a, b, params, k, interval):
     """(flow, log, convergence checks) of the C oracle's building blocks with the median"""
     op = {n: v for n, v in params.items() if n in ("nscales", "warps", "iterations", "epsilon")}
-    return R.tvl1_calc(a, b, k, interval, **op)
+    return T.tvl1_calc(a, b, median_filtering=k, median_interval=interval, **op)
 
 
 def _bits_equal(got, want, what):
@@ -80,7 +80,7 @@ def test_median_stage_equals_oracle(oracle, variant, lanes, k):
         got, _ = e.debug_run_kernel("tvl1_median", [fs._stack([c[q] for c in cases]) for q in range(2)], 2, [k, lanes])
         for i, c in enumerate(cases):
             for q in range(2):
-                _bits_equal(fs._split(got[q], lanes)[i], R.median_blur(c[q], k), "%dx%d k %d lane %d/%d u%d" % (w, h, k, i, lanes, q + 1))
+                _bits_equal(fs._split(got[q], lanes)[i], T.median_blur(c[q], k), "%dx%d k %d lane %d/%d u%d" % (w, h, k, i, lanes, q + 1))
 
 
 # ---- strict build: the whole flow ----------------------------------------------------------------------------------------
@@ -116,7 +116,7 @@ def test_strict_batch_is_bit_exact(oracle, lanes):
     e = _new(w, h, lanes=lanes, median_filtering=5, median_interval=7)
     flows = e.calc_batch(list(fr), step=1)
     pin.finish([pin.check(oracle, fr[j], fr[j + 1], flows[j], e.tvl1_pair_stats(j), "lanes %d pair %d" % (lanes, j),
-                          oracle_out=R.tvl1_calc(fr[j], fr[j + 1], 5, 7)) for j in range(flows.shape[0])])
+                          oracle_out=T.tvl1_calc(fr[j], fr[j + 1], median_filtering=5, median_interval=7)) for j in range(flows.shape[0])])
     e.release()
 
 
@@ -129,7 +129,7 @@ def test_strict_1080p_two_lanes_is_bit_exact(oracle):
     e = _new(w, h, lanes=2, median_filtering=3, median_interval=30)
     flows = e.calc_batch(list(fr), step=1)
     notes = [pin.check(oracle, fr[j], fr[j + 1], flows[j], e.tvl1_pair_stats(j), "1080p pair %d" % j,
-                       oracle_out=R.tvl1_calc(fr[j], fr[j + 1], 3, 30)) for j in range(2)]
+                       oracle_out=T.tvl1_calc(fr[j], fr[j + 1], median_filtering=3, median_interval=30)) for j in range(2)]
     oracle.lib().orc_set_num_threads(min(8, oracle.usable_cores()))
     e.release()
     pin.finish(notes)
@@ -158,7 +158,7 @@ def test_default_knobs_and_schedules_are_bit_identical(oracle, k, interval):
     for lanes in (1, 3, 0):  # lanes of a batch: the same bits as the single pair
         e.set("lanes", lanes)
         _bits_equal(e.calc_batch([a, b, a], step=1)[0], ref, "lanes %d" % lanes)
-    o = R.tvl1_calc(a, b, k, interval)[0]
+    o = T.tvl1_calc(a, b, median_filtering=k, median_interval=interval)[0]
     epe = np.hypot(*(ref.astype(np.float64) - o).transpose(2, 0, 1))
     aee, p999 = epe.mean(), np.percentile(epe, 99.9)
     print("default build with median k %d I %d vs oracle: AEE %.3g, p99.9 EPE %.3g px" % (k, interval, aee, p999))
