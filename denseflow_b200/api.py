@@ -121,7 +121,9 @@ class DenseOpticalFlow:
         "median_filtering" (0 or 1 = off [default], 3 or 5 = the window of a median of the flow between iterations) and
         "median_interval" (>= 1, default 30: the median runs before iterations 0, I, 2I, ... of every warp) and "gamma"
         (finite, >= 0, default 0: OpenCV's setGamma, the weight of an illumination field that absorbs brightness changes
-        between the two frames; both schedules take it and give the same bits).  Both algorithms
+        between the two frames; both schedules take it and give the same bits).  Farneback also takes "gaussian_window"
+        (0 [default] or 1: OPTFLOW_FARNEBACK_GAUSSIAN, a 13x13 Gaussian window instead of the box in every iteration) and
+        "fast_pyramids" (0 [default] or 1: OpenCV's fastPyramids, level images by a chain of pyrDown).  Both algorithms
         take "use_initial_flow" (0 [default] or 1: OpenCV's useInitialFlow / OPTFLOW_USE_INITIAL_FLOW): with 1, the flow
         buffers of calc, calc_batch, calc_batch_device, calc_batch_planes and calc_batch_device_planes are read as each
         pair's starting flow before they are overwritten, so they must be passed, and every other flow call is refused.  A

@@ -5,7 +5,9 @@
 //
 // Per level (coarse -> fine): Gaussian blur of the FULL-resolution frame + bilinear resize to the level
 // (B.2), polynomial expansion (B.3), then 10 x [13x13 box mean of the five M planes -> per-pixel 2x2
-// solve -> rebuild M] (B.4, B.5).  All planes are fp32 with 128-byte-aligned rows; the five planes of
+// solve -> rebuild M] (B.4, B.5).  Two create() options change that (B.7): "gaussian_window"
+// (OPTFLOW_FARNEBACK_GAUSSIAN) averages M over a 13x13 Gaussian window instead of the box, and "fast_pyramids" builds the
+// level images by a chain of pyrDown from the unblurred frame instead of blur + resize.  All planes are fp32 with 128-byte-aligned rows; the five planes of
 // R / M are stored as five separate planes of one pitch (the reference stacks them in a 5H x W matrix).
 // These kernels are HBM-bound 2-D stencils: separable passes staged through shared-memory tiles,
 // float4 on the interior, index-clamp / reflect-101 border rules applied on image coordinates.
@@ -153,6 +155,35 @@ __global__ void __launch_bounds__(256) k_gauss_horz_resize(const __grid_constant
     dst.p[(size_t)dy * dst.pitch + dx] = out;
 }
 
+// ---- B.7 fastPyramids: level k = pyrDown(level k - 1), batched like the preparation stages (blockIdx.z = frame) --------------
+// cv::cuda::pyrDown, BORDER_REFLECT_101: output (x, y) is the 5-tap [1 4 6 4 1] / 16 filter at source column / row 2x / 2y,
+// the vertical pass first, each pass summed left to right in fp32.  The 25 taps of a pixel come through L1; the levels it
+// runs on are a quarter of the frame and smaller.
+struct PyrBatch {
+    const float *src[kMaxPrep];
+    float *dst[kMaxPrep];
+};
+
+__global__ void __launch_bounds__(256) k_pyr_down(const __grid_constant__ PyrBatch pb, int sw, int sh, int spitch, int dw, int dh, int dpitch) {
+    const int x = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
+    if (x >= dw || y >= dh) return;
+    const float *src = pb.src[blockIdx.z];
+    const float k[5] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f};
+    size_t rows[5];
+#pragma unroll
+    for (int d = 0; d < 5; ++d) rows[d] = (size_t)reflect101(2 * y + d - 2, sh) * spitch;
+    float out = 0.f;
+#pragma unroll
+    for (int e = 0; e < 5; ++e) {
+        const int c = reflect101(2 * x + e - 2, sw);
+        float v = src[rows[0] + c] * k[0];
+#pragma unroll
+        for (int d = 1; d < 5; ++d) v = v + src[rows[d] + c] * k[d];
+        out = e == 0 ? v * k[0] : out + v * k[e];
+    }
+    pb.dst[blockIdx.z][(size_t)y * dpitch + x] = out;
+}
+
 // ---- B.3 polynomial expansion (polyN = 5): vertical pass (t0,t1,t2) then horizontal, index-clamped ----
 constexpr int PT = 32;
 
@@ -210,6 +241,8 @@ __global__ void __launch_bounds__(256) k_poly_exp(const __grid_constant__ PrepBa
 }
 
 __constant__ float c_border[6] = {0.14f, 0.14f, 0.4472f, 0.4472f, 0.4472f, 1.f};
+// B.7 Gaussian window: getGaussianKernel(13, 6 * 0.3f, CV_32F), centre and right half (set by the engine's constructor)
+__constant__ float c_gauss_win[7];
 
 // ---- B.4 updateMatrices ------------------------------------------------------------------------------
 // ---- B.4 in three steps, so that two horizontally adjacent pixels can share their R1 taps -----------------------------------
@@ -345,6 +378,7 @@ __global__ void __launch_bounds__(256) k_update_matrices(const __grid_constant__
 }
 
 // ---- B.5 fused iteration: 13x13 box mean of the 5 planes of M -> 2x2 solve -> (optionally) rebuild M ------
+// GAUSS (B.7): the 13x13 Gaussian window c_gauss_win instead of the box mean; everything else is shared.
 // One CTA produces a 32 x 32 tile of flow.  The (32+12) x (32+12) window of each of the five M planes is staged
 // in shared memory once (index-clamped), summed vertically (centre + symmetric pairs, the reference's order) into a
 // second shared buffer, then horizontally; the solve and the rebuild of M for the next iteration happen in
@@ -363,7 +397,7 @@ constexpr int kBoxPlaneSlot = ((RW * (BH + 12) + 31) / 32) * 32;  // floats per 
 // (index-clamped), vs = scratch for the vertical sums.
 // after_vertical() runs once the vertical sums are in `vs` and every thread is done with `raw` (the kernel asks for the
 // next tile's windows there, so they land while this tile's long half — solve, gathers, rebuild — is still running).
-template <int HALF, typename Hook>
+template <int HALF, bool GAUSS, typename Hook>
 __device__ __forceinline__ void box_tile_compute(const float *raw /* [5][kBoxPlaneSlot] */, float (*vs)[BH][BW + 2 * HALF], const PairArgs &a, int mb,
                                                  int rebuild, int x0, int y0, int tid, Hook after_vertical) {
     const Plane5 Mout = a.M[mb ^ 1], R0 = a.R0, R1 = a.R1;
@@ -396,9 +430,16 @@ __device__ __forceinline__ void box_tile_compute(const float *raw /* [5][kBoxPla
         for (int q = 0; q < VG + 2 * HALF; ++q) v[q] = raw[k * kBoxPlaneSlot + (g * VG + q) * RW + tx + (HX - HALF)];
 #pragma unroll
         for (int o = 0; o < VG; ++o) {
-            float acc = v[o + HALF];
+            float acc;
+            if constexpr (GAUSS) {
+                acc = v[o + HALF] * c_gauss_win[0];
 #pragma unroll
-            for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]);
+                for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]) * c_gauss_win[j];
+            } else {
+                acc = v[o + HALF];
+#pragma unroll
+                for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]);
+            }
             vs[k][g * VG + o][tx] = acc;
         }
     }
@@ -438,10 +479,17 @@ __device__ __forceinline__ void box_tile_compute(const float *raw /* [5][kBoxPla
             }
 #pragma unroll
             for (int o = 0; o < PX; ++o) {
-                float acc = v[o + HALF];
+                if constexpr (GAUSS) {
+                    float acc = v[o + HALF] * c_gauss_win[0];
 #pragma unroll
-                for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]);
-                b[o][k] = acc * area_inv;
+                    for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]) * c_gauss_win[j];
+                    b[o][k] = acc;
+                } else {
+                    float acc = v[o + HALF];
+#pragma unroll
+                    for (int j = 1; j <= HALF; ++j) acc = acc + (v[o + HALF - j] + v[o + HALF + j]);
+                    b[o][k] = acc * area_inv;
+                }
             }
         }
         // all pixels' gathers are issued before any of them is consumed: coordinates are clamped into the image
@@ -493,7 +541,7 @@ struct BoxTmaSmem {
     unsigned long long bar;
 };
 
-template <int HALF>
+template <int HALF, bool GAUSS = false>
 __global__ void __launch_bounds__(256, kBoxMinBlocks) k_box_solve_update(const __grid_constant__ FarnBatchArgs args, const char *maps, int nb, int ntx, int nty,
                                                                  int mb, int rebuild) {
     constexpr int sh = BH + 2 * HALF;
@@ -533,7 +581,7 @@ __global__ void __launch_bounds__(256, kBoxMinBlocks) k_box_solve_update(const _
             __syncthreads();
         }
         const int tn = t + (int)gridDim.x;
-        box_tile_compute<HALF>(&sm.raw[0][0], sm.vs, a, mb, rebuild, x0, y0, tid, [&]() {
+        box_tile_compute<HALF, GAUSS>(&sm.raw[0][0], sm.vs, a, mb, rebuild, x0, y0, tid, [&]() {
             // every thread has passed the barrier behind the vertical sums: the staging buffer is dead
             if (tn < total && tid == 0) {
                 fence_proxy_async();
@@ -604,6 +652,8 @@ struct FarnParams {
     int poly_n = 5;
     double poly_sigma = 1.1;
     int use_initial_flow = 0;  // 1: each pair starts from the flow its call passes in (PairJob::init_x; DESIGN §1)
+    int gaussian_window = 0;   // 1: OPTFLOW_FARNEBACK_GAUSSIAN, the 13x13 Gaussian window in every iteration (B.7)
+    int fast_pyramids = 0;     // 1: fastPyramids, level images by a pyrDown chain (B.7)
 };
 
 inline int cv_round(double v) { return (int)std::nearbyint(v); }
@@ -709,20 +759,27 @@ class Farneback final : public FlowAlgorithm {
         pitch0_ = round_up(max_w_, 32);
         plane_elems_ = (size_t)pitch0_ * (max_h_ + 1);
         // a frame slot holds the polynomial expansion of every level (5 planes each): everything that depends on
-        // one frame only, so a frame shared by two consecutive pairs is blurred / resized / expanded once
-        LevelSet ls = levels_for(max_w_, max_h_, /*max_depth=*/true);
+        // one frame only, so a frame shared by two consecutive pairs is blurred / resized / expanded once.  The pyrDown
+        // levels of fast_pyramids are at least as large as B.1's at every level, so slots sized for them hold both.
+        LevelSet ls = levels_for(max_w_, max_h_, /*max_depth=*/true, /*fast=*/true);
         slab_.reserve(kInitialSlots * Slab::padded(ls.total_r_elems, 4) + (1 << 12));
         carve_slots(slab_, ls.total_r_elems);
         slab_.zero();
         ensure_lanes(1);
         ensure_prep_scratch(1);
         DFB_CUDA(cudaFuncSetAttribute(k_gauss_blur, cudaFuncAttributeMaxDynamicSharedMemorySize, GT * (GT + 2 * kMaxHalf) * 4));
-        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoxTmaSmem<6>)));
-        DFB_CUDA(cudaFuncSetAttribute(k_box_solve_update<6>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        int per_sm = 0, sms = 0;
-        DFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_box_solve_update<6>, 256, sizeof(BoxTmaSmem<6>)));
+        int sms = 0;
         DFB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_));
-        persistent_ctas_ = std::max(1, per_sm) * sms;
+        for (int g = 0; g < 2; ++g) {
+            const auto kern = g ? k_box_solve_update<6, true> : k_box_solve_update<6>;
+            DFB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoxTmaSmem<6>)));
+            DFB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+            int per_sm = 0;
+            DFB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, sizeof(BoxTmaSmem<6>)));
+            persistent_ctas_[g] = std::max(1, per_sm) * sms;
+        }
+        const GaussKernel win = gaussian_kernel(13, (double)(6.f * 0.3f));  // (float)(winSize / 2) * 0.3f, as upstream
+        DFB_CUDA(cudaMemcpyToSymbol(c_gauss_win, win.k, sizeof(float) * 7));
         d_maps_.allocate(kMapBytes);
     }
     ~Farneback() override { cudaSetDevice(device_); }
@@ -736,6 +793,8 @@ class Farneback final : public FlowAlgorithm {
         else if (k == "win_size" || k == "poly_n") return (k == "win_size" ? v == 13 : v == 5);  // compiled-in stencils
         else if (k == "time_kernels") { if (!is_flag(v)) return false; time_kernels_ = v != 0; }
         else if (k == "use_initial_flow") { if (!is_flag(v)) return false; prm_.use_initial_flow = (int)v; }
+        else if (k == "gaussian_window") { if (!is_flag(v)) return false; prm_.gaussian_window = (int)v; }
+        else if (k == "fast_pyramids") { if (!is_flag(v)) return false; prm_.fast_pyramids = (int)v; }
         else return false;
         return true;
     }
@@ -748,14 +807,18 @@ class Farneback final : public FlowAlgorithm {
         else if (k == "poly_sigma") *v = prm_.poly_sigma;
         else if (k == "time_kernels") *v = time_kernels_;
         else if (k == "use_initial_flow") *v = prm_.use_initial_flow;
+        else if (k == "gaussian_window") *v = prm_.gaussian_window;
+        else if (k == "fast_pyramids") *v = prm_.fast_pyramids;
         else return false;
         return true;
     }
 
     // per-frame work (B.2, B.3): u8 -> fp32, then for every level: Gaussian blur of the FULL-resolution frame,
-    // bilinear resize to the level, polynomial expansion into the slot's R planes
+    // bilinear resize to the level, polynomial expansion into the slot's R planes.  fast_pyramids (B.7): level 0 is the
+    // fp32 frame and level k the pyrDown of level k - 1, finest first; the blur and resize kernels are not launched.
+    // Slots hold a frame only within the call that prepares it, so a parameter change applies from the next call on.
     void prepare_frames(int n, const uint8_t *const *srcs, size_t pitch_bytes, int w, int h, const int *slots, cudaStream_t s) override {
-        const LevelSet ls = levels_for(w, h, false);
+        const LevelSet ls = levels_for(w, h, false, prm_.fast_pyramids);
         const int pitch_full = round_up(w, 32);
         const FarnConsts pc = poly_constants(prm_.poly_n, prm_.poly_sigma);
         for (int f0 = 0; f0 < n; f0 += kMaxPrep) {
@@ -763,6 +826,25 @@ class Farneback final : public FlowAlgorithm {
             PrepBatch pb = prep_batch(nf);
             for (int i = 0; i < nf; ++i) pb.src[i] = srcs[f0 + i];
             launch_u8_to_f32(pb, nf, pitch_bytes, w, h, pitch_full, s);
+            if (prm_.fast_pyramids) {
+                PrepBatch lb = pb;  // lb.img: the level being expanded; levels k >= 1 alternate between the img and vn scratch
+                for (int l = ls.n - 1; l >= 0; --l) {
+                    const Level &L = ls.lv[l];
+                    if (l == ls.n - 1) {
+                        for (int i = 0; i < nf; ++i) lb.img[i] = pb.frame[i];
+                    } else {
+                        PyrBatch py{};
+                        for (int i = 0; i < nf; ++i) {
+                            py.src[i] = lb.img[i];
+                            py.dst[i] = lb.img[i] = ((ls.n - 1 - l) & 1) ? pb.img[i] : pb.vn[i];
+                        }
+                        launch_pyr_down(py, nf, ls.lv[l + 1], L, s);
+                    }
+                    for (int i = 0; i < nf; ++i) lb.r[i] = slots_.at(slots[f0 + i]) + L.r_off;
+                    launch_poly_exp(lb, nf, L, pc, s);
+                }
+                continue;
+            }
             for (int l = 0; l < ls.n; ++l) {
                 const Level &L = ls.lv[l];
                 for (int i = 0; i < nf; ++i) pb.r[i] = slots_.at(slots[f0 + i]) + L.r_off;
@@ -776,7 +858,7 @@ class Farneback final : public FlowAlgorithm {
 
     // per-pair work (B.4, B.5): coarse -> fine, 10 fused box / solve / rebuild iterations per level
     void solve_batch(const PairJob *jobs, int count, int w, int h, cudaStream_t s) override {
-        const LevelSet ls = levels_for(w, h, false);
+        const LevelSet ls = levels_for(w, h, false, prm_.fast_pyramids);
         for (int j0 = 0; j0 < count; j0 += kMaxFarnBatch) {
             const int nb = std::min(kMaxFarnBatch, count - j0);
             ensure_lanes(nb);
@@ -823,7 +905,7 @@ class Farneback final : public FlowAlgorithm {
         if (k == "farn_level_image") {  // in {frame (u8 values as floats)}  out {level image}  scalars {k}
             need(1, 1);
             fits(w, h);
-            const LevelSet ls = levels_for(w, h, false);
+            const LevelSet ls = levels_for(w, h, false, false);  // B.2's level image whatever fast_pyramids says
             const int lk = (int)sc(0, 0);
             if (lk < 0 || lk >= ls.n) throw std::runtime_error(k + ": level k must be in [0, " + std::to_string(ls.n) + ")");
             const Level &L = ls.lv[ls.n - 1 - lk];
@@ -833,6 +915,20 @@ class Farneback final : public FlowAlgorithm {
             launch_level_image(pb, 1, w, h, pitch_full, L, s);
             DFB_CUDA(cudaDeviceSynchronize());
             download_rows(out[0], Plane{pb.img[0], L.w, L.h, L.pitch}, 0);
+            return true;
+        }
+        if (k == "farn_pyr_down") {  // in {image}  out {pyrDown of it, (w + 1) / 2 x (h + 1) / 2}
+            need(1, 1);
+            fits(w, h);
+            const Level S{w, h, round_up(w, 32), 0, 0.0, 0}, D{(w + 1) / 2, (h + 1) / 2, round_up((w + 1) / 2, 32), 0, 0.0, 0};
+            PrepBatch pb = prep_batch(1);
+            upload_rows(Plane{pb.frame[0], S.w, S.h, S.pitch}, in[0], 0);
+            PyrBatch py{};
+            py.src[0] = pb.frame[0];
+            py.dst[0] = pb.img[0];
+            launch_pyr_down(py, 1, S, D, s);
+            DFB_CUDA(cudaDeviceSynchronize());
+            download_rows(out[0], Plane{pb.img[0], D.w, D.h, D.pitch}, 0);
             return true;
         }
         if (k == "farn_poly_exp") {  // in {level image}  out {R0 .. R4}
@@ -881,7 +977,7 @@ class Farneback final : public FlowAlgorithm {
             fits(w, ph);
             const size_t row = (size_t)w * step, pitch = sc(1, 0) > 0 ? (size_t)sc(1, 0) : row;
             if (pitch < row) throw std::runtime_error(k + ": pitch smaller than a row");
-            const LevelSet ls = levels_for(w, ph, false);
+            const LevelSet ls = levels_for(w, ph, false, prm_.fast_pyramids);
             const Level &L = ls.lv[0];
             ensure_slots(2 * nb);
             ensure_lanes(nb);
@@ -921,7 +1017,7 @@ class Farneback final : public FlowAlgorithm {
         const int ph = h / nb;
         um ? need(12, 5) : need(15, 7);
         fits(w, ph);
-        const LevelSet ls = levels_for(w, ph, false);
+        const LevelSet ls = levels_for(w, ph, false, prm_.fast_pyramids);
         const int l = ls.n - 1;  // full resolution
         ensure_slots(2 * nb);
         ensure_lanes(nb);
@@ -971,8 +1067,8 @@ class Farneback final : public FlowAlgorithm {
         Level lv[kMaxLevels];
         size_t total_r_elems = 0;
     };
-    // B.1 level list in processing order (coarsest first)
-    LevelSet levels_for(int w, int h, bool max_depth) const {
+    // B.1 level list in processing order (coarsest first); fast: the same count, sizes of the pyrDown chain (B.7)
+    LevelSet levels_for(int w, int h, bool max_depth, bool fast) const {
         LevelSet ls;
         const int depth = max_depth ? 5 : prm_.num_levels;
         int cropped = 0;
@@ -990,6 +1086,14 @@ class Farneback final : public FlowAlgorithm {
             L.smooth = std::max(cv_round(L.sigma * 5) | 1, 3);
             L.w = cv_round(w * scale);
             L.h = cv_round(h * scale);
+            if (fast) {
+                L.w = w;
+                L.h = h;
+                for (int i = 0; i < k; ++i) {
+                    L.w = (L.w + 1) / 2;
+                    L.h = (L.h + 1) / 2;
+                }
+            }
             L.pitch = round_up(L.w, 32);
             L.r_off = off;
             off += 5 * (((size_t)L.pitch * (L.h + 1) + 63) & ~size_t(63));
@@ -1022,11 +1126,12 @@ class Farneback final : public FlowAlgorithm {
     // TMA descriptors of the M planes: [level][lane][buffer][plane], rebuilt when the frame geometry or the lane count changes
     static constexpr size_t kMapBytes = (size_t)kMaxLevels * kMaxFarnBatch * 10 * kTensorMapBytes;
     DeviceBuffer<char> d_maps_;
-    int maps_w_ = 0, maps_h_ = 0, maps_lanes_ = 0, maps_levels_ = 0;
-    int persistent_ctas_ = 132;
+    std::vector<int> maps_key_;  // lane count, then every level's size: the maps of one frame size differ with fast_pyramids
+    int persistent_ctas_[2] = {132, 132};  // box, Gaussian window
     void ensure_tensor_maps(const LevelSet &ls) {
-        const Level &F = ls.lv[ls.n - 1];
-        if (maps_w_ == F.w && maps_h_ == F.h && maps_lanes_ == (int)lanes_.size() && maps_levels_ == ls.n) return;
+        std::vector<int> key{(int)lanes_.size()};
+        for (int l = 0; l < ls.n; ++l) key.insert(key.end(), {ls.lv[l].w, ls.lv[l].h});
+        if (key == maps_key_) return;
         std::vector<char> host(kMapBytes, 0);
         for (int l = 0; l < ls.n; ++l)
             for (int i = 0; i < (int)lanes_.size() && i < kMaxFarnBatch; ++i)
@@ -1036,10 +1141,7 @@ class Farneback final : public FlowAlgorithm {
                                              ls.lv[l].w, ls.lv[l].h, ls.lv[l].pitch, RW, BH + 12);
         DFB_CUDA(cudaDeviceSynchronize());  // a launch with the previous descriptors may still be running
         DFB_CUDA(cudaMemcpy(d_maps_, host.data(), host.size(), cudaMemcpyHostToDevice));
-        maps_w_ = F.w;
-        maps_h_ = F.h;
-        maps_lanes_ = (int)lanes_.size();
-        maps_levels_ = ls.n;
+        maps_key_ = key;
     }
     int time_kernels_ = 0;
     void ensure_lanes(int n) {
@@ -1098,6 +1200,12 @@ class Farneback final : public FlowAlgorithm {
             DFB_KERNEL_CHECK();
             launches += 2;
         }
+    }
+    // level S -> level D = pyrDown(S) of every frame of py
+    void launch_pyr_down(const PyrBatch &py, int nf, const Level &S, const Level &D, cudaStream_t s) {
+        k_pyr_down<<<dim3(ceil_div(D.w, 32), ceil_div(D.h, 8), nf), dim3(32, 8), 0, s>>>(py, S.w, S.h, S.pitch, D.w, D.h, D.pitch);
+        DFB_KERNEL_CHECK();
+        launches += 1;
     }
     // pb.img (level L) -> the five R planes at pb.r
     void launch_poly_exp(const PrepBatch &pb, int nf, const Level &L, const FarnConsts &pc, cudaStream_t s) {
@@ -1163,14 +1271,18 @@ class Farneback final : public FlowAlgorithm {
         DFB_KERNEL_CHECK();
         ++launches;
     }
-    // one iteration (box mean of M[mb] -> solve -> rebuild into M[mb ^ 1]); the kernel reads level l's tensor maps, which
-    // ensure_tensor_maps(ls) must have encoded
+    // one iteration (box mean, or the Gaussian window with gaussian_window, of M[mb] -> solve -> rebuild into M[mb ^ 1]); the
+    // kernel reads level l's tensor maps, which ensure_tensor_maps(ls) must have encoded
     void launch_iteration(const FarnBatchArgs &args, int nb, const LevelSet &ls, int l, int mb, int rebuild, cudaStream_t s) {
         const Level &L = ls.lv[l];
         const int ntx = ceil_div(L.w, BW), nty = ceil_div(L.h, BH);
-        const int grid = std::min(persistent_ctas_, ntx * nty * nb);
-        k_box_solve_update<6><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(args, d_maps_ + (size_t)l * kMaxFarnBatch * 10 * kTensorMapBytes, nb, ntx, nty, mb,
-                                                                      rebuild);
+        const int g = prm_.gaussian_window;
+        const int grid = std::min(persistent_ctas_[g], ntx * nty * nb);
+        const char *maps = d_maps_ + (size_t)l * kMaxFarnBatch * 10 * kTensorMapBytes;
+        if (g)
+            k_box_solve_update<6, true><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(args, maps, nb, ntx, nty, mb, rebuild);
+        else
+            k_box_solve_update<6><<<grid, 256, sizeof(BoxTmaSmem<6>), s>>>(args, maps, nb, ntx, nty, mb, rebuild);
         DFB_KERNEL_CHECK();
         ++launches;
     }

@@ -85,6 +85,13 @@ const char *dfb_last_error(const dfb_handle *h);
  * (explicit size, CUDA convention) times (float)pyrScale^k instead of 0.  A null flow buffer, and every other flow call
  * (_u8, _png, the dfb_process_* chains), return DFB_ERR_INVALID_ARG with a message naming use_initial_flow before anything
  * is enqueued; the handle stays usable.  The list runner opens its own handles and never reads an initial flow.
+ * farn: "gaussian_window" (0 [default] or 1; OpenCV's OPTFLOW_FARNEBACK_GAUSSIAN): every iteration averages M over a 13x13
+ * Gaussian window (getGaussianKernel(13, 6 * 0.3f), replicate borders, vertical pass first) instead of the 13x13 box.
+ * farn: "fast_pyramids" (0 [default] or 1; OpenCV's fastPyramids): level 0 is the unblurred frame and level k the pyrDown
+ * (BORDER_REFLECT_101) of level k - 1, size ((w + 1) / 2, (h + 1) / 2), instead of B.1's blur and resize; the level count
+ * is unchanged.  Both compose with each other, with use_initial_flow and with every accepted num_levels / num_iters /
+ * poly_sigma, and every Farneback flow call takes them; the list runner never sets them.  A frame's pyramid lives only
+ * within the call that prepares it, so a change applies from the next call on.
  * Both algorithms: "jpeg_exact" (0 [default] = JPEG files through nvJPEG; 1 = every JPEG this handle writes is exactly the
  * file cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality]) writes with OpenCV's other defaults, libjpeg-turbo 3.x:
  * baseline, standard Huffman tables, islow DCT, gray or YCbCr 4:2:0, no restart markers).  It covers
@@ -437,7 +444,9 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *   "resize"        in {src (w x h)}                         out {dst (scalars[0] x scalars[1])}; scalars {dw, dh, fx, fy, post_mul}
  * On a "farn" handle, single Farneback stages, launched by the engine's own launch code on its frame slots and lanes (w, h
  * at most the handle's maximum frame size):
- *   "farn_level_image"     in {frame (u8 values as floats)}  out {level image, level k size}; scalars {k}
+ *   "farn_level_image"     in {frame (u8 values as floats)}  out {level image, level k size}; scalars {k} (B.1 / B.2's blur
+ *     and resize whatever fast_pyramids says)
+ *   "farn_pyr_down"        in {image}                        out {its pyrDown, (w + 1) / 2 x (h + 1) / 2} (fast_pyramids' level step)
  *   "farn_poly_exp"        in {level image}                  out {R0 .. R4}
  *   "farn_flow_init"       in {fx, fy of the coarser level}  out {fx, fy (scalars[0] x scalars[1])}; scalars {level w, level h}
  *   "farn_initial_flow"    in {x, y of the initial flow}     out {fx, fy of the coarsest level}; scalars {step, pitch, pairs}
@@ -445,7 +454,8 @@ int dfb_jpeg_info(const uint8_t *jpeg, size_t len, int *width, int *height);
  *     pyrScale^k; step 2 uploads the start as a float2 field, step 1 as two planes, rows `pitch` floats apart, 0 = dense)
  *   "farn_update_matrices" in {fx, fy, R0 x 5 (frame a), R1 x 5 (frame b)}  out {M0 .. M4}; scalars {pairs}
  *   "farn_iteration"       in {M x 5, R0 x 5, R1 x 5}        out {fx, fy, M'0 .. M'4}; scalars {rebuild, pairs}
- *     (one box mean -> 2x2 solve -> rebuild of M iteration; M' is written only with rebuild = 1)
+ *     (one box mean -> 2x2 solve -> rebuild of M iteration, the Gaussian window instead of the box mean with
+ *     gaussian_window = 1; M' is written only with rebuild = 1)
  *   The two pair stages run `pairs` (1..8, default 1) pairs in one launch: every plane then stacks the pairs' planes along
  *   its rows (height = pairs x the pair's height).
  * On a "tvl1" handle, single phases of the fused pair kernel, run by one cooperative launch of its own device code on the
