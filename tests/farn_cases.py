@@ -1,7 +1,9 @@
-"""Inputs of the Farneback stage tests and the oracle's building blocks chained as the engine chains its kernels.
+"""Inputs of the Farneback stage tests, the oracle's building blocks chained as the engine chains its kernels, and the
+checks every stage test makes.
 
-Shared by tests/test_farneback_reference_cpu.py (oracle vs the float64 bounds of tests/farn_ref64.py) and
-tests/test_farneback_kernels_gpu.py (kernels vs the oracle and vs the float64 bounds)."""
+Shared by tests/test_farneback_reference_cpu.py (oracle vs the float64 bounds of tests/farn_ref64.py),
+tests/test_farneback_kernels_gpu.py (kernels vs the oracle and vs the float64 bounds) and tests/test_farn_window_gpu.py
+(the B.7 kernels vs tests/farn_restate.py and vs the float64 bounds)."""
 import numpy as np
 
 from denseflow_b200 import synth
@@ -53,6 +55,34 @@ def flow(kind, w, h, seed):
     else:
         raise ValueError(kind)
     return np.ascontiguousarray(fx, np.float32), np.ascontiguousarray(fy, np.float32)
+
+
+def stack(planes):
+    """the planes of several pairs as one launch's input plane, pair after pair down the rows"""
+    return np.ascontiguousarray(np.concatenate(planes, axis=0))
+
+
+def split(a, n):
+    """one launch's output plane back into its n pairs' planes"""
+    return np.split(a, n, axis=0)
+
+
+def within(name, got, ref):
+    """every element of `got` within the float64 bound: ref = (float64 value, bound)"""
+    v, b = ref
+    bad = ~(np.abs(got.astype(np.float64) - v) <= b)
+    assert not bad.any(), "%s: %d elements outside the float64 bound, first at %s: got %r, float64 %r, bound %r" % (
+        name, bad.sum(), tuple(np.argwhere(bad)[0]), got[bad][0], v[bad][0], b[bad][0])
+
+
+def check(variant, name, got, exact, ref64):
+    """strict build: `got` equals `exact` by value; default build: `got` within the float64 bound `ref64`"""
+    if variant == "strict":
+        diff = got != exact
+        assert not diff.any(), "%s: %d elements differ, first at %s: got %r, want %r" % (
+            name, diff.sum(), tuple(np.argwhere(diff)[0]), got[diff][0], exact[diff][0])
+    else:
+        within(name, got, ref64)
 
 
 class Oracle:

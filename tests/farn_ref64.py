@@ -198,6 +198,21 @@ def level_image(frame, lw, lh, ksize, sigma):
     return _bilinear4(b, sx[None, :], x1[None, :], sy[:, None], y1[:, None]).out()
 
 
+def pyr_down(img):
+    """B.7 pyrDown (BORDER_REFLECT_101, vertical pass first, source row / column 2y / 2x); the dyadic weights are exact"""
+    img = np.asarray(img, np.float32)
+    h, w = img.shape
+    ry, cx = 2 * np.arange((h + 1) // 2), 2 * np.arange((w + 1) // 2)
+    k = [E(x) for x in (0.0625, 0.25, 0.375, 0.25, 0.0625)]
+    v = E(img[reflect101(ry - 2, h)]) * k[0]
+    for d in range(1, 5):
+        v = v + E(img[reflect101(ry + d - 2, h)]) * k[d]
+    out = v[:, reflect101(cx - 2, w)] * k[0]
+    for e in range(1, 5):
+        out = out + v[:, reflect101(cx + e - 2, w)] * k[e]
+    return out.out()
+
+
 def poly_exp(img, n=5, sigma=1.1):
     """B.3: polynomial expansion, index-clamped borders, vertical pass (t0, t1, t2) then horizontal: R0 .. R4"""
     img = np.asarray(img, np.float32)
@@ -327,6 +342,29 @@ def iteration(M, R0, R1, fx_at=None, fy_at=None, ksize=13):
     fx, fy = solve(box_mean(M, ksize))
     Mp = update_matrices(fx_at, fy_at, R0, R1) if fx_at is not None else None
     return fx, fy, Mp
+
+
+def gauss_iteration(M, R0, R1, fx_at, fy_at, weights):
+    """one B.7 Gaussian-window iteration: window -> solve (fx, fy), and M' at the flow (fx_at, fy_at) the device returned.
+    `weights` is the window's centre and right half as the engine computes it (fp32 constants, one rounding away), index-
+    clamped, vertical pass first: acc = s(0) g0, then acc += (s(-j) + s(+j)) gj"""
+    g = [const(x) for x in weights]
+    half = len(g) - 1
+    planes = []
+    for P in M:
+        P = np.asarray(P, np.float32)
+        h, w = P.shape
+        yi, xi = np.arange(h), np.arange(w)
+        acc = E(P) * g[0]
+        for j in range(1, half + 1):
+            acc = acc + (E(P[np.maximum(yi - j, 0)]) + E(P[np.minimum(yi + j, h - 1)])) * g[j]
+        v = acc
+        acc = v * g[0]
+        for j in range(1, half + 1):
+            acc = acc + (v[:, np.maximum(xi - j, 0)] + v[:, np.minimum(xi + j, w - 1)]) * g[j]
+        planes.append(acc)
+    fx, fy = solve(planes)
+    return fx, fy, update_matrices(fx_at, fy_at, R0, R1)
 
 
 def flow_init(pfx, pfy, lw, lh, pyr_scale=0.5):

@@ -1,8 +1,8 @@
 """Farneback's Gaussian window (`gaussian_window`) and fast pyramids (`fast_pyramids`; SURVEY B.7) on the GPU.
 
 * Stages: `farn_iteration` on a Gaussian handle (k_box_solve_update<6, true>) and `farn_pyr_down` (k_pyr_down) equal the
-  restatement (tests/farn_window_restate.py) bit for bit in the strict build; in the default build every element is within
-  a forward-error bound derived as in tests/farn_ref64.py.
+  restatement (tests/farn_restate.py) bit for bit in the strict build; in the default build every element is within the
+  forward-error bound of tests/farn_ref64.py's float64 restatement.
 * Whole flows of the four option combinations through dfb_calc_batch_host: the strict build equals the restatement bit for
   bit, the default build is within AEE 0.01 px of it, at frame sizes from 1 x 200 to 1920 x 1080.
 * Batches equal their one-pair calls; every Farneback entry point takes the options; warm starts; a handle switched back
@@ -15,7 +15,7 @@ import pytest
 
 import farn_cases as fc
 import farn_ref64 as r64
-import farn_window_restate as fw
+import farn_restate as R
 from denseflow_b200 import _lib, synth
 from oracle import cv_restate
 
@@ -44,55 +44,6 @@ def _bits_equal(got, want, name):
         name, diff.sum(), tuple(np.argwhere(diff)[0]), np.abs(got.astype(np.float64) - want).max())
 
 
-def _check(variant, name, got, exact, ref64):
-    if variant == "strict":
-        _bits_equal(got, exact, name)
-    else:
-        v, b = ref64
-        bad = ~(np.abs(got.astype(np.float64) - v) <= b)
-        assert not bad.any(), "%s: %d elements outside the float64 bound, first at %s: got %r, float64 %r, bound %r" % (
-            name, bad.sum(), tuple(np.argwhere(bad)[0]), got[bad][0], v[bad][0], b[bad][0])
-
-
-# ---- float64 restatements with forward-error bounds (tests/farn_ref64.py's method) -----------------------------------------
-
-def gauss_iteration64(M, R0, R1, fx_at, fy_at):
-    """one Gaussian-window iteration in float64 with the fp32 evaluation's bound: window -> solve (fx, fy), and M' at the
-    flow the device returned.  The weights are fp32 constants one rounding away."""
-    g = [r64.const(x) for x in fw.gauss_weights()]
-    half = len(g) - 1
-    planes = []
-    for P in M:
-        P = np.asarray(P, np.float32)
-        h, w = P.shape
-        yi, xi = np.arange(h), np.arange(w)
-        acc = r64.E(P) * g[0]
-        for j in range(1, half + 1):
-            acc = acc + (r64.E(P[np.maximum(yi - j, 0)]) + r64.E(P[np.minimum(yi + j, h - 1)])) * g[j]
-        v = acc
-        acc = v * g[0]
-        for j in range(1, half + 1):
-            acc = acc + (v[:, np.maximum(xi - j, 0)] + v[:, np.minimum(xi + j, w - 1)]) * g[j]
-        planes.append(acc)
-    fx, fy = r64.solve(planes)
-    return fx, fy, r64.update_matrices(fx_at, fy_at, R0, R1)
-
-
-def pyr_down64(img):
-    """pyrDown in float64 with the fp32 evaluation's bound (the dyadic weights are exact)"""
-    img = np.asarray(img, np.float32)
-    h, w = img.shape
-    ry, cx = 2 * np.arange((h + 1) // 2), 2 * np.arange((w + 1) // 2)
-    k = [r64.E(x) for x in fw.PYR_K]
-    v = r64.E(img[fw.reflect101(ry - 2, h)]) * k[0]
-    for d in range(1, 5):
-        v = v + r64.E(img[fw.reflect101(ry + d - 2, h)]) * k[d]
-    out = v[:, fw.reflect101(cx - 2, w)] * k[0]
-    for e in range(1, 5):
-        out = out + v[:, fw.reflect101(cx + e - 2, w)] * k[e]
-    return out.out()
-
-
 # ---- stages ------------------------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope="module", autouse=True)
@@ -113,10 +64,6 @@ def _engine(variant):
     return _handles[variant]
 
 
-def _stack(planes):
-    return np.ascontiguousarray(np.concatenate(planes, axis=0))
-
-
 ITER_SHAPES = fc.ITER_SHAPES[::3] + fc.ITER_SMALL[::2] + [(1, 1), (13, 13), (340, 256)]
 
 
@@ -126,21 +73,22 @@ def test_gaussian_iteration_stage(oracle, pairs, variant):
     e, orc = _engine(variant), fc.Oracle(oracle)
     for si, (w, h) in enumerate(ITER_SHAPES):
         cases = [orc.pair_case(w, h, 1000 * si + p, fc.FLOW_KINDS[(si + p) % 4]) for p in range(pairs)]
-        ins = [_stack([c[2][k] for c in cases]) for k in range(5)]
-        ins += [_stack([c[0][k] for c in cases]) for k in range(5)] + [_stack([c[1][k] for c in cases]) for k in range(5)]
+        ins = [fc.stack([c[2][k] for c in cases]) for k in range(5)]
+        ins += [fc.stack([c[0][k] for c in cases]) for k in range(5)] + [fc.stack([c[1][k] for c in cases]) for k in range(5)]
         for rebuild in (0, 1):
             out, _ = e.debug_run_kernel("farn_iteration", ins, 7, [rebuild, pairs])
             for p, (R0, R1, M) in enumerate(cases):
                 tag = "%dx%d pair %d/%d rebuild %d" % (w, h, p, pairs, rebuild)
-                gx, gy = (np.split(out[i], pairs)[p] for i in (0, 1))
-                fx, fy = orc.update_flow(fw.gauss_window5(M))
-                rx, ry, rM = gauss_iteration64(M, R0, R1, gx, gy) if variant == "default" else (None, None, [None] * 5)
-                _check(variant, tag + " fx", gx, fx, rx)
-                _check(variant, tag + " fy", gy, fy, ry)
+                gx, gy = (fc.split(out[i], pairs)[p] for i in (0, 1))
+                fx, fy = orc.update_flow(R.gauss_window5(M))
+                rx, ry, rM = (r64.gauss_iteration(M, R0, R1, gx, gy, R.gauss_weights()) if variant == "default"
+                              else (None, None, [None] * 5))
+                fc.check(variant, tag + " fx", gx, fx, rx)
+                fc.check(variant, tag + " fy", gy, fy, ry)
                 if rebuild:
                     Mp = orc.update_matrices(fx, fy, R0, R1) if variant == "strict" else [None] * 5
                     for k in range(5):
-                        _check(variant, "%s M'%d" % (tag, k), np.split(out[2 + k], pairs)[p], Mp[k], rM[k])
+                        fc.check(variant, "%s M'%d" % (tag, k), fc.split(out[2 + k], pairs)[p], Mp[k], rM[k])
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
@@ -150,7 +98,7 @@ def test_pyr_down_stage(variant):
         img = fc.frame_f32(w, h, 5)
         img[::3] -= 128.0  # signed values too
         (got,), _ = e.debug_run_kernel("farn_pyr_down", [img], 1, out_shape=((h + 1) // 2, (w + 1) // 2))
-        _check(variant, "%dx%d pyrDown" % (w, h), got, fw.pyr_down(img), None if variant == "strict" else pyr_down64(img))
+        fc.check(variant, "%dx%d pyrDown" % (w, h), got, R.pyr_down(img), None if variant == "strict" else r64.pyr_down(img))
 
 
 # ---- whole flows -------------------------------------------------------------------------------------------------------------
@@ -161,7 +109,7 @@ _restated = {}
 def _restatement(a, b, key, combo, init=None, params=None):
     k = (key, combo, init is not None)
     if k not in _restated:
-        _restated[k] = fw.farn_calc(a, b, init, params, *combo)
+        _restated[k] = R.farn_calc(a, b, init=init, params=params, **_opts(combo))
     return _restated[k]
 
 
@@ -244,15 +192,15 @@ def test_every_entry_point_takes_the_options(oracle, combo):
 def test_warm_start(oracle, shape, levels, combo, variant):
     h, w = shape
     a, b, _ = synth.pair(h, w, 9)
-    init = np.ascontiguousarray(fw.farn_calc(a, b) * np.float32(0.6) + np.float32(0.25))
+    init = np.ascontiguousarray(R.farn_calc(a, b) * np.float32(0.6) + np.float32(0.25))
     e = _new(w, h, variant, num_levels=levels, use_initial_flow=1, **_opts(combo))
     got = e.calc(a, b, flow=init.copy())
-    want = fw.farn_calc(a, b, init, oracle.farn_params(num_levels=levels), *combo)
+    want = R.farn_calc(a, b, init=init, params=oracle.farn_params(num_levels=levels), **_opts(combo))
     if variant == "strict":
         _bits_equal(got, want, "%dx%d levels %d %s" % (w, h, levels, combo))
     else:
         assert float(np.hypot(*(got.astype(np.float64) - want).transpose(2, 0, 1)).mean()) <= AEE_TOL
-    cold = fw.farn_calc(a, b, None, oracle.farn_params(num_levels=levels), *combo)
+    cold = R.farn_calc(a, b, params=oracle.farn_params(num_levels=levels), **_opts(combo))
     assert (want != cold).any()
     e.release()
 

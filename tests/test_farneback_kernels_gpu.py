@@ -25,18 +25,6 @@ def _engine(variant):
     return _handles[variant]
 
 
-def _check(variant, name, got, exact, ref64):
-    if variant == "strict":
-        diff = got != exact
-        assert not diff.any(), "%s: %d elements differ from the oracle, first at %s: %r vs %r" % (
-            name, diff.sum(), tuple(np.argwhere(diff)[0]), got[diff][0], exact[diff][0])
-    else:
-        v, b = ref64
-        bad = ~(np.abs(got.astype(np.float64) - v) <= b)
-        assert not bad.any(), "%s: %d elements outside the float64 bound, first at %s: got %r, float64 %r, bound %r" % (
-            name, bad.sum(), tuple(np.argwhere(bad)[0]), got[bad][0], v[bad][0], b[bad][0])
-
-
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("shape", fc.FRAME_SHAPES + fc.SMALL_FRAMES)
 def test_level_image_and_poly_exp(oracle, shape, variant):
@@ -47,20 +35,12 @@ def test_level_image_and_poly_exp(oracle, shape, variant):
     for k in range(len(oracle.farn_levels(w, h))):
         want, (lw, lh, smooth, sigma) = orc.level_image(frame, k)
         (img,), _ = e.debug_run_kernel("farn_level_image", [frame], 1, [k], out_shape=(lh, lw))
-        _check(variant, "%dx%d level %d image" % (w, h, k), img, want, None if variant == "strict" else r64.level_image(frame, lw, lh, smooth, sigma))
+        fc.check(variant, "%dx%d level %d image" % (w, h, k), img, want, None if variant == "strict" else r64.level_image(frame, lw, lh, smooth, sigma))
         R, _ = e.debug_run_kernel("farn_poly_exp", [want], 5)
         Rw = orc.poly_exp(want)
         refs = r64.poly_exp(want) if variant == "default" else [None] * 5
         for i in range(5):
-            _check(variant, "%dx%d level %d R%d" % (w, h, k, i), R[i], Rw[i], refs[i])
-
-
-def _stack(planes):
-    return np.ascontiguousarray(np.concatenate(planes, axis=0))
-
-
-def _split(a, nb):
-    return np.split(a, nb, axis=0)
+            fc.check(variant, "%dx%d level %d R%d" % (w, h, k, i), R[i], Rw[i], refs[i])
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
@@ -74,14 +54,14 @@ def test_update_matrices(oracle, w, variant):
         for p, kind in enumerate(fc.FLOW_KINDS):
             R0, R1 = orc.expansions(w, h, 100 + p)
             cases.append((kind, fc.flow(kind, w, h, w * 7 + h + p), R0, R1))
-        ins = [_stack([c[1][0] for c in cases]), _stack([c[1][1] for c in cases])]
-        ins += [_stack([c[2][k] for c in cases]) for k in range(5)] + [_stack([c[3][k] for c in cases]) for k in range(5)]
+        ins = [fc.stack([c[1][0] for c in cases]), fc.stack([c[1][1] for c in cases])]
+        ins += [fc.stack([c[2][k] for c in cases]) for k in range(5)] + [fc.stack([c[3][k] for c in cases]) for k in range(5)]
         M, _ = e.debug_run_kernel("farn_update_matrices", ins, 5, [len(cases)])
         for p, (kind, (fx, fy), R0, R1) in enumerate(cases):
             want = orc.update_matrices(fx, fy, R0, R1)
             refs = r64.update_matrices(fx, fy, R0, R1) if variant == "default" else [None] * 5
             for k in range(5):
-                _check(variant, "%dx%d %s M%d" % (w, h, kind, k), _split(M[k], len(cases))[p], want[k], refs[k])
+                fc.check(variant, "%dx%d %s M%d" % (w, h, kind, k), fc.split(M[k], len(cases))[p], want[k], refs[k])
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
@@ -92,20 +72,20 @@ def test_iteration(oracle, pairs, variant):
     e, orc = _engine(variant), fc.Oracle(oracle)
     for si, (w, h) in enumerate(fc.ITER_SHAPES + fc.ITER_SMALL):
         cases = [orc.pair_case(w, h, 1000 * si + p, fc.FLOW_KINDS[(si + p) % 4]) for p in range(pairs)]
-        ins = [_stack([c[2][k] for c in cases]) for k in range(5)]
-        ins += [_stack([c[0][k] for c in cases]) for k in range(5)] + [_stack([c[1][k] for c in cases]) for k in range(5)]
+        ins = [fc.stack([c[2][k] for c in cases]) for k in range(5)]
+        ins += [fc.stack([c[0][k] for c in cases]) for k in range(5)] + [fc.stack([c[1][k] for c in cases]) for k in range(5)]
         for rebuild in (0, 1):
             out, _ = e.debug_run_kernel("farn_iteration", ins, 7, [rebuild, pairs])
             for p, (R0, R1, M) in enumerate(cases):
                 tag = "%dx%d pair %d/%d rebuild %d" % (w, h, p, pairs, rebuild)
-                gx, gy = (_split(out[i], pairs)[p] for i in (0, 1))
+                gx, gy = (fc.split(out[i], pairs)[p] for i in (0, 1))
                 fx, fy, Mp = orc.iteration(M, R0, R1, rebuild)
                 rx, ry, rM = r64.iteration(M, R0, R1, gx, gy) if variant == "default" else (None, None, [None] * 5)
-                _check(variant, tag + " fx", gx, fx, rx)
-                _check(variant, tag + " fy", gy, fy, ry)
+                fc.check(variant, tag + " fx", gx, fx, rx)
+                fc.check(variant, tag + " fy", gy, fy, ry)
                 if rebuild:
                     for k in range(5):
-                        _check(variant, "%s M'%d" % (tag, k), _split(out[2 + k], pairs)[p], Mp[k], rM[k])
+                        fc.check(variant, "%s M'%d" % (tag, k), fc.split(out[2 + k], pairs)[p], Mp[k], rM[k])
 
 
 @pytest.mark.parametrize("variant", VARIANTS)
@@ -122,7 +102,7 @@ def test_flow_init(oracle, variant):
             want = orc.flow_init(pfx, pfy, lw, lh)
             refs = r64.flow_init(pfx, pfy, lw, lh) if variant == "default" else [None, None]
             for c in range(2):
-                _check(variant, "%dx%d -> %dx%d flow %d" % (pw, ph, lw, lh, c), got[c], want[c], refs[c])
+                fc.check(variant, "%dx%d -> %dx%d flow %d" % (pw, ph, lw, lh, c), got[c], want[c], refs[c])
 
 
 # ---- end to end ---------------------------------------------------------------------------------------------------------

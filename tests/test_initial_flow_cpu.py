@@ -1,4 +1,4 @@
-"""`use_initial_flow` in its restatements (tests/tvl1_restate.py, tests/initial_flow_ref.py), before the GPU builds are
+"""`use_initial_flow` in its restatements (tests/tvl1_restate.py, tests/farn_restate.py), before the GPU builds are
 pinned to them (tests/test_initial_flow_gpu.py).
 
 * TV-L1: the initial-flow pyramid over the C oracle's building blocks and over oracle/tvl1_numpy.py's agree bit for bit,
@@ -13,7 +13,7 @@ pinned to them (tests/test_initial_flow_gpu.py).
 import numpy as np
 import pytest
 
-import initial_flow_ref as R
+import farn_restate as R
 import tvl1_restate as T
 from denseflow_b200 import synth
 
@@ -102,9 +102,9 @@ def test_farneback_restatement_zero_start_is_orc_farn_calc(oracle, num_levels):
     p = oracle.farn_params(num_levels=num_levels)
     ref = oracle.farn_calc(a, b, p)
     for init in (None, np.zeros((96, 128, 2), F)):
-        got = R.farn_calc(a, b, init, p)
+        got = R.farn_calc(a, b, init=init, params=p)
         assert np.array_equal(got.view(np.int32), ref.view(np.int32))
-    assert not np.array_equal(R.farn_calc(a, b, smooth_field(96, 128, 4), p), ref)
+    assert not np.array_equal(R.farn_calc(a, b, init=smooth_field(96, 128, 4), params=p), ref)
 
 
 @pytest.mark.parametrize("hw", [(256, 256, 0), (256, 340, 100)])
@@ -114,12 +114,12 @@ def test_farneback_one_level_matches_live_opencv_with_initial_flow(oracle, hw):
     a, b, _ = synth.pair(h, w, seed)
     init = smooth_field(h, w, seed + 1, amp=8.0)
     p = oracle.farn_params(num_levels=0, resize_convention=oracle.RESIZE_HALF_PIXEL)
-    mine = R.farn_calc(a, b, init, p)
+    mine = R.farn_calc(a, b, init=init, params=p)
     live = cv2.calcOpticalFlowFarneback(a, b, init.copy(), 0.5, 0, 13, 10, 5, 1.1, cv2.OPTFLOW_USE_INITIAL_FLOW)
     assert synth.aee(mine, live) < 5e-6
     cold = cv2.calcOpticalFlowFarneback(a, b, None, 0.5, 0, 13, 10, 5, 1.1, 0)
     assert np.abs(live - cold).max() > 1e-2  # the initial flow is really used
     # more levels: CPU OpenCV resizes the initial flow with INTER_AREA, the CUDA module (and this contract) with INTER_LINEAR
-    multi = R.farn_calc(a, b, init, oracle.farn_params(resize_convention=oracle.RESIZE_HALF_PIXEL))
+    multi = R.farn_calc(a, b, init=init, params=oracle.farn_params(resize_convention=oracle.RESIZE_HALF_PIXEL))
     live5 = cv2.calcOpticalFlowFarneback(a, b, init.copy(), 0.5, 5, 13, 10, 5, 1.1, cv2.OPTFLOW_USE_INITIAL_FLOW)
     print("farneback %dx%d, 5 levels from an initial flow: AEE vs cv2 (INTER_AREA start) = %.3e px" % (w, h, synth.aee(multi, live5)))

@@ -5,7 +5,7 @@
 * At 131 x 97, from a smooth random field, a field past `bound` and the oracle's own cold flow: the TV-L1 strict build's
   flows and per-(scale, warp) iteration logs equal the restatement over the C oracle's building blocks
   (tests/tvl1_restate.py) bit for bit, fused and unfused, and the Farneback strict build's flows equal
-  tests/initial_flow_ref.py's; the default builds are within 0.01 px.  Other frame sizes, lane counts, groups and chained
+  tests/farn_restate.py's; the default builds are within 0.01 px.  Other frame sizes, lane counts, groups and chained
   starts: tests/test_initial_flow_paths_gpu.py; the start pyramids alone: tests/test_initial_flow_stages_gpu.py.
 * Host batch = per-pair calls, device batch = host batch, planes = the float2 field; pageable and page-locked host buffers
   and a non-default stream.
@@ -15,7 +15,7 @@
 import numpy as np
 import pytest
 
-import initial_flow_ref as R
+import farn_restate as R
 import tvl1_pin as pin
 import tvl1_restate as T
 from denseflow_b200 import synth
@@ -125,8 +125,8 @@ def test_tvl1_matches_the_restatement(oracle, variant, fused, median):
 def test_farneback_matches_the_restatement(oracle, variant, num_levels):
     a, b, _ = synth.pair(H, W, 7)
     e = _new("farn", W, H, variant, use_initial_flow=1, num_levels=num_levels)
-    for init in (smooth_field(H, W, 3, amp=6.0), R.farn_calc(a, b, None, oracle.farn_params(num_levels=num_levels))):
-        ref = R.farn_calc(a, b, init, oracle.farn_params(num_levels=num_levels))
+    for init in (smooth_field(H, W, 3, amp=6.0), R.farn_calc(a, b, params=oracle.farn_params(num_levels=num_levels))):
+        ref = R.farn_calc(a, b, init=init, params=oracle.farn_params(num_levels=num_levels))
         flow = e.calc(a, b, flow=init.copy())
         if variant == "strict":
             _bits_equal(flow, ref, "num_levels %d" % num_levels)

@@ -1,6 +1,6 @@
 """Warm starts (`use_initial_flow`, DESIGN §1) end to end, through the paths a start takes beyond the one 131 x 97 corner of
 tests/test_initial_flow_gpu.py.  The strict build is pinned bit for bit (flows and TV-L1 iteration logs, tests/tvl1_pin.py)
-to the restatements of tests/tvl1_restate.py (TV-L1) and tests/initial_flow_ref.py (Farneback); the default build is held
+to the restatements of tests/tvl1_restate.py (TV-L1) and tests/farn_restate.py (Farneback); the default build is held
 to 0.01 px and to its own bits across lane counts and entry points.
 
 * Geometry: tiny frames, the squares around the tile and level cuts, 7 x 1080 / 1080 x 7, both engines; TV-L1 at the
@@ -16,7 +16,7 @@ to 0.01 px and to its own bits across lane counts and entry points.
 import numpy as np
 import pytest
 
-import initial_flow_ref as R
+import farn_restate as R
 import tvl1_pin as pin
 import tvl1_restate as T
 from denseflow_b200 import synth
@@ -68,7 +68,7 @@ def test_geometry_strict_bit_exact(oracle, alg):
         if alg == "tvl1":
             notes.append(pin.check(oracle, a, b, flow, e.tvl1_stats()[0], "%dx%d" % (w, h), oracle_out=T.tvl1_calc(a, b, init=init, **SMALL)))
         else:
-            _bits_equal(flow, R.farn_calc(a, b, init, _farn_params(oracle)), "%dx%d" % (w, h))
+            _bits_equal(flow, R.farn_calc(a, b, init=init, params=_farn_params(oracle)), "%dx%d" % (w, h))
     e.release()
     if alg == "tvl1":  # the create() defaults
         h, w = 256, 340
@@ -157,7 +157,7 @@ def test_host_groups(oracle, alg, variant):
                 notes.append(pin.check(oracle, fr[j], fr[j + 1], host[j], iters[j], "pair %d" % j,
                                        oracle_out=T.tvl1_calc(fr[j], fr[j + 1], init=starts[j], **SMALL)))
             else:
-                _bits_equal(host[j], R.farn_calc(fr[j], fr[j + 1], starts[j], _farn_params(oracle)), "pair %d" % j)
+                _bits_equal(host[j], R.farn_calc(fr[j], fr[j + 1], init=starts[j], params=_farn_params(oracle)), "pair %d" % j)
         pin.finish(notes)
 
 
@@ -168,7 +168,7 @@ def test_farneback_strict_bit_exact(oracle, num_levels):
     for k, (w, h) in enumerate([(340, 256), (131, 97), (64, 64), (63, 64), (33, 33), (8, 8), (3, 2)]):
         a, b, _ = synth.pair(h, w, 40 + k)
         for init in (smooth_field(h, w, 50 + k, amp=6.0), (np.random.default_rng(k).uniform(-4, 4, (h, w, 2)) * [w, h]).astype(np.float32)):
-            ref = R.farn_calc(a, b, init, _farn_params(oracle, num_levels))
+            ref = R.farn_calc(a, b, init=init, params=_farn_params(oracle, num_levels))
             _bits_equal(e.calc(a, b, flow=init.copy()), ref, "%dx%d num_levels %d" % (w, h, num_levels))
     # 19 pairs: three launches of at most 8
     h, w = 97, 131
@@ -176,7 +176,7 @@ def test_farneback_strict_bit_exact(oracle, num_levels):
     starts = _starts(19, h, w, 60)
     flows = e.calc_batch(list(fr), step=1, flows=starts.copy())
     for j in (0, 7, 8, 15, 16, 18):
-        _bits_equal(flows[j], R.farn_calc(fr[j], fr[j + 1], starts[j], _farn_params(oracle, num_levels)), "batch pair %d" % j)
+        _bits_equal(flows[j], R.farn_calc(fr[j], fr[j + 1], init=starts[j], params=_farn_params(oracle, num_levels)), "batch pair %d" % j)
     e.release()
 
 
@@ -190,7 +190,7 @@ def test_chained_starts(oracle, alg):
     kw = SMALL if alg == "tvl1" else {}
     refs, prev, notes = [], np.zeros((h, w, 2), np.float32), []
     for j in range(n - 1):
-        out = T.tvl1_calc(fr[j], fr[j + 1], init=prev, **kw) if alg == "tvl1" else (R.farn_calc(fr[j], fr[j + 1], prev, _farn_params(oracle)),)
+        out = T.tvl1_calc(fr[j], fr[j + 1], init=prev, **kw) if alg == "tvl1" else (R.farn_calc(fr[j], fr[j + 1], init=prev, params=_farn_params(oracle)),)
         refs.append(out)
         prev = out[0]
     e = _new(alg, w, h, "strict", **kw)
@@ -248,7 +248,7 @@ def test_default_warm_regression_guard(oracle, alg):
     e = _new(alg, w, h, "default")
     flow = e.calc(a, b, flow=init.copy())
     e.release()
-    ref = T.tvl1_calc(a, b, init=init)[0] if alg == "tvl1" else R.farn_calc(a, b, init, _farn_params(oracle))
+    ref = T.tvl1_calc(a, b, init=init)[0] if alg == "tvl1" else R.farn_calc(a, b, init=init, params=_farn_params(oracle))
     epe = np.hypot(*(flow.astype(np.float64) - ref).transpose(2, 0, 1))
     band = np.ones((h, w), bool)
     band[6:-6, 6:-6] = False

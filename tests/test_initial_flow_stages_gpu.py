@@ -4,8 +4,8 @@
 * TV-L1: every level of every lane's start pyramid.  Strict build: equal to tests/tvl1_restate.tvl1_init_pyramid bit
   for bit.  Default build: level 0 is the start itself, every coarser level within the float64 bound of
   tvl1_ref64.upsample(level above, ..., float(scale_step)), element by element.
-* Farneback: the coarsest level's start.  Strict build: equal to initial_flow_ref.farn_start (orc_resize_linear x
-  float(pyrScale^k), as in initial_flow_ref.farn_calc) bit for bit.  Default build: within farn_ref64.level_start's bound.
+* Farneback: the coarsest level's start.  Strict build: equal to farn_restate.farn_start (orc_resize_linear x
+  float(pyrScale^k), as in farn_restate.farn_calc) bit for bit.  Default build: within farn_ref64.level_start's bound.
 
 Covered: the frame shapes of tests/farn_cases.py and 4K, geometry_cases' tiny frames, small planes, strips and the sizes at
 and just below every level cut; TV-L1 at the nscales / scale_step pairs of the CPU pyramid tests, Farneback at num_levels
@@ -18,8 +18,8 @@ import pytest
 
 import farn_cases as fc
 import farn_ref64 as f64
+import farn_restate as R
 import geometry_cases as gc
-import initial_flow_ref as R
 import tvl1_ref64 as t64
 import tvl1_restate as T
 from test_initial_flow_cpu import PYRAMIDS, smooth_field
